@@ -1,20 +1,23 @@
 #!/usr/bin/env python
-"""bench.py -- AlexNet product-quantized forward throughput (images/s) on N B200s, the metric of BASELINE.json.
+"""bench.py -- AlexNet product-quantized forward throughput (images/s) on N H100s, the metric of BASELINE.json.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl b200|reference] [--dump-outputs bench_out]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
 A "step" is one PQ forward pass (23 layers: 8 PQ layers + ReLU/LRN/pool/softmax) over B synthetic 227x227x3 images
 per GPU (default B = 256, BASELINE.json configs[2]; `--batch 1024` with --gpus 8 is configs[3]).  Images are
 batch-sharded, weights replicated, and for N > 1 the only exchange is one all-gather of the [B,1000] logits
-(NCCL over NVLink) inside the step.  One JSON line is printed by rank 0 (see the task contract):
+(NCCL over NVLink) inside the step.  One JSON line is printed by rank 0:
   value     device-resident images/s, whole job (inputs already in HBM), CUDA events, max over ranks
   e2e       the same metric through the host-buffer C-ABI call qcnn_net_forward_h (pinned host in -> host out)
   roofline  dominant kernel: executed tensor flops (decode-at-use GEMM) or algorithmic bytes / CUDA-event time vs the
-            measured peaks of MEASURED_PEAKS.json
+            peaks of MEASURED_PEAKS.json when that file exists, else the H100 SXM data-sheet figures
   cpu_baseline  the reference's own CPU path timed on this box (rank 0, N = 1 only, bounded sample)
 `--impl reference` times the reference CPU implementation with all host cores instead (no GPU work at all).
+At least three warm-up steps always run (the library times its tilings on the device during the first passes).
+`--dump-outputs DIR` writes what the last timed step computed -- DIR/prob.npy and DIR/logits.npy, float32 [B,1000] of
+rank 0 -- so that two builds can be compared output for output (the inputs are the same seeded images in every run).
 """
 import argparse
 import importlib
@@ -79,7 +82,7 @@ def lcg_images(n, seed0, tables=None):
 
 def write_synthetic_alexnet(writer, dirpath, pfx, seed=1):
     """Random-init parameters of the AlexNet PQ architecture in the reference's .bin/.cbn formats.  `writer` supplies
-    write_bin_f32 / write_cbn_u8: the product's own writers on the B200 arm (qcnn_write_bin_f32 / qcnn_write_cbn_u8),
+    write_bin_f32 / write_cbn_u8: the product's own writers on the GPU arm (qcnn_write_bin_f32 / qcnn_write_cbn_u8),
     the oracle's on the reference arm (which must not load the product library).  Codebooks ~ N(0, 1/fan_in)."""
     rng = np.random.RandomState(seed)
     os.makedirs(dirpath, exist_ok=True)
@@ -303,11 +306,11 @@ def workload_config(args, what, world):
                         "227x227x3 LCG images" % args.batch,
             "global_batch": args.batch * world, "per_gpu_batch": args.batch, "parallelism": "dp%d" % world,
             "weights": what, "collective": "all_gather(logits [B,1000]) on a side stream, overlapped with the next step" if world > 1 else "none",
-            "l2": "inputs (%.0f MB/step) exceed the 126 MB L2; two input sets alternate" % (args.batch * IMG_LEN * 4 / 1e6)}
+            "l2": "inputs (%.0f MB/step) exceed the 50 MB L2; two input sets alternate" % (args.batch * IMG_LEN * 4 / 1e6)}
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# the B200 arm
+# the GPU arm
 # ---------------------------------------------------------------------------------------------------------------
 def run_b200_arm(args, q):
     import torch
@@ -331,8 +334,8 @@ def run_b200_arm(args, q):
     net = q.Net(ctx, dirpath, pfx, "AlexNet")
 
     # NUMA placement of the pinned staging buffers: run this rank on the CPUs next to its GPU (NVML's ideal affinity)
-    # before anything is pinned -- on a two-socket host a remote pinned buffer copies at ~30 instead of ~55 GB/s
-    # (tools/h2d_bw.py), and the end-to-end number is bound by that copy
+    # before anything is pinned -- on a two-socket host a remote pinned buffer copies more slowly (tools/h2d_bw.py
+    # measures it), and the end-to-end number is bound by that copy
     numa = "unbound"
     try:
         import pynvml
@@ -388,6 +391,12 @@ def run_b200_arm(args, q):
     barrier()
     if in_range:
         torch.cuda.cudart().cudaProfilerStop()
+    if args.dump_outputs and rank == 0:
+        # outputs of the last timed step, before the sections below reuse the buffers
+        last = gather.rows(args.steps - 1) if world > 1 else logits
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "prob.npy"), prob.cpu().numpy().astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), last.cpu().numpy().astype(np.float32))
     ms_total = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(ms_total, op=dist.ReduceOp.MAX)
@@ -461,8 +470,8 @@ def run_b200_arm(args, q):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except (OSError, ValueError):
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s (not measured)"
     names = {0: "conv1", 4: "conv2", 8: "conv3", 10: "conv4", 12: "conv5", 15: "fc6", 18: "fc7", 21: "fc8",
              2: "lrn1+pool1", 6: "lrn2+pool2", 14: "pool5", 22: "softmax"}
     per_layer = {}
@@ -476,20 +485,15 @@ def run_b200_arm(args, q):
     pq_layers = [l for l in ALEXNET_PQ if layer_ms[l] > 0]
     dom = max(pq_layers, key=lambda l: layer_ms[l])
     wd = net.layer_work(dom, B)
-    sm_clk = (clocks or {}).get("sm_mhz") or float(peaks.get("sm_max_mhz", 1965.0))
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(names[dom])
-    except (OSError, ValueError, KeyError):
-        pass
+    sm_clk = (clocks or {}).get("sm_mhz") or float(peaks.get("sm_max_mhz", 1980.0))
 
-    # Tensor-core work of a pq_gemm_tc launch, from the plan the library reports: every CTA runs `ksteps` k-steps of
-    # three kind::tf32 MMAs (3xTF32) of 128 channels x NT positions x 8 (DESIGN.md 5): executed MACs, padding included.
+    # Tensor-core work of a pq_gemm_tc launch, from the plan the library reports: every CTA runs `ksteps` k-steps over
+    # 128 channels x NT positions (DESIGN.md 5): executed MACs, padding included.
     import re
 
     def tc_macs(l):
-        # executed MACs of the launch, padding included: per k-step (8 input values) either THREE kind::tf32 MMAs of
-        # 128 x NT x 8 (3xTF32 operands) or TWO kind::f16 MMAs of 128 x NT x 16 (bf16x2 operands, the default)
+        # executed MACs of the launch, padding included: per k-step (8 input values) either THREE tf32 MMAs of
+        # 128 x NT x 8 (3xTF32 operands) or TWO bf16 MMAs of 128 x NT x 16 (bf16x2 operands, the default)
         d = net.pq_layer(l).describe(B)
         m = re.search(r"pq_gemm_tc.*?NT=(\d+).*?grid=(\d+).*?ksteps=(\d+)", d)
         if not m:
@@ -506,18 +510,18 @@ def run_b200_arm(args, q):
     ach_gbs = wd["alg_bytes"] / (layer_ms[dom] * 1e-3) / 1e9
     dom_macs = tc_macs(dom)
     # SURVEY.md 8(d): the declared roofline of every kernel of this path is HBM -- algorithmic bytes of the launch over
-    # its CUDA-event time against the measured copy bandwidth.  That is `frac`.  The batched kernels are NOT bound by HBM
-    # (DESIGN.md 5): what limits the dominant launch is in `tensor` (decode-at-use GEMM: executed 3xTF32 flops incl.
-    # padding, and the useful dense-equivalent flops, against measured bf16 / 2) or in `gather` (LUT + gather family).
+    # its CUDA-event time against the HBM peak (MEASURED_PEAKS.json, else the data sheet).  That is `frac`.  The batched kernels are NOT bound by HBM
+    # (DESIGN.md 5): what limits the dominant launch is in `tensor` (decode-at-use GEMM: executed flops incl.
+    # padding, and the useful dense-equivalent flops, against the dense bf16 peak, halved for tf32 operands) or in `gather` (LUT + gather family).
     roofline = {"bound": "hbm", "kernel": ("pq_gemm_tc_kernel (%s)" if dom_macs else "%s") % names[dom],
                 "achieved": round(ach_gbs, 2), "peak": hbm_peak, "unit": "GB/s", "frac": round(ach_gbs / hbm_peak, 5),
-                "traffic": traffic, "peak_source": peak_src, "alg_bytes_per_launch": wd["alg_bytes"],
+                "peak_source": peak_src, "alg_bytes_per_launch": wd["alg_bytes"],
                 "ms_per_launch": round(float(layer_ms[dom]), 4),
-                "definition": "SURVEY.md 8(d) algorithmic bytes per launch / CUDA-event time of that launch / measured HBM peak"}
+                "definition": "SURVEY.md 8(d) algorithmic bytes per launch / CUDA-event time of that launch / HBM peak (see peak_source)"}
     if dom_macs:
-        # tf32 MMAs run at half the bf16 rate: peak = measured dense bf16 (cuBLAS, MEASURED_PEAKS.json) / 2
-        bf16 = float(peaks.get("bf16_tflops", 1650.0))
-        peak_tc = bf16 if tc_is_bf(dom) else bf16 / 2.0     # kind::tf32 issues at half the bf16 rate
+        # tf32 MMAs run at half the bf16 rate: peak = dense bf16 (MEASURED_PEAKS.json, else the H100 SXM data sheet) / 2
+        bf16 = float(peaks.get("bf16_tflops", 989.0))
+        peak_tc = bf16 if tc_is_bf(dom) else bf16 / 2.0
         ach = 2.0 * dom_macs / (layer_ms[dom] * 1e-3) / 1e12
         dense = {0: 105415200.0, 4: 223948800.0, 8: 149520384.0, 10: 112140288.0, 12: 74760192.0,
                  15: 37748736.0, 18: 16777216.0, 21: 4096000.0}       # dense-equivalent MACs per image (SURVEY.md App. C)
@@ -527,9 +531,9 @@ def run_b200_arm(args, q):
             "executed_TFLOPs": round(ach, 1), "useful_TFLOPs": round(useful, 1), "peak_TFLOPs": round(peak_tc, 1),
             "frac_executed": round(ach / peak_tc, 4), "frac_useful": round(useful / peak_tc, 4),
             "flops_per_launch_executed": 2.0 * dom_macs, "flops_per_launch_useful": 2.0 * dense[dom] * B,
-            "operands": "bf16x2 (two kind::f16 MMAs of K = 16 per k-step)" if tc_is_bf(dom) else "3xTF32 (three kind::tf32 MMAs of K = 8 per k-step)",
-            "peak_source": ("MEASURED_PEAKS.json bf16_tflops" if "bf16_tflops" in peaks else "fallback 1650") +
-                           ("" if tc_is_bf(dom) else " / 2 (kind::tf32 issues at half the bf16 rate)"),
+            "operands": "bf16x2 (two bf16 MMAs of K = 16 per k-step)" if tc_is_bf(dom) else "3xTF32 (three tf32 MMAs of K = 8 per k-step)",
+            "peak_source": ("MEASURED_PEAKS.json bf16_tflops" if "bf16_tflops" in peaks else "H100 SXM data sheet, 989 TFLOP/s dense (not measured)") +
+                           ("" if tc_is_bf(dom) else " / 2 (tf32 issues at half the bf16 rate)"),
             "all_pq_gemm_launches": {"launches": len(all_tc),
                                      "executed_TFLOPs": round(sum(2.0 * m for m, _ in all_tc) / (sum(t for _, t in all_tc) * 1e-3) / 1e12, 1),
                                      "ms": round(float(sum(t for _, t in all_tc)), 4)},
@@ -586,7 +590,7 @@ def run_b200_arm(args, q):
         def timed(fn, reps=12, use_stamps=True):
             ev, sp = [], []
             for k in range(reps):
-                flush.fill_(k & 0xFF)          # evict the 126 MB L2
+                flush.fill_(k & 0xFF)          # evict the 50 MB L2
                 a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 a.record()
                 fn()
@@ -729,14 +733,22 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
-    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--warmup", type=int, default=3,
+                    help="un-timed steps before the timed ones; at least 3 are run, because the library times its tilings "
+                         "on the device and captures its batch-1 graph during the first passes (the JSON line says how many ran)")
     ap.add_argument("--batch", type=int, default=256, help="images per GPU per step")
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--cpu-images", type=int, default=100, help="cpu_baseline sample size (images)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-config4", action="store_true", help="skip the 1024-per-GPU (configs[3]) timing")
     ap.add_argument("--no-strict", action="store_true", help="skip the strict-path (tensor_core = 0) timing")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step (prob.npy, logits.npy; float32) into DIR")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the outputs of the GPU path; it cannot be combined with --impl reference")
     if args.impl == "reference":
         return run_reference_arm(args)
     q = importlib.import_module("quantized-cnn_b200")   # raises if libqcnn_b200.so is missing: no fallback

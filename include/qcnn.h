@@ -1,5 +1,5 @@
 /*
- * qcnn.h -- C ABI of the B200-native product-quantized (PQ) forward path.
+ * qcnn.h -- C ABI of the H100-native (sm_90a) product-quantized (PQ) forward path.
  *
  * Drop-in boundary for the reference's CalcFeatMap_ConvAprx / CalcFeatMap_FCntAprx path
  * (CAS-CLab/quantized-cnn, src/CaffeEva.cc).  The reference has no FFI of its own: the path sits behind
@@ -15,7 +15,7 @@
  *     assignment indices are uint8, 0-based, "file order" as CaffePara::layerParaLst holds them after
  *     LoadLayerPara (src/CaffePara.cc:239-306).
  *   - one qcnn_ctx per GPU; a ctx and its layers are not thread-safe; distinct ctxs may be used concurrently.
- *   - there is NO CPU fallback: every compute entry point fails with an error if no sm_100 device is usable.
+ *   - there is NO CPU fallback: every compute entry point fails with an error if no sm_90 device is usable.
  */
 #ifndef QCNN_H_
 #define QCNN_H_

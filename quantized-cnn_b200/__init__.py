@@ -1,9 +1,9 @@
-"""quantized-cnn_b200: Python binding (ctypes) of the B200-native PQ forward path.
+"""quantized-cnn_b200: Python binding (ctypes) of the H100-native (sm_90a) PQ forward path.
 
-The product is ``libqcnn_b200.so`` (hand-written sm_100a CUDA + C++ host code behind the C ABI of
+The product is ``libqcnn_b200.so`` (hand-written sm_90a CUDA + C++ host code behind the C ABI of
 ``include/qcnn.h``).  This module only marshals pointers: torch supplies device memory and streams, every
 computation happens inside the shared library.  There is no CPU or PyTorch fallback -- if the library is
-missing or no B200 is visible the calls raise.
+missing or no H100 is visible the calls raise.
 
 The directory name contains a hyphen, so import it with::
 
@@ -24,7 +24,7 @@ class QcnnError(RuntimeError):
 
 
 def build(verbose=False):
-    """Compile libqcnn_b200.so in-tree with nvcc for sm_100a (see Makefile)."""
+    """Compile libqcnn_b200.so in-tree with nvcc for sm_90a (see Makefile)."""
     import subprocess
     cmd = ["make", "-C", _HERE, "-j8"]
     if not verbose:

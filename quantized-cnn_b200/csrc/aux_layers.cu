@@ -380,7 +380,7 @@ int LaunchLrnMaxPool(qcnn_ctx* ctx, const float* src, float* dst, int N, int H, 
   // output rows per CTA: as many as keep two CTAs per SM (less re-normalisation of shared input rows)
   int ro = 1;
   static const int roMax = getenv("QCNN_LRN_RO") ? atoi(getenv("QCNN_LRN_RO")) : 1;
-  static const int lrnThreads = getenv("QCNN_LRN_THREADS") ? atoi(getenv("QCNN_LRN_THREADS")) : 512;   // measured: 512 > 384 > 256 threads
+  static const int lrnThreads = getenv("QCNN_LRN_THREADS") ? atoi(getenv("QCNN_LRN_THREADS")) : 512;   // threads per CTA of the LRN kernels
   while (ro < roMax && ro < Ho && sizeof(float) * static_cast<size_t>(ro * stride + ksz) * W * C <= 110 * 1024) ro++;
   const size_t tileBytes = sizeof(float) * static_cast<size_t>((ro - 1) * stride + ksz) * W * C;
   if (tileBytes <= 160 * 1024 && N <= 65535) {

@@ -1,4 +1,4 @@
-// Fused PQ convolution for sm_100a: per-subspace LUT (codebook x input inner products) built in shared memory
+// Fused PQ convolution for sm_90a: per-subspace LUT (codebook x input inner products) built in shared memory
 // and consumed by the uint8 gather-accumulate of the same CTA -- the LUT never touches HBM.
 // Replaces CaffeEva::CalcFeatMap_ConvAprx + GetInPdMat (reference src/CaffeEva.cc:760-868, 1261-1296):
 //     LUT[n][hi][wi][s][k] = sum_j src[n][hi][wi][g*Cg + s*d + j] * ctrd[s][k][j]
@@ -11,11 +11,11 @@
 //   * zero padding is realised by zero LUT columns (padded flat grid), so no per-lane bounds predicate exists in
 //     the inner loop -- out-of-image taps add +0.0f, which is what the reference's tap skipping amounts to;
 //   * a thread owns J positions x CPT channels (<= 64 accumulators, held as float2 pairs so two positions are
-//     accumulated by one FADD2); per 4 channels it issues one 128-bit broadcast load of 4 pre-multiplied LUT row
-//     offsets, then 4 x (1 IADD + J LDS + J/2 FADD2);
+//     accumulated as a float2); per 4 channels it issues one 128-bit broadcast load of 4 pre-multiplied LUT row
+//     offsets, then 4 x (1 IADD + J LDS + J FADD);
 //   * the per-(s) assignment slice is staged in shared memory already multiplied by the LUT row pitch.
 // The LUT stage is a [K x d] x [d x positions] contraction per subspace.  It runs on the FP32 pipe as a
-// register-blocked mini-GEMM: 8 codewords x 4 positions per thread, packed FFMA2 (two FMAs per issue slot), codebook
+// register-blocked mini-GEMM: 8 codewords x 4 positions per thread, float2 FFMA pairs, codebook
 // rows broadcast from shared memory, 128-bit LUT stores.  (fp32, ascending j: parity with the reference's saxpy
 // order up to FMA contraction; tensor-core TF32 would break the fp32 tolerance -- SURVEY.md 7.5.)
 // Two kernels share both stages:
@@ -26,12 +26,17 @@
 //                    owned by a different "row group" of warps; columns are de-interleaved by stride phase so
 //                    that a tap again is a constant shift.
 #include "qcnn_internal.h"
+#include "wgmma.h"
 
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
 
 namespace {
+
+// float2 arithmetic, element by element (sm_90 has no packed fp32 instructions)
+__device__ __forceinline__ float2 Ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 Fadd2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 
 constexpr int kMaxThreads = 512;
 
@@ -115,10 +120,10 @@ __device__ __forceinline__ void LutStep(float2 (&acc)[8][2], const float2* __res
   for (int kk = 0; kk < 4; kk++) {
     const float4 cc = cp[kk];  // (c[2kk], c[2kk], c[2kk+1], c[2kk+1])
     const float2 ca = make_float2(cc.x, cc.y), cb = make_float2(cc.z, cc.w);
-    acc[2 * kk][0] = __ffma2_rn(ca, x01, acc[2 * kk][0]);
-    acc[2 * kk][1] = __ffma2_rn(ca, x23, acc[2 * kk][1]);
-    acc[2 * kk + 1][0] = __ffma2_rn(cb, x01, acc[2 * kk + 1][0]);
-    acc[2 * kk + 1][1] = __ffma2_rn(cb, x23, acc[2 * kk + 1][1]);
+    acc[2 * kk][0] = Ffma2(ca, x01, acc[2 * kk][0]);
+    acc[2 * kk][1] = Ffma2(ca, x23, acc[2 * kk][1]);
+    acc[2 * kk + 1][0] = Ffma2(cb, x01, acc[2 * kk + 1][0]);
+    acc[2 * kk + 1][1] = Ffma2(cb, x23, acc[2 * kk + 1][1]);
   }
 }
 
@@ -160,7 +165,7 @@ __device__ __forceinline__ void BuildLut(float* __restrict__ lut, const float2* 
 // gather stage
 // ------------------------------------------------------------------------------------------------------------
 // Accumulators of one thread: J positions x CPT channels.  For even J two positions share a float2 so that one
-// FADD2 retires two lookups.
+// float2 add retires two lookups.
 template <int CPT, int J>
 struct Acc {
   static constexpr int JP = (J % 2 == 0) ? J / 2 : J;
@@ -194,7 +199,7 @@ __device__ __forceinline__ void GatherTap(Acc<CPT, J>& acc, const char* base, co
         for (int jp = 0; jp < J / 2; jp++) {
           const float2 val = make_float2(*reinterpret_cast<const float*>(b[u] + (2 * jp) * 128),
                                          *reinterpret_cast<const float*>(b[u] + (2 * jp + 1) * 128));
-          acc.v[jp][c4 + u] = __fadd2_rn(acc.v[jp][c4 + u], val);
+          acc.v[jp][c4 + u] = Fadd2(acc.v[jp][c4 + u], val);
         }
       } else {
 #pragma unroll
@@ -356,43 +361,53 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_kernel(const ConvArgs a) {
 // stride-1 kernel, tensor-core LUT stage (K = 128 codewords, subspaces of <= 8 dims)
 //
 // The LUT of a subspace is the dense contraction  LUT[k][p] = sum_j ctrd[s][k][j] * x[p][j]  = C (128 x 8) * X^T (8 x N).
-// Here it runs on the 5th-generation tensor cores: ONE thread issues three tcgen05.mma kind::tf32 (M = 128, N <= 256,
-// K = 8) per subspace -- the 3xTF32 split  C_hi*X_hi + C_hi*X_lo + C_lo*X_hi  keeps fp32-level accuracy (measured
-// 7e-7 of the LUT magnitude, tools/tc_lut_test.cu) -- with the accumulator in TMEM (lane = codeword, column =
-// position).  The MMA of subspace s+1 executes asynchronously WHILE the CUDA cores gather subspace s out of shared
-// memory; at the stage boundary the finished accumulator is drained TMEM -> registers -> lut[k][p] (tcgen05.ld +
-// 128-bit stores, bank-conflict free because the row pitch is 4 mod 32 words).  Operands reach the canonical K-major
-// no-swizzle UMMA tiles through cp.async (raw) + a hi/lo split pass.
+// Here it runs on the Hopper tensor cores: per 32 LUT columns a warpgroup issues three wgmma.mma_async of tf32 operands
+// (M = 64 codewords, N = 32, K = 8) -- the 3xTF32 split  C_hi*X_hi + C_hi*X_lo + C_lo*X_hi  keeps fp32-level accuracy --
+// with both operands in shared memory and the accumulator in its registers, which it then writes to lut[k][p].  The
+// first two warpgroups of the CTA (the first one alone in CTAs of fewer than eight warps) produce the LUT of a subspace
+// at the stage boundary; all warps gather.  Operands reach the canonical K-major unswizzled tiles through cp.async (raw)
+// + a hi/lo split pass.
 // ------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t SmemU32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
-// canonical K-major / SWIZZLE_NONE operand tile (tf32): rows in groups of 8, per group K-chunk 0 (8 rows x 16 B) then
+// canonical K-major operand tile without swizzle (tf32): rows in groups of 8, per group K-chunk 0 (8 rows x 16 B) then
 // K-chunk 1; element (row r, k) -> float index below.  Descriptor: LBO = 128 B (K chunks), SBO = 256 B (row groups).
-__device__ __forceinline__ int UmmaIdx(int r, int k) { return (r >> 3) * 64 + (k >> 2) * 32 + (r & 7) * 4 + (k & 3); }
-__device__ __forceinline__ uint64_t UmmaDesc(const void* smem) {
-  uint64_t d = (static_cast<uint64_t>(SmemU32(smem)) >> 4) & 0x3FFF;
-  d |= static_cast<uint64_t>(8) << 16;    // leading byte offset 128 B >> 4
-  d |= static_cast<uint64_t>(16) << 32;   // stride byte offset 256 B >> 4
-  d |= static_cast<uint64_t>(1) << 46;    // descriptor version: Blackwell
-  return d;
-}
-__device__ __forceinline__ void UmmaTf32(uint32_t tmemD, uint64_t descA, uint64_t descB, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmemD), "l"(descA), "l"(descB),
-               "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void MbarWait(uint64_t* mbar, uint32_t parity) {
-  uint32_t done = 0;
-  while (!done) {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(SmemU32(mbar)), "r"(parity) : "memory");
-  }
-}
+__device__ __forceinline__ int TileIdx(int r, int k) { return (r >> 3) * 64 + (k >> 2) * 32 + (r & 7) * 4 + (k & 3); }
 // hi = value truncated to tf32 (what the tensor core reads), lo = exact remainder
 __device__ __forceinline__ void SplitTf32(float v, float& hi, float& lo) {
   hi = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
   lo = v - hi;
 }
+// LUT[128][NM] = A (128 codewords x 8) * B^T (NM positions x 8) as 3xTF32, written to lut (row pitch PP floats).
+// Called by all threads of warps 0 .. 4 nwg - 1 (nwg = 1 or 2 warpgroups); the tiles are published to the async proxy.
+__device__ __forceinline__ void LutMma(const float* aHi, const float* aLo, const float* bHi, const float* bLo, float* lut,
+                                       int PP, int NM, int warp, int lane, int nwg) {
+  const int wg = warp >> 2;
+  for (int half = wg; half < 2; half += nwg) {          // codewords [64 half, +64)
+    const uint64_t dAh = qcnn::WgmmaDesc(qcnn::SmemU32(aHi + half * 512), 128, 256);
+    const uint64_t dAl = qcnn::WgmmaDesc(qcnn::SmemU32(aLo + half * 512), 128, 256);
+    const int r0 = half * 64 + (warp & 3) * 16 + (lane >> 2);
+    for (int c = 0; c < (NM >> 5); c++) {               // 32 LUT columns = 4 row groups of the B tile
+      const uint64_t dBh = qcnn::WgmmaDesc(qcnn::SmemU32(bHi + c * 256), 128, 256);
+      const uint64_t dBl = qcnn::WgmmaDesc(qcnn::SmemU32(bLo + c * 256), 128, 256);
+      float d[16];
+#pragma unroll
+      for (int i = 0; i < 16; i++) d[i] = 0.0f;
+      qcnn::WgmmaFence();
+      qcnn::Wgmma<32>::Tf32SS(d, dAh, dBh);
+      qcnn::Wgmma<32>::Tf32SS(d, dAh, dBl);
+      qcnn::Wgmma<32>::Tf32SS(d, dAl, dBh);
+      qcnn::WgmmaCommit();
+      qcnn::WgmmaWaitAll();
+      // fragment: d[4 i + {0, 1}] = row r0, columns 8 i + 2 (lane % 4) + {0, 1}; d[4 i + {2, 3}] = row r0 + 8
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        const int col = c * 32 + 8 * i + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(lut + r0 * PP + col) = make_float2(d[4 * i], d[4 * i + 1]);
+        *reinterpret_cast<float2*>(lut + (r0 + 8) * PP + col) = make_float2(d[4 * i + 2], d[4 * i + 3]);
+      }
+    }
+  }
+}
+
 
 struct SmemLayoutTc {
   float* lut;       // [128][PP]
@@ -405,8 +420,6 @@ struct SmemLayoutTc {
   float* cr;        // [128][8] raw codebook of the next subspace
   uint8_t* idN;     // [taps*CT] raw assignment slice
   int* posoff;      // [NM]
-  uint64_t* mbar;
-  uint32_t* tmemBase;
 };
 __device__ __forceinline__ SmemLayoutTc CarveTc(unsigned char* smem, int PP, int NM, int taps, int CT) {
   SmemLayoutTc s;
@@ -419,9 +432,7 @@ __device__ __forceinline__ SmemLayoutTc CarveTc(unsigned char* smem, int PP, int
   s.xr = s.bLo + NM * 8;
   s.cr = s.xr + NM * 8;
   s.posoff = reinterpret_cast<int*>(s.cr + 1024);
-  s.mbar = reinterpret_cast<uint64_t*>(s.posoff + NM);
-  s.tmemBase = reinterpret_cast<uint32_t*>(s.mbar + 1);
-  s.idN = reinterpret_cast<uint8_t*>(s.tmemBase + 2);
+  s.idN = reinterpret_cast<uint8_t*>(s.posoff + NM + 4);
   return s;
 }
 
@@ -458,14 +469,6 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_tc_kernel(const ConvArgs a) {
     }
     sm.posoff[pos] = off;
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(SmemU32(sm.tmemBase)), "r"(256) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(SmemU32(sm.mbar)), "r"(1) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
 
   Acc<CPT, J> acc;
   {
@@ -474,11 +477,8 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_tc_kernel(const ConvArgs a) {
     for (int c = 0; c < CPT; c++) bv[c] = __ldg(a.bias + g * a.Kg + cbase + c);
     acc.Fill(bv);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();  // posoff, mbarrier, TMEM base visible
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmemD = *sm.tmemBase;
-  const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(NM >> 3) << 17) | (8u << 24);
+  __syncthreads();  // posoff visible
+  const int nwg = nwarps >= 8 ? 2 : 1;   // warpgroups that run the LUT MMAs
   const uint32_t rowBytes = static_cast<uint32_t>(a.PP) * 4u;
 
   // raw operands of subspace s: pixels [NM][8] and codebook [128][8], zero beyond the subspace's real dims
@@ -497,32 +497,25 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_tc_kernel(const ConvArgs a) {
       CpAsync4(sm.xr + e, src + (ok ? off + ch0 + jj : 0), ok);
     }
   };
-  // raw -> hi/lo canonical UMMA tiles (generic-proxy writes, published to the async proxy by the caller's fence)
+  // raw -> hi/lo canonical operand tiles (generic-proxy writes, published to the async proxy by the caller's fence)
   auto splitOperands = [&]() {
     for (int e = tid; e < 1024; e += T) {
       float hi, lo;
       SplitTf32(sm.cr[e], hi, lo);
-      const int i = UmmaIdx(e >> 3, e & 7);
+      const int i = TileIdx(e >> 3, e & 7);
       sm.aHi[i] = hi;
       sm.aLo[i] = lo;
     }
     for (int e = tid; e < NM * 8; e += T) {
       float hi, lo;
       SplitTf32(sm.xr[e], hi, lo);
-      const int i = UmmaIdx(e >> 3, e & 7);
+      const int i = TileIdx(e >> 3, e & 7);
       sm.bHi[i] = hi;
       sm.bLo[i] = lo;
     }
   };
-  auto issueMma = [&]() {  // one thread: D = Ah*Bh + Ah*Bl + Al*Bh, then signal the mbarrier when all three retire
-    const uint64_t dAh = UmmaDesc(sm.aHi), dAl = UmmaDesc(sm.aLo), dBh = UmmaDesc(sm.bHi), dBl = UmmaDesc(sm.bLo);
-    UmmaTf32(tmemD, dAh, dBh, idesc, 0);
-    UmmaTf32(tmemD, dAh, dBl, idesc, 1);
-    UmmaTf32(tmemD, dAl, dBh, idesc, 1);
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(SmemU32(sm.mbar)) : "memory");
-  };
 
-  // prologue: LUT(0) on the tensor core, operands of subspace 1 + assignment slice 0 in flight
+  // prologue: operand tiles of subspace 0 published, raw operands of subspace 1 + assignment slice 0 in flight
   fetchRaw(0);
   CpAsyncCommit();
   CpAsyncWaitAll();
@@ -530,47 +523,23 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_tc_kernel(const ConvArgs a) {
   splitOperands();
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   __syncthreads();
-  if (tid == 0) issueMma();
   if (a.S > 1) fetchRaw(1);
   FetchOffsets(sm.idN, asmtG, taps, a.CT, a.KgPad, tid, T);
   CpAsyncCommit();
 
   for (int s = 0; s < a.S; s++) {
-    MbarWait(sm.mbar, s & 1);   // LUT(s) is complete in TMEM; the operand tiles are free again
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     CpAsyncWaitAll();
-    __syncthreads();            // (A) gather(s-1) is done with lut/idx; raw operands of s+1 and idN(s) are visible
-    // drain TMEM -> lut: warp w owns TMEM lanes [32 (w%4), +32) = codewords; 32 columns (positions) per load
-    {
-      const int q = warp & 3;
-      const int k = q * 32 + lane;
-      float* row = sm.lut + k * a.PP;
-      for (int c = warp >> 2; c < (NM >> 5); c += (nwarps + 3 - q) >> 2) {
-        uint32_t r[32];
-        const uint32_t taddr = tmemD + (static_cast<uint32_t>(q * 32) << 16) + c * 32;
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                     "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-                     "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                       "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-                       "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-                       "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-                       "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                     : "r"(taddr) : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 32; i += 4)
-          *reinterpret_cast<uint4*>(row + c * 32 + i) = make_uint4(r[i], r[i + 1], r[i + 2], r[i + 3]);
-      }
-    }
+    __syncthreads();            // (A) gather(s-1) is done with lut/idx; operand tiles of s, raw operands of s+1 and idN(s) are visible
+    // LUT(s): tensor cores -> accumulator fragments -> lut
+    if (warp < 4 * nwg) LutMma(sm.aHi, sm.aLo, sm.bHi, sm.bLo, sm.lut, a.PP, NM, warp, lane, nwg);
     CommitOffsets(sm.idN, sm.idx, taps, a.CT, rowBytes, tid, T);
-    if (s + 1 < a.S) splitOperands();
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();            // (B) lut + idx ready, TMEM drained, operand tiles of s+1 published
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     if (s + 1 < a.S) {
-      if (tid == 0) issueMma();                  // LUT(s+1) is computed while subspace s is gathered
+      __syncthreads();          // the MMAs of subspace s have read the operand tiles
+      splitOperands();
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    }
+    __syncthreads();            // (B) lut + idx ready, operand tiles of s+1 published
+    if (s + 1 < a.S) {
       if (s + 2 < a.S) fetchRaw(s + 2);
       FetchOffsets(sm.idN, asmtG + static_cast<size_t>(s + 1) * taps * a.KgPad, taps, a.CT, a.KgPad, tid, T);
       CpAsyncCommit();
@@ -596,9 +565,6 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_tc_kernel(const ConvArgs a) {
       StoreChannels<CPT, J>(out, acc, j, a.relu);
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmemD), "r"(256) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -733,8 +699,8 @@ __global__ void __launch_bounds__(MAXT, 1) conv_roll_kernel(const ConvArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// rolling-row kernel, tensor-core LUT stage: same row-group structure as conv_roll_kernel; the LUT of the NEXT
-// (input row, subspace) step is produced by tcgen05.mma into TMEM while the CUDA cores gather the current one.
+// rolling-row kernel, tensor-core LUT stage: same row-group structure as conv_roll_kernel; the LUT of an
+// (input row, subspace) step is produced by wgmma (LutMma) instead of the FFMA build.
 // ------------------------------------------------------------------------------------------------------------
 template <int CPT, int J, int MAXT>
 __global__ void __launch_bounds__(MAXT, 1) conv_roll_tc_kernel(const ConvArgs a) {
@@ -769,25 +735,14 @@ __global__ void __launch_bounds__(MAXT, 1) conv_roll_tc_kernel(const ConvArgs a)
     const int wi = i * a.stride + phase - a.pad;
     sm.posoff[pos] = (phase < a.stride && wi >= 0 && wi < a.Wi) ? wi * pixStride : -1;
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(SmemU32(sm.tmemBase)), "r"(256) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(SmemU32(sm.mbar)), "r"(1) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
   float bias[CPT];
 #pragma unroll
   for (int c = 0; c < CPT; c++) bias[c] = __ldg(a.bias + g * a.Kg + cbase + c);
   Acc<CPT, J> acc;
   acc.Fill(bias);
   int ho_cur = ho0 + rg;
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmemD = *sm.tmemBase;
-  const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(NM >> 3) << 17) | (8u << 24);
+  const int nwg = nwarps >= 8 ? 2 : 1;   // warpgroups that run the LUT MMAs
   const uint32_t rowBytes = static_cast<uint32_t>(a.PP) * 4u;
 
   const int hi_begin = ho0 * a.stride - a.pad;
@@ -816,24 +771,17 @@ __global__ void __launch_bounds__(MAXT, 1) conv_roll_tc_kernel(const ConvArgs a)
     for (int e = tid; e < 1024; e += T) {
       float hi, lo;
       SplitTf32(sm.cr[e], hi, lo);
-      const int i = UmmaIdx(e >> 3, e & 7);
+      const int i = TileIdx(e >> 3, e & 7);
       sm.aHi[i] = hi;
       sm.aLo[i] = lo;
     }
     for (int e = tid; e < NM * 8; e += T) {
       float hi, lo;
       SplitTf32(sm.xr[e], hi, lo);
-      const int i = UmmaIdx(e >> 3, e & 7);
+      const int i = TileIdx(e >> 3, e & 7);
       sm.bHi[i] = hi;
       sm.bLo[i] = lo;
     }
-  };
-  auto issueMma = [&]() {
-    const uint64_t dAh = UmmaDesc(sm.aHi), dAl = UmmaDesc(sm.aLo), dBh = UmmaDesc(sm.bHi), dBl = UmmaDesc(sm.bLo);
-    UmmaTf32(tmemD, dAh, dBh, idesc, 0);
-    UmmaTf32(tmemD, dAh, dBl, idesc, 1);
-    UmmaTf32(tmemD, dAl, dBh, idesc, 1);
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(SmemU32(sm.mbar)) : "memory");
   };
 
   if (steps > 0) {
@@ -844,7 +792,6 @@ __global__ void __launch_bounds__(MAXT, 1) conv_roll_tc_kernel(const ConvArgs a)
     splitOperands();
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
-    if (tid == 0) issueMma();
     if (steps > 1) fetchRaw(1);
     FetchOffsets(sm.idN, asmtG, taps, a.CT, a.KgPad, tid, T);
     CpAsyncCommit();
@@ -853,42 +800,19 @@ __global__ void __launch_bounds__(MAXT, 1) conv_roll_tc_kernel(const ConvArgs a)
   for (int it = 0; it < steps; it++) {
     const int kh = hi + a.pad - ho_cur * a.stride;  // warp-uniform
     const bool active = ho_cur < ho_end && kh >= 0 && kh < a.ksz;
-    MbarWait(sm.mbar, it & 1);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     CpAsyncWaitAll();
     __syncthreads();  // (A)
-    {
-      const int q = warp & 3;
-      const int k = q * 32 + lane;
-      float* row = sm.lut + k * a.PP;
-      for (int c = warp >> 2; c < (NM >> 5); c += (nwarps + 3 - q) >> 2) {
-        uint32_t r[32];
-        const uint32_t taddr = tmemD + (static_cast<uint32_t>(q * 32) << 16) + c * 32;
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                     "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-                     "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                       "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-                       "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-                       "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-                       "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                     : "r"(taddr) : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 32; i += 4)
-          *reinterpret_cast<uint4*>(row + c * 32 + i) = make_uint4(r[i], r[i + 1], r[i + 2], r[i + 3]);
-      }
-    }
+    if (warp < 4 * nwg) LutMma(sm.aHi, sm.aLo, sm.bHi, sm.bLo, sm.lut, a.PP, NM, warp, lane, nwg);
     if (a.S > 1 || it == 0) CommitOffsets(sm.idN, sm.idx, taps, a.CT, rowBytes, tid, T);
-    if (it + 1 < steps) splitOperands();
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    if (it + 1 < steps) {
+      __syncthreads();  // the MMAs of this step have read the operand tiles
+      splitOperands();
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    }
     __syncthreads();  // (B)
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     int hin = hi, sn = s + 1;
     if (sn == a.S) { sn = 0; hin = hi + 1; }
     if (it + 1 < steps) {
-      if (tid == 0) issueMma();
       if (it + 2 < steps) fetchRaw(it + 2);
       if (a.S > 1) FetchOffsets(sm.idN, asmtG + static_cast<size_t>(sn) * taps * a.KgPad, taps, a.CT, a.KgPad, tid, T);
       CpAsyncCommit();
@@ -931,9 +855,6 @@ __global__ void __launch_bounds__(MAXT, 1) conv_roll_tc_kernel(const ConvArgs a)
       ho_cur += a.rgroups;
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmemD), "r"(256) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -942,7 +863,7 @@ __global__ void __launch_bounds__(MAXT, 1) conv_roll_tc_kernel(const ConvArgs a)
 // so tabulating costs more than it saves.  This kernel keeps the layer in PQ form (codebook + uint8 assignments) but
 // evaluates the inner product where it is consumed:  acc[p][c] += <x[p + tap], c_{asmt[tap][c]}>  -- the same sum,
 // the codeword (not the partial product) is what the warp-uniform assignment index gathers (128-bit broadcast load).
-// A thread owns 2 output rows x 2 columns x CPT channels (float2 pairs, FFMA2); the strip's input rows live in shared
+// A thread owns 2 output rows x 2 columns x CPT channels (float2 pairs); the strip's input rows live in shared
 // memory, de-interleaved by stride phase, so a tap is a constant shift and there are no barriers after the tile load.
 // ------------------------------------------------------------------------------------------------------------
 template <int CPT, int NJ, int ROWS>
@@ -1042,10 +963,10 @@ __global__ void __launch_bounds__(384, 1) conv_direct_kernel(const ConvArgs a) {
             const int c = c4 + u;
 #pragma unroll
             for (int r = 0; r < ROWS; r++) {
-              acc[r][c] = __ffma2_rn(make_float2(c01.x, c01.y), x[r][0], acc[r][c]);
-              if (NJ > 1) acc[r][c] = __ffma2_rn(make_float2(c01.z, c01.w), x[r][1 % NJ], acc[r][c]);
-              if (NJ > 2) acc[r][c] = __ffma2_rn(c2, x[r][2 % NJ], acc[r][c]);
-              if (NJ > 3) acc[r][c] = __ffma2_rn(c3, x[r][3 % NJ], acc[r][c]);
+              acc[r][c] = Ffma2(make_float2(c01.x, c01.y), x[r][0], acc[r][c]);
+              if (NJ > 1) acc[r][c] = Ffma2(make_float2(c01.z, c01.w), x[r][1 % NJ], acc[r][c]);
+              if (NJ > 2) acc[r][c] = Ffma2(c2, x[r][2 % NJ], acc[r][c]);
+              if (NJ > 3) acc[r][c] = Ffma2(c3, x[r][3 % NJ], acc[r][c]);
             }
           }
         }
@@ -1169,7 +1090,7 @@ int PlanConv(qcnn_layer* L, int N) {
                 const int NM = RoundUp(std::max(need1, need2), 32);  // MMA N = LUT columns per subspace
                 if (NM > 256 || warps < 4) continue;
                 a.RI = NM;          // the tensor-core kernel receives NM in this field
-                a.PP = NM + 4;      // row pitch = 4 (mod 32) words: conflict-free 128-bit drains from TMEM
+                a.PP = NM + 4;      // row pitch = 4 (mod 32) words
                 smemFloats = 128 * static_cast<size_t>(a.PP) + static_cast<size_t>(taps) * CT + 2048 + 25 * static_cast<size_t>(NM) + 1024 + 8;
               } else {
                 a.PP = RoundUp(std::max(need1, need2), 4);
@@ -1211,14 +1132,14 @@ int PlanConv(qcnn_layer* L, int N) {
             // FFMA path: lut + idx + cb2 + xs[2] + posoff + cbN; tensor path: lut + idx + A/B tiles + raw staging
             p.smem = sizeof(float) * smemFloats + RoundUp(taps * CT, 16);
             if (p.smem > smemMax) continue;
-            // measured on B200 (profiles/): ~1.3 clk per gather wavefront; FFMA LUT stage ~0.12 clk per entry at d = 8;
-            // tensor-core LUT stage: the MMA is hidden behind the gather, what remains is the TMEM drain + operand split
-            // gather latency hiding improves with resident warps (9 warps: 1.37 clk/wavefront measured, 12: 1.28)
+            // model constants (they only order the candidates; on-device timing picks among the cheapest): ~1.3 clk per
+            // gather wavefront, FFMA LUT stage ~0.12 clk per entry at d = 8, tensor-core LUT stage = MMA + fragment
+            // stores + operand split; gather latency hiding improves with resident warps
             const double gather = gatherSlots * (1.0 + 1.0 / (4.0 * J)) * (1.15 + 1.6 / warps);
             const double build = tc ? builtEntries * 0.02 + 300.0 * phases : builtEntries * ipe / 5.5 * 0.12;
             const double perCta = gather + build + 400.0 * phases;
             // few resident warps cannot keep ~30 LDS in flight per SM nor feed the FMA pipe during the LUT stage
-            // (measured: 2-warp CTAs run the build at ~0.5 IPC); 64 accumulators at 512 threads spill
+            // (model constants, not measurements); 64 accumulators at 512 threads spill
             double occPenalty = warps < 4 ? 2.5 : (warps < 6 ? 1.6 : (warps < 8 ? 1.25 : 1.0));
             if (p.threads > 384 && J * CPT >= 64) occPenalty *= 1.1;
             const double ctas = static_cast<double>(G) * nct * a.nstrips * N;
@@ -1263,7 +1184,7 @@ int PlanConv(qcnn_layer* L, int N) {
                                       static_cast<size_t>(taps) * CT);
             if (p.smem > smemMax) continue;
             const int pairs = CeilDiv(a.R, rowsPer);
-            // issue slots: per (row pair, tap, channel) 2 loads + 2*NJ FFMA2, plus 4*NJ pixel loads per tap
+            // issue slots: per (row pair, tap, channel) 2 loads + 2*NJ FFMA pairs, plus 4*NJ pixel loads per tap
             const double perWarp = static_cast<double>(CeilDiv(pairs, rgroups)) * taps * (CPT * (2.0 + rowsPer * NJ) + 2.0 * rowsPer * NJ + CPT / 4.0);
             const double perCta = perWarp * cwarps * rgroups / 2.6 + rowsIn * NJ * a.PP * 0.5;
             const double ctas = static_cast<double>(G) * nct * a.nstrips * N;
@@ -1418,8 +1339,8 @@ int LaunchConv(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
       if (!ok) continue;
       static const bool tuneLog = getenv("QCNN_AUTOTUNE_LOG") != nullptr;
       if (tuneLog)
-        fprintf(stderr, "[qcnn autotune] N=%d Cout=%d k=%d cand %zu: kernel=%d NT/CPT=%d GT/J=%d lite=%d wide=%d bf=%d nsplit=%d smem=%zu -> %.4f ms\n",
-                N, L->Cout, L->ksz, i, c.kernel, c.CPT, c.kernel == 6 ? c.g.GT : c.J, c.g.lite, c.g.wide, c.g.bf, c.g.nsplit, c.smem, ms);
+        fprintf(stderr, "[qcnn autotune] N=%d Cout=%d k=%d cand %zu: kernel=%d NT/CPT=%d GT/J=%d bf=%d nsplit=%d smem=%zu -> %.4f ms\n",
+                N, L->Cout, L->ksz, i, c.kernel, c.CPT, c.kernel == 6 ? c.g.GT : c.J, c.g.bf, c.g.nsplit, c.smem, ms);
       if (ms < bestMs) { bestMs = ms; bestI = i; }
     }
     cudaEventDestroy(e0);
@@ -1441,15 +1362,14 @@ int DescribeConv(qcnn_layer* L, int N, char* buf, size_t cap) {
   if (p.kernel == 6) {
     int ksteps = 0;
     for (int c = 0; c < p.g.nChunks; c++) ksteps += p.g.chunkCount[p.g.mode == 1 ? c : 0];
-    snprintf(buf, cap, "pq_gemm_tc(tcgen05, weights decoded into TMEM%s) mode=%d NT=%d GT=%d slots=%d smem=%zuB grid=%d NPOS=%d "
-             "chunks=%d ksteps=%d nsplit=%d", p.g.bf ? (p.g.lite ? ", bf16x2, 2 CTAs/SM" : (p.g.wide ? ", bf16x2, 8 decoder warps" : (p.g.xl ? ", bf16x2, 16 warps" : ", bf16x2")))
-                    : (p.g.lite ? ", 2 CTAs/SM" : (p.g.wide ? ", 8 decoder warps" : "")), p.g.mode, p.g.NT, p.g.GT, p.g.NSLOT, p.smem,
+    snprintf(buf, cap, "pq_gemm_tc(wgmma, weights decoded into registers%s) mode=%d NT=%d GT=%d smem=%zuB grid=%d NPOS=%d "
+             "chunks=%d ksteps=%d nsplit=%d", p.g.bf ? ", bf16x2" : "", p.g.mode, p.g.NT, p.g.GT, p.smem,
              CeilDiv(N * p.g.IB, p.g.NT) * L->grp * p.g.nct * std::max(1, p.g.nsplit), p.g.NPOS, p.g.nChunks,
              ksteps / std::max(1, p.g.nsplit), std::max(1, p.g.nsplit));
     return 0;
   }
   snprintf(buf, cap, "%s CPT=%d J=%d threads=%d smem=%zuB grid=(%d,%d) R=%d strips=%d CT=%d nct=%d PP=%d pwarps=%d "
-           "cwarps=%d rgroups=%d", p.kernel == 0 ? "conv_s1" : (p.kernel == 2 ? "conv_s1_tc(tcgen05 LUT)" : (p.kernel == 3 ? "conv_roll_tc(tcgen05 LUT)" : (p.kernel == 4 ? "conv_direct" : "conv_roll"))), p.CPT, p.J, p.threads, p.smem,
+           "cwarps=%d rgroups=%d", p.kernel == 0 ? "conv_s1" : (p.kernel == 2 ? "conv_s1_tc(wgmma LUT)" : (p.kernel == 3 ? "conv_roll_tc(wgmma LUT)" : (p.kernel == 4 ? "conv_direct" : "conv_roll"))), p.CPT, p.J, p.threads, p.smem,
            p.a.G * p.a.nct * p.a.nstrips, N, p.a.R, p.a.nstrips, p.a.CT, p.a.nct, p.a.PP, p.a.pwarps, p.a.cwarps,
            p.a.rgroups);
   return 0;

@@ -1,4 +1,4 @@
-// Fused PQ fully-connected layer for sm_100a: LUT stage + uint8 gather-accumulate in ONE kernel.
+// Fused PQ fully-connected layer for sm_90a: LUT stage + uint8 gather-accumulate in ONE kernel.
 // Replaces CaffeEva::CalcFeatMap_FCntAprx + GetInPdMat (reference src/CaffeEva.cc:968-1025, 1261-1296):
 //     LUT[n][s][k] = sum_j x[n][s*d+j] * ctrd[s][k][j]        (ascending j, rounded mul then rounded add)
 //     dst[n][o]    = bias[o] + sum_s LUT[n][s][asmt[s][o]]    (ascending s)
@@ -14,7 +14,7 @@
 //     <= 128 B = one bank sweep: distinct codewords hit distinct banks and equal codewords broadcast, so the
 //     lane-dependent gather is bank-conflict free by construction.
 //   * assignments are stored pre-multiplied by 4 (byte offsets) when K <= 64, saving the shift per lookup.
-//   * S can be split over blockIdx.z (needed at small N to fill 148 SMs); partial sums are reduced in a fixed
+//   * S can be split over blockIdx.z (needed at small N to fill the SMs); partial sums are reduced in a fixed
 //     order by fc_reduce_kernel (deterministic; no atomics).  With nsplit == 1 the accumulation order is
 //     exactly the reference's (bias, then s ascending) and the result is bit-identical to the CPU path.
 #include "qcnn_internal.h"
@@ -342,7 +342,7 @@ static int ChunkLen(int K, int tn) {
 }
 
 // Large batches: the layer as a decode-at-use GEMM on the tensor cores (pq_gemm_tc.cu, mode 2): M = 128 outputs per CTA,
-// N = up to 256 images, K split over CTAs so that the grid fills the GPU; partial sums are reduced in fixed order by
+// N = up to 128 images, K split over CTAs so that the grid fills the GPU; partial sums are reduced in fixed order by
 // fc_reduce_kernel.  QCNN_FC_TC=0 keeps the gather kernel, QCNN_FC_TC=1 forces the tensor-core path for any N.
 // dst[r][c] = sum over splits of partial[split][r][c] (+ ReLU); split 0 carries the bias.  Also used by the K-split
 // convolutions of pq_gemm_tc (rows = positions).
@@ -368,12 +368,12 @@ static bool FcTcEligible(const qcnn_layer* L, int N) {
 void DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap) {
   buf[0] = 0;
   if (!FcTcEligible(L, N)) return;
-  const int NT = std::min(256, RoundUp(N, 16)), KS = 3;
+  const int NT = N > 64 ? 128 : 64, KS = 3;
   const int nct = CeilDiv(L->Dout, 128), tiles = CeilDiv(N, NT), kAll = L->Din / 8;
   int nsplit = std::max(1, L->ctx->sm_count / (tiles * nct));
   const int kPerSplit = RoundUp(CeilDiv(kAll, nsplit), KS);
   nsplit = CeilDiv(kAll, kPerSplit);
-  snprintf(buf, cap, "pq_gemm_tc(tcgen05, weights decoded into TMEM%s) mode=2 NT=%d GT=3 slots=5 grid=%d nsplit=%d ksteps=%d",
+  snprintf(buf, cap, "pq_gemm_tc(wgmma, weights decoded into registers%s) mode=2 NT=%d GT=3 grid=%d nsplit=%d ksteps=%d",
            L->opt_tc_bf ? ", bf16x2" : "", NT, tiles * nsplit * nct, nsplit, kPerSplit);
 }
 
@@ -382,7 +382,7 @@ int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
   if (!FcTcEligible(L, N)) return 0;
   qcnn_ctx* ctx = L->ctx;
   const int KS = 3;                 // k-steps per chunk (plane image of a chunk: 2 * 3 halves x NT images, hi + lo)
-  const int NTq = std::min(256, RoundUp(N, 16));
+  const int NTq = N > 64 ? 128 : 64;   // the two wgmma N of pq_gemm_tc
   const int tilesq = CeilDiv(N, NTq), nChunksAll = CeilDiv(L->Din / 8, KS);
   GemmArgs a;
   memset(&a, 0, sizeof(a));
@@ -393,10 +393,10 @@ int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
   a.srcImg = L->Din; a.dstImg = 0;
   a.IB = 1; a.PW = 1;
   a.NT = NTq;
-  a.aOff = 256; a.corr = NTq <= 128 ? 1 : 0; a.lite = 0;
-  a.bf = L->opt_tc_bf ? 1 : 0; a.wide = 0;
+  a.corr = NTq <= 64 ? 1 : 0;
+  a.bf = L->opt_tc_bf ? 1 : 0;
   if (a.bf && L->d_ctrd_bf) { a.ctrd = reinterpret_cast<const float*>(L->d_ctrd_bf); a.cbPre = 1; }   // (d % 4 == 0)
-  a.GT = 3; a.NSLOT = 5;
+  a.GT = 3;
   a.nPB = 3; a.xprep = L->d_flat; a.nChunksAll = nChunksAll;
   a.planeF4 = KS * 2 * a.NT;
   a.planeRows = a.bf ? KS * a.NT : a.planeF4;

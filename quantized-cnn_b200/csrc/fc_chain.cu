@@ -10,7 +10,7 @@
 //     layers back to back, it never waits for the arithmetic -- into a shared-memory ring with cp.async.bulk
 //     (mbarrier complete_tx); with ~150 KB of ring per SM the whole 17.7 MB of AlexNet's three FC layers is in flight
 //     from the first cycle of the kernel, so the HBM stream is not interrupted by the layer-to-layer dependency.
-//   * a CTA builds only the LUT rows of its own subspaces (its 1/148 of the codebook arrives by one bulk copy), then
+//   * a CTA builds only the LUT rows of its own subspaces (its share of the codebook, one CTA per SM, arrives by one bulk copy), then
 //     512 consumer threads gather: thread = 4/8/16 consecutive output channels, one 32/64/128-bit shared-memory load
 //     of assignment bytes per row, LUT row = one bank sweep for K <= 32 (conflict-free by construction).
 //   * a CTA's result is a partial sum over ITS subspaces for ALL output channels.  It is published to an L2-resident

@@ -1,4 +1,4 @@
-// PQ layers as decode-at-use GEMMs on the 5th-generation tensor cores, weights decoded straight into tensor memory.
+// PQ layers as decode-at-use GEMMs on the Hopper tensor cores (wgmma), weights decoded straight into registers.
 //
 //     dst[q][c] = bias[c] + sum_{k-steps} sum_{j<8}  W_kstep[c][j] * X_kstep[q][j]
 //
@@ -7,27 +7,25 @@
 // gather kernels use (reference CaffeEva::CalcFeatMap_ConvAprx / _FCntAprx + GetInPdMat, src/CaffeEva.cc:760-868,
 // 968-1025, 1261-1296, evaluated as x . (decoded w) instead of gather(LUT(x)); same sums, different association).
 //
-// Roles inside a CTA (warp-specialised, mbarrier pipelines, no CTA-wide barrier in the main loop):
-//   warps 0-3  decoders: thread = output channel (= TMEM lane).  Per k-step: index byte(s) -> codeword piece(s) from the
-//   (+ 8-11)   staged codebook slice -> tcgen05.st into the A ring in TMEM (16 columns per k-step).  Decoded weights never
-//              touch shared memory.  bf16x2 operands (default): the codebook was split into bf16 pieces {w1, w2} once at
-//              layer creation, the decoders convert nothing; conv layers: all tap indices of a chunk sit in registers
-//              (channel-major index block, one or two 128-bit loads per chunk), so a k-step costs ONE dependent
-//              shared-memory round trip (the codeword gather) -- under the MMAs' operand fetch a round trip is ~450 clk.
-//   warp 4     one elected thread issues tcgen05.mma (M = 128 channels, N = NT positions) with A in TMEM and B = the
-//              position planes in shared memory: two kind::f16 MMAs of K = 16 per k-step (bf16x2:
-//              [w1|w1].[x1|x2] + [w2|w2].[x1|x2]) or three kind::tf32 MMAs of K = 8 (3xTF32: Ah*Bh + Ah*Bl + Al*Bh).
-//   warps 5-7  stagers: the next chunk's positions go global -> registers -> planes (K-major, SWIZZLE_NONE core matrices:
-//   (+ 12-15)  8 positions x 16 B, SBO = 128 B, LBO = distance between the two halves / pieces), buffered against the MMAs
-//              of the current chunk (3x3 tiles: two register sets, loads two chunks ahead); a chunk's codebook slices and
-//              index blocks arrive by cp.async.bulk counted on the chunk's mbarrier (3xTF32: cp.async), four chunks deep.
+// Roles inside a CTA of twelve warps (warp-specialised, mbarrier pipelines, no CTA-wide barrier in the main loop):
+//   warps 0-7  two consumer warpgroups, 64 of the tile's 128 output channels each.  A thread decodes exactly the elements
+//              of the wgmma A fragment it owns (two channels x one or two value pairs per k-step): index byte -> codeword
+//              piece from the staged codebook slice -> registers, then the warpgroup issues wgmma.mma_async (M = 64,
+//              N = NT positions) with A from those registers and B = the position planes in shared memory.  Decoded
+//              weights never touch shared memory.  bf16x2 operands (default): the codebook was split into bf16 pieces
+//              {w1, w2} once at layer creation and the decoders convert nothing; per k-step two MMAs of K = 16
+//              ([w1|w1].[x1|x2] + [w2|w2].[x1|x2]).  3xTF32: three MMAs of K = 8 (Ah*Bh + Ah*Bl + Al*Bh).  Conv layers: all
+//              tap indices of a chunk sit in registers (channel-major index block, one or two 128-bit loads per chunk).
+//              A stage of up to four k-steps is decoded, issued and waited for; the two warpgroups overlap each other.
+//   warps 8-11 stagers: the next chunk's positions go global -> registers -> planes (K-major core matrices without
+//              swizzle: 8 positions x 16 B, SBO = 128 B, LBO = distance between the two halves / pieces), double-buffered
+//              against the MMAs of the current chunk; a chunk's codebook slices and index blocks arrive by
+//              cp.async.bulk counted on the chunk's mbarrier (3xTF32: cp.async), four chunks deep.
 //              FC layers: the planes were pre-split by fc_prep_kernel and arrive by one cp.async.bulk per chunk.
-//   all warps  epilogue: TMEM (lane = channel, column = position) -> + bias, ReLU -> NHWC stores (a warp writes 32
-//              consecutive channels of one position: 128 B).
-// Instantiations: 8 warps (FC tiles, 3xTF32), LITE = 8 warps at <= 128 registers, two CTAs per SM (tiles of <= 128
-// positions), WIDE = 12 warps (second decoder group; conv2-5), XL = 16 warps (second decoder group + seven stager warps;
-// conv1).  What paces the kernel is the latency of shared memory under load (MMA operand fetch + codeword gathers keep the
-// pipe 65-70 % busy), not a throughput limit: profiles/README.md, "Role cycle counters".
+//   epilogue   the consumers add the bias (+ ReLU) to their accumulator fragments and store them NHWC.
+// Instantiations: operands (bf16x2 | 3xTF32) x positions per CTA (NT = 128: one accumulator; NT = 64: the terms with a
+// low-order operand piece have an accumulator of their own, added in the epilogue -- the tensor core's accumulation
+// error grows with the number of chained MMAs per accumulator, DESIGN.md 2).
 //
 // Layer geometries are expressed as a table of k-steps (KStep: B start / half distance inside the staged planes, index
 // row and codebook slot of either half), so one main loop serves
@@ -39,6 +37,7 @@
 //           a chunk is one phase row;
 //   mode 2  fully-connected layers: position = image, a chunk is a run of k-steps over consecutive input features.
 #include "qcnn_internal.h"
+#include "wgmma.h"
 
 #include <algorithm>
 #include <cmath>
@@ -48,21 +47,16 @@
 
 namespace {
 
-constexpr int kThreads = 256;
-constexpr int kDecoders = 128;   // warps 0-3
-constexpr int kStagers = 96;     // warps 5-7
-constexpr int kStager0 = 160;
-constexpr int kMaxSlots = 5;
-constexpr int kMaxGT = 8;        // k-steps per stage (TMEM ring: NSLOT * GT * 16 columns <= 256)
-constexpr int kRegPos = 16;     // float4 a stager thread holds in registers (convolution modes: planeF4 <= 16 * 96)
-// "lite" instantiation: TWO CTAs per SM (<= 128 registers per thread, 256 TMEM columns and ~110 KB of shared memory each),
-// so that one CTA's set-up, first-plane wait and epilogue overlap the other's MMA phase -- with one CTA per SM the tensor
-// pipe idles 35-45 % of a CTA's life (profiles/README.md).  Tiles of <= 128 positions, shorter register windows.
-constexpr int kRegPosLite = 11;
-constexpr int kMaxGTLite = 4;
-constexpr int kCbBufs = 4;      // codebook / index buffers: the decoders run ahead of the position planes
+using qcnn::SmemU32;
+using qcnn::Wgmma;
 
-__device__ __forceinline__ uint32_t SmemU32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
+constexpr int kThreads = 384;
+constexpr int kConsumers = 256;  // warps 0-7
+constexpr int kStagers = 128;    // warps 8-11
+constexpr int kMaxGT = 4;        // k-steps per stage (decoded A fragments of a stage live in registers)
+constexpr int kRegPos = 12;      // float4 a stager thread holds in registers (convolution modes: planeF4 <= 12 * 128)
+constexpr int kCbBufs = 4;       // codebook / index buffers: the decoders run ahead of the position planes
+
 __device__ __forceinline__ void CpAsync16(void* smemDst, const void* gsrc, bool valid) {
   const int sz = valid ? 16 : 0;  // src-size 0: nothing is read, the 16 destination bytes are zero-filled
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(SmemU32(smemDst)), "l"(gsrc), "r"(sz) : "memory");
@@ -85,45 +79,14 @@ __device__ __forceinline__ void MbarWait(uint64_t* mbar, uint32_t parity) {
     if (spins > (1u << 24)) __trap();
   }
 }
-__device__ __forceinline__ void UmmaCommit(uint64_t* mbar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(SmemU32(mbar)) : "memory");
-}
-// one lane of the (converged) warp
-__device__ __forceinline__ bool ElectOne() {
-  uint32_t pred = 0;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-// D[tmem] (+)= A[tmem] * B[smem descriptor]
-__device__ __forceinline__ void UmmaTf32Ts(uint32_t tmemD, uint32_t tmemA, uint64_t descB, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmemD), "r"(tmemA), "l"(descB),
-               "r"(idesc), "r"(accumulate) : "memory");
-}
 // 3xTF32 operand split: hi = v truncated to tf32 (what the tensor core reads), lo = exact remainder (the tensor core
-// truncates it to tf32 in turn).  Rounding both pieces to nearest instead was measured to change the end error by < 10 %:
-// the error of this path (1e-5 .. 2e-5 of max|out| per layer, ~n * 2^-24) comes from the tensor core's fp32
-// ACCUMULATION over the n = 3 * k-steps chained MMAs, not from the operand representation (tools/accuracy.py).
+// truncates it to tf32 in turn).  The error of this path grows with the tensor core's fp32 ACCUMULATION over the
+// n = 3 * k-steps chained MMAs (~n * 2^-24), not with the operand representation (tools/accuracy.py measures it).
 __device__ __forceinline__ void SplitTf32x4(const float4 v, float4& hi, float4& lo) {
   hi.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); lo.x = v.x - hi.x;
   hi.y = __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u); lo.y = v.y - hi.y;
   hi.z = __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); lo.z = v.z - hi.z;
   hi.w = __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u); lo.w = v.w - hi.w;
-}
-
-// one k-step of decoded weights (two 4-float halves) -> hi | lo -> 16 TMEM columns of this thread's lane
-__device__ __forceinline__ void StoreWeights(uint32_t taddr, const float4 w0, const float4 w1) {
-  float4 h0, l0, h1, l1;
-  SplitTf32x4(w0, h0, l0);
-  SplitTf32x4(w1, h1, l1);
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-               "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-               :: "r"(taddr),
-                  "r"(__float_as_uint(h0.x)), "r"(__float_as_uint(h0.y)), "r"(__float_as_uint(h0.z)), "r"(__float_as_uint(h0.w)),
-                  "r"(__float_as_uint(h1.x)), "r"(__float_as_uint(h1.y)), "r"(__float_as_uint(h1.z)), "r"(__float_as_uint(h1.w)),
-                  "r"(__float_as_uint(l0.x)), "r"(__float_as_uint(l0.y)), "r"(__float_as_uint(l0.z)), "r"(__float_as_uint(l0.w)),
-                  "r"(__float_as_uint(l1.x)), "r"(__float_as_uint(l1.y)), "r"(__float_as_uint(l1.z)), "r"(__float_as_uint(l1.w))
-               : "memory");
 }
 
 // ---- bf16x2 operands: v = v1 + v2 with v1 = bf16(v), v2 = bf16(v - v1) (|v - v1 - v2| <= 2^-18 |v|).  One k-step of
@@ -142,31 +105,6 @@ __device__ __forceinline__ void SplitBf16x4(const float4 v, uint2& p1, uint2& p2
   const float rz = v.z - __uint_as_float(p1.y << 16), rw = v.w - __uint_as_float(p1.y & 0xFFFF0000u);
   p2.x = PackBf16x2(rx, ry);
   p2.y = PackBf16x2(rz, rw);
-}
-// one k-step of decoded weights -> [w1 | w1 | w2 | w2] (8 bf16 = 4 columns each) -> 16 TMEM columns of this thread's lane.
-// PRE: the staged codebook already holds {w1, w2} per 4-float piece (qcnn_layer::d_ctrd_bf, split once at layer creation):
-// the decoders convert nothing; otherwise split here.
-template <bool PRE>
-__device__ __forceinline__ void StoreWeightsBf(uint32_t taddr, const float4 w0, const float4 w1) {
-  uint2 a1, a2, b1, b2;
-  if (PRE) {
-    a1 = make_uint2(__float_as_uint(w0.x), __float_as_uint(w0.y)); a2 = make_uint2(__float_as_uint(w0.z), __float_as_uint(w0.w));
-    b1 = make_uint2(__float_as_uint(w1.x), __float_as_uint(w1.y)); b2 = make_uint2(__float_as_uint(w1.z), __float_as_uint(w1.w));
-  } else {
-    SplitBf16x4(w0, a1, a2);
-    SplitBf16x4(w1, b1, b2);
-  }
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-               "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-               :: "r"(taddr),
-                  "r"(a1.x), "r"(a1.y), "r"(b1.x), "r"(b1.y), "r"(a1.x), "r"(a1.y), "r"(b1.x), "r"(b1.y),
-                  "r"(a2.x), "r"(a2.y), "r"(b2.x), "r"(b2.y), "r"(a2.x), "r"(a2.y), "r"(b2.x), "r"(b2.y)
-               : "memory");
-}
-__device__ __forceinline__ void UmmaF16Ts(uint32_t tmemD, uint32_t tmemA, uint64_t descB, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(tmemD), "r"(tmemA), "l"(descB),
-               "r"(idesc), "r"(accumulate) : "memory");
 }
 
 // fp32 codebook [S][K][P pieces of 4 floats] -> [S][P][K] x {w1, w2}: the K pieces of one (subspace, piece) are contiguous
@@ -202,44 +140,36 @@ __device__ __forceinline__ int ByteOf48(const uint4 q0, const uint4 q1, const ui
 }
 
 struct SmemMap {  // byte offsets inside the dynamic shared memory
-  int planes, cbs, ids, tab, posoff, posrow, posdst, outoff, bias, bars, tmem, total;
+  int planes, cbs, ids, tab, posoff, posrow, posdst, outoff, bias, bars, total;
 };
 __host__ __device__ inline SmemMap MapSmem(const GemmArgs& a) {
   SmemMap m;
   int o = 0;
   m.planes = o; o += a.nPB * 2 * a.planeRows * 16;      // [buf][hi,lo | x1,x2][planeRows] 16-byte rows
-  m.cbs = o;    o += kCbBufs * a.cbSlots * a.cbF4 * 16; // [cbuf][slot][cbF4] codeword pieces (raw fp32)
+  m.cbs = o;    o += kCbBufs * a.cbSlots * a.cbF4 * 16; // [cbuf][slot][cbF4] codeword pieces
   m.ids = o;    o += kCbBufs * a.idRows * 128;          // [cbuf][row][128 channels] assignment indices
   m.tab = o;    o += a.ntab * 16;                       // k-step table for the decoders that do not keep their indices in registers
   m.posoff = o; o += a.planeF4 * 4;                     // source element offset of every staged float4 (-1: zero)
   m.posrow = o; o += a.mode == 1 ? a.planeF4 * 4 : 0;   // mode 1: first input row of the position (phase row 0)
   m.posdst = o; o += (a.bf && a.mode != 2) ? a.planeF4 * 4 : 0;   // bf16x2: byte offset of every staged float4 inside a plane
-  m.outoff = o; o += 256 * 4;                           // destination element offset of every position (-1: none)
+  m.outoff = o; o += 128 * 4;                           // destination element offset of every position (-1: none)
   m.bias = o;   o += 128 * 4;
-  m.bars = o;   o += 8 * (2 * kMaxSlots + 2 * kCbBufs + 9);
-  m.tmem = o;   o += 16;
+  m.bars = o;   o += 8 * (8 + 2 * kCbBufs);
   m.total = o;
   return m;
 }
 
-// DBG: cycle counters of the three roles (QCNN_GEMM_DBG=1) -- a separate instantiation, the production kernel reads no clocks
-// WIDE: a SECOND group of four decoder warps (warps 8-11; 384 threads): the two groups take the stages alternately.  The
-// decoders -- one warp per SM sub-partition, a chain of dependent shared-memory reads, the split and a tcgen05.st per
-// k-step -- are what paces the kernel (~400 clk per k-step against 384 clk of 3xTF32 MMAs or 256 clk of bf16x2 MMAs).
-// XL: sixteen warps (512 threads, <= 128 registers): two decoder groups AND seven stager warps (5-7, 12-15) -- conv1's tiles
-// (16-18 k-steps per phase row, four phase columns of 3-channel pixels to stage per row) need both to keep the MMAs fed.
-template <bool DBG, bool LITE, bool BF, bool WIDE, bool XL = false>
-__global__ void __launch_bounds__(XL ? 512 : (WIDE ? 384 : kThreads), LITE ? 2 : 1) pq_gemm_tc_kernel(const GemmArgs a) {
-  constexpr int NTHR = XL ? 512 : (WIDE ? 384 : kThreads);
-  constexpr int NSTG = XL ? kStagers + 128 : kStagers;      // stager threads
-  constexpr bool TWOG = WIDE || XL;                          // two decoder groups (warps 0-3 and 8-11)
-  constexpr int RP = XL ? 7 : ((LITE || WIDE) ? kRegPosLite : kRegPos);
-  constexpr int MG = (LITE || XL) ? kMaxGTLite : (WIDE ? 5 : kMaxGT);
-  constexpr uint32_t kTmemCols = LITE ? 256u : 512u;
+// BF: bf16x2 operands (else 3xTF32); NT: positions per CTA = wgmma N; NT = 64 keeps the second accumulator (a.corr)
+template <bool BF, int NT>
+__global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_kernel(const GemmArgs a) {
+  constexpr int NTHR = kThreads;
+  constexpr int NSTG = kStagers;
+  constexpr int RP = kRegPos;
+  constexpr bool CORR = NT <= 64;
   extern __shared__ __align__(128) unsigned char smem[];
   const SmemMap sm = MapSmem(a);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int K = a.K, NT = a.NT, GT = a.GT, NSLOT = a.NSLOT;
+  const int K = a.K, GT = a.GT;
 
   float4* planes = reinterpret_cast<float4*>(smem + sm.planes);
   float4* cbs = reinterpret_cast<float4*>(smem + sm.cbs);
@@ -250,15 +180,10 @@ __global__ void __launch_bounds__(XL ? 512 : (WIDE ? 384 : kThreads), LITE ? 2 :
   int* posdst = reinterpret_cast<int*>(smem + sm.posdst);
   int* outoff = reinterpret_cast<int*>(smem + sm.outoff);
   float* biasS = reinterpret_cast<float*>(smem + sm.bias);
-  uint64_t* fullA = reinterpret_cast<uint64_t*>(smem + sm.bars);   // [kMaxSlots] decoders -> issuer
-  uint64_t* emptyA = fullA + kMaxSlots;                            // [kMaxSlots] MMAs retired -> decoders
-  uint64_t* fullB = emptyA + kMaxSlots;                            // [<=4] position planes: stagers -> issuer
+  uint64_t* fullB = reinterpret_cast<uint64_t*>(smem + sm.bars);   // [<=4] position planes: stagers -> consumers
   uint64_t* emptyB = fullB + 4;                                    // [<=4] chunk's MMAs retired -> stagers
-  uint64_t* fullC = emptyB + 4;                                    // [kCbBufs] codebook + indices: stagers -> decoders
-  uint64_t* emptyC = fullC + kCbBufs;                              // [kCbBufs] decoders done with the chunk -> stagers
-  uint64_t* doneBar = emptyC + kCbBufs;
-  uint32_t* tmemBase = reinterpret_cast<uint32_t*>(smem + sm.tmem);
-
+  uint64_t* fullC = emptyB + 4;                                    // [kCbBufs] codebook + indices: stagers -> consumers
+  uint64_t* emptyC = fullC + kCbBufs;                              // [kCbBufs] consumers done with the chunk -> stagers
   int b = blockIdx.x;
   const int ct = b % a.nct; b /= a.nct;
   int g = 0, split = 0;
@@ -313,7 +238,7 @@ __global__ void __launch_bounds__(XL ? 512 : (WIDE ? 384 : kThreads), LITE ? 2 :
       posdst[p] = a.mode == 0 ? pos * 16 + grp * 8 : ((grp >> 1) * a.NPOS + pos) * 16 + (grp & 1) * 8;
     }
   }
-  for (int p = tid; p < 256; p += NTHR) {
+  for (int p = tid; p < 128; p += NTHR) {
     int off = -1;
     if (p < NT) {
       const int Q = Q0 + p;
@@ -327,27 +252,17 @@ __global__ void __launch_bounds__(XL ? 512 : (WIDE ? 384 : kThreads), LITE ? 2 :
   if (a.mode == 1 && a.bulkC)      // slot 1 (unpaired taps) stays zero; slot 0 arrives by bulk copy
     for (int e = tid; e < kCbBufs * K; e += NTHR) cbs[(e / K) * a.cbSlots * K + K + (e % K)] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
   for (int c = tid; c < 128; c += NTHR) biasS[c] = (c < CTv && split == 0) ? __ldg(a.bias + g * a.Kg + ch0 + c) : 0.0f;
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(SmemU32(tmemBase)), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (tid == 0) {
-    for (int i = 0; i < kMaxSlots; i++) { MbarInit(fullA + i, kDecoders); MbarInit(emptyA + i, 1); }
-    for (int i = 0; i < 4; i++) { MbarInit(fullB + i, NSTG); MbarInit(emptyB + i, 1); }
-    for (int i = 0; i < kCbBufs; i++) { MbarInit(fullC + i, a.bulkC ? 1 : NSTG); MbarInit(emptyC + i, TWOG ? 2 * kDecoders : kDecoders); }
-    MbarInit(doneBar, 1);
+    for (int i = 0; i < 4; i++) { MbarInit(fullB + i, NSTG); MbarInit(emptyB + i, kConsumers / 32); }
+    for (int i = 0; i < kCbBufs; i++) { MbarInit(fullC + i, a.bulkC ? 1 : NSTG); MbarInit(emptyC + i, kConsumers / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmemD = *tmemBase;          // D: columns [0, NT)
-  const uint32_t tmemA = tmemD + static_cast<uint32_t>(a.aOff);   // A ring: columns [aOff, aOff + NSLOT*GT*16)
 
   const int warpU = __shfl_sync(0xffffffffu, warp, 0);   // provably warp-uniform role selector
-  if ((warpU >= 5 && warpU < 8) || (XL && warpU >= 12)) {
+  if (warpU >= kConsumers / 32) {
     // =========================== stagers ===========================
-    const int st = warpU < 8 ? tid - kStager0 : kStagers + tid - 384;
+    const int st = tid - kConsumers;
     const int sw = st >> 5;                      // stager warp 0 .. NSTG/32 - 1
     // 4-float piece j0/4 of codeword k of subspace s: fp32 codebook [S][K][d] or the pre-split one [S][d/4][K][4 words]
     auto piece = [&](int s, int j0, int k) -> const float* {
@@ -488,8 +403,8 @@ __global__ void __launch_bounds__(XL ? 512 : (WIDE ? 384 : kThreads), LITE ? 2 :
       CpAsyncCommit();
     };
     // Positions of the convolution modes: global -> registers -> hi/lo planes.  (16-byte cp.async of scattered pieces
-    // costs one shared-memory wavefront per THREAD -- profiles/README.md, "staging" -- whereas a 128-bit store of 32
-    // consecutive float4 costs four per warp.)  A thread owns float4 st, st+96, ...: at most kRegPos of them.
+    // costs one shared-memory wavefront per THREAD, whereas a 128-bit store of 32 consecutive float4 costs four per
+    // warp.)  A thread owns float4 st, st + kStagers, ...: at most kRegPos of them.
     float4 rg[RP];
     int poffR[RP];        // chunk-invariant source offset of the thread's float4 (mode 0: incl. the half's +4)
     int prowR[RP];        // mode 1: first input row (phase row 0), very negative when the column is outside
@@ -542,100 +457,18 @@ __global__ void __launch_bounds__(XL ? 512 : (WIDE ? 384 : kThreads), LITE ? 2 :
         }
       }
     };
-    long long sCp = 0, sEB = 0, sEC = 0, sT0 = (DBG ? clock64() : 0ll);
-    // Twelve-warp tiles of 3x3 layers (<= 6 float4 per stager thread, chunks of 9 k-steps): TWO register sets, the loads of
-    // chunk kc+2 are issued right after the stores of chunk kc, so a global-load latency (~1-1.5 k clk under load) overlaps
-    // a whole chunk instead of being waited for in every iteration -- with one set the stagers, not the MMAs, paced these
-    // layers (role counters: 3.8 k clk per chunk against 2.4 k clk of MMAs).
-    constexpr int H = 6;
-    const bool dbl = WIDE && a.mode == 0 && a.planeF4 <= H * NSTG;
-    if (WIDE && dbl) {
-      float4 rg2[WIDE ? H : 1];
-      int pdst[WIDE ? H : 1];           // bf16x2: byte offset of the element inside a plane (chunk-invariant)
-#pragma unroll
-      for (int i = 0; i < H; i++) {
-        const int p = st + i * NSTG;
-        const int grp = p >= a.NPOS ? 1 : 0;
-        pdst[i] = (p - grp * a.NPOS) * 16 + grp * 8;
-      }
-      auto loadH = [&](int kc, auto& r) {
-        const int chA = (kcBase + kc) * 8;
-        uint32_t m = pvalid;
-        if (chA >= a.Cg) m = 0;
-        else if (chA + 4 >= a.Cg) m &= ~phalf;
-        const float* srcG = srcBase + g * a.Cg + chA;
-#pragma unroll
-        for (int i = 0; i < H; i++) {
-          r[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-          if ((m >> i) & 1u) r[i] = __ldg(reinterpret_cast<const float4*>(srcG + poffR[i]));
-        }
-      };
-      auto iter = [&](int kc, auto& r) {
-        const int buf = kc % a.nPB;
-        long long c0 = (DBG ? clock64() : 0ll);
-        if (!a.bulkC) {
-          if (kc + 1 < nChunks) asm volatile("cp.async.wait_group 1;" ::: "memory");
-          else CpAsyncWaitAll();
-          sCp += (DBG ? clock64() : 0ll) - c0;
-          MbarArrive(fullC + kc % kCbBufs);
-        }
-        c0 = (DBG ? clock64() : 0ll);
-        if (kc >= a.nPB) MbarWait(emptyB + buf, ((kc / a.nPB) - 1) & 1);
-        sEB += (DBG ? clock64() : 0ll) - c0;
-        float4* pHi = planes + (buf * 2 + 0) * a.planeRows;
-        float4* pLo = planes + (buf * 2 + 1) * a.planeRows;
-#pragma unroll
-        for (int i = 0; i < H; i++) {
-          const int p = st + i * NSTG;
-          if (p < a.planeF4) {
-            if (BF) {
-              uint2 p1, p2;
-              SplitBf16x4(r[i], p1, p2);
-              *reinterpret_cast<uint2*>(reinterpret_cast<char*>(pHi) + pdst[i]) = p1;
-              *reinterpret_cast<uint2*>(reinterpret_cast<char*>(pLo) + pdst[i]) = p2;
-            } else {
-              float4 hi, lo;
-              SplitTf32x4(r[i], hi, lo);
-              pHi[p] = hi;
-              pLo[p] = lo;
-            }
-          }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        MbarArrive(fullB + buf);
-        if (kc + 2 < nChunks) {
-          loadH(kc + 2, r);
-          const int nb = (kc + 2) % kCbBufs;
-          c0 = (DBG ? clock64() : 0ll);
-          if (kc + 2 >= kCbBufs) MbarWait(emptyC + nb, (((kc + 2) / kCbBufs) - 1) & 1);
-          sEC += (DBG ? clock64() : 0ll) - c0;
-          fetchChunk(kc + 2);
-        }
-      };
-      fetchChunk(0);
-      loadH(0, rg);
-      if (nChunks > 1) { fetchChunk(1); loadH(1, rg2); }
-      for (int kc = 0; kc < nChunks; kc += 2) {
-        iter(kc, rg);
-        if (kc + 1 < nChunks) iter(kc + 1, rg2);
-      }
-    } else {
     fetchChunk(0);
     if (a.mode != 2) loadPos(0);
     if (nChunks > 1) fetchChunk(1);
     for (int kc = 0; kc < nChunks; kc++) {
       const int buf = kc % a.nPB;
-      long long c0 = (DBG ? clock64() : 0ll);
       if (!a.bulkC) {
         if (kc + 1 < nChunks) asm volatile("cp.async.wait_group 1;" ::: "memory");   // chunk kc landed, kc+1 may be in flight
         else CpAsyncWaitAll();
-        // (each stager arrives after its own copies have landed; the barrier completes when all 96 have)
-        sCp += (DBG ? clock64() : 0ll) - c0;
-        MbarArrive(fullC + kc % kCbBufs);                  // the decoders may start on chunk kc
+        // (each stager arrives after its own copies have landed; the barrier completes when all of them have)
+        MbarArrive(fullC + kc % kCbBufs);                  // the consumers may start on chunk kc
       }
-      c0 = (DBG ? clock64() : 0ll);
       if (kc >= a.nPB) MbarWait(emptyB + buf, ((kc / a.nPB) - 1) & 1);   // planes last read by the MMAs of chunk kc-nPB
-      sEB += (DBG ? clock64() : 0ll) - c0;
       float4* pHi = planes + (buf * 2 + 0) * a.planeRows;
       float4* pLo = planes + (buf * 2 + 1) * a.planeRows;
       if (a.mode == 2) {
@@ -669,312 +502,194 @@ __global__ void __launch_bounds__(XL ? 512 : (WIDE ? 384 : kThreads), LITE ? 2 :
             }
           }
         }
-      }
-      if (a.mode != 2) {
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // planes are read by the tensor core
         MbarArrive(fullB + buf);
         if (kc + 1 < nChunks) loadPos(kc + 1);
       }
       if (kc + 2 < nChunks) {
         const int nb = (kc + 2) % kCbBufs;
-        c0 = (DBG ? clock64() : 0ll);
         if (kc + 2 >= kCbBufs) MbarWait(emptyC + nb, (((kc + 2) / kCbBufs) - 1) & 1);
-        sEC += (DBG ? clock64() : 0ll) - c0;
         fetchChunk(kc + 2);
       }
     }
-    }
-    if (DBG && a.dbg && st == 0) {
-      atomicAdd(a.dbg + 8, static_cast<unsigned long long>((DBG ? clock64() : 0ll) - sT0));
-      atomicAdd(a.dbg + 9, static_cast<unsigned long long>(sCp));
-      atomicAdd(a.dbg + 10, static_cast<unsigned long long>(sEB));
-      atomicAdd(a.dbg + 11, static_cast<unsigned long long>(sEC));
-    }
-  } else if (warpU == 4) {
-    // =========================== MMA issuer ===========================
-    // The whole warp runs the loop on warp-uniform values (k-step table read from the kernel parameters, i.e. the
-    // constant bank, so descriptors stay in uniform registers); one elected lane issues the tcgen05 instructions.
-    // (Issued from a single divergent thread, every UTCHMMA is wrapped in an ELECT / BRA.U.ANY loop with R2UR moves; in
-    //  this form the SASS issues them back to back -- profiles/README.md, "MMA issue".)
-    {
-      // instruction descriptor: D = F32, A = B = TF32, K-major, N = NT, M = 128
-      // (bf16x2: A = B = BF16, format code 1; same N / M fields)
-      const uint32_t idesc = BF ? ((1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(NT >> 3) << 17) | (8u << 24))
-                                : ((1u << 4) | (2u << 7) | (2u << 10) | (static_cast<uint32_t>(NT >> 3) << 17) | (8u << 24));
-      const uint64_t descFixed = (static_cast<uint64_t>(8) << 32) | (static_cast<uint64_t>(1) << 46);  // SBO = 128 B
-      const uint32_t planes0 = SmemU32(planes);
-      int t = 0, islot = 0, iround = 0;
-      uint32_t acc = 0;
-      // NT <= 128 leaves room for a second accumulator: the hi*hi products go to D, the two cross terms to D + NT, and
-      // the epilogue adds them -- the tensor core's accumulation error grows with the number of chained MMAs per
-      // accumulator (DESIGN.md 2), and the chain of the dominant term is three times shorter this way
-      const uint32_t corrOff = a.corr ? static_cast<uint32_t>(NT) : 0u;
-      uint32_t accCorr = 0;
-      long long wBC = 0, wA = 0, tStart = (DBG ? clock64() : 0ll);
-      for (int kc = 0; kc < nChunks; kc++) {
-        const int buf = kc % a.nPB;
-        long long c0 = (DBG ? clock64() : 0ll);
-        MbarWait(fullB + buf, (kc / a.nPB) & 1);
-        wBC += (DBG ? clock64() : 0ll) - c0;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t dHi = descFixed | (((planes0 + static_cast<uint32_t>((buf * 2 + 0) * a.planeRows) * 16u) >> 4) & 0x3FFFu);
-        const uint64_t dLo = descFixed | (((planes0 + static_cast<uint32_t>((buf * 2 + 1) * a.planeRows) * 16u) >> 4) & 0x3FFFu);
-        const int e0 = a.chunkFirst[a.mode == 1 ? kcBase + kc : 0];
-        const int ne = a.mode == 2 ? min(a.chunkCount[0], kTotal - kc * a.chunkCount[0]) : a.chunkCount[a.mode == 1 ? kcBase + kc : 0];
-        for (int s0 = 0; s0 < ne; s0 += GT, t++) {
-          const int slot = islot;                         // = t % NSLOT, ring round = t / NSLOT (kept incrementally)
-          c0 = (DBG ? clock64() : 0ll);
-          MbarWait(fullA + slot, iround & 1);
-          if (++islot == NSLOT) { islot = 0; iround++; }
-          wA += (DBG ? clock64() : 0ll) - c0;
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const int n = min(GT, ne - s0);
-          if (ElectOne()) {
-            for (int i = 0; i < n; i++) {
-              const KStep ks = a.tab[e0 + s0 + i];
-              const uint64_t off = static_cast<uint64_t>(static_cast<uint32_t>(ks.bStart)) |
-                                   (static_cast<uint64_t>(static_cast<uint32_t>(ks.lbo)) << 16);
-              const uint32_t aHi = tmemA + static_cast<uint32_t>((slot * GT + i) * 16), aLo = aHi + 8;
-              if (BF) {
-                // B = [x1 | x2]: K-core-matrix 0 in the first plane, 1 in the second (the table's lbo is the plane distance);
-                // A = [w1 | w1] then [w2 | w2] (columns 0-7 / 8-15 of the slot)
-                UmmaF16Ts(tmemD, aHi, dHi + off, idesc, acc);
-                UmmaF16Ts(tmemD + corrOff, aLo, dHi + off, idesc, corrOff ? accCorr : 1u);
-              } else {
-                UmmaTf32Ts(tmemD, aHi, dHi + off, idesc, acc);
-                UmmaTf32Ts(tmemD + corrOff, aHi, dLo + off, idesc, corrOff ? accCorr : 1u);
-                UmmaTf32Ts(tmemD + corrOff, aLo, dHi + off, idesc, 1u);
-              }
-              acc = 1u;
-              accCorr = 1u;
-            }
-            // commits are issued by the thread that issued the MMAs they track
-            UmmaCommit(emptyA + slot);
-            if (s0 + GT >= ne) {
-              UmmaCommit(emptyB + buf);
-              if (kc == nChunks - 1) UmmaCommit(doneBar);
-            }
-          }
-          acc = 1u;
-          accCorr = 1u;
-          __syncwarp();
-        }
-      }
-      if (DBG && a.dbg && lane == 0) {
-        const long long tIssue = (DBG ? clock64() : 0ll) - tStart;
-        long long c0 = (DBG ? clock64() : 0ll);
-        MbarWait(doneBar, 0);
-        atomicAdd(a.dbg + 0, static_cast<unsigned long long>(tIssue));
-        atomicAdd(a.dbg + 1, static_cast<unsigned long long>(wBC));
-        atomicAdd(a.dbg + 2, static_cast<unsigned long long>(wA));
-        atomicAdd(a.dbg + 3, static_cast<unsigned long long>((DBG ? clock64() : 0ll) - c0));
-        atomicAdd(a.dbg + 5, 1ull);
-      }
-    }
-  } else {
-    // =========================== decoders ===========================
-    const int c = (warp & 3) * 32 + lane;           // channel row = TMEM lane (a warp reaches the lanes of its sub-partition)
-    const int cc = min(c, CTv - 1);                 // rows beyond the valid channels decode a copy (never stored)
-    const uint32_t laneBase = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    const int grp = (TWOG && warp >= 8) ? 1 : 0;    // WIDE: group 0 decodes the even stages, group 1 the odd ones
-    const bool pre = BF && a.cbPre != 0;
-    int t = 0, dslot = 0, dround = 0;
-    long long dP1 = 0, dP2 = 0, dP3 = 0, dP4 = 0, dP3s = 0;   // DBG: index loads / codeword loads / split + tcgen05.st issue / wait::st
-    long long dFC = 0, dEA = 0, dT0 = (DBG ? clock64() : 0ll);
-    for (int kc = 0; kc < nChunks; kc++) {
-      const int cbuf = kc % kCbBufs;
-      long long c0 = (DBG ? clock64() : 0ll);
-      MbarWait(fullC + cbuf, (kc / kCbBufs) & 1);
-      dFC += (DBG ? clock64() : 0ll) - c0;
-      const uint8_t* idb = ids + cbuf * a.idRows * 128 + cc;
-      const float4* cb = cbs + cbuf * a.cbSlots * a.cbF4;
-      const float* cbf = reinterpret_cast<const float*>(cb);
-      const int e0 = a.chunkFirst[a.mode == 1 ? kcBase + kc : 0];
-      const int ne = a.mode == 2 ? min(a.chunkCount[0], kTotal - kc * a.chunkCount[0]) : a.chunkCount[a.mode == 1 ? kcBase + kc : 0];
-      // idxT: every tap index of this channel for the chunk's two halves in registers (one or two 128-bit loads each): the
-      // per-k-step chain loses two dependent shared-memory round trips (table entry, index byte) -- under the load of the
-      // MMAs' operand fetch a round trip costs ~450 clk (role counters, profiles/README.md)
-      uint4 iA0 = make_uint4(0, 0, 0, 0), iA1 = iA0, iB0 = iA0, iB1 = iA0;
-      if (a.idxT) {
-        const uint4* ip = reinterpret_cast<const uint4*>(ids + cbuf * a.idRows * 128);
-        const int W = a.tapsPad >> 4;
-        iA0 = ip[cc * W];
-        if (a.mode == 1) {          // one block of <= 48 rows: iA0, iA1, iB0
-          if (W > 1) iA1 = ip[cc * W + 1];
-          if (W > 2) iB0 = ip[cc * W + 2];
-        } else {
-          iB0 = ip[(128 + cc) * W];
-          if (W > 1) { iA1 = ip[cc * W + 1]; iB1 = ip[(128 + cc) * W + 1]; }
-        }
-      }
-      for (int s0 = 0; s0 < ne; s0 += GT, t++) {
-        const int slot = dslot, round = dround;           // = t % NSLOT, t / NSLOT (kept incrementally: no divisions)
-        if (++dslot == NSLOT) { dslot = 0; dround++; }
-        if (TWOG && (t & 1) != grp) continue;
-        if (round > 0) {
-          c0 = (DBG ? clock64() : 0ll);
-          MbarWait(emptyA + slot, (round - 1) & 1);
-          dEA += (DBG ? clock64() : 0ll) - c0;
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-        const int n = min(GT, ne - s0);
-        if (a.d == 1) {
-          for (int i = 0; i < n; i++) {
-            // scalar codewords: every feature is its own subspace (rows / slots idx0 .. idx0+3 and idx1 .. idx1+3)
-            const KStep ks = tabS[e0 + s0 + i];
-            const uint8_t* r0 = idb + ks.idx0 * 128;
-            const uint8_t* r1 = idb + ks.idx1 * 128;
-            const float* c0p = cbf + ks.cb0 * K;
-            const float* c1p = cbf + ks.cb1 * K;
-            float4 w0, w1;
-            w0.x = c0p[r0[0] >> a.kshift];           w0.y = c0p[K + (r0[128] >> a.kshift)];
-            w0.z = c0p[2 * K + (r0[256] >> a.kshift)]; w0.w = c0p[3 * K + (r0[384] >> a.kshift)];
-            w1.x = c1p[r1[0] >> a.kshift];           w1.y = c1p[K + (r1[128] >> a.kshift)];
-            w1.z = c1p[2 * K + (r1[256] >> a.kshift)]; w1.w = c1p[3 * K + (r1[384] >> a.kshift)];
-            if (BF) StoreWeightsBf<false>(tmemA + laneBase + static_cast<uint32_t>((slot * GT + i) * 16), w0, w1);
-            else StoreWeights(tmemA + laneBase + static_cast<uint32_t>((slot * GT + i) * 16), w0, w1);
-          }
-        } else {
-          // the stage's k-steps are independent: table entries, index bytes and codeword pieces of all of them are in
-          // flight together (one decoder warp per SM sub-partition: latency, not bandwidth, paces this role)
-          int i0x[MG], i1x[MG];
-          long long p0 = (DBG ? clock64() : 0ll);
-          // (the operand-source choice is hoisted out of the unrolled loops: inside them it would serialise the loads)
-          if (a.idxT && a.mode == 1) {     // rows and codebook slots from the k-step table (constant bank), bytes from registers
-#pragma unroll
-            for (int i = 0; i < MG; i++) {
-              if (i < n) {
-                const KStep ks = a.tab[e0 + s0 + i];
-                i0x[i] = ks.cb0 * K + ByteOf48(iA0, iA1, iB0, ks.idx0);
-                i1x[i] = ks.cb1 * K + ByteOf48(iA0, iA1, iB0, ks.idx1);
-              }
-            }
-          } else if (a.idxT) {             // mode 0: k-step = tap s0 + i, codebook slots 0 / 1
-#pragma unroll
-            for (int i = 0; i < MG; i++) {
-              if (i < n) {
-                i0x[i] = ByteOf32(iA0, iA1, s0 + i);
-                i1x[i] = K + ByteOf32(iB0, iB1, s0 + i);
-              }
-            }
-          } else {                         // table entries and index bytes of all k-steps in flight together
-            KStep ks[MG];
-#pragma unroll
-            for (int i = 0; i < MG; i++)
-              if (i < n) ks[i] = tabS[e0 + s0 + i];
-#pragma unroll
-            for (int i = 0; i < MG; i++) {
-              if (i < n) {
-                i0x[i] = ks[i].cb0 * K + (idb[ks[i].idx0 * 128] >> a.kshift);
-                i1x[i] = ks[i].cb1 * K + (idb[ks[i].idx1 * 128] >> a.kshift);
-              }
-            }
-          }
-          if (DBG) { asm volatile("" :: "r"(i0x[0]), "r"(i1x[0]) : "memory"); dP1 += clock64() - p0; p0 = clock64(); }
-          float4 w0[MG], w1[MG];
-#pragma unroll
-          for (int i = 0; i < MG; i++) {
-            if (i < n) { w0[i] = cb[i0x[i]]; w1[i] = cb[i1x[i]]; }
-          }
-          if (DBG) { asm volatile("" :: "f"(w0[0].x), "f"(w1[0].x) : "memory"); dP2 += clock64() - p0; dP3s = clock64(); }
-#pragma unroll
-          for (int i = 0; i < MG; i++) {
-            if (i < n) {
-              if (BF && pre) StoreWeightsBf<true>(tmemA + laneBase + static_cast<uint32_t>((slot * GT + i) * 16), w0[i], w1[i]);
-              else if (BF) StoreWeightsBf<false>(tmemA + laneBase + static_cast<uint32_t>((slot * GT + i) * 16), w0[i], w1[i]);
-              else StoreWeights(tmemA + laneBase + static_cast<uint32_t>((slot * GT + i) * 16), w0[i], w1[i]);
-            }
-          }
-        }
-        if (DBG) { dP3 += clock64() - dP3s; dP3s = clock64(); }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        if (DBG) { dP4 += clock64() - dP3s; }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        MbarArrive(fullA + slot);
-      }
-      MbarArrive(emptyC + cbuf);
-    }
-    if (DBG && a.dbg && tid == 0) {
-      atomicAdd(a.dbg + 12, static_cast<unsigned long long>((DBG ? clock64() : 0ll) - dT0));
-      atomicAdd(a.dbg + 13, static_cast<unsigned long long>(dFC));
-      atomicAdd(a.dbg + 14, static_cast<unsigned long long>(dEA));
-      atomicAdd(a.dbg + 4, static_cast<unsigned long long>(dP1));
-      atomicAdd(a.dbg + 6, static_cast<unsigned long long>(dP2));
-      atomicAdd(a.dbg + 7, static_cast<unsigned long long>(dP3));
-      atomicAdd(a.dbg + 15, static_cast<unsigned long long>(dP4));
-    }
+    return;
   }
 
-  // ---- epilogue: TMEM (lane = channel, column = position) -> + bias, ReLU -> NHWC global ----
-  MbarWait(doneBar, 0);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  {
-    const int q = warp & 3, hsel = warp >> 2;     // (warps 4-7 and, WIDE, 8-11 take the other position blocks)
-    const int c = q * 32 + lane;
-    const bool chOk = c < CTv;
-    const float bv = biasS[c];
-    const int nblk = NT >> 4;   // 16-position blocks
-    for (int blk = hsel; blk < nblk; blk += NTHR / 128) {
-      uint32_t r[16];
-      const uint32_t taddr = tmemD + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(blk * 16);
-      asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                   "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                   : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                     "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                   : "r"(taddr) : "memory");
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (a.corr) {   // second accumulator (cross terms of the 3xTF32 split)
-        uint32_t r2[16];
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                     "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                     : "=r"(r2[0]), "=r"(r2[1]), "=r"(r2[2]), "=r"(r2[3]), "=r"(r2[4]), "=r"(r2[5]), "=r"(r2[6]), "=r"(r2[7]),
-                       "=r"(r2[8]), "=r"(r2[9]), "=r"(r2[10]), "=r"(r2[11]), "=r"(r2[12]), "=r"(r2[13]), "=r"(r2[14]), "=r"(r2[15])
-                     : "r"(taddr + static_cast<uint32_t>(NT)) : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  // =========================== consumers: decode + wgmma ===========================
+  // Fragment ownership (wgmma A / D, one 16-row slice per warp): this thread holds rows r0 = 16 * (warp in group) + lane / 4
+  // and r0 + 8 of its warpgroup's 64 channels; of a k-step's eight values it holds the pair 2 * (lane % 4), +1 (bf16x2: both
+  // copies of [w | w]) or the values lane % 4 of either half (tf32).
+  const int gid = lane >> 2, t4 = lane & 3;
+  const int row0 = (warp >> 2) * 64 + (warp & 3) * 16 + gid, row1 = row0 + 8;
+  const int cc0 = min(row0, CTv - 1), cc1 = min(row1, CTv - 1);   // rows beyond the valid channels decode a copy (never stored)
+  const int myHalf = t4 >> 1, myWord = t4 & 1;                    // bf16x2: the half and the value pair inside its piece
+  const bool pre = BF && a.cbPre != 0;
+  float acc[NT / 2], acc2[CORR ? NT / 2 : 1];
 #pragma unroll
-        for (int j = 0; j < 16; j++) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(r2[j]));
-      }
+  for (int i = 0; i < NT / 2; i++) acc[i] = 0.0f;
 #pragma unroll
-      for (int j = 0; j < 16; j++) {
-        const int off = outoff[blk * 16 + j];
-        if (off >= 0 && chOk) {
-          float v = __uint_as_float(r[j]) + bv;
-          if (a.relu) v = fmaxf(v, 0.0f);   // (never set together with split-K partial sums)
-          dstBase[off + c] = v;
+  for (int i = 0; i < (CORR ? NT / 2 : 1); i++) acc2[i] = 0.0f;
+  float (&accLo)[CORR ? NT / 2 : 1] = acc2;
+  const uint64_t descFixed = static_cast<uint64_t>(8) << 32;     // SBO = 128 B; LBO and the start address come per k-step
+  const uint32_t planes0 = SmemU32(planes);
+
+  for (int kc = 0; kc < nChunks; kc++) {
+    const int cbuf = kc % kCbBufs, buf = kc % a.nPB;
+    MbarWait(fullC + cbuf, (kc / kCbBufs) & 1);
+    const uint8_t* idb = ids + cbuf * a.idRows * 128;
+    const float4* cb = cbs + cbuf * a.cbSlots * a.cbF4;
+    const float* cbf = reinterpret_cast<const float*>(cb);
+    const uint32_t* cbw = reinterpret_cast<const uint32_t*>(cb);
+    const int e0 = a.chunkFirst[a.mode == 1 ? kcBase + kc : 0];
+    const int ne = a.mode == 2 ? min(a.chunkCount[0], kTotal - kc * a.chunkCount[0]) : a.chunkCount[a.mode == 1 ? kcBase + kc : 0];
+    // idxT: every tap index of the thread's two channels for the chunk in registers (one to three 128-bit loads each): the
+    // per-k-step chain is one dependent shared-memory round trip (the codeword piece)
+    //   mode 0: iq[ch][2 h], iq[ch][2 h + 1] = the taps of half-slot h (bf16x2: the thread's own half; tf32: both halves)
+    //   mode 1: iq[ch][0..2] = the <= 48 rows of the phase row
+    uint4 iq[2][4];
+#pragma unroll
+    for (int c = 0; c < 2; c++)
+#pragma unroll
+      for (int j = 0; j < 4; j++) iq[c][j] = make_uint4(0, 0, 0, 0);
+    if (a.idxT) {
+      const uint4* ip = reinterpret_cast<const uint4*>(idb);
+      const int W = a.tapsPad >> 4;
+#pragma unroll
+      for (int c = 0; c < 2; c++) {
+        const int cc = c ? cc1 : cc0;
+        if (a.mode == 1) {
+          iq[c][0] = ip[cc * W];
+          if (W > 1) iq[c][1] = ip[cc * W + 1];
+          if (W > 2) iq[c][2] = ip[cc * W + 2];
+        } else {
+#pragma unroll
+          for (int h = 0; h < (BF ? 1 : 2); h++) {
+            const int half = BF ? myHalf : h;
+            iq[c][2 * h] = ip[(half * 128 + cc) * W];
+            if (W > 1) iq[c][2 * h + 1] = ip[(half * 128 + cc) * W + 1];
+          }
         }
       }
     }
+    // float4 index (inside the chunk's staged codebook) of the piece that `half` of k-step (ks, tap) takes for channel c
+    auto pieceOf = [&](const KStep& ks, int tap, int half, int c) -> int {
+      if (a.idxT && a.mode == 1)
+        return (half ? ks.cb1 : ks.cb0) * K + ByteOf48(iq[c][0], iq[c][1], iq[c][2], half ? ks.idx1 : ks.idx0);
+      if (a.idxT) {
+        const int h = BF ? 0 : half;
+        return half * K + ByteOf32(iq[c][2 * h], iq[c][2 * h + 1], tap);
+      }
+      return (half ? ks.cb1 : ks.cb0) * K + (idb[(half ? ks.idx1 : ks.idx0) * 128 + (c ? cc1 : cc0)] >> a.kshift);
+    };
+    // scalar codewords (d = 1): value j (< 4) of `half` is its own subspace: row / slot idx + j
+    auto scalarOf = [&](const KStep& ks, int half, int j, int c) -> float {
+      const int row = (half ? ks.idx1 : ks.idx0) + j, slot = (half ? ks.cb1 : ks.cb0) + j;
+      return cbf[slot * K + (idb[row * 128 + (c ? cc1 : cc0)] >> a.kshift)];
+    };
+    MbarWait(fullB + buf, (kc / a.nPB) & 1);
+    const uint64_t dHi = descFixed | (((planes0 + static_cast<uint32_t>((buf * 2 + 0) * a.planeRows) * 16u) >> 4) & 0x3FFFu);
+    const uint64_t dLo = descFixed | (((planes0 + static_cast<uint32_t>((buf * 2 + 1) * a.planeRows) * 16u) >> 4) & 0x3FFFu);
+    for (int s0 = 0; s0 < ne; s0 += GT) {
+      const int n = min(GT, ne - s0);
+      // the stage's k-steps are independent: index bytes and codeword pieces of all of them are in flight together
+      uint32_t fa[kMaxGT][BF ? 4 : 8];
+      uint64_t boff[kMaxGT];
+#pragma unroll
+      for (int i = 0; i < kMaxGT; i++) {
+        if (i < n) {
+          const KStep ks = (a.idxT || a.mode != 2) ? a.tab[e0 + s0 + i] : tabS[e0 + s0 + i];
+          boff[i] = static_cast<uint64_t>(static_cast<uint32_t>(ks.bStart)) | (static_cast<uint64_t>(static_cast<uint32_t>(ks.lbo)) << 16);
+          if constexpr (BF) {
+            // [w1 | w1] -> fa[0..1] (rows r0, r1; both K halves read the same registers), [w2 | w2] -> fa[2..3]
+#pragma unroll
+            for (int c = 0; c < 2; c++) {
+              if (a.d == 1) {
+                const float v0 = scalarOf(ks, myHalf, 2 * myWord, c), v1 = scalarOf(ks, myHalf, 2 * myWord + 1, c);
+                const uint32_t p1 = PackBf16x2(v0, v1);
+                fa[i][c] = p1;
+                fa[i][2 + c] = PackBf16x2(v0 - __uint_as_float(p1 << 16), v1 - __uint_as_float(p1 & 0xFFFF0000u));
+              } else {
+                const int pi = pieceOf(ks, s0 + i, myHalf, c);
+                if (pre) {
+                  fa[i][c] = cbw[pi * 4 + myWord];
+                  fa[i][2 + c] = cbw[pi * 4 + 2 + myWord];
+                } else {
+                  const float2 v = reinterpret_cast<const float2*>(cb)[pi * 2 + myWord];
+                  const uint32_t p1 = PackBf16x2(v.x, v.y);
+                  fa[i][c] = p1;
+                  fa[i][2 + c] = PackBf16x2(v.x - __uint_as_float(p1 << 16), v.y - __uint_as_float(p1 & 0xFFFF0000u));
+                }
+              }
+            }
+          } else {
+            // tf32 fragment: (r0, half 0), (r1, half 0), (r0, half 1), (r1, half 1), value t4 of the half; hi -> fa[0..3], lo -> fa[4..7]
+#pragma unroll
+            for (int h = 0; h < 2; h++)
+#pragma unroll
+              for (int c = 0; c < 2; c++) {
+                const float v = a.d == 1 ? scalarOf(ks, h, t4, c) : cbf[pieceOf(ks, s0 + i, h, c) * 4 + t4];
+                const uint32_t hi = __float_as_uint(v) & 0xFFFFE000u;
+                fa[i][2 * h + c] = hi;
+                fa[i][4 + 2 * h + c] = __float_as_uint(v - __uint_as_float(hi));
+              }
+          }
+        }
+      }
+      qcnn::WgmmaFence();
+#pragma unroll
+      for (int i = 0; i < kMaxGT; i++) {
+        if (i < n) {
+          if constexpr (BF) {
+            // B = [x1 | x2]: K-core-matrix 0 in the first plane, 1 in the second (the table's lbo is the plane distance)
+            Wgmma<NT>::Bf16RS(acc, fa[i][0], fa[i][1], fa[i][0], fa[i][1], dHi + boff[i]);
+            if constexpr (CORR) Wgmma<NT>::Bf16RS(accLo, fa[i][2], fa[i][3], fa[i][2], fa[i][3], dHi + boff[i]);
+            else Wgmma<NT>::Bf16RS(acc, fa[i][2], fa[i][3], fa[i][2], fa[i][3], dHi + boff[i]);
+          } else {
+            Wgmma<NT>::Tf32RS(acc, fa[i][0], fa[i][1], fa[i][2], fa[i][3], dHi + boff[i]);
+            if constexpr (CORR) {
+              Wgmma<NT>::Tf32RS(accLo, fa[i][0], fa[i][1], fa[i][2], fa[i][3], dLo + boff[i]);
+              Wgmma<NT>::Tf32RS(accLo, fa[i][4], fa[i][5], fa[i][6], fa[i][7], dHi + boff[i]);
+            } else {
+              Wgmma<NT>::Tf32RS(acc, fa[i][0], fa[i][1], fa[i][2], fa[i][3], dLo + boff[i]);
+              Wgmma<NT>::Tf32RS(acc, fa[i][4], fa[i][5], fa[i][6], fa[i][7], dHi + boff[i]);
+            }
+          }
+        }
+      }
+      qcnn::WgmmaCommit();
+      qcnn::WgmmaWaitAll();
+    }
+    // the chunk's MMAs have retired: its planes and its codebook / index buffer may be refilled
+    __syncwarp();
+    if (lane == 0) { MbarArrive(emptyB + buf); MbarArrive(emptyC + cbuf); }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmemD), "r"(kTmemCols) : "memory");
+
+  // ---- epilogue: accumulator fragments (rows = channels r0, r1; columns = positions 8 i + 2 t4, +1) -> + bias, ReLU -> NHWC ----
+  {
+    const bool ok0 = row0 < CTv, ok1 = row1 < CTv;
+    const float b0 = biasS[row0], b1 = biasS[row1];
+#pragma unroll
+    for (int i = 0; i < NT / 8; i++) {
+#pragma unroll
+      for (int j = 0; j < 2; j++) {
+        const int off = outoff[8 * i + 2 * t4 + j];
+        if (off < 0) continue;
+        float v0 = acc[4 * i + j] + b0, v1 = acc[4 * i + 2 + j] + b1;
+        if constexpr (CORR) { v0 += acc2[CORR ? 4 * i + j : 0]; v1 += acc2[CORR ? 4 * i + 2 + j : 0]; }
+        if (a.relu) { v0 = fmaxf(v0, 0.0f); v1 = fmaxf(v1, 0.0f); }   // (never set together with split-K partial sums)
+        if (ok0) dstBase[off + row0] = v0;
+        if (ok1) dstBase[off + row1] = v1;
+      }
+    }
+  }
 }
 
 }  // namespace
 
 namespace qcnn {
 
-// Candidate tilings for batch N (cost in SM-cycles, comparable with PlanConv's model): 3 MMAs of NT/2 clk per k-step.
-void AddLitePqGemm(const qcnn_layer* L, std::vector<std::pair<double, ConvPlan>>* cands, size_t first);
-void AddWidePqGemm(const qcnn_layer* L, std::vector<std::pair<double, ConvPlan>>* cands, size_t first);
-void AddXlPqGemm(const qcnn_layer* L, std::vector<std::pair<double, ConvPlan>>* cands, size_t first);
-static void PlanPqGemmFull(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands);
+// Candidate tilings for batch N (cost in SM-cycles, comparable with PlanConv's model); on-device timing chooses among them.
 void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands) {
-  const size_t first = cands->size();
-  PlanPqGemmFull(L, N, cands);
-  static const bool lite = !(getenv("QCNN_GEMM_LITE") && getenv("QCNN_GEMM_LITE")[0] == '0');
-  static const bool wide = !(getenv("QCNN_GEMM_WIDE") && getenv("QCNN_GEMM_WIDE")[0] == '0');
-  const size_t mid = cands->size();
-  static const bool xl = !(getenv("QCNN_GEMM_XL") && getenv("QCNN_GEMM_XL")[0] == '0');
-  if (xl) AddXlPqGemm(L, cands, first);
-  if (wide) AddWidePqGemm(L, cands, first);
-  if (lite) {
-    const size_t end = cands->size();
-    AddLitePqGemm(L, cands, first);
-    (void)mid; (void)end;
-  }
-}
-static void PlanPqGemmFull(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands) {
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, taps = L->ksz * L->ksz;
   if (L->K < 1 || L->K > 256 || Kg % 16 != 0) return;
   const size_t smemMax0 = L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024;
@@ -987,22 +702,22 @@ static void PlanPqGemmFull(const qcnn_layer* L, int N, std::vector<std::pair<dou
     const int PWp = CeilDiv(L->Win + 2 * L->pad, st), PHp = CeilDiv(L->Hin + 2 * L->pad, st);
     const int IB = PHp * PWp;
     if (static_cast<double>(N) * IB > 2.0e9 || static_cast<double>(L->Hin) * L->Win * L->Cin * 4 > 2.0e9) return;
-    const int nts1[2] = {256, 128};
+    const int nts1[2] = {128, 64};
     for (int ni = 0; ni < 2; ni++) {
       const int NT = nts1[ni];
-      const int gts1[3] = {6, 4, 8};
-      for (int gi = 0; gi < 3; gi++) {
+      const int gts1[2] = {4, 3};
+      for (int gi = 0; gi < 2; gi++) {
         const int GT = gts1[gi];
         ConvPlan p;
         memset(&p, 0, sizeof(p));
         p.kernel = 6; p.CPT = NT; p.J = GT; p.threads = kThreads;
         GemmArgs& ga = p.g;
         ga.mode = 1;
-        ga.PW = PWp; ga.IB = IB; ga.NT = NT; ga.GT = GT; ga.NSLOT = std::min(kMaxSlots, 16 / GT);
+        ga.PW = PWp; ga.IB = IB; ga.NT = NT; ga.GT = GT;
         ga.NPOS = RoundUp(NT + ((L->ksz - 1) / st) * (PWp + 1), 8);
         ga.planeF4 = st * ga.NPOS;
         if (ga.planeF4 > kRegPos * kStagers) continue;
-        ga.aOff = 256; ga.corr = NT <= 128 ? 1 : 0; ga.lite = 0;
+        ga.corr = NT <= 64 ? 1 : 0;
         ga.bf = L->opt_tc_bf ? 1 : 0;
         if (ga.bf && (st & 1)) continue;       // bf16x2 rows hold a PAIR of phase columns
         ga.planeRows = ga.bf ? (st / 2) * ga.NPOS : ga.planeF4;
@@ -1065,23 +780,23 @@ static void PlanPqGemmFull(const qcnn_layer* L, int N, std::vector<std::pair<dou
   if (L->Ho > L->Hin + L->pad || L->Wo > PW) return;
   if (static_cast<double>(N) * IB > 2.0e9) return;
   const size_t smemMax = L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024;
-  const int nts[3] = {256, 128, 64};
-  for (int ni = 0; ni < 3; ni++) {
+  const int nts[2] = {128, 64};
+  for (int ni = 0; ni < 2; ni++) {
     const int NT = nts[ni];
-    const int gts[3] = {4, 5, 8};
-    for (int gi = 0; gi < 3; gi++) {
+    const int gts[2] = {4, 3};
+    for (int gi = 0; gi < 2; gi++) {
       const int GT = gts[gi];
       ConvPlan p;
       memset(&p, 0, sizeof(p));
       p.kernel = 6; p.CPT = NT; p.J = GT; p.threads = kThreads;
       GemmArgs& ga = p.g;
       ga.mode = 0;
-      ga.PW = PW; ga.IB = IB; ga.NT = NT; ga.GT = GT; ga.NSLOT = std::min(kMaxSlots, 16 / GT);
+      ga.PW = PW; ga.IB = IB; ga.NT = NT; ga.GT = GT;
       ga.NPOS = RoundUp(NT + (L->ksz - 1) * (PW + 1), 8);
       if (ga.NPOS > 16000) continue;
       ga.planeF4 = 2 * ga.NPOS;
       if (ga.planeF4 > kRegPos * kStagers) continue;
-      ga.aOff = 256; ga.corr = NT <= 128 ? 1 : 0; ga.lite = 0;
+      ga.corr = NT <= 64 ? 1 : 0;
       ga.bf = L->opt_tc_bf ? 1 : 0;
       ga.planeRows = ga.bf ? ga.NPOS : ga.planeF4;   // (bf16x2: lbo = NPOS rows is the x1 -> x2 plane distance as well)
       ga.cbSlots = 2; ga.idRows = 2 * taps;
@@ -1119,77 +834,30 @@ static void PlanPqGemmFull(const qcnn_layer* L, int N, std::vector<std::pair<dou
     }
   }
 }
-
-// Two-CTAs-per-SM variants of the candidates above (see kRegPosLite): tiles of <= 128 positions whose register windows,
-// TMEM columns (accumulators + weight ring <= 256) and shared memory (two CTAs + their 1 KB reservations per SM) fit
-// twice.  The fixed part of the cost model is halved: it overlaps the neighbour CTA's MMA phase.
-// Twelve-warp variants (second decoder group): stages of <= 5 k-steps, register windows of the lite size.
-void AddWidePqGemm(const qcnn_layer* L, std::vector<std::pair<double, ConvPlan>>* cands, size_t first) {
-  (void)L;
-  const size_t n = cands->size();
-  for (size_t i = first; i < n; i++) {
-    ConvPlan p = (*cands)[i].second;
-    GemmArgs& ga = p.g;
-    if (p.kernel != 6 || ga.lite || ga.xl || ga.GT > 5 || ga.planeF4 > kRegPosLite * kStagers || ga.NSLOT < 2) continue;
-    ga.wide = 1;
-    p.threads = 384;
-    p.J = ga.GT + 200;     // (candidate de-duplication key)
-    cands->emplace_back((*cands)[i].first * 0.85, p);
-  }
-}
-
-// Sixteen-warp variants for mode 1 (conv1): tiles of 256 positions, stages of <= 4 k-steps, 224 stager threads
-void AddXlPqGemm(const qcnn_layer* L, std::vector<std::pair<double, ConvPlan>>* cands, size_t first) {
-  (void)L;
-  const size_t n = cands->size();
-  for (size_t i = first; i < n; i++) {
-    ConvPlan p = (*cands)[i].second;
-    GemmArgs& ga = p.g;
-    if (p.kernel != 6 || ga.lite || ga.wide || ga.mode != 1 || !ga.bf || ga.GT > kMaxGTLite || ga.NSLOT < 2 ||
-        ga.planeF4 > 7 * (kStagers + 128)) continue;
-    ga.xl = 1;
-    p.threads = 512;
-    p.J = ga.GT + 300;     // (candidate de-duplication key)
-    cands->emplace_back((*cands)[i].first * 0.7, p);
-  }
-}
-
-void AddLitePqGemm(const qcnn_layer* L, std::vector<std::pair<double, ConvPlan>>* cands, size_t first) {
-  const size_t smemMax = L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024;
-  const size_t perCtaSmem = (smemMax + 1024) / 2 - 1024 - 512;
-  const size_t n = cands->size();
-  for (size_t i = first; i < n; i++) {
-    ConvPlan p = (*cands)[i].second;
-    GemmArgs& ga = p.g;
-    if (p.kernel != 6 || ga.wide || ga.xl || ga.NT > 128 || ga.GT > kMaxGTLite || ga.planeF4 > kRegPosLite * kStagers || p.smem > perCtaSmem) continue;
-    const int ring = ga.NSLOT * ga.GT * 16;
-    ga.NSLOT = std::min(ga.NSLOT, (256 - ga.NT) / (ga.GT * 16));
-    if (ga.NSLOT < 2) continue;
-    (void)ring;
-    ga.corr = (2 * ga.NT + ga.NSLOT * ga.GT * 16 <= 256) ? 1 : 0;
-    ga.aOff = ga.corr ? 2 * ga.NT : ga.NT;
-    ga.lite = 1;
-    p.J = ga.GT + 100;     // (candidate de-duplication key: distinct from the one-CTA-per-SM twin)
-    cands->emplace_back((*cands)[i].first * 0.8, p);
-  }
-}
-
-// dynamic shared-memory limit of both instantiations: raised once per device to the opt-in maximum (not per launch,
+// dynamic shared-memory limit of the instantiations: raised once per device to the opt-in maximum (not per launch,
 // which would make the limit follow whichever layer ran last -- fragile under graph capture / concurrent streams)
 static int SetSmemLimitOnce(qcnn_ctx* ctx) {
   static bool done[64] = {false};
   if (ctx->device >= 0 && ctx->device < 64 && done[ctx->device]) return 0;
   const int lim = static_cast<int>(ctx->smem_optin ? ctx->smem_optin : 227 * 1024);
 #define QCNN_SMEM_ATTR(...) QCNN_CUDA(cudaFuncSetAttribute(pq_gemm_tc_kernel<__VA_ARGS__>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim))
-  QCNN_SMEM_ATTR(false, false, false, false); QCNN_SMEM_ATTR(true, false, false, false); QCNN_SMEM_ATTR(false, true, false, false);
-  QCNN_SMEM_ATTR(false, false, true, false);  QCNN_SMEM_ATTR(true, false, true, false);  QCNN_SMEM_ATTR(false, true, true, false);
-  QCNN_SMEM_ATTR(false, false, false, true);  QCNN_SMEM_ATTR(false, false, true, true);  QCNN_SMEM_ATTR(true, false, true, true);
-  QCNN_SMEM_ATTR(false, false, true, false, true);  QCNN_SMEM_ATTR(true, false, true, false, true);
+  QCNN_SMEM_ATTR(true, 128); QCNN_SMEM_ATTR(true, 64); QCNN_SMEM_ATTR(false, 128); QCNN_SMEM_ATTR(false, 64);
 #undef QCNN_SMEM_ATTR
-  // the lite kernels' CTAs must really pair up: ask for the largest shared-memory carve-out
-  QCNN_CUDA(cudaFuncSetAttribute(pq_gemm_tc_kernel<false, true, false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-  QCNN_CUDA(cudaFuncSetAttribute(pq_gemm_tc_kernel<false, true, true, false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
   if (ctx->device >= 0 && ctx->device < 64) done[ctx->device] = true;
+  return 0;
+}
+
+static int LaunchKernel(const GemmArgs& a, unsigned blocks, size_t smem, cudaStream_t st) {
+  QCNN_CHECK((a.NT == 128 || a.NT == 64) && a.corr == (a.NT == 64 ? 1 : 0) && a.GT >= 1 && a.GT <= kMaxGT,
+             "pq_gemm_tc: no instantiation for NT=%d GT=%d", a.NT, a.GT);
+  if (a.bf) {
+    if (a.NT == 128) pq_gemm_tc_kernel<true, 128><<<blocks, kThreads, smem, st>>>(a);
+    else pq_gemm_tc_kernel<true, 64><<<blocks, kThreads, smem, st>>>(a);
+  } else {
+    if (a.NT == 128) pq_gemm_tc_kernel<false, 128><<<blocks, kThreads, smem, st>>>(a);
+    else pq_gemm_tc_kernel<false, 64><<<blocks, kThreads, smem, st>>>(a);
+  }
+  QCNN_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -1236,40 +904,7 @@ int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, floa
     a.partial = L->d_partial;
   }
   if (int rc = SetSmemLimitOnce(L->ctx)) return rc;
-  static const bool dbg = getenv("QCNN_GEMM_DBG") != nullptr;
-  if (dbg) {
-    QCNN_CUDA(cudaMalloc(&a.dbg, 128));
-    QCNN_CUDA(cudaMemsetAsync(a.dbg, 0, 128, st));
-  }
-  const unsigned nb = static_cast<unsigned>(blocks);
-  if (a.xl) {
-    if (dbg) pq_gemm_tc_kernel<true, false, true, false, true><<<nb, 512, p.smem, st>>>(a);
-    else pq_gemm_tc_kernel<false, false, true, false, true><<<nb, 512, p.smem, st>>>(a);
-  } else if (a.wide) {
-    if (a.bf) { if (dbg) pq_gemm_tc_kernel<true, false, true, true><<<nb, 384, p.smem, st>>>(a); else pq_gemm_tc_kernel<false, false, true, true><<<nb, 384, p.smem, st>>>(a); }
-    else pq_gemm_tc_kernel<false, false, false, true><<<nb, 384, p.smem, st>>>(a);
-  } else if (a.bf) {
-    if (dbg && !a.lite) pq_gemm_tc_kernel<true, false, true, false><<<nb, kThreads, p.smem, st>>>(a);
-    else if (a.lite) pq_gemm_tc_kernel<false, true, true, false><<<nb, kThreads, p.smem, st>>>(a);
-    else pq_gemm_tc_kernel<false, false, true, false><<<nb, kThreads, p.smem, st>>>(a);
-  } else {
-    if (dbg && !a.lite) pq_gemm_tc_kernel<true, false, false, false><<<nb, kThreads, p.smem, st>>>(a);
-    else if (a.lite) pq_gemm_tc_kernel<false, true, false, false><<<nb, kThreads, p.smem, st>>>(a);
-    else pq_gemm_tc_kernel<false, false, false, false><<<nb, kThreads, p.smem, st>>>(a);
-  }
-  QCNN_CUDA(cudaGetLastError());
-  if (dbg) {
-    unsigned long long h[16];
-    QCNN_CUDA(cudaStreamSynchronize(st));
-    QCNN_CUDA(cudaMemcpy(h, a.dbg, 128, cudaMemcpyDeviceToHost));
-    const double n = h[5] ? static_cast<double>(h[5]) : 1.0;
-    fprintf(stderr, "[pq_gemm dbg] ctas=%llu NT=%d GT=%d chunks=%d ksteps=%d | per CTA: issue-loop %.0f clk (wait planes %.0f, wait weights %.0f), "
-            "drain %.0f | stager loop %.0f (wait copies %.0f, wait planes free %.0f, wait cb free %.0f) | decoder loop %.0f (wait cb %.0f, "
-            "wait ring %.0f; index loads %.0f, codeword loads %.0f, split + tcgen05.st %.0f, wait::st %.0f)\n", h[5], a.NT, a.GT, a.nChunks,
-            a.chunkCount[0], h[0] / n, h[1] / n, h[2] / n, h[3] / n, h[8] / n, h[9] / n,
-            h[10] / n, h[11] / n, h[12] / n, h[13] / n, h[14] / n, h[4] / n, h[6] / n, h[7] / n, h[15] / n);
-    cudaFree(a.dbg);
-  }
+  if (int rc = LaunchKernel(a, static_cast<unsigned>(blocks), p.smem, st)) return rc;
   if (a.nsplit > 1)
     return LaunchSplitReduce(L->ctx, a.partial, dst, N * a.Ho * a.Wo, a.Cout, a.Cout, a.nsplit, relu, st);
   return 0;
@@ -1278,13 +913,9 @@ int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, floa
 // generic entry for callers that fill GemmArgs themselves (the fully-connected path in fc_aprx.cu)
 size_t PqGemmSmemBytes(const GemmArgs& a) { return static_cast<size_t>(MapSmem(a).total); }
 int LaunchPqGemmArgs(qcnn_ctx* ctx, const GemmArgs& a, long long blocks, cudaStream_t st) {
-  const size_t smem = PqGemmSmemBytes(a);
   QCNN_CHECK(blocks >= 1 && blocks <= 2147483647LL, "pq_gemm_tc: bad grid");
   if (int rc = SetSmemLimitOnce(ctx)) return rc;
-  if (a.bf) pq_gemm_tc_kernel<false, false, true, false><<<static_cast<unsigned>(blocks), kThreads, smem, st>>>(a);
-  else pq_gemm_tc_kernel<false, false, false, false><<<static_cast<unsigned>(blocks), kThreads, smem, st>>>(a);
-  QCNN_CUDA(cudaGetLastError());
-  return 0;
+  return LaunchKernel(a, static_cast<unsigned>(blocks), PqGemmSmemBytes(a), st);
 }
 
 }  // namespace qcnn

@@ -35,7 +35,7 @@ using namespace qcnn;
 
 extern "C" {
 
-const char* qcnn_version(void) { return "qcnn-b200 0.1 (sm_100a)"; }
+const char* qcnn_version(void) { return "qcnn-b200 0.1 (sm_90a)"; }
 const char* qcnn_last_error(void) { return g_err; }
 
 int qcnn_ctx_create(int device, qcnn_ctx** out) {
@@ -51,7 +51,7 @@ int qcnn_ctx_create(int device, qcnn_ctx** out) {
   QCNN_CHECK(device >= 0 && device < cnt, "qcnn_ctx_create: device %d out of range (have %d)", device, cnt);
   cudaDeviceProp prop;
   QCNN_CUDA(cudaGetDeviceProperties(&prop, device));
-  QCNN_CHECK(prop.major == 10, "qcnn_ctx_create: device %d is sm_%d%d; this build carries sm_100a code only", device,
+  QCNN_CHECK(prop.major == 9 && prop.minor == 0, "qcnn_ctx_create: device %d is sm_%d%d; this build carries sm_90a code only", device,
              prop.major, prop.minor);
   QCNN_ON_DEVICE(device);
   qcnn_ctx* ctx = new qcnn_ctx();
@@ -105,8 +105,8 @@ static qcnn_layer* NewLayer(qcnn_ctx* ctx, int kind) {
   memset(static_cast<void*>(L), 0, sizeof(*L));
   L->ctx = ctx;
   L->kind = kind;
-  // default operand format of the tensor-core GEMMs: bf16x2 (two MMAs per k-step at twice the tf32 rate; measured error
-  // at the level of 3xTF32's, DESIGN.md 2); tensor_core = 1 or QCNN_TC_BF=0 selects 3xTF32
+  // default operand format of the tensor-core GEMMs: bf16x2 (two MMAs per k-step at twice the tf32 rate; error at the
+  // level of 3xTF32's, DESIGN.md 2); tensor_core = 1 or QCNN_TC_BF=0 selects 3xTF32
   static const bool bfDefault = !(getenv("QCNN_TC_BF") && getenv("QCNN_TC_BF")[0] == '0');
   L->opt_tc_bf = bfDefault ? 1 : 0;
   // process-wide default of "tensor_core": QCNN_NO_DECTC=1 starts every layer on the strict LUT + gather path
@@ -286,7 +286,7 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
   else if (!strcmp(name, "force_kernel") || !strcmp(name, "autotune") || !strcmp(name, "gemm_nt")) {
     // conv only.  force_kernel: -1 none, else 0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc;
     // autotune: 0 keeps the cost model's first tiling instead of timing the candidates on the device;
-    // gemm_nt: positions per CTA of the pq_gemm_tc tilings (0 = any; 256 = one TMEM accumulator, <= 128 = two)
+    // gemm_nt: positions per CTA of the pq_gemm_tc tilings (0 = any; 128 = one accumulator, 64 = two)
     QCNN_CHECK(L->kind == QCNN_KIND_CONV, "qcnn_layer_set_param: '%s' applies to conv layers", name);
     if (name[0] == 'f') L->opt_force_kernel = value < 0 ? 0 : value + 1;
     else if (name[0] == 'g') L->opt_gemm_nt = value < 0 ? 0 : value;

@@ -115,7 +115,6 @@ struct GemmArgs {
   const float* ctrd;
   const uint8_t* asmt;
   const float* bias;
-  unsigned long long* dbg;    // optional cycle counters of the MMA issuer (QCNN_GEMM_DBG=1)
   long long srcImg, dstImg;   // elements per source / destination image
   int N, Hi, Wi, Cin, Ho, Wo, Cout, ksz, pad, stride, G, Cg, Kg, KgPad, S, K, d;
   int mode;                   // 0 stride-1 conv, 1 strided conv on phase planes, 2 fully connected
@@ -129,14 +128,10 @@ struct GemmArgs {
   const float* xprep;           // mode 2: activations pre-split into the plane image (fc_prep_kernel), [tile][chunk][hi,lo][2KS][NT][4]
   int nChunksAll;               // mode 2: chunks of the whole layer (xprep indexing)
   int cbF4;                     // float4 per codebook slot (K for d % 4 == 0 pieces, K/4 for d == 1 scalars)
-  int NT;                     // positions per CTA = MMA N (multiple of 16, <= 256)
-  int aOff;                   // first TMEM column of the decoded-weight ring (after the accumulator(s))
-  int corr;                   // 1: the 3xTF32 cross terms have their own accumulator at column NT (added in the epilogue)
-  int lite;                   // 1: the two-CTAs-per-SM instantiation (256 TMEM columns, short register windows)
-  int wide;                   // 1: the twelve-warp instantiation (second decoder warp group)
-  int xl;                     // 1: the sixteen-warp instantiation (second decoder group + 224 stager threads; mode 1)
-  int bf;                     // 1: bf16x2 operands (x = x1 + x2, w = w1 + w2 as bf16 pieces; TWO kind::f16 MMAs of K = 16 per
-                              //    k-step: [w1|w1].[x1|x2] + [w2|w2].[x1|x2]) instead of 3xTF32 (three kind::tf32 MMAs of K = 8)
+  int NT;                     // positions per CTA = wgmma N (128 or 64)
+  int corr;                   // 1 (NT = 64): the terms with a low-order operand piece have their own accumulator (added in the epilogue)
+  int bf;                     // 1: bf16x2 operands (x = x1 + x2, w = w1 + w2 as bf16 pieces; TWO bf16 MMAs of K = 16 per
+                              //    k-step: [w1|w1].[x1|x2] + [w2|w2].[x1|x2]) instead of 3xTF32 (three tf32 MMAs of K = 8)
   const uint8_t* asmtT;       // qcnn_layer::d_asmt_t (mode 0 with idxT)
   int idxT, tapsPad;          // 1: the chunk's indices are staged channel-major ([half][128 channels][tapsPad bytes])
   int bulkC;                  // mode 0 with idxT and cbPre: codebook slices + index blocks arrive by four cp.async.bulk per chunk
@@ -146,7 +141,7 @@ struct GemmArgs {
   int planeF4;                // float4 per staged plane set (one of hi / lo, one buffer)
   int cbSlots, idRows;        // codebook slices / index rows staged per chunk
   int nChunks;
-  int GT, NSLOT;              // k-steps per stage, stages in the TMEM weight ring
+  int GT;                     // k-steps per stage (decoded into registers together, <= 4)
   int nct;                    // 128-channel tiles per group
   int relu;
   int ntab;
@@ -155,7 +150,7 @@ struct GemmArgs {
 };
 
 struct ConvPlan {
-  int kernel;           // 0 s1, 1 roll, 2 s1_tc, 3 roll_tc, 4 direct, 6 pq_gemm_tc (decode-at-use GEMMs on tcgen05); 5 retired
+  int kernel;           // 0 s1, 1 roll, 2 s1_tc, 3 roll_tc, 4 direct, 6 pq_gemm_tc (decode-at-use GEMMs on wgmma); 5 retired
   int CPT, J;
   int threads;
   size_t smem;

@@ -1,5 +1,5 @@
 // Network executor with the reference's CaffeEva interface (/root/reference/include/CaffeEva.h:60-195), running the
-// PQ forward pass on a B200 through the C ABI of include/qcnn.h -- this file uses NOTHING but that C ABI, so it is
+// PQ forward pass on the GPU through the C ABI of include/qcnn.h -- this file uses NOTHING but that C ABI, so it is
 // also the template for the binding a maintainer adds to the reference's own CaffeEva.cc (see INTEGRATION.md).
 //
 // Same public methods and semantics; differences:

@@ -1,6 +1,6 @@
 // Single-image classification API, same interface as the reference's CaffeEvaWrapper
 // (/root/reference/include/CaffeEvaWrapper.h:38-142): SetPath / SetModel / Proc / GetErrorMsg / ClrErrorMsg and the
-// CaffeEvaRslt result record.  Host glue only; the forward pass runs on the B200 through CaffeEva -> C ABI.
+// CaffeEvaRslt result record.  Host glue only; the forward pass runs on the GPU through CaffeEva -> C ABI.
 #ifndef QCNN_HOST_CAFFEEVAWRAPPER_H_
 #define QCNN_HOST_CAFFEEVAWRAPPER_H_
 

@@ -3,7 +3,7 @@ C ABI (qcnn_fc_chain_forward, and qcnn_fc_aprx_forward / qcnn_net_forward, which
 the CPU oracle.
 
 Tolerance: the kernel adds the same fp32 LUT entries as the reference (LUT entries bit-identical: separate rounded
-multiply and add, ascending j) but associates the sum differently -- per CTA s-ascending over its 1/148 of the
+multiply and add, ascending j) but associates the sum differently -- per CTA s-ascending over its share (one CTA per SM) of the
 subspaces, then a fixed tree over the CTAs -- so results agree to fp32 re-association noise: RTOL = 1e-4 under the
 metric of test_gpu_layers.close (measured ~1e-6), and are bit-identical from run to run (no atomics)."""
 import numpy as np

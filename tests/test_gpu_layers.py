@@ -13,8 +13,8 @@ import numpy as np
 import pytest
 
 RTOL = 1e-4
-# decode-at-use tensor-core kernels (3xTF32, fp32 accumulation inside the tensor core over all k-steps): measured
-# <= 1e-4 per layer on the AlexNet shapes (tools/accuracy.py); the LUT + gather kernels stay within RTOL (measured 5e-6)
+# decode-at-use tensor-core kernels (bf16x2 or 3xTF32 operands, fp32 accumulation inside the tensor core over all k-steps): measured
+# on an H100 <= 1.1e-4 per layer on the AlexNet shapes at batch 256; the LUT + gather kernels stay within RTOL (measured 5.5e-6)
 RTOL_TC = 3e-4
 
 

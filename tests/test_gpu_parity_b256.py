@@ -1,6 +1,6 @@
-"""Parity of the BENCHMARKED configuration: batch 256, where every conv layer runs the decode-at-use tensor-core GEMM with
-256-position tiles and ONE TMEM accumulator (pq_gemm_tc NT = 256) and the FC layers run its split-K mode -- a different
-numerical path from the small-batch tilings the other tests exercise (two accumulators, K-split).
+"""Parity of the BENCHMARKED configuration: batch 256, where every conv layer runs the decode-at-use tensor-core GEMM
+(pq_gemm_tc; both of its tile widths are pinned in turn: NT = 128 with ONE accumulator, NT = 64 with two) and the FC layers
+run its split-K mode -- a different numerical path from the small-batch tilings the other tests exercise (K-split).
 
 What is checked, against the CPU oracle (oracle/pq_oracle.c, pinned bit-for-bit to the compiled reference):
   * every conv layer of AlexNet alone at N = 256 with the kernel family PINNED (force_kernel) and the plan asserted from
@@ -60,7 +60,7 @@ CONV_LAYERS = {
     "conv4": (13, 13, 384, 384, 3, 1, 1, 2, 24, 128, 8),
     "conv5": (13, 13, 384, 256, 3, 1, 1, 2, 24, 128, 8),
 }
-# kernel families pinned per layer: 6 = pq_gemm_tc (what the bench runs; both accumulator layouts, NT = 256 and 128, are
+# kernel families pinned per layer: 6 = pq_gemm_tc (what the bench runs; both accumulator layouts, NT = 128 and 64, are
 # pinned in turn) and the strict path's family at the same batch
 PINS = {"conv1": [6, 4], "conv2": [6, 2], "conv3": [6, 2], "conv4": [6, 2], "conv5": [6, 2]}
 KNAME = {6: "pq_gemm_tc", 4: "conv_direct", 2: "conv_s1_tc", 0: "conv_s1", 1: "conv_roll", 3: "conv_roll_tc"}
@@ -83,7 +83,7 @@ def test_conv_layer_b256_pinned_kernel(name, po, qcnn, ctx):
     layer = qcnn.ConvLayer(ctx, Cin, Hi, Wi, Cout, k, pad, stride, G, ctrd, asmt, bias)
     xd = torch.from_numpy(x).cuda()
     # tensor_core: 1 = 3xTF32 operands, 2 = bf16x2 operands (two MMAs per k-step), 0 = LUT + gather kernels
-    for kern, nt, tc in [(6, 256, 1), (6, 128, 1), (6, 256, 2), (6, 128, 2)] + [(k_, 0, 0) for k_ in PINS[name] if k_ != 6]:
+    for kern, nt, tc in [(6, 128, 1), (6, 64, 1), (6, 128, 2), (6, 64, 2)] + [(k_, 0, 0) for k_ in PINS[name] if k_ != 6]:
         layer.set_param("tensor_core", tc)
         layer.set_param("force_kernel", kern)
         layer.set_param("gemm_nt", nt)
@@ -91,7 +91,7 @@ def test_conv_layer_b256_pinned_kernel(name, po, qcnn, ctx):
         desc = layer.describe(N)          # after the forward: the plan the autotuner settled on and just ran
         assert KNAME[kern] in desc, desc
         if kern == 6:
-            # NT=256: ONE TMEM accumulator (all 3xTF32 terms chained in it); NT=128: the cross terms have their own
+            # NT=128: ONE accumulator (all terms of the operand split chained in it); NT=64: the low-order terms have their own
             assert "NT=%d" % nt in desc and "nsplit=1" in desc, desc
             assert ("bf16x2" in desc) == (tc == 2), desc
         a, b = e1(y, ref), close(y, ref)

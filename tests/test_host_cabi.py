@@ -20,7 +20,7 @@ def test_library_exports_every_declared_symbol(qcnn):
     assert not missing, missing
     # the binding knows every declared symbol too (no silently unbound entry point)
     assert sorted(qcnn.EXPORTS) == declared
-    assert b"sm_100a" in qcnn.lib.qcnn_version()
+    assert b"sm_90a" in qcnn.lib.qcnn_version()
 
 
 def test_no_cpu_fallback_without_gpu(qcnn):

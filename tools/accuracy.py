@@ -1,5 +1,5 @@
 """Per-layer error of the conv kernel families against the CPU oracle (same metric as the parity tests).
-    python tools/accuracy.py            # on a B200
+    python tools/accuracy.py            # on an H100
 """
 import importlib
 import os

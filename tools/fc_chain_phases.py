@@ -20,7 +20,7 @@ def main():
     import torch
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=10)
-    ap.add_argument("--mhz", type=float, default=1965.0)
+    ap.add_argument("--mhz", type=float, default=1980.0, help="SM clock the cycle stamps are converted with (H100 maximum: 1980)")
     args = ap.parse_args()
     q = importlib.import_module("quantized-cnn_b200")
     ctx = q.Context(0)

@@ -4,8 +4,8 @@ reports time (CUDA events, median of reps), achieved GB/s on the algorithmic byt
 measured HBM peak, lookups/s against the shared-memory gather bound and -- when the layer ran as a decode-at-use GEMM --
 the executed tensor-core TFLOP/s.  EVERY row (N = 1 and N = 256) is checked against the CPU oracle (tolerance of the
 path; both error metrics of tests/test_gpu_parity_b256.py are recorded).
-    python tools/sweep.py [--reps 5] [--strict] [--out profiles/r02_sweep.csv]
---strict: tensor_core = 0 (LUT + gather kernels only; results in profiles/r02_sweep_strict.csv)
+    python tools/sweep.py [--reps 5] [--strict] [--out sweep.csv]
+--strict: tensor_core = 0 (LUT + gather kernels only)
 """
 import argparse
 import importlib
@@ -29,7 +29,7 @@ GEOM = {  # name: (Hi, Cin, Cout, k, pad, G)   SURVEY.md 8(d) config 5
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "r02_sweep.csv"))
+    ap.add_argument("--out", default="sweep.csv")
     ap.add_argument("--no-check", action="store_true")
     ap.add_argument("--strict", action="store_true")
     args = ap.parse_args()
@@ -42,8 +42,10 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except (OSError, ValueError):
         pass
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
-    gather_peak = 32.0 * ctx.sm_count * float(peaks.get("sm_max_mhz", 1965.0)) * 1e6
+    # without MEASURED_PEAKS.json: H100 SXM data sheet (3350 GB/s of HBM3) and the H100's maximum SM clock
+    hbm = float(peaks.get("hbm_gbs", 3350.0))
+    hbm_src = "MEASURED_PEAKS.json" if "hbm_gbs" in peaks else "H100 SXM data sheet, not measured"
+    gather_peak = 32.0 * ctx.sm_count * float(peaks.get("sm_max_mhz", 1980.0)) * 1e6
     import re
     tol = 1e-4 if args.strict else 3e-4
     from concurrent.futures import ThreadPoolExecutor
@@ -99,7 +101,7 @@ def main():
                     print(rows[-1], flush=True)
                 layer.close()
     with open(args.out, "w") as f:
-        f.write("# BASELINE.json configs[4] sweep; HBM peak %.1f GB/s (MEASURED_PEAKS.json), smem-gather bound %.3e lookups/s\n" % (hbm, gather_peak))
+        f.write("# BASELINE.json configs[4] sweep; HBM peak %.1f GB/s (%s), smem-gather bound %.3e lookups/s\n" % (hbm, hbm_src, gather_peak))
         f.write("\n".join(rows) + "\n")
 
 
