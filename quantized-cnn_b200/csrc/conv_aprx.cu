@@ -14,18 +14,23 @@
 //     accumulated as a float2); per 4 channels it issues one 128-bit broadcast load of 4 pre-multiplied LUT row
 //     offsets, then 4 x (1 IADD + J LDS + J FADD);
 //   * the per-(s) assignment slice is staged in shared memory already multiplied by the LUT row pitch.
-// The LUT stage is a [K x d] x [d x positions] contraction per subspace.  It runs on the FP32 pipe as a
-// register-blocked mini-GEMM: 8 codewords x 4 positions per thread, float2 FFMA pairs, codebook
-// rows broadcast from shared memory, 128-bit LUT stores.  (fp32, ascending j: parity with the reference's saxpy
-// order up to FMA contraction; tensor-core TF32 would break the fp32 tolerance -- SURVEY.md 7.5.)
-// Two kernels share both stages:
+// Two kernel templates walk the LUT + gather steps; the kernel body owns the CTA decode, the LUT position -> pixel
+// table, the gather and the epilogue:
 //   conv_s1_kernel   stride 1 (conv2..conv5, sweep): a CTA owns (image, row strip, group, channel tile) and the
-//                    flat padded grid of the strip; tap (kh,kw) is a constant shift kh*PW+kw of the position.
-//   conv_roll_kernel any stride (conv1: 11x11 / 4): a CTA walks the input rows of its strip once; each input
-//                    row's LUT is built once and used by the <= ceil(k/stride) output rows that see it, each
-//                    owned by a different "row group" of warps; columns are de-interleaved by stride phase so
-//                    that a tap again is a constant shift.
+//                    flat padded grid of the strip; a step is a subspace; tap (kh,kw) is a constant shift kh*PW+kw.
+//   conv_roll_kernel any stride (conv1: 11x11 / 4): a CTA walks the input rows of its strip once; a step is an
+//                    (input row, subspace) pair, and each input row's LUT is used by the <= ceil(k/stride) output rows
+//                    that see it, each owned by a different "row group" of warps; columns are de-interleaved by stride
+//                    phase so that a tap again is a constant shift.
+// The LUT stage of a step is a [K x d] x [d x positions] contraction, produced by one of two policies (template
+// argument Lut) that own their shared-memory carve and operand staging:
+//   FfmaLut   the FP32 pipe, a register-blocked mini-GEMM: 8 codewords x 4 positions per thread, float2 FFMA pairs,
+//             codebook rows broadcast from shared memory, 128-bit LUT stores (fp32, ascending j: parity with the
+//             reference's saxpy order up to FMA contraction -- SURVEY.md 7.5).  Any K, subspaces wider than 8 dims in
+//             chunks of 8.
+//   WgmmaLut  the tensor cores (K = 128, d <= 8): 3xTF32 wgmma, ~5e-6 from the FFMA stage.
 #include "qcnn_internal.h"
+#include "async_copy.h"
 #include "wgmma.h"
 
 #include <algorithm>
@@ -34,26 +39,32 @@
 
 namespace {
 
+using qcnn::CpAsync4;
+using qcnn::CpAsyncCommit;
+using qcnn::CpAsyncWaitAll;
+
 // float2 arithmetic, element by element (sm_90 has no packed fp32 instructions)
 __device__ __forceinline__ float2 Ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ float2 Fadd2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 
 constexpr int kMaxThreads = 512;
 
+// describe() names of the LUT + gather kernels, and whether their LUT stage runs on the tensor cores (the two numerical
+// classes of the family)
+struct ConvKernelInfo {
+  const char* name;
+  bool tcLut;
+};
+constexpr ConvKernelInfo kConvKernelInfo[kConvDirect + 1] = {
+    {"conv_s1", false}, {"conv_roll", false}, {"conv_s1_tc(wgmma LUT)", true}, {"conv_roll_tc(wgmma LUT)", true},
+    {"conv_direct", false}};
+
 // ------------------------------------------------------------------------------------------------------------
-// Operand staging.  Everything the LUT stage of subspace s+1 needs from global memory (input pixels of the
+// Operand staging.  Everything the LUT stage of step i+1 needs from global memory (input pixels of the
 // subspace's channels, its codebook rows, its assignment slice) is copied ASYNCHRONOUSLY (cp.async, no registers)
-// into shared-memory staging buffers right before the gather of subspace s starts, and picked up after it ends,
+// into shared-memory staging buffers right before the gather of step i starts, and picked up after it ends,
 // so no global-load latency is exposed between the two stages.
 // ------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void CpAsync4(void* smemDst, const void* gsrc, bool valid) {
-  const uint32_t d = static_cast<uint32_t>(__cvta_generic_to_shared(smemDst));
-  const int sz = valid ? 4 : 0;  // src-size 0: nothing is read, the 4 destination bytes are zero-filled
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(d), "l"(gsrc), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void CpAsyncCommit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void CpAsyncWaitAll() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
-
 // raw codebook chunk: cbN[k*8 + jj] <- ctrd[s][k][jc + jj]   (zero beyond the subspace's real dims)
 __device__ __forceinline__ void FetchCodebook(float* __restrict__ cbN, const float* __restrict__ ctrd, int s, int K,
                                               int d, int jc, int nj, int tid, int T) {
@@ -107,8 +118,13 @@ __device__ __forceinline__ void FetchPixels(float* __restrict__ xs, const float*
   }
 }
 
+// dims of subspace s that exist (reference CaffeEva.cc:1277)
+__device__ __forceinline__ int SubspaceDims(const ConvArgs& a, int s) { return min(a.Cg - s * a.d, a.d); }
+// ... of them in the first chunk of 8
+__device__ __forceinline__ int FirstChunkDims(const ConvArgs& a, int s) { return max(0, min(8, SubspaceDims(a, s))); }
+
 // ------------------------------------------------------------------------------------------------------------
-// LUT stage: lut[k][p] (+)= sum_{jj<nj} cb[jj][k] * xs[jj][p], tile of 8 codewords x 4 positions per thread.
+// FFMA LUT stage: lut[k][p] (+)= sum_{jj<nj} cb[jj][k] * xs[jj][p], tile of 8 codewords x 4 positions per thread.
 // Lanes walk the position tiles (128-bit LUT stores and x loads are conflict-free, codebook loads broadcast).
 // ------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void LutStep(float2 (&acc)[8][2], const float2* __restrict__ cb2, const float* __restrict__ xs,
@@ -160,6 +176,283 @@ __device__ __forceinline__ void BuildLut(float* __restrict__ lut, const float2* 
       *reinterpret_cast<float4*>(lut + (k0 + k) * PP + p0) = make_float4(acc[k][0].x, acc[k][0].y, acc[k][1].x, acc[k][1].y);
   }
 }
+
+// ------------------------------------------------------------------------------------------------------------
+// wgmma LUT stage (K = 128 codewords, subspaces of <= 8 dims)
+//
+// The LUT of a step is the dense contraction  LUT[k][p] = sum_j ctrd[s][k][j] * x[p][j]  = C (128 x 8) * X^T (8 x N).
+// Per 32 LUT columns a warpgroup issues three wgmma.mma_async of tf32 operands (M = 64 codewords, N = 32, K = 8) -- the
+// 3xTF32 split  C_hi*X_hi + C_hi*X_lo + C_lo*X_hi  keeps fp32-level accuracy -- with both operands in shared memory and
+// the accumulator in its registers, which it then writes to lut[k][p].  The first two warpgroups of the CTA (the first
+// one alone in CTAs of fewer than eight warps) produce the LUT of a step at the stage boundary; all warps gather.
+// Operands reach the canonical K-major unswizzled tiles through cp.async (raw) + a hi/lo split pass.
+// ------------------------------------------------------------------------------------------------------------
+// canonical K-major operand tile without swizzle (tf32): rows in groups of 8, per group K-chunk 0 (8 rows x 16 B) then
+// K-chunk 1; element (row r, k) -> float index below.  Descriptor: LBO = 128 B (K chunks), SBO = 256 B (row groups).
+__device__ __forceinline__ int TileIdx(int r, int k) { return (r >> 3) * 64 + (k >> 2) * 32 + (r & 7) * 4 + (k & 3); }
+// LUT[128][NM] = A (128 codewords x 8) * B^T (NM positions x 8) as 3xTF32, written to lut (row pitch PP floats).
+// Called by all threads of warps 0 .. 4 nwg - 1 (nwg = 1 or 2 warpgroups); the tiles are published to the async proxy.
+__device__ __forceinline__ void LutMma(const float* aHi, const float* aLo, const float* bHi, const float* bLo, float* lut,
+                                       int PP, int NM, int warp, int lane, int nwg) {
+  const int wg = warp >> 2;
+  for (int half = wg; half < 2; half += nwg) {          // codewords [64 half, +64)
+    const uint64_t dAh = qcnn::WgmmaDesc(qcnn::SmemU32(aHi + half * 512), 128, 256);
+    const uint64_t dAl = qcnn::WgmmaDesc(qcnn::SmemU32(aLo + half * 512), 128, 256);
+    const int r0 = half * 64 + (warp & 3) * 16 + (lane >> 2);
+    for (int c = 0; c < (NM >> 5); c++) {               // 32 LUT columns = 4 row groups of the B tile
+      const uint64_t dBh = qcnn::WgmmaDesc(qcnn::SmemU32(bHi + c * 256), 128, 256);
+      const uint64_t dBl = qcnn::WgmmaDesc(qcnn::SmemU32(bLo + c * 256), 128, 256);
+      float d[16];
+#pragma unroll
+      for (int i = 0; i < 16; i++) d[i] = 0.0f;
+      qcnn::WgmmaFence();
+      qcnn::Wgmma<32>::Tf32SS(d, dAh, dBh);
+      qcnn::Wgmma<32>::Tf32SS(d, dAh, dBl);
+      qcnn::Wgmma<32>::Tf32SS(d, dAl, dBh);
+      qcnn::WgmmaCommit();
+      qcnn::WgmmaWaitAll();
+      // fragment: d[4 i + {0, 1}] = row r0, columns 8 i + 2 (lane % 4) + {0, 1}; d[4 i + {2, 3}] = row r0 + 8
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        const int col = c * 32 + 8 * i + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(lut + r0 * PP + col) = make_float2(d[4 * i], d[4 * i + 1]);
+        *reinterpret_cast<float2*>(lut + (r0 + 8) * PP + col) = make_float2(d[4 * i + 2], d[4 * i + 3]);
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// LUT stage policies.  A kernel walks steps 0 .. steps-1 as
+//     Prologue                                  operands of step 0 (wgmma: also step 1) in flight
+//     per step:  cp.async.wait_all; __syncthreads()   (A) staged operands have landed; the previous gather is done
+//                Produce(step)                  lut + idx of the step, complete for every thread on return
+//                Prefetch(step)                 operands of later steps fly in while this one is gathered
+//                gather
+// A step reads input LutSrc::src (the strip of the image, or one input row, of the CTA's group) and subspace
+// LutSrc::s; `at(i)` gives those of step i.  idx holds the LUT row offsets of the step's assignment slice; the rolling-row
+// kernel with one subspace keeps the slice of step 0 (commitOffsets / fetchOffsets false).
+// ------------------------------------------------------------------------------------------------------------
+struct LutSrc {
+  const float* src;
+  int s;
+};
+
+// What both policies take from the kernel
+struct LutBase {
+  const ConvArgs& a;
+  size_t chStride;        // source element stride between channels
+  const uint8_t* asmtG;   // assignments of the CTA's group and channel tile, subspace 0
+  int taps, tid, T;
+  uint32_t rowBytes;      // LUT row pitch in bytes
+  __device__ LutBase(const ConvArgs& a_, size_t chStride_, const uint8_t* asmtG_, int taps_)
+      : a(a_), chStride(chStride_), asmtG(asmtG_), taps(taps_), tid(threadIdx.x), T(blockDim.x),
+        rowBytes(static_cast<uint32_t>(a_.PP) * 4u) {}
+};
+
+struct FfmaLut : LutBase {
+  float* lut;      // [K][PP]
+  uint32_t* idx;   // [taps][CT]   LUT row byte offsets of the current step
+  float2* cb2;     // [8][K]       duplicated codebook chunk of the current step
+  float* xs;       // [2][8][PP]   input pixels, double-buffered (even / odd steps)
+  int* posoff;     // [PP]         LUT position -> element offset of its pixel (-1: zero padding), written by the kernel
+  float* cbN;      // [K*8]        raw codebook chunk of the next step (cp.async target)
+  uint8_t* idN;    // [taps*CT]    raw assignment slice of the next step (cp.async target)
+  int npos;        // entries of posoff
+
+  struct Map { int idx, cb2, xs, posoff, cbN, idN, bytes; };   // byte offsets; bytes = dynamic shared memory of a CTA
+  static __host__ __device__ Map MapSmem(int K, int PP, int NM, int taps, int CT) {
+    Map m;
+    int o = 4 * K * PP;                         // lut
+    m.idx = o;    o += 4 * taps * CT;
+    m.cb2 = o;    o += 8 * 8 * K;
+    m.xs = o;     o += 2 * 4 * 8 * PP;
+    m.posoff = o; o += 4 * PP;
+    m.cbN = o;    o += 4 * 8 * K;
+    m.idN = o;    o += (taps * CT + 15) & ~15;
+    m.bytes = o;
+    return m;
+  }
+
+  __device__ FfmaLut(unsigned char* smem, const LutBase& b) : LutBase(b), npos(b.a.PP) {
+    const Map m = MapSmem(a.K, a.PP, a.NM, taps, a.CT);
+    lut = reinterpret_cast<float*>(smem);
+    idx = reinterpret_cast<uint32_t*>(smem + m.idx);
+    cb2 = reinterpret_cast<float2*>(smem + m.cb2);
+    xs = reinterpret_cast<float*>(smem + m.xs);
+    posoff = reinterpret_cast<int*>(smem + m.posoff);
+    cbN = reinterpret_cast<float*>(smem + m.cbN);
+    idN = smem + m.idN;
+  }
+
+  __device__ float* Xs(int step) const { return xs + (step & 1) * 8 * a.PP; }
+
+  template <class At>
+  __device__ void Prologue(At at, int) {
+    const LutSrc in = at(0);
+    const int nj0 = FirstChunkDims(a, in.s);
+    FetchCodebook(cbN, a.ctrd, in.s, a.K, a.d, 0, nj0, tid, T);
+    FetchOffsets(idN, asmtG, taps, a.CT, a.KgPad, tid, T);
+    FetchPixels(Xs(0), in.src, posoff, a.PP, in.s * a.d, chStride, nj0, tid, T);
+    CpAsyncCommit();
+  }
+
+  __device__ void Produce(int step, int, LutSrc in, bool commitOffsets) {
+    const int dsel = SubspaceDims(a, in.s);
+    float* x = Xs(step);
+    CommitCodebook(cbN, cb2, a.K, tid, T);
+    if (commitOffsets) CommitOffsets(idN, idx, taps, a.CT, rowBytes, tid, T);
+    __syncthreads();  // (B)
+    BuildLut(lut, cb2, x, a.K, a.PP, max(0, min(8, dsel)), true, tid, T);
+    // the rare further chunks of subspaces wider than 8 dims, staged with exposed latency
+    for (int jc = 8; jc < dsel; jc += 8) {
+      const int nj = min(8, dsel - jc);
+      __syncthreads();
+      FetchCodebook(cbN, a.ctrd, in.s, a.K, a.d, jc, nj, tid, T);
+      FetchPixels(x, in.src, posoff, a.PP, in.s * a.d + jc, chStride, nj, tid, T);
+      CpAsyncCommit();
+      CpAsyncWaitAll();
+      __syncthreads();
+      CommitCodebook(cbN, cb2, a.K, tid, T);
+      __syncthreads();
+      BuildLut(lut, cb2, x, a.K, a.PP, nj, false, tid, T);
+    }
+    __syncthreads();  // (C) lut complete; cbN / idN / the other xs buffer are free
+  }
+
+  // operands of step + 1 (= next)
+  template <class At>
+  __device__ void Prefetch(int step, int steps, LutSrc next, At, bool fetchOffsets) {
+    if (step + 1 < steps) {
+      const int njn = FirstChunkDims(a, next.s);
+      FetchCodebook(cbN, a.ctrd, next.s, a.K, a.d, 0, njn, tid, T);
+      if (fetchOffsets) FetchOffsets(idN, asmtG + static_cast<size_t>(next.s) * taps * a.KgPad, taps, a.CT, a.KgPad, tid, T);
+      FetchPixels(Xs(step + 1), next.src, posoff, a.PP, next.s * a.d, chStride, njn, tid, T);
+      CpAsyncCommit();
+    }
+  }
+};
+
+struct WgmmaLut : LutBase {
+  float* lut;       // [128][PP]
+  uint32_t* idx;    // [taps][CT]
+  float* aHi;       // [128 x 8] canonical
+  float* aLo;
+  float* bHi;       // [NM x 8] canonical
+  float* bLo;
+  float* xr;        // [NM][8] raw pixels of a later step (cp.async target)
+  float* cr;        // [128][8] raw codebook of a later step
+  int* posoff;      // [NM]
+  uint8_t* idN;     // [taps*CT] raw assignment slice of the next step
+  int npos;         // entries of posoff: NM
+  int warp, lane;
+  int nwg;          // warpgroups that run the LUT MMAs
+
+  struct Map { int idx, aHi, aLo, bHi, bLo, xr, cr, posoff, idN, bytes; };
+  static __host__ __device__ Map MapSmem(int, int PP, int NM, int taps, int CT) {
+    Map m;
+    int o = 4 * 128 * PP;                       // lut
+    m.idx = o;    o += 4 * taps * CT;
+    m.aHi = o;    o += 4 * 1024;
+    m.aLo = o;    o += 4 * 1024;
+    m.bHi = o;    o += 4 * 8 * NM;
+    m.bLo = o;    o += 4 * 8 * NM;
+    m.xr = o;     o += 4 * 8 * NM;
+    m.cr = o;     o += 4 * 1024;
+    m.posoff = o; o += 4 * (NM + 8);
+    m.idN = o;    o += (taps * CT + 15) & ~15;
+    m.bytes = o;
+    return m;
+  }
+
+  __device__ WgmmaLut(unsigned char* smem, const LutBase& b) : LutBase(b), npos(b.a.NM) {
+    const Map m = MapSmem(a.K, a.PP, a.NM, taps, a.CT);
+    lut = reinterpret_cast<float*>(smem);
+    idx = reinterpret_cast<uint32_t*>(smem + m.idx);
+    aHi = reinterpret_cast<float*>(smem + m.aHi);
+    aLo = reinterpret_cast<float*>(smem + m.aLo);
+    bHi = reinterpret_cast<float*>(smem + m.bHi);
+    bLo = reinterpret_cast<float*>(smem + m.bLo);
+    xr = reinterpret_cast<float*>(smem + m.xr);
+    cr = reinterpret_cast<float*>(smem + m.cr);
+    posoff = reinterpret_cast<int*>(smem + m.posoff);
+    idN = smem + m.idN;
+    warp = tid >> 5;
+    lane = tid & 31;
+    nwg = (T >> 5) >= 8 ? 2 : 1;
+  }
+
+  // raw operands of a step: pixels [NM][8] and codebook [128][8], zero beyond the subspace's real dims
+  __device__ void FetchRaw(LutSrc in) {
+    const int nj = FirstChunkDims(a, in.s);
+    const float* cg = a.ctrd + static_cast<size_t>(in.s) * 128 * a.d;
+    for (int e = tid; e < 1024; e += T) {
+      const int k = e >> 3, jj = e & 7;
+      CpAsync4(cr + e, cg + (jj < nj ? k * a.d + jj : 0), jj < nj);
+    }
+    const int ch0 = in.s * a.d;
+    for (int e = tid; e < a.NM * 8; e += T) {
+      const int pos = e >> 3, jj = e & 7;
+      const int off = posoff[pos];
+      const bool ok = off >= 0 && jj < nj;
+      CpAsync4(xr + e, in.src + (ok ? off + (ch0 + jj) * chStride : 0), ok);
+    }
+  }
+  // raw -> hi/lo canonical operand tiles (generic-proxy writes, published to the async proxy by the caller's fence)
+  __device__ void SplitOperands() {
+    for (int e = tid; e < 1024; e += T) {
+      float hi, lo;
+      qcnn::SplitTf32(cr[e], hi, lo);
+      const int i = TileIdx(e >> 3, e & 7);
+      aHi[i] = hi;
+      aLo[i] = lo;
+    }
+    for (int e = tid; e < a.NM * 8; e += T) {
+      float hi, lo;
+      qcnn::SplitTf32(xr[e], hi, lo);
+      const int i = TileIdx(e >> 3, e & 7);
+      bHi[i] = hi;
+      bLo[i] = lo;
+    }
+  }
+
+  // operand tiles of step 0 published, raw operands of step 1 + assignment slice 0 in flight
+  template <class At>
+  __device__ void Prologue(At at, int steps) {
+    FetchRaw(at(0));
+    CpAsyncCommit();
+    CpAsyncWaitAll();
+    __syncthreads();
+    SplitOperands();
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    if (steps > 1) FetchRaw(at(1));
+    FetchOffsets(idN, asmtG, taps, a.CT, a.KgPad, tid, T);
+    CpAsyncCommit();
+  }
+
+  // tensor cores -> accumulator fragments -> lut; the operand tiles of step + 1 are split from the raw operands
+  __device__ void Produce(int step, int steps, LutSrc, bool commitOffsets) {
+    if (warp < 4 * nwg) LutMma(aHi, aLo, bHi, bLo, lut, a.PP, a.NM, warp, lane, nwg);
+    if (commitOffsets) CommitOffsets(idN, idx, taps, a.CT, rowBytes, tid, T);
+    if (step + 1 < steps) {
+      __syncthreads();  // the MMAs of this step have read the operand tiles
+      SplitOperands();
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    }
+    __syncthreads();  // (B) lut + idx ready, operand tiles of step + 1 published
+  }
+
+  // raw operands of step + 2, assignment slice of step + 1 (= next)
+  template <class At>
+  __device__ void Prefetch(int step, int steps, LutSrc next, At at, bool fetchOffsets) {
+    if (step + 1 < steps) {
+      if (step + 2 < steps) FetchRaw(at(step + 2));
+      if (fetchOffsets) FetchOffsets(idN, asmtG + static_cast<size_t>(next.s) * taps * a.KgPad, taps, a.CT, a.KgPad, tid, T);
+      CpAsyncCommit();
+    }
+  }
+};
 
 // ------------------------------------------------------------------------------------------------------------
 // gather stage
@@ -221,67 +514,40 @@ __device__ __forceinline__ void StoreChannels(float* __restrict__ out, const Acc
   }
 }
 
-struct SmemLayout {
-  float* lut;      // [K][PP]
-  uint32_t* idx;   // [taps][CT]   LUT row byte offsets of the current subspace
-  float2* cb2;     // [8][K]       duplicated codebook chunk of the current subspace
-  float* xs[2];    // [8][PP]      input pixels, double-buffered (current / next subspace)
-  int* posoff;     // [PP]
-  float* cbN;      // [K*8]        raw codebook chunk of the next subspace (cp.async target)
-  uint8_t* idN;    // [taps*CT]    raw assignment slice of the next subspace (cp.async target)
+// CTA coordinates of the LUT + gather and direct kernels: blockIdx.x = (group, channel tile, strip), strip fastest;
+// blockIdx.y = image
+struct CtaTile {
+  int strip, ct, g, n;
+  __device__ explicit CtaTile(const ConvArgs& a) {
+    int b = blockIdx.x;
+    strip = b % a.nstrips; b /= a.nstrips;
+    ct = b % a.nct;
+    g = b / a.nct;
+    n = blockIdx.y;
+  }
 };
-
-__device__ __forceinline__ SmemLayout Carve(unsigned char* smem, int K, int PP, int taps, int CT) {
-  SmemLayout s;
-  s.lut = reinterpret_cast<float*>(smem);
-  s.idx = reinterpret_cast<uint32_t*>(s.lut + static_cast<size_t>(K) * PP);
-  s.cb2 = reinterpret_cast<float2*>(s.idx + taps * CT);
-  s.xs[0] = reinterpret_cast<float*>(s.cb2 + 8 * K);
-  s.xs[1] = s.xs[0] + 8 * PP;
-  s.posoff = reinterpret_cast<int*>(s.xs[1] + 8 * PP);
-  s.cbN = reinterpret_cast<float*>(s.posoff + PP);
-  s.idN = reinterpret_cast<uint8_t*>(s.cbN + 8 * K);
-  return s;
-}
-
-// stage one (s, jc) chunk with exposed latency: only for the rare jc > 0 chunks of subspaces wider than 8 dims
-__device__ __forceinline__ void StageChunkDirect(const SmemLayout& sm, float* xs, const ConvArgs& a, const float* src,
-                                                 int s, int jc, int nj, int ch0, size_t chStride, int tid, int T) {
-  FetchCodebook(sm.cbN, a.ctrd, s, a.K, a.d, jc, nj, tid, T);
-  FetchPixels(xs, src, sm.posoff, a.PP, ch0, chStride, nj, tid, T);
-  CpAsyncCommit();
-  CpAsyncWaitAll();
-  __syncthreads();
-  CommitCodebook(sm.cbN, sm.cb2, a.K, tid, T);
-}
 
 // ------------------------------------------------------------------------------------------------------------
 // stride-1 kernel
 // ------------------------------------------------------------------------------------------------------------
 // MAXT: launch bound (256 / 384 / 512 threads) -> register cap 255 / 168 / 128, so small CTAs never spill
-template <int CPT, int J, int MAXT>
+template <class Lut, int CPT, int J, int MAXT>
 __global__ void __launch_bounds__(MAXT, 1) conv_s1_kernel(const ConvArgs a) {
-  extern __shared__ __align__(16) unsigned char smem[];
+  extern __shared__ __align__(128) unsigned char smem[];
   const int taps = a.ksz * a.ksz;
-  const SmemLayout sm = Carve(smem, a.K, a.PP, taps, a.CT);
-
   const int tid = threadIdx.x, T = blockDim.x;
   const int warp = tid >> 5, lane = tid & 31;
   const int pw = warp % a.pwarps, cw = warp / a.pwarps;
-  int b = blockIdx.x;
-  const int strip = b % a.nstrips; b /= a.nstrips;
-  const int ct = b % a.nct;
-  const int g = b / a.nct;
-  const int n = blockIdx.y;
-  const int r0 = strip * a.R;            // first output row of the strip
-  const int hin0 = r0 - a.pad;           // input row held at ri = 0
-  const int q0 = pw * 32 * J + lane;     // first flat position of this thread (others at +32 j)
-  const int cbase = ct * a.CT + cw * CPT;  // first channel (within the group) of this thread
-  const float* src = a.src + static_cast<size_t>(n) * a.Hi * a.Wi * a.Cin + g * a.Cg;
-  const uint8_t* asmtG = a.asmt + static_cast<size_t>(g) * a.S * taps * a.KgPad + ct * a.CT;
+  const CtaTile t(a);
+  const int r0 = t.strip * a.R;            // first output row of the strip
+  const int hin0 = r0 - a.pad;             // input row held at ri = 0
+  const int q0 = pw * 32 * J + lane;       // first flat position of this thread (others at +32 j)
+  const int cbase = t.ct * a.CT + cw * CPT;  // first channel (within the group) of this thread
+  const float* src = a.src + static_cast<size_t>(t.n) * a.Hi * a.Wi * a.Cin + t.g * a.Cg;
+  Lut lut(smem, LutBase(a, 1, a.asmt + static_cast<size_t>(t.g) * a.S * taps * a.KgPad + t.ct * a.CT, taps));
 
   // LUT position -> source pixel (NHWC element offset within this image/group), -1 = zero padding
-  for (int pos = tid; pos < a.PP; pos += T) {
+  for (int pos = tid; pos < lut.npos; pos += T) {
     int off = -1;
     const int pp = pos - a.pad;
     if (pp >= 0) {
@@ -289,54 +555,27 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_kernel(const ConvArgs a) {
       const int hi = hin0 + ri;
       if (ri < a.RI && wi < a.Wi && hi >= 0 && hi < a.Hi) off = (hi * a.Wi + wi) * a.Cin;
     }
-    sm.posoff[pos] = off;
+    lut.posoff[pos] = off;
   }
 
   Acc<CPT, J> acc;
   {
     float bv[CPT];
 #pragma unroll
-    for (int c = 0; c < CPT; c++) bv[c] = __ldg(a.bias + g * a.Kg + cbase + c);
+    for (int c = 0; c < CPT; c++) bv[c] = __ldg(a.bias + t.g * a.Kg + cbase + c);
     acc.Fill(bv);
   }
   __syncthreads();  // posoff visible
 
-  const uint32_t rowBytes = static_cast<uint32_t>(a.PP) * 4u;
-  {
-    const int nj0 = max(0, min(8, min(a.Cg, a.d)));
-    FetchCodebook(sm.cbN, a.ctrd, 0, a.K, a.d, 0, nj0, tid, T);
-    FetchOffsets(sm.idN, asmtG, taps, a.CT, a.KgPad, tid, T);
-    FetchPixels(sm.xs[0], src, sm.posoff, a.PP, 0, 1, nj0, tid, T);
-    CpAsyncCommit();
-  }
+  const auto at = [&](int s) { return LutSrc{src, s}; };   // step = subspace
+  lut.Prologue(at, a.S);
   for (int s = 0; s < a.S; s++) {
-    const int dsel = min(a.Cg - s * a.d, a.d);  // dims of this subspace that exist (reference CaffeEva.cc:1277)
-    float* xs = sm.xs[s & 1];
-    // ---- LUT stage ----
     CpAsyncWaitAll();
-    __syncthreads();  // (A) staged operands of s have landed; the previous gather is done with lut / idx
-    CommitCodebook(sm.cbN, sm.cb2, a.K, tid, T);
-    CommitOffsets(sm.idN, sm.idx, taps, a.CT, rowBytes, tid, T);
-    __syncthreads();  // (B)
-    BuildLut(sm.lut, sm.cb2, xs, a.K, a.PP, max(0, min(8, dsel)), true, tid, T);
-    for (int jc = 8; jc < dsel; jc += 8) {
-      const int nj = min(8, dsel - jc);
-      __syncthreads();
-      StageChunkDirect(sm, xs, a, src, s, jc, nj, s * a.d + jc, 1, tid, T);
-      __syncthreads();
-      BuildLut(sm.lut, sm.cb2, xs, a.K, a.PP, nj, false, tid, T);
-    }
-    __syncthreads();  // (C) lut complete; cbN / idN / the other xs buffer are free
-    if (s + 1 < a.S) {  // operands of the next subspace fly in while this one is gathered
-      const int njn = max(0, min(8, min(a.Cg - (s + 1) * a.d, a.d)));
-      FetchCodebook(sm.cbN, a.ctrd, s + 1, a.K, a.d, 0, njn, tid, T);
-      FetchOffsets(sm.idN, asmtG + static_cast<size_t>(s + 1) * taps * a.KgPad, taps, a.CT, a.KgPad, tid, T);
-      FetchPixels(sm.xs[(s + 1) & 1], src, sm.posoff, a.PP, (s + 1) * a.d, 1, njn, tid, T);
-      CpAsyncCommit();
-    }
-    // ---- gather stage ----
-    const char* lutq = reinterpret_cast<const char*>(sm.lut) + q0 * 4;
-    const uint32_t* ip = sm.idx + cw * CPT;
+    __syncthreads();  // (A)
+    lut.Produce(s, a.S, at(s), true);
+    lut.Prefetch(s, a.S, at(s + 1), at, true);
+    const char* lutq = reinterpret_cast<const char*>(lut.lut) + q0 * 4;
+    const uint32_t* ip = lut.idx + cw * CPT;
     for (int kh = 0; kh < a.ksz; kh++) {
       for (int kw = 0; kw < a.ksz; kw++) {
         GatherTap<CPT, J>(acc, lutq + (kh * a.PW + kw) * 4, ip);
@@ -351,217 +590,7 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_kernel(const ConvArgs a) {
     const int r = q / a.PW, wo = q - r * a.PW;
     const int ho = r0 + r;
     if (r < a.R && wo < a.Wo && ho < a.Ho) {
-      float* out = a.dst + ((static_cast<size_t>(n) * a.Ho + ho) * a.Wo + wo) * a.Cout + g * a.Kg + cbase;
-      StoreChannels<CPT, J>(out, acc, j, a.relu);
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// stride-1 kernel, tensor-core LUT stage (K = 128 codewords, subspaces of <= 8 dims)
-//
-// The LUT of a subspace is the dense contraction  LUT[k][p] = sum_j ctrd[s][k][j] * x[p][j]  = C (128 x 8) * X^T (8 x N).
-// Here it runs on the Hopper tensor cores: per 32 LUT columns a warpgroup issues three wgmma.mma_async of tf32 operands
-// (M = 64 codewords, N = 32, K = 8) -- the 3xTF32 split  C_hi*X_hi + C_hi*X_lo + C_lo*X_hi  keeps fp32-level accuracy --
-// with both operands in shared memory and the accumulator in its registers, which it then writes to lut[k][p].  The
-// first two warpgroups of the CTA (the first one alone in CTAs of fewer than eight warps) produce the LUT of a subspace
-// at the stage boundary; all warps gather.  Operands reach the canonical K-major unswizzled tiles through cp.async (raw)
-// + a hi/lo split pass.
-// ------------------------------------------------------------------------------------------------------------
-// canonical K-major operand tile without swizzle (tf32): rows in groups of 8, per group K-chunk 0 (8 rows x 16 B) then
-// K-chunk 1; element (row r, k) -> float index below.  Descriptor: LBO = 128 B (K chunks), SBO = 256 B (row groups).
-__device__ __forceinline__ int TileIdx(int r, int k) { return (r >> 3) * 64 + (k >> 2) * 32 + (r & 7) * 4 + (k & 3); }
-// hi = value truncated to tf32 (what the tensor core reads), lo = exact remainder
-__device__ __forceinline__ void SplitTf32(float v, float& hi, float& lo) {
-  hi = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
-  lo = v - hi;
-}
-// LUT[128][NM] = A (128 codewords x 8) * B^T (NM positions x 8) as 3xTF32, written to lut (row pitch PP floats).
-// Called by all threads of warps 0 .. 4 nwg - 1 (nwg = 1 or 2 warpgroups); the tiles are published to the async proxy.
-__device__ __forceinline__ void LutMma(const float* aHi, const float* aLo, const float* bHi, const float* bLo, float* lut,
-                                       int PP, int NM, int warp, int lane, int nwg) {
-  const int wg = warp >> 2;
-  for (int half = wg; half < 2; half += nwg) {          // codewords [64 half, +64)
-    const uint64_t dAh = qcnn::WgmmaDesc(qcnn::SmemU32(aHi + half * 512), 128, 256);
-    const uint64_t dAl = qcnn::WgmmaDesc(qcnn::SmemU32(aLo + half * 512), 128, 256);
-    const int r0 = half * 64 + (warp & 3) * 16 + (lane >> 2);
-    for (int c = 0; c < (NM >> 5); c++) {               // 32 LUT columns = 4 row groups of the B tile
-      const uint64_t dBh = qcnn::WgmmaDesc(qcnn::SmemU32(bHi + c * 256), 128, 256);
-      const uint64_t dBl = qcnn::WgmmaDesc(qcnn::SmemU32(bLo + c * 256), 128, 256);
-      float d[16];
-#pragma unroll
-      for (int i = 0; i < 16; i++) d[i] = 0.0f;
-      qcnn::WgmmaFence();
-      qcnn::Wgmma<32>::Tf32SS(d, dAh, dBh);
-      qcnn::Wgmma<32>::Tf32SS(d, dAh, dBl);
-      qcnn::Wgmma<32>::Tf32SS(d, dAl, dBh);
-      qcnn::WgmmaCommit();
-      qcnn::WgmmaWaitAll();
-      // fragment: d[4 i + {0, 1}] = row r0, columns 8 i + 2 (lane % 4) + {0, 1}; d[4 i + {2, 3}] = row r0 + 8
-#pragma unroll
-      for (int i = 0; i < 4; i++) {
-        const int col = c * 32 + 8 * i + 2 * (lane & 3);
-        *reinterpret_cast<float2*>(lut + r0 * PP + col) = make_float2(d[4 * i], d[4 * i + 1]);
-        *reinterpret_cast<float2*>(lut + (r0 + 8) * PP + col) = make_float2(d[4 * i + 2], d[4 * i + 3]);
-      }
-    }
-  }
-}
-
-
-struct SmemLayoutTc {
-  float* lut;       // [128][PP]
-  uint32_t* idx;    // [taps][CT]
-  float* aHi;       // [128 x 8] canonical
-  float* aLo;
-  float* bHi;       // [NM x 8] canonical
-  float* bLo;
-  float* xr;        // [NM][8] raw pixels of the next subspace (cp.async target)
-  float* cr;        // [128][8] raw codebook of the next subspace
-  uint8_t* idN;     // [taps*CT] raw assignment slice
-  int* posoff;      // [NM]
-};
-__device__ __forceinline__ SmemLayoutTc CarveTc(unsigned char* smem, int PP, int NM, int taps, int CT) {
-  SmemLayoutTc s;
-  s.lut = reinterpret_cast<float*>(smem);
-  s.idx = reinterpret_cast<uint32_t*>(s.lut + 128 * PP);
-  s.aHi = reinterpret_cast<float*>(s.idx + taps * CT);
-  s.aLo = s.aHi + 1024;
-  s.bHi = s.aLo + 1024;
-  s.bLo = s.bHi + NM * 8;
-  s.xr = s.bLo + NM * 8;
-  s.cr = s.xr + NM * 8;
-  s.posoff = reinterpret_cast<int*>(s.cr + 1024);
-  s.idN = reinterpret_cast<uint8_t*>(s.posoff + NM + 4);
-  return s;
-}
-
-template <int CPT, int J, int MAXT>
-__global__ void __launch_bounds__(MAXT, 1) conv_s1_tc_kernel(const ConvArgs a) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  const int taps = a.ksz * a.ksz;
-  const int NM = a.RI;  // MMA N: LUT columns produced per subspace (multiple of 32, <= 256); a.RI is reused for it
-  const SmemLayoutTc sm = CarveTc(smem, a.PP, NM, taps, a.CT);
-
-  const int tid = threadIdx.x, T = blockDim.x;
-  const int warp = tid >> 5, lane = tid & 31, nwarps = T >> 5;
-  const int pw = warp % a.pwarps, cw = warp / a.pwarps;
-  int b = blockIdx.x;
-  const int strip = b % a.nstrips; b /= a.nstrips;
-  const int ct = b % a.nct;
-  const int g = b / a.nct;
-  const int n = blockIdx.y;
-  const int r0 = strip * a.R;
-  const int hin0 = r0 - a.pad;
-  const int rowsIn = a.R + a.ksz - 1;
-  const int q0 = pw * 32 * J + lane;
-  const int cbase = ct * a.CT + cw * CPT;
-  const float* src = a.src + static_cast<size_t>(n) * a.Hi * a.Wi * a.Cin + g * a.Cg;
-  const uint8_t* asmtG = a.asmt + static_cast<size_t>(g) * a.S * taps * a.KgPad + ct * a.CT;
-
-  for (int pos = tid; pos < NM; pos += T) {
-    int off = -1;
-    const int pp = pos - a.pad;
-    if (pp >= 0) {
-      const int ri = pp / a.PW, wi = pp - ri * a.PW;
-      const int hi = hin0 + ri;
-      if (ri < rowsIn && wi < a.Wi && hi >= 0 && hi < a.Hi) off = (hi * a.Wi + wi) * a.Cin;
-    }
-    sm.posoff[pos] = off;
-  }
-
-  Acc<CPT, J> acc;
-  {
-    float bv[CPT];
-#pragma unroll
-    for (int c = 0; c < CPT; c++) bv[c] = __ldg(a.bias + g * a.Kg + cbase + c);
-    acc.Fill(bv);
-  }
-  __syncthreads();  // posoff visible
-  const int nwg = nwarps >= 8 ? 2 : 1;   // warpgroups that run the LUT MMAs
-  const uint32_t rowBytes = static_cast<uint32_t>(a.PP) * 4u;
-
-  // raw operands of subspace s: pixels [NM][8] and codebook [128][8], zero beyond the subspace's real dims
-  auto fetchRaw = [&](int s) {
-    const int nj = max(0, min(8, min(a.Cg - s * a.d, a.d)));
-    const float* cg = a.ctrd + static_cast<size_t>(s) * 128 * a.d;
-    for (int e = tid; e < 1024; e += T) {
-      const int k = e >> 3, jj = e & 7;
-      CpAsync4(sm.cr + e, cg + (jj < nj ? k * a.d + jj : 0), jj < nj);
-    }
-    const int ch0 = s * a.d;
-    for (int e = tid; e < NM * 8; e += T) {
-      const int pos = e >> 3, jj = e & 7;
-      const int off = sm.posoff[pos];
-      const bool ok = off >= 0 && jj < nj;
-      CpAsync4(sm.xr + e, src + (ok ? off + ch0 + jj : 0), ok);
-    }
-  };
-  // raw -> hi/lo canonical operand tiles (generic-proxy writes, published to the async proxy by the caller's fence)
-  auto splitOperands = [&]() {
-    for (int e = tid; e < 1024; e += T) {
-      float hi, lo;
-      SplitTf32(sm.cr[e], hi, lo);
-      const int i = TileIdx(e >> 3, e & 7);
-      sm.aHi[i] = hi;
-      sm.aLo[i] = lo;
-    }
-    for (int e = tid; e < NM * 8; e += T) {
-      float hi, lo;
-      SplitTf32(sm.xr[e], hi, lo);
-      const int i = TileIdx(e >> 3, e & 7);
-      sm.bHi[i] = hi;
-      sm.bLo[i] = lo;
-    }
-  };
-
-  // prologue: operand tiles of subspace 0 published, raw operands of subspace 1 + assignment slice 0 in flight
-  fetchRaw(0);
-  CpAsyncCommit();
-  CpAsyncWaitAll();
-  __syncthreads();
-  splitOperands();
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  __syncthreads();
-  if (a.S > 1) fetchRaw(1);
-  FetchOffsets(sm.idN, asmtG, taps, a.CT, a.KgPad, tid, T);
-  CpAsyncCommit();
-
-  for (int s = 0; s < a.S; s++) {
-    CpAsyncWaitAll();
-    __syncthreads();            // (A) gather(s-1) is done with lut/idx; operand tiles of s, raw operands of s+1 and idN(s) are visible
-    // LUT(s): tensor cores -> accumulator fragments -> lut
-    if (warp < 4 * nwg) LutMma(sm.aHi, sm.aLo, sm.bHi, sm.bLo, sm.lut, a.PP, NM, warp, lane, nwg);
-    CommitOffsets(sm.idN, sm.idx, taps, a.CT, rowBytes, tid, T);
-    if (s + 1 < a.S) {
-      __syncthreads();          // the MMAs of subspace s have read the operand tiles
-      splitOperands();
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    __syncthreads();            // (B) lut + idx ready, operand tiles of s+1 published
-    if (s + 1 < a.S) {
-      if (s + 2 < a.S) fetchRaw(s + 2);
-      FetchOffsets(sm.idN, asmtG + static_cast<size_t>(s + 1) * taps * a.KgPad, taps, a.CT, a.KgPad, tid, T);
-      CpAsyncCommit();
-    }
-    // ---- gather stage ----
-    const char* lutq = reinterpret_cast<const char*>(sm.lut) + q0 * 4;
-    const uint32_t* ip = sm.idx + cw * CPT;
-    for (int kh = 0; kh < a.ksz; kh++) {
-      for (int kw = 0; kw < a.ksz; kw++) {
-        GatherTap<CPT, J>(acc, lutq + (kh * a.PW + kw) * 4, ip);
-        ip += a.CT;
-      }
-    }
-  }
-
-#pragma unroll
-  for (int j = 0; j < J; j++) {
-    const int q = q0 + 32 * j;
-    const int r = q / a.PW, wo = q - r * a.PW;
-    const int ho = r0 + r;
-    if (r < a.R && wo < a.Wo && ho < a.Ho) {
-      float* out = a.dst + ((static_cast<size_t>(n) * a.Ho + ho) * a.Wo + wo) * a.Cout + g * a.Kg + cbase;
+      float* out = a.dst + ((static_cast<size_t>(t.n) * a.Ho + ho) * a.Wo + wo) * a.Cout + t.g * a.Kg + cbase;
       StoreChannels<CPT, J>(out, acc, j, a.relu);
     }
   }
@@ -570,290 +599,89 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_tc_kernel(const ConvArgs a) {
 // ------------------------------------------------------------------------------------------------------------
 // rolling-row kernel (any stride)
 // ------------------------------------------------------------------------------------------------------------
-template <int CPT, int J, int MAXT>
+template <class Lut, int CPT, int J, int MAXT>
 __global__ void __launch_bounds__(MAXT, 1) conv_roll_kernel(const ConvArgs a) {
-  extern __shared__ __align__(16) unsigned char smem[];
+  extern __shared__ __align__(128) unsigned char smem[];
   const int taps = a.ksz * a.ksz;
-  const SmemLayout sm = Carve(smem, a.K, a.PP, taps, a.CT);  // PP = stride * PH (rounded)
-
   const int tid = threadIdx.x, T = blockDim.x;
   const int warp = tid >> 5, lane = tid & 31;
   const int rg = warp % a.rgroups;
   const int rest = warp / a.rgroups;
   const int pw = rest % a.pwarps, cw = rest / a.pwarps;
-  int b = blockIdx.x;
-  const int strip = b % a.nstrips; b /= a.nstrips;
-  const int ct = b % a.nct;
-  const int g = b / a.nct;
-  const int n = blockIdx.y;
-  const int ho0 = strip * a.R;
+  const CtaTile t(a);
+  const int ho0 = t.strip * a.R;
   const int ho_end = min(a.Ho, ho0 + a.R);
   const int PH = a.PW;
   const int wo0 = pw * 32 * J + lane;
-  const int cbase = ct * a.CT + cw * CPT;
+  const int cbase = t.ct * a.CT + cw * CPT;
   // source addressing: pixel (hi, wi), channel ch  ->  base + hi*rowStride + wi*pixStride + ch*chStride
   const size_t chStride = a.src_nchw ? static_cast<size_t>(a.Hi) * a.Wi : 1;
   const int pixStride = a.src_nchw ? 1 : a.Cin;
   const size_t rowStride = static_cast<size_t>(a.Wi) * pixStride;
-  const float* src = a.src + static_cast<size_t>(n) * a.Hi * a.Wi * a.Cin + static_cast<size_t>(g) * a.Cg * chStride;
-  const uint8_t* asmtG = a.asmt + static_cast<size_t>(g) * a.S * taps * a.KgPad + ct * a.CT;
+  const float* src = a.src + static_cast<size_t>(t.n) * a.Hi * a.Wi * a.Cin + static_cast<size_t>(t.g) * a.Cg * chStride;
+  Lut lut(smem, LutBase(a, chStride, a.asmt + static_cast<size_t>(t.g) * a.S * taps * a.KgPad + t.ct * a.CT, taps));
 
   // LUT position (phase-major de-interleaved column) -> element offset of the pixel inside its input row
-  for (int pos = tid; pos < a.PP; pos += T) {
+  for (int pos = tid; pos < lut.npos; pos += T) {
     const int phase = pos / PH, i = pos - phase * PH;
     const int wi = i * a.stride + phase - a.pad;
-    sm.posoff[pos] = (phase < a.stride && wi >= 0 && wi < a.Wi) ? wi * pixStride : -1;
+    lut.posoff[pos] = (phase < a.stride && wi >= 0 && wi < a.Wi) ? wi * pixStride : -1;
   }
 
   float bias[CPT];
 #pragma unroll
-  for (int c = 0; c < CPT; c++) bias[c] = __ldg(a.bias + g * a.Kg + cbase + c);
+  for (int c = 0; c < CPT; c++) bias[c] = __ldg(a.bias + t.g * a.Kg + cbase + c);
   Acc<CPT, J> acc;
   acc.Fill(bias);
   int ho_cur = ho0 + rg;  // output row this warp is accumulating
   __syncthreads();        // posoff visible
 
-  const uint32_t rowBytes = static_cast<uint32_t>(a.PP) * 4u;
   const int hi_begin = ho0 * a.stride - a.pad;
   const int hi_end = (ho_end - 1) * a.stride - a.pad + a.ksz;
   const int hi_lo = max(hi_begin, 0), hi_hi = min(hi_end, a.Hi);  // rows outside the image contribute nothing
   const int steps = (hi_hi - hi_lo) * a.S;                         // (input row, subspace) pairs, row-major
+  const auto at = [&](int step) { return LutSrc{src + (hi_lo + step / a.S) * rowStride, step % a.S}; };
+  // the current output row has seen its last input row: store it and move on to the row group's next one
+  const auto emitRow = [&]() {
+#pragma unroll
+    for (int j = 0; j < J; j++) {
+      const int wo = wo0 + 32 * j;
+      if (wo < a.Wo) {
+        float* out = a.dst + ((static_cast<size_t>(t.n) * a.Ho + ho_cur) * a.Wo + wo) * a.Cout + t.g * a.Kg + cbase;
+        StoreChannels<CPT, J>(out, acc, j, a.relu);
+      }
+    }
+    acc.Fill(bias);
+    ho_cur += a.rgroups;
+  };
 
-  if (steps > 0) {
-    const int nj0 = max(0, min(8, min(a.Cg, a.d)));
-    FetchCodebook(sm.cbN, a.ctrd, 0, a.K, a.d, 0, nj0, tid, T);
-    FetchOffsets(sm.idN, asmtG, taps, a.CT, a.KgPad, tid, T);
-    FetchPixels(sm.xs[0], src + hi_lo * rowStride, sm.posoff, a.PP, 0, chStride, nj0, tid, T);
-    CpAsyncCommit();
-  }
+  if (steps > 0) lut.Prologue(at, steps);
   int hi = hi_lo, s = 0;
   for (int it = 0; it < steps; it++) {
-    const int dsel = min(a.Cg - s * a.d, a.d);
     const int kh = hi + a.pad - ho_cur * a.stride;  // warp-uniform
     const bool active = ho_cur < ho_end && kh >= 0 && kh < a.ksz;
-    float* xs = sm.xs[it & 1];
     CpAsyncWaitAll();
     __syncthreads();  // (A)
-    CommitCodebook(sm.cbN, sm.cb2, a.K, tid, T);
-    if (a.S > 1 || it == 0) CommitOffsets(sm.idN, sm.idx, taps, a.CT, rowBytes, tid, T);
-    __syncthreads();  // (B)
-    BuildLut(sm.lut, sm.cb2, xs, a.K, a.PP, max(0, min(8, dsel)), true, tid, T);
-    for (int jc = 8; jc < dsel; jc += 8) {
-      const int nj = min(8, dsel - jc);
-      __syncthreads();
-      StageChunkDirect(sm, xs, a, src + hi * rowStride, s, jc, nj, s * a.d + jc, chStride, tid, T);
-      __syncthreads();
-      BuildLut(sm.lut, sm.cb2, xs, a.K, a.PP, nj, false, tid, T);
-    }
-    __syncthreads();  // (C)
-    // next (row, subspace)
-    int hin = hi, sn = s + 1;
+    lut.Produce(it, steps, LutSrc{src + hi * rowStride, s}, a.S > 1 || it == 0);
+    int hin = hi, sn = s + 1;  // next (row, subspace)
     if (sn == a.S) { sn = 0; hin = hi + 1; }
-    if (it + 1 < steps) {
-      const int njn = max(0, min(8, min(a.Cg - sn * a.d, a.d)));
-      FetchCodebook(sm.cbN, a.ctrd, sn, a.K, a.d, 0, njn, tid, T);
-      if (a.S > 1) FetchOffsets(sm.idN, asmtG + static_cast<size_t>(sn) * taps * a.KgPad, taps, a.CT, a.KgPad, tid, T);
-      FetchPixels(sm.xs[(it + 1) & 1], src + hin * rowStride, sm.posoff, a.PP, sn * a.d, chStride, njn, tid, T);
-      CpAsyncCommit();
-    }
+    lut.Prefetch(it, steps, LutSrc{src + hin * rowStride, sn}, at, a.S > 1);
     if (active) {
-      const char* lutq = reinterpret_cast<const char*>(sm.lut) + wo0 * 4;
-      const uint32_t* ip = sm.idx + (kh * a.ksz) * a.CT + cw * CPT;
+      const char* lutq = reinterpret_cast<const char*>(lut.lut) + wo0 * 4;
+      const uint32_t* ip = lut.idx + (kh * a.ksz) * a.CT + cw * CPT;
       for (int kw = 0; kw < a.ksz; kw++) {
         const int phase = kw % a.stride, sh = kw / a.stride;
         GatherTap<CPT, J>(acc, lutq + (phase * PH + sh) * 4, ip);
         ip += a.CT;
       }
     }
-    // this input row was the last one the current output row needs: emit it and move on
-    if (s == a.S - 1 && ho_cur < ho_end && kh == a.ksz - 1) {
-#pragma unroll
-      for (int j = 0; j < J; j++) {
-        const int wo = wo0 + 32 * j;
-        if (wo < a.Wo) {
-          float* out = a.dst + ((static_cast<size_t>(n) * a.Ho + ho_cur) * a.Wo + wo) * a.Cout + g * a.Kg + cbase;
-          StoreChannels<CPT, J>(out, acc, j, a.relu);
-        }
-      }
-      acc.Fill(bias);
-      ho_cur += a.rgroups;
-    }
+    if (s == a.S - 1 && ho_cur < ho_end && kh == a.ksz - 1) emitRow();
     hi = hin; s = sn;
   }
   // output rows whose window ends below the image (padding rows were skipped above)
   for (int h = max(hi_hi, hi_begin); h < hi_end; h++) {
     const int kh = h + a.pad - ho_cur * a.stride;
-    if (ho_cur < ho_end && kh == a.ksz - 1) {
-#pragma unroll
-      for (int j = 0; j < J; j++) {
-        const int wo = wo0 + 32 * j;
-        if (wo < a.Wo) {
-          float* out = a.dst + ((static_cast<size_t>(n) * a.Ho + ho_cur) * a.Wo + wo) * a.Cout + g * a.Kg + cbase;
-          StoreChannels<CPT, J>(out, acc, j, a.relu);
-        }
-      }
-      acc.Fill(bias);
-      ho_cur += a.rgroups;
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// rolling-row kernel, tensor-core LUT stage: same row-group structure as conv_roll_kernel; the LUT of an
-// (input row, subspace) step is produced by wgmma (LutMma) instead of the FFMA build.
-// ------------------------------------------------------------------------------------------------------------
-template <int CPT, int J, int MAXT>
-__global__ void __launch_bounds__(MAXT, 1) conv_roll_tc_kernel(const ConvArgs a) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  const int taps = a.ksz * a.ksz;
-  const int NM = a.RI;  // MMA N (multiple of 32, <= 256)
-  const SmemLayoutTc sm = CarveTc(smem, a.PP, NM, taps, a.CT);
-
-  const int tid = threadIdx.x, T = blockDim.x;
-  const int warp = tid >> 5, lane = tid & 31, nwarps = T >> 5;
-  const int rg = warp % a.rgroups;
-  const int rest = warp / a.rgroups;
-  const int pw = rest % a.pwarps, cw = rest / a.pwarps;
-  int b = blockIdx.x;
-  const int strip = b % a.nstrips; b /= a.nstrips;
-  const int ct = b % a.nct;
-  const int g = b / a.nct;
-  const int n = blockIdx.y;
-  const int ho0 = strip * a.R;
-  const int ho_end = min(a.Ho, ho0 + a.R);
-  const int PH = a.PW;
-  const int wo0 = pw * 32 * J + lane;
-  const int cbase = ct * a.CT + cw * CPT;
-  const size_t chStride = a.src_nchw ? static_cast<size_t>(a.Hi) * a.Wi : 1;
-  const int pixStride = a.src_nchw ? 1 : a.Cin;
-  const size_t rowStride = static_cast<size_t>(a.Wi) * pixStride;
-  const float* src = a.src + static_cast<size_t>(n) * a.Hi * a.Wi * a.Cin + static_cast<size_t>(g) * a.Cg * chStride;
-  const uint8_t* asmtG = a.asmt + static_cast<size_t>(g) * a.S * taps * a.KgPad + ct * a.CT;
-
-  for (int pos = tid; pos < NM; pos += T) {
-    const int phase = pos / PH, i = pos - phase * PH;
-    const int wi = i * a.stride + phase - a.pad;
-    sm.posoff[pos] = (phase < a.stride && wi >= 0 && wi < a.Wi) ? wi * pixStride : -1;
-  }
-  float bias[CPT];
-#pragma unroll
-  for (int c = 0; c < CPT; c++) bias[c] = __ldg(a.bias + g * a.Kg + cbase + c);
-  Acc<CPT, J> acc;
-  acc.Fill(bias);
-  int ho_cur = ho0 + rg;
-  __syncthreads();
-  const int nwg = nwarps >= 8 ? 2 : 1;   // warpgroups that run the LUT MMAs
-  const uint32_t rowBytes = static_cast<uint32_t>(a.PP) * 4u;
-
-  const int hi_begin = ho0 * a.stride - a.pad;
-  const int hi_end = (ho_end - 1) * a.stride - a.pad + a.ksz;
-  const int hi_lo = max(hi_begin, 0), hi_hi = min(hi_end, a.Hi);
-  const int steps = (hi_hi - hi_lo) * a.S;
-
-  auto fetchRaw = [&](int step) {  // step = (hi - hi_lo) * S + s
-    const int hi = hi_lo + step / a.S, s = step % a.S;
-    const int nj = max(0, min(8, min(a.Cg - s * a.d, a.d)));
-    const float* cg = a.ctrd + static_cast<size_t>(s) * 128 * a.d;
-    for (int e = tid; e < 1024; e += T) {
-      const int k = e >> 3, jj = e & 7;
-      CpAsync4(sm.cr + e, cg + (jj < nj ? k * a.d + jj : 0), jj < nj);
-    }
-    const float* rowp = src + hi * rowStride;
-    const int ch0 = s * a.d;
-    for (int e = tid; e < NM * 8; e += T) {
-      const int pos = e >> 3, jj = e & 7;
-      const int off = sm.posoff[pos];
-      const bool ok = off >= 0 && jj < nj;
-      CpAsync4(sm.xr + e, rowp + (ok ? off + (ch0 + jj) * chStride : 0), ok);
-    }
-  };
-  auto splitOperands = [&]() {
-    for (int e = tid; e < 1024; e += T) {
-      float hi, lo;
-      SplitTf32(sm.cr[e], hi, lo);
-      const int i = TileIdx(e >> 3, e & 7);
-      sm.aHi[i] = hi;
-      sm.aLo[i] = lo;
-    }
-    for (int e = tid; e < NM * 8; e += T) {
-      float hi, lo;
-      SplitTf32(sm.xr[e], hi, lo);
-      const int i = TileIdx(e >> 3, e & 7);
-      sm.bHi[i] = hi;
-      sm.bLo[i] = lo;
-    }
-  };
-
-  if (steps > 0) {
-    fetchRaw(0);
-    CpAsyncCommit();
-    CpAsyncWaitAll();
-    __syncthreads();
-    splitOperands();
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    if (steps > 1) fetchRaw(1);
-    FetchOffsets(sm.idN, asmtG, taps, a.CT, a.KgPad, tid, T);
-    CpAsyncCommit();
-  }
-  int hi = hi_lo, s = 0;
-  for (int it = 0; it < steps; it++) {
-    const int kh = hi + a.pad - ho_cur * a.stride;  // warp-uniform
-    const bool active = ho_cur < ho_end && kh >= 0 && kh < a.ksz;
-    CpAsyncWaitAll();
-    __syncthreads();  // (A)
-    if (warp < 4 * nwg) LutMma(sm.aHi, sm.aLo, sm.bHi, sm.bLo, sm.lut, a.PP, NM, warp, lane, nwg);
-    if (a.S > 1 || it == 0) CommitOffsets(sm.idN, sm.idx, taps, a.CT, rowBytes, tid, T);
-    if (it + 1 < steps) {
-      __syncthreads();  // the MMAs of this step have read the operand tiles
-      splitOperands();
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    __syncthreads();  // (B)
-    int hin = hi, sn = s + 1;
-    if (sn == a.S) { sn = 0; hin = hi + 1; }
-    if (it + 1 < steps) {
-      if (it + 2 < steps) fetchRaw(it + 2);
-      if (a.S > 1) FetchOffsets(sm.idN, asmtG + static_cast<size_t>(sn) * taps * a.KgPad, taps, a.CT, a.KgPad, tid, T);
-      CpAsyncCommit();
-    }
-    if (active) {
-      const char* lutq = reinterpret_cast<const char*>(sm.lut) + wo0 * 4;
-      const uint32_t* ip = sm.idx + (kh * a.ksz) * a.CT + cw * CPT;
-      for (int kw = 0; kw < a.ksz; kw++) {
-        const int phase = kw % a.stride, sh = kw / a.stride;
-        GatherTap<CPT, J>(acc, lutq + (phase * PH + sh) * 4, ip);
-        ip += a.CT;
-      }
-    }
-    if (s == a.S - 1 && ho_cur < ho_end && kh == a.ksz - 1) {
-#pragma unroll
-      for (int j = 0; j < J; j++) {
-        const int wo = wo0 + 32 * j;
-        if (wo < a.Wo) {
-          float* out = a.dst + ((static_cast<size_t>(n) * a.Ho + ho_cur) * a.Wo + wo) * a.Cout + g * a.Kg + cbase;
-          StoreChannels<CPT, J>(out, acc, j, a.relu);
-        }
-      }
-      acc.Fill(bias);
-      ho_cur += a.rgroups;
-    }
-    hi = hin; s = sn;
-  }
-  for (int h = max(hi_hi, hi_begin); h < hi_end; h++) {
-    const int kh = h + a.pad - ho_cur * a.stride;
-    if (ho_cur < ho_end && kh == a.ksz - 1) {
-#pragma unroll
-      for (int j = 0; j < J; j++) {
-        const int wo = wo0 + 32 * j;
-        if (wo < a.Wo) {
-          float* out = a.dst + ((static_cast<size_t>(n) * a.Ho + ho_cur) * a.Wo + wo) * a.Cout + g * a.Kg + cbase;
-          StoreChannels<CPT, J>(out, acc, j, a.relu);
-        }
-      }
-      acc.Fill(bias);
-      ho_cur += a.rgroups;
-    }
+    if (ho_cur < ho_end && kh == a.ksz - 1) emitRow();
   }
 }
 
@@ -998,23 +826,16 @@ __global__ void __launch_bounds__(384, 1) conv_direct_kernel(const ConvArgs a) {
 template <int CPT, int J, int MAXT>
 int LaunchBound(const ConvPlan& p, const ConvArgs& a, cudaStream_t st) {
   dim3 grid(a.G * a.nct * a.nstrips, a.N);
-  if (p.kernel == 0) {
-    auto kern = conv_s1_kernel<CPT, J, MAXT>;
-    QCNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-    kern<<<grid, p.threads, p.smem, st>>>(a);
-  } else if (p.kernel == 2) {
-    auto kern = conv_s1_tc_kernel<CPT, J, MAXT>;
-    QCNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-    kern<<<grid, p.threads, p.smem, st>>>(a);
-  } else if (p.kernel == 3) {
-    auto kern = conv_roll_tc_kernel<CPT, J, MAXT>;
-    QCNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-    kern<<<grid, p.threads, p.smem, st>>>(a);
-  } else {
-    auto kern = conv_roll_kernel<CPT, J, MAXT>;
-    QCNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
-    kern<<<grid, p.threads, p.smem, st>>>(a);
+  void (*kern)(ConvArgs);
+  switch (p.kernel) {
+    case kConvS1: kern = conv_s1_kernel<FfmaLut, CPT, J, MAXT>; break;
+    case kConvS1Tc: kern = conv_s1_kernel<WgmmaLut, CPT, J, MAXT>; break;
+    case kConvRoll: kern = conv_roll_kernel<FfmaLut, CPT, J, MAXT>; break;
+    case kConvRollTc: kern = conv_roll_kernel<WgmmaLut, CPT, J, MAXT>; break;
+    default: ::qcnn::SetError("internal: kernel %d is not a LUT + gather kernel", p.kernel); return 1;
   }
+  QCNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+  kern<<<grid, p.threads, p.smem, st>>>(a);
   QCNN_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1053,8 +874,8 @@ int PlanConv(qcnn_layer* L, int N) {
   double dimsSum = 0;  // sum over subspaces of the dims that exist
   for (int s = 0; s < L->S; s++) dimsSum += std::max(0, std::min(Cg - s * L->d, L->d));
   const double ipe = 0.66 * (dimsSum / L->S) + 0.3;  // issue slots per LUT entry
-  // tensor-core LUT stage: 128 codewords (MMA M), every subspace <= 8 dims (one K = 8 tf32 step); env QCNN_NO_TC=1 disables
-  const bool tcOk = L->K == 128 && L->d <= 8 && getenv("QCNN_NO_TC") == nullptr;
+  // tensor-core LUT stage: 128 codewords (MMA M), every subspace <= 8 dims (one K = 8 tf32 step)
+  const bool tcOk = L->K == 128 && L->d <= 8;
   const int cpts[2] = {32, 16};
   for (int ci = 0; ci < 2; ci++) {
     const int CPT = cpts[ci];
@@ -1073,12 +894,10 @@ int PlanConv(qcnn_layer* L, int N) {
             a.R = R;
             a.nstrips = CeilDiv(L->Ho, R);
             a.CT = CT; a.nct = nct; a.cwarps = cwarps;
-            a.ksplit = 1;
             double gatherSlots, builtEntries, phases;
             int warps;
-            size_t smemFloats;
             if (L->stride == 1) {
-              p.kernel = tc ? 2 : 0;
+              p.kernel = tc ? kConvS1Tc : kConvS1;
               a.PW = L->Win + L->pad;
               a.RI = R + L->ksz - 1;
               a.pwarps = CeilDiv(R * a.PW, 32 * J);
@@ -1087,20 +906,17 @@ int PlanConv(qcnn_layer* L, int N) {
               const int need2 = a.pwarps * 32 * J + (L->ksz - 1) * a.PW + (L->ksz - 1) + 1;
               warps = a.pwarps * cwarps;
               if (tc) {
-                const int NM = RoundUp(std::max(need1, need2), 32);  // MMA N = LUT columns per subspace
-                if (NM > 256 || warps < 4) continue;
-                a.RI = NM;          // the tensor-core kernel receives NM in this field
-                a.PP = NM + 4;      // row pitch = 4 (mod 32) words
-                smemFloats = 128 * static_cast<size_t>(a.PP) + static_cast<size_t>(taps) * CT + 2048 + 25 * static_cast<size_t>(NM) + 1024 + 8;
+                a.NM = RoundUp(std::max(need1, need2), 32);  // MMA N = LUT columns per subspace
+                if (a.NM > 256 || warps < 4) continue;
+                a.PP = a.NM + 4;    // row pitch = 4 (mod 32) words
               } else {
                 a.PP = RoundUp(std::max(need1, need2), 4);
-                smemFloats = static_cast<size_t>(L->K) * a.PP + static_cast<size_t>(taps) * CT + 24 * static_cast<size_t>(L->K) + 17 * static_cast<size_t>(a.PP);
               }
               gatherSlots = static_cast<double>(a.pwarps) * J * taps * L->S * CT;   // wavefronts of LUT reads
               builtEntries = static_cast<double>(a.PP) * L->K * L->S;
               phases = L->S;
             } else {
-              p.kernel = tc ? 3 : 1;
+              p.kernel = tc ? kConvRollTc : kConvRoll;
               a.rgroups = CeilDiv(L->ksz, L->stride);
               a.pwarps = CeilDiv(L->Wo, 32 * J);
               const int ph1 = CeilDiv(L->Win + 2 * L->pad, L->stride);
@@ -1111,16 +927,12 @@ int PlanConv(qcnn_layer* L, int N) {
                 // phase length = the real columns only; idle lanes beyond Wo then read into the next phase's columns
                 // (valid shared memory, results discarded), so the row must hold (stride-1)*PH + lanes + shift entries
                 a.PW = ph1;
-                const int NM = RoundUp(std::max(ph1 * L->stride, (L->stride - 1) * ph1 + ph2), 32);
-                if (NM > 256 || warps < 4) continue;
-                a.RI = NM;
-                a.PP = NM + 4;
-                smemFloats = 128 * static_cast<size_t>(a.PP) + static_cast<size_t>(taps) * CT + 2048 + 25 * static_cast<size_t>(NM) + 1024 + 8;
+                a.NM = RoundUp(std::max(ph1 * L->stride, (L->stride - 1) * ph1 + ph2), 32);
+                if (a.NM > 256 || warps < 4) continue;
+                a.PP = a.NM + 4;
               } else {
                 a.PW = std::max(ph1, ph2);           // phase length
                 a.PP = RoundUp(a.PW * L->stride, 4);
-                a.RI = 0;
-                smemFloats = static_cast<size_t>(L->K) * a.PP + static_cast<size_t>(taps) * CT + 24 * static_cast<size_t>(L->K) + 17 * static_cast<size_t>(a.PP);
               }
               gatherSlots = static_cast<double>(a.pwarps) * J * R * taps * L->S * CT;
               builtEntries = static_cast<double>(a.PP) * L->K * L->S * rowsIn;
@@ -1129,8 +941,7 @@ int PlanConv(qcnn_layer* L, int N) {
             p.CPT = CPT; p.J = J;
             p.threads = warps * 32;
             if (p.threads > kMaxThreads || p.threads < 64) continue;
-            // FFMA path: lut + idx + cb2 + xs[2] + posoff + cbN; tensor path: lut + idx + A/B tiles + raw staging
-            p.smem = sizeof(float) * smemFloats + RoundUp(taps * CT, 16);
+            p.smem = tc ? WgmmaLut::MapSmem(L->K, a.PP, a.NM, taps, CT).bytes : FfmaLut::MapSmem(L->K, a.PP, a.NM, taps, CT).bytes;
             if (p.smem > smemMax) continue;
             // model constants (they only order the candidates; on-device timing picks among the cheapest): ~1.3 clk per
             // gather wavefront, FFMA LUT stage ~0.12 clk per entry at d = 8, tensor-core LUT stage = MMA + fragment
@@ -1153,7 +964,7 @@ int PlanConv(qcnn_layer* L, int N) {
     }
   }
   // single subspace of <= 4 existing dims: evaluate <x, codeword> at the point of use (conv_direct_kernel)
-  if (L->S == 1 && std::min(Cg, L->d) <= 4 && L->Wo <= 64 && getenv("QCNN_NO_DIRECT") == nullptr) {
+  if (L->S == 1 && std::min(Cg, L->d) <= 4 && L->Wo <= 64) {
     const int NJ = std::min(Cg, L->d) <= 3 ? 3 : 4;
     const int dcpts[2] = {16, 8};
     for (int ci = 0; ci < 2; ci++) {
@@ -1172,9 +983,9 @@ int PlanConv(qcnn_layer* L, int N) {
             ConvPlan p;
             memset(&p, 0, sizeof(p));
             ConvArgs& a = p.a;
-            p.kernel = 4; p.CPT = CPT; p.J = rowsPer;
+            p.kernel = kConvDirect; p.CPT = CPT; p.J = rowsPer;
             a.R = std::min(R, L->Ho + (L->Ho & 1)); a.nstrips = CeilDiv(L->Ho, a.R);
-            a.CT = CT; a.nct = nct; a.cwarps = cwarps; a.pwarps = 1; a.rgroups = rgroups; a.ksplit = 1;
+            a.CT = CT; a.nct = nct; a.cwarps = cwarps; a.pwarps = 1; a.rgroups = rgroups;
             a.PW = CeilDiv(L->Win + 2 * L->pad, L->stride);       // phase length
             a.PP = RoundUp(a.PW * L->stride, 4);                   // row pitch
             p.threads = 32 * cwarps * rgroups;
@@ -1217,16 +1028,16 @@ int PlanConv(qcnn_layer* L, int N) {
   // Within the LUT + gather family the kernels come in two numerical classes -- fp32 LUT / decode (s1, roll, direct) and
   // 3xTF32 tensor-core LUT stage (s1_tc, roll_tc; ~5e-6 apart) -- and on-device timing must not pick between classes
   // either: the class of the cost model's favourite is kept, timing chooses among its tilings only.
-  if (!cands.empty() && cands[0].second.kernel != 6 && !L->opt_force_kernel && getenv("QCNN_FORCE_KERNEL") == nullptr) {
-    auto cls = [](int k) { return (k == 2 || k == 3) ? 1 : 0; };
-    const int want = cls(cands[0].second.kernel);
+  if (!cands.empty() && cands[0].second.kernel != kPqGemmTc && !L->opt_force_kernel && getenv("QCNN_FORCE_KERNEL") == nullptr) {
+    const bool want = kConvKernelInfo[cands[0].second.kernel].tcLut;
     std::vector<std::pair<double, ConvPlan>> kept;
-    for (const auto& c : cands) if (c.second.kernel != 6 && cls(c.second.kernel) == want) kept.push_back(c);
+    for (const auto& c : cands)
+      if (c.second.kernel != kPqGemmTc && kConvKernelInfo[c.second.kernel].tcLut == want) kept.push_back(c);
     cands.swap(kept);
   }
   if (L->opt_gemm_nt) {   // layer parameter "gemm_nt": only pq_gemm_tc tilings with that many positions per CTA
     std::vector<std::pair<double, ConvPlan>> kept;
-    for (const auto& c : cands) if (c.second.kernel != 6 || c.second.g.NT == L->opt_gemm_nt) kept.push_back(c);
+    for (const auto& c : cands) if (c.second.kernel != kPqGemmTc || c.second.g.NT == L->opt_gemm_nt) kept.push_back(c);
     QCNN_CHECK(!kept.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d has no tiling for this layer at batch %d", L->opt_gemm_nt, N);
     cands.swap(kept);
   }
@@ -1240,10 +1051,10 @@ int PlanConv(qcnn_layer* L, int N) {
   }
   // every kernel family that has a feasible tiling gets at least two seats among the candidates
   for (int pass = 0; pass < 2; pass++) {
-    int perKernel[7] = {0, 0, 0, 0, 0, 0, 0};
+    int perKernel[kConvKernelIds] = {};
     for (size_t i = 0; i < cands.size() && L->cands->size() < kMaxCand; i++) {
       ConvPlan c = cands[i].second;
-      if (pass == 0 && perKernel[c.kernel] >= (c.kernel == 4 ? 8 : (c.kernel == 6 ? 6 : 2))) continue;
+      if (pass == 0 && perKernel[c.kernel] >= (c.kernel == kConvDirect ? 8 : (c.kernel == kPqGemmTc ? 6 : 2))) continue;
       ConvArgs& a = c.a;
       a.Hi = L->Hin; a.Wi = L->Win; a.Cin = L->Cin; a.Ho = L->Ho; a.Wo = L->Wo; a.Cout = L->Cout;
       a.ksz = L->ksz; a.pad = L->pad; a.stride = L->stride; a.G = G; a.Cg = Cg; a.Kg = Kg;
@@ -1253,7 +1064,7 @@ int PlanConv(qcnn_layer* L, int N) {
       bool dup = false;
       for (const ConvPlan& e : *L->cands)
         if (e.kernel == c.kernel && e.CPT == c.CPT && e.J == c.J && e.a.nct == c.a.nct && e.a.nstrips == c.a.nstrips &&
-            e.a.rgroups == c.a.rgroups && e.a.R == c.a.R && (e.kernel != 4 || e.J == c.J)) dup = true;
+            e.a.rgroups == c.a.rgroups && e.a.R == c.a.R && (e.kernel != kConvDirect || e.J == c.J)) dup = true;
       if (dup) continue;
       L->cands->push_back(c);
       perKernel[c.kernel]++;
@@ -1288,15 +1099,15 @@ static int LaunchPlan(qcnn_layer* L, const ConvPlan& p, const float* src, int N,
   ConvArgs a = p.a;
   a.src = src; a.dst = dst; a.ctrd = L->d_ctrd; a.asmt = L->d_asmt; a.bias = L->d_bias;
   a.N = N; a.relu = relu; a.src_nchw = L->src_nchw;
-  if (p.kernel == 6) return LaunchPqGemm(L, p, src, N, dst, relu, st);
-  if (p.kernel == 4) {
+  if (p.kernel == kPqGemmTc) return LaunchPqGemm(L, p, src, N, dst, relu, st);
+  if (p.kernel == kConvDirect) {
     const int nj = std::min(a.Cg, a.d);
     // p.J carries the output rows per thread (2 or 4)
     if (p.CPT == 16) return nj <= 3 ? LaunchDirect<16, 3, 2>(p, a, st) : LaunchDirect<16, 4, 2>(p, a, st);
     if (p.J == 4) return nj <= 3 ? LaunchDirect<8, 3, 4>(p, a, st) : LaunchDirect<8, 4, 4>(p, a, st);
     return nj <= 3 ? LaunchDirect<8, 3, 2>(p, a, st) : LaunchDirect<8, 4, 2>(p, a, st);
   }
-  QCNN_CHECK(!(a.src_nchw && (p.kernel == 0 || p.kernel == 2)), "qcnn_conv_aprx_forward: NCHW source is only supported by the strided kernel");
+  QCNN_CHECK(!(a.src_nchw && (p.kernel == kConvS1 || p.kernel == kConvS1Tc)), "qcnn_conv_aprx_forward: NCHW source is only supported by the strided kernel");
   int rc = 1;
 #define QCNN_DISPATCH(C, JJ) if (p.CPT == C && p.J == JJ) rc = LaunchOne<C, JJ>(p, a, st); else
   QCNN_DISPATCH(32, 1) QCNN_DISPATCH(32, 2) QCNN_DISPATCH(16, 1) QCNN_DISPATCH(16, 2) QCNN_DISPATCH(16, 3)
@@ -1340,7 +1151,7 @@ int LaunchConv(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
       static const bool tuneLog = getenv("QCNN_AUTOTUNE_LOG") != nullptr;
       if (tuneLog)
         fprintf(stderr, "[qcnn autotune] N=%d Cout=%d k=%d cand %zu: kernel=%d NT/CPT=%d GT/J=%d bf=%d nsplit=%d smem=%zu -> %.4f ms\n",
-                N, L->Cout, L->ksz, i, c.kernel, c.CPT, c.kernel == 6 ? c.g.GT : c.J, c.g.bf, c.g.nsplit, c.smem, ms);
+                N, L->Cout, L->ksz, i, c.kernel, c.CPT, c.kernel == kPqGemmTc ? c.g.GT : c.J, c.g.bf, c.g.nsplit, c.smem, ms);
       if (ms < bestMs) { bestMs = ms; bestI = i; }
     }
     cudaEventDestroy(e0);
@@ -1359,7 +1170,7 @@ int LaunchConv(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
 int DescribeConv(qcnn_layer* L, int N, char* buf, size_t cap) {
   if (int prc = PlanConv(L, N)) return prc;
   const ConvPlan& p = L->plan;
-  if (p.kernel == 6) {
+  if (p.kernel == kPqGemmTc) {
     int ksteps = 0;
     for (int c = 0; c < p.g.nChunks; c++) ksteps += p.g.chunkCount[p.g.mode == 1 ? c : 0];
     snprintf(buf, cap, "pq_gemm_tc(wgmma, weights decoded into registers%s) mode=%d NT=%d GT=%d smem=%zuB grid=%d NPOS=%d "
@@ -1369,7 +1180,7 @@ int DescribeConv(qcnn_layer* L, int N, char* buf, size_t cap) {
     return 0;
   }
   snprintf(buf, cap, "%s CPT=%d J=%d threads=%d smem=%zuB grid=(%d,%d) R=%d strips=%d CT=%d nct=%d PP=%d pwarps=%d "
-           "cwarps=%d rgroups=%d", p.kernel == 0 ? "conv_s1" : (p.kernel == 2 ? "conv_s1_tc(wgmma LUT)" : (p.kernel == 3 ? "conv_roll_tc(wgmma LUT)" : (p.kernel == 4 ? "conv_direct" : "conv_roll"))), p.CPT, p.J, p.threads, p.smem,
+           "cwarps=%d rgroups=%d", kConvKernelInfo[p.kernel].name, p.CPT, p.J, p.threads, p.smem,
            p.a.G * p.a.nct * p.a.nstrips, N, p.a.R, p.a.nstrips, p.a.CT, p.a.nct, p.a.PP, p.a.pwarps, p.a.cwarps,
            p.a.rgroups);
   return 0;

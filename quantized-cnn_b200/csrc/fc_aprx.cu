@@ -18,6 +18,7 @@
 //     order by fc_reduce_kernel (deterministic; no atomics).  With nsplit == 1 the accumulation order is
 //     exactly the reference's (bias, then s ascending) and the result is bit-identical to the CPU path.
 #include "qcnn_internal.h"
+#include "async_copy.h"
 
 #include <algorithm>
 #include <cstdlib>
@@ -25,6 +26,11 @@
 #include <cstdio>
 
 namespace {
+
+using qcnn::CpAsync16;
+using qcnn::CpAsync4;
+using qcnn::CpAsyncCommit;
+using qcnn::CpAsyncWaitAll;
 
 constexpr int kFcThreads = 256;
 
@@ -57,19 +63,6 @@ __device__ __forceinline__ uint32_t Word(const uint2& v, int i) { return i == 0 
 __device__ __forceinline__ uint32_t Word(const uint4& v, int i) {
   return i == 0 ? v.x : (i == 1 ? v.y : (i == 2 ? v.z : v.w));
 }
-
-__device__ __forceinline__ void CpAsync4(void* smemDst, const void* gsrc, bool valid) {
-  const uint32_t d = static_cast<uint32_t>(__cvta_generic_to_shared(smemDst));
-  const int sz = valid ? 4 : 0;  // src-size 0: nothing is read, destination zero-filled
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(d), "l"(gsrc), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void CpAsync16(void* smemDst, const void* gsrc, bool valid) {
-  const uint32_t d = static_cast<uint32_t>(__cvta_generic_to_shared(smemDst));
-  const int sz = valid ? 16 : 0;
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(gsrc), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void CpAsyncCommit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void CpAsyncWaitAll() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
 constexpr int kRowBlock = 8;  // assignment rows held in registers per block of the rolling prefetch window
 

@@ -23,6 +23,7 @@
 // Accumulation order: per CTA s ascending, then CTAs in a fixed tree -- a re-association of the reference's
 // bias + s-ascending sum (fp32 adds only; tolerance in tests/test_gpu_layers.py).  fc_nsplit = 1 keeps the bit-exact kernel.
 #include "qcnn_internal.h"
+#include "async_copy.h"
 
 #include <algorithm>
 #include <cmath>
@@ -31,6 +32,13 @@
 #include <cstring>
 
 namespace {
+
+using qcnn::BulkLoad;
+using qcnn::MbarArrive;
+using qcnn::MbarExpectTx;
+using qcnn::MbarInit;
+using qcnn::MbarWait;   // the chain's waits trap after 2^26 polls
+using qcnn::SmemU32;
 
 constexpr int kConsumers = 512;
 constexpr int kConsumerWarps = kConsumers / 32;
@@ -75,29 +83,6 @@ struct ChainArgs {
 
 static_assert(8 * (2 * kMaxStage + kMaxChain) <= kBarBytes, "shared-memory header layout");
 
-__device__ __forceinline__ uint32_t SmemU32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void MbarInit(uint64_t* b, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(SmemU32(b)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void MbarArrive(uint64_t* b) {
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(SmemU32(b)) : "memory");
-}
-__device__ __forceinline__ void MbarExpectTx(uint64_t* b, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(SmemU32(b)), "r"(bytes) : "memory");
-}
-// bounded spin: a protocol error traps (launch failure) instead of hanging the GPU
-__device__ __forceinline__ void MbarWait(uint64_t* b, uint32_t parity) {
-  uint32_t ok = 0;
-  for (uint32_t spins = 0; !ok; spins++) {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(SmemU32(b)), "r"(parity) : "memory");
-    if (spins > (1u << 26)) __trap();
-  }
-}
-__device__ __forceinline__ void BulkLoad(void* smemDst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(SmemU32(smemDst)), "l"(gsrc), "r"(bytes), "r"(SmemU32(bar)) : "memory");
-}
 __device__ __forceinline__ void ConsumerSync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory"); }
 __device__ __forceinline__ unsigned long long GlobalTimer() {
   unsigned long long t;
@@ -251,7 +236,7 @@ __device__ __forceinline__ void GatherAndPublish(const ChainLayer& L, int rows, 
   int stage = *stagep;
   uint32_t round = *roundp;
   for (int r = 0; r < rows; r += L.rpc) {
-    MbarWait(fullB + stage, round & 1u);
+    MbarWait<26>(fullB + stage, round & 1u);
     if (dbg && tid == 0 && r == 0) dbg[0] = clock64();
     if (active) {
       const uint8_t* chunk = ring + static_cast<size_t>(stage) * kChunkBytes + cgIdx * CPT;
@@ -348,7 +333,7 @@ __global__ void __launch_bounds__(kThreads, 1) fc_chain_kernel(const __grid_cons
         int r0, r1;
         RowRange(L, cta, &r0, &r1);
         for (int r = r0; r < r1; r += L.rpc, issued++) {
-          if (round > 0) MbarWait(emptyB + stage, (round - 1) & 1u);
+          if (round > 0) MbarWait<26>(emptyB + stage, (round - 1) & 1u);
           const uint32_t bytes = static_cast<uint32_t>(min(L.rpc, r1 - r)) * L.DoutPad;
           MbarExpectTx(fullB + stage, bytes);
           BulkLoad(ring + static_cast<size_t>(stage) * kChunkBytes, L.asmt + static_cast<size_t>(r) * L.DoutPad, bytes, fullB + stage);
@@ -373,7 +358,7 @@ __global__ void __launch_bounds__(kThreads, 1) fc_chain_kernel(const __grid_cons
       if (a.dbg) {   // measurement only: when the first 8 chunks landed ([24 + i]); only while the ring is not recycled
         a.dbg[32 * cta + 23] = clock64();   // all copies issued
         for (int i = 0; i < (issued <= a.nStage ? min(issued, 8) : 0); i++) {
-          MbarWait(fullB + i, 0);
+          MbarWait<26>(fullB + i, 0);
           a.dbg[32 * cta + 24 + i] = clock64();
         }
       }
@@ -427,7 +412,7 @@ __global__ void __launch_bounds__(kThreads, 1) fc_chain_kernel(const __grid_cons
     if (a.dbg && tid == 0) a.dbg[32 * cta + 4 + 5 * l] = clock64();
     // (2) LUT rows of the CTA's subspaces (reference GetInPdMat: ascending j, separate multiply and add)
     if (rows > 0) {
-      MbarWait(ctrdB + l, 0);
+      MbarWait<26>(ctrdB + l, 0);
       const float* cs = ctrdS + L.ctrdOff;
       const int d = L.d, kmask = L.K - 1, lutRowF = L.lutPitch >> 2;
       for (int e = tid; e < rows * L.K; e += kConsumers) {

@@ -47,7 +47,16 @@
 
 namespace {
 
+using qcnn::BulkLoad;
+using qcnn::CpAsync16;
+using qcnn::CpAsyncCommit;
+using qcnn::CpAsyncWaitAll;
+using qcnn::MbarArrive;
+using qcnn::MbarExpectTx;
+using qcnn::MbarInit;
+using qcnn::MbarWait;
 using qcnn::SmemU32;
+using qcnn::SplitTf32x4;
 using qcnn::Wgmma;
 
 constexpr int kThreads = 384;
@@ -56,38 +65,6 @@ constexpr int kStagers = 128;    // warps 8-11
 constexpr int kMaxGT = 4;        // k-steps per stage (decoded A fragments of a stage live in registers)
 constexpr int kRegPos = 12;      // float4 a stager thread holds in registers (convolution modes: planeF4 <= 12 * 128)
 constexpr int kCbBufs = 4;       // codebook / index buffers: the decoders run ahead of the position planes
-
-__device__ __forceinline__ void CpAsync16(void* smemDst, const void* gsrc, bool valid) {
-  const int sz = valid ? 16 : 0;  // src-size 0: nothing is read, the 16 destination bytes are zero-filled
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(SmemU32(smemDst)), "l"(gsrc), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void CpAsyncCommit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void CpAsyncWaitAll() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
-
-__device__ __forceinline__ void MbarInit(uint64_t* mbar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(SmemU32(mbar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void MbarArrive(uint64_t* mbar) {
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(SmemU32(mbar)) : "memory");
-}
-// bounded spin: a protocol error traps (launch failure) instead of hanging the GPU
-__device__ __forceinline__ void MbarWait(uint64_t* mbar, uint32_t parity) {
-  uint32_t done = 0;
-  for (uint32_t spins = 0; !done; spins++) {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(done) : "r"(SmemU32(mbar)), "r"(parity) : "memory");
-    if (spins > (1u << 24)) __trap();
-  }
-}
-// 3xTF32 operand split: hi = v truncated to tf32 (what the tensor core reads), lo = exact remainder (the tensor core
-// truncates it to tf32 in turn).  The error of this path grows with the tensor core's fp32 ACCUMULATION over the
-// n = 3 * k-steps chained MMAs (~n * 2^-24), not with the operand representation (tools/accuracy.py measures it).
-__device__ __forceinline__ void SplitTf32x4(const float4 v, float4& hi, float4& lo) {
-  hi.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); lo.x = v.x - hi.x;
-  hi.y = __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u); lo.y = v.y - hi.y;
-  hi.z = __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); lo.z = v.z - hi.z;
-  hi.w = __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u); lo.w = v.w - hi.w;
-}
 
 // ---- bf16x2 operands: v = v1 + v2 with v1 = bf16(v), v2 = bf16(v - v1) (|v - v1 - v2| <= 2^-18 |v|).  One k-step of
 // eight values is TWO kind::f16 MMAs of K = 16: [w1 | w1] . [x1 | x2] + [w2 | w2] . [x1 | x2] = (w1 + w2)(x1 + x2) --
@@ -287,18 +264,15 @@ __global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_kernel(const GemmArgs 
           // a half beyond the group's channels stages valid data (its positions are staged as zeros)
           if (st == 0) {
             const uint32_t cbBytes = static_cast<uint32_t>(K) * 16u, idBytes = static_cast<uint32_t>(CTv * a.tapsPad);
-            const uint32_t bar = SmemU32(fullC + cbuf);
+            uint64_t* bar = fullC + cbuf;
             uint8_t* idst = ids + cbuf * a.idRows * 128;
             const uint8_t* tA = a.asmtT + (static_cast<size_t>(g * a.S + sA) * a.KgPad + ch0) * a.tapsPad;
             const uint8_t* tB = a.asmtT + (static_cast<size_t>(g * a.S + sB) * a.KgPad + ch0) * a.tapsPad;
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(2u * cbBytes + 2u * idBytes) : "memory");
-#define QCNN_BULK(dst, src, bytes) asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" \
-                                                ::"r"(SmemU32(dst)), "l"(src), "r"(bytes), "r"(bar) : "memory")
-            QCNN_BULK(cdst, piece(sA, jA, 0), cbBytes);
-            QCNN_BULK(cdst + K, piece(sB, jB, 0), cbBytes);
-            QCNN_BULK(idst, tA, idBytes);
-            QCNN_BULK(idst + 128 * a.tapsPad, tB, idBytes);
-#undef QCNN_BULK
+            MbarExpectTx(bar, 2u * cbBytes + 2u * idBytes);
+            BulkLoad(cdst, piece(sA, jA, 0), cbBytes, bar);
+            BulkLoad(cdst + K, piece(sB, jB, 0), cbBytes, bar);
+            BulkLoad(idst, tA, idBytes, bar);
+            BulkLoad(idst + 128 * a.tapsPad, tB, idBytes, bar);
           }
           return;
         }
@@ -340,13 +314,11 @@ __global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_kernel(const GemmArgs 
         if (a.bulkC) {
           if (st == 0) {
             const uint32_t cbBytes = static_cast<uint32_t>(K) * 16u, idBytes = static_cast<uint32_t>(CTv * a.tapsPad);
-            const uint32_t bar = SmemU32(fullC + cbuf);
+            uint64_t* bar = fullC + cbuf;
             const uint8_t* tA = a.asmtT + (static_cast<size_t>(g * a.stride + ph) * a.KgPad + ch0) * a.tapsPad;
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(cbBytes + idBytes) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(SmemU32(cdst)), "l"(piece(0, 0, 0)), "r"(cbBytes), "r"(bar) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(SmemU32(ids + cbuf * a.idRows * 128)), "l"(tA), "r"(idBytes), "r"(bar) : "memory");
+            MbarExpectTx(bar, cbBytes + idBytes);
+            BulkLoad(cdst, piece(0, 0, 0), cbBytes, bar);
+            BulkLoad(ids + cbuf * a.idRows * 128, tA, idBytes, bar);
           }
           return;
         }
@@ -468,7 +440,7 @@ __global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_kernel(const GemmArgs 
         // (each stager arrives after its own copies have landed; the barrier completes when all of them have)
         MbarArrive(fullC + kc % kCbBufs);                  // the consumers may start on chunk kc
       }
-      if (kc >= a.nPB) MbarWait(emptyB + buf, ((kc / a.nPB) - 1) & 1);   // planes last read by the MMAs of chunk kc-nPB
+      if (kc >= a.nPB) MbarWait<24>(emptyB + buf, ((kc / a.nPB) - 1) & 1);   // planes last read by the MMAs of chunk kc-nPB
       float4* pHi = planes + (buf * 2 + 0) * a.planeRows;
       float4* pLo = planes + (buf * 2 + 1) * a.planeRows;
       if (a.mode == 2) {
@@ -477,9 +449,8 @@ __global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_kernel(const GemmArgs 
         if (st == 0) {
           const uint32_t bytes = static_cast<uint32_t>(a.planeRows) * 32u;
           const float* gsrc = a.xprep + (static_cast<size_t>(tile) * a.nChunksAll + (k0 / a.chunkCount[0] + kc)) * a.planeRows * 8;
-          asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(SmemU32(fullB + buf)), "r"(bytes) : "memory");
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                       ::"r"(SmemU32(pHi)), "l"(gsrc), "r"(bytes), "r"(SmemU32(fullB + buf)) : "memory");
+          MbarExpectTx(fullB + buf, bytes);
+          BulkLoad(pHi, gsrc, bytes, fullB + buf);
         } else {
           MbarArrive(fullB + buf);
         }
@@ -508,7 +479,7 @@ __global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_kernel(const GemmArgs 
       }
       if (kc + 2 < nChunks) {
         const int nb = (kc + 2) % kCbBufs;
-        if (kc + 2 >= kCbBufs) MbarWait(emptyC + nb, (((kc + 2) / kCbBufs) - 1) & 1);
+        if (kc + 2 >= kCbBufs) MbarWait<24>(emptyC + nb, (((kc + 2) / kCbBufs) - 1) & 1);
         fetchChunk(kc + 2);
       }
     }
@@ -535,7 +506,7 @@ __global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_kernel(const GemmArgs 
 
   for (int kc = 0; kc < nChunks; kc++) {
     const int cbuf = kc % kCbBufs, buf = kc % a.nPB;
-    MbarWait(fullC + cbuf, (kc / kCbBufs) & 1);
+    MbarWait<24>(fullC + cbuf, (kc / kCbBufs) & 1);
     const uint8_t* idb = ids + cbuf * a.idRows * 128;
     const float4* cb = cbs + cbuf * a.cbSlots * a.cbF4;
     const float* cbf = reinterpret_cast<const float*>(cb);
@@ -586,7 +557,7 @@ __global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_kernel(const GemmArgs 
       const int row = (half ? ks.idx1 : ks.idx0) + j, slot = (half ? ks.cb1 : ks.cb0) + j;
       return cbf[slot * K + (idb[row * 128 + (c ? cc1 : cc0)] >> a.kshift)];
     };
-    MbarWait(fullB + buf, (kc / a.nPB) & 1);
+    MbarWait<24>(fullB + buf, (kc / a.nPB) & 1);
     const uint64_t dHi = descFixed | (((planes0 + static_cast<uint32_t>((buf * 2 + 0) * a.planeRows) * 16u) >> 4) & 0x3FFFu);
     const uint64_t dLo = descFixed | (((planes0 + static_cast<uint32_t>((buf * 2 + 1) * a.planeRows) * 16u) >> 4) & 0x3FFFu);
     for (int s0 = 0; s0 < ne; s0 += GT) {
@@ -710,7 +681,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
         const int GT = gts1[gi];
         ConvPlan p;
         memset(&p, 0, sizeof(p));
-        p.kernel = 6; p.CPT = NT; p.J = GT; p.threads = kThreads;
+        p.kernel = kPqGemmTc; p.CPT = NT; p.J = GT; p.threads = kThreads;
         GemmArgs& ga = p.g;
         ga.mode = 1;
         ga.PW = PWp; ga.IB = IB; ga.NT = NT; ga.GT = GT;
@@ -788,7 +759,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
       const int GT = gts[gi];
       ConvPlan p;
       memset(&p, 0, sizeof(p));
-      p.kernel = 6; p.CPT = NT; p.J = GT; p.threads = kThreads;
+      p.kernel = kPqGemmTc; p.CPT = NT; p.J = GT; p.threads = kThreads;
       GemmArgs& ga = p.g;
       ga.mode = 0;
       ga.PW = PW; ga.IB = IB; ga.NT = NT; ga.GT = GT;

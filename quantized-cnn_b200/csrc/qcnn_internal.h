@@ -95,9 +95,9 @@ struct ConvArgs {
   int PW;               // s1: row pitch of the flat padded grid; roll: phase length PH
   int RI;               // s1: input rows held per strip
   int PP;               // LUT pitch in floats (positions per codeword row), multiple of 4
+  int NM;               // wgmma LUT stage: LUT columns produced per step (MMA N, multiple of 32, <= 256)
   int CT, nct;          // output channels per CTA (per group) / channel tiles per group
   int pwarps, cwarps, rgroups;
-  int ksplit;           // LUT build: K is split over ksplit thread groups
   int relu;
 };
 
@@ -149,8 +149,19 @@ struct GemmArgs {
   KStep tab[kMaxKSteps];
 };
 
+// ConvPlan::kernel.  The values are the "force_kernel" / QCNN_FORCE_KERNEL numbers of include/qcnn.h (5 is retired).
+enum ConvKernel {
+  kConvS1 = 0,        // LUT + gather, stride 1, FFMA LUT stage
+  kConvRoll = 1,      // LUT + gather, rolling rows (any stride), FFMA LUT stage
+  kConvS1Tc = 2,      // as kConvS1 with the 3xTF32 wgmma LUT stage
+  kConvRollTc = 3,    // as kConvRoll with the 3xTF32 wgmma LUT stage
+  kConvDirect = 4,    // single narrow subspace, codewords evaluated at the point of use
+  kPqGemmTc = 6,      // decode-at-use GEMMs on wgmma (pq_gemm_tc.cu)
+  kConvKernelIds = 7
+};
+
 struct ConvPlan {
-  int kernel;           // 0 s1, 1 roll, 2 s1_tc, 3 roll_tc, 4 direct, 6 pq_gemm_tc (decode-at-use GEMMs on wgmma); 5 retired
+  int kernel;           // ConvKernel
   int CPT, J;
   int threads;
   size_t smem;

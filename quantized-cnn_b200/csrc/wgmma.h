@@ -8,9 +8,10 @@
 
 #include <stdint.h>
 
+#include "async_copy.h"
+
 namespace qcnn {
 
-__device__ __forceinline__ uint32_t SmemU32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 // descriptor of a K-major, unswizzled operand: address, LBO and SBO in units of 16 bytes
 __device__ __forceinline__ uint64_t WgmmaDesc(uint32_t smemAddr, uint32_t lboBytes, uint32_t sboBytes) {
   return static_cast<uint64_t>((smemAddr >> 4) & 0x3FFFu) | (static_cast<uint64_t>((lboBytes >> 4) & 0x3FFFu) << 16) |
@@ -20,6 +21,20 @@ __device__ __forceinline__ uint64_t WgmmaDesc(uint32_t smemAddr, uint32_t lboByt
 __device__ __forceinline__ void WgmmaFence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void WgmmaCommit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void WgmmaWaitAll() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// 3xTF32 operand split: hi = v truncated to tf32 (what the tensor core reads), lo = exact remainder (the tensor core
+// truncates it to tf32 in turn).  The error of this path grows with the tensor core's fp32 ACCUMULATION over the
+// n = 3 * k-steps chained MMAs (~n * 2^-24), not with the operand representation (tools/accuracy.py measures it).
+__device__ __forceinline__ void SplitTf32(float v, float& hi, float& lo) {
+  hi = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
+  lo = v - hi;
+}
+__device__ __forceinline__ void SplitTf32x4(const float4 v, float4& hi, float4& lo) {
+  SplitTf32(v.x, hi.x, lo.x);
+  SplitTf32(v.y, hi.y, lo.y);
+  SplitTf32(v.z, hi.z, lo.z);
+  SplitTf32(v.w, hi.w, lo.w);
+}
 
 template <int N> struct Wgmma;
 

@@ -226,6 +226,40 @@ def test_conv_parity(case, po, qcnn, ctx):
     layer.close()
 
 
+# Each LUT + gather family pinned on CONV_CASES shapes (with the cost model alone some families never run): (case index,
+# force_kernel id); every family twice, both rolling-row families on an NCHW source too.
+CONV_FAMILY_NAMES = {0: "conv_s1 ", 1: "conv_roll ", 2: "conv_s1_tc(", 3: "conv_roll_tc(", 4: "conv_direct "}
+CONV_FAMILY_PAIRS = [(0, 0), (8, 0), (9, 1), (10, 1), (1, 2), (3, 2), (4, 3), (9, 3), (4, 4), (11, 4)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("idx,family", CONV_FAMILY_PAIRS)
+def test_conv_family_pinned(idx, family, po, qcnn, ctx):
+    import torch
+    case = CONV_CASES[idx]
+    N, Hi, Wi, Cin, Cout, k, pad, stride, G, S, K, d = case
+    rng = np.random.RandomState(hash(case) % (2 ** 31))
+    ctrd = (rng.randn(S, K, d) * 0.05).astype(np.float32)
+    asmt = rng.randint(0, K, size=(Cout, k, k, S)).astype(np.uint8)
+    bias = (rng.randn(Cout) * 0.1).astype(np.float32)
+    x = rand_act(rng, (N, Hi, Wi, Cin))
+    ref = po.conv_aprx(x, po.conv(pad, k, Cout, G, stride), ctrd, asmt, bias)
+    layer = qcnn.ConvLayer(ctx, Cin, Hi, Wi, Cout, k, pad, stride, G, ctrd, asmt, bias)
+    layer.set_param("tensor_core", 0)
+    layer.set_param("force_kernel", family)
+    assert layer.describe(N).startswith(CONV_FAMILY_NAMES[family]), layer.describe(N)
+    xd = torch.from_numpy(x).cuda()
+    y = layer.forward(xd).cpu().numpy()
+    assert close(y, ref) <= RTOL, close(y, ref)
+    yr = layer.forward(xd, relu=True).cpu().numpy()
+    assert close(yr, np.maximum(ref, 0)) <= RTOL
+    if family in (1, 3):
+        layer.set_src_nchw(True)
+        yn = layer.forward(torch.from_numpy(po.nhwc_to_nchw(x)).cuda()).cpu().numpy()
+        assert np.array_equal(yn, y)
+    layer.close()
+
+
 @pytest.mark.gpu
 def test_supporting_layers(po, qcnn, ctx):
     import torch
