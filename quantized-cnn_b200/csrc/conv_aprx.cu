@@ -1008,9 +1008,9 @@ int PlanConv(qcnn_layer* L, int N) {
     }
   }
   // decode-at-use GEMMs on the tensor cores (pq_gemm_tc.cu).  The kernel FAMILY is a setting, not a timing result:
-  // with tensor_core = 1 (default) an eligible layer always runs pq_gemm_tc (3xTF32; tolerance in DESIGN.md 2), with
-  // tensor_core = 0 always the LUT + gather kernels; on-device timing only chooses among tilings of that family, so the
-  // numerical path of a (layer, batch size) is the same in every process.
+  // with tensor_core = 2 (default, bf16x2 operands) or 1 (3xTF32 operands) an eligible layer always runs pq_gemm_tc
+  // (tolerances in DESIGN.md 2), with tensor_core = 0 always the LUT + gather kernels; on-device timing only chooses
+  // among tilings of that family, so the numerical path of a (layer, batch size) is the same in every process.
   if (!L->opt_no_tc) {
     std::vector<std::pair<double, ConvPlan>> tc;
     PlanPqGemm(L, N, &tc);
@@ -1035,10 +1035,17 @@ int PlanConv(qcnn_layer* L, int N) {
       if (c.second.kernel != kPqGemmTc && kConvKernelInfo[c.second.kernel].tcLut == want) kept.push_back(c);
     cands.swap(kept);
   }
-  if (L->opt_gemm_nt) {   // layer parameter "gemm_nt": only pq_gemm_tc tilings with that many positions per CTA
+  // layer parameters "gemm_nt" / "gemm_gt" / "gemm_nsplit": only pq_gemm_tc tilings with that many positions per CTA,
+  // k-steps per stage and K-split factor (0 = any)
+  if (L->opt_gemm_nt || L->opt_gemm_gt || L->opt_gemm_nsplit) {
     std::vector<std::pair<double, ConvPlan>> kept;
-    for (const auto& c : cands) if (c.second.kernel != kPqGemmTc || c.second.g.NT == L->opt_gemm_nt) kept.push_back(c);
-    QCNN_CHECK(!kept.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d has no tiling for this layer at batch %d", L->opt_gemm_nt, N);
+    for (const auto& c : cands)
+      if (c.second.kernel != kPqGemmTc || ((!L->opt_gemm_nt || c.second.g.NT == L->opt_gemm_nt) &&
+                                           (!L->opt_gemm_gt || c.second.g.GT == L->opt_gemm_gt) &&
+                                           (!L->opt_gemm_nsplit || c.second.g.nsplit == L->opt_gemm_nsplit)))
+        kept.push_back(c);
+    QCNN_CHECK(!kept.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d gemm_gt=%d gemm_nsplit=%d has no tiling for this layer at "
+               "batch %d", L->opt_gemm_nt, L->opt_gemm_gt, L->opt_gemm_nsplit, N);
     cands.swap(kept);
   }
   const char* force = getenv("QCNN_FORCE_KERNEL");

@@ -66,7 +66,7 @@ constexpr int kMaxGT = 4;        // k-steps per stage (decoded A fragments of a 
 constexpr int kRegPos = 12;      // float4 a stager thread holds in registers (convolution modes: planeF4 <= 12 * 128)
 constexpr int kCbBufs = 4;       // codebook / index buffers: the decoders run ahead of the position planes
 
-// ---- bf16x2 operands: v = v1 + v2 with v1 = bf16(v), v2 = bf16(v - v1) (|v - v1 - v2| <= 2^-18 |v|).  One k-step of
+// ---- bf16x2 operands: v = v1 + v2 with v1 = bf16(v), v2 = bf16(v - v1) (|v - v1 - v2| <= 2^-17 |v|).  One k-step of
 // eight values is TWO kind::f16 MMAs of K = 16: [w1 | w1] . [x1 | x2] + [w2 | w2] . [x1 | x2] = (w1 + w2)(x1 + x2) --
 // all four cross terms, at the fp16/bf16 rate (twice tf32's), against three K = 8 tf32 MMAs for 3xTF32.
 __device__ __forceinline__ uint32_t PackBf16x2(float lo, float hi) {   // low 16 bits = bf16(lo), high 16 bits = bf16(hi)
@@ -180,7 +180,9 @@ __global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_kernel(const GemmArgs 
   const int kcBase = a.mode == 2 ? 0 : split * a.kPerSplit;
   const int nChunks = a.mode == 2 ? (kTotal + a.chunkCount[0] - 1) / a.chunkCount[0]
                                   : (a.nsplit > 1 ? min(a.kPerSplit, a.nChunks - kcBase) : a.nChunks);
-  if (a.mode == 2 && a.nsplit > 1) dstBase = a.partial + (static_cast<size_t>(split) * a.N + Q0) * a.dstRow + ch0;
+  // mode 2: rows = images, so the tile starts at row Q0 of the output (or of this split's partial sums)
+  if (a.mode == 2)
+    dstBase = (a.nsplit > 1 ? a.partial + static_cast<size_t>(split) * a.N * a.dstRow : a.dst) + static_cast<size_t>(Q0) * a.dstRow + ch0;
   if (a.mode != 2 && a.nsplit > 1)
     dstBase = a.partial + (static_cast<size_t>(split) * a.N + i0) * a.dstImg + g * a.Kg + ch0;
 
@@ -712,7 +714,10 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
               // partner in the next phase column, same shift (bf16x2: the partner must be the odd column of the same pair)
               const bool paired = kw + 1 < L->ksz && (kw % st) + 1 < st && !(ga.bf && ((kw % st) & 1));
               ks.bStart = (kw % st) * ga.NPOS + (kh / st) * PWp + kw / st;
-              ks.lbo = paired ? ga.NPOS : 1;
+              // an unpaired tap's second half (zero codebook slot) aliases its first half (LBO = 0): a shift would read
+              // the next position -- for a tile's last position, or a tap at the end of an image, another image's
+              // pixel -- and 0 * NaN / Inf would carry that image's non-finite values into this one's output
+              ks.lbo = paired ? ga.NPOS : 0;
               if (ga.bf) {   // row = (pair of phase columns, position); K-core-matrix 1 = the x2 plane
                 ks.bStart = ((kw % st) >> 1) * ga.NPOS + (kh / st) * PWp + kw / st;
                 ks.lbo = ga.planeRows;

@@ -277,19 +277,25 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
   else if (!strcmp(name, "fc_tn")) L->opt_fc_tn = value;
   else if (!strcmp(name, "tensor_core")) {
     // 0: LUT + gather kernels only (fp32 adds in the reference's association; the strict-parity path);
-    // 1 (default): large batches may use the decode-at-use tensor-core GEMMs (3xTF32, wider tolerance: DESIGN.md)
+    // 2 (default): eligible layers run the decode-at-use tensor-core GEMMs with bf16x2 operands (two MMAs per k-step at
+    // the bf16 rate); 1: the same GEMMs with 3xTF32 operands (both with a wider tolerance: DESIGN.md)
     L->opt_no_tc = value ? 0 : 1;
-    L->opt_tc_bf = value == 2 ? 1 : 0;   // 2: bf16x2 operands (two MMAs per k-step at the bf16 rate) instead of 3xTF32
+    L->opt_tc_bf = value == 2 ? 1 : 0;
     L->plan_N = 0; L->tuned = 0;
     if (L->tunedPlans) L->tunedPlans->clear();
   }
-  else if (!strcmp(name, "force_kernel") || !strcmp(name, "autotune") || !strcmp(name, "gemm_nt")) {
+  else if (!strcmp(name, "force_kernel") || !strcmp(name, "autotune") || !strcmp(name, "gemm_nt") ||
+           !strcmp(name, "gemm_gt") || !strcmp(name, "gemm_nsplit")) {
     // conv only.  force_kernel: -1 none, else 0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc;
     // autotune: 0 keeps the cost model's first tiling instead of timing the candidates on the device;
-    // gemm_nt: positions per CTA of the pq_gemm_tc tilings (0 = any; 128 = one accumulator, 64 = two)
+    // gemm_nt: positions per CTA of the pq_gemm_tc tilings (0 = any; 128 = one accumulator, 64 = two);
+    // gemm_gt: k-steps per stage of those tilings (0 = any; 4 or 3); gemm_nsplit: their K-split factor (0 = any; 1 = no
+    // split, > 1 = partial sums reduced by a second kernel).  A pin that no tiling of the layer matches fails the forward.
     QCNN_CHECK(L->kind == QCNN_KIND_CONV, "qcnn_layer_set_param: '%s' applies to conv layers", name);
     if (name[0] == 'f') L->opt_force_kernel = value < 0 ? 0 : value + 1;
-    else if (name[0] == 'g') L->opt_gemm_nt = value < 0 ? 0 : value;
+    else if (!strcmp(name, "gemm_nt")) L->opt_gemm_nt = value < 0 ? 0 : value;
+    else if (!strcmp(name, "gemm_gt")) L->opt_gemm_gt = value < 0 ? 0 : value;
+    else if (!strcmp(name, "gemm_nsplit")) L->opt_gemm_nsplit = value < 0 ? 0 : value;
     else L->opt_no_autotune = value ? 0 : 1;
     L->plan_N = 0; L->tuned = 0;
     if (L->tunedPlans) L->tunedPlans->clear();

@@ -211,6 +211,8 @@ struct qcnn_layer {
   int opt_force_kernel;  // conv: 1 + kernel id the plan is restricted to (0 = none); tests pin the kernel they check
   int opt_no_autotune;   // conv: 1 = keep the cost model's first tiling (no on-device timing)
   int opt_gemm_nt;       // conv: restrict pq_gemm_tc tilings to this many positions per CTA (0 = any)
+  int opt_gemm_gt;       // conv: ... to this many k-steps per stage (0 = any)
+  int opt_gemm_nsplit;   // conv: ... to this K-split factor (0 = any)
 };
 
 namespace qcnn {
