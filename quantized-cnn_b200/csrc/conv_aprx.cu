@@ -863,9 +863,8 @@ constexpr size_t kMaxCand = 18;
 // The two stages do not overlap inside a CTA (one CTA per SM), so the costs add.
 int PlanConv(qcnn_layer* L, int N) {
   if (L->plan_N == N) return 0;
-  if (L->tunedPlans)  // a batch size seen (and timed) before: reuse its plan
-    for (const std::pair<int, ConvPlan>& e : *L->tunedPlans)
-      if (e.first == N) { L->plan = e.second; L->plan_N = N; L->tuned = 1; return 0; }
+  for (const std::pair<int, ConvPlan>& e : L->tunedPlans)  // a batch size seen (and timed) before: reuse its plan
+    if (e.first == N) { L->plan = e.second; L->plan_N = N; L->tuned = 1; return 0; }
   std::vector<std::pair<double, ConvPlan>> cands;
   bool found = false;
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G;
@@ -1021,8 +1020,7 @@ int PlanConv(qcnn_layer* L, int N) {
   // keep the kMaxCand cheapest tilings (by the model); LaunchConv times them on the device the first time a batch size
   // is seen (QCNN_AUTOTUNE=0 keeps the model's first choice)
   std::stable_sort(cands.begin(), cands.end(), [](const std::pair<double, ConvPlan>& x, const std::pair<double, ConvPlan>& y) { return x.first < y.first; });
-  if (!L->cands) L->cands = new std::vector<ConvPlan>();
-  L->cands->clear();
+  L->cands.clear();
   // layer parameter "force_kernel" / QCNN_FORCE_KERNEL=<0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc>
   // restricts the choice (tests pin the kernel they check; fails when that kernel has no tiling for the layer)
   // Within the LUT + gather family the kernels come in two numerical classes -- fp32 LUT / decode (s1, roll, direct) and
@@ -1059,7 +1057,7 @@ int PlanConv(qcnn_layer* L, int N) {
   // every kernel family that has a feasible tiling gets at least two seats among the candidates
   for (int pass = 0; pass < 2; pass++) {
     int perKernel[kConvKernelIds] = {};
-    for (size_t i = 0; i < cands.size() && L->cands->size() < kMaxCand; i++) {
+    for (size_t i = 0; i < cands.size() && L->cands.size() < kMaxCand; i++) {
       ConvPlan c = cands[i].second;
       if (pass == 0 && perKernel[c.kernel] >= (c.kernel == kConvDirect ? 8 : (c.kernel == kPqGemmTc ? 6 : 2))) continue;
       ConvArgs& a = c.a;
@@ -1069,23 +1067,23 @@ int PlanConv(qcnn_layer* L, int N) {
       a.S = L->S; a.K = L->K; a.d = L->d;
       // skip near-duplicates: same kernel/CPT/J/channel tiling and a strip count already present
       bool dup = false;
-      for (const ConvPlan& e : *L->cands)
+      for (const ConvPlan& e : L->cands)
         if (e.kernel == c.kernel && e.CPT == c.CPT && e.J == c.J && e.a.nct == c.a.nct && e.a.nstrips == c.a.nstrips &&
             e.a.rgroups == c.a.rgroups && e.a.R == c.a.R && (e.kernel != kConvDirect || e.J == c.J)) dup = true;
       if (dup) continue;
-      L->cands->push_back(c);
+      L->cands.push_back(c);
       perKernel[c.kernel]++;
     }
   }
   // the model's overall favourite first (it is the plan used when autotuning is off)
-  for (size_t i = 1; i < L->cands->size(); i++)
-    if ((*L->cands)[i].kernel == cands[0].second.kernel && (*L->cands)[i].CPT == cands[0].second.CPT &&
-        (*L->cands)[i].J == cands[0].second.J && (*L->cands)[i].a.nct == cands[0].second.a.nct &&
-        (*L->cands)[i].a.nstrips == cands[0].second.a.nstrips && (*L->cands)[i].a.rgroups == cands[0].second.a.rgroups) {
-      std::swap((*L->cands)[0], (*L->cands)[i]);
+  for (size_t i = 1; i < L->cands.size(); i++)
+    if (L->cands[i].kernel == cands[0].second.kernel && L->cands[i].CPT == cands[0].second.CPT &&
+        L->cands[i].J == cands[0].second.J && L->cands[i].a.nct == cands[0].second.a.nct &&
+        L->cands[i].a.nstrips == cands[0].second.a.nstrips && L->cands[i].a.rgroups == cands[0].second.a.rgroups) {
+      std::swap(L->cands[0], L->cands[i]);
       break;
     }
-  const ConvPlan best = (*L->cands)[0];
+  const ConvPlan best = L->cands[0];
   L->plan = best;
   L->plan_N = N;
   L->tuned = 0;
@@ -1104,7 +1102,7 @@ static int LaunchDirect(const ConvPlan& p, const ConvArgs& a, cudaStream_t st) {
 
 static int LaunchPlan(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
   ConvArgs a = p.a;
-  a.src = src; a.dst = dst; a.ctrd = L->d_ctrd; a.asmt = L->d_asmt; a.bias = L->d_bias;
+  a.src = src; a.dst = dst; a.ctrd = L->d_ctrd.as<float>(); a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
   a.N = N; a.relu = relu; a.src_nchw = L->src_nchw;
   if (p.kernel == kPqGemmTc) return LaunchPqGemm(L, p, src, N, dst, relu, st);
   if (p.kernel == kConvDirect) {
@@ -1131,14 +1129,14 @@ int LaunchConv(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
   static const bool autotune = !(getenv("QCNN_AUTOTUNE") && getenv("QCNN_AUTOTUNE")[0] == '0');
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(st, &cap);
-  if (autotune && !L->opt_no_autotune && !L->tuned && L->cands && L->cands->size() > 1 && cap == cudaStreamCaptureStatusNone) {
+  if (autotune && !L->opt_no_autotune && !L->tuned && L->cands.size() > 1 && cap == cudaStreamCaptureStatusNone) {
     cudaEvent_t e0, e1;
     QCNN_CUDA(cudaEventCreate(&e0));
     if (cudaEventCreate(&e1) != cudaSuccess) { cudaEventDestroy(e0); return CudaFail(cudaGetLastError(), "cudaEventCreate", __FILE__, __LINE__); }
     float bestMs = 1e30f;
     size_t bestI = 0;
-    for (size_t i = 0; i < L->cands->size(); i++) {
-      const ConvPlan& c = (*L->cands)[i];
+    for (size_t i = 0; i < L->cands.size(); i++) {
+      const ConvPlan& c = L->cands[i];
       if (LaunchPlan(L, c, src, N, dst, relu, st)) continue;   // warm-up (also sets the smem attribute)
       // best of two timed samples (a sample = 1 launch at large batches, 3 at small ones): single samples made the choice
       // between near-equal candidates vary from run to run
@@ -1163,10 +1161,9 @@ int LaunchConv(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
     }
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
-    L->plan = (*L->cands)[bestI];
+    L->plan = L->cands[bestI];
     L->tuned = 1;
-    if (!L->tunedPlans) L->tunedPlans = new std::vector<std::pair<int, ConvPlan>>();
-    L->tunedPlans->emplace_back(N, L->plan);
+    L->tunedPlans.emplace_back(N, L->plan);
   }
   const int rc = LaunchPlan(L, L->plan, src, N, dst, relu, st);
   if (rc == 0) L->ctx->launches++;

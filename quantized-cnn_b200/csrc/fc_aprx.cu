@@ -357,52 +357,39 @@ static bool FcTcEligible(const qcnn_layer* L, int N) {
   return true;
 }
 
-// "pq_gemm_tc mode=2 ..." when batch N takes the tensor-core path, empty otherwise (bench / DESIGN bookkeeping)
-void DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap) {
-  buf[0] = 0;
-  if (!FcTcEligible(L, N)) return;
-  const int NT = N > 64 ? 128 : 64, KS = 3;
-  const int nct = CeilDiv(L->Dout, 128), tiles = CeilDiv(N, NT), kAll = L->Din / 8;
-  int nsplit = std::max(1, L->ctx->sm_count / (tiles * nct));
-  const int kPerSplit = RoundUp(CeilDiv(kAll, nsplit), KS);
-  nsplit = CeilDiv(kAll, kPerSplit);
-  snprintf(buf, cap, "pq_gemm_tc(wgmma, weights decoded into registers%s) mode=2 NT=%d GT=3 grid=%d nsplit=%d ksteps=%d",
-           L->opt_tc_bf ? ", bf16x2" : "", NT, tiles * nsplit * nct, nsplit, kPerSplit);
-}
+// k-steps per chunk of the tensor-core FC path (plane image of a chunk: 2 * 3 halves x NT images, hi + lo)
+constexpr int kFcKs = 3;
 
-int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled) {
-  *handled = false;
-  if (!FcTcEligible(L, N)) return 0;
-  qcnn_ctx* ctx = L->ctx;
-  const int KS = 3;                 // k-steps per chunk (plane image of a chunk: 2 * 3 halves x NT images, hi + lo)
-  const int NTq = N > 64 ? 128 : 64;   // the two wgmma N of pq_gemm_tc
-  const int tilesq = CeilDiv(N, NTq), nChunksAll = CeilDiv(L->Din / 8, KS);
-  GemmArgs a;
+// The tensor-core plan of the layer at batch N (everything but the activations, the output, the plane images and the
+// partial sums); false when the layer does not take that path.
+static bool PlanFcTc(const qcnn_layer* L, int N, GemmArgs* out) {
+  if (!FcTcEligible(L, N)) return false;
+  GemmArgs& a = *out;
   memset(&a, 0, sizeof(a));
   a.mode = 2;
-  a.src = src; a.dst = dst; a.ctrd = L->d_ctrd; a.asmt = L->d_asmt; a.bias = L->d_bias;
+  a.ctrd = L->d_ctrd.as<float>(); a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
   a.N = N; a.Cin = L->Din; a.Cout = L->Dout; a.G = 1; a.Cg = L->Din; a.Kg = L->Dout; a.KgPad = L->DoutPad;
   a.S = L->S; a.K = L->K; a.d = L->d; a.kshift = L->kshift;
   a.srcImg = L->Din; a.dstImg = 0;
   a.IB = 1; a.PW = 1;
-  a.NT = NTq;
-  a.corr = NTq <= 64 ? 1 : 0;
+  a.NT = N > 64 ? 128 : 64;   // the two wgmma N of pq_gemm_tc
+  a.corr = a.NT <= 64 ? 1 : 0;
   a.bf = L->opt_tc_bf ? 1 : 0;
-  if (a.bf && L->d_ctrd_bf) { a.ctrd = reinterpret_cast<const float*>(L->d_ctrd_bf); a.cbPre = 1; }   // (d % 4 == 0)
-  a.GT = 3;
-  a.nPB = 3; a.xprep = L->d_flat; a.nChunksAll = nChunksAll;
-  a.planeF4 = KS * 2 * a.NT;
-  a.planeRows = a.bf ? KS * a.NT : a.planeF4;
+  if (a.bf && L->d_ctrd_bf.get()) { a.ctrd = L->d_ctrd_bf.as<float>(); a.cbPre = 1; }   // (d % 4 == 0)
+  a.GT = kFcKs;
+  a.nPB = 3; a.nChunksAll = CeilDiv(L->Din / 8, kFcKs);
+  a.planeF4 = kFcKs * 2 * a.NT;
+  a.planeRows = a.bf ? kFcKs * a.NT : a.planeF4;
   a.NPOS = a.NT;
-  a.cbSlots = L->d == 1 ? 8 * KS : 2 * KS;
+  a.cbSlots = L->d == 1 ? 8 * kFcKs : 2 * kFcKs;
   a.idRows = a.cbSlots;
   a.cbF4 = L->d == 1 ? L->K / 4 : L->K;
-  a.ntab = KS;
-  a.chunkFirst[0] = 0; a.chunkCount[0] = KS;
-  for (int i = 0; i < KS; i++) {
+  a.ntab = kFcKs;
+  a.chunkFirst[0] = 0; a.chunkCount[0] = kFcKs;
+  for (int i = 0; i < kFcKs; i++) {
     KStep& ks = a.tab[i];
     ks.bStart = 2 * i * a.NT; ks.lbo = a.NT;
-    if (a.bf) { ks.bStart = i * a.NT; ks.lbo = KS * a.NT; }   // row = (k-step, image); x2 plane = K-core-matrix 1
+    if (a.bf) { ks.bStart = i * a.NT; ks.lbo = kFcKs * a.NT; }   // row = (k-step, image); x2 plane = K-core-matrix 1
     if (L->d == 1) { ks.idx0 = static_cast<short>(8 * i); ks.idx1 = static_cast<short>(8 * i + 4); }
     else { ks.idx0 = static_cast<short>(2 * i); ks.idx1 = static_cast<short>(2 * i + 1); }
     ks.cb0 = ks.idx0; ks.cb1 = ks.idx1;
@@ -410,53 +397,51 @@ int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
   a.nct = CeilDiv(L->Dout, 128);
   const int tiles = CeilDiv(N, a.NT);
   a.kAll = L->Din / 8;
-  int nsplit = std::max(1, ctx->sm_count / (tiles * a.nct));
-  a.kPerSplit = RoundUp(CeilDiv(a.kAll, nsplit), KS);
-  nsplit = CeilDiv(a.kAll, a.kPerSplit);
-  a.nsplit = nsplit;
-  a.dstRow = nsplit > 1 ? L->DoutPad : L->Dout;
-  a.relu = nsplit > 1 ? 0 : relu;
-  if (PqGemmSmemBytes(a) > (ctx->smem_optin ? ctx->smem_optin : 227 * 1024)) return 0;   // before any launch / allocation
+  a.nsplit = std::max(1, L->ctx->sm_count / (tiles * a.nct));
+  a.kPerSplit = RoundUp(CeilDiv(a.kAll, a.nsplit), kFcKs);
+  a.nsplit = CeilDiv(a.kAll, a.kPerSplit);
+  a.dstRow = a.nsplit > 1 ? L->DoutPad : L->Dout;
+  return PqGemmSmemBytes(a) <= (L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024);
+}
+
+// "pq_gemm_tc mode=2 ..." when batch N takes the tensor-core path, empty otherwise (bench / DESIGN bookkeeping)
+void DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap) {
+  buf[0] = 0;
+  GemmArgs a;
+  if (!PlanFcTc(L, N, &a)) return;
+  snprintf(buf, cap, "pq_gemm_tc(wgmma, weights decoded into registers%s) mode=2 NT=%d GT=3 grid=%d nsplit=%d ksteps=%d",
+           a.bf ? ", bf16x2" : "", a.NT, CeilDiv(N, a.NT) * a.nsplit * a.nct, a.nsplit, a.kPerSplit);
+}
+
+int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled) {
+  *handled = false;
+  GemmArgs a;
+  if (!PlanFcTc(L, N, &a)) return 0;   // before any launch / allocation
+  qcnn_ctx* ctx = L->ctx;
+  const int tiles = CeilDiv(N, a.NT);
+  a.src = src; a.dst = dst;
+  a.relu = a.nsplit > 1 ? 0 : relu;
   {
-    const size_t per = a.bf ? static_cast<size_t>(KS) * NTq : static_cast<size_t>(2 * KS) * NTq;   // 16-byte rows per plane
-    const size_t total = static_cast<size_t>(tilesq) * nChunksAll * per;
-    const size_t need = total * 2 * sizeof(float4);
-    if (need > L->flat_bytes) {
-      if (L->d_flat) QCNN_CUDA(cudaFree(L->d_flat));
-      L->d_flat = nullptr; L->flat_bytes = 0;
-      QCNN_CUDA(cudaMalloc(&L->d_flat, need));
-      L->ctx->alloc_epoch++;
-      L->flat_bytes = need;
-    }
-    a.xprep = L->d_flat;
+    const size_t total = static_cast<size_t>(tiles) * a.nChunksAll * a.planeRows;   // 16-byte rows of one plane (hi or lo)
+    QCNN_CUDA(L->d_flat.Reserve(ctx, total * 2 * sizeof(float4), st));
+    a.xprep = L->d_flat.as<float>();
     if (a.bf)
-      fc_prep_bf_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(src, L->d_srcoff, reinterpret_cast<uint4*>(L->d_flat),
-                                                                                 N, L->Din, NTq, KS, nChunksAll, tilesq);
+      fc_prep_bf_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(src, L->d_srcoff.as<int>(), L->d_flat.as<uint4>(),
+                                                                                 N, L->Din, a.NT, kFcKs, a.nChunksAll, tiles);
     else
-      fc_prep_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(src, L->d_srcoff, reinterpret_cast<float4*>(L->d_flat),
-                                                                              N, L->Din, NTq, KS, nChunksAll, tilesq);
+      fc_prep_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(src, L->d_srcoff.as<int>(), L->d_flat.as<float4>(),
+                                                                              N, L->Din, a.NT, kFcKs, a.nChunksAll, tiles);
     QCNN_CUDA(cudaGetLastError());
     ctx->launches++;
   }
-  if (nsplit > 1) {
-    const size_t need = sizeof(float) * static_cast<size_t>(nsplit) * N * L->DoutPad;
-    if (need > L->partial_bytes) {
-      if (L->d_partial) QCNN_CUDA(cudaFree(L->d_partial));
-      L->d_partial = nullptr; L->partial_bytes = 0;
-      QCNN_CUDA(cudaMalloc(&L->d_partial, need));
-      L->ctx->alloc_epoch++;
-      L->partial_bytes = need;
-    }
-    a.partial = L->d_partial;
+  if (a.nsplit > 1) {
+    QCNN_CUDA(L->d_partial.Reserve(ctx, sizeof(float) * static_cast<size_t>(a.nsplit) * N * L->DoutPad, st));
+    a.partial = L->d_partial.as<float>();
   }
-  if (int rc = LaunchPqGemmArgs(ctx, a, static_cast<long long>(tiles) * nsplit * a.nct, st)) return rc;
+  if (int rc = LaunchPqGemmArgs(ctx, a, static_cast<long long>(tiles) * a.nsplit * a.nct, st)) return rc;
   ctx->launches++;
-  if (nsplit > 1) {
-    const int total = N * L->Dout;
-    fc_reduce_kernel<<<CeilDiv(total, 256), 256, 0, st>>>(a.partial, dst, N, L->Dout, L->DoutPad, nsplit, relu);
-    QCNN_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
+  if (a.nsplit > 1)
+    if (int rc = LaunchSplitReduce(ctx, a.partial, dst, N, L->Dout, L->DoutPad, a.nsplit, relu, st)) return rc;
   *handled = true;
   return 0;
 }
@@ -475,9 +460,9 @@ int LaunchFc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaS
   qcnn_ctx* ctx = L->ctx;
   FcArgs a;
   a.src = src; a.dst = dst; a.partial = nullptr;
-  a.ctrd = L->d_ctrd; a.asmt = L->d_asmt; a.bias = L->d_bias;
+  a.ctrd = L->d_ctrd.as<float>(); a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
   a.N = N; a.Din = L->Din; a.Dout = L->Dout; a.DoutPad = L->DoutPad; a.S = L->S; a.K = L->K; a.d = L->d;
-  a.srcoff = L->d_srcoff;
+  a.srcoff = L->d_srcoff.as<int>();
   a.relu = relu;
 
   // batch tile: 1 (latency path, 16 channels/thread, 128-bit loads), 4 or 8 images per CTA
@@ -501,16 +486,8 @@ int LaunchFc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaS
   a.s_per_split = chunks_per_split * pf;
   a.nsplit = nsplit;
   if (nsplit > 1) {
-    const size_t need = sizeof(float) * static_cast<size_t>(nsplit) * N * L->DoutPad;
-    if (need > L->partial_bytes) {
-      if (L->d_partial) QCNN_CUDA(cudaFree(L->d_partial));
-      L->d_partial = nullptr;
-      L->partial_bytes = 0;
-      QCNN_CUDA(cudaMalloc(&L->d_partial, need));
-      L->ctx->alloc_epoch++;
-      L->partial_bytes = need;
-    }
-    a.partial = L->d_partial;
+    QCNN_CUDA(L->d_partial.Reserve(ctx, sizeof(float) * static_cast<size_t>(nsplit) * N * L->DoutPad, st));
+    a.partial = L->d_partial.as<float>();
   }
   dim3 grid(gx, gy, nsplit);
   int rc;
@@ -527,12 +504,7 @@ int LaunchFc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaS
   }
   if (rc) return rc;
   ctx->launches++;
-  if (nsplit > 1) {
-    const int total = N * L->Dout;
-    fc_reduce_kernel<<<CeilDiv(total, 256), 256, 0, st>>>(a.partial, dst, N, L->Dout, L->DoutPad, nsplit, relu);
-    QCNN_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
+  if (nsplit > 1) return LaunchSplitReduce(ctx, a.partial, dst, N, L->Dout, L->DoutPad, nsplit, relu, st);
   return 0;
 }
 

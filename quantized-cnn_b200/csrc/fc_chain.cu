@@ -495,10 +495,11 @@ static bool PlanChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu,
   for (int l = 0; l < n; l++) {
     const qcnn_layer* Q = layers[l];
     if (Q->kind != QCNN_KIND_FC || Q->opt_fc_nsplit || Q->opt_fc_tn) return false;
-    if (l > 0 && (Q->Din != layers[l - 1]->Dout || Q->d_srcoff)) return false;
+    if (l > 0 && (Q->Din != layers[l - 1]->Dout || Q->d_srcoff.get())) return false;
     if (Q->DoutPad > kChunkBytes || Q->K * Q->d % 4 != 0) return false;
     ChainLayer& L = a.L[l];
-    L.ctrd = Q->d_ctrd; L.asmt = Q->d_asmt; L.bias = Q->d_bias; L.srcoff = Q->d_srcoff; L.partial = Q->d_cpart;
+    L.ctrd = Q->d_ctrd.as<float>(); L.asmt = Q->d_asmt.as<uint8_t>(); L.bias = Q->d_bias.as<float>(); L.srcoff = Q->d_srcoff.as<int>();
+    L.partial = Q->d_cpart.as<float>();
     L.Din = Q->Din; L.Dout = Q->Dout; L.DoutPad = Q->DoutPad; L.S = Q->S; L.K = Q->K; L.d = Q->d;
     L.log2K = 0;
     while ((1 << L.log2K) < Q->K) L.log2K++;
@@ -513,8 +514,8 @@ static bool PlanChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu,
     L.tprInv = 1.0f / static_cast<float>(L.tpr);
     for (int t = 0; t < kConsumers; t++)     // the kernel divides by multiplying: must be exact for every thread index
       if (static_cast<int>(floorf((static_cast<float>(t) + 0.5f) * L.tprInv)) != t / L.tpr) return false;
-    if (Q->d_srcoff && Q->src_h > 0 && l == 0) {   // NHWC fold by arithmetic (same check); otherwise the offset table is used
-                                                   // (d_srcoff is NULL while qcnn_fc_aprx_forward_flat passes a flat vector)
+    if (Q->d_srcoff.get() && Q->src_h > 0 && l == 0) {   // NHWC fold by arithmetic (same check); otherwise the offset table is used
+                                                         // (d_srcoff is empty while qcnn_fc_aprx_forward_flat passes a flat vector)
       const int hw = Q->src_h * Q->src_w;
       const float inv = 1.0f / static_cast<float>(hw);
       bool exact = true;
@@ -578,17 +579,11 @@ int LaunchFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int
     qcnn_layer* Q = layers[l];
     if (Q->kind != QCNN_KIND_FC) return 0;
     const size_t need = sizeof(float) * static_cast<size_t>(ctx->sm_count) * Q->DoutPad;
-    if (Q->cpart_bytes < need) {
-      cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-      if (st) cudaStreamIsCapturing(st, &cap);
-      if (cap != cudaStreamCaptureStatusNone) return 0;   // cannot allocate inside a capture: per-layer kernels this time
-      if (Q->d_cpart) QCNN_CUDA(cudaFree(Q->d_cpart));
-      Q->d_cpart = nullptr; Q->cpart_bytes = 0;
-      QCNN_CUDA(cudaMalloc(&Q->d_cpart, need));
-      QCNN_CUDA(cudaMemsetAsync(Q->d_cpart, 0xFF, need, st));
-      Q->cpart_bytes = need;
-      ctx->alloc_epoch++;
-    }
+    bool grown = false;
+    const cudaError_t e = Q->d_cpart.Reserve(ctx, need, st, &grown);
+    if (e == cudaErrorStreamCaptureUnsupported) return 0;   // cannot allocate inside a capture: per-layer kernels this time
+    QCNN_CUDA(e);
+    if (grown) QCNN_CUDA(cudaMemsetAsync(Q->d_cpart.get(), 0xFF, need, st));
   }
   ChainArgs a;
   size_t smem = 0;

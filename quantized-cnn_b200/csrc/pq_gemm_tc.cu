@@ -696,7 +696,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
         ga.planeRows = ga.bf ? (st / 2) * ga.NPOS : ga.planeF4;
         ga.cbSlots = 2; ga.idRows = rowsPer * L->ksz;
         ga.tapsPad = RoundUp(rowsPer * L->ksz, 16);
-        ga.idxT = (ga.tapsPad <= 48 && L->d_asmt_t && L->asmt_t_mode == 1) ? 1 : 0;
+        ga.idxT = (ga.tapsPad <= 48 && L->d_asmt_t.get() && L->asmt_t_mode == 1) ? 1 : 0;
         if (ga.idxT) ga.idRows = ga.tapsPad;       // [128 channels][tapsPad] bytes
         ga.nChunks = st;
         ga.K = L->K; ga.cbF4 = L->K; ga.nPB = 2;
@@ -777,7 +777,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
       ga.planeRows = ga.bf ? ga.NPOS : ga.planeF4;   // (bf16x2: lbo = NPOS rows is the x1 -> x2 plane distance as well)
       ga.cbSlots = 2; ga.idRows = 2 * taps;
       ga.tapsPad = RoundUp(taps, 16);
-      ga.idxT = (ga.tapsPad <= 32 && L->d_asmt_t && L->asmt_t_mode == 0) ? 1 : 0;
+      ga.idxT = (ga.tapsPad <= 32 && L->d_asmt_t.get() && L->asmt_t_mode == 0) ? 1 : 0;
       if (ga.idxT) ga.idRows = 2 * ga.tapsPad;      // [half][128 channels][tapsPad] bytes = 2 * tapsPad rows of 128
       ga.nChunks = CeilDiv(Cg, 8);
       ga.ntab = taps;
@@ -840,11 +840,11 @@ static int LaunchKernel(const GemmArgs& a, unsigned blocks, size_t smem, cudaStr
 // bf16x2 form of the codebook, made once per layer: every aligned 4-float piece becomes {w1 (4 x bf16), w2 (4 x bf16)},
 // stored [S][d/4][K] so that the K pieces a chunk stages are one contiguous run (bulk-copyable)
 int BuildCtrdBf(qcnn_layer* L) {
-  if (L->d % 4 != 0 || L->d_ctrd_bf) return 0;
+  if (L->d % 4 != 0 || L->d_ctrd_bf.get()) return 0;
   const size_t n = static_cast<size_t>(L->S) * L->K * L->d / 4;
-  QCNN_CUDA(cudaMalloc(&L->d_ctrd_bf, n * sizeof(uint4)));
+  QCNN_CUDA(L->d_ctrd_bf.Reserve(L->ctx, n * sizeof(uint4)));
   split_codebook_kernel<<<static_cast<unsigned>(std::min<size_t>((n + 255) / 256, 1024)), 256>>>(
-      reinterpret_cast<const float4*>(L->d_ctrd), reinterpret_cast<uint4*>(L->d_ctrd_bf), L->S, L->K, L->d / 4);
+      L->d_ctrd.as<const float4>(), L->d_ctrd_bf.as<uint4>(), L->S, L->K, L->d / 4);
   QCNN_CUDA(cudaGetLastError());
   QCNN_CUDA(cudaDeviceSynchronize());
   return 0;
@@ -852,9 +852,9 @@ int BuildCtrdBf(qcnn_layer* L) {
 
 int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
   GemmArgs a = p.g;
-  a.src = src; a.dst = dst; a.ctrd = L->d_ctrd; a.asmt = L->d_asmt; a.bias = L->d_bias;
-  if (a.bf && L->d_ctrd_bf) { a.ctrd = reinterpret_cast<const float*>(L->d_ctrd_bf); a.cbPre = 1; }
-  a.asmtT = L->d_asmt_t;
+  a.src = src; a.dst = dst; a.ctrd = L->d_ctrd.as<float>(); a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
+  if (a.bf && L->d_ctrd_bf.get()) { a.ctrd = L->d_ctrd_bf.as<float>(); a.cbPre = 1; }
+  a.asmtT = L->d_asmt_t.as<uint8_t>();
   a.bulkC = (a.mode != 2 && a.idxT && a.cbPre) ? 1 : 0;
   if (a.mode == 1 && !a.bulkC) a.idxT = 0;   // (3xTF32 operands: index rows by cp.async in tap-major order; the planned buffer is large enough)
   a.N = N; a.relu = a.nsplit > 1 ? 0 : relu;
@@ -869,15 +869,8 @@ int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, floa
   const long long blocks = static_cast<long long>(CeilDiv(N * a.IB, a.NT)) * a.G * a.nct * a.nsplit;
   QCNN_CHECK(blocks <= 2147483647LL, "qcnn_conv_aprx_forward: batch too large for the tensor-core tiling");
   if (a.nsplit > 1) {
-    const size_t need = sizeof(float) * static_cast<size_t>(a.nsplit) * N * a.dstImg;
-    if (need > L->partial_bytes) {
-      if (L->d_partial) QCNN_CUDA(cudaFree(L->d_partial));
-      L->d_partial = nullptr; L->partial_bytes = 0;
-      QCNN_CUDA(cudaMalloc(&L->d_partial, need));
-      L->ctx->alloc_epoch++;
-      L->partial_bytes = need;
-    }
-    a.partial = L->d_partial;
+    QCNN_CUDA(L->d_partial.Reserve(L->ctx, sizeof(float) * static_cast<size_t>(a.nsplit) * N * a.dstImg, st));
+    a.partial = L->d_partial.as<float>();
   }
   if (int rc = SetSmemLimitOnce(L->ctx)) return rc;
   if (int rc = LaunchKernel(a, static_cast<unsigned>(blocks), p.smem, st)) return rc;

@@ -7,7 +7,6 @@
 // All arithmetic follows the reference expression by expression (same float / double steps, no FMA contraction), so the
 // preprocessing is bit-identical to the CPU path (tests/test_gpu_preproc.py).
 #include <float.h>
-#include <string.h>
 
 #include <vector>
 
@@ -20,9 +19,8 @@ struct qcnn_preproc {
   int reszType, meanType;      // ENUM_ReszType { Strict, Relaxed }, ENUM_MeanType { Full, Crop } (include/BmpImgIO.h:19-20)
   int heiFull, widFull, heiCrop, widCrop;
   int meanHei, meanWid;
-  float* d_mean;               // [3][meanHei][meanWid]
-  void* d_desc;                // per-image descriptors of the last run
-  size_t descCap;
+  DeviceBuffer d_mean;         // float [3][meanHei][meanWid]
+  DeviceBuffer d_desc;         // per-image descriptors of the last run
 };
 
 namespace {
@@ -184,14 +182,12 @@ int qcnn_preproc_create(qcnn_ctx* ctx, int resz_type, int mean_type, int hei_ful
   }
   QCNN_ON_DEVICE(ctx->device);
   qcnn_preproc* p = new qcnn_preproc();
-  memset(static_cast<void*>(p), 0, sizeof(*p));
   p->ctx = ctx; p->reszType = resz_type; p->meanType = mean_type;
   p->heiFull = hei_full; p->widFull = wid_full; p->heiCrop = hei_crop; p->widCrop = wid_crop;
   p->meanHei = mean_hei; p->meanWid = mean_wid;
   const size_t bytes = sizeof(float) * 3 * static_cast<size_t>(mean_hei) * mean_wid;
-  if (cudaMalloc(&p->d_mean, bytes) != cudaSuccess || cudaMemcpy(p->d_mean, mean_h, bytes, cudaMemcpyHostToDevice) != cudaSuccess) {
-    CudaFail(cudaGetLastError(), "preproc mean upload", __FILE__, __LINE__);
-    if (p->d_mean) cudaFree(p->d_mean);
+  if (cudaError_t e = p->d_mean.Upload(ctx, mean_h, bytes)) {
+    CudaFail(e, "preproc mean upload", __FILE__, __LINE__);
     delete p;
     return 2;
   }
@@ -202,8 +198,6 @@ int qcnn_preproc_create(qcnn_ctx* ctx, int resz_type, int mean_type, int hei_ful
 void qcnn_preproc_destroy(qcnn_preproc* p) {
   if (!p) return;
   DeviceGuard guard(p->ctx->device);
-  if (p->d_mean) cudaFree(p->d_mean);
-  if (p->d_desc) cudaFree(p->d_desc);
   delete p;
 }
 
@@ -230,16 +224,11 @@ int qcnn_preproc_run(qcnn_preproc* p, const uint8_t* pix, const long long* off_h
     desc[i].off = off_h[i]; desc[i].hs = hs; desc[i].ws = ws; desc[i].hd = hd; desc[i].wd = wd; desc[i].sh = sh; desc[i].sw = sw;
   }
   const size_t need = sizeof(ImgDesc) * N;
-  if (need > p->descCap) {
-    if (p->d_desc) QCNN_CUDA(cudaFree(p->d_desc));
-    p->d_desc = nullptr; p->descCap = 0;
-    QCNN_CUDA(cudaMalloc(&p->d_desc, need));
-    p->descCap = need;
-  }
+  QCNN_CUDA(p->d_desc.Reserve(p->ctx, need, st));
   // (pageable source: the copy is staged by the runtime before the call returns, so `desc` may go out of scope)
-  QCNN_CUDA(cudaMemcpyAsync(p->d_desc, desc.data(), need, cudaMemcpyHostToDevice, st));
+  QCNN_CUDA(cudaMemcpyAsync(p->d_desc.get(), desc.data(), need, cudaMemcpyHostToDevice, st));
   dim3 grid(CeilDiv(p->heiCrop * p->widCrop, 256), N);
-  bmp_preproc_kernel<<<grid, 256, 0, st>>>(pix, static_cast<const ImgDesc*>(p->d_desc), p->d_mean, p->meanHei, p->meanWid,
+  bmp_preproc_kernel<<<grid, 256, 0, st>>>(pix, p->d_desc.as<const ImgDesc>(), p->d_mean.as<float>(), p->meanHei, p->meanWid,
                                            p->meanType == 0 ? 1 : 0, p->heiCrop, p->widCrop, dst);
   QCNN_CUDA(cudaGetLastError());
   p->ctx->launches++;

@@ -102,7 +102,6 @@ int qcnn_stream_sync(qcnn_ctx* ctx, void* stream) {
 
 static qcnn_layer* NewLayer(qcnn_ctx* ctx, int kind) {
   qcnn_layer* L = new qcnn_layer();
-  memset(static_cast<void*>(L), 0, sizeof(*L));
   L->ctx = ctx;
   L->kind = kind;
   // default operand format of the tensor-core GEMMs: bf16x2 (two MMAs per k-step at twice the tf32 rate; error at the
@@ -155,7 +154,6 @@ int qcnn_conv_layer_create(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, i
         for (int s = 0; s < S; s++)
           dev[((static_cast<size_t>(g) * S + s) * taps + t) * KgPad + c] =
               asmt_h[((static_cast<size_t>(g) * Kg + c) * taps + t) * S + s];
-  L->asmt_bytes = dev.size();
   // channel-major copy for the tensor-core GEMM's decoders: [grp][S][KgPad][tapsPad]
   const int tapsPad = RoundUp(taps, 16);
   std::vector<uint8_t> devT;
@@ -179,19 +177,12 @@ int qcnn_conv_layer_create(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, i
           for (int t = 0; t < taps; t++)
             devT[((static_cast<size_t>(g) * S + s) * KgPad + c) * tapsPad + t] = dev[((static_cast<size_t>(g) * S + s) * taps + t) * KgPad + c];
   }
-  int rc = 0;
-  do {
-    if ((rc = (cudaMalloc(&L->d_asmt, dev.size()) != cudaSuccess))) break;
-    if ((rc = (cudaMalloc(&L->d_asmt_t, devT.size()) != cudaSuccess))) break;
-    if ((rc = (cudaMemcpy(L->d_asmt_t, devT.data(), devT.size(), cudaMemcpyHostToDevice) != cudaSuccess))) break;
-    if ((rc = (cudaMalloc(&L->d_ctrd, sizeof(float) * S * K * d) != cudaSuccess))) break;
-    if ((rc = (cudaMalloc(&L->d_bias, sizeof(float) * Cout) != cudaSuccess))) break;
-    if ((rc = (cudaMemcpy(L->d_asmt, dev.data(), dev.size(), cudaMemcpyHostToDevice) != cudaSuccess))) break;
-    if ((rc = (cudaMemcpy(L->d_ctrd, ctrd_h, sizeof(float) * S * K * d, cudaMemcpyHostToDevice) != cudaSuccess))) break;
-    if ((rc = (cudaMemcpy(L->d_bias, bias_h, sizeof(float) * Cout, cudaMemcpyHostToDevice) != cudaSuccess))) break;
-  } while (0);
-  if (rc) {
-    CudaFail(cudaGetLastError(), "conv layer upload", __FILE__, __LINE__);
+  cudaError_t e = L->d_asmt.Upload(ctx, dev.data(), dev.size());
+  if (!e) e = L->d_asmt_t.Upload(ctx, devT.data(), devT.size());
+  if (!e) e = L->d_ctrd.Upload(ctx, ctrd_h, sizeof(float) * S * K * d);
+  if (!e) e = L->d_bias.Upload(ctx, bias_h, sizeof(float) * Cout);
+  if (e) {
+    CudaFail(e, "conv layer upload", __FILE__, __LINE__);
     qcnn_layer_destroy(L);
     return 2;
   }
@@ -224,18 +215,11 @@ int qcnn_fc_layer_create(qcnn_ctx* ctx, int Din, int Dout, int S, int K, int d, 
   for (int o = 0; o < Dout; o++)
     for (int s = 0; s < S; s++)
       dev[static_cast<size_t>(s) * L->DoutPad + o] = static_cast<uint8_t>(asmt_h[static_cast<size_t>(o) * S + s] << L->kshift);
-  L->asmt_bytes = dev.size();
-  int rc = 0;
-  do {
-    if ((rc = (cudaMalloc(&L->d_asmt, dev.size()) != cudaSuccess))) break;
-    if ((rc = (cudaMalloc(&L->d_ctrd, sizeof(float) * S * K * d) != cudaSuccess))) break;
-    if ((rc = (cudaMalloc(&L->d_bias, sizeof(float) * Dout) != cudaSuccess))) break;
-    if ((rc = (cudaMemcpy(L->d_asmt, dev.data(), dev.size(), cudaMemcpyHostToDevice) != cudaSuccess))) break;
-    if ((rc = (cudaMemcpy(L->d_ctrd, ctrd_h, sizeof(float) * S * K * d, cudaMemcpyHostToDevice) != cudaSuccess))) break;
-    if ((rc = (cudaMemcpy(L->d_bias, bias_h, sizeof(float) * Dout, cudaMemcpyHostToDevice) != cudaSuccess))) break;
-  } while (0);
-  if (rc) {
-    CudaFail(cudaGetLastError(), "fc layer upload", __FILE__, __LINE__);
+  cudaError_t e = L->d_asmt.Upload(ctx, dev.data(), dev.size());
+  if (!e) e = L->d_ctrd.Upload(ctx, ctrd_h, sizeof(float) * S * K * d);
+  if (!e) e = L->d_bias.Upload(ctx, bias_h, sizeof(float) * Dout);
+  if (e) {
+    CudaFail(e, "fc layer upload", __FILE__, __LINE__);
     qcnn_layer_destroy(L);
     return 2;
   }
@@ -248,7 +232,7 @@ int qcnn_fc_layer_set_src_nhwc(qcnn_layer* L, int H, int W, int C) {
   QCNN_CHECK(L && L->kind == QCNN_KIND_FC, "qcnn_fc_layer_set_src_nhwc: not an FC layer");
   QCNN_ON_DEVICE(L->ctx->device);
   L->ctx->alloc_epoch++;   // captured graphs may hold the old offset table / kernel choice
-  if (L->d_srcoff) { cudaFree(L->d_srcoff); L->d_srcoff = nullptr; }
+  QCNN_CUDA(L->d_srcoff.Release());
   if (H == 0 && W == 0 && C == 0) { L->src_h = L->src_w = L->src_c = 0; return 0; }
   QCNN_CHECK(H >= 1 && W >= 1 && C >= 1 && H * W * C == L->Din, "qcnn_fc_layer_set_src_nhwc: H*W*C=%d != Din=%d",
              H * W * C, L->Din);
@@ -257,8 +241,7 @@ int qcnn_fc_layer_set_src_nhwc(qcnn_layer* L, int H, int W, int C) {
   std::vector<int> off(L->Din);
   const int hw = H * W;
   for (int f = 0; f < L->Din; f++) off[f] = (f % hw) * C + f / hw;
-  QCNN_CUDA(cudaMalloc(&L->d_srcoff, sizeof(int) * L->Din));
-  QCNN_CUDA(cudaMemcpy(L->d_srcoff, off.data(), sizeof(int) * L->Din, cudaMemcpyHostToDevice));
+  QCNN_CUDA(L->d_srcoff.Upload(L->ctx, off.data(), sizeof(int) * L->Din));
   return 0;
 }
 
@@ -282,7 +265,7 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
     L->opt_no_tc = value ? 0 : 1;
     L->opt_tc_bf = value == 2 ? 1 : 0;
     L->plan_N = 0; L->tuned = 0;
-    if (L->tunedPlans) L->tunedPlans->clear();
+    L->tunedPlans.clear();
   }
   else if (!strcmp(name, "force_kernel") || !strcmp(name, "autotune") || !strcmp(name, "gemm_nt") ||
            !strcmp(name, "gemm_gt") || !strcmp(name, "gemm_nsplit")) {
@@ -298,7 +281,7 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
     else if (!strcmp(name, "gemm_nsplit")) L->opt_gemm_nsplit = value < 0 ? 0 : value;
     else L->opt_no_autotune = value ? 0 : 1;
     L->plan_N = 0; L->tuned = 0;
-    if (L->tunedPlans) L->tunedPlans->clear();
+    L->tunedPlans.clear();
   }
   else { SetError("qcnn_layer_set_param: unknown parameter '%s'", name); return 1; }
   return 0;
@@ -320,17 +303,6 @@ int qcnn_layer_describe(qcnn_layer* L, int N, char* buf, size_t cap) {
 void qcnn_layer_destroy(qcnn_layer* L) {
   if (!L) return;
   DeviceGuard guard(L->ctx->device);
-  if (L->d_asmt) cudaFree(L->d_asmt);
-  if (L->d_asmt_t) cudaFree(L->d_asmt_t);
-  if (L->d_ctrd) cudaFree(L->d_ctrd);
-  if (L->d_bias) cudaFree(L->d_bias);
-  if (L->d_partial) cudaFree(L->d_partial);
-  if (L->d_flat) cudaFree(L->d_flat);
-  if (L->d_cpart) cudaFree(L->d_cpart);
-  if (L->d_ctrd_bf) cudaFree(L->d_ctrd_bf);
-  if (L->d_srcoff) cudaFree(L->d_srcoff);
-  delete L->cands;
-  delete L->tunedPlans;
   delete L;
 }
 
@@ -382,8 +354,8 @@ int qcnn_layer_work(const qcnn_layer* L, int N, double* alg_bytes, double* looku
 int qcnn_layer_read_asmt_h(const qcnn_layer* L, uint8_t* out_h, size_t cap) {
   QCNN_CHECK(L && out_h, "qcnn_layer_read_asmt_h: NULL argument");
   QCNN_ON_DEVICE(L->ctx->device);
-  std::vector<uint8_t> dev(L->asmt_bytes);
-  QCNN_CUDA(cudaMemcpy(dev.data(), L->d_asmt, dev.size(), cudaMemcpyDeviceToHost));
+  std::vector<uint8_t> dev(L->d_asmt.bytes());
+  QCNN_CUDA(cudaMemcpy(dev.data(), L->d_asmt.get(), dev.size(), cudaMemcpyDeviceToHost));
   if (L->kind == QCNN_KIND_CONV) {
     const int taps = L->ksz * L->ksz, Kg = L->Cout / L->grp, KgPad = RoundUp(Kg, 16);
     QCNN_CHECK(cap >= static_cast<size_t>(taps) * L->S * L->Cout, "qcnn_layer_read_asmt_h: buffer too small");
@@ -418,10 +390,9 @@ int qcnn_fc_aprx_forward(qcnn_layer* L, const float* src, int N, float* dst, int
 int qcnn_fc_aprx_forward_flat(qcnn_layer* L, const float* src, int N, float* dst, int fuse_relu, void* stream) {
   QCNN_CHECK(L && src && dst, "qcnn_fc_aprx_forward_flat: NULL argument");
   QCNN_ON_DEVICE(L->ctx->device);
-  int* saved = L->d_srcoff;
-  L->d_srcoff = nullptr;
+  DeviceBuffer saved = std::move(L->d_srcoff);   // every FC path sees no offset table while the source is flat
   const int rc = LaunchFc(L, src, N, dst, fuse_relu, static_cast<cudaStream_t>(stream));
-  L->d_srcoff = saved;
+  L->d_srcoff = std::move(saved);
   return rc;
 }
 

@@ -66,6 +66,74 @@ struct qcnn_ctx {
   unsigned long long alloc_epoch;  // bumped whenever a device scratch buffer is (re)allocated: captured graphs go stale
 };
 
+namespace qcnn {
+
+// The one owner of every device allocation the library makes for itself (layer parameters, scratch, executor staging).
+// Invariant: bytes() > 0 if and only if get() owns that many bytes on device().  Freed on destruction.
+class DeviceBuffer {
+ public:
+  DeviceBuffer() = default;
+  ~DeviceBuffer() { Release(); }
+  DeviceBuffer(DeviceBuffer&& o) noexcept : ptr_(o.ptr_), bytes_(o.bytes_), device_(o.device_) { o.ptr_ = nullptr; o.bytes_ = 0; }
+  DeviceBuffer& operator=(DeviceBuffer&& o) noexcept {
+    if (this != &o) {
+      Release();
+      ptr_ = o.ptr_; bytes_ = o.bytes_; device_ = o.device_;
+      o.ptr_ = nullptr; o.bytes_ = 0;
+    }
+    return *this;
+  }
+  DeviceBuffer(const DeviceBuffer&) = delete;
+  DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+
+  // Grow-only: makes the buffer hold at least `bytes` on ctx's device (the contents do not survive a growth).  A real
+  // (re)allocation bumps ctx->alloc_epoch, since graphs captured before hold the old address, and sets *grown for
+  // first-use initialisation.  Refused with cudaErrorStreamCaptureUnsupported while `st` is being captured.
+  cudaError_t Reserve(qcnn_ctx* ctx, size_t bytes, cudaStream_t st = nullptr, bool* grown = nullptr) {
+    if (grown) *grown = false;
+    if (bytes <= bytes_) return cudaSuccess;
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    if (st) cudaStreamIsCapturing(st, &cap);
+    if (cap != cudaStreamCaptureStatusNone) return cudaErrorStreamCaptureUnsupported;
+    if (cudaError_t e = Release()) return e;
+    DeviceGuard guard(ctx->device);
+    if (guard.error()) return guard.error();
+    if (cudaError_t e = cudaMalloc(&ptr_, bytes)) { ptr_ = nullptr; return e; }
+    bytes_ = bytes;
+    device_ = ctx->device;
+    ctx->alloc_epoch++;
+    if (grown) *grown = true;
+    return cudaSuccess;
+  }
+  // Immutable contents: exactly `bytes` copied from the host.
+  cudaError_t Upload(qcnn_ctx* ctx, const void* host, size_t bytes) {
+    if (cudaError_t e = Release()) return e;
+    if (cudaError_t e = Reserve(ctx, bytes)) return e;
+    DeviceGuard guard(device_);
+    return cudaMemcpy(ptr_, host, bytes, cudaMemcpyHostToDevice);
+  }
+  cudaError_t Release() {
+    cudaError_t e = cudaSuccess;
+    if (ptr_) {
+      DeviceGuard guard(device_);
+      e = guard.error() ? guard.error() : cudaFree(ptr_);
+    }
+    ptr_ = nullptr;
+    bytes_ = 0;
+    return e;
+  }
+  void* get() const { return ptr_; }
+  template <class T> T* as() const { return static_cast<T*>(ptr_); }
+  size_t bytes() const { return bytes_; }
+
+ private:
+  void* ptr_ = nullptr;
+  size_t bytes_ = 0;
+  int device_ = 0;
+};
+
+}  // namespace qcnn
+
 enum { QCNN_KIND_CONV = 0, QCNN_KIND_FC = 1 };
 
 // ---- kernel argument blocks --------------------------------------------------------------------------------
@@ -170,49 +238,45 @@ struct ConvPlan {
 };
 
 struct qcnn_layer {
-  qcnn_ctx* ctx;
-  int kind;
+  qcnn_ctx* ctx = nullptr;
+  int kind = 0;
   // geometry
-  int Cin, Hin, Win, Cout, ksz, pad, stride, grp, S, K, d;
-  int Ho, Wo;
-  int Din, Dout, DoutPad;
+  int Cin = 0, Hin = 0, Win = 0, Cout = 0, ksz = 0, pad = 0, stride = 0, grp = 0, S = 0, K = 0, d = 0;
+  int Ho = 0, Wo = 0;
+  int Din = 0, Dout = 0, DoutPad = 0;
   // FC source permutation (NHWC map) / conv NCHW source
-  int src_h, src_w, src_c;
-  int* d_srcoff;        // FC: NCHW-flatten index -> NHWC element offset (NULL when the source is flat)
-  int src_nchw;
+  int src_h = 0, src_w = 0, src_c = 0;
+  qcnn::DeviceBuffer d_srcoff;  // FC: int [Din], NCHW-flatten index -> NHWC element offset (empty when the source is flat)
+  int src_nchw = 0;
   // device parameters
-  float* d_ctrd;
-  uint8_t* d_asmt;
-  int asmt_t_mode;        // layout of d_asmt_t: 0 = [grp][S][KgPad][tapsPad] (stride 1), 1 = [grp][stride phase rows][KgPad][rowsPad] (strided, S = 1)
-  uint8_t* d_asmt_t;      // conv layers: the same indices as [grp][S][KgPad][tapsPad] (tapsPad = taps rounded up to 16): a decoder thread
-                          // (= channel) reads all taps of a chunk with one or two 128-bit loads (pq_gemm_tc.cu, mode 0)
-  float* d_bias;
-  size_t asmt_bytes;
-  int kshift;           // FC: stored assignment = idx << kshift
+  qcnn::DeviceBuffer d_ctrd;    // float
+  qcnn::DeviceBuffer d_asmt;    // uint8_t
+  int asmt_t_mode = 0;    // layout of d_asmt_t: 0 = [grp][S][KgPad][tapsPad] (stride 1), 1 = [grp][stride phase rows][KgPad][rowsPad] (strided, S = 1)
+  qcnn::DeviceBuffer d_asmt_t;  // conv layers: the same indices as [grp][S][KgPad][tapsPad] (tapsPad = taps rounded up to 16): a decoder thread
+                                // (= channel) reads all taps of a chunk with one or two 128-bit loads (pq_gemm_tc.cu, mode 0)
+  qcnn::DeviceBuffer d_bias;    // float
+  int kshift = 0;       // FC: stored assignment = idx << kshift
   // plans
-  ConvPlan plan;
-  int plan_N;            // batch size the cached plan was made for (0 = none)
-  int tuned;             // the plan for plan_N was confirmed by on-device timing
-  std::vector<ConvPlan>* cands;  // the model's best tilings for plan_N (autotune candidates)
-  std::vector<std::pair<int, ConvPlan>>* tunedPlans;  // timed winners per batch size
+  ConvPlan plan{};
+  int plan_N = 0;        // batch size the cached plan was made for (0 = none)
+  int tuned = 0;         // the plan for plan_N was confirmed by on-device timing
+  std::vector<ConvPlan> cands;  // the model's best tilings for plan_N (autotune candidates)
+  std::vector<std::pair<int, ConvPlan>> tunedPlans;  // timed winners per batch size
   // FC scratch
-  float* d_partial;
-  size_t partial_bytes;
-  float* d_flat;         // tensor-core FC path: source pre-split into hi/lo plane images (fc_prep_kernel)
-  size_t flat_bytes;
-  void* d_ctrd_bf;        // codebook pre-split into bf16 pieces (pq_gemm_tc.cu, bf16x2 operands): [S][d/4 pieces][K] x {w1 (4 x bf16), w2 (4 x bf16)}: a (subspace, piece) slice is contiguous
-  float* d_cpart;        // chain kernel (fc_chain.cu): per-CTA partial sums [sm_count][DoutPad], words double as ready flags
-  size_t cpart_bytes;
+  qcnn::DeviceBuffer d_partial;  // float
+  qcnn::DeviceBuffer d_flat;     // tensor-core FC path: source pre-split into hi/lo plane images (fc_prep_kernel)
+  qcnn::DeviceBuffer d_ctrd_bf;  // codebook pre-split into bf16 pieces (pq_gemm_tc.cu, bf16x2 operands): [S][d/4 pieces][K] x {w1 (4 x bf16), w2 (4 x bf16)}: a (subspace, piece) slice is contiguous
+  qcnn::DeviceBuffer d_cpart;    // chain kernel (fc_chain.cu): per-CTA partial sums [sm_count][DoutPad], words double as ready flags
   // tuning overrides (0 = automatic)
-  int opt_fc_nsplit;
-  int opt_fc_tn;
-  int opt_no_tc;         // 1: never use the decode-at-use tensor-core kernels for this layer
-  int opt_tc_bf;         // 1: the tensor-core kernels take bf16x2 operands (tensor_core = 2) instead of 3xTF32
-  int opt_force_kernel;  // conv: 1 + kernel id the plan is restricted to (0 = none); tests pin the kernel they check
-  int opt_no_autotune;   // conv: 1 = keep the cost model's first tiling (no on-device timing)
-  int opt_gemm_nt;       // conv: restrict pq_gemm_tc tilings to this many positions per CTA (0 = any)
-  int opt_gemm_gt;       // conv: ... to this many k-steps per stage (0 = any)
-  int opt_gemm_nsplit;   // conv: ... to this K-split factor (0 = any)
+  int opt_fc_nsplit = 0;
+  int opt_fc_tn = 0;
+  int opt_no_tc = 0;         // 1: never use the decode-at-use tensor-core kernels for this layer
+  int opt_tc_bf = 0;         // 1: the tensor-core kernels take bf16x2 operands (tensor_core = 2) instead of 3xTF32
+  int opt_force_kernel = 0;  // conv: 1 + kernel id the plan is restricted to (0 = none); tests pin the kernel they check
+  int opt_no_autotune = 0;   // conv: 1 = keep the cost model's first tiling (no on-device timing)
+  int opt_gemm_nt = 0;       // conv: restrict pq_gemm_tc tilings to this many positions per CTA (0 = any)
+  int opt_gemm_gt = 0;       // conv: ... to this many k-steps per stage (0 = any)
+  int opt_gemm_nsplit = 0;   // conv: ... to this K-split factor (0 = any)
 };
 
 namespace qcnn {

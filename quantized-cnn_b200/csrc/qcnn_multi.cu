@@ -80,11 +80,9 @@ struct qcnn_multi {
   std::vector<NcclComm> comm;
   std::vector<cudaStream_t> stComp, stGath;
   std::vector<cudaEvent_t> evFwd[2], evGath[2];   // per buffer set: forward of the shard done / gather done
-  std::vector<float*> dImg;                       // host-buffer entry: device copy of the rank's image shard
-  std::vector<float*> dShard[2];                  // [per][out] probabilities of the rank's shard (two sets)
-  std::vector<float*> dAll[2];                    // [R * per][out] gathered probabilities (two sets)
-  size_t capPer;                                  // rows the shard / gather buffers hold per rank
-  size_t capImg;                                  // images dImg holds per rank
+  std::vector<DeviceBuffer> dImg;                 // host-buffer entry: device copy of the rank's image shard
+  std::vector<DeviceBuffer> dShard[2];            // [per][out] probabilities of the rank's shard (two sets)
+  std::vector<DeviceBuffer> dAll[2];              // [R * per][out] gathered probabilities (two sets)
   unsigned long long step;
   NcclApi* nccl;
   int outLen, imgLen;
@@ -96,28 +94,18 @@ static int NcclFail(qcnn_multi* m, int rc, const char* what) {
 }
 
 static int EnsureMultiCapacity(qcnn_multi* m, int per, bool needImg) {
-  if (static_cast<size_t>(per) > m->capPer) {
-    for (int r = 0; r < m->R; r++) {
-      QCNN_CUDA(cudaSetDevice(m->dev[r]));
-      for (int b = 0; b < 2; b++) {
-        if (m->dShard[b][r]) QCNN_CUDA(cudaFree(m->dShard[b][r]));
-        if (m->dAll[b][r]) QCNN_CUDA(cudaFree(m->dAll[b][r]));
-        m->dShard[b][r] = m->dAll[b][r] = nullptr;
-        QCNN_CUDA(cudaMalloc(&m->dShard[b][r], sizeof(float) * per * m->outLen));
-        QCNN_CUDA(cudaMalloc(&m->dAll[b][r], sizeof(float) * static_cast<size_t>(m->R) * per * m->outLen));
-        QCNN_CUDA(cudaMemset(m->dShard[b][r], 0, sizeof(float) * per * m->outLen));
+  const size_t shard = sizeof(float) * static_cast<size_t>(per) * m->outLen;
+  for (int r = 0; r < m->R; r++) {
+    for (int b = 0; b < 2; b++) {
+      bool grown = false;
+      QCNN_CUDA(m->dShard[b][r].Reserve(m->ctx[r], shard, nullptr, &grown));
+      if (grown) {
+        QCNN_ON_DEVICE(m->dev[r]);
+        QCNN_CUDA(cudaMemset(m->dShard[b][r].get(), 0, shard));
       }
+      QCNN_CUDA(m->dAll[b][r].Reserve(m->ctx[r], m->R * shard));
     }
-    m->capPer = per;
-  }
-  if (needImg && static_cast<size_t>(per) > m->capImg) {
-    for (int r = 0; r < m->R; r++) {
-      QCNN_CUDA(cudaSetDevice(m->dev[r]));
-      if (m->dImg[r]) QCNN_CUDA(cudaFree(m->dImg[r]));
-      m->dImg[r] = nullptr;
-      QCNN_CUDA(cudaMalloc(&m->dImg[r], sizeof(float) * static_cast<size_t>(per) * m->imgLen));
-    }
-    m->capImg = per;
+    if (needImg) QCNN_CUDA(m->dImg[r].Reserve(m->ctx[r], sizeof(float) * static_cast<size_t>(per) * m->imgLen));
   }
   return 0;
 }
@@ -159,10 +147,10 @@ static qcnn_multi* NewMulti(int R, const int* devices) {
   m->stComp.assign(R, nullptr); m->stGath.assign(R, nullptr);
   for (int b = 0; b < 2; b++) {
     m->evFwd[b].assign(R, nullptr); m->evGath[b].assign(R, nullptr);
-    m->dShard[b].assign(R, nullptr); m->dAll[b].assign(R, nullptr);
+    m->dShard[b].resize(R); m->dAll[b].resize(R);
   }
-  m->dImg.assign(R, nullptr);
-  m->capPer = 0; m->capImg = 0; m->step = 0; m->nccl = nullptr; m->outLen = 0; m->imgLen = 0;
+  m->dImg.resize(R);
+  m->step = 0; m->nccl = nullptr; m->outLen = 0; m->imgLen = 0;
   return m;
 }
 
@@ -182,12 +170,9 @@ void qcnn_multi_destroy(qcnn_multi* m) {
     cudaSetDevice(m->dev[r]);
     if (m->comm[r] && m->nccl) m->nccl->CommDestroy(m->comm[r]);
     for (int b = 0; b < 2; b++) {
-      if (m->dShard[b][r]) cudaFree(m->dShard[b][r]);
-      if (m->dAll[b][r]) cudaFree(m->dAll[b][r]);
       if (m->evFwd[b][r]) cudaEventDestroy(m->evFwd[b][r]);
       if (m->evGath[b][r]) cudaEventDestroy(m->evGath[b][r]);
     }
-    if (m->dImg[r]) cudaFree(m->dImg[r]);
     if (m->stComp[r]) cudaStreamDestroy(m->stComp[r]);
     if (m->stGath[r]) cudaStreamDestroy(m->stGath[r]);
     if (m->net[r]) qcnn_net_destroy(m->net[r]);
@@ -263,7 +248,7 @@ int qcnn_multi_forward(qcnn_multi* m, const float* const* img_dev, int N, const 
     if (m->step >= 2) QCNN_CUDA(cudaStreamWaitEvent(m->stComp[r], m->evGath[b][r], 0));
     if (hi > lo) {
       QCNN_CHECK(img_dev[r] != nullptr, "qcnn_multi_forward: img_dev[%d] is NULL", r);
-      if (int rc = qcnn_net_forward(m->net[r], img_dev[r], hi - lo, m->dShard[b][r], nullptr, m->stComp[r])) return rc;
+      if (int rc = qcnn_net_forward(m->net[r], img_dev[r], hi - lo, m->dShard[b][r].as<float>(), nullptr, m->stComp[r])) return rc;
     }
     QCNN_CUDA(cudaEventRecord(m->evFwd[b][r], m->stComp[r]));
     QCNN_CUDA(cudaStreamWaitEvent(m->stGath[r], m->evFwd[b][r], 0));
@@ -272,8 +257,8 @@ int qcnn_multi_forward(qcnn_multi* m, const float* const* img_dev, int N, const 
   int rc = m->nccl->GroupStart();
   if (rc != 0) return NcclFail(m, rc, "ncclGroupStart");
   for (int r = 0; r < m->R; r++) {
-    rc = m->nccl->AllGather(m->dShard[b][r], m->dAll[b][r], static_cast<size_t>(per) * m->outLen, 7 /* ncclFloat32 */, m->comm[r],
-                            m->stGath[r]);
+    rc = m->nccl->AllGather(m->dShard[b][r].get(), m->dAll[b][r].get(), static_cast<size_t>(per) * m->outLen, 7 /* ncclFloat32 */,
+                            m->comm[r], m->stGath[r]);
     if (rc != 0) { m->nccl->GroupEnd(); return NcclFail(m, rc, "ncclAllGather"); }
   }
   rc = m->nccl->GroupEnd();
@@ -281,7 +266,7 @@ int qcnn_multi_forward(qcnn_multi* m, const float* const* img_dev, int N, const 
   for (int r = 0; r < m->R; r++) {
     QCNN_CUDA(cudaSetDevice(m->dev[r]));
     QCNN_CUDA(cudaEventRecord(m->evGath[b][r], m->stGath[r]));
-    if (prob_all_dev) prob_all_dev[r] = m->dAll[b][r];
+    if (prob_all_dev) prob_all_dev[r] = m->dAll[b][r].as<float>();
   }
   m->step++;
   return 0;
@@ -312,9 +297,9 @@ int qcnn_multi_forward_h(qcnn_multi* m, const float* img_h, int N, float* prob_h
     ShardRange(N, m->R, r, &per, &lo, &hi);
     QCNN_CUDA(cudaSetDevice(m->dev[r]));
     if (hi > lo)
-      QCNN_CUDA(cudaMemcpyAsync(m->dImg[r], img_h + static_cast<size_t>(lo) * m->imgLen, sizeof(float) * (hi - lo) * m->imgLen,
+      QCNN_CUDA(cudaMemcpyAsync(m->dImg[r].get(), img_h + static_cast<size_t>(lo) * m->imgLen, sizeof(float) * (hi - lo) * m->imgLen,
                                 cudaMemcpyHostToDevice, m->stComp[r]));
-    img[r] = m->dImg[r];
+    img[r] = m->dImg[r].as<float>();
   }
   std::vector<const float*> all(m->R, nullptr);
   if (int rc = qcnn_multi_forward(m, img.data(), N, all.data())) return rc;

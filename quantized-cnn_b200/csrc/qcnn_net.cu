@@ -27,41 +27,34 @@ struct NetLayer {
 };
 
 struct qcnn_net {
-  qcnn_ctx* ctx;
+  qcnn_ctx* ctx = nullptr;
   std::vector<NetLayer> layers;
-  int imgC, imgH, imgW;
-  int keep;
-  int profiling;
-  int capN;
-  std::vector<float*> maps;  // device buffers for featMapLst[0..L]; maps[0] only used when the input must be permuted
+  int imgC = 0, imgH = 0, imgW = 0;
+  int keep = 0;
+  int profiling = 0;
+  std::vector<DeviceBuffer> maps;  // featMapLst[0..L] (float); maps[0] only used when the input must be permuted
   std::vector<const float*> mapPtr;  // where featMapLst[i] of the last forward actually lives (NULL if fused away)
   std::vector<cudaEvent_t> evBeg, evEnd;
   std::vector<char> evUsed;
-  unsigned long long lastLaunches;
-  // host-buffer forward: double-buffered input chunks + output staging
-  float* d_in[2];
-  size_t d_in_cap;
+  unsigned long long lastLaunches = 0;
+  // host-buffer forward: double-buffered input chunks (float) + output staging
+  DeviceBuffer d_in[2];
   // uint8 entry points: crop-sized mean image, staging of the uint8 chunks, on-device top-k results
-  float* d_mean;            // [C][H][W] or NULL
-  uint8_t* d_in8[2];
-  size_t d_in8_cap;
-  float* d_f32;             // converted chunk (device-resident uint8 entry)
-  size_t d_f32_cap;
-  int* d_topi;
-  float* d_topv;
-  size_t d_top_cap;
+  DeviceBuffer d_mean;      // float [C][H][W] or empty
+  DeviceBuffer d_in8[2];    // uint8_t
+  DeviceBuffer d_f32;       // converted chunk (device-resident uint8 entry)
+  DeviceBuffer d_topi;      // int
+  DeviceBuffer d_topv;      // float
   // asynchronous host-buffer steps (qcnn_net_submit_u8_h): two input slots so that the copy of step i+1 overlaps step i
-  uint8_t* d_sub8[2];
-  size_t d_sub8_cap;
-  cudaEvent_t evSubIn[2], evSubRead[2], evSubDone[2];
-  int subInit;
-  unsigned long long subCount;
-  float* d_prob;
-  float* d_logit;
-  size_t d_out_cap;
-  cudaStream_t stCopy, stComp;
-  cudaEvent_t evH2D[2], evDone[2];
-  int chunk;
+  DeviceBuffer d_sub8[2];   // uint8_t
+  cudaEvent_t evSubIn[2] = {}, evSubRead[2] = {}, evSubDone[2] = {};
+  int subInit = 0;
+  unsigned long long subCount = 0;
+  DeviceBuffer d_prob;      // float
+  DeviceBuffer d_logit;     // float
+  cudaStream_t stCopy = nullptr, stComp = nullptr;
+  cudaEvent_t evH2D[2] = {}, evDone[2] = {};
+  int chunk = 128;
   // small batches: the launch sequence of a forward pass is captured once per (N, buffers, stream) and replayed
   struct GraphEntry {
     int N; const float* img; float* prob; float* logits; cudaStream_t st;
@@ -74,40 +67,17 @@ struct qcnn_net {
   std::vector<GraphEntry> graphs;
 };
 
-static void FreeMaps(qcnn_net* net) {
-  for (float*& p : net->maps) {
-    if (p) cudaFree(p);
-    p = nullptr;
-  }
-  net->capN = 0;
-}
 static size_t MapElems(const NetLayer& L) { return static_cast<size_t>(L.Hout) * L.Wout * L.Cout; }
 
-// Feature-map buffers are allocated on first use at the current batch capacity: the fused production path touches
-// about half of featMapLst (ReLU / LRN / dropout outputs are fused away), so the other half is never allocated unless
-// keep_maps asks for it.  A larger batch frees everything and raises the capacity.
-static int EnsureCapacity(qcnn_net* net, int N) {
-  if (net->maps.empty()) net->maps.assign(net->layers.size() + 1, nullptr);
-  if (N <= net->capN) return 0;
-  FreeMaps(net);
-  net->ctx->alloc_epoch++;
-  net->capN = N;
-  return 0;
-}
-
-static float* MapBuf(qcnn_net* net, int idx, cudaStream_t st) {
-  if (net->maps[idx]) return net->maps[idx];
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (st) cudaStreamIsCapturing(st, &cap);
-  if (cap != cudaStreamCaptureStatusNone) { SetError("internal: feature map %d is not allocated inside a stream capture", idx); return nullptr; }
+// Feature-map buffers are reserved on first use for the batch at hand: the fused production path touches about half of
+// featMapLst (ReLU / LRN / dropout outputs are fused away), so the other half is never allocated unless keep_maps asks
+// for it.
+static float* MapBuf(qcnn_net* net, int idx, int N, cudaStream_t st) {
   const size_t elems = idx == 0 ? static_cast<size_t>(net->imgC) * net->imgH * net->imgW : MapElems(net->layers[idx - 1]);
-  if (cudaMalloc(&net->maps[idx], sizeof(float) * net->capN * elems) != cudaSuccess) {
-    CudaFail(cudaGetLastError(), "cudaMalloc(feature map)", __FILE__, __LINE__);
-    net->maps[idx] = nullptr;
-    return nullptr;
-  }
-  net->ctx->alloc_epoch++;
-  return net->maps[idx];
+  const cudaError_t e = net->maps[idx].Reserve(net->ctx, sizeof(float) * N * elems, st);
+  if (e == cudaErrorStreamCaptureUnsupported) { SetError("internal: feature map %d is not allocated inside a stream capture", idx); return nullptr; }
+  if (e) { CudaFail(e, "feature map reservation", __FILE__, __LINE__); return nullptr; }
+  return net->maps[idx].as<float>();
 }
 
 static int BuildNet(qcnn_ctx* ctx, int layerCnt, const qcnn_layer_info* infos, const qcnn_layer_para* paras, int imgC, int imgH,
@@ -115,14 +85,6 @@ static int BuildNet(qcnn_ctx* ctx, int layerCnt, const qcnn_layer_info* infos, c
   qcnn_net* net = new qcnn_net();
   net->ctx = ctx;
   net->imgC = imgC; net->imgH = imgH; net->imgW = imgW;
-  net->keep = 0; net->profiling = 0; net->capN = 0; net->lastLaunches = 0;
-  net->d_in[0] = net->d_in[1] = nullptr; net->d_in_cap = 0;
-  net->d_mean = nullptr; net->d_in8[0] = net->d_in8[1] = nullptr; net->d_in8_cap = 0; net->d_f32 = nullptr; net->d_f32_cap = 0;
-  net->d_topi = nullptr; net->d_topv = nullptr; net->d_top_cap = 0;
-  net->d_sub8[0] = net->d_sub8[1] = nullptr; net->d_sub8_cap = 0; net->subInit = 0; net->subCount = 0;
-  net->d_prob = net->d_logit = nullptr; net->d_out_cap = 0;
-  net->stCopy = net->stComp = nullptr;
-  net->chunk = 128;
   int H = imgH, W = imgW, C = imgC;
   bool seenFc = false;
   int rc = 0;
@@ -180,6 +142,7 @@ static int BuildNet(qcnn_ctx* ctx, int layerCnt, const qcnn_layer_info* infos, c
       net->layers[0].info.stride > 1)
     qcnn_conv_layer_set_src_nchw(net->layers[0].pq, 1);
   const size_t L = net->layers.size();
+  net->maps.resize(L + 1);
   net->mapPtr.assign(L + 1, nullptr);
   net->evBeg.resize(L); net->evEnd.resize(L); net->evUsed.assign(L, 0);
   for (size_t l = 0; l < L; l++) {
@@ -269,26 +232,16 @@ int qcnn_net_create_custom(qcnn_ctx* ctx, int layer_cnt, const qcnn_layer_info* 
 void qcnn_net_destroy(qcnn_net* net) {
   if (!net) return;
   DeviceGuard guard(net->ctx->device);
-  FreeMaps(net);
   for (NetLayer& L : net->layers) qcnn_layer_destroy(L.pq);
   for (size_t l = 0; l < net->evBeg.size(); l++) {
     cudaEventDestroy(net->evBeg[l]);
     cudaEventDestroy(net->evEnd[l]);
   }
-  if (net->d_mean) cudaFree(net->d_mean);
-  if (net->d_f32) cudaFree(net->d_f32);
-  if (net->d_topi) cudaFree(net->d_topi);
-  if (net->d_topv) cudaFree(net->d_topv);
   for (int i = 0; i < 2; i++) {
-    if (net->d_sub8[i]) cudaFree(net->d_sub8[i]);
     if (net->subInit) { cudaEventDestroy(net->evSubIn[i]); cudaEventDestroy(net->evSubRead[i]); cudaEventDestroy(net->evSubDone[i]); }
-    if (net->d_in8[i]) cudaFree(net->d_in8[i]);
-    if (net->d_in[i]) cudaFree(net->d_in[i]);
     if (net->stCopy) { cudaEventDestroy(net->evH2D[i]); cudaEventDestroy(net->evDone[i]); }
   }
   for (qcnn_net::GraphEntry& g : net->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-  if (net->d_prob) cudaFree(net->d_prob);
-  if (net->d_logit) cudaFree(net->d_logit);
   if (net->stCopy) cudaStreamDestroy(net->stCopy);
   if (net->stComp) cudaStreamDestroy(net->stComp);
   delete net;
@@ -395,7 +348,6 @@ int qcnn_net_forward(qcnn_net* net, const float* img, int N, float* prob, float*
 
 static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, float* logits, cudaStream_t st) {
   qcnn_ctx* ctx = net->ctx;
-  if (int rc = EnsureCapacity(net, N)) return rc;
   const int L = static_cast<int>(net->layers.size());
   const unsigned long long launches0 = ctx->launches;
   std::fill(net->mapPtr.begin(), net->mapPtr.end(), nullptr);
@@ -410,16 +362,16 @@ static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, flo
   } else {
     if (firstReadsNchw) {
       cur = img;  // conv still reads the NCHW input; also materialise the NHWC map for inspection
-      float* m0 = MapBuf(net, 0, st);
+      float* m0 = MapBuf(net, 0, N, st);
       if (!m0) return 2;
       if (int rc = LaunchNchwToNhwc(ctx, img, m0, N, net->imgC, net->imgH, net->imgW, st)) return rc;
     } else {
-      float* m0 = MapBuf(net, 0, st);
+      float* m0 = MapBuf(net, 0, N, st);
       if (!m0) return 2;
       if (int rc = LaunchNchwToNhwc(ctx, img, m0, N, net->imgC, net->imgH, net->imgW, st)) return rc;
       cur = m0;
     }
-    net->mapPtr[0] = net->maps[0];
+    net->mapPtr[0] = net->maps[0].as<float>();
   }
 
   int l = 0;
@@ -451,7 +403,7 @@ static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, flo
           }
           if (n >= 1 && FcChainEligible(ctx, chain, crelu, n, N)) {
             bool handled = false;
-            float* dst = MapBuf(net, outIdx, st);
+            float* dst = MapBuf(net, outIdx, N, st);
         if (!dst) return 2;
             rc = LaunchFcChain(ctx, chain, crelu, n, cur, N, dst, st, nullptr, &handled);
             if (rc) break;
@@ -465,7 +417,7 @@ static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, flo
         }
         const bool fuse = !net->keep && l + 1 < L && net->layers[l + 1].info.type == QCNN_RELU;
         const int outIdx = fuse ? l + 2 : l + 1;
-        float* dst = MapBuf(net, outIdx, st);
+        float* dst = MapBuf(net, outIdx, N, st);
         if (!dst) return 2;
         if (type == QCNN_CONV) rc = LaunchConv(nl.pq, cur, N, dst, fuse ? 1 : 0, st);
         else rc = LaunchFc(nl.pq, cur, N, dst, fuse ? 1 : 0, st);
@@ -475,7 +427,7 @@ static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, flo
         break;
       }
       case QCNN_RELU: {
-        float* dst = MapBuf(net, l + 1, st);
+        float* dst = MapBuf(net, l + 1, N, st);
         if (!dst) return 2;
         rc = LaunchRelu(ctx, cur, dst, static_cast<size_t>(N) * MapElems(nl), st);
         net->mapPtr[l + 1] = dst; cur = dst; l++;
@@ -485,13 +437,13 @@ static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, flo
         const bool fuse = !net->keep && l + 1 < L && net->layers[l + 1].info.type == QCNN_POOL;
         if (fuse) {
           const NetLayer& pl = net->layers[l + 1];
-          float* dst = MapBuf(net, l + 2, st);
+          float* dst = MapBuf(net, l + 2, N, st);
         if (!dst) return 2;
           rc = LaunchLrnMaxPool(ctx, cur, dst, N, nl.Hin, nl.Win, nl.Cin, nl.info.lrnSiz, nl.info.lrnAlp,
                                 nl.info.lrnBet, nl.info.lrnIni, pl.info.knlSiz, pl.info.padSiz, pl.info.stride, st);
           net->mapPtr[l + 2] = dst; cur = dst; l += 2;
         } else {
-          float* dst = MapBuf(net, l + 1, st);
+          float* dst = MapBuf(net, l + 1, N, st);
         if (!dst) return 2;
           rc = LaunchLrn(ctx, cur, dst, static_cast<size_t>(N) * nl.Hin * nl.Win, nl.Cin, nl.info.lrnSiz,
                          nl.info.lrnAlp, nl.info.lrnBet, nl.info.lrnIni, st);
@@ -500,7 +452,7 @@ static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, flo
         break;
       }
       case QCNN_POOL: {
-        float* dst = MapBuf(net, l + 1, st);
+        float* dst = MapBuf(net, l + 1, N, st);
         if (!dst) return 2;
         rc = LaunchMaxPool(ctx, cur, dst, N, nl.Hin, nl.Win, nl.Cin, nl.info.knlSiz, nl.info.padSiz, nl.info.stride, st);
         net->mapPtr[l + 1] = dst; cur = dst; l++;
@@ -508,7 +460,7 @@ static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, flo
       }
       case QCNN_DRPT: {
         if (net->keep) {
-          float* dst = MapBuf(net, l + 1, st);
+          float* dst = MapBuf(net, l + 1, N, st);
         if (!dst) return 2;
           QCNN_CUDA(cudaMemcpyAsync(dst, cur, sizeof(float) * N * MapElems(nl), cudaMemcpyDeviceToDevice, st));
           net->mapPtr[l + 1] = dst; cur = dst;
@@ -521,7 +473,7 @@ static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, flo
       case QCNN_SMAX: {
         if (logits && lastLayer)
           QCNN_CUDA(cudaMemcpyAsync(logits, cur, sizeof(float) * N * MapElems(nl), cudaMemcpyDeviceToDevice, st));
-        float* dst = lastLayer ? prob : MapBuf(net, l + 1, st);
+        float* dst = lastLayer ? prob : MapBuf(net, l + 1, N, st);
         if (!dst) return 2;
         rc = LaunchSoftmax(ctx, cur, dst, N, nl.Hout * nl.Wout * nl.Cout, st);
         net->mapPtr[l + 1] = dst; cur = dst; l++;
@@ -546,6 +498,28 @@ static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, flo
   return 0;
 }
 
+// The copy and compute streams of the host-buffer pipelines and their events, created on first use
+static int CreatePipeline(qcnn_net* net) {
+  if (net->stCopy) return 0;
+  QCNN_CUDA(cudaStreamCreateWithFlags(&net->stCopy, cudaStreamNonBlocking));
+  QCNN_CUDA(cudaStreamCreateWithFlags(&net->stComp, cudaStreamNonBlocking));
+  for (int i = 0; i < 2; i++) {
+    QCNN_CUDA(cudaEventCreateWithFlags(&net->evH2D[i], cudaEventDisableTiming));
+    QCNN_CUDA(cudaEventCreateWithFlags(&net->evDone[i], cudaEventDisableTiming));
+  }
+  return 0;
+}
+
+// Device-side results of a host-buffer call for N images: probabilities, logits and (topk > 0) the top-k pairs
+static int ReserveOutputs(qcnn_net* net, int N, int topk) {
+  const size_t out = sizeof(float) * static_cast<size_t>(N) * qcnn_net_out_len(net), top = static_cast<size_t>(N) * topk;
+  QCNN_CUDA(net->d_prob.Reserve(net->ctx, out));
+  QCNN_CUDA(net->d_logit.Reserve(net->ctx, out));
+  QCNN_CUDA(net->d_topi.Reserve(net->ctx, sizeof(int) * top));
+  QCNN_CUDA(net->d_topv.Reserve(net->ctx, sizeof(float) * top));
+  return 0;
+}
+
 // Host-buffer forward pass: a pipeline of chunks on two streams -- H2D of chunk c+1 (copy stream) overlaps the layers of
 // chunk c (compute stream).  Images arrive as fp32 NCHW (ExecForwardPass's own input) or as uint8 HWC pixels that are
 // converted (and mean-subtracted) on the device: 4x fewer bytes over the host link.  With topk > 0 the k-fold arg-max runs
@@ -553,51 +527,14 @@ static int ForwardEager(qcnn_net* net, const float* img, int N, float* prob, flo
 static int ForwardHost(qcnn_net* net, const float* img_h, const uint8_t* img8_h, int N, float* prob_h, float* logits_h, int topk,
                        int topk_mode, int* topi_h, float* topv_h) {
   QCNN_ON_DEVICE(net->ctx->device);
-  if (!net->stCopy) {
-    QCNN_CUDA(cudaStreamCreateWithFlags(&net->stCopy, cudaStreamNonBlocking));
-    QCNN_CUDA(cudaStreamCreateWithFlags(&net->stComp, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; i++) {
-      QCNN_CUDA(cudaEventCreateWithFlags(&net->evH2D[i], cudaEventDisableTiming));
-      QCNN_CUDA(cudaEventCreateWithFlags(&net->evDone[i], cudaEventDisableTiming));
-    }
-  }
+  if (int rc = CreatePipeline(net)) return rc;
   const size_t imgLen = static_cast<size_t>(net->imgC) * net->imgH * net->imgW;
   const int outLen = qcnn_net_out_len(net);
   const int chunk = std::min(N, net->chunk);
-  if (static_cast<size_t>(chunk) > net->d_in_cap) {
-    for (int i = 0; i < 2; i++) {
-      if (net->d_in[i]) QCNN_CUDA(cudaFree(net->d_in[i]));
-      net->d_in[i] = nullptr;
-      QCNN_CUDA(cudaMalloc(&net->d_in[i], sizeof(float) * chunk * imgLen));
-    }
-    net->d_in_cap = chunk;
-    net->ctx->alloc_epoch++;
-  }
-  if (img8_h && static_cast<size_t>(chunk) > net->d_in8_cap) {
-    for (int i = 0; i < 2; i++) {
-      if (net->d_in8[i]) QCNN_CUDA(cudaFree(net->d_in8[i]));
-      net->d_in8[i] = nullptr;
-      QCNN_CUDA(cudaMalloc(&net->d_in8[i], chunk * imgLen));
-    }
-    net->d_in8_cap = chunk;
-  }
-  if (static_cast<size_t>(N) > net->d_out_cap) {
-    if (net->d_prob) QCNN_CUDA(cudaFree(net->d_prob));
-    if (net->d_logit) QCNN_CUDA(cudaFree(net->d_logit));
-    net->d_prob = net->d_logit = nullptr;
-    QCNN_CUDA(cudaMalloc(&net->d_prob, sizeof(float) * N * outLen));
-    QCNN_CUDA(cudaMalloc(&net->d_logit, sizeof(float) * N * outLen));
-    net->d_out_cap = N;
-    net->ctx->alloc_epoch++;
-  }
-  if (topk > 0 && static_cast<size_t>(N) * topk > net->d_top_cap) {
-    if (net->d_topi) QCNN_CUDA(cudaFree(net->d_topi));
-    if (net->d_topv) QCNN_CUDA(cudaFree(net->d_topv));
-    net->d_topi = nullptr; net->d_topv = nullptr;
-    QCNN_CUDA(cudaMalloc(&net->d_topi, sizeof(int) * N * topk));
-    QCNN_CUDA(cudaMalloc(&net->d_topv, sizeof(float) * N * topk));
-    net->d_top_cap = static_cast<size_t>(N) * topk;
-  }
+  for (DeviceBuffer& b : net->d_in) QCNN_CUDA(b.Reserve(net->ctx, sizeof(float) * chunk * imgLen));
+  if (img8_h)
+    for (DeviceBuffer& b : net->d_in8) QCNN_CUDA(b.Reserve(net->ctx, chunk * imgLen));
+  if (int rc = ReserveOutputs(net, N, topk)) return rc;
   unsigned long long launches = 0;
   int ci = 0;
   // the first chunk is a quarter of the others: its host-to-device copy is the only one nothing overlaps
@@ -607,31 +544,35 @@ static int ForwardHost(qcnn_net* net, const float* img_h, const uint8_t* img8_h,
     const int b = ci & 1;
     if (ci >= 2) QCNN_CUDA(cudaStreamWaitEvent(net->stCopy, net->evDone[b], 0));
     if (img8_h)
-      QCNN_CUDA(cudaMemcpyAsync(net->d_in8[b], img8_h + n0 * imgLen, cn * imgLen, cudaMemcpyHostToDevice, net->stCopy));
+      QCNN_CUDA(cudaMemcpyAsync(net->d_in8[b].get(), img8_h + n0 * imgLen, cn * imgLen, cudaMemcpyHostToDevice, net->stCopy));
     else
-      QCNN_CUDA(cudaMemcpyAsync(net->d_in[b], img_h + n0 * imgLen, sizeof(float) * cn * imgLen, cudaMemcpyHostToDevice, net->stCopy));
+      QCNN_CUDA(cudaMemcpyAsync(net->d_in[b].get(), img_h + n0 * imgLen, sizeof(float) * cn * imgLen, cudaMemcpyHostToDevice, net->stCopy));
     QCNN_CUDA(cudaEventRecord(net->evH2D[b], net->stCopy));
     QCNN_CUDA(cudaStreamWaitEvent(net->stComp, net->evH2D[b], 0));
     if (img8_h) {
-      if (int rc = LaunchU8ToF32(net->ctx, net->d_in8[b], net->d_mean, net->d_in[b], cn, net->imgC, net->imgH * net->imgW, net->stComp)) return rc;
+      if (int rc = LaunchU8ToF32(net->ctx, net->d_in8[b].as<uint8_t>(), net->d_mean.as<float>(), net->d_in[b].as<float>(), cn,
+                                 net->imgC, net->imgH * net->imgW, net->stComp))
+        return rc;
       launches++;
     }
-    if (int rc = qcnn_net_forward(net, net->d_in[b], cn, net->d_prob + static_cast<size_t>(n0) * outLen,
-                                  logits_h ? net->d_logit + static_cast<size_t>(n0) * outLen : nullptr, net->stComp))
+    if (int rc = qcnn_net_forward(net, net->d_in[b].as<float>(), cn, net->d_prob.as<float>() + static_cast<size_t>(n0) * outLen,
+                                  logits_h ? net->d_logit.as<float>() + static_cast<size_t>(n0) * outLen : nullptr, net->stComp))
       return rc;
     launches += net->lastLaunches;
     QCNN_CUDA(cudaEventRecord(net->evDone[b], net->stComp));
     n0 += cn;
   }
   if (topk > 0) {
-    if (int rc = LaunchTopK(net->ctx, net->d_prob, N, outLen, topk, topk_mode, net->d_topi, net->d_topv, net->stComp)) return rc;
+    if (int rc = LaunchTopK(net->ctx, net->d_prob.as<float>(), N, outLen, topk, topk_mode, net->d_topi.as<int>(), net->d_topv.as<float>(),
+                            net->stComp))
+      return rc;
     launches++;
-    QCNN_CUDA(cudaMemcpyAsync(topi_h, net->d_topi, sizeof(int) * N * topk, cudaMemcpyDeviceToHost, net->stComp));
-    QCNN_CUDA(cudaMemcpyAsync(topv_h, net->d_topv, sizeof(float) * N * topk, cudaMemcpyDeviceToHost, net->stComp));
+    QCNN_CUDA(cudaMemcpyAsync(topi_h, net->d_topi.get(), sizeof(int) * N * topk, cudaMemcpyDeviceToHost, net->stComp));
+    QCNN_CUDA(cudaMemcpyAsync(topv_h, net->d_topv.get(), sizeof(float) * N * topk, cudaMemcpyDeviceToHost, net->stComp));
   }
-  if (prob_h) QCNN_CUDA(cudaMemcpyAsync(prob_h, net->d_prob, sizeof(float) * N * outLen, cudaMemcpyDeviceToHost, net->stComp));
+  if (prob_h) QCNN_CUDA(cudaMemcpyAsync(prob_h, net->d_prob.get(), sizeof(float) * N * outLen, cudaMemcpyDeviceToHost, net->stComp));
   if (logits_h)
-    QCNN_CUDA(cudaMemcpyAsync(logits_h, net->d_logit, sizeof(float) * N * outLen, cudaMemcpyDeviceToHost, net->stComp));
+    QCNN_CUDA(cudaMemcpyAsync(logits_h, net->d_logit.get(), sizeof(float) * N * outLen, cudaMemcpyDeviceToHost, net->stComp));
   QCNN_CUDA(cudaStreamSynchronize(net->stComp));
   net->lastLaunches = launches;
   return 0;
@@ -653,11 +594,11 @@ int qcnn_net_forward_topk_h(qcnn_net* net, const float* img_h, int N, int topk, 
 int qcnn_net_set_input_mean(qcnn_net* net, const float* mean_h) {
   QCNN_CHECK(net, "qcnn_net_set_input_mean: NULL net");
   QCNN_ON_DEVICE(net->ctx->device);
-  if (net->d_mean) { QCNN_CUDA(cudaFree(net->d_mean)); net->d_mean = nullptr; }
-  if (!mean_h) return 0;
-  const size_t bytes = sizeof(float) * net->imgC * net->imgH * net->imgW;
-  QCNN_CUDA(cudaMalloc(&net->d_mean, bytes));
-  QCNN_CUDA(cudaMemcpy(net->d_mean, mean_h, bytes, cudaMemcpyHostToDevice));
+  if (!mean_h) {
+    QCNN_CUDA(net->d_mean.Release());
+    return 0;
+  }
+  QCNN_CUDA(net->d_mean.Upload(net->ctx, mean_h, sizeof(float) * net->imgC * net->imgH * net->imgW));
   return 0;
 }
 
@@ -665,16 +606,11 @@ int qcnn_net_forward_u8(qcnn_net* net, const uint8_t* img, int N, float* prob, f
   QCNN_CHECK(net && img && prob && N >= 1, "qcnn_net_forward_u8: bad argument");
   QCNN_ON_DEVICE(net->ctx->device);
   const size_t imgLen = static_cast<size_t>(net->imgC) * net->imgH * net->imgW;
-  if (static_cast<size_t>(N) > net->d_f32_cap) {
-    if (net->d_f32) QCNN_CUDA(cudaFree(net->d_f32));
-    net->d_f32 = nullptr; net->d_f32_cap = 0;
-    QCNN_CUDA(cudaMalloc(&net->d_f32, sizeof(float) * N * imgLen));
-    net->d_f32_cap = N;
-    net->ctx->alloc_epoch++;
-  }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = LaunchU8ToF32(net->ctx, img, net->d_mean, net->d_f32, N, net->imgC, net->imgH * net->imgW, st)) return rc;
-  return qcnn_net_forward(net, net->d_f32, N, prob, logits, st);
+  QCNN_CUDA(net->d_f32.Reserve(net->ctx, sizeof(float) * N * imgLen, st));
+  if (int rc = LaunchU8ToF32(net->ctx, img, net->d_mean.as<float>(), net->d_f32.as<float>(), N, net->imgC, net->imgH * net->imgW, st))
+    return rc;
+  return qcnn_net_forward(net, net->d_f32.as<float>(), N, prob, logits, st);
 }
 
 int qcnn_net_forward_u8_h(qcnn_net* net, const uint8_t* img_h, int N, int topk, int topk_mode, int* topk_idx_h, float* topk_prob_h,
@@ -696,14 +632,7 @@ int qcnn_net_submit_u8_h(qcnn_net* net, const uint8_t* img_h, int N, int topk, i
   QCNN_CHECK(topk == 0 || (topk_idx_h && topk_prob_h), "qcnn_net_submit_u8_h: topk > 0 needs the index and probability buffers");
   QCNN_CHECK(topk > 0 || prob_h, "qcnn_net_submit_u8_h: nothing to return (topk == 0 and prob_h == NULL)");
   QCNN_ON_DEVICE(net->ctx->device);
-  if (!net->stCopy) {
-    QCNN_CUDA(cudaStreamCreateWithFlags(&net->stCopy, cudaStreamNonBlocking));
-    QCNN_CUDA(cudaStreamCreateWithFlags(&net->stComp, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; i++) {
-      QCNN_CUDA(cudaEventCreateWithFlags(&net->evH2D[i], cudaEventDisableTiming));
-      QCNN_CUDA(cudaEventCreateWithFlags(&net->evDone[i], cudaEventDisableTiming));
-    }
-  }
+  if (int rc = CreatePipeline(net)) return rc;
   if (!net->subInit) {
     for (int i = 0; i < 2; i++) {
       QCNN_CUDA(cudaEventCreateWithFlags(&net->evSubIn[i], cudaEventDisableTiming));
@@ -717,58 +646,34 @@ int qcnn_net_submit_u8_h(qcnn_net* net, const uint8_t* img_h, int N, int topk, i
   const int s = static_cast<int>(net->subCount & 1);
   if (net->subCount >= 2) QCNN_CUDA(cudaEventSynchronize(net->evSubDone[s]));   // the ticket two steps back must be over
   // (re)allocations only while nothing is in flight that uses the buffers
-  if (static_cast<size_t>(N) > net->d_sub8_cap || static_cast<size_t>(N) > net->d_f32_cap || static_cast<size_t>(N) > net->d_out_cap ||
-      (topk > 0 && static_cast<size_t>(N) * topk > net->d_top_cap)) {
+  const size_t in8 = static_cast<size_t>(N) * imgLen;
+  if (net->d_sub8[0].bytes() < in8 || net->d_f32.bytes() < sizeof(float) * in8 ||
+      net->d_prob.bytes() < sizeof(float) * N * outLen || net->d_topi.bytes() < sizeof(int) * N * topk) {
     QCNN_CUDA(cudaStreamSynchronize(net->stCopy));
     QCNN_CUDA(cudaStreamSynchronize(net->stComp));
-    if (static_cast<size_t>(N) > net->d_sub8_cap) {
-      for (int i = 0; i < 2; i++) {
-        if (net->d_sub8[i]) QCNN_CUDA(cudaFree(net->d_sub8[i]));
-        net->d_sub8[i] = nullptr;
-        QCNN_CUDA(cudaMalloc(&net->d_sub8[i], N * imgLen));
-      }
-      net->d_sub8_cap = N;
-    }
-    if (static_cast<size_t>(N) > net->d_f32_cap) {
-      if (net->d_f32) QCNN_CUDA(cudaFree(net->d_f32));
-      net->d_f32 = nullptr; net->d_f32_cap = 0;
-      QCNN_CUDA(cudaMalloc(&net->d_f32, sizeof(float) * N * imgLen));
-      net->d_f32_cap = N;
-      net->ctx->alloc_epoch++;
-    }
-    if (static_cast<size_t>(N) > net->d_out_cap) {
-      if (net->d_prob) QCNN_CUDA(cudaFree(net->d_prob));
-      if (net->d_logit) QCNN_CUDA(cudaFree(net->d_logit));
-      net->d_prob = net->d_logit = nullptr;
-      QCNN_CUDA(cudaMalloc(&net->d_prob, sizeof(float) * N * outLen));
-      QCNN_CUDA(cudaMalloc(&net->d_logit, sizeof(float) * N * outLen));
-      net->d_out_cap = N;
-      net->ctx->alloc_epoch++;
-    }
-    if (topk > 0 && static_cast<size_t>(N) * topk > net->d_top_cap) {
-      if (net->d_topi) QCNN_CUDA(cudaFree(net->d_topi));
-      if (net->d_topv) QCNN_CUDA(cudaFree(net->d_topv));
-      net->d_topi = nullptr; net->d_topv = nullptr;
-      QCNN_CUDA(cudaMalloc(&net->d_topi, sizeof(int) * N * topk));
-      QCNN_CUDA(cudaMalloc(&net->d_topv, sizeof(float) * N * topk));
-      net->d_top_cap = static_cast<size_t>(N) * topk;
-    }
   }
+  for (DeviceBuffer& b : net->d_sub8) QCNN_CUDA(b.Reserve(net->ctx, in8));
+  QCNN_CUDA(net->d_f32.Reserve(net->ctx, sizeof(float) * in8));
+  if (int rc = ReserveOutputs(net, N, topk)) return rc;
   // copy stream: the slot's pixels were last read by the conversion two steps back
   if (net->subCount >= 2) QCNN_CUDA(cudaStreamWaitEvent(net->stCopy, net->evSubRead[s], 0));
-  QCNN_CUDA(cudaMemcpyAsync(net->d_sub8[s], img_h, N * imgLen, cudaMemcpyHostToDevice, net->stCopy));
+  QCNN_CUDA(cudaMemcpyAsync(net->d_sub8[s].get(), img_h, in8, cudaMemcpyHostToDevice, net->stCopy));
   QCNN_CUDA(cudaEventRecord(net->evSubIn[s], net->stCopy));
   // compute stream: conversion, layers, top-k, results home
   QCNN_CUDA(cudaStreamWaitEvent(net->stComp, net->evSubIn[s], 0));
-  if (int rc = LaunchU8ToF32(net->ctx, net->d_sub8[s], net->d_mean, net->d_f32, N, net->imgC, net->imgH * net->imgW, net->stComp)) return rc;
+  if (int rc = LaunchU8ToF32(net->ctx, net->d_sub8[s].as<uint8_t>(), net->d_mean.as<float>(), net->d_f32.as<float>(), N, net->imgC,
+                             net->imgH * net->imgW, net->stComp))
+    return rc;
   QCNN_CUDA(cudaEventRecord(net->evSubRead[s], net->stComp));
-  if (int rc = qcnn_net_forward(net, net->d_f32, N, net->d_prob, nullptr, net->stComp)) return rc;
+  if (int rc = qcnn_net_forward(net, net->d_f32.as<float>(), N, net->d_prob.as<float>(), nullptr, net->stComp)) return rc;
   if (topk > 0) {
-    if (int rc = LaunchTopK(net->ctx, net->d_prob, N, outLen, topk, topk_mode, net->d_topi, net->d_topv, net->stComp)) return rc;
-    QCNN_CUDA(cudaMemcpyAsync(topk_idx_h, net->d_topi, sizeof(int) * N * topk, cudaMemcpyDeviceToHost, net->stComp));
-    QCNN_CUDA(cudaMemcpyAsync(topk_prob_h, net->d_topv, sizeof(float) * N * topk, cudaMemcpyDeviceToHost, net->stComp));
+    if (int rc = LaunchTopK(net->ctx, net->d_prob.as<float>(), N, outLen, topk, topk_mode, net->d_topi.as<int>(), net->d_topv.as<float>(),
+                            net->stComp))
+      return rc;
+    QCNN_CUDA(cudaMemcpyAsync(topk_idx_h, net->d_topi.get(), sizeof(int) * N * topk, cudaMemcpyDeviceToHost, net->stComp));
+    QCNN_CUDA(cudaMemcpyAsync(topk_prob_h, net->d_topv.get(), sizeof(float) * N * topk, cudaMemcpyDeviceToHost, net->stComp));
   }
-  if (prob_h) QCNN_CUDA(cudaMemcpyAsync(prob_h, net->d_prob, sizeof(float) * N * outLen, cudaMemcpyDeviceToHost, net->stComp));
+  if (prob_h) QCNN_CUDA(cudaMemcpyAsync(prob_h, net->d_prob.get(), sizeof(float) * N * outLen, cudaMemcpyDeviceToHost, net->stComp));
   QCNN_CUDA(cudaEventRecord(net->evSubDone[s], net->stComp));
   *ticket = s;
   net->subCount++;
