@@ -80,14 +80,22 @@ QCNN_API int qcnn_conv_layer_set_src_nchw(qcnn_layer* layer, int enable);
  * 3 roll_tc | 4 direct | 6 pq_gemm_tc), "gemm_nt" (positions per CTA of the pq_gemm_tc tilings, 0 = any), "gemm_gt"
  * (k-steps per stage of those tilings, 0 = any), "gemm_nsplit" (their K-split factor, 0 = any; a pq_gemm_tc pin that no
  * tiling of the layer matches makes the forward fail), "autotune"
- * (0 = keep the cost model's first tiling instead of timing the candidates of the chosen family on the device) */
+ * (0 = keep the cost model's first tiling instead of timing the candidates of the chosen family on the device);
+ * FC layers only: "asmt_packed" (1 = keep the assignment table in device memory bit-packed at b = log2(K) bits per
+ * index instead of one byte, and unpack it inside the FC kernels; 0 = the byte table, the default).  Switching repacks the
+ * table on the host, waits for the work queued on the layer's device, frees the previous table and makes graphs captured
+ * before stale.  Every FC path (batch <= 4 chain, gather kernel, tensor-core GEMM) makes the same plan and adds the same
+ * LUT entries in the same order either way, so outputs are bit-identical; K = 256 is accepted and keeps its byte table.
+ * Device layout: row s at byte s * RoundUp(DoutPad * b / 8, 16) (DoutPad = Dout rounded up to 16), channel o in bits
+ * [o b, o b + b) of the row as a little-endian bit string.  Fails on a conv layer. */
 QCNN_API int qcnn_layer_set_param(qcnn_layer* layer, const char* name, int value);
-/* one-line description of the kernel + tiling chosen for batch N */
+/* one-line description of the kernel + tiling chosen for batch N (FC layers with a packed table end in " asmt=<b>bit") */
 QCNN_API int qcnn_layer_describe(qcnn_layer* layer, int N, char* buf, size_t cap);
 QCNN_API void qcnn_layer_destroy(qcnn_layer* layer);
 /* out[0..2] = Ho, Wo, Cout (FC: 1, 1, Dout) */
 QCNN_API int qcnn_layer_out_dims(const qcnn_layer* layer, int* out3);
-/* algorithmic HBM bytes of one forward launch at batch N (SURVEY.md 8(d)) and lookup-add / LUT MAC counts */
+/* algorithmic HBM bytes of one forward launch at batch N (SURVEY.md 8(d)) and lookup-add / LUT MAC counts; the
+ * assignment term of a packed FC table is S * ceil(Dout * b / 8) bytes */
 QCNN_API int qcnn_layer_work(const qcnn_layer* layer, int N, double* alg_bytes, double* lookups, double* lut_macs);
 /* device copy of the re-laid-out assignment table, decoded back to plain 0-based indices in the reference's
  * asmtBuf order ([kh][kw][S][Cout] / [S][Dout], CaffeEva.cc:585-586, 610-611) -- for bit-exact index tests */
@@ -195,6 +203,9 @@ QCNN_API int qcnn_net_wait(qcnn_net* net, int ticket);
 /* images per pipeline chunk of the host-buffer entry points (default 128; the first chunk of a call is a quarter of
  * that): H2D of chunk c+1 overlaps the layers of chunk c */
 QCNN_API int qcnn_net_set_chunk(qcnn_net* net, int chunk);
+/* qcnn_layer_set_param(layer, "asmt_packed", enable) for every FC layer of the net (multi-GPU: call it on every
+ * replica, qcnn_multi_net); the batch-1 graph is recaptured on the next forward */
+QCNN_API int qcnn_net_set_asmt_packed(qcnn_net* net, int enable);
 /* after a forward with keep_maps: device pointer + dims [N,H,W,C] of featMapLst[idx] */
 QCNN_API int qcnn_net_featmap(qcnn_net* net, int idx, const float** ptr, int* dims4);
 /* per-layer CUDA-event timing of the LAST forward (ms); enable before the forward.  Mirrors the reference's

@@ -100,6 +100,7 @@ _SIGS = {
     "qcnn_net_submit_u8_h": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, C.POINTER(_i)]),
     "qcnn_net_wait": (_i, [_vp, _i]),
     "qcnn_net_set_chunk": (_i, [_vp, _i]),
+    "qcnn_net_set_asmt_packed": (_i, [_vp, _i]),
     "qcnn_net_featmap": (_i, [_vp, _i, C.POINTER(_vp), C.POINTER(_i)]),
     "qcnn_net_set_profiling": (_i, [_vp, _i]),
     "qcnn_net_layer_time_ms": (_i, [_vp, _i, C.POINTER(_f)]),
@@ -368,6 +369,10 @@ class Net(object):
 
     def set_chunk(self, n):
         _check(lib.qcnn_net_set_chunk(self.h, n))
+
+    def set_asmt_packed(self, enable=True):
+        """Keep every FC assignment table bit-packed at log2(K) bits per index on the device (outputs are unchanged)."""
+        _check(lib.qcnn_net_set_asmt_packed(self.h, int(enable)))
 
     def forward(self, img, prob=None, logits=None, stream=None):
         """img: CUDA float32 [N,C,H,W]; returns prob [N,out_len] (device)."""

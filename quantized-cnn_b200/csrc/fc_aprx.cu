@@ -19,6 +19,7 @@
 //     exactly the reference's (bias, then s ascending) and the result is bit-identical to the CPU path.
 #include "qcnn_internal.h"
 #include "async_copy.h"
+#include "packed_asmt.h"
 
 #include <algorithm>
 #include <cstdlib>
@@ -73,10 +74,32 @@ constexpr int kRowBlock = 8;  // assignment rows held in registers per block of 
 // cp.async while the PREVIOUS chunk was being gathered; (2) the LUT slice [TN][PFL][K] is built from them
 // (shared -> shared, no global latency); (3) the chunk's assignment rows stream through a rolling register window
 // (block r+1 is in flight while block r is consumed) and are gathered against the LUT slice.
-template <int K, int CPT, int TN, int PFL, bool PRE>
-__global__ void __launch_bounds__(kFcThreads, 2) fc_aprx_kernel(const FcArgs a) {
+//
+// PACKED: the bit-packed table of packed_asmt.h (rows of `pitch` bytes, b = log2(K) bits per channel).  A thread streams the
+// aligned words that cover its CPT * b bits of a row and unpacks them just before the lookups; tiling, chunking and the
+// order of the adds are those of the byte table, so both give bit-identical sums.
+template <int CPT, int NW> struct PackedWords { uint32_t w[NW]; };
+template <bool PACKED, typename A, typename B> struct Pick { using type = A; };
+template <typename A, typename B> struct Pick<false, A, B> { using type = B; };
+template <int CPT, int NW>
+__device__ __forceinline__ PackedWords<CPT, NW> LoadStream(const PackedWords<CPT, NW>* p) {
+  PackedWords<CPT, NW> v;
+#pragma unroll
+  for (int i = 0; i < NW; i++) v.w[i] = LoadStream(reinterpret_cast<const uint32_t*>(p) + i);
+  return v;
+}
+template <int CPT, int NW>
+__device__ __forceinline__ void Zero(PackedWords<CPT, NW>& v) {
+#pragma unroll
+  for (int i = 0; i < NW; i++) v.w[i] = 0u;
+}
+
+template <int K, int CPT, int TN, int PFL, bool PRE, bool PACKED>
+__device__ __forceinline__ void FcAprxBody(const FcArgs a, int pitch) {
   extern __shared__ __align__(16) unsigned char smraw[];
-  using AV = typename AsmtVec<CPT>::type;
+  constexpr int B = PACKED ? (K == 16 ? 4 : (K == 32 ? 5 : (K == 64 ? 6 : 7))) : 8;
+  constexpr int NW = qcnn::PackedSpan<B, CPT>::kWords;
+  using AV = typename Pick<PACKED, PackedWords<CPT, NW>, typename AsmtVec<CPT>::type>::type;
   constexpr int U = kRowBlock;
   static_assert(PFL % U == 0, "chunk must be a whole number of row blocks");
   const int d = a.d;
@@ -94,6 +117,13 @@ __global__ void __launch_bounds__(kFcThreads, 2) fc_aprx_kernel(const FcArgs a) 
   const int s_begin = split * a.s_per_split;
   const int s_end = min(a.S, s_begin + a.s_per_split);
   const bool live = o0 < a.DoutPad;
+  // PACKED: first bit of the thread's channels inside a row -> its first aligned word, and the bit offset inside that word
+  const uint32_t bit0 = static_cast<uint32_t>(o0) * B, sh = bit0 & 31u;
+  const uint8_t* pbase = a.asmt + (bit0 >> 5) * 4;
+  auto rowPtr = [&](int s) -> const AV* {
+    if constexpr (PACKED) return reinterpret_cast<const AV*>(pbase + static_cast<size_t>(s) * pitch);
+    else return reinterpret_cast<const AV*>(a.asmt + static_cast<size_t>(s) * a.DoutPad + o0);
+  };
 
   // asynchronous staging of chunk `sc` into buffer `buf`
   auto fetch = [&](int sc, int buf) {
@@ -133,7 +163,7 @@ __global__ void __launch_bounds__(kFcThreads, 2) fc_aprx_kernel(const FcArgs a) 
 #pragma unroll
     for (int r = 0; r < U; r++) {
       const int s = sc + r;
-      if (live && s < s_end) win[r] = LoadStream(reinterpret_cast<const AV*>(a.asmt + static_cast<size_t>(s) * a.DoutPad + o0));
+      if (live && s < s_end) win[r] = LoadStream(rowPtr(s));
       else Zero(win[r]);
     }
     // (1) staged operands of this chunk have landed; the previous gather is done with `lut`
@@ -181,21 +211,33 @@ __global__ void __launch_bounds__(kFcThreads, 2) fc_aprx_kernel(const FcArgs a) 
 #pragma unroll
         for (int r = 0; r < U; r++) {
           const int s = sc + rb + U + r;
-          if (live && s < s_end) win[r] = LoadStream(reinterpret_cast<const AV*>(a.asmt + static_cast<size_t>(s) * a.DoutPad + o0));
+          if (live && s < s_end) win[r] = LoadStream(rowPtr(s));
           else Zero(win[r]);
         }
       }
       // rows past s_end hold index 0 and their LUT rows are zero, so no tail guard is needed
 #pragma unroll
       for (int r = 0; r < U; r++) {
+        if constexpr (PACKED) {
+          uint32_t idx[CPT];
+          qcnn::UnpackFields<B, CPT, NW>(cur[r].w, sh, idx);
 #pragma unroll
-        for (int c = 0; c < CPT; c++) {
-          const uint32_t w = Word(cur[r], c >> 2);
-          uint32_t off = (w >> (8 * (c & 3))) & 0xFFu;
-          if (!PRE) off <<= 2;
+          for (int c = 0; c < CPT; c++) {
+            const uint32_t off = idx[c] << 2;
 #pragma unroll
-          for (int nl = 0; nl < TN; nl++)
-            acc[nl][c] += *reinterpret_cast<const float*>(lutb + (nl * PFL + rb + r) * K * 4 + off);
+            for (int nl = 0; nl < TN; nl++)
+              acc[nl][c] += *reinterpret_cast<const float*>(lutb + (nl * PFL + rb + r) * K * 4 + off);
+          }
+        } else {
+#pragma unroll
+          for (int c = 0; c < CPT; c++) {
+            const uint32_t w = Word(cur[r], c >> 2);
+            uint32_t off = (w >> (8 * (c & 3))) & 0xFFu;
+            if (!PRE) off <<= 2;
+#pragma unroll
+            for (int nl = 0; nl < TN; nl++)
+              acc[nl][c] += *reinterpret_cast<const float*>(lutb + (nl * PFL + rb + r) * K * 4 + off);
+          }
         }
       }
     }
@@ -218,6 +260,15 @@ __global__ void __launch_bounds__(kFcThreads, 2) fc_aprx_kernel(const FcArgs a) 
       for (int c = 0; c < CPT; c++) out[o0 + c] = acc[nl][c];
     }
   }
+}
+
+template <int K, int CPT, int TN, int PFL, bool PRE>
+__global__ void __launch_bounds__(kFcThreads, 2) fc_aprx_kernel(const FcArgs a) {
+  FcAprxBody<K, CPT, TN, PFL, PRE, false>(a, 0);
+}
+template <int K, int CPT, int TN, int PFL>
+__global__ void __launch_bounds__(kFcThreads, 2) fc_aprx_packed_kernel(const FcArgs a, int pitch) {
+  FcAprxBody<K, CPT, TN, PFL, false, true>(a, pitch);
 }
 
 // dst[n][o] = sum over splits (ascending; split 0 already carries the bias)
@@ -299,28 +350,35 @@ __global__ void fc_prep_bf_kernel(const float* __restrict__ src, const int* __re
   base[per + r] = make_uint4(p2[0], p2[1], p2[2], p2[3]);
 }
 
-template <int K, int CPT, int TN, int PF, bool PRE>
-int Launch(const FcArgs& a, dim3 grid, cudaStream_t st) {
+// PACKED: the bit-packed table, rows of `pitch` bytes (PRE is then false: the kernel scales the unpacked index itself)
+template <int K, int CPT, int TN, int PF, bool PRE, bool PACKED>
+int Launch(const FcArgs& a, int pitch, dim3 grid, cudaStream_t st) {
   const size_t xpad = (static_cast<size_t>(TN) * PF * a.d + 3) & ~static_cast<size_t>(3);
   const size_t smem = sizeof(float) * (static_cast<size_t>(TN) * PF * K + 2 * xpad + 2 * static_cast<size_t>(PF) * K * a.d);
   if (smem > 200 * 1024) {
     qcnn::SetError("qcnn_fc_aprx_forward: K=%d d=%d needs %zu bytes of shared memory per CTA", K, a.d, smem);
     return 1;
   }
-  auto kern = fc_aprx_kernel<K, CPT, TN, PF, PRE>;
-  if (smem > 48 * 1024) QCNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<grid, kFcThreads, smem, st>>>(a);
+  if constexpr (PACKED) {
+    auto kern = fc_aprx_packed_kernel<K, CPT, TN, PF>;
+    if (smem > 48 * 1024) QCNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, kFcThreads, smem, st>>>(a, pitch);
+  } else {
+    auto kern = fc_aprx_kernel<K, CPT, TN, PF, PRE>;
+    if (smem > 48 * 1024) QCNN_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid, kFcThreads, smem, st>>>(a);
+  }
   QCNN_CUDA(cudaGetLastError());
   return 0;
 }
 
-template <int K, bool PRE>
-int LaunchK(const FcArgs& a, int tn, int cpt, dim3 grid, cudaStream_t st) {
-  if (cpt == 4 && tn == 8) return Launch<K, 4, 8, (K <= 32 ? 32 : (K <= 64 ? 16 : 8)), PRE>(a, grid, st);
+template <int K, bool PRE, bool PACKED = false>
+int LaunchK(const FcArgs& a, int tn, int cpt, dim3 grid, cudaStream_t st, int pitch = 0) {
+  if (cpt == 4 && tn == 8) return Launch<K, 4, 8, (K <= 32 ? 32 : (K <= 64 ? 16 : 8)), PRE, PACKED>(a, pitch, grid, st);
   switch (tn) {
-    case 1: return Launch<K, 16, 1, (K <= 64 ? 16 : 8), PRE>(a, grid, st);
-    case 4: return Launch<K, 8, 4, (K <= 32 ? 32 : (K <= 64 ? 16 : 8)), PRE>(a, grid, st);
-    default: return Launch<K, 8, 8, (K <= 32 ? 32 : (K <= 64 ? 16 : 8)), PRE>(a, grid, st);
+    case 1: return Launch<K, 16, 1, (K <= 64 ? 16 : 8), PRE, PACKED>(a, pitch, grid, st);
+    case 4: return Launch<K, 8, 4, (K <= 32 ? 32 : (K <= 64 ? 16 : 8)), PRE, PACKED>(a, pitch, grid, st);
+    default: return Launch<K, 8, 8, (K <= 32 ? 32 : (K <= 64 ? 16 : 8)), PRE, PACKED>(a, pitch, grid, st);
   }
 }
 
@@ -438,7 +496,7 @@ int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
     QCNN_CUDA(L->d_partial.Reserve(ctx, sizeof(float) * static_cast<size_t>(a.nsplit) * N * L->DoutPad, st));
     a.partial = L->d_partial.as<float>();
   }
-  if (int rc = LaunchPqGemmArgs(ctx, a, static_cast<long long>(tiles) * a.nsplit * a.nct, st)) return rc;
+  if (int rc = LaunchPqGemmArgs(ctx, a, static_cast<long long>(tiles) * a.nsplit * a.nct, st, L->asmt_bits, L->asmt_pitch)) return rc;
   ctx->launches++;
   if (a.nsplit > 1)
     if (int rc = LaunchSplitReduce(ctx, a.partial, dst, N, L->Dout, L->DoutPad, a.nsplit, relu, st)) return rc;
@@ -492,7 +550,18 @@ int LaunchFc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaS
   dim3 grid(gx, gy, nsplit);
   int rc;
   const bool pre = L->kshift == 2;
-  switch (L->K) {
+  if (L->asmt_bits) {   // bit-packed table: same grid, chunking and splits as the byte table
+    const int p = L->asmt_pitch;
+    switch (L->K) {
+      case 16:  rc = LaunchK<16, false, true>(a, tn, cpt, grid, st, p); break;
+      case 32:  rc = LaunchK<32, false, true>(a, tn, cpt, grid, st, p); break;
+      case 64:  rc = LaunchK<64, false, true>(a, tn, cpt, grid, st, p); break;
+      case 128: rc = LaunchK<128, false, true>(a, tn, cpt, grid, st, p); break;
+      default:
+        SetError("qcnn_fc_aprx_forward: no packed-table kernel for K=%d", L->K);
+        return 1;
+    }
+  } else switch (L->K) {
     case 16:  rc = pre ? LaunchK<16, true>(a, tn, cpt, grid, st) : LaunchK<16, false>(a, tn, cpt, grid, st); break;
     case 32:  rc = pre ? LaunchK<32, true>(a, tn, cpt, grid, st) : LaunchK<32, false>(a, tn, cpt, grid, st); break;
     case 64:  rc = pre ? LaunchK<64, true>(a, tn, cpt, grid, st) : LaunchK<64, false>(a, tn, cpt, grid, st); break;

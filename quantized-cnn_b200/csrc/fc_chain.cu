@@ -24,6 +24,7 @@
 // bias + s-ascending sum (fp32 adds only; tolerance in tests/test_gpu_layers.py).  fc_nsplit = 1 keeps the bit-exact kernel.
 #include "qcnn_internal.h"
 #include "async_copy.h"
+#include "packed_asmt.h"
 
 #include <algorithm>
 #include <cmath>
@@ -218,13 +219,30 @@ __device__ __forceinline__ void GatherRow(const IV& w, uint32_t lr, float (&acc)
   }
 }
 
+// the CPT lookups of one row of the bit-packed table (packed_asmt.h): w = the NW aligned words that cover the thread's
+// CPT * B bits, the first one starting at bit `sh`.  The LUT row is at lr either way (PRE rows are 256 bytes apart).
+template <int CPT, int B, int NW>
+__device__ __forceinline__ void GatherRowPacked(const uint32_t (&w)[NW], uint32_t sh, uint32_t lr, float (&acc)[CPT]) {
+  uint32_t idx[CPT];
+  qcnn::UnpackFields<B, CPT, NW>(w, sh, idx);
+#pragma unroll
+  for (int c = 0; c < CPT; c++) acc[c] += LdShared(lr + (idx[c] << 2));
+}
+template <int NW>
+__device__ __forceinline__ void LoadWords(const uint8_t* p, uint32_t (&w)[NW]) {
+#pragma unroll
+  for (int i = 0; i < NW; i++) w[i] = reinterpret_cast<const uint32_t*>(p)[i];
+}
+
 // Steps (3) and (4) of a layer for one consumer thread: gather-accumulate the CTA's assignment rows as their ring chunks
 // arrive (thread = CPT consecutive channels of the rows rgIdx, rgIdx + rg, ...; four rows are in flight together), then
-// publish the partial sums.
-template <int CPT, bool PRE>
+// publish the partial sums.  B < 8: the rows are bit-packed at B bits per index, packedPitch bytes apart in the ring (the row
+// groups own the same rows as with the byte table, so the partial sums are the same).
+template <int CPT, bool PRE, int B = 8>
 __device__ __forceinline__ void GatherAndPublish(const ChainLayer& L, int rows, int nStage, uint64_t* fullB, uint64_t* emptyB,
                                                  const uint8_t* ring, const float* lut, float* rgred, float* out, int tid,
-                                                 int lane, int* stagep, uint32_t* roundp, unsigned long long* dbg) {
+                                                 int lane, int* stagep, uint32_t* roundp, unsigned long long* dbg,
+                                                 int packedPitch = 0) {
   using IV = typename Idx<CPT>::type;
   float acc[CPT];
 #pragma unroll
@@ -238,7 +256,34 @@ __device__ __forceinline__ void GatherAndPublish(const ChainLayer& L, int rows, 
   for (int r = 0; r < rows; r += L.rpc) {
     MbarWait<26>(fullB + stage, round & 1u);
     if (dbg && tid == 0 && r == 0) dbg[0] = clock64();
-    if (active) {
+    if constexpr (B < 8) {
+      if (active) {
+        constexpr int NW = qcnn::PackedSpan<B, CPT>::kWords;
+        const uint32_t bit0 = static_cast<uint32_t>(cgIdx) * CPT * B, sh = bit0 & 31u;
+        const uint8_t* chunk = ring + static_cast<size_t>(stage) * kChunkBytes + (bit0 >> 5) * 4;
+        const int n = min(L.rpc, rows - r), pp = packedPitch;
+        const uint32_t lr0 = lutBase + static_cast<uint32_t>(r) * rowBytes;
+        int q = rgIdx;
+        for (; q + 3 * rg < n; q += 4 * rg) {
+          const uint8_t* p = chunk + static_cast<size_t>(q) * pp;
+          uint32_t w0[NW], w1[NW], w2[NW], w3[NW];
+          LoadWords(p, w0);
+          LoadWords(p + static_cast<size_t>(rg) * pp, w1);
+          LoadWords(p + static_cast<size_t>(2 * rg) * pp, w2);
+          LoadWords(p + static_cast<size_t>(3 * rg) * pp, w3);
+          const uint32_t lr = lr0 + static_cast<uint32_t>(q) * rowBytes, dl = static_cast<uint32_t>(rg) * rowBytes;
+          GatherRowPacked<CPT, B>(w0, sh, lr, acc);
+          GatherRowPacked<CPT, B>(w1, sh, lr + dl, acc);
+          GatherRowPacked<CPT, B>(w2, sh, lr + 2 * dl, acc);
+          GatherRowPacked<CPT, B>(w3, sh, lr + 3 * dl, acc);
+        }
+        for (; q < n; q += rg) {
+          uint32_t w0[NW];
+          LoadWords(chunk + static_cast<size_t>(q) * pp, w0);
+          GatherRowPacked<CPT, B>(w0, sh, lr0 + static_cast<uint32_t>(q) * rowBytes, acc);
+        }
+      }
+    } else if (active) {
       const uint8_t* chunk = ring + static_cast<size_t>(stage) * kChunkBytes + cgIdx * CPT;
       const int n = min(L.rpc, rows - r);
       const uint32_t lr0 = lutBase + static_cast<uint32_t>(r) * rowBytes;
@@ -290,7 +335,15 @@ __device__ __forceinline__ void GatherAndPublish(const ChainLayer& L, int rows, 
   if (dbg && tid == 0) dbg[2] = clock64();
 }
 
-__global__ void __launch_bounds__(kThreads, 1) fc_chain_kernel(const __grid_constant__ ChainArgs a) {
+// layers whose assignment table is bit-packed (packed_asmt.h): bits[l] (0 = byte table) and the bytes per table row
+struct ChainPack {
+  int bits[kMaxChain];
+  int pitch[kMaxChain];
+};
+
+// PK: some layer of the chain has a bit-packed table (fc_chain_packed_kernel), pk describes them; else pk is NULL
+template <bool PK>
+__device__ __forceinline__ void ChainBody(const ChainArgs& a, const ChainPack* pk) {
   extern __shared__ __align__(128) unsigned char sm[];
   uint64_t* fullB = reinterpret_cast<uint64_t*>(sm);
   uint64_t* emptyB = fullB + kMaxStage;
@@ -332,11 +385,12 @@ __global__ void __launch_bounds__(kThreads, 1) fc_chain_kernel(const __grid_cons
         const ChainLayer& L = a.L[l];
         int r0, r1;
         RowRange(L, cta, &r0, &r1);
+        const int rowB = PK ? pk->pitch[l] : L.DoutPad;   // bytes per table row
         for (int r = r0; r < r1; r += L.rpc, issued++) {
           if (round > 0) MbarWait<26>(emptyB + stage, (round - 1) & 1u);
-          const uint32_t bytes = static_cast<uint32_t>(min(L.rpc, r1 - r)) * L.DoutPad;
+          const uint32_t bytes = static_cast<uint32_t>(min(L.rpc, r1 - r)) * rowB;
           MbarExpectTx(fullB + stage, bytes);
-          BulkLoad(ring + static_cast<size_t>(stage) * kChunkBytes, L.asmt + static_cast<size_t>(r) * L.DoutPad, bytes, fullB + stage);
+          BulkLoad(ring + static_cast<size_t>(stage) * kChunkBytes, L.asmt + static_cast<size_t>(r) * rowB, bytes, fullB + stage);
           if (++stage == a.nStage) { stage = 0; round++; }
         }
       }
@@ -440,8 +494,19 @@ __global__ void __launch_bounds__(kThreads, 1) fc_chain_kernel(const __grid_cons
     float* out = L.partial + static_cast<size_t>(cta) * L.DoutPad;
 #define QCNN_GP(C, P) GatherAndPublish<C, P>(L, rows, a.nStage, fullB, emptyB, ring, lut, rgred, out, tid, lane, &stage, &round, \
                                              a.dbg ? a.dbg + 32 * cta + 6 + 5 * l : nullptr)
-    if (L.pre) { if (L.cpt == 8) QCNN_GP(8, true); else if (L.cpt == 4) QCNN_GP(4, true); else QCNN_GP(16, true); }
+#define QCNN_GPK(C, B) GatherAndPublish<C, false, B>(L, rows, a.nStage, fullB, emptyB, ring, lut, rgred, out, tid, lane, &stage, \
+                                                      &round, a.dbg ? a.dbg + 32 * cta + 6 + 5 * l : nullptr, pk->pitch[l])
+#define QCNN_GPK_B(B) do { if (L.cpt == 8) QCNN_GPK(8, B); else if (L.cpt == 4) QCNN_GPK(4, B); else QCNN_GPK(16, B); } while (0)
+    if (PK && pk->bits[l]) {
+      if (pk->bits[l] == 5) QCNN_GPK_B(5);
+      else if (pk->bits[l] == 4) QCNN_GPK_B(4);
+      else if (pk->bits[l] == 6) QCNN_GPK_B(6);
+      else QCNN_GPK_B(7);
+    }
+    else if (L.pre) { if (L.cpt == 8) QCNN_GP(8, true); else if (L.cpt == 4) QCNN_GP(4, true); else QCNN_GP(16, true); }
     else { if (L.cpt == 8) QCNN_GP(8, false); else if (L.cpt == 4) QCNN_GP(4, false); else QCNN_GP(16, false); }
+#undef QCNN_GPK_B
+#undef QCNN_GPK
 #undef QCNN_GP
   }
 
@@ -468,6 +533,12 @@ __global__ void __launch_bounds__(kThreads, 1) fc_chain_kernel(const __grid_cons
   if (a.dbg && tid == 0) { a.dbg[32 * cta + 1] = GlobalTimer(); a.dbg[32 * cta + 3] = clock64(); }
 }
 
+__global__ void __launch_bounds__(kThreads, 1) fc_chain_kernel(const __grid_constant__ ChainArgs a) { ChainBody<false>(a, nullptr); }
+__global__ void __launch_bounds__(kThreads, 1) fc_chain_packed_kernel(const __grid_constant__ ChainArgs a,
+                                                                      const __grid_constant__ ChainPack pk) {
+  ChainBody<true>(a, &pk);
+}
+
 int Gcd(int a, int b) { return b ? Gcd(b, a % b) : a; }
 
 }  // namespace
@@ -484,12 +555,19 @@ static bool ChainEnabled() {
 
 // Fills the kernel arguments for a run of FC layers; false when the kernel does not apply (the caller falls back to
 // the per-layer kernels of fc_aprx.cu).
-static bool PlanChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int n, ChainArgs* out, size_t* smemBytes) {
+// *packed: some layer keeps a bit-packed table (launch fc_chain_packed_kernel with *pk).  Eligibility and every figure
+// but the ring chunking of a packed layer are those of the byte table.
+static bool PlanChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int n, ChainArgs* out, size_t* smemBytes,
+                      ChainPack* pk = nullptr, bool* packed = nullptr) {
   if (!ChainEnabled() || n < 1 || n > kMaxChain) return false;
   const int G = ctx->sm_count;
   if (G < 1 || G > kMaxParts) return false;
   ChainArgs& a = *out;
   memset(&a, 0, sizeof(a));
+  ChainPack pkLocal;
+  if (!pk) pk = &pkLocal;
+  memset(pk, 0, sizeof(*pk));
+  if (packed) *packed = false;
   a.nLayers = n; a.G = G;
   int xF = 64, lutF = 64, ctrdF = 0, rgF = 0;
   for (int l = 0; l < n; l++) {
@@ -523,6 +601,19 @@ static bool PlanChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu,
       if (exact) { L.srcHW = hw; L.srcC = Q->src_c; L.srcHWInv = inv; }
     }
     L.rpc = std::max(1, kChunkBytes / Q->DoutPad);
+    pk->bits[l] = Q->asmt_bits;
+    pk->pitch[l] = Q->asmt_bits ? Q->asmt_pitch : Q->DoutPad;
+    if (Q->asmt_bits) {
+      // packed rows are shorter, so a chunk holds more of them; the count stays a multiple of rg when the byte table's
+      // is (row group g then owns rows g, g + rg, ... of the CTA's share either way: same partial sums), and leaves
+      // room after the last row for the aligned word reads that run past it (packed_asmt.h)
+      const int P = Q->asmt_pitch;
+      int rpc = L.rpc;
+      if (rpc % L.rg == 0) rpc = (kChunkBytes - qcnn::kPackedTail) / P / L.rg * L.rg;
+      if (rpc < 1 || rpc * P + qcnn::kPackedTail > kChunkBytes) return false;
+      L.rpc = rpc;
+      if (packed) *packed = true;
+    }
     L.unit = 4 / Gcd(Q->d, 4);
     const int units = CeilDiv(Q->S, L.unit);
     L.unitsBase = units / G; L.unitsRem = units % G;
@@ -586,12 +677,15 @@ int LaunchFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int
     if (grown) QCNN_CUDA(cudaMemsetAsync(Q->d_cpart.get(), 0xFF, need, st));
   }
   ChainArgs a;
+  ChainPack pk;
+  bool packed = false;
   size_t smem = 0;
-  if (!PlanChain(ctx, layers, relu, n, &a, &smem)) return 0;
+  if (!PlanChain(ctx, layers, relu, n, &a, &smem, &pk, &packed)) return 0;
   static bool attrSet[64] = {false};
   if (ctx->device < 64 && !attrSet[ctx->device]) {
-    QCNN_CUDA(cudaFuncSetAttribute(fc_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   static_cast<int>(ctx->smem_optin ? ctx->smem_optin : 227 * 1024)));
+    const int lim = static_cast<int>(ctx->smem_optin ? ctx->smem_optin : 227 * 1024);
+    QCNN_CUDA(cudaFuncSetAttribute(fc_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    QCNN_CUDA(cudaFuncSetAttribute(fc_chain_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     attrSet[ctx->device] = true;
   }
   a.dbg = dbg;
@@ -606,7 +700,8 @@ int LaunchFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int
     attr[0].id = cudaLaunchAttributeCooperative;   // all CTAs co-resident (they wait for each other's partial sums)
     attr[0].val.cooperative = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    QCNN_CUDA(cudaLaunchKernelEx(&cfg, fc_chain_kernel, a));
+    if (packed) QCNN_CUDA(cudaLaunchKernelEx(&cfg, fc_chain_packed_kernel, a, pk));
+    else QCNN_CUDA(cudaLaunchKernelEx(&cfg, fc_chain_kernel, a));
     ctx->launches++;
   }
   *handled = true;

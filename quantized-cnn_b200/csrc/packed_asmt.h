@@ -1,0 +1,59 @@
+// Bit-packed assignment tables of the fully-connected layers (qcnn_layer_set_param "asmt_packed"), shared by the three FC
+// paths (fc_chain.cu, fc_aprx.cu, pq_gemm_tc.cu mode 2).
+//
+// Layout: b = log2(K) bits per index (4..7; K = 256 keeps its byte table).  Row s of the [S][DoutPad] table starts at byte
+// s * pitch, pitch = RoundUp(DoutPad * b / 8, 16), so rows stay 16-byte aligned for cp.async / cp.async.bulk.  Inside a
+// row, channel o occupies bits [o b, o b + b) of a little-endian bit string (bit i = bit i % 8 of byte i / 8).  The value
+// is the plain 0-based index (the byte table stores idx << kshift); padding channels hold 0.
+//
+// A thread that owns CPT consecutive channels starting at a multiple of CPT reads the aligned 32-bit words covering its
+// CPT * b bits: the first bit sits at a multiple of gcd(CPT b, 32) inside the first word, so PackedSpan<b, CPT>::kWords
+// words always suffice.  Those reads may run up to 15 bytes past the end of a row; the table carries kPackedTail bytes
+// after its last row, and the chain kernel leaves as many free after the rows of a ring chunk.
+#ifndef QCNN_PACKED_ASMT_H_
+#define QCNN_PACKED_ASMT_H_
+
+#include <stdint.h>
+
+namespace qcnn {
+
+constexpr int kPackedTail = 16;
+
+// bits per packed index of a codebook of K (a power of two) words; 8 = the byte table is kept
+inline int PackedBits(int K) {
+  int b = 0;
+  while ((1 << b) < K) b++;
+  return b;
+}
+inline int PackedPitch(int DoutPad, int b) { return (DoutPad * b / 8 + 15) / 16 * 16; }
+
+template <int B, int CPT>
+struct PackedSpan {
+  static constexpr int kBits = CPT * B;
+  static constexpr int kAlign = kBits % 32 == 0 ? 32 : (kBits % 16 == 0 ? 16 : (kBits % 8 == 0 ? 8 : 4));   // gcd(kBits, 32)
+  static constexpr int kWords = (32 - kAlign + kBits + 31) / 32;
+};
+
+#ifdef __CUDACC__
+// idx[c] = field c (B bits) of the bit string that starts at bit `sh` of the words w[0..NW): the words are first shifted
+// down by `sh` (NW - 1 funnel shifts), then every field is one compile-time shift (or funnel shift) and a mask
+template <int B, int CPT, int NW>
+__device__ __forceinline__ void UnpackFields(const uint32_t (&w)[NW], uint32_t sh, uint32_t (&idx)[CPT]) {
+  uint32_t u[NW];
+#pragma unroll
+  for (int i = 0; i + 1 < NW; i++) u[i] = __funnelshift_r(w[i], w[i + 1], sh);
+  u[NW - 1] = w[NW - 1] >> sh;
+#pragma unroll
+  for (int c = 0; c < CPT; c++) {
+    const int bit = c * B, j = bit >> 5, o = bit & 31;
+    uint32_t v;
+    if (o + B <= 32 || j + 1 >= NW) v = u[j] >> o;
+    else v = __funnelshift_r(u[j], u[j + 1], o);
+    idx[c] = v & ((1u << B) - 1u);
+  }
+}
+#endif
+
+}  // namespace qcnn
+
+#endif  // QCNN_PACKED_ASMT_H_

@@ -10,6 +10,7 @@
 
 #include "../host/CaffePara.h"
 #include "../host/FileIO.h"
+#include "packed_asmt.h"
 #include "qcnn_internal.h"
 
 namespace qcnn {
@@ -208,6 +209,7 @@ int qcnn_fc_layer_create(qcnn_ctx* ctx, int Din, int Dout, int S, int K, int d, 
   L->Din = Din; L->Dout = Dout; L->S = S; L->K = K; L->d = d;
   L->Ho = 1; L->Wo = 1; L->Cout = Dout;
   L->DoutPad = RoundUp(Dout, 16);
+  L->asmt_pitch = L->DoutPad;
   L->kshift = (K <= 64) ? 2 : 0;
   // assignments: file order [Dout][S] -> device [S][DoutPad] (reference asmtBuf [S][Dout], CaffeEva.cc:610-611),
   // stored as byte offsets into a LUT row (idx * 4) when that fits a byte
@@ -253,9 +255,73 @@ int qcnn_conv_layer_set_src_nchw(qcnn_layer* L, int enable) {
   return 0;
 }
 
+}  // extern "C"
+
+// FC assignment table on the host as plain 0-based indices [S][DoutPad], whichever form d_asmt holds
+static int ReadFcIndices(const qcnn_layer* L, std::vector<uint8_t>* idx) {
+  std::vector<uint8_t> dev(L->d_asmt.bytes());
+  QCNN_CUDA(cudaMemcpy(dev.data(), L->d_asmt.get(), dev.size(), cudaMemcpyDeviceToHost));
+  idx->assign(static_cast<size_t>(L->S) * L->DoutPad, 0);
+  const int b = L->asmt_bits;
+  for (int s = 0; s < L->S; s++) {
+    const uint8_t* row = dev.data() + static_cast<size_t>(s) * L->asmt_pitch;
+    uint8_t* out = idx->data() + static_cast<size_t>(s) * L->DoutPad;
+    for (int o = 0; o < L->DoutPad; o++) {
+      if (!b) { out[o] = row[o] >> L->kshift; continue; }
+      int v = 0;
+      for (int i = 0; i < b; i++) {
+        const int bit = o * b + i;
+        v |= ((row[bit >> 3] >> (bit & 7)) & 1) << i;
+      }
+      out[o] = static_cast<uint8_t>(v);
+    }
+  }
+  return 0;
+}
+
+// Replaces d_asmt by the byte table (enable = 0) or the bit-packed table (packed_asmt.h).  Layers with K = 256 keep the
+// byte table either way: at 8 bits packing changes nothing.
+static int SetAsmtPacked(qcnn_layer* L, int enable) {
+  const int b = (enable && PackedBits(L->K) < 8) ? PackedBits(L->K) : 0;
+  if (b == L->asmt_bits) return 0;
+  QCNN_ON_DEVICE(L->ctx->device);
+  std::vector<uint8_t> idx;
+  if (int rc = ReadFcIndices(L, &idx)) return rc;
+  const int pitch = b ? PackedPitch(L->DoutPad, b) : L->DoutPad;
+  std::vector<uint8_t> host(static_cast<size_t>(L->S) * pitch + (b ? kPackedTail : 0), 0);
+  for (int s = 0; s < L->S; s++) {
+    uint8_t* row = host.data() + static_cast<size_t>(s) * pitch;
+    const uint8_t* in = idx.data() + static_cast<size_t>(s) * L->DoutPad;
+    for (int o = 0; o < L->DoutPad; o++) {
+      if (!b) { row[o] = static_cast<uint8_t>(in[o] << L->kshift); continue; }
+      for (int i = 0; i < b; i++) {
+        const int bit = o * b + i;
+        row[bit >> 3] |= static_cast<uint8_t>(((in[o] >> i) & 1) << (bit & 7));
+      }
+    }
+  }
+  // kernels still queued on any stream may read the old table
+  QCNN_CUDA(cudaDeviceSynchronize());
+  DeviceBuffer nb;
+  QCNN_CUDA(nb.Upload(L->ctx, host.data(), host.size()));   // (bumps alloc_epoch: graphs captured before hold the old table)
+  L->d_asmt = std::move(nb);                                 // the old table is freed here
+  L->asmt_bits = b;
+  L->asmt_pitch = pitch;
+  return 0;
+}
+
+extern "C" {
+
 int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
   QCNN_CHECK(L && name, "qcnn_layer_set_param: NULL argument");
   L->ctx->alloc_epoch++;   // every parameter changes kernel choice or buffers: graphs captured before are stale
+  if (!strcmp(name, "asmt_packed")) {
+    // FC only: 1 keeps the assignment table bit-packed at log2(K) bits per index (kernels unpack it), 0 = byte table
+    QCNN_CHECK(L->kind == QCNN_KIND_FC, "qcnn_layer_set_param: 'asmt_packed' applies to FC layers");
+    L->plan_N = 0; L->tuned = 0;
+    L->tunedPlans.clear();
+    return SetAsmtPacked(L, value);
+  }
   if (!strcmp(name, "fc_nsplit")) L->opt_fc_nsplit = value;
   else if (!strcmp(name, "fc_tn")) L->opt_fc_tn = value;
   else if (!strcmp(name, "tensor_core")) {
@@ -296,7 +362,10 @@ int qcnn_layer_describe(qcnn_layer* L, int N, char* buf, size_t cap) {
     const int relu0 = 0;
     DescribeFcChain(L->ctx, &L, &relu0, 1, tc, sizeof(tc));
   }
-  snprintf(buf, cap, "fc_aprx Din=%d Dout=%d S=%d K=%d d=%d%s%s", L->Din, L->Dout, L->S, L->K, L->d, tc[0] ? " via " : "", tc);
+  char packed[16] = "";
+  if (L->asmt_bits) snprintf(packed, sizeof(packed), " asmt=%dbit", L->asmt_bits);
+  snprintf(buf, cap, "fc_aprx Din=%d Dout=%d S=%d K=%d d=%d%s%s%s", L->Din, L->Dout, L->S, L->K, L->d, tc[0] ? " via " : "", tc,
+           packed);
   return 0;
 }
 
@@ -338,7 +407,9 @@ int qcnn_layer_work(const qcnn_layer* L, int N, double* alg_bytes, double* looku
     for (int s = 0; s < L->S; s++) dims += std::max(0, std::min(Cg - s * L->d, L->d));
     macs = static_cast<double>(N) * L->Hin * L->Win * L->grp * dims * L->K;
   } else {
-    bytes = 4.0 * N * L->Din + 4.0 * N * L->Dout + static_cast<double>(L->S) * L->Dout + 4.0 * L->S * L->K * L->d +
+    // assignment term: S * Dout bytes, or S * ceil(Dout * b / 8) when the table is bit-packed
+    const double asmtRow = L->asmt_bits ? static_cast<double>((L->Dout * L->asmt_bits + 7) / 8) : static_cast<double>(L->Dout);
+    bytes = 4.0 * N * L->Din + 4.0 * N * L->Dout + static_cast<double>(L->S) * asmtRow + 4.0 * L->S * L->K * L->d +
             4.0 * L->Dout;
     lk = static_cast<double>(N) * L->S * L->Dout;
     double dims = 0;
@@ -354,24 +425,25 @@ int qcnn_layer_work(const qcnn_layer* L, int N, double* alg_bytes, double* looku
 int qcnn_layer_read_asmt_h(const qcnn_layer* L, uint8_t* out_h, size_t cap) {
   QCNN_CHECK(L && out_h, "qcnn_layer_read_asmt_h: NULL argument");
   QCNN_ON_DEVICE(L->ctx->device);
+  if (L->kind != QCNN_KIND_CONV) {
+    QCNN_CHECK(cap >= static_cast<size_t>(L->S) * L->Dout, "qcnn_layer_read_asmt_h: buffer too small");
+    std::vector<uint8_t> idx;
+    if (int rc = ReadFcIndices(L, &idx)) return rc;
+    for (int s = 0; s < L->S; s++)
+      memcpy(out_h + static_cast<size_t>(s) * L->Dout, idx.data() + static_cast<size_t>(s) * L->DoutPad, L->Dout);
+    return 0;
+  }
   std::vector<uint8_t> dev(L->d_asmt.bytes());
   QCNN_CUDA(cudaMemcpy(dev.data(), L->d_asmt.get(), dev.size(), cudaMemcpyDeviceToHost));
-  if (L->kind == QCNN_KIND_CONV) {
-    const int taps = L->ksz * L->ksz, Kg = L->Cout / L->grp, KgPad = RoundUp(Kg, 16);
-    QCNN_CHECK(cap >= static_cast<size_t>(taps) * L->S * L->Cout, "qcnn_layer_read_asmt_h: buffer too small");
-    for (int t = 0; t < taps; t++)
-      for (int s = 0; s < L->S; s++)
-        for (int c = 0; c < L->Cout; c++) {
-          const int g = c / Kg, cl = c % Kg;
-          out_h[(static_cast<size_t>(t) * L->S + s) * L->Cout + c] =
-              dev[((static_cast<size_t>(g) * L->S + s) * taps + t) * KgPad + cl];
-        }
-  } else {
-    QCNN_CHECK(cap >= static_cast<size_t>(L->S) * L->Dout, "qcnn_layer_read_asmt_h: buffer too small");
+  const int taps = L->ksz * L->ksz, Kg = L->Cout / L->grp, KgPad = RoundUp(Kg, 16);
+  QCNN_CHECK(cap >= static_cast<size_t>(taps) * L->S * L->Cout, "qcnn_layer_read_asmt_h: buffer too small");
+  for (int t = 0; t < taps; t++)
     for (int s = 0; s < L->S; s++)
-      for (int o = 0; o < L->Dout; o++)
-        out_h[static_cast<size_t>(s) * L->Dout + o] = dev[static_cast<size_t>(s) * L->DoutPad + o] >> L->kshift;
-  }
+      for (int c = 0; c < L->Cout; c++) {
+        const int g = c / Kg, cl = c % Kg;
+        out_h[(static_cast<size_t>(t) * L->S + s) * L->Cout + c] =
+            dev[((static_cast<size_t>(g) * L->S + s) * taps + t) * KgPad + cl];
+      }
   return 0;
 }
 

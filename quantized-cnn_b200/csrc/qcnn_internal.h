@@ -256,6 +256,8 @@ struct qcnn_layer {
                                 // (= channel) reads all taps of a chunk with one or two 128-bit loads (pq_gemm_tc.cu, mode 0)
   qcnn::DeviceBuffer d_bias;    // float
   int kshift = 0;       // FC: stored assignment = idx << kshift
+  int asmt_bits = 0;    // FC: 0 = d_asmt is the byte table [S][DoutPad]; 4..7 = bit-packed rows of asmt_pitch bytes (packed_asmt.h)
+  int asmt_pitch = 0;   // FC: bytes per row of d_asmt (DoutPad for the byte table)
   // plans
   ConvPlan plan{};
   int plan_N = 0;        // batch size the cached plan was made for (0 = none)
@@ -293,7 +295,8 @@ int LaunchFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int
 // pq_gemm_tc.cu
 void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands);
 size_t PqGemmSmemBytes(const GemmArgs& a);
-int LaunchPqGemmArgs(qcnn_ctx* ctx, const GemmArgs& a, long long blocks, cudaStream_t st);
+// asmtBits != 0 (mode 2): a.asmt is the bit-packed FC table of packed_asmt.h with rows of asmtPitch bytes
+int LaunchPqGemmArgs(qcnn_ctx* ctx, const GemmArgs& a, long long blocks, cudaStream_t st, int asmtBits = 0, int asmtPitch = 0);
 int BuildCtrdBf(qcnn_layer* L);   // layer creation: the bf16x2 form of the codebook (d % 4 == 0)
 int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows, int cols, int colsPad, int nsplit, int relu,
                       cudaStream_t st);

@@ -693,6 +693,14 @@ int qcnn_net_set_chunk(qcnn_net* net, int chunk) {
   return 0;
 }
 
+int qcnn_net_set_asmt_packed(qcnn_net* net, int enable) {
+  QCNN_CHECK(net, "qcnn_net_set_asmt_packed: NULL net");
+  for (const NetLayer& nl : net->layers)
+    if (nl.pq && nl.pq->kind == QCNN_KIND_FC)
+      if (int rc = qcnn_layer_set_param(nl.pq, "asmt_packed", enable ? 1 : 0)) return rc;
+  return 0;
+}
+
 int qcnn_net_featmap(qcnn_net* net, int idx, const float** ptr, int* dims4) {
   QCNN_CHECK(net && ptr && dims4, "qcnn_net_featmap: NULL argument");
   const int L = static_cast<int>(net->layers.size());
