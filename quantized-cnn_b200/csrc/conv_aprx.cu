@@ -58,6 +58,8 @@ struct ConvKernelInfo {
 constexpr ConvKernelInfo kConvKernelInfo[kConvDirect + 1] = {
     {"conv_s1", false}, {"conv_roll", false}, {"conv_s1_tc(wgmma LUT)", true}, {"conv_roll_tc(wgmma LUT)", true},
     {"conv_direct", false}};
+// the tensor-core GEMM family (tensor_core = 1 / 2): decode-at-use pq_gemm_tc and the weight-stationary conv_ws
+constexpr bool IsGemmTc(int kernel) { return kernel == kPqGemmTc || kernel == kConvWs; }
 
 // ------------------------------------------------------------------------------------------------------------
 // Operand staging.  Everything the LUT stage of step i+1 needs from global memory (input pixels of the
@@ -1006,13 +1008,15 @@ int PlanConv(qcnn_layer* L, int N) {
       }
     }
   }
-  // decode-at-use GEMMs on the tensor cores (pq_gemm_tc.cu).  The kernel FAMILY is a setting, not a timing result:
-  // with tensor_core = 2 (default, bf16x2 operands) or 1 (3xTF32 operands) an eligible layer always runs pq_gemm_tc
-  // (tolerances in DESIGN.md 2), with tensor_core = 0 always the LUT + gather kernels; on-device timing only chooses
-  // among tilings of that family, so the numerical path of a (layer, batch size) is the same in every process.
+  // tensor-core GEMMs: decode-at-use pq_gemm_tc.cu and, for strided narrow-input layers with bf16x2 operands, the
+  // weight-stationary conv_ws.cu.  The operand format is a setting, not a timing result: with tensor_core = 2 (default,
+  // bf16x2) or 1 (3xTF32) an eligible layer always runs one of these GEMMs (tolerances in DESIGN.md 2), with
+  // tensor_core = 0 always the LUT + gather kernels.  On-device timing chooses among the GEMM tilings of that format --
+  // for a conv1-type layer at bf16x2 between conv_ws and pq_gemm_tc mode 1, which share the k-step chain and its bound.
   if (!L->opt_no_tc) {
     std::vector<std::pair<double, ConvPlan>> tc;
     PlanPqGemm(L, N, &tc);
+    PlanConvWs(L, N, &tc);
     if (!tc.empty()) { cands.swap(tc); found = true; }
   }
   QCNN_CHECK(found, "qcnn_conv_layer_create: no tiling fits (Cout/grp=%d must be a multiple of 16; K=%d must be a "
@@ -1021,26 +1025,28 @@ int PlanConv(qcnn_layer* L, int N) {
   // is seen (QCNN_AUTOTUNE=0 keeps the model's first choice)
   std::stable_sort(cands.begin(), cands.end(), [](const std::pair<double, ConvPlan>& x, const std::pair<double, ConvPlan>& y) { return x.first < y.first; });
   L->cands.clear();
-  // layer parameter "force_kernel" / QCNN_FORCE_KERNEL=<0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc>
+  // layer parameter "force_kernel" / QCNN_FORCE_KERNEL=<0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc |
+  // 7 conv_ws>
   // restricts the choice (tests pin the kernel they check; fails when that kernel has no tiling for the layer)
   // Within the LUT + gather family the kernels come in two numerical classes -- fp32 LUT / decode (s1, roll, direct) and
   // 3xTF32 tensor-core LUT stage (s1_tc, roll_tc; ~5e-6 apart) -- and on-device timing must not pick between classes
   // either: the class of the cost model's favourite is kept, timing chooses among its tilings only.
-  if (!cands.empty() && cands[0].second.kernel != kPqGemmTc && !L->opt_force_kernel && getenv("QCNN_FORCE_KERNEL") == nullptr) {
+  if (!cands.empty() && !IsGemmTc(cands[0].second.kernel) && !L->opt_force_kernel && getenv("QCNN_FORCE_KERNEL") == nullptr) {
     const bool want = kConvKernelInfo[cands[0].second.kernel].tcLut;
     std::vector<std::pair<double, ConvPlan>> kept;
     for (const auto& c : cands)
-      if (c.second.kernel != kPqGemmTc && kConvKernelInfo[c.second.kernel].tcLut == want) kept.push_back(c);
+      if (!IsGemmTc(c.second.kernel) && kConvKernelInfo[c.second.kernel].tcLut == want) kept.push_back(c);
     cands.swap(kept);
   }
   // layer parameters "gemm_nt" / "gemm_gt" / "gemm_nsplit": only pq_gemm_tc tilings with that many positions per CTA,
-  // k-steps per stage and K-split factor (0 = any)
+  // k-steps per stage and K-split factor (0 = any); "gemm_nt" also restricts the positions per CTA of conv_ws
   if (L->opt_gemm_nt || L->opt_gemm_gt || L->opt_gemm_nsplit) {
     std::vector<std::pair<double, ConvPlan>> kept;
     for (const auto& c : cands)
-      if (c.second.kernel != kPqGemmTc || ((!L->opt_gemm_nt || c.second.g.NT == L->opt_gemm_nt) &&
-                                           (!L->opt_gemm_gt || c.second.g.GT == L->opt_gemm_gt) &&
-                                           (!L->opt_gemm_nsplit || c.second.g.nsplit == L->opt_gemm_nsplit)))
+      if ((c.second.kernel == kConvWs && (!L->opt_gemm_nt || c.second.g.NT == L->opt_gemm_nt)) ||
+          (c.second.kernel != kPqGemmTc && c.second.kernel != kConvWs) ||
+          ((!L->opt_gemm_nt || c.second.g.NT == L->opt_gemm_nt) && (!L->opt_gemm_gt || c.second.g.GT == L->opt_gemm_gt) &&
+           (!L->opt_gemm_nsplit || c.second.g.nsplit == L->opt_gemm_nsplit)))
         kept.push_back(c);
     QCNN_CHECK(!kept.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d gemm_gt=%d gemm_nsplit=%d has no tiling for this layer at "
                "batch %d", L->opt_gemm_nt, L->opt_gemm_gt, L->opt_gemm_nsplit, N);
@@ -1059,7 +1065,7 @@ int PlanConv(qcnn_layer* L, int N) {
     int perKernel[kConvKernelIds] = {};
     for (size_t i = 0; i < cands.size() && L->cands.size() < kMaxCand; i++) {
       ConvPlan c = cands[i].second;
-      if (pass == 0 && perKernel[c.kernel] >= (c.kernel == kConvDirect ? 8 : (c.kernel == kPqGemmTc ? 6 : 2))) continue;
+      if (pass == 0 && perKernel[c.kernel] >= (c.kernel == kConvDirect ? 8 : (IsGemmTc(c.kernel) ? 6 : 2))) continue;
       ConvArgs& a = c.a;
       a.Hi = L->Hin; a.Wi = L->Win; a.Cin = L->Cin; a.Ho = L->Ho; a.Wo = L->Wo; a.Cout = L->Cout;
       a.ksz = L->ksz; a.pad = L->pad; a.stride = L->stride; a.G = G; a.Cg = Cg; a.Kg = Kg;
@@ -1105,6 +1111,7 @@ static int LaunchPlan(qcnn_layer* L, const ConvPlan& p, const float* src, int N,
   a.src = src; a.dst = dst; a.ctrd = L->d_ctrd.as<float>(); a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
   a.N = N; a.relu = relu; a.src_nchw = L->src_nchw;
   if (p.kernel == kPqGemmTc) return LaunchPqGemm(L, p, src, N, dst, relu, st);
+  if (p.kernel == kConvWs) return LaunchConvWs(L, p, src, N, dst, relu, st);
   if (p.kernel == kConvDirect) {
     const int nj = std::min(a.Cg, a.d);
     // p.J carries the output rows per thread (2 or 4)
@@ -1156,7 +1163,7 @@ int LaunchConv(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
       static const bool tuneLog = getenv("QCNN_AUTOTUNE_LOG") != nullptr;
       if (tuneLog)
         fprintf(stderr, "[qcnn autotune] N=%d Cout=%d k=%d cand %zu: kernel=%d NT/CPT=%d GT/J=%d bf=%d nsplit=%d smem=%zu -> %.4f ms\n",
-                N, L->Cout, L->ksz, i, c.kernel, c.CPT, c.kernel == kPqGemmTc ? c.g.GT : c.J, c.g.bf, c.g.nsplit, c.smem, ms);
+                N, L->Cout, L->ksz, i, c.kernel, c.CPT, IsGemmTc(c.kernel) ? c.g.GT : c.J, c.g.bf, c.g.nsplit, c.smem, ms);
       if (ms < bestMs) { bestMs = ms; bestI = i; }
     }
     cudaEventDestroy(e0);
@@ -1181,6 +1188,15 @@ int DescribeConv(qcnn_layer* L, int N, char* buf, size_t cap) {
              "chunks=%d ksteps=%d nsplit=%d", p.g.bf ? ", bf16x2" : "", p.g.mode, p.g.NT, p.g.GT, p.smem,
              CeilDiv(N * p.g.IB, p.g.NT) * L->grp * p.g.nct * std::max(1, p.g.nsplit), p.g.NPOS, p.g.nChunks,
              ksteps / std::max(1, p.g.nsplit), std::max(1, p.g.nsplit));
+    return 0;
+  }
+  if (p.kernel == kConvWs) {
+    // (no "NT=": the executed-MAC count that bench.py derives from pq_gemm_tc( plans assumes 128-channel tiles)
+    int stages = 0;
+    for (int c = 0; c < p.g.nChunks; c++) stages += CeilDiv(p.g.chunkCount[c], p.g.GT);
+    snprintf(buf, cap, "pq_gemm_tc_ws(weight-stationary wgmma, weights decoded once per CTA into shared memory, bf16x2) "
+             "N=%d positions=%d KS=%d smem=%zuB grid=%d NPOS=%d chunks=%d stages=%d ksteps=%d",
+             p.g.Kg, p.g.NT, p.g.GT, p.smem, CeilDiv(N * p.g.IB, p.g.NT) * L->grp, p.g.NPOS, p.g.nChunks, stages, p.g.ntab);
     return 0;
   }
   snprintf(buf, cap, "%s CPT=%d J=%d threads=%d smem=%zuB grid=(%d,%d) R=%d strips=%d CT=%d nct=%d PP=%d pwarps=%d "

@@ -1,0 +1,315 @@
+// Strided convolutions over few input channels (the mode-1 geometry of pq_gemm_tc.cu, i.e. conv1: 11x11 / 4 over 3
+// channels) as a weight-stationary GEMM on the Hopper tensor cores, with the roles of pq_gemm_tc transposed:
+//
+//     dst[q][c] = bias[c] + sum_{k-steps} sum_{j<16} X_kstep[q][j] * W_kstep[c][j]       (M = positions, N = channels)
+//
+// A = positions: the bf16x2 phase planes of mode 1 (x = x1 + x2; a 16-byte row holds two phase columns x 4 channels of
+//     one position; K-core-matrix 0 in the x1 plane, 1 in the x2 plane), read by descriptor; a tap is a start-address shift.
+// B = decoded weights in shared memory, N = Cout / grp channels (any instantiated width up to 256: no channel padding).
+//     Per k-step, [w1 | w1] and [w2 | w2] are 16-byte rows per channel; the duplicated half is the same core matrix read
+//     twice (LBO = 0).  Two MMAs per k-step into one accumulator: [x1|x2].[w1|w1] + [x1|x2].[w2|w2] = (x1 + x2)(w1 + w2),
+//     the same k-steps in the same order as mode 1 (the error bound depends on that chain, DESIGN.md 2).
+//
+// Roles inside a CTA of twelve warps:
+//   warps 0-7   two consumer warpgroups; each owns MB m64 blocks of the CTA's 128 MB positions and issues
+//               wgmma.mma_async (both operands in shared memory) into MB accumulators of N / 2 registers per thread.
+//   warps 8-11  producers: stage the position planes of every phase row (global -> bf16x2 split -> planes, all phase rows
+//               resident), and decode the weights of one stage (<= KS k-steps of a phase row, all N channels) from the
+//               pre-split codebook and the channel-major index block into one of two weight buffers.  The decode is done
+//               once per CTA and reused by both warpgroups and every m64 block; decoded weights never reach global memory.
+//   epilogue    the consumers add the bias (+ ReLU) and store pairs of consecutive channels of one NHWC pixel.
+#include "qcnn_internal.h"
+#include "wgmma.h"
+
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+
+namespace {
+
+using qcnn::MbarArrive;
+using qcnn::MbarInit;
+using qcnn::MbarWait;
+using qcnn::SmemU32;
+using qcnn::WgmmaDesc;
+
+constexpr int kWsThreads = 384;
+constexpr int kWsConsumers = 256;   // warps 0-7
+constexpr int kWsProducers = 128;   // warps 8-11
+
+__device__ __forceinline__ uint32_t PackBf16x2(float lo, float hi) {   // low 16 bits = bf16(lo), high 16 bits = bf16(hi)
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+
+// Shared-memory carve, read by the planner (fits / does not fit) and by the kernel.  a.NT = positions per CTA,
+// a.GT = k-steps per weight stage (KS), a.Kg = channels (N of the MMA).
+struct WsSmem {  // byte offsets inside the dynamic shared memory
+  int planes, wts, cb, outoff, bias, bars, total;
+};
+__host__ __device__ inline WsSmem MapWsSmem(const GemmArgs& a) {
+  WsSmem m;
+  int o = 0;
+  m.planes = o; o += a.stride * 2 * a.planeRows * 16;   // [phase row][x1, x2][planeRows] 16-byte rows
+  m.wts = o;    o += 2 * a.GT * 2 * a.Kg * 16;           // [buffer][k-step][w1, w2][channel] 16-byte rows
+  m.cb = o;     o += a.K * 16;                           // pre-split codebook slice: {w1, w2} of the first 4 values
+  m.outoff = o; o += a.NT * 4;                           // destination element offset of every position (-1: none)
+  m.bias = o;   o += a.Kg * 4;                           // (Kg is a multiple of 16: the barriers stay 8-byte aligned)
+  m.bars = o;   o += 8 * (a.stride + 4);
+  m.total = o;
+  return m;
+}
+
+template <int NC, int MB>
+__global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a) {
+  constexpr int P = 128 * MB;   // positions per CTA
+  extern __shared__ __align__(128) unsigned char smem[];
+  const WsSmem sm = MapWsSmem(a);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int st = a.stride, KS = a.GT;
+  uint4* planes = reinterpret_cast<uint4*>(smem + sm.planes);
+  uint4* wts = reinterpret_cast<uint4*>(smem + sm.wts);
+  uint4* cb = reinterpret_cast<uint4*>(smem + sm.cb);
+  int* outoff = reinterpret_cast<int*>(smem + sm.outoff);
+  float* biasS = reinterpret_cast<float*>(smem + sm.bias);
+  uint64_t* fullP = reinterpret_cast<uint64_t*>(smem + sm.bars);   // [st] planes of phase row ph: producers -> consumers
+  uint64_t* fullW = fullP + st;                                     // [2] weight buffer decoded: producers -> consumers
+  uint64_t* emptyW = fullW + 2;                                     // [2] weight buffer's MMAs retired: consumers -> producers
+  const int g = blockIdx.x % a.G, tile = blockIdx.x / a.G;
+  const int Q0 = tile * P;                  // first flat position (phase grid of IB positions per image)
+  const int i0 = Q0 / a.IB;                 // first image touched
+  const float* srcBase = a.src + static_cast<size_t>(i0) * a.srcImg + static_cast<size_t>(g) * a.Cg * a.chStride;
+  float* dstBase = a.dst + static_cast<size_t>(i0) * a.dstImg + g * a.Kg;
+
+  // ---- set-up (all threads) ----
+  for (int p = tid; p < P; p += kWsThreads) {
+    const int Q = Q0 + p;
+    const int i = Q / a.IB, rem = Q - i * a.IB;
+    const int ho = rem / a.PW, wo = rem - ho * a.PW;
+    outoff[p] = (i < a.N && ho < a.Ho && wo < a.Wo) ? (((i - i0) * a.Ho + ho) * a.Wo + wo) * a.Cout : -1;
+  }
+  for (int k = tid; k < a.K; k += kWsThreads) cb[k] = __ldg(reinterpret_cast<const uint4*>(a.ctrd) + k);
+  for (int c = tid; c < a.Kg; c += kWsThreads) biasS[c] = __ldg(a.bias + g * a.Kg + c);
+  if (tid == 0) {
+    for (int i = 0; i < st; i++) MbarInit(fullP + i, kWsProducers);
+    for (int i = 0; i < 2; i++) { MbarInit(fullW + i, kWsProducers); MbarInit(emptyW + i, kWsConsumers / 32); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  const int warpU = __shfl_sync(0xffffffffu, warp, 0);   // provably warp-uniform role selector
+  if (warpU >= kWsConsumers / 32) {
+    // =========================== producers ===========================
+    const int pt = tid - kWsConsumers;
+    int j = 0;   // weight stage counter (buffer j & 1)
+    for (int ph = 0; ph < st; ph++) {
+      // planes of phase row ph: staged float4 p = (phase column pw, position pos) -> pixel (r*stride + ph - pad,
+      // c*stride + pw - pad) of image i; zero outside the image (and beyond the batch)
+      char* x1 = reinterpret_cast<char*>(planes + ph * 2 * a.planeRows);
+      char* x2 = x1 + a.planeRows * 16;
+      for (int p = pt; p < st * a.NPOS; p += kWsProducers) {
+        const int pw = p / a.NPOS, pos = p - pw * a.NPOS;
+        const int F = Q0 + pos;
+        const int i = F / a.IB, rem = F - i * a.IB;
+        const int r = rem / a.PW, c = rem - r * a.PW;
+        const int hi = r * st + ph - a.pad, wi = c * st + pw - a.pad;
+        float4 v = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (i < a.N && static_cast<unsigned>(hi) < static_cast<unsigned>(a.Hi) && static_cast<unsigned>(wi) < static_cast<unsigned>(a.Wi)) {
+          const float* px = srcBase + static_cast<size_t>(i - i0) * a.srcImg + hi * a.rowStride + wi * a.colStride;
+          v.x = __ldg(px);
+          if (a.Cg > 1) v.y = __ldg(px + a.chStride);
+          if (a.Cg > 2) v.z = __ldg(px + 2 * a.chStride);
+          if (a.Cg > 3) v.w = __ldg(px + 3 * a.chStride);
+        }
+        // bf16x2 split: x1 = bf16(x), x2 = bf16(x - x1); row = (pair of phase columns, position), the parity selects the half
+        uint2 p1, p2;
+        p1.x = PackBf16x2(v.x, v.y);
+        p1.y = PackBf16x2(v.z, v.w);
+        p2.x = PackBf16x2(v.x - __uint_as_float(p1.x << 16), v.y - __uint_as_float(p1.x & 0xFFFF0000u));
+        p2.y = PackBf16x2(v.z - __uint_as_float(p1.y << 16), v.w - __uint_as_float(p1.y & 0xFFFF0000u));
+        const int db = ((pw >> 1) * a.NPOS + pos) * 16 + (pw & 1) * 8;
+        *reinterpret_cast<uint2*>(x1 + db) = p1;
+        *reinterpret_cast<uint2*>(x2 + db) = p2;
+      }
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // planes are read by the tensor core
+      MbarArrive(fullP + ph);
+      // weights of the phase row's stages: a thread owns channel c, its index row is [tapsPad] bytes of d_asmt_t
+      const int first = a.chunkFirst[ph], cnt = a.chunkCount[ph];
+      for (int s0 = 0; s0 < cnt; s0 += KS, j++) {
+        const int n = min(KS, cnt - s0), b = j & 1;
+        if (j >= 2) MbarWait<24>(emptyW + b, ((j >> 1) - 1) & 1);   // buffer last read by the MMAs of stage j - 2
+        uint4* w = wts + b * KS * 2 * NC;
+        for (int c = pt; c < NC; c += kWsProducers) {
+          const uint8_t* row = a.asmtT + (static_cast<size_t>(g * st + ph) * a.KgPad + c) * a.tapsPad;
+          // (no unroll pragma here: under `#pragma unroll 3` the compiled loop was seen running an iteration with e == n
+          // for n = 8 on the device, writing past the weight buffer into the codebook / offset regions)
+          for (int e = 0; e < n; e++) {
+            const KStep ks = a.tab[first + s0 + e];
+            const uint4 q0 = cb[__ldg(row + ks.idx0)];
+            const uint4 q1 = ks.cb1 ? make_uint4(0u, 0u, 0u, 0u) : cb[__ldg(row + ks.idx1)];   // unpaired tap: zero half
+            w[(2 * e + 0) * NC + c] = make_uint4(q0.x, q0.y, q1.x, q1.y);   // [w1 of half 0 | w1 of half 1]
+            w[(2 * e + 1) * NC + c] = make_uint4(q0.z, q0.w, q1.z, q1.w);   // [w2 of half 0 | w2 of half 1]
+          }
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        MbarArrive(fullW + b);
+      }
+    }
+    return;
+  }
+
+  // =========================== consumers: wgmma ===========================
+  const int wg = warp >> 2;
+  float acc[MB][NC / 2];
+#pragma unroll
+  for (int m = 0; m < MB; m++)
+#pragma unroll
+    for (int i = 0; i < NC / 2; i++) acc[m][i] = 0.0f;
+  const uint32_t planes0 = SmemU32(planes), wts0 = SmemU32(wts);
+  int j = 0;
+  for (int ph = 0; ph < st; ph++) {
+    MbarWait<24>(fullP + ph, 0);
+    const uint32_t plA = planes0 + static_cast<uint32_t>(ph * 2 * a.planeRows) * 16u + static_cast<uint32_t>(wg * MB * 64) * 16u;
+    const int first = a.chunkFirst[ph], cnt = a.chunkCount[ph];
+    for (int s0 = 0; s0 < cnt; s0 += KS, j++) {
+      const int n = min(KS, cnt - s0), b = j & 1;
+      MbarWait<24>(fullW + b, (j >> 1) & 1);
+      qcnn::WgmmaFence();
+      for (int e = 0; e < n; e++) {
+        const KStep ks = a.tab[first + s0 + e];
+        const uint32_t wb = wts0 + static_cast<uint32_t>((b * KS + e) * 2 * NC) * 16u;
+        const uint64_t d1 = WgmmaDesc(wb, 0, 128), d2 = WgmmaDesc(wb + NC * 16, 0, 128);
+#pragma unroll
+        for (int m = 0; m < MB; m++) {
+          const uint64_t dA = WgmmaDesc(plA + static_cast<uint32_t>(ks.bStart + m * 64) * 16u, static_cast<uint32_t>(a.planeRows) * 16u, 128);
+          qcnn::WgmmaSS<NC>::Bf16(acc[m], dA, d1);
+          qcnn::WgmmaSS<NC>::Bf16(acc[m], dA, d2);
+        }
+      }
+      qcnn::WgmmaCommit();
+      qcnn::WgmmaWaitAll();
+      __syncwarp();
+      if (lane == 0) MbarArrive(emptyW + b);
+    }
+  }
+
+  // ---- epilogue: accumulator fragments (rows = positions r0, r0 + 8; columns = channels 8 i + 2 t4, +1) -> NHWC ----
+  const int r0 = (warp & 3) * 16 + (lane >> 2), t4 = lane & 3;
+  const bool v2 = (reinterpret_cast<uintptr_t>(a.dst) & 7u) == 0;   // (Cout and g * Kg are even: pairs are 8-byte aligned)
+#pragma unroll
+  for (int m = 0; m < MB; m++) {
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int off = outoff[(wg * MB + m) * 64 + r0 + 8 * h];
+      if (off < 0) continue;
+      float* o = dstBase + off;
+#pragma unroll
+      for (int i = 0; i < NC / 8; i++) {
+        const int ch = 8 * i + 2 * t4;
+        float v0 = acc[m][4 * i + 2 * h] + biasS[ch], v1 = acc[m][4 * i + 2 * h + 1] + biasS[ch + 1];
+        if (a.relu) { v0 = fmaxf(v0, 0.0f); v1 = fmaxf(v1, 0.0f); }
+        if (v2) *reinterpret_cast<float2*>(o + ch) = make_float2(v0, v1);
+        else { o[ch] = v0; o[ch + 1] = v1; }
+      }
+    }
+  }
+}
+
+// channel counts with an instantiation: N of the MMA is Cout / grp exactly
+constexpr int kWsWidths[] = {16, 32, 64, 96, 128, 256};
+
+// the dynamic shared-memory limit of an instantiation is raised once per device to the opt-in maximum (as in pq_gemm_tc.cu)
+template <int NC, int MB>
+int SetSmemAndLaunch(const GemmArgs& a, unsigned blocks, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
+  static bool done[64] = {false};
+  if (ctx->device < 0 || ctx->device >= 64 || !done[ctx->device]) {
+    const int lim = static_cast<int>(ctx->smem_optin ? ctx->smem_optin : 227 * 1024);
+    QCNN_CUDA(cudaFuncSetAttribute(conv_ws_kernel<NC, MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    if (ctx->device >= 0 && ctx->device < 64) done[ctx->device] = true;
+  }
+  conv_ws_kernel<NC, MB><<<blocks, kWsThreads, smem, st>>>(a);
+  QCNN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+}  // namespace
+
+namespace qcnn {
+
+// Candidate tilings for batch N (cost in SM-cycles, the scale of PlanPqGemm's model): positions per CTA x k-steps per
+// weight stage.  Eligible: the mode-1 geometry with bf16x2 operands, an instantiated channel width, the pre-split
+// codebook and the channel-major index block.
+void PlanConvWs(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands) {
+  const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, st = L->stride;
+  if (!L->opt_tc_bf || st < 2 || st > 4 || (st & 1) || L->K < 1 || L->K > 256) return;
+  if (Cg > 4 || L->S != 1 || L->d < Cg || L->d % 4 != 0 || !L->d_ctrd_bf.get() || !L->d_asmt_t.get() || L->asmt_t_mode != 1) return;
+  if (std::find(std::begin(kWsWidths), std::end(kWsWidths), Kg) == std::end(kWsWidths)) return;
+  const int PWp = CeilDiv(L->Win + 2 * L->pad, st), PHp = CeilDiv(L->Hin + 2 * L->pad, st);
+  if (L->Wo > PWp) return;
+  const int IB = PHp * PWp;
+  if (static_cast<double>(N) * IB > 2.0e9 || static_cast<double>(L->Hin) * L->Win * L->Cin * 4 > 2.0e9) return;
+  const size_t smemMax = L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024;
+  for (int MB = 2; MB >= 1; MB--) {
+    if (MB == 2 && Kg > 128) continue;   // (2 x 128 accumulator registers do not fit)
+    const int P = 128 * MB;
+    ConvPlan p;
+    memset(&p, 0, sizeof(p));
+    p.kernel = kConvWs; p.CPT = P; p.threads = kWsThreads;
+    GemmArgs& ga = p.g;
+    ga.mode = 1; ga.bf = 1;
+    ga.PW = PWp; ga.IB = IB; ga.NT = P;
+    ga.NPOS = RoundUp(P + ((L->ksz - 1) / st) * (PWp + 1), 8);
+    ga.planeRows = (st / 2) * ga.NPOS;
+    ga.planeF4 = st * ga.NPOS;
+    ga.nChunks = st; ga.nct = 1; ga.nsplit = 1;
+    ga.stride = st; ga.Kg = Kg; ga.K = L->K;
+    ga.tapsPad = RoundUp(CeilDiv(L->ksz, st) * L->ksz, 16);
+    const int ne = Mode1Table(L, ga);
+    if (ne > kMaxKSteps) continue;
+    int maxCnt = 0;
+    for (int ph = 0; ph < st; ph++) maxCnt = std::max(maxCnt, ga.chunkCount[ph]);
+    // k-steps per weight stage: a whole phase row when it fits, else the largest count that does
+    for (ga.GT = maxCnt; ga.GT >= 1 && static_cast<size_t>(MapWsSmem(ga).total) > smemMax; ga.GT--) {}
+    if (ga.GT < 1) continue;
+    p.smem = static_cast<size_t>(MapWsSmem(ga).total);
+    p.J = ga.GT;
+    p.a.CT = Kg; p.a.nct = 1; p.a.R = P; p.a.nstrips = ga.GT; p.a.rgroups = 1;
+    int stages = 0;
+    for (int ph = 0; ph < st; ph++) stages += CeilDiv(ga.chunkCount[ph], ga.GT);
+    // tensor work on PlanPqGemm's scale (its 4 MMAs of m64 n128 k16 per k-step cost 3 * 64 * 1.15), a pipeline drain per
+    // weight stage, the set-up and the staging of the first phase row
+    const double perCta = ne * 2.0 * (P / 64) * (Kg / 128.0) * (3.0 * 64.0 * 1.15 / 4.0) + 600.0 * stages + 9000.0 + P * 24.0;
+    const double ctas = static_cast<double>(CeilDiv(N * IB, P)) * G;
+    cands->emplace_back(perCta * std::ceil(ctas / L->ctx->sm_count), p);
+  }
+}
+
+int LaunchConvWs(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
+  GemmArgs a = p.g;
+  a.src = src; a.dst = dst; a.ctrd = L->d_ctrd_bf.as<float>(); a.bias = L->d_bias.as<float>();
+  a.asmtT = L->d_asmt_t.as<uint8_t>();
+  a.N = N; a.relu = relu;
+  a.Hi = L->Hin; a.Wi = L->Win; a.Cin = L->Cin; a.Ho = L->Ho; a.Wo = L->Wo; a.Cout = L->Cout;
+  a.ksz = L->ksz; a.pad = L->pad; a.stride = L->stride; a.G = L->grp; a.Cg = L->Cin / L->grp; a.Kg = L->Cout / L->grp;
+  a.KgPad = RoundUp(a.Kg, 16); a.S = L->S; a.K = L->K; a.d = L->d;
+  a.srcImg = static_cast<long long>(a.Hi) * a.Wi * a.Cin;
+  if (L->src_nchw) { a.rowStride = a.Wi; a.colStride = 1; a.chStride = a.Hi * a.Wi; }
+  else { a.rowStride = a.Wi * a.Cin; a.colStride = a.Cin; a.chStride = 1; }
+  a.dstImg = static_cast<long long>(a.Ho) * a.Wo * a.Cout;
+  const long long blocks = static_cast<long long>(CeilDiv(N * a.IB, a.NT)) * a.G;
+  QCNN_CHECK(blocks <= 2147483647LL, "qcnn_conv_aprx_forward: batch too large for the weight-stationary tiling");
+  QCNN_CHECK(static_cast<size_t>(MapWsSmem(a).total) == p.smem, "internal: conv_ws shared-memory carve changed after planning");
+  qcnn_ctx* ctx = L->ctx;
+  const unsigned nb = static_cast<unsigned>(blocks);
+#define QCNN_WS(NC)                                                                        \
+  if (a.Kg == NC) return a.NT == 256 ? SetSmemAndLaunch<NC, 2>(a, nb, p.smem, st, ctx)     \
+                                     : SetSmemAndLaunch<NC, 1>(a, nb, p.smem, st, ctx);
+  QCNN_WS(16) QCNN_WS(32) QCNN_WS(64) QCNN_WS(96) QCNN_WS(128)
+#undef QCNN_WS
+  if (a.Kg == 256 && a.NT == 128) return SetSmemAndLaunch<256, 1>(a, nb, p.smem, st, ctx);
+  SetError("internal: no conv_ws instantiation for N=%d positions=%d", a.Kg, a.NT);
+  return 1;
+}
+
+}  // namespace qcnn

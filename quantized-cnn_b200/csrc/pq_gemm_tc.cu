@@ -176,6 +176,40 @@ __global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_packed_kernel(const Ge
 
 namespace qcnn {
 
+// Mode 1 k-step table (strided layer on phase planes): for every phase row ph, its k-steps in (kh, kw) order, as entries
+// [chunkFirst[ph], + chunkCount[ph]) of ga.tab.  Reads ga.NPOS, ga.bf and ga.planeRows.  Returns the number of k-steps
+// (> kMaxKSteps: the table does not fit) and sets ga.ntab.  The weight-stationary kernel (conv_ws.cu) runs the same table.
+int Mode1Table(const qcnn_layer* L, GemmArgs& ga) {
+  const int st = L->stride, PWp = CeilDiv(L->Win + 2 * L->pad, st);
+  int ne = 0;
+  for (int ph = 0; ph < st; ph++) {
+    ga.chunkFirst[ph] = ne;
+    for (int kh = ph; kh < L->ksz; kh += st)
+      for (int kw = 0; kw < L->ksz; kw += 2, ne++) {
+        if (ne >= kMaxKSteps) { ne = kMaxKSteps + 1000; break; }
+        KStep& ks = ga.tab[ne];
+        // partner in the next phase column, same shift (bf16x2: the partner must be the odd column of the same pair)
+        const bool paired = kw + 1 < L->ksz && (kw % st) + 1 < st && !(ga.bf && ((kw % st) & 1));
+        ks.bStart = (kw % st) * ga.NPOS + (kh / st) * PWp + kw / st;
+        // an unpaired tap's second half (zero codebook slot) aliases its first half (LBO = 0): a shift would read
+        // the next position -- for a tile's last position, or a tap at the end of an image, another image's
+        // pixel -- and 0 * NaN / Inf would carry that image's non-finite values into this one's output
+        ks.lbo = paired ? ga.NPOS : 0;
+        if (ga.bf) {   // row = (pair of phase columns, position); K-core-matrix 1 = the x2 plane
+          ks.bStart = ((kw % st) >> 1) * ga.NPOS + (kh / st) * PWp + kw / st;
+          ks.lbo = ga.planeRows;
+        }
+        ks.idx0 = static_cast<short>((kh - ph) / st * L->ksz + kw);
+        ks.idx1 = static_cast<short>(paired ? ks.idx0 + 1 : ks.idx0);
+        ks.cb0 = 0; ks.cb1 = paired ? 0 : 1;
+        if (!paired && kw + 1 < L->ksz) kw--;   // the partner starts its own k-step
+      }
+    ga.chunkCount[ph] = ne - ga.chunkFirst[ph];
+  }
+  ga.ntab = ne;
+  return ne;
+}
+
 // Candidate tilings for batch N (cost in SM-cycles, comparable with PlanConv's model); on-device timing chooses among them.
 void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands) {
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, taps = L->ksz * L->ksz;
@@ -219,33 +253,8 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
         // never wait for the MMAs and the few k-steps of a phase row (conv1: 16-18) are not what hides a global-load latency
         if (ga.bf && st <= 4) ga.nPB = st;
         ga.nct = CeilDiv(Kg, 128);
-        int ne = 0;
-        for (int ph = 0; ph < st; ph++) {
-          ga.chunkFirst[ph] = ne;
-          for (int kh = ph; kh < L->ksz; kh += st)
-            for (int kw = 0; kw < L->ksz; kw += 2, ne++) {
-              if (ne >= kMaxKSteps) { ne = kMaxKSteps + 1000; break; }
-              KStep& ks = ga.tab[ne];
-              // partner in the next phase column, same shift (bf16x2: the partner must be the odd column of the same pair)
-              const bool paired = kw + 1 < L->ksz && (kw % st) + 1 < st && !(ga.bf && ((kw % st) & 1));
-              ks.bStart = (kw % st) * ga.NPOS + (kh / st) * PWp + kw / st;
-              // an unpaired tap's second half (zero codebook slot) aliases its first half (LBO = 0): a shift would read
-              // the next position -- for a tile's last position, or a tap at the end of an image, another image's
-              // pixel -- and 0 * NaN / Inf would carry that image's non-finite values into this one's output
-              ks.lbo = paired ? ga.NPOS : 0;
-              if (ga.bf) {   // row = (pair of phase columns, position); K-core-matrix 1 = the x2 plane
-                ks.bStart = ((kw % st) >> 1) * ga.NPOS + (kh / st) * PWp + kw / st;
-                ks.lbo = ga.planeRows;
-              }
-              ks.idx0 = static_cast<short>((kh - ph) / st * L->ksz + kw);
-              ks.idx1 = static_cast<short>(paired ? ks.idx0 + 1 : ks.idx0);
-              ks.cb0 = 0; ks.cb1 = paired ? 0 : 1;
-              if (!paired && kw + 1 < L->ksz) kw--;   // the partner starts its own k-step
-            }
-          ga.chunkCount[ph] = ne - ga.chunkFirst[ph];
-        }
+        const int ne = Mode1Table(L, ga);
         if (ne > kMaxKSteps) continue;
-        ga.ntab = ne;
         p.smem = static_cast<size_t>(MapSmem(ga).total);
         if (p.smem > smemMax0) continue;
         p.a.CT = 128; p.a.nct = ga.nct; p.a.R = NT; p.a.nstrips = GT;

@@ -335,7 +335,7 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
   }
   else if (!strcmp(name, "force_kernel") || !strcmp(name, "autotune") || !strcmp(name, "gemm_nt") ||
            !strcmp(name, "gemm_gt") || !strcmp(name, "gemm_nsplit")) {
-    // conv only.  force_kernel: -1 none, else 0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc;
+    // conv only.  force_kernel: -1 none, else 0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc | 7 conv_ws;
     // autotune: 0 keeps the cost model's first tiling instead of timing the candidates on the device;
     // gemm_nt: positions per CTA of the pq_gemm_tc tilings (0 = any; 128 = one accumulator, 64 = two);
     // gemm_gt: k-steps per stage of those tilings (0 = any; 4 or 3); gemm_nsplit: their K-split factor (0 = any; 1 = no

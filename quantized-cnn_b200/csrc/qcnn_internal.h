@@ -225,7 +225,8 @@ enum ConvKernel {
   kConvRollTc = 3,    // as kConvRoll with the 3xTF32 wgmma LUT stage
   kConvDirect = 4,    // single narrow subspace, codewords evaluated at the point of use
   kPqGemmTc = 6,      // decode-at-use GEMMs on wgmma (pq_gemm_tc.cu)
-  kConvKernelIds = 7
+  kConvWs = 7,        // strided narrow-input layers (mode-1 geometry, bf16x2) as a weight-stationary wgmma GEMM (conv_ws.cu)
+  kConvKernelIds = 8
 };
 
 struct ConvPlan {
@@ -234,7 +235,7 @@ struct ConvPlan {
   int threads;
   size_t smem;
   ConvArgs a;           // geometry + tiling (pointers/N filled at launch)
-  GemmArgs g;           // kernel 6 (pq_gemm_tc)
+  GemmArgs g;           // kernels 6 (pq_gemm_tc) and 7 (conv_ws)
 };
 
 struct qcnn_layer {
@@ -303,6 +304,10 @@ int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows,
 void DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap);
 int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled);
 int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
+int Mode1Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a strided layer on bf16x2 / tf32 phase planes
+// conv_ws.cu: the tensor-core family's weight-stationary tilings of strided narrow-input layers (mode-1 geometry)
+void PlanConvWs(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands);
+int LaunchConvWs(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
 
 int LaunchRelu(qcnn_ctx* ctx, const float* src, float* dst, size_t n, cudaStream_t st);
 int LaunchLrn(qcnn_ctx* ctx, const float* src, float* dst, size_t pixels, int C, int size, float alpha, float beta,
