@@ -77,11 +77,11 @@ QCNN_API int qcnn_conv_layer_set_src_nchw(qcnn_layer* layer, int enable);
  * run as decode-at-use GEMMs on the tensor cores with bf16x2 operands; 1 = the same GEMMs with 3xTF32 operands; 0 = LUT +
  * gather kernels only, the fp32 strict-parity path -- tolerances of all three in DESIGN.md);
  * conv layers, for tests that must know which kernel they check: "force_kernel" (-1 none | 0 s1 | 1 roll | 2 s1_tc |
- * 3 roll_tc | 4 direct | 6 pq_gemm_tc | 7 conv_ws: strided layers over <= 4 input channels per group with bf16x2 operands
- * (tensor_core = 2) as a weight-stationary GEMM, N = Cout/grp in {16, 32, 64, 96, 128, 256}; describe() names it
- * pq_gemm_tc_ws), "gemm_nt" (positions per CTA of the pq_gemm_tc tilings, and 128 / 256 for conv_ws; 0 = any), "gemm_gt"
- * (k-steps per stage of those tilings, 0 = any), "gemm_nsplit" (their K-split factor, 0 = any; a pq_gemm_tc pin that no
- * tiling of the layer matches makes the forward fail), "autotune"
+ * 3 roll_tc | 4 direct | 6 pq_gemm_tc | 7 conv_ws: stride-1 layers (NHWC source) and strided layers over <= 4 input
+ * channels per group, with bf16x2 operands (tensor_core = 2), as a weight-stationary GEMM whose N is the channels of one
+ * CTA: Cout/grp or a tile of it, in {16, 32, 64, 96, 128, 192, 256}; describe() names it pq_gemm_tc_ws), "gemm_nt" (positions per CTA of the pq_gemm_tc tilings, and 128 / 256 for conv_ws; 0 = any), "gemm_gt"
+ * (k-steps per stage of those tilings, 0 = any), "gemm_nsplit" (their K-split factor, 0 = any), "gemm_ct" (channels per
+ * CTA of the conv_ws tilings, 0 = any; a pin that no tiling of the layer matches makes the forward fail), "autotune"
  * (0 = keep the cost model's first tiling instead of timing the candidates of the chosen family on the device);
  * FC layers only: "asmt_packed" (1 = keep the assignment table in device memory bit-packed at b = log2(K) bits per
  * index instead of one byte, and unpack it inside the FC kernels; 0 = the byte table, the default).  Switching repacks the

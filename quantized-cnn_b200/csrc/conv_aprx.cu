@@ -1008,11 +1008,12 @@ int PlanConv(qcnn_layer* L, int N) {
       }
     }
   }
-  // tensor-core GEMMs: decode-at-use pq_gemm_tc.cu and, for strided narrow-input layers with bf16x2 operands, the
-  // weight-stationary conv_ws.cu.  The operand format is a setting, not a timing result: with tensor_core = 2 (default,
-  // bf16x2) or 1 (3xTF32) an eligible layer always runs one of these GEMMs (tolerances in DESIGN.md 2), with
+  // tensor-core GEMMs: decode-at-use pq_gemm_tc.cu and, with bf16x2 operands, the weight-stationary conv_ws.cu (stride-1
+  // layers and strided narrow-input layers).  The operand format is a setting, not a timing result: with tensor_core = 2
+  // (default, bf16x2) or 1 (3xTF32) an eligible layer always runs one of these GEMMs (tolerances in DESIGN.md 2), with
   // tensor_core = 0 always the LUT + gather kernels.  On-device timing chooses among the GEMM tilings of that format --
-  // for a conv1-type layer at bf16x2 between conv_ws and pq_gemm_tc mode 1, which share the k-step chain and its bound.
+  // at bf16x2 between conv_ws and pq_gemm_tc of the same geometry (mode 0 / mode 1 at NT = 128), which share the k-step
+  // chain and its bound.
   if (!L->opt_no_tc) {
     std::vector<std::pair<double, ConvPlan>> tc;
     PlanPqGemm(L, N, &tc);
@@ -1038,20 +1039,7 @@ int PlanConv(qcnn_layer* L, int N) {
       if (!IsGemmTc(c.second.kernel) && kConvKernelInfo[c.second.kernel].tcLut == want) kept.push_back(c);
     cands.swap(kept);
   }
-  // layer parameters "gemm_nt" / "gemm_gt" / "gemm_nsplit": only pq_gemm_tc tilings with that many positions per CTA,
-  // k-steps per stage and K-split factor (0 = any); "gemm_nt" also restricts the positions per CTA of conv_ws
-  if (L->opt_gemm_nt || L->opt_gemm_gt || L->opt_gemm_nsplit) {
-    std::vector<std::pair<double, ConvPlan>> kept;
-    for (const auto& c : cands)
-      if ((c.second.kernel == kConvWs && (!L->opt_gemm_nt || c.second.g.NT == L->opt_gemm_nt)) ||
-          (c.second.kernel != kPqGemmTc && c.second.kernel != kConvWs) ||
-          ((!L->opt_gemm_nt || c.second.g.NT == L->opt_gemm_nt) && (!L->opt_gemm_gt || c.second.g.GT == L->opt_gemm_gt) &&
-           (!L->opt_gemm_nsplit || c.second.g.nsplit == L->opt_gemm_nsplit)))
-        kept.push_back(c);
-    QCNN_CHECK(!kept.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d gemm_gt=%d gemm_nsplit=%d has no tiling for this layer at "
-               "batch %d", L->opt_gemm_nt, L->opt_gemm_gt, L->opt_gemm_nsplit, N);
-    cands.swap(kept);
-  }
+  // (the family first: a gemm_* pin that no tiling of the pinned family matches is reported as such)
   const char* force = getenv("QCNN_FORCE_KERNEL");
   if (L->opt_force_kernel || force) {
     const int want = L->opt_force_kernel ? L->opt_force_kernel - 1 : atoi(force);
@@ -1059,6 +1047,23 @@ int PlanConv(qcnn_layer* L, int N) {
     for (const auto& c : cands) if (c.second.kernel == want) kept.push_back(c);
     QCNN_CHECK(!kept.empty() || !L->opt_force_kernel, "qcnn_conv_aprx_forward: force_kernel=%d has no tiling for this layer at batch %d", want, N);
     if (!kept.empty()) cands.swap(kept);
+  }
+  // layer parameters "gemm_nt" / "gemm_gt" / "gemm_nsplit": only pq_gemm_tc tilings with that many positions per CTA,
+  // k-steps per stage and K-split factor (0 = any); "gemm_nt" also restricts the positions per CTA of conv_ws, and
+  // "gemm_ct" its channels per CTA
+  if (L->opt_gemm_nt || L->opt_gemm_gt || L->opt_gemm_nsplit || L->opt_gemm_ct) {
+    std::vector<std::pair<double, ConvPlan>> kept;
+    for (const auto& c : cands)
+      if ((c.second.kernel == kConvWs && (!L->opt_gemm_nt || c.second.g.NT == L->opt_gemm_nt) &&
+           (!L->opt_gemm_ct || c.second.g.Kg / c.second.g.nct == L->opt_gemm_ct)) ||
+          (c.second.kernel != kPqGemmTc && c.second.kernel != kConvWs) ||
+          (c.second.kernel == kPqGemmTc && (!L->opt_gemm_nt || c.second.g.NT == L->opt_gemm_nt) &&
+           (!L->opt_gemm_gt || c.second.g.GT == L->opt_gemm_gt) &&
+           (!L->opt_gemm_nsplit || c.second.g.nsplit == L->opt_gemm_nsplit)))
+        kept.push_back(c);
+    QCNN_CHECK(!kept.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d gemm_gt=%d gemm_nsplit=%d gemm_ct=%d has no tiling for this "
+               "layer at batch %d", L->opt_gemm_nt, L->opt_gemm_gt, L->opt_gemm_nsplit, L->opt_gemm_ct, N);
+    cands.swap(kept);
   }
   // every kernel family that has a feasible tiling gets at least two seats among the candidates
   for (int pass = 0; pass < 2; pass++) {
@@ -1188,6 +1193,16 @@ int DescribeConv(qcnn_layer* L, int N, char* buf, size_t cap) {
              "chunks=%d ksteps=%d nsplit=%d", p.g.bf ? ", bf16x2" : "", p.g.mode, p.g.NT, p.g.GT, p.smem,
              CeilDiv(N * p.g.IB, p.g.NT) * L->grp * p.g.nct * std::max(1, p.g.nsplit), p.g.NPOS, p.g.nChunks,
              ksteps / std::max(1, p.g.nsplit), std::max(1, p.g.nsplit));
+    return 0;
+  }
+  if (p.kernel == kConvWs && p.g.mode == 0) {
+    // stride 1: N = channels per CTA, ctiles = channel tiles per group, ksteps = chunks x taps (a CTA's k-steps), so
+    // that grid x ksteps x 32 x positions x N is the executed MAC count
+    const int stages = p.g.nChunks * CeilDiv(p.g.ntab, p.g.GT);
+    snprintf(buf, cap, "pq_gemm_tc_ws(weight-stationary wgmma, weights decoded once per CTA into shared memory, bf16x2) "
+             "mode=0 N=%d positions=%d ctiles=%d KS=%d smem=%zuB grid=%d NPOS=%d planebufs=%d chunks=%d stages=%d ksteps=%d",
+             p.g.Kg / p.g.nct, p.g.NT, p.g.nct, p.g.GT, p.smem, CeilDiv(N * p.g.IB, p.g.NT) * L->grp * p.g.nct, p.g.NPOS,
+             p.g.nPB, p.g.nChunks, stages, p.g.nChunks * p.g.ntab);
     return 0;
   }
   if (p.kernel == kConvWs) {

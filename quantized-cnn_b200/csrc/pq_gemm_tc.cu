@@ -210,6 +210,24 @@ int Mode1Table(const qcnn_layer* L, GemmArgs& ga) {
   return ne;
 }
 
+// Mode 0 k-step table (stride-1 layer on the flat padded grid): the taps of a chunk in (kh, kw) order, a tap being a shift
+// of the position operand's start by kh * PW + kw rows, K-core-matrix 1 (the chunk's second half / the x2 plane) NPOS rows
+// further; index row and codebook slot = (half, tap).  Reads ga.PW and ga.NPOS, sets ga.ntab and the chunk range, returns
+// the number of k-steps per chunk.  The weight-stationary kernel (conv_ws.cu) runs the same table.
+int Mode0Table(const qcnn_layer* L, GemmArgs& ga) {
+  const int taps = L->ksz * L->ksz;
+  ga.ntab = taps;
+  ga.chunkFirst[0] = 0; ga.chunkCount[0] = taps;
+  for (int t = 0; t < taps; t++) {
+    KStep& ks = ga.tab[t];
+    ks.bStart = (t / L->ksz) * ga.PW + (t % L->ksz);
+    ks.lbo = ga.NPOS;
+    ks.idx0 = static_cast<short>(t); ks.idx1 = static_cast<short>(taps + t);
+    ks.cb0 = 0; ks.cb1 = 1;
+  }
+  return taps;
+}
+
 // Candidate tilings for batch N (cost in SM-cycles, comparable with PlanConv's model); on-device timing chooses among them.
 void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands) {
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, taps = L->ksz * L->ksz;
@@ -304,15 +322,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
       ga.idxT = (ga.tapsPad <= 32 && L->d_asmt_t.get() && L->asmt_t_mode == 0) ? 1 : 0;
       if (ga.idxT) ga.idRows = 2 * ga.tapsPad;      // [half][128 channels][tapsPad] bytes = 2 * tapsPad rows of 128
       ga.nChunks = CeilDiv(Cg, 8);
-      ga.ntab = taps;
-      ga.chunkFirst[0] = 0; ga.chunkCount[0] = taps;
-      for (int t = 0; t < taps; t++) {
-        KStep& ks = ga.tab[t];
-        ks.bStart = (t / L->ksz) * PW + (t % L->ksz);
-        ks.lbo = ga.NPOS;
-        ks.idx0 = static_cast<short>(t); ks.idx1 = static_cast<short>(taps + t);
-        ks.cb0 = 0; ks.cb1 = 1;
-      }
+      Mode0Table(L, ga);
       ga.K = L->K; ga.cbF4 = L->K; ga.nPB = 2;
       ga.nct = CeilDiv(Kg, 128);
       p.smem = static_cast<size_t>(MapSmem(ga).total);

@@ -334,17 +334,19 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
     L->tunedPlans.clear();
   }
   else if (!strcmp(name, "force_kernel") || !strcmp(name, "autotune") || !strcmp(name, "gemm_nt") ||
-           !strcmp(name, "gemm_gt") || !strcmp(name, "gemm_nsplit")) {
+           !strcmp(name, "gemm_gt") || !strcmp(name, "gemm_nsplit") || !strcmp(name, "gemm_ct")) {
     // conv only.  force_kernel: -1 none, else 0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc | 7 conv_ws;
     // autotune: 0 keeps the cost model's first tiling instead of timing the candidates on the device;
     // gemm_nt: positions per CTA of the pq_gemm_tc tilings (0 = any; 128 = one accumulator, 64 = two);
     // gemm_gt: k-steps per stage of those tilings (0 = any; 4 or 3); gemm_nsplit: their K-split factor (0 = any; 1 = no
-    // split, > 1 = partial sums reduced by a second kernel).  A pin that no tiling of the layer matches fails the forward.
+    // split, > 1 = partial sums reduced by a second kernel); gemm_ct: channels per CTA of the conv_ws tilings (0 = any).
+    // A pin that no tiling of the layer matches fails the forward.
     QCNN_CHECK(L->kind == QCNN_KIND_CONV, "qcnn_layer_set_param: '%s' applies to conv layers", name);
     if (name[0] == 'f') L->opt_force_kernel = value < 0 ? 0 : value + 1;
     else if (!strcmp(name, "gemm_nt")) L->opt_gemm_nt = value < 0 ? 0 : value;
     else if (!strcmp(name, "gemm_gt")) L->opt_gemm_gt = value < 0 ? 0 : value;
     else if (!strcmp(name, "gemm_nsplit")) L->opt_gemm_nsplit = value < 0 ? 0 : value;
+    else if (!strcmp(name, "gemm_ct")) L->opt_gemm_ct = value < 0 ? 0 : value;
     else L->opt_no_autotune = value ? 0 : 1;
     L->plan_N = 0; L->tuned = 0;
     L->tunedPlans.clear();

@@ -192,7 +192,7 @@ struct GemmArgs {
   int kshift;                   // stored assignment byte = index << kshift
   float* partial;               // mode 2, nsplit > 1: [nsplit][N][dstRow]
   int dstRow;                   // mode 2: floats per destination row
-  int nPB;                      // position-plane buffers (2; 3 for mode 2, whose planes arrive by bulk copy)
+  int nPB;                      // position-plane buffers (2; 3 for mode 2, whose planes arrive by bulk copy; conv_ws: its ring / phase rows)
   const float* xprep;           // mode 2: activations pre-split into the plane image (fc_prep_kernel), [tile][chunk][hi,lo][2KS][NT][4]
   int nChunksAll;               // mode 2: chunks of the whole layer (xprep indexing)
   int cbF4;                     // float4 per codebook slot (K for d % 4 == 0 pieces, K/4 for d == 1 scalars)
@@ -210,7 +210,7 @@ struct GemmArgs {
   int cbSlots, idRows;        // codebook slices / index rows staged per chunk
   int nChunks;
   int GT;                     // k-steps per stage (decoded into registers together, <= 4)
-  int nct;                    // 128-channel tiles per group
+  int nct;                    // channel tiles per group (pq_gemm_tc: of 128 channels; conv_ws: of Kg / nct channels)
   int relu;
   int ntab;
   int chunkFirst[8], chunkCount[8];   // k-step table range of a chunk (mode 1: per phase row; else entry 0)
@@ -225,7 +225,7 @@ enum ConvKernel {
   kConvRollTc = 3,    // as kConvRoll with the 3xTF32 wgmma LUT stage
   kConvDirect = 4,    // single narrow subspace, codewords evaluated at the point of use
   kPqGemmTc = 6,      // decode-at-use GEMMs on wgmma (pq_gemm_tc.cu)
-  kConvWs = 7,        // strided narrow-input layers (mode-1 geometry, bf16x2) as a weight-stationary wgmma GEMM (conv_ws.cu)
+  kConvWs = 7,        // stride-1 and strided narrow-input layers (bf16x2) as a weight-stationary wgmma GEMM (conv_ws.cu)
   kConvKernelIds = 8
 };
 
@@ -280,6 +280,7 @@ struct qcnn_layer {
   int opt_gemm_nt = 0;       // conv: restrict pq_gemm_tc tilings to this many positions per CTA (0 = any)
   int opt_gemm_gt = 0;       // conv: ... to this many k-steps per stage (0 = any)
   int opt_gemm_nsplit = 0;   // conv: ... to this K-split factor (0 = any)
+  int opt_gemm_ct = 0;       // conv: restrict conv_ws tilings to this many channels per CTA (0 = any)
 };
 
 namespace qcnn {
@@ -304,8 +305,10 @@ int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows,
 void DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap);
 int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled);
 int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
+int Mode0Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a stride-1 layer on the flat padded grid
 int Mode1Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a strided layer on bf16x2 / tf32 phase planes
-// conv_ws.cu: the tensor-core family's weight-stationary tilings of strided narrow-input layers (mode-1 geometry)
+// conv_ws.cu: the tensor-core family's weight-stationary tilings of stride-1 layers (mode-0 geometry, channel tiles) and
+// of strided narrow-input layers (mode-1 geometry)
 void PlanConvWs(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands);
 int LaunchConvWs(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
 
