@@ -77,7 +77,8 @@ QCNN_API int qcnn_conv_layer_set_src_nchw(qcnn_layer* layer, int enable);
  * run as decode-at-use GEMMs on the tensor cores with bf16x2 operands; 1 = the same GEMMs with 3xTF32 operands; 0 = LUT +
  * gather kernels only, the fp32 strict-parity path -- tolerances of all three in DESIGN.md);
  * conv layers, for tests that must know which kernel they check: "force_kernel" (-1 none | 0 s1 | 1 roll | 2 s1_tc |
- * 3 roll_tc | 4 direct | 6 pq_gemm_tc | 7 conv_ws: stride-1 layers (NHWC source) and strided layers over <= 4 input
+ * 3 roll_tc | 4 direct | 6 pq_gemm_tc | 7 conv_ws: stride-1 layers (NHWC source; Cg % 4 == 0 or Cg <= 3, d % 4 == 0,
+ * S*d >= Cg, <= 32 taps, any width whose plane ring fits in shared memory) and strided layers over <= 4 input
  * channels per group, with bf16x2 operands (tensor_core = 2), as a weight-stationary GEMM whose N is the channels of one
  * CTA: Cout/grp or a tile of it, in {16, 32, 64, 96, 128, 192, 256}; describe() names it pq_gemm_tc_ws), "gemm_nt" (positions per CTA of the pq_gemm_tc tilings, and 128 / 256 for conv_ws; 0 = any), "gemm_gt"
  * (k-steps per stage of those tilings, 0 = any), "gemm_nsplit" (their K-split factor, 0 = any), "gemm_ct" (channels per

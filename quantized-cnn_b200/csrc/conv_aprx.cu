@@ -541,7 +541,13 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_kernel(const ConvArgs a) {
   const int warp = tid >> 5, lane = tid & 31;
   const int pw = warp % a.pwarps, cw = warp / a.pwarps;
   const CtaTile t(a);
-  const int r0 = t.strip * a.R;            // first output row of the strip
+  // strip = row strip x ncol + column tile.  Whole rows (ncol = 1) share their padding: the right padding of a row is
+  // the left padding of the next (pitch Win + pad, positions shifted by pad).  A column tile (rows wider than a LUT
+  // holds) has pitch CW + ksz - 1 with its own left halo.
+  const int r0 = (t.strip / a.ncol) * a.R;   // first output row of the strip
+  const int c0 = (t.strip % a.ncol) * a.CW;  // first output column of the tile
+  const int shift = a.ncol > 1 ? 0 : a.pad, wi0 = a.ncol > 1 ? c0 - a.pad : 0;
+  const int Wt = a.ncol > 1 ? min(a.CW, a.Wo - c0) : a.Wo;   // output columns of the tile
   const int hin0 = r0 - a.pad;             // input row held at ri = 0
   const int q0 = pw * 32 * J + lane;       // first flat position of this thread (others at +32 j)
   const int cbase = t.ct * a.CT + cw * CPT;  // first channel (within the group) of this thread
@@ -551,11 +557,11 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_kernel(const ConvArgs a) {
   // LUT position -> source pixel (NHWC element offset within this image/group), -1 = zero padding
   for (int pos = tid; pos < lut.npos; pos += T) {
     int off = -1;
-    const int pp = pos - a.pad;
+    const int pp = pos - shift;
     if (pp >= 0) {
-      const int ri = pp / a.PW, wi = pp - ri * a.PW;
+      const int ri = pp / a.PW, wi = wi0 + pp - ri * a.PW;
       const int hi = hin0 + ri;
-      if (ri < a.RI && wi < a.Wi && hi >= 0 && hi < a.Hi) off = (hi * a.Wi + wi) * a.Cin;
+      if (ri < a.RI && wi >= 0 && wi < a.Wi && hi >= 0 && hi < a.Hi) off = (hi * a.Wi + wi) * a.Cin;
     }
     lut.posoff[pos] = off;
   }
@@ -591,8 +597,8 @@ __global__ void __launch_bounds__(MAXT, 1) conv_s1_kernel(const ConvArgs a) {
     const int q = q0 + 32 * j;
     const int r = q / a.PW, wo = q - r * a.PW;
     const int ho = r0 + r;
-    if (r < a.R && wo < a.Wo && ho < a.Ho) {
-      float* out = a.dst + ((static_cast<size_t>(t.n) * a.Ho + ho) * a.Wo + wo) * a.Cout + t.g * a.Kg + cbase;
+    if (r < a.R && wo < Wt && ho < a.Ho) {
+      float* out = a.dst + ((static_cast<size_t>(t.n) * a.Ho + ho) * a.Wo + c0 + wo) * a.Cout + t.g * a.Kg + cbase;
       StoreChannels<CPT, J>(out, acc, j, a.relu);
     }
   }
@@ -878,6 +884,8 @@ int PlanConv(qcnn_layer* L, int N) {
   // tensor-core LUT stage: 128 codewords (MMA M), every subspace <= 8 dims (one K = 8 tf32 step)
   const bool tcOk = L->K == 128 && L->d <= 8;
   const int cpts[2] = {32, 16};
+  // stride 1: whole rows per CTA; column tiles (ncol > 1) only for layers whose rows fit no LUT (VGG16's 224-wide block 1)
+  for (int ncol = 1; ncol <= (L->stride == 1 ? std::min(16, L->Wo) : 1) && !(ncol > 1 && found); ncol++)
   for (int ci = 0; ci < 2; ci++) {
     const int CPT = cpts[ci];
     if (Kg % CPT != 0) continue;
@@ -893,13 +901,14 @@ int PlanConv(qcnn_layer* L, int N) {
             memset(&p, 0, sizeof(p));
             ConvArgs& a = p.a;
             a.R = R;
-            a.nstrips = CeilDiv(L->Ho, R);
+            a.nstrips = CeilDiv(L->Ho, R) * ncol;
+            a.ncol = ncol; a.CW = CeilDiv(L->Wo, ncol);
             a.CT = CT; a.nct = nct; a.cwarps = cwarps;
             double gatherSlots, builtEntries, phases;
             int warps;
             if (L->stride == 1) {
               p.kernel = tc ? kConvS1Tc : kConvS1;
-              a.PW = L->Win + L->pad;
+              a.PW = ncol > 1 ? a.CW + L->ksz - 1 : L->Win + L->pad;
               a.RI = R + L->ksz - 1;
               a.pwarps = CeilDiv(R * a.PW, 32 * J);
               a.rgroups = 1;

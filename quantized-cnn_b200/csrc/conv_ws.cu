@@ -3,8 +3,9 @@
 //     dst[q][c] = bias[c] + sum_{k-steps} sum_{j<16} X_kstep[q][j] * W_kstep[c][j]       (M = positions, N = channels)
 //
 // Two position geometries, the ones pq_gemm_tc uses for the same layers (its k-step tables, Mode0Table / Mode1Table):
-//   stride 1 (mode 0, conv2-conv5): all images form one flat padded grid; a chunk is 8 input channels x all taps, and a
-//     16-byte row of a plane holds the 8 channels of one position; a tap is a start-address shift of the A descriptor.
+//   stride 1 (mode 0, conv2-conv5, VGG16): all images form one flat padded grid; a chunk is 8 input channels x all taps,
+//     and a 16-byte row of a plane holds the 8 channels of one position; a tap is a start-address shift of the A
+//     descriptor.  A group of <= 3 channels (an RGB first layer) is one chunk whose second half is zeros.
 //   strided over <= 4 input channels (mode 1, conv1: 11x11 / 4 over 3 channels): the input is de-interleaved into phase
 //     planes; a 16-byte row holds two phase columns x 4 channels of one position; a chunk is one phase row.
 //
@@ -43,7 +44,7 @@ using qcnn::WgmmaDesc;
 constexpr int kWsThreads = 384;
 constexpr int kWsConsumers = 256;   // warps 0-7
 constexpr int kWsProducers = 128;   // warps 8-11
-constexpr int kWsRegPos = 8;        // mode 0: float4 of a chunk's planes a producer thread stages (2 NPOS <= 8 * 128)
+constexpr int kWsRegPos = 8;        // mode 0: float4 of a chunk's planes a producer thread stages per register pass
 
 __device__ __forceinline__ uint32_t PackBf16x2(float lo, float hi) {   // low 16 bits = bf16(lo), high 16 bits = bf16(hi)
   uint32_t r;
@@ -87,8 +88,10 @@ __host__ __device__ inline WsSmem MapWsSmem(const GemmArgs& a) {
   return m;
 }
 
-// NC: channels per CTA; MB: m64 blocks per consumer warpgroup; S1: the stride-1 geometry (mode 0), else mode 1
-template <int NC, int MB, bool S1>
+// NC: channels per CTA; MB: m64 blocks per consumer warpgroup; S1: the stride-1 geometry (mode 0), else mode 1;
+// WIDE (stride 1): a chunk's planes take more than one register pass of the producers, or a group has <= 3 channels
+// (kept apart so that the single-pass kernels AlexNet runs carry none of that staging)
+template <int NC, int MB, bool S1, bool WIDE>
 __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a) {
   constexpr int P = 128 * MB;   // positions per CTA
   extern __shared__ __align__(128) unsigned char smem[];
@@ -136,62 +139,100 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
     const int pt = tid - kWsConsumers;
     int j = 0;   // weight stage counter (buffer j & 1)
     if constexpr (S1) {
-      // float4 p = pt + i * kWsProducers of a chunk's planes: half = p / NPOS (channels 0-3 / 4-7 of the chunk), position
-      // = p % NPOS -> pixel (r - pad, c - pad) of image i of the flat padded grid; the source offset and validity are
-      // chunk-invariant and computed once
+      // float4 p = pt + (q * kWsRegPos + i) * kWsProducers of pass q of a chunk's planes: half = p / NPOS (channels 0-3 /
+      // 4-7 of the chunk), position = p % NPOS -> pixel (r - pad, c - pad) of image i of the flat padded grid.  The 2 NPOS
+      // float4 of a chunk take nPass register passes; the source offsets and validity of a pass are chunk-invariant
+      // (computed once with a single pass, per pass otherwise)
       const int taps = a.ntab;
+      const int nPass = WIDE ? (2 * a.NPOS + kWsRegPos * kWsProducers - 1) / (kWsRegPos * kWsProducers) : 1;
       const float* srcBase = a.src + static_cast<size_t>(i0) * a.srcImg + g * a.Cg;
       int poff[kWsRegPos];
       uint32_t pvalid = 0, phalf = 0;
+      auto passPos = [&](int q) {
+        pvalid = 0; phalf = 0;
 #pragma unroll
-      for (int i = 0; i < kWsRegPos; i++) {
-        const int p = pt + i * kWsProducers;
-        poff[i] = 0;
-        if (p < 2 * a.NPOS) {
-          const bool hb = p >= a.NPOS;
-          const int F = Q0 + (hb ? p - a.NPOS : p);
-          const int im = F / a.IB, rem = F - im * a.IB;
-          const int r = rem / a.PW, c = rem - r * a.PW;
-          if (im < a.N && r >= a.pad && c >= a.pad) {
-            poff[i] = (((im - i0) * a.Hi + (r - a.pad)) * a.Wi + (c - a.pad)) * a.Cin + (hb ? 4 : 0);
-            pvalid |= 1u << i;
+        for (int i = 0; i < kWsRegPos; i++) {
+          const int p = pt + (q * kWsRegPos + i) * kWsProducers;
+          poff[i] = 0;
+          if (p < 2 * a.NPOS) {
+            const bool hb = p >= a.NPOS;
+            const int F = Q0 + (hb ? p - a.NPOS : p);
+            const int im = F / a.IB, rem = F - im * a.IB;
+            const int r = rem / a.PW, c = rem - r * a.PW;
+            if (im < a.N && r >= a.pad && c >= a.pad) {
+              poff[i] = (((im - i0) * a.Hi + (r - a.pad)) * a.Wi + (c - a.pad)) * a.Cin + (hb ? 4 : 0);
+              pvalid |= 1u << i;
+            }
+            if (hb) phalf |= 1u << i;
           }
-          if (hb) phalf |= 1u << i;
         }
-      }
+      };
       float4 rg[kWsRegPos];
-      // the positions of chunk kc into registers; a half beyond the group's channels (Cg % 8 == 4) stages zeros
+      // the current pass's positions of chunk kc into registers; a half beyond the group's channels (Cg % 8 == 4, Cg <= 3)
+      // stages zeros
       auto loadPos = [&](int kc) {
         const int chA = kc * 8;
         const uint32_t m = chA + 4 >= a.Cg ? pvalid & ~phalf : pvalid;
         const float* srcG = srcBase + chA;
+        if (!WIDE || a.Cg >= 4) {
 #pragma unroll
-        for (int i = 0; i < kWsRegPos; i++) {
-          rg[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-          if ((m >> i) & 1u) rg[i] = __ldg(reinterpret_cast<const float4*>(srcG + poff[i]));
+          for (int i = 0; i < kWsRegPos; i++) {
+            rg[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+            if ((m >> i) & 1u) rg[i] = __ldg(reinterpret_cast<const float4*>(srcG + poff[i]));
+          }
+        } else {
+          // <= 3 channels (one chunk): the pixel pitch is not 16-byte aligned, the channels are read as scalars
+#pragma unroll
+          for (int i = 0; i < kWsRegPos; i++) {
+            rg[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+            if ((m >> i) & 1u) {
+              const float* px = srcG + poff[i];
+              rg[i].x = __ldg(px);
+              if (a.Cg > 1) rg[i].y = __ldg(px + 1);
+              if (a.Cg > 2) rg[i].z = __ldg(px + 2);
+            }
+          }
         }
       };
-      loadPos(0);
-      for (int kc = 0; kc < nCh; kc++) {
-        const int pb = kc % nPB;
-        if (kc >= nPB) MbarWait<24>(emptyP + pb, ((kc / nPB) - 1) & 1);   // buffer last read by the MMAs of chunk kc - nPB
-        // row = position (16 bytes = the chunk's 8 channels), the half selects bytes 0-7 / 8-15
-        char* x1 = reinterpret_cast<char*>(planes + pb * 2 * a.planeRows);
-        char* x2 = x1 + a.planeRows * 16;
+      // pass q of the registers v into the plane buffer {x1, x2}: row = position (16 bytes = the chunk's 8 channels), the
+      // half selects bytes 0-7 / 8-15
+      auto storePass = [&](const float4 (&v)[kWsRegPos], int q, char* x1, char* x2) {
 #pragma unroll
         for (int i = 0; i < kWsRegPos; i++) {
-          const int p = pt + i * kWsProducers;
+          const int p = pt + (q * kWsRegPos + i) * kWsProducers;
           if (p < 2 * a.NPOS) {
             uint2 p1, p2;
-            SplitBf16x4(rg[i], p1, p2);
+            SplitBf16x4(v[i], p1, p2);
             const int db = p >= a.NPOS ? (p - a.NPOS) * 16 + 8 : p * 16;
             *reinterpret_cast<uint2*>(x1 + db) = p1;
             *reinterpret_cast<uint2*>(x2 + db) = p2;
           }
         }
+      };
+      passPos(0);
+      loadPos(0);
+      for (int kc = 0; kc < nCh; kc++) {
+        const int pb = kc % nPB;
+        if (kc >= nPB) MbarWait<24>(emptyP + pb, ((kc / nPB) - 1) & 1);   // buffer last read by the MMAs of chunk kc - nPB
+        char* x1 = reinterpret_cast<char*>(planes + pb * 2 * a.planeRows);
+        char* x2 = x1 + a.planeRows * 16;
+        if (nPass == 1) {
+          storePass(rg, 0, x1, x2);
+        } else {
+          for (int q = 0; q < nPass; q++) {
+            float4 cur[kWsRegPos];
+#pragma unroll
+            for (int i = 0; i < kWsRegPos; i++) cur[i] = rg[i];
+            if (q + 1 < nPass) { passPos(q + 1); loadPos(kc); }   // the next pass's loads are in flight during this split
+            storePass(cur, q, x1, x2);
+          }
+        }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // planes are read by the tensor core
         MbarArrive(fullP + pb);
-        if (kc + 1 < nCh) loadPos(kc + 1);   // in flight during the decode below
+        if (kc + 1 < nCh) {   // in flight during the decode below
+          if (nPass > 1) passPos(0);
+          loadPos(kc + 1);
+        }
         // the chunk's two 4-channel halves: subspace and piece of each (as pq_gemm_tc's fetchChunk); a half beyond the
         // group's channels gets a zero codebook slice (its positions are zeros too)
         const int chA = kc * 8, chB = chA + 4;
@@ -355,28 +396,28 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
 constexpr int kWsWidths[] = {16, 32, 64, 96, 128, 192, 256};
 
 // the dynamic shared-memory limit of an instantiation is raised once per device to the opt-in maximum (as in pq_gemm_tc.cu)
-template <int NC, int MB, bool S1>
+template <int NC, int MB, bool S1, bool WIDE>
 int SetSmemAndLaunch(const GemmArgs& a, unsigned blocks, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
   static bool done[64] = {false};
   if (ctx->device < 0 || ctx->device >= 64 || !done[ctx->device]) {
     const int lim = static_cast<int>(ctx->smem_optin ? ctx->smem_optin : 227 * 1024);
-    QCNN_CUDA(cudaFuncSetAttribute(conv_ws_kernel<NC, MB, S1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    QCNN_CUDA(cudaFuncSetAttribute(conv_ws_kernel<NC, MB, S1, WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     if (ctx->device >= 0 && ctx->device < 64) done[ctx->device] = true;
   }
-  conv_ws_kernel<NC, MB, S1><<<blocks, kWsThreads, smem, st>>>(a);
+  conv_ws_kernel<NC, MB, S1, WIDE><<<blocks, kWsThreads, smem, st>>>(a);
   QCNN_CUDA(cudaGetLastError());
   return 0;
 }
 
-template <bool S1>
+template <bool S1, bool WIDE>
 int LaunchWidth(const GemmArgs& a, int nc, unsigned nb, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
 #define QCNN_WS(NC)                                                                               \
-  if (nc == NC) return a.NT == 256 ? SetSmemAndLaunch<NC, 2, S1>(a, nb, smem, st, ctx)            \
-                                   : SetSmemAndLaunch<NC, 1, S1>(a, nb, smem, st, ctx);
+  if (nc == NC) return a.NT == 256 ? SetSmemAndLaunch<NC, 2, S1, WIDE>(a, nb, smem, st, ctx)      \
+                                   : SetSmemAndLaunch<NC, 1, S1, WIDE>(a, nb, smem, st, ctx);
   QCNN_WS(16) QCNN_WS(32) QCNN_WS(64) QCNN_WS(96) QCNN_WS(128)
 #undef QCNN_WS
-  if (nc == 192 && a.NT == 128) return SetSmemAndLaunch<192, 1, S1>(a, nb, smem, st, ctx);
-  if (nc == 256 && a.NT == 128) return SetSmemAndLaunch<256, 1, S1>(a, nb, smem, st, ctx);
+  if (nc == 192 && a.NT == 128) return SetSmemAndLaunch<192, 1, S1, WIDE>(a, nb, smem, st, ctx);
+  if (nc == 256 && a.NT == 128) return SetSmemAndLaunch<256, 1, S1, WIDE>(a, nb, smem, st, ctx);
   qcnn::SetError("internal: no conv_ws instantiation for N=%d positions=%d", nc, a.NT);
   return 1;
 }
@@ -388,11 +429,13 @@ bool WsWidth(int w) { return std::find(std::begin(kWsWidths), std::end(kWsWidths
 namespace qcnn {
 
 // Stride-1 tilings (mode-0 geometry): positions per CTA x channels per CTA (an instantiated width dividing Cout / grp)
-// x k-steps per weight stage, under the conditions of pq_gemm_tc mode 0 plus the pre-split codebook and the channel-major
-// index block of at most 32 taps.
+// x k-steps per weight stage, under the conditions of pq_gemm_tc mode 0 (or <= 3 channels per group) plus the pre-split
+// codebook and the channel-major index block of at most 32 taps.  The positions of a CTA need not fit one register pass
+// of the producers: any plane ring that fits in shared memory is a tiling.
 static void PlanConvWsS1(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands) {
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, taps = L->ksz * L->ksz;
-  if (L->src_nchw || L->d % 4 != 0 || Cg % 4 != 0 || L->Cin % 4 != 0 || L->S * L->d < Cg || taps > kMaxKSteps) return;
+  // (Cg <= 3: one chunk, half A read as scalars; wider groups: whole 4-channel halves read as float4)
+  if (L->src_nchw || L->d % 4 != 0 || (Cg > 3 && (Cg % 4 != 0 || L->Cin % 4 != 0)) || L->S * L->d < Cg || taps > kMaxKSteps) return;
   if (!L->d_ctrd_bf.get() || !L->d_asmt_t.get() || L->asmt_t_mode != 0 || RoundUp(taps, 16) > 32) return;
   const int PW = L->Win + L->pad, IB = (L->Hin + L->pad) * PW;
   if (L->Ho > L->Hin + L->pad || L->Wo > PW || static_cast<double>(N) * IB > 2.0e9) return;
@@ -413,7 +456,6 @@ static void PlanConvWsS1(const qcnn_layer* L, int N, std::vector<std::pair<doubl
       ga.mode = 0; ga.bf = 1;
       ga.PW = PW; ga.IB = IB; ga.NT = P;
       ga.NPOS = RoundUp(P + (L->ksz - 1) * (PW + 1), 8);
-      if (2 * ga.NPOS > kWsRegPos * kWsProducers) continue;
       ga.planeRows = ga.NPOS; ga.planeF4 = 2 * ga.NPOS;
       ga.nChunks = CeilDiv(Cg, 8); ga.nct = Kg / W; ga.nsplit = 1;
       ga.stride = 1; ga.Kg = Kg; ga.K = L->K;
@@ -509,7 +551,9 @@ int LaunchConvWs(qcnn_layer* L, const ConvPlan& p, const float* src, int N, floa
   QCNN_CHECK(static_cast<size_t>(MapWsSmem(a).total) == p.smem, "internal: conv_ws shared-memory carve changed after planning");
   const unsigned nb = static_cast<unsigned>(blocks);
   const int nc = a.Kg / a.nct;
-  return a.mode == 0 ? LaunchWidth<true>(a, nc, nb, p.smem, st, L->ctx) : LaunchWidth<false>(a, nc, nb, p.smem, st, L->ctx);
+  if (a.mode == 1) return LaunchWidth<false, false>(a, nc, nb, p.smem, st, L->ctx);
+  const bool wide = 2 * a.NPOS > kWsRegPos * kWsProducers || a.Cg < 4;
+  return wide ? LaunchWidth<true, true>(a, nc, nb, p.smem, st, L->ctx) : LaunchWidth<true, false>(a, nc, nb, p.smem, st, L->ctx);
 }
 
 }  // namespace qcnn

@@ -162,6 +162,7 @@ struct ConvArgs {
   int R, nstrips;       // output rows per CTA / strips per image
   int PW;               // s1: row pitch of the flat padded grid; roll: phase length PH
   int RI;               // s1: input rows held per strip
+  int CW, ncol;         // s1: output columns per column tile / column tiles per row (1: whole rows)
   int PP;               // LUT pitch in floats (positions per codeword row), multiple of 4
   int NM;               // wgmma LUT stage: LUT columns produced per step (MMA N, multiple of 32, <= 256)
   int CT, nct;          // output channels per CTA (per group) / channel tiles per group

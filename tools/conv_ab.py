@@ -1,16 +1,19 @@
 #!/usr/bin/env python
-"""AlexNet conv layers alone (bf16x2 operands): the weight-stationary family conv_ws (force_kernel = 7) against the
-decode-at-use pq_gemm_tc (force_kernel = 6) -- mode 1 for conv1, mode 0 for conv2-conv5 -- in one process on one GPU.
+"""AlexNet and VGG16 block-1 conv layers alone (bf16x2 operands): the weight-stationary family conv_ws (force_kernel = 7)
+against the decode-at-use pq_gemm_tc (force_kernel = 6) -- mode 1 for conv1, mode 0 for conv2-conv5 and VGG16 conv1_2 --
+or, for VGG16 conv1_1 (3 input channels, which pq_gemm_tc does not take), against the LUT + gather kernels
+(tensor_core = 0, the tiling timed on the device), in one process on one GPU.
 
 For every layer and batch size the two families alternate, round by round; a round is `iters` back-to-back launches
 between CUDA events.  Each family is a layer object of its own (same parameters, the family pinned once), so that its
 tiling is chosen on the device by one untimed launch per batch size and no timed round re-tunes.  Per
 family the tool prints the median and min-max of the per-launch time over the rounds, the executed tensor-core TFLOP/s
 (every MMA the plan issues, padding included) and the useful TFLOP/s (2 x N x Ho x Wo x Cout x k^2 x Cin/grp flops of the
-dense layer), the plan, and the card name, power limit and maximum SM clock.
+dense layer; not given for the LUT + gather kernels), the plan, and the card name, power limit and maximum SM clock.
 
     python tools/conv_ab.py [--layers conv1,conv2,conv3,conv4,conv5] [--batches 1,4,40,256,1024] [--rounds 7]
                             [--iters 20] [--out conv_ab.json]
+    python tools/conv_ab.py --layers vgg_conv1_1,vgg_conv1_2 --batches 1,64,256
 """
 import argparse
 import ctypes
@@ -26,15 +29,20 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-# name: (Hi, Wi, Cin, Cout, k, pad, stride, groups, S, K, d) -- the AlexNet layers of bench.py
+# name: (Hi, Wi, Cin, Cout, k, pad, stride, groups, S, K, d) -- the AlexNet layers of bench.py, VGG16's block 1 with the
+# subspaces of tests/test_oracle_vgg16.py
 LAYERS = {
     "conv1": (227, 227, 3, 96, 11, 0, 4, 1, 1, 128, 8),
     "conv2": (27, 27, 96, 256, 5, 2, 1, 2, 6, 128, 8),
     "conv3": (13, 13, 256, 384, 3, 1, 1, 1, 32, 128, 8),
     "conv4": (13, 13, 384, 384, 3, 1, 1, 2, 24, 128, 8),
     "conv5": (13, 13, 384, 256, 3, 1, 1, 2, 24, 128, 8),
+    "vgg_conv1_1": (224, 224, 3, 64, 3, 1, 1, 1, 1, 128, 4),
+    "vgg_conv1_2": (224, 224, 64, 64, 3, 1, 1, 1, 8, 128, 8),
 }
-FAMILIES = {7: "conv_ws", 6: "pq_gemm_tc"}
+# the two sides of a layer: name -> (tensor_core, force_kernel or None)
+FAMILIES = {"conv_ws": (2, 7), "pq_gemm_tc": (2, 6)}
+LUT_RIVAL = {"vgg_conv1_1": {"conv_ws": (2, 7), "lut_gather": (0, None)}}
 
 
 def card():
@@ -55,6 +63,8 @@ def executed_macs(desc):
         n, p, grid, ks = (float(v) for v in m.groups())
         return grid * ks * 2 * 16 * p * n
     m = re.search(r"pq_gemm_tc\(.*?NT=(\d+) .*?grid=(\d+) .*?ksteps=(\d+)", desc)
+    if not m:
+        return None   # (LUT + gather: no tensor-core GEMM)
     nt, grid, ks = (float(v) for v in m.groups())
     return grid * ks * 2 * 16 * 128 * nt
 
@@ -70,12 +80,14 @@ def run_layer(q, ctx, name, batches, args, rng, res):
     ctrd = (rng.randn(S, K, d) / np.sqrt(Cin // G * k * k)).astype(np.float32)
     asmt = rng.randint(0, K, size=(Cout, k, k, S)).astype(np.uint8)
     bias = (rng.randn(Cout) * 0.1).astype(np.float32)
+    fams = LUT_RIVAL.get(name, FAMILIES)
     lay = {}
-    for kern in FAMILIES:
-        lay[kern] = q.ConvLayer(ctx, Cin, Hi, Wi, Cout, k, pad, stride, G, ctrd, asmt, bias)
-        lay[kern].set_param("tensor_core", 2)
-        lay[kern].set_param("force_kernel", kern)
-    ho, wo, co = lay[7].out_dims()
+    for fam, (tc, kern) in fams.items():
+        lay[fam] = q.ConvLayer(ctx, Cin, Hi, Wi, Cout, k, pad, stride, G, ctrd, asmt, bias)
+        lay[fam].set_param("tensor_core", tc)
+        if kern is not None:
+            lay[fam].set_param("force_kernel", kern)
+    ho, wo, co = lay["conv_ws"].out_dims()
     stream = torch.cuda.current_stream()
     res[name] = {}
     for N in batches:
@@ -86,9 +98,9 @@ def run_layer(q, ctx, name, batches, args, rng, res):
         def launch(L):
             q._check(q.lib.qcnn_conv_aprx_forward(L.h, ctypes.c_void_p(x.data_ptr()), N, ctypes.c_void_p(y.data_ptr()), 1,
                                                   ctypes.c_void_p(stream.cuda_stream)))
-        plans, times = {}, {kern: [] for kern in FAMILIES}
+        plans, times = {}, {fam: [] for fam in fams}
         for r in range(args.rounds + 1):
-            for kern in FAMILIES:
+            for kern in fams:
                 if r == 0:
                     launch(lay[kern])          # tiling chosen on the device for this batch size
                     torch.cuda.synchronize()
@@ -102,14 +114,15 @@ def run_layer(q, ctx, name, batches, args, rng, res):
                 torch.cuda.synchronize()
                 times[kern].append(a.elapsed_time(b) / args.iters)
         out = {}
-        for kern, fam in FAMILIES.items():
-            s = stats(times[kern])
-            ex = 2.0 * executed_macs(plans[kern])
-            out[fam] = dict(ms=s, executed_TFLOPs=ex / (s["median"] * 1e-3) / 1e12,
-                            useful_TFLOPs=useful / (s["median"] * 1e-3) / 1e12, plan=plans[kern])
-            print("%s N=%-5d %-11s %8.4f ms (%.4f - %.4f)  executed %6.1f TFLOP/s  useful %6.1f TFLOP/s  %s"
-                  % (name, N, fam, s["median"], s["min"], s["max"], out[fam]["executed_TFLOPs"], out[fam]["useful_TFLOPs"],
-                     plans[kern].split(" smem")[0]), flush=True)
+        for fam in fams:
+            s = stats(times[fam])
+            em = executed_macs(plans[fam])
+            out[fam] = dict(ms=s, executed_TFLOPs=2.0 * em / (s["median"] * 1e-3) / 1e12 if em else None,
+                            useful_TFLOPs=useful / (s["median"] * 1e-3) / 1e12, plan=plans[fam])
+            print("%s N=%-5d %-11s %8.4f ms (%.4f - %.4f)  executed %s TFLOP/s  useful %6.1f TFLOP/s  %s"
+                  % (name, N, fam, s["median"], s["min"], s["max"],
+                     "%6.1f" % out[fam]["executed_TFLOPs"] if em else "     -", out[fam]["useful_TFLOPs"],
+                     plans[fam].split(" smem")[0]), flush=True)
         res[name][str(N)] = out
         del x, y
         torch.cuda.empty_cache()
