@@ -49,18 +49,6 @@ __device__ __forceinline__ float2 Fadd2(float2 a, float2 b) { return make_float2
 
 constexpr int kMaxThreads = 512;
 
-// describe() names of the LUT + gather kernels, and whether their LUT stage runs on the tensor cores (the two numerical
-// classes of the family)
-struct ConvKernelInfo {
-  const char* name;
-  bool tcLut;
-};
-constexpr ConvKernelInfo kConvKernelInfo[kConvDirect + 1] = {
-    {"conv_s1", false}, {"conv_roll", false}, {"conv_s1_tc(wgmma LUT)", true}, {"conv_roll_tc(wgmma LUT)", true},
-    {"conv_direct", false}};
-// the tensor-core GEMM family (tensor_core = 1 / 2): decode-at-use pq_gemm_tc and the weight-stationary conv_ws
-constexpr bool IsGemmTc(int kernel) { return kernel == kPqGemmTc || kernel == kConvWs; }
-
 // ------------------------------------------------------------------------------------------------------------
 // Operand staging.  Everything the LUT stage of step i+1 needs from global memory (input pixels of the
 // subspace's channels, its codebook rows, its assignment slice) is copied ASYNCHRONOUSLY (cp.async, no registers)
@@ -859,9 +847,7 @@ int LaunchOne(const ConvPlan& p, const ConvArgs& a, cudaStream_t st) {
 
 namespace qcnn {
 
-constexpr size_t kMaxCand = 18;
-
-// Chooses the tiling of a conv layer for batch size N.  Cost model in SM-cycles per CTA, times the number of
+// Candidate tilings of the LUT + gather kernels for batch size N.  Cost model in SM-cycles per CTA, times the number of
 // waves the whole batch needs on this GPU (so small batches trade LUT rebuilds for parallelism):
 //   gather  = shared-memory wavefronts: one per (warp, tap, s, channel, position-slot) plus one 128-bit offset load
 //             per 4 channels -> (1 + 1/(4J)) per lookup slot, 1 wavefront / clk / SM
@@ -869,25 +855,26 @@ constexpr size_t kMaxCand = 18;
 //             (0.66 * dims + 0.3) issue slots / 32 lanes / ~2.5 warp-instructions per clk
 //   sync    = ~300 clk per (s [, input row]) phase pair
 // The two stages do not overlap inside a CTA (one CTA per SM), so the costs add.
-int PlanConv(qcnn_layer* L, int N) {
-  if (L->plan_N == N) return 0;
-  for (const std::pair<int, ConvPlan>& e : L->tunedPlans)  // a batch size seen (and timed) before: reuse its plan
-    if (e.first == N) { L->plan = e.second; L->plan_N = N; L->tuned = 1; return 0; }
-  std::vector<std::pair<double, ConvPlan>> cands;
-  bool found = false;
+void PlanLutGather(const qcnn_layer* L, int N, ConvCands* cands) {
+  bool found = false;   // a tiling exists (while ncol = 1: a whole-row one)
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G;
   const int taps = L->ksz * L->ksz;
-  const size_t smemMax = L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024;
+  const size_t smemMax = SmemOptin(L->ctx);
+  ConvPlan p0;   // every candidate: the layer's geometry, the tiling fields zero
+  memset(&p0, 0, sizeof(p0));
+  ConvArgs& a0 = p0.a;
+  a0.Hi = L->Hin; a0.Wi = L->Win; a0.Cin = L->Cin; a0.Ho = L->Ho; a0.Wo = L->Wo; a0.Cout = L->Cout;
+  a0.ksz = L->ksz; a0.pad = L->pad; a0.stride = L->stride; a0.G = G; a0.Cg = Cg; a0.Kg = Kg;
+  a0.KgPad = RoundUp(Kg, 16);
+  a0.S = L->S; a0.K = L->K; a0.d = L->d;
   double dimsSum = 0;  // sum over subspaces of the dims that exist
   for (int s = 0; s < L->S; s++) dimsSum += std::max(0, std::min(Cg - s * L->d, L->d));
   const double ipe = 0.66 * (dimsSum / L->S) + 0.3;  // issue slots per LUT entry
   // tensor-core LUT stage: 128 codewords (MMA M), every subspace <= 8 dims (one K = 8 tf32 step)
   const bool tcOk = L->K == 128 && L->d <= 8;
-  const int cpts[2] = {32, 16};
   // stride 1: whole rows per CTA; column tiles (ncol > 1) only for layers whose rows fit no LUT (VGG16's 224-wide block 1)
   for (int ncol = 1; ncol <= (L->stride == 1 ? std::min(16, L->Wo) : 1) && !(ncol > 1 && found); ncol++)
-  for (int ci = 0; ci < 2; ci++) {
-    const int CPT = cpts[ci];
+  for (const int CPT : {32, 16}) {
     if (Kg % CPT != 0) continue;
     for (int J = 1; J * CPT <= 64 && J <= 4; J++) {
       for (int nct = 1; nct <= Kg / CPT; nct++) {
@@ -897,8 +884,7 @@ int PlanConv(qcnn_layer* L, int N) {
         const int cwarps = CT / CPT;
         for (int R = 1; R <= L->Ho; R++) {
           for (int tc = 0; tc <= (tcOk ? 1 : 0); tc++) {
-            ConvPlan p;
-            memset(&p, 0, sizeof(p));
+            ConvPlan p = p0;
             ConvArgs& a = p.a;
             a.R = R;
             a.nstrips = CeilDiv(L->Ho, R) * ncol;
@@ -966,7 +952,8 @@ int PlanConv(qcnn_layer* L, int N) {
             const double ctas = static_cast<double>(G) * nct * a.nstrips * N;
             const double waves = std::ceil(ctas / L->ctx->sm_count);
             const double cost = perCta * waves * occPenalty;
-            cands.emplace_back(cost, p);
+            p.key = {CPT, J, nct, a.nstrips, a.rgroups, R};
+            cands->emplace_back(cost, p);
             found = true;
           }
         }
@@ -976,22 +963,17 @@ int PlanConv(qcnn_layer* L, int N) {
   // single subspace of <= 4 existing dims: evaluate <x, codeword> at the point of use (conv_direct_kernel)
   if (L->S == 1 && std::min(Cg, L->d) <= 4 && L->Wo <= 64) {
     const int NJ = std::min(Cg, L->d) <= 3 ? 3 : 4;
-    const int dcpts[2] = {16, 8};
-    for (int ci = 0; ci < 2; ci++) {
-      const int CPT = dcpts[ci];
+    for (const int CPT : {16, 8}) {
       if (Kg % CPT != 0 || Kg % 16 != 0) continue;
       for (int nct = 1; nct <= 2; nct++) {
         if (Kg % nct != 0 || (Kg / nct) % 16 != 0 || (Kg / nct) % CPT != 0) continue;
         const int CT = Kg / nct, cwarps = CT / CPT;
-        const int Rs[5] = {2, 4, 6, 8, 14};
-        for (int ri = 0; ri < 5; ri++) {
-          const int R = Rs[ri];
+        for (const int R : {2, 4, 6, 8, 14}) {
           if (R > L->Ho + 1) continue;
           for (int rgroups = 1; rgroups <= 2; rgroups++)
           for (int rowsPer = 2; rowsPer <= (CPT == 8 ? 4 : 2); rowsPer += 2) {
             if (rgroups > R / rowsPer) continue;
-            ConvPlan p;
-            memset(&p, 0, sizeof(p));
+            ConvPlan p = p0;
             ConvArgs& a = p.a;
             p.kernel = kConvDirect; p.CPT = CPT; p.J = rowsPer;
             a.R = std::min(R, L->Ho + (L->Ho & 1)); a.nstrips = CeilDiv(L->Ho, a.R);
@@ -1010,104 +992,13 @@ int PlanConv(qcnn_layer* L, int N) {
             const double perCta = perWarp * cwarps * rgroups / 2.6 + rowsIn * NJ * a.PP * 0.5;
             const double ctas = static_cast<double>(G) * nct * a.nstrips * N;
             const double waves = std::ceil(ctas / L->ctx->sm_count);
-            cands.emplace_back(perCta * waves, p);
-            found = true;
+            p.key = {CPT, rowsPer, nct, a.nstrips, rgroups, a.R};
+            cands->emplace_back(perCta * waves, p);
           }
         }
       }
     }
   }
-  // tensor-core GEMMs: decode-at-use pq_gemm_tc.cu and, with bf16x2 operands, the weight-stationary conv_ws.cu (stride-1
-  // layers and strided narrow-input layers).  The operand format is a setting, not a timing result: with tensor_core = 2
-  // (default, bf16x2) or 1 (3xTF32) an eligible layer always runs one of these GEMMs (tolerances in DESIGN.md 2), with
-  // tensor_core = 0 always the LUT + gather kernels.  On-device timing chooses among the GEMM tilings of that format --
-  // at bf16x2 between conv_ws and pq_gemm_tc of the same geometry (mode 0 / mode 1 at NT = 128), which share the k-step
-  // chain and its bound.
-  if (!L->opt_no_tc) {
-    std::vector<std::pair<double, ConvPlan>> tc;
-    PlanPqGemm(L, N, &tc);
-    PlanConvWs(L, N, &tc);
-    if (!tc.empty()) { cands.swap(tc); found = true; }
-  }
-  QCNN_CHECK(found, "qcnn_conv_layer_create: no tiling fits (Cout/grp=%d must be a multiple of 16; K=%d must be a "
-             "multiple of 8; k=%d, W=%d)", Kg, L->K, L->ksz, L->Win);
-  // keep the kMaxCand cheapest tilings (by the model); LaunchConv times them on the device the first time a batch size
-  // is seen (QCNN_AUTOTUNE=0 keeps the model's first choice)
-  std::stable_sort(cands.begin(), cands.end(), [](const std::pair<double, ConvPlan>& x, const std::pair<double, ConvPlan>& y) { return x.first < y.first; });
-  L->cands.clear();
-  // layer parameter "force_kernel" / QCNN_FORCE_KERNEL=<0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc |
-  // 7 conv_ws>
-  // restricts the choice (tests pin the kernel they check; fails when that kernel has no tiling for the layer)
-  // Within the LUT + gather family the kernels come in two numerical classes -- fp32 LUT / decode (s1, roll, direct) and
-  // 3xTF32 tensor-core LUT stage (s1_tc, roll_tc; ~5e-6 apart) -- and on-device timing must not pick between classes
-  // either: the class of the cost model's favourite is kept, timing chooses among its tilings only.
-  if (!cands.empty() && !IsGemmTc(cands[0].second.kernel) && !L->opt_force_kernel && getenv("QCNN_FORCE_KERNEL") == nullptr) {
-    const bool want = kConvKernelInfo[cands[0].second.kernel].tcLut;
-    std::vector<std::pair<double, ConvPlan>> kept;
-    for (const auto& c : cands)
-      if (!IsGemmTc(c.second.kernel) && kConvKernelInfo[c.second.kernel].tcLut == want) kept.push_back(c);
-    cands.swap(kept);
-  }
-  // (the family first: a gemm_* pin that no tiling of the pinned family matches is reported as such)
-  const char* force = getenv("QCNN_FORCE_KERNEL");
-  if (L->opt_force_kernel || force) {
-    const int want = L->opt_force_kernel ? L->opt_force_kernel - 1 : atoi(force);
-    std::vector<std::pair<double, ConvPlan>> kept;
-    for (const auto& c : cands) if (c.second.kernel == want) kept.push_back(c);
-    QCNN_CHECK(!kept.empty() || !L->opt_force_kernel, "qcnn_conv_aprx_forward: force_kernel=%d has no tiling for this layer at batch %d", want, N);
-    if (!kept.empty()) cands.swap(kept);
-  }
-  // layer parameters "gemm_nt" / "gemm_gt" / "gemm_nsplit": only pq_gemm_tc tilings with that many positions per CTA,
-  // k-steps per stage and K-split factor (0 = any); "gemm_nt" also restricts the positions per CTA of conv_ws, and
-  // "gemm_ct" its channels per CTA
-  if (L->opt_gemm_nt || L->opt_gemm_gt || L->opt_gemm_nsplit || L->opt_gemm_ct) {
-    std::vector<std::pair<double, ConvPlan>> kept;
-    for (const auto& c : cands)
-      if ((c.second.kernel == kConvWs && (!L->opt_gemm_nt || c.second.g.NT == L->opt_gemm_nt) &&
-           (!L->opt_gemm_ct || c.second.g.Kg / c.second.g.nct == L->opt_gemm_ct)) ||
-          (c.second.kernel != kPqGemmTc && c.second.kernel != kConvWs) ||
-          (c.second.kernel == kPqGemmTc && (!L->opt_gemm_nt || c.second.g.NT == L->opt_gemm_nt) &&
-           (!L->opt_gemm_gt || c.second.g.GT == L->opt_gemm_gt) &&
-           (!L->opt_gemm_nsplit || c.second.g.nsplit == L->opt_gemm_nsplit)))
-        kept.push_back(c);
-    QCNN_CHECK(!kept.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d gemm_gt=%d gemm_nsplit=%d gemm_ct=%d has no tiling for this "
-               "layer at batch %d", L->opt_gemm_nt, L->opt_gemm_gt, L->opt_gemm_nsplit, L->opt_gemm_ct, N);
-    cands.swap(kept);
-  }
-  // every kernel family that has a feasible tiling gets at least two seats among the candidates
-  for (int pass = 0; pass < 2; pass++) {
-    int perKernel[kConvKernelIds] = {};
-    for (size_t i = 0; i < cands.size() && L->cands.size() < kMaxCand; i++) {
-      ConvPlan c = cands[i].second;
-      if (pass == 0 && perKernel[c.kernel] >= (c.kernel == kConvDirect ? 8 : (IsGemmTc(c.kernel) ? 6 : 2))) continue;
-      ConvArgs& a = c.a;
-      a.Hi = L->Hin; a.Wi = L->Win; a.Cin = L->Cin; a.Ho = L->Ho; a.Wo = L->Wo; a.Cout = L->Cout;
-      a.ksz = L->ksz; a.pad = L->pad; a.stride = L->stride; a.G = G; a.Cg = Cg; a.Kg = Kg;
-      a.KgPad = RoundUp(Kg, 16);
-      a.S = L->S; a.K = L->K; a.d = L->d;
-      // skip near-duplicates: same kernel/CPT/J/channel tiling and a strip count already present
-      bool dup = false;
-      for (const ConvPlan& e : L->cands)
-        if (e.kernel == c.kernel && e.CPT == c.CPT && e.J == c.J && e.a.nct == c.a.nct && e.a.nstrips == c.a.nstrips &&
-            e.a.rgroups == c.a.rgroups && e.a.R == c.a.R && (e.kernel != kConvDirect || e.J == c.J)) dup = true;
-      if (dup) continue;
-      L->cands.push_back(c);
-      perKernel[c.kernel]++;
-    }
-  }
-  // the model's overall favourite first (it is the plan used when autotuning is off)
-  for (size_t i = 1; i < L->cands.size(); i++)
-    if (L->cands[i].kernel == cands[0].second.kernel && L->cands[i].CPT == cands[0].second.CPT &&
-        L->cands[i].J == cands[0].second.J && L->cands[i].a.nct == cands[0].second.a.nct &&
-        L->cands[i].a.nstrips == cands[0].second.a.nstrips && L->cands[i].a.rgroups == cands[0].second.a.rgroups) {
-      std::swap(L->cands[0], L->cands[i]);
-      break;
-    }
-  const ConvPlan best = L->cands[0];
-  L->plan = best;
-  L->plan_N = N;
-  L->tuned = 0;
-  return 0;
 }
 
 template <int CPT, int NJ, int ROWS>
@@ -1120,12 +1011,10 @@ static int LaunchDirect(const ConvPlan& p, const ConvArgs& a, cudaStream_t st) {
   return 0;
 }
 
-static int LaunchPlan(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
+int LaunchLutGather(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
   ConvArgs a = p.a;
   a.src = src; a.dst = dst; a.ctrd = L->d_ctrd.as<float>(); a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
   a.N = N; a.relu = relu; a.src_nchw = L->src_nchw;
-  if (p.kernel == kPqGemmTc) return LaunchPqGemm(L, p, src, N, dst, relu, st);
-  if (p.kernel == kConvWs) return LaunchConvWs(L, p, src, N, dst, relu, st);
   if (p.kernel == kConvDirect) {
     const int nj = std::min(a.Cg, a.d);
     // p.J carries the output rows per thread (2 or 4)
@@ -1142,92 +1031,10 @@ static int LaunchPlan(qcnn_layer* L, const ConvPlan& p, const float* src, int N,
   return rc;
 }
 
-int LaunchConv(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st) {
-  QCNN_CHECK(L->kind == QCNN_KIND_CONV, "qcnn_conv_aprx_forward: layer is not convolutional");
-  QCNN_CHECK(N >= 1 && N <= 65535, "qcnn_conv_aprx_forward: N must be in [1, 65535] (got %d)", N);
-  if (int prc = PlanConv(L, N)) return prc;
-  // empirical choice among the model's best tilings: time each once on this device for this batch size
-  static const bool autotune = !(getenv("QCNN_AUTOTUNE") && getenv("QCNN_AUTOTUNE")[0] == '0');
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(st, &cap);
-  if (autotune && !L->opt_no_autotune && !L->tuned && L->cands.size() > 1 && cap == cudaStreamCaptureStatusNone) {
-    cudaEvent_t e0, e1;
-    QCNN_CUDA(cudaEventCreate(&e0));
-    if (cudaEventCreate(&e1) != cudaSuccess) { cudaEventDestroy(e0); return CudaFail(cudaGetLastError(), "cudaEventCreate", __FILE__, __LINE__); }
-    float bestMs = 1e30f;
-    size_t bestI = 0;
-    for (size_t i = 0; i < L->cands.size(); i++) {
-      const ConvPlan& c = L->cands[i];
-      if (LaunchPlan(L, c, src, N, dst, relu, st)) continue;   // warm-up (also sets the smem attribute)
-      // best of two timed samples (a sample = 1 launch at large batches, 3 at small ones): single samples made the choice
-      // between near-equal candidates vary from run to run
-      const int reps = N >= 64 ? 1 : 3;
-      float ms = 1e30f;
-      bool ok = true;
-      for (int sample = 0; sample < 2 && ok; sample++) {
-        if (cudaEventRecord(e0, st) != cudaSuccess) { cudaGetLastError(); ok = false; break; }
-        for (int r = 0; r < reps; r++) LaunchPlan(L, c, src, N, dst, relu, st);
-        if (cudaEventRecord(e1, st) != cudaSuccess) { cudaGetLastError(); ok = false; break; }
-        if (cudaEventSynchronize(e1) != cudaSuccess) { cudaGetLastError(); ok = false; break; }
-        float t = 0.0f;
-        cudaEventElapsedTime(&t, e0, e1);
-        ms = std::min(ms, t);
-      }
-      if (!ok) continue;
-      static const bool tuneLog = getenv("QCNN_AUTOTUNE_LOG") != nullptr;
-      if (tuneLog)
-        fprintf(stderr, "[qcnn autotune] N=%d Cout=%d k=%d cand %zu: kernel=%d NT/CPT=%d GT/J=%d bf=%d nsplit=%d smem=%zu -> %.4f ms\n",
-                N, L->Cout, L->ksz, i, c.kernel, c.CPT, IsGemmTc(c.kernel) ? c.g.GT : c.J, c.g.bf, c.g.nsplit, c.smem, ms);
-      if (ms < bestMs) { bestMs = ms; bestI = i; }
-    }
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    L->plan = L->cands[bestI];
-    L->tuned = 1;
-    L->tunedPlans.emplace_back(N, L->plan);
-  }
-  const int rc = LaunchPlan(L, L->plan, src, N, dst, relu, st);
-  if (rc == 0) L->ctx->launches++;
-  return rc;
-}
-
-// human-readable tiling of the plan for batch N (bench / DESIGN bookkeeping)
-int DescribeConv(qcnn_layer* L, int N, char* buf, size_t cap) {
-  if (int prc = PlanConv(L, N)) return prc;
-  const ConvPlan& p = L->plan;
-  if (p.kernel == kPqGemmTc) {
-    int ksteps = 0;
-    for (int c = 0; c < p.g.nChunks; c++) ksteps += p.g.chunkCount[p.g.mode == 1 ? c : 0];
-    snprintf(buf, cap, "pq_gemm_tc(wgmma, weights decoded into registers%s) mode=%d NT=%d GT=%d smem=%zuB grid=%d NPOS=%d "
-             "chunks=%d ksteps=%d nsplit=%d", p.g.bf ? ", bf16x2" : "", p.g.mode, p.g.NT, p.g.GT, p.smem,
-             CeilDiv(N * p.g.IB, p.g.NT) * L->grp * p.g.nct * std::max(1, p.g.nsplit), p.g.NPOS, p.g.nChunks,
-             ksteps / std::max(1, p.g.nsplit), std::max(1, p.g.nsplit));
-    return 0;
-  }
-  if (p.kernel == kConvWs && p.g.mode == 0) {
-    // stride 1: N = channels per CTA, ctiles = channel tiles per group, ksteps = chunks x taps (a CTA's k-steps), so
-    // that grid x ksteps x 32 x positions x N is the executed MAC count
-    const int stages = p.g.nChunks * CeilDiv(p.g.ntab, p.g.GT);
-    snprintf(buf, cap, "pq_gemm_tc_ws(weight-stationary wgmma, weights decoded once per CTA into shared memory, bf16x2) "
-             "mode=0 N=%d positions=%d ctiles=%d KS=%d smem=%zuB grid=%d NPOS=%d planebufs=%d chunks=%d stages=%d ksteps=%d",
-             p.g.Kg / p.g.nct, p.g.NT, p.g.nct, p.g.GT, p.smem, CeilDiv(N * p.g.IB, p.g.NT) * L->grp * p.g.nct, p.g.NPOS,
-             p.g.nPB, p.g.nChunks, stages, p.g.nChunks * p.g.ntab);
-    return 0;
-  }
-  if (p.kernel == kConvWs) {
-    // (no "NT=": the executed-MAC count that bench.py derives from pq_gemm_tc( plans assumes 128-channel tiles)
-    int stages = 0;
-    for (int c = 0; c < p.g.nChunks; c++) stages += CeilDiv(p.g.chunkCount[c], p.g.GT);
-    snprintf(buf, cap, "pq_gemm_tc_ws(weight-stationary wgmma, weights decoded once per CTA into shared memory, bf16x2) "
-             "N=%d positions=%d KS=%d smem=%zuB grid=%d NPOS=%d chunks=%d stages=%d ksteps=%d",
-             p.g.Kg, p.g.NT, p.g.GT, p.smem, CeilDiv(N * p.g.IB, p.g.NT) * L->grp, p.g.NPOS, p.g.nChunks, stages, p.g.ntab);
-    return 0;
-  }
-  snprintf(buf, cap, "%s CPT=%d J=%d threads=%d smem=%zuB grid=(%d,%d) R=%d strips=%d CT=%d nct=%d PP=%d pwarps=%d "
-           "cwarps=%d rgroups=%d", kConvKernelInfo[p.kernel].name, p.CPT, p.J, p.threads, p.smem,
-           p.a.G * p.a.nct * p.a.nstrips, N, p.a.R, p.a.nstrips, p.a.CT, p.a.nct, p.a.PP, p.a.pwarps, p.a.cwarps,
-           p.a.rgroups);
-  return 0;
+void DescribeLutGather(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap) {
+  snprintf(buf, cap, " CPT=%d J=%d threads=%d smem=%zuB grid=(%d,%d) R=%d strips=%d CT=%d nct=%d PP=%d pwarps=%d "
+           "cwarps=%d rgroups=%d", p.CPT, p.J, p.threads, p.smem, p.a.G * p.a.nct * p.a.nstrips, N, p.a.R, p.a.nstrips,
+           p.a.CT, p.a.nct, p.a.PP, p.a.pwarps, p.a.cwarps, p.a.rgroups);
 }
 
 }  // namespace qcnn

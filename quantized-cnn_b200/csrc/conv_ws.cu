@@ -31,14 +31,17 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 
 namespace {
 
+using qcnn::ByteOf32;
 using qcnn::MbarArrive;
 using qcnn::MbarInit;
 using qcnn::MbarWait;
 using qcnn::SmemU32;
+using qcnn::SplitBf16x4;
 using qcnn::WgmmaDesc;
 
 constexpr int kWsThreads = 384;
@@ -46,25 +49,6 @@ constexpr int kWsConsumers = 256;   // warps 0-7
 constexpr int kWsProducers = 128;   // warps 8-11
 constexpr int kWsRegPos = 8;        // mode 0: float4 of a chunk's planes a producer thread stages per register pass
 
-__device__ __forceinline__ uint32_t PackBf16x2(float lo, float hi) {   // low 16 bits = bf16(lo), high 16 bits = bf16(hi)
-  uint32_t r;
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
-}
-// bf16x2 split of four values: x1 = bf16(x), x2 = bf16(x - x1) (the residuals are exact in fp32)
-__device__ __forceinline__ void SplitBf16x4(const float4 v, uint2& p1, uint2& p2) {
-  p1.x = PackBf16x2(v.x, v.y);
-  p1.y = PackBf16x2(v.z, v.w);
-  p2.x = PackBf16x2(v.x - __uint_as_float(p1.x << 16), v.y - __uint_as_float(p1.x & 0xFFFF0000u));
-  p2.y = PackBf16x2(v.z - __uint_as_float(p1.y << 16), v.w - __uint_as_float(p1.y & 0xFFFF0000u));
-}
-// byte t (< 32, warp-uniform: selects, no local memory) of the 32 bytes {lo, hi}
-__device__ __forceinline__ int ByteOf32(const uint4 lo, const uint4 hi, int t) {
-  const uint32_t x = (t & 16) ? hi.x : lo.x, y = (t & 16) ? hi.y : lo.y, z = (t & 16) ? hi.z : lo.z, w = (t & 16) ? hi.w : lo.w;
-  const uint32_t xy = (t & 4) ? y : x, zw = (t & 4) ? w : z;
-  const uint32_t v = (t & 8) ? zw : xy;
-  return static_cast<int>((v >> ((t & 3) * 8)) & 0xFFu);
-}
 // the four producer warps only (named barrier 1; barrier 0 is __syncthreads)
 __device__ __forceinline__ void ProducerSync() { asm volatile("bar.sync 1, %0;" :: "n"(kWsProducers) : "memory"); }
 
@@ -400,7 +384,7 @@ template <int NC, int MB, bool S1, bool WIDE>
 int SetSmemAndLaunch(const GemmArgs& a, unsigned blocks, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
   static bool done[64] = {false};
   if (ctx->device < 0 || ctx->device >= 64 || !done[ctx->device]) {
-    const int lim = static_cast<int>(ctx->smem_optin ? ctx->smem_optin : 227 * 1024);
+    const int lim = static_cast<int>(qcnn::SmemOptin(ctx));
     QCNN_CUDA(cudaFuncSetAttribute(conv_ws_kernel<NC, MB, S1, WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     if (ctx->device >= 0 && ctx->device < 64) done[ctx->device] = true;
   }
@@ -432,14 +416,14 @@ namespace qcnn {
 // x k-steps per weight stage, under the conditions of pq_gemm_tc mode 0 (or <= 3 channels per group) plus the pre-split
 // codebook and the channel-major index block of at most 32 taps.  The positions of a CTA need not fit one register pass
 // of the producers: any plane ring that fits in shared memory is a tiling.
-static void PlanConvWsS1(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands) {
+static void PlanConvWsS1(const qcnn_layer* L, int N, ConvCands* cands) {
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, taps = L->ksz * L->ksz;
   // (Cg <= 3: one chunk, half A read as scalars; wider groups: whole 4-channel halves read as float4)
   if (L->src_nchw || L->d % 4 != 0 || (Cg > 3 && (Cg % 4 != 0 || L->Cin % 4 != 0)) || L->S * L->d < Cg || taps > kMaxKSteps) return;
-  if (!L->d_ctrd_bf.get() || !L->d_asmt_t.get() || L->asmt_t_mode != 0 || RoundUp(taps, 16) > 32) return;
+  if (L->asmt_t_mode != 0 || RoundUp(taps, 16) > 32) return;
   const int PW = L->Win + L->pad, IB = (L->Hin + L->pad) * PW;
   if (L->Ho > L->Hin + L->pad || L->Wo > PW || static_cast<double>(N) * IB > 2.0e9) return;
-  const size_t smemMax = L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024;
+  const size_t smemMax = SmemOptin(L->ctx);
   // widths: every instantiated divisor of Kg from 64 up (narrower tiles re-stage the same positions for few channels),
   // or the widest divisor when all are narrower
   int widest = 0;
@@ -451,7 +435,7 @@ static void PlanConvWsS1(const qcnn_layer* L, int N, std::vector<std::pair<doubl
       const int P = 128 * MB;
       ConvPlan p;
       memset(&p, 0, sizeof(p));
-      p.kernel = kConvWs; p.CPT = P; p.threads = kWsThreads;
+      p.kernel = kConvWs; p.threads = kWsThreads;
       GemmArgs& ga = p.g;
       ga.mode = 0; ga.bf = 1;
       ga.PW = PW; ga.IB = IB; ga.NT = P;
@@ -470,8 +454,7 @@ static void PlanConvWsS1(const qcnn_layer* L, int N, std::vector<std::pair<doubl
       }
       if (!fit) continue;
       p.smem = static_cast<size_t>(MapWsSmem(ga).total);
-      p.J = ga.GT;
-      p.a.CT = W; p.a.nct = ga.nct; p.a.R = P; p.a.nstrips = ga.GT; p.a.rgroups = 1;
+      p.key = {P, ga.GT, ga.nct};
       const int stages = ga.nChunks * CeilDiv(taps, ga.GT);
       const double ne = static_cast<double>(ga.nChunks) * taps;
       // tensor work on PlanPqGemm's scale (as PlanConvWs below), a pipeline drain per weight stage, the set-up
@@ -486,24 +469,24 @@ static void PlanConvWsS1(const qcnn_layer* L, int N, std::vector<std::pair<doubl
 // weight stage (x channel tiles, stride 1).  Eligible: bf16x2 operands, an instantiated channel width, the pre-split
 // codebook and the channel-major index block; stride 1 under the conditions of pq_gemm_tc mode 0, strided layers under
 // those of its mode 1.
-void PlanConvWs(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands) {
+void PlanConvWs(const qcnn_layer* L, int N, ConvCands* cands) {
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, st = L->stride;
   if (!L->opt_tc_bf || L->K < 1 || L->K > 256) return;
   if (st == 1) { PlanConvWsS1(L, N, cands); return; }
   if (st < 2 || st > 4 || (st & 1)) return;
-  if (Cg > 4 || L->S != 1 || L->d < Cg || L->d % 4 != 0 || !L->d_ctrd_bf.get() || !L->d_asmt_t.get() || L->asmt_t_mode != 1) return;
+  if (Cg > 4 || L->S != 1 || L->d < Cg || L->d % 4 != 0 || L->asmt_t_mode != 1) return;
   if (!WsWidth(Kg)) return;
   const int PWp = CeilDiv(L->Win + 2 * L->pad, st), PHp = CeilDiv(L->Hin + 2 * L->pad, st);
   if (L->Wo > PWp) return;
   const int IB = PHp * PWp;
   if (static_cast<double>(N) * IB > 2.0e9 || static_cast<double>(L->Hin) * L->Win * L->Cin * 4 > 2.0e9) return;
-  const size_t smemMax = L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024;
+  const size_t smemMax = SmemOptin(L->ctx);
   for (int MB = 2; MB >= 1; MB--) {
     if (MB == 2 && Kg > 128) continue;   // (2 x 128 accumulator registers do not fit)
     const int P = 128 * MB;
     ConvPlan p;
     memset(&p, 0, sizeof(p));
-    p.kernel = kConvWs; p.CPT = P; p.threads = kWsThreads;
+    p.kernel = kConvWs; p.threads = kWsThreads;
     GemmArgs& ga = p.g;
     ga.mode = 1; ga.bf = 1;
     ga.PW = PWp; ga.IB = IB; ga.NT = P;
@@ -521,8 +504,7 @@ void PlanConvWs(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
     for (ga.GT = maxCnt; ga.GT >= 1 && static_cast<size_t>(MapWsSmem(ga).total) > smemMax; ga.GT--) {}
     if (ga.GT < 1) continue;
     p.smem = static_cast<size_t>(MapWsSmem(ga).total);
-    p.J = ga.GT;
-    p.a.CT = Kg; p.a.nct = 1; p.a.R = P; p.a.nstrips = ga.GT; p.a.rgroups = 1;
+    p.key = {P, ga.GT, ga.nct};
     int stages = 0;
     for (int ph = 0; ph < st; ph++) stages += CeilDiv(ga.chunkCount[ph], ga.GT);
     // tensor work on PlanPqGemm's scale (its 4 MMAs of m64 n128 k16 per k-step cost 3 * 64 * 1.15), a pipeline drain per
@@ -538,13 +520,7 @@ int LaunchConvWs(qcnn_layer* L, const ConvPlan& p, const float* src, int N, floa
   a.src = src; a.dst = dst; a.ctrd = L->d_ctrd_bf.as<float>(); a.bias = L->d_bias.as<float>();
   a.asmtT = L->d_asmt_t.as<uint8_t>();
   a.N = N; a.relu = relu;
-  a.Hi = L->Hin; a.Wi = L->Win; a.Cin = L->Cin; a.Ho = L->Ho; a.Wo = L->Wo; a.Cout = L->Cout;
-  a.ksz = L->ksz; a.pad = L->pad; a.stride = L->stride; a.G = L->grp; a.Cg = L->Cin / L->grp; a.Kg = L->Cout / L->grp;
-  a.KgPad = RoundUp(a.Kg, 16); a.S = L->S; a.K = L->K; a.d = L->d;
-  a.srcImg = static_cast<long long>(a.Hi) * a.Wi * a.Cin;
-  if (L->src_nchw) { a.rowStride = a.Wi; a.colStride = 1; a.chStride = a.Hi * a.Wi; }
-  else { a.rowStride = a.Wi * a.Cin; a.colStride = a.Cin; a.chStride = 1; }
-  a.dstImg = static_cast<long long>(a.Ho) * a.Wo * a.Cout;
+  SetGemmGeometry(L, a);
   QCNN_CHECK(a.mode == 1 || !L->src_nchw, "qcnn_conv_aprx_forward: the stride-1 weight-stationary tiling reads NHWC sources only");
   const long long blocks = static_cast<long long>(CeilDiv(N * a.IB, a.NT)) * a.G * a.nct;
   QCNN_CHECK(blocks <= 2147483647LL, "qcnn_conv_aprx_forward: batch too large for the weight-stationary tiling");
@@ -554,6 +530,23 @@ int LaunchConvWs(qcnn_layer* L, const ConvPlan& p, const float* src, int N, floa
   if (a.mode == 1) return LaunchWidth<false, false>(a, nc, nb, p.smem, st, L->ctx);
   const bool wide = 2 * a.NPOS > kWsRegPos * kWsProducers || a.Cg < 4;
   return wide ? LaunchWidth<true, true>(a, nc, nb, p.smem, st, L->ctx) : LaunchWidth<true, false>(a, nc, nb, p.smem, st, L->ctx);
+}
+
+void DescribeConvWs(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap) {
+  if (p.g.mode == 0) {
+    // stride 1: N = channels per CTA, ctiles = channel tiles per group, ksteps = chunks x taps (a CTA's k-steps), so
+    // that grid x ksteps x 32 x positions x N is the executed MAC count
+    const int stages = p.g.nChunks * CeilDiv(p.g.ntab, p.g.GT);
+    snprintf(buf, cap, " mode=0 N=%d positions=%d ctiles=%d KS=%d smem=%zuB grid=%d NPOS=%d planebufs=%d chunks=%d stages=%d "
+             "ksteps=%d", p.g.Kg / p.g.nct, p.g.NT, p.g.nct, p.g.GT, p.smem, CeilDiv(N * p.g.IB, p.g.NT) * L->grp * p.g.nct,
+             p.g.NPOS, p.g.nPB, p.g.nChunks, stages, p.g.nChunks * p.g.ntab);
+    return;
+  }
+  // (no "NT=": the executed-MAC count that bench.py derives from pq_gemm_tc( plans assumes 128-channel tiles)
+  int stages = 0;
+  for (int c = 0; c < p.g.nChunks; c++) stages += CeilDiv(p.g.chunkCount[c], p.g.GT);
+  snprintf(buf, cap, " N=%d positions=%d KS=%d smem=%zuB grid=%d NPOS=%d chunks=%d stages=%d ksteps=%d", p.g.Kg, p.g.NT,
+           p.g.GT, p.smem, CeilDiv(N * p.g.IB, p.g.NT) * L->grp, p.g.NPOS, p.g.nChunks, stages, p.g.ntab);
 }
 
 }  // namespace qcnn

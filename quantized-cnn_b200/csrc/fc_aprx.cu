@@ -459,7 +459,7 @@ static bool PlanFcTc(const qcnn_layer* L, int N, GemmArgs* out) {
   a.kPerSplit = RoundUp(CeilDiv(a.kAll, a.nsplit), kFcKs);
   a.nsplit = CeilDiv(a.kAll, a.kPerSplit);
   a.dstRow = a.nsplit > 1 ? L->DoutPad : L->Dout;
-  return PqGemmSmemBytes(a) <= (L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024);
+  return PqGemmSmemBytes(a) <= SmemOptin(L->ctx);
 }
 
 // "pq_gemm_tc mode=2 ..." when batch N takes the tensor-core path, empty otherwise (bench / DESIGN bookkeeping)

@@ -637,7 +637,7 @@ static bool PlanChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu,
   a.xFloats = xF; a.lutFloats = lutF; a.ctrdFloats = ctrdF; a.rgFloats = rgF;
   const size_t fixed = kBarBytes + sizeof(float) * (static_cast<size_t>(xF) + lutF + ctrdF + rgF + a.scrFloats);
   a.ringOff = static_cast<int>((fixed + 127) & ~static_cast<size_t>(127));
-  const size_t cap = ctx->smem_optin ? ctx->smem_optin : 227 * 1024;
+  const size_t cap = SmemOptin(ctx);
   if (static_cast<size_t>(a.ringOff) + 2 * kChunkBytes > cap) return false;
   a.nStage = static_cast<int>(std::min<size_t>(kMaxStage, (cap - a.ringOff) / kChunkBytes));
   *smemBytes = a.ringOff + static_cast<size_t>(a.nStage) * kChunkBytes;
@@ -683,7 +683,7 @@ int LaunchFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int
   if (!PlanChain(ctx, layers, relu, n, &a, &smem, &pk, &packed)) return 0;
   static bool attrSet[64] = {false};
   if (ctx->device < 64 && !attrSet[ctx->device]) {
-    const int lim = static_cast<int>(ctx->smem_optin ? ctx->smem_optin : 227 * 1024);
+    const int lim = static_cast<int>(SmemOptin(ctx));
     QCNN_CUDA(cudaFuncSetAttribute(fc_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     QCNN_CUDA(cudaFuncSetAttribute(fc_chain_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     attrSet[ctx->device] = true;

@@ -48,6 +48,7 @@
 namespace {
 
 using qcnn::BulkLoad;
+using qcnn::ByteOf32;
 using qcnn::CpAsync16;
 using qcnn::CpAsyncCommit;
 using qcnn::CpAsyncWaitAll;
@@ -55,7 +56,9 @@ using qcnn::MbarArrive;
 using qcnn::MbarExpectTx;
 using qcnn::MbarInit;
 using qcnn::MbarWait;
+using qcnn::PackBf16x2;
 using qcnn::SmemU32;
+using qcnn::SplitBf16x4;
 using qcnn::SplitTf32x4;
 using qcnn::Wgmma;
 
@@ -65,24 +68,6 @@ constexpr int kStagers = 128;    // warps 8-11
 constexpr int kMaxGT = 4;        // k-steps per stage (decoded A fragments of a stage live in registers)
 constexpr int kRegPos = 12;      // float4 a stager thread holds in registers (convolution modes: planeF4 <= 12 * 128)
 constexpr int kCbBufs = 4;       // codebook / index buffers: the decoders run ahead of the position planes
-
-// ---- bf16x2 operands: v = v1 + v2 with v1 = bf16(v), v2 = bf16(v - v1) (|v - v1 - v2| <= 2^-17 |v|).  One k-step of
-// eight values is TWO kind::f16 MMAs of K = 16: [w1 | w1] . [x1 | x2] + [w2 | w2] . [x1 | x2] = (w1 + w2)(x1 + x2) --
-// all four cross terms, at the fp16/bf16 rate (twice tf32's), against three K = 8 tf32 MMAs for 3xTF32.
-__device__ __forceinline__ uint32_t PackBf16x2(float lo, float hi) {   // low 16 bits = bf16(lo), high 16 bits = bf16(hi)
-  uint32_t r;
-  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
-}
-__device__ __forceinline__ void SplitBf16x4(const float4 v, uint2& p1, uint2& p2) {
-  p1.x = PackBf16x2(v.x, v.y);
-  p1.y = PackBf16x2(v.z, v.w);
-  // residuals against the rounded pieces (exact in fp32)
-  const float rx = v.x - __uint_as_float(p1.x << 16), ry = v.y - __uint_as_float(p1.x & 0xFFFF0000u);
-  const float rz = v.z - __uint_as_float(p1.y << 16), rw = v.w - __uint_as_float(p1.y & 0xFFFF0000u);
-  p2.x = PackBf16x2(rx, ry);
-  p2.y = PackBf16x2(rz, rw);
-}
 
 // fp32 codebook [S][K][P pieces of 4 floats] -> [S][P][K] x {w1, w2}: the K pieces of one (subspace, piece) are contiguous
 __global__ void split_codebook_kernel(const float4* __restrict__ src, uint4* __restrict__ dst, int S, int K, int P) {
@@ -97,14 +82,6 @@ __global__ void split_codebook_kernel(const float4* __restrict__ src, uint4* __r
     SplitBf16x4(src[i], p1, p2);
     dst[(sidx * P + pc) * K + k] = make_uint4(p1.x, p1.y, p2.x, p2.y);
   }
-}
-
-// byte t (< 32) of the 32 bytes {lo, hi} held in registers (t is warp-uniform: selects, no local memory)
-__device__ __forceinline__ int ByteOf32(const uint4 lo, const uint4 hi, int t) {
-  const uint32_t x = (t & 16) ? hi.x : lo.x, y = (t & 16) ? hi.y : lo.y, z = (t & 16) ? hi.z : lo.z, w = (t & 16) ? hi.w : lo.w;
-  const uint32_t xy = (t & 4) ? y : x, zw = (t & 4) ? w : z;
-  const uint32_t v = (t & 8) ? zw : xy;
-  return static_cast<int>((v >> ((t & 3) * 8)) & 0xFFu);
 }
 
 // byte t (< 48) of the 48 bytes {q0, q1, q2}
@@ -228,11 +205,11 @@ int Mode0Table(const qcnn_layer* L, GemmArgs& ga) {
   return taps;
 }
 
-// Candidate tilings for batch N (cost in SM-cycles, comparable with PlanConv's model); on-device timing chooses among them.
-void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands) {
+// Candidate tilings for batch N (cost in SM-cycles, comparable with PlanLutGather's model); on-device timing chooses among them.
+void PlanPqGemm(const qcnn_layer* L, int N, ConvCands* cands) {
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, taps = L->ksz * L->ksz;
   if (L->K < 1 || L->K > 256 || Kg % 16 != 0) return;
-  const size_t smemMax0 = L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024;
+  const size_t smemMax = SmemOptin(L->ctx);
   if (L->stride > 1) {
     // mode 1: strided convolution with one subspace over <= 4 input channels (conv1), input on stride x stride phase planes
     const int st = L->stride, rowsPer = CeilDiv(L->ksz, st);
@@ -242,15 +219,11 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
     const int PWp = CeilDiv(L->Win + 2 * L->pad, st), PHp = CeilDiv(L->Hin + 2 * L->pad, st);
     const int IB = PHp * PWp;
     if (static_cast<double>(N) * IB > 2.0e9 || static_cast<double>(L->Hin) * L->Win * L->Cin * 4 > 2.0e9) return;
-    const int nts1[2] = {128, 64};
-    for (int ni = 0; ni < 2; ni++) {
-      const int NT = nts1[ni];
-      const int gts1[2] = {4, 3};
-      for (int gi = 0; gi < 2; gi++) {
-        const int GT = gts1[gi];
+    for (const int NT : {128, 64}) {
+      for (const int GT : {4, 3}) {
         ConvPlan p;
         memset(&p, 0, sizeof(p));
-        p.kernel = kPqGemmTc; p.CPT = NT; p.J = GT; p.threads = kThreads;
+        p.kernel = kPqGemmTc; p.threads = kThreads;
         GemmArgs& ga = p.g;
         ga.mode = 1;
         ga.PW = PWp; ga.IB = IB; ga.NT = NT; ga.GT = GT;
@@ -263,7 +236,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
         ga.planeRows = ga.bf ? (st / 2) * ga.NPOS : ga.planeF4;
         ga.cbSlots = 2; ga.idRows = rowsPer * L->ksz;
         ga.tapsPad = RoundUp(rowsPer * L->ksz, 16);
-        ga.idxT = (ga.tapsPad <= 48 && L->d_asmt_t.get() && L->asmt_t_mode == 1) ? 1 : 0;
+        ga.idxT = (ga.tapsPad <= 48 && L->asmt_t_mode == 1) ? 1 : 0;
         if (ga.idxT) ga.idRows = ga.tapsPad;       // [128 channels][tapsPad] bytes
         ga.nChunks = st;
         ga.K = L->K; ga.cbF4 = L->K; ga.nPB = 2;
@@ -274,8 +247,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
         const int ne = Mode1Table(L, ga);
         if (ne > kMaxKSteps) continue;
         p.smem = static_cast<size_t>(MapSmem(ga).total);
-        if (p.smem > smemMax0) continue;
-        p.a.CT = 128; p.a.nct = ga.nct; p.a.R = NT; p.a.nstrips = GT;
+        if (p.smem > smemMax) continue;
         const double ctas0 = static_cast<double>(CeilDiv(N * IB, NT)) * G * ga.nct;
         // small batches: split the phase rows over CTAs (partial sums reduced by LaunchSplitReduce)
         for (int nsplit = 1; nsplit <= st; nsplit *= 2) {
@@ -283,7 +255,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
           ga.kPerSplit = CeilDiv(st, nsplit);
           ga.nsplit = CeilDiv(st, ga.kPerSplit);
           if (ga.nsplit != nsplit) continue;
-          p.a.rgroups = nsplit;
+          p.key = {NT, GT, ga.nct, nsplit};
           const double perCta = ne * 3.0 * (NT / 2.0) * 1.15 / nsplit + 120.0 * ne / GT / nsplit + 9000.0 + NT * 24.0 +
                                 (nsplit > 1 ? 6000.0 : 0.0);
           cands->emplace_back(perCta * std::ceil(ctas0 * nsplit / L->ctx->sm_count), p);
@@ -297,16 +269,11 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
   const int PW = L->Win + L->pad, IB = (L->Hin + L->pad) * PW;
   if (L->Ho > L->Hin + L->pad || L->Wo > PW) return;
   if (static_cast<double>(N) * IB > 2.0e9) return;
-  const size_t smemMax = L->ctx->smem_optin ? L->ctx->smem_optin : 227 * 1024;
-  const int nts[2] = {128, 64};
-  for (int ni = 0; ni < 2; ni++) {
-    const int NT = nts[ni];
-    const int gts[2] = {4, 3};
-    for (int gi = 0; gi < 2; gi++) {
-      const int GT = gts[gi];
+  for (const int NT : {128, 64}) {
+    for (const int GT : {4, 3}) {
       ConvPlan p;
       memset(&p, 0, sizeof(p));
-      p.kernel = kPqGemmTc; p.CPT = NT; p.J = GT; p.threads = kThreads;
+      p.kernel = kPqGemmTc; p.threads = kThreads;
       GemmArgs& ga = p.g;
       ga.mode = 0;
       ga.PW = PW; ga.IB = IB; ga.NT = NT; ga.GT = GT;
@@ -319,7 +286,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
       ga.planeRows = ga.bf ? ga.NPOS : ga.planeF4;   // (bf16x2: lbo = NPOS rows is the x1 -> x2 plane distance as well)
       ga.cbSlots = 2; ga.idRows = 2 * taps;
       ga.tapsPad = RoundUp(taps, 16);
-      ga.idxT = (ga.tapsPad <= 32 && L->d_asmt_t.get() && L->asmt_t_mode == 0) ? 1 : 0;
+      ga.idxT = (ga.tapsPad <= 32 && L->asmt_t_mode == 0) ? 1 : 0;
       if (ga.idxT) ga.idRows = 2 * ga.tapsPad;      // [half][128 channels][tapsPad] bytes = 2 * tapsPad rows of 128
       ga.nChunks = CeilDiv(Cg, 8);
       Mode0Table(L, ga);
@@ -327,7 +294,6 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
       ga.nct = CeilDiv(Kg, 128);
       p.smem = static_cast<size_t>(MapSmem(ga).total);
       if (p.smem > smemMax) continue;
-      p.a.CT = 128; p.a.nct = ga.nct; p.a.R = NT; p.a.nstrips = GT;   // (candidate de-duplication keys)
       const double ksteps = static_cast<double>(ga.nChunks) * taps;
       const double ctas0 = static_cast<double>(CeilDiv(N * IB, NT)) * G * ga.nct;
       // small batches: split the 8-channel chunks over CTAs (partial sums reduced by LaunchSplitReduce)
@@ -336,7 +302,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
         ga.kPerSplit = CeilDiv(ga.nChunks, nsplit);
         ga.nsplit = CeilDiv(ga.nChunks, ga.kPerSplit);
         if (ga.nsplit != nsplit) continue;
-        p.a.rgroups = nsplit;
+        p.key = {NT, GT, ga.nct, nsplit};
         const double perCta = ksteps * 3.0 * (NT / 2.0) * 1.1 / nsplit + 120.0 * ksteps / GT / nsplit + 4000.0 + NT * 24.0 +
                               (nsplit > 1 ? 6000.0 : 0.0);
         cands->emplace_back(perCta * std::ceil(ctas0 * nsplit / L->ctx->sm_count), p);
@@ -349,7 +315,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPl
 static int SetSmemLimitOnce(qcnn_ctx* ctx) {
   static bool done[64] = {false};
   if (ctx->device >= 0 && ctx->device < 64 && done[ctx->device]) return 0;
-  const int lim = static_cast<int>(ctx->smem_optin ? ctx->smem_optin : 227 * 1024);
+  const int lim = static_cast<int>(SmemOptin(ctx));
 #define QCNN_SMEM_ATTR(...) QCNN_CUDA(cudaFuncSetAttribute(pq_gemm_tc_kernel<__VA_ARGS__>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim))
   QCNN_SMEM_ATTR(true, 128); QCNN_SMEM_ATTR(true, 64); QCNN_SMEM_ATTR(false, 128); QCNN_SMEM_ATTR(false, 64);
 #undef QCNN_SMEM_ATTR
@@ -396,6 +362,16 @@ int BuildCtrdBf(qcnn_layer* L) {
   return 0;
 }
 
+void SetGemmGeometry(const qcnn_layer* L, GemmArgs& a) {
+  a.Hi = L->Hin; a.Wi = L->Win; a.Cin = L->Cin; a.Ho = L->Ho; a.Wo = L->Wo; a.Cout = L->Cout;
+  a.ksz = L->ksz; a.pad = L->pad; a.stride = L->stride; a.G = L->grp; a.Cg = L->Cin / L->grp; a.Kg = L->Cout / L->grp;
+  a.KgPad = RoundUp(a.Kg, 16); a.S = L->S; a.K = L->K; a.d = L->d;
+  a.srcImg = static_cast<long long>(a.Hi) * a.Wi * a.Cin;
+  if (L->src_nchw) { a.rowStride = a.Wi; a.colStride = 1; a.chStride = a.Hi * a.Wi; }
+  else { a.rowStride = a.Wi * a.Cin; a.colStride = a.Cin; a.chStride = 1; }
+  a.dstImg = static_cast<long long>(a.Ho) * a.Wo * a.Cout;
+}
+
 int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
   GemmArgs a = p.g;
   a.src = src; a.dst = dst; a.ctrd = L->d_ctrd.as<float>(); a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
@@ -405,13 +381,7 @@ int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, floa
   if (a.mode == 1 && !a.bulkC) a.idxT = 0;   // (3xTF32 operands: index rows by cp.async in tap-major order; the planned buffer is large enough)
   a.N = N; a.relu = a.nsplit > 1 ? 0 : relu;
   if (a.nsplit < 1) a.nsplit = 1;
-  a.Hi = L->Hin; a.Wi = L->Win; a.Cin = L->Cin; a.Ho = L->Ho; a.Wo = L->Wo; a.Cout = L->Cout;
-  a.ksz = L->ksz; a.pad = L->pad; a.stride = L->stride; a.G = L->grp; a.Cg = L->Cin / L->grp; a.Kg = L->Cout / L->grp;
-  a.KgPad = RoundUp(a.Kg, 16); a.S = L->S; a.K = L->K; a.d = L->d;
-  a.srcImg = static_cast<long long>(a.Hi) * a.Wi * a.Cin;
-  if (L->src_nchw) { a.rowStride = a.Wi; a.colStride = 1; a.chStride = a.Hi * a.Wi; }
-  else { a.rowStride = a.Wi * a.Cin; a.colStride = a.Cin; a.chStride = 1; }
-  a.dstImg = static_cast<long long>(a.Ho) * a.Wo * a.Cout;
+  SetGemmGeometry(L, a);
   const long long blocks = static_cast<long long>(CeilDiv(N * a.IB, a.NT)) * a.G * a.nct * a.nsplit;
   QCNN_CHECK(blocks <= 2147483647LL, "qcnn_conv_aprx_forward: batch too large for the tensor-core tiling");
   if (a.nsplit > 1) {
@@ -423,6 +393,15 @@ int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, floa
   if (a.nsplit > 1)
     return LaunchSplitReduce(L->ctx, a.partial, dst, N * a.Ho * a.Wo, a.Cout, a.Cout, a.nsplit, relu, st);
   return 0;
+}
+
+void DescribePqGemm(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap) {
+  int ksteps = 0;
+  for (int c = 0; c < p.g.nChunks; c++) ksteps += p.g.chunkCount[p.g.mode == 1 ? c : 0];
+  snprintf(buf, cap, "(wgmma, weights decoded into registers%s) mode=%d NT=%d GT=%d smem=%zuB grid=%d NPOS=%d "
+           "chunks=%d ksteps=%d nsplit=%d", p.g.bf ? ", bf16x2" : "", p.g.mode, p.g.NT, p.g.GT, p.smem,
+           CeilDiv(N * p.g.IB, p.g.NT) * L->grp * p.g.nct * std::max(1, p.g.nsplit), p.g.NPOS, p.g.nChunks,
+           ksteps / std::max(1, p.g.nsplit), std::max(1, p.g.nsplit));
 }
 
 // generic entry for callers that fill GemmArgs themselves (the fully-connected path in fc_aprx.cu)

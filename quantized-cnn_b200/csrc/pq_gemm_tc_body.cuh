@@ -1,6 +1,6 @@
 // Body of the decode-at-use GEMM kernels (pq_gemm_tc.cu), included inside pq_gemm_tc_kernel and pq_gemm_tc_packed_kernel:
 // in scope are the kernel parameter `a` (GemmArgs), the template parameters BF and NT, and PK / pkBits / pkPitch (mode 2
-// index rows come from a bit-packed FC table).  Not a header: no include guard.
+// index rows come from a bit-packed FC table), and the device helpers of wgmma.h.  Not a header: no include guard.
   constexpr int NTHR = kThreads;
   constexpr int NSTG = kStagers;
   constexpr int RP = kRegPos;

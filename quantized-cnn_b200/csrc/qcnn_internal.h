@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <array>
 #include <string>
 #include <utility>
 #include <vector>
@@ -67,6 +68,9 @@ struct qcnn_ctx {
 };
 
 namespace qcnn {
+
+// dynamic shared memory a block may opt in to (the H100's 227 KiB when the device did not report it)
+inline size_t SmemOptin(const qcnn_ctx* ctx) { return ctx->smem_optin ? ctx->smem_optin : 227 * 1024; }
 
 // The one owner of every device allocation the library makes for itself (layer parameters, scratch, executor staging).
 // Invariant: bytes() > 0 if and only if get() owns that many bytes on device().  Freed on destruction.
@@ -232,10 +236,12 @@ enum ConvKernel {
 
 struct ConvPlan {
   int kernel;           // ConvKernel
-  int CPT, J;
+  int CPT, J;           // LUT + gather kernels: channels per thread / positions per lane (conv_direct: output rows)
   int threads;
   size_t smem;
-  ConvArgs a;           // geometry + tiling (pointers/N filled at launch)
+  std::array<int, 6> key;   // equal keys of one kernel: near-duplicates.  LUT + gather: CPT, J, nct, nstrips, rgroups, R;
+                            // pq_gemm_tc: NT, GT, nct, nsplit; conv_ws: positions, GT, nct (unused entries 0)
+  ConvArgs a;           // kernels 0-4: geometry + tiling (pointers/N filled at launch)
   GemmArgs g;           // kernels 6 (pq_gemm_tc) and 7 (conv_ws)
 };
 
@@ -254,8 +260,8 @@ struct qcnn_layer {
   qcnn::DeviceBuffer d_ctrd;    // float
   qcnn::DeviceBuffer d_asmt;    // uint8_t
   int asmt_t_mode = 0;    // layout of d_asmt_t: 0 = [grp][S][KgPad][tapsPad] (stride 1), 1 = [grp][stride phase rows][KgPad][rowsPad] (strided, S = 1)
-  qcnn::DeviceBuffer d_asmt_t;  // conv layers: the same indices as [grp][S][KgPad][tapsPad] (tapsPad = taps rounded up to 16): a decoder thread
-                                // (= channel) reads all taps of a chunk with one or two 128-bit loads (pq_gemm_tc.cu, mode 0)
+  qcnn::DeviceBuffer d_asmt_t;  // every conv layer: the same indices channel-major (layout: asmt_t_mode; tapsPad = taps rounded up to 16): a
+                                // decoder thread (= channel) reads a chunk's taps with one or two 128-bit loads (pq_gemm_tc.cu modes 0-1, conv_ws.cu)
   qcnn::DeviceBuffer d_bias;    // float
   int kshift = 0;       // FC: stored assignment = idx << kshift
   int asmt_bits = 0;    // FC: 0 = d_asmt is the byte table [S][DoutPad]; 4..7 = bit-packed rows of asmt_pitch bytes (packed_asmt.h)
@@ -269,7 +275,7 @@ struct qcnn_layer {
   // FC scratch
   qcnn::DeviceBuffer d_partial;  // float
   qcnn::DeviceBuffer d_flat;     // tensor-core FC path: source pre-split into hi/lo plane images (fc_prep_kernel)
-  qcnn::DeviceBuffer d_ctrd_bf;  // codebook pre-split into bf16 pieces (pq_gemm_tc.cu, bf16x2 operands): [S][d/4 pieces][K] x {w1 (4 x bf16), w2 (4 x bf16)}: a (subspace, piece) slice is contiguous
+  qcnn::DeviceBuffer d_ctrd_bf;  // present exactly when d % 4 == 0: codebook pre-split into bf16 pieces (pq_gemm_tc.cu, conv_ws.cu, bf16x2 operands): [S][d/4 pieces][K] x {w1 (4 x bf16), w2 (4 x bf16)}: a (subspace, piece) slice is contiguous
   qcnn::DeviceBuffer d_cpart;    // chain kernel (fc_chain.cu): per-CTA partial sums [sm_count][DoutPad], words double as ready flags
   // tuning overrides (0 = automatic)
   int opt_fc_nsplit = 0;
@@ -286,9 +292,17 @@ struct qcnn_layer {
 
 namespace qcnn {
 
+// conv_plan.cu: the choice among the conv kernel families, their launch and describe()
 int PlanConv(qcnn_layer* L, int N);
 int DescribeConv(qcnn_layer* L, int N, char* buf, size_t cap);
 int LaunchConv(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st);
+// Every conv family provides a planner (candidate tilings for batch N, each with its cost in SM-cycles on one scale), a
+// launch of a plan and a describe() that writes the plan's text after the family's name (conv_plan.cu adds the name).
+using ConvCands = std::vector<std::pair<double, ConvPlan>>;
+// conv_aprx.cu: the LUT + gather kernels (ids 0-4)
+void PlanLutGather(const qcnn_layer* L, int N, ConvCands* cands);
+int LaunchLutGather(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
+void DescribeLutGather(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap);
 int LaunchFc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st);
 // fc_chain.cu: one persistent launch for a run of consecutive FC layers at batch <= 4 (relu[l]: ReLU after layer l)
 bool FcChainEligible(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int n, int N);
@@ -296,7 +310,9 @@ void DescribeFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, 
 int LaunchFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int n, const float* src, int N, float* dst,
                   cudaStream_t st, unsigned long long* dbg, bool* handled);
 // pq_gemm_tc.cu
-void PlanPqGemm(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands);
+void PlanPqGemm(const qcnn_layer* L, int N, ConvCands* cands);
+void DescribePqGemm(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap);
+void SetGemmGeometry(const qcnn_layer* L, GemmArgs& a);   // a conv layer's geometry and image strides, at launch
 size_t PqGemmSmemBytes(const GemmArgs& a);
 // asmtBits != 0 (mode 2): a.asmt is the bit-packed FC table of packed_asmt.h with rows of asmtPitch bytes
 int LaunchPqGemmArgs(qcnn_ctx* ctx, const GemmArgs& a, long long blocks, cudaStream_t st, int asmtBits = 0, int asmtPitch = 0);
@@ -310,8 +326,9 @@ int Mode0Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a stride
 int Mode1Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a strided layer on bf16x2 / tf32 phase planes
 // conv_ws.cu: the tensor-core family's weight-stationary tilings of stride-1 layers (mode-0 geometry, channel tiles) and
 // of strided narrow-input layers (mode-1 geometry)
-void PlanConvWs(const qcnn_layer* L, int N, std::vector<std::pair<double, ConvPlan>>* cands);
+void PlanConvWs(const qcnn_layer* L, int N, ConvCands* cands);
 int LaunchConvWs(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
+void DescribeConvWs(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap);
 
 int LaunchRelu(qcnn_ctx* ctx, const float* src, float* dst, size_t n, cudaStream_t st);
 int LaunchLrn(qcnn_ctx* ctx, const float* src, float* dst, size_t pixels, int C, int size, float alpha, float beta,

@@ -36,6 +36,31 @@ __device__ __forceinline__ void SplitTf32x4(const float4 v, float4& hi, float4& 
   SplitTf32(v.w, hi.w, lo.w);
 }
 
+// bf16x2 operand split: v = v1 + v2 with v1 = bf16(v), v2 = bf16(v - v1) (|v - v1 - v2| <= 2^-17 |v|).  One k-step of
+// eight values is TWO kind::f16 MMAs of K = 16: [w1 | w1] . [x1 | x2] + [w2 | w2] . [x1 | x2] = (w1 + w2)(x1 + x2) --
+// all four cross terms, at the fp16/bf16 rate (twice tf32's), against three K = 8 tf32 MMAs for 3xTF32.
+__device__ __forceinline__ uint32_t PackBf16x2(float lo, float hi) {   // low 16 bits = bf16(lo), high 16 bits = bf16(hi)
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// four values: p1 = their v1 pieces, p2 = their v2 pieces (the residuals are exact in fp32)
+__device__ __forceinline__ void SplitBf16x4(const float4 v, uint2& p1, uint2& p2) {
+  p1.x = PackBf16x2(v.x, v.y);
+  p1.y = PackBf16x2(v.z, v.w);
+  p2.x = PackBf16x2(v.x - __uint_as_float(p1.x << 16), v.y - __uint_as_float(p1.x & 0xFFFF0000u));
+  p2.y = PackBf16x2(v.z - __uint_as_float(p1.y << 16), v.w - __uint_as_float(p1.y & 0xFFFF0000u));
+}
+
+// byte t (< 32) of the 32 bytes {lo, hi} held in registers, e.g. a channel's tap indices (t is warp-uniform: selects,
+// no local memory)
+__device__ __forceinline__ int ByteOf32(const uint4 lo, const uint4 hi, int t) {
+  const uint32_t x = (t & 16) ? hi.x : lo.x, y = (t & 16) ? hi.y : lo.y, z = (t & 16) ? hi.z : lo.z, w = (t & 16) ? hi.w : lo.w;
+  const uint32_t xy = (t & 4) ? y : x, zw = (t & 4) ? w : z;
+  const uint32_t v = (t & 8) ? zw : xy;
+  return static_cast<int>((v >> ((t & 3) * 8)) & 0xFFu);
+}
+
 template <int N> struct Wgmma;
 
 template <> struct Wgmma<32> {
