@@ -84,7 +84,11 @@ QCNN_API int qcnn_conv_layer_set_src_nchw(qcnn_layer* layer, int enable);
  * (k-steps per stage of those tilings, 0 = any), "gemm_nsplit" (their K-split factor, 0 = any), "gemm_ct" (channels per
  * CTA of the conv_ws tilings, 0 = any; a pin that no tiling of the layer matches makes the forward fail), "autotune"
  * (0 = keep the cost model's first tiling instead of timing the candidates of the chosen family on the device);
- * FC layers only: "asmt_packed" (1 = keep the assignment table in device memory bit-packed at b = log2(K) bits per
+ * FC layers only: "fc_ws" (1 = at N >= 96 with bf16x2 operands, run the layer as a weight-stationary
+ * GEMM, describe() "pq_gemm_tc_ws(...) mode=2"; 0 = pq_gemm_tc mode 2, the default of a standalone layer; the network
+ * executor sets 1 on every FC layer it creates), where "gemm_nt" (images per CTA: 128 / 256), "gemm_gt" (k-steps per
+ * stage: 8 / 4), "gemm_ct" (channels per CTA: 64 / 128 / 256) and "gemm_nsplit" (K-split) restrict its tilings, and
+ * "asmt_packed" (1 = keep the assignment table in device memory bit-packed at b = log2(K) bits per
  * index instead of one byte, and unpack it inside the FC kernels; 0 = the byte table, the default).  Switching repacks the
  * table on the host, waits for the work queued on the layer's device, frees the previous table and makes graphs captured
  * before stale.  Every FC path (batch <= 4 chain, gather kernel, tensor-core GEMM) makes the same plan and adds the same

@@ -28,6 +28,7 @@
 //   epilogue    the consumers add the bias (+ ReLU) and store pairs of consecutive channels of one NHWC pixel.
 #include "qcnn_internal.h"
 #include "wgmma.h"
+#include "ws_common.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -37,20 +38,15 @@
 namespace {
 
 using qcnn::ByteOf32;
+using qcnn::kWsConsumers;
+using qcnn::kWsProducers;
+using qcnn::kWsThreads;
 using qcnn::MbarArrive;
-using qcnn::MbarInit;
 using qcnn::MbarWait;
 using qcnn::SmemU32;
 using qcnn::SplitBf16x4;
-using qcnn::WgmmaDesc;
 
-constexpr int kWsThreads = 384;
-constexpr int kWsConsumers = 256;   // warps 0-7
-constexpr int kWsProducers = 128;   // warps 8-11
 constexpr int kWsRegPos = 8;        // mode 0: float4 of a chunk's planes a producer thread stages per register pass
-
-// the four producer warps only (named barrier 1; barrier 0 is __syncthreads)
-__device__ __forceinline__ void ProducerSync() { asm volatile("bar.sync 1, %0;" :: "n"(kWsProducers) : "memory"); }
 
 // Shared-memory carve, read by the planner (fits / does not fit) and by the kernel.  a.NT = positions per CTA,
 // a.GT = k-steps per weight stage (KS), a.Kg / a.nct = channels per CTA (N of the MMA), a.nPB = plane buffers (mode 1:
@@ -110,11 +106,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
   if (!S1)
     for (int k = tid; k < a.K; k += kWsThreads) cb[k] = __ldg(reinterpret_cast<const uint4*>(a.ctrd) + k);
   for (int c = tid; c < NC; c += kWsThreads) biasS[c] = __ldg(a.bias + g * a.Kg + ch0 + c);
-  if (tid == 0) {
-    for (int i = 0; i < nPB; i++) { MbarInit(fullP + i, kWsProducers); MbarInit(emptyP + i, kWsConsumers / 32); }
-    for (int i = 0; i < 2; i++) { MbarInit(fullW + i, kWsProducers); MbarInit(emptyW + i, kWsConsumers / 32); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  if (tid == 0) qcnn::WsInitBarriers(fullP, emptyP, nPB, kWsProducers, fullW, emptyW);
   __syncthreads();
 
   const int warpU = __shfl_sync(0xffffffffu, warp, 0);   // provably warp-uniform role selector
@@ -225,12 +217,12 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
         const int sB = okB ? chB / a.d : 0, jB = okB ? chB - sB * a.d : 0;
         const uint4* cA = reinterpret_cast<const uint4*>(a.ctrd) + static_cast<size_t>(sA * (a.d >> 2) + (jA >> 2)) * a.K;
         const uint4* cB = reinterpret_cast<const uint4*>(a.ctrd) + static_cast<size_t>(sB * (a.d >> 2) + (jB >> 2)) * a.K;
-        ProducerSync();   // every producer is done decoding from the previous chunk's slices
+        qcnn::WsProducerSync();   // every producer is done decoding from the previous chunk's slices
         for (int k = pt; k < a.K; k += kWsProducers) {
           cb[k] = __ldg(cA + k);
           cb[a.K + k] = okB ? __ldg(cB + k) : make_uint4(0u, 0u, 0u, 0u);
         }
-        ProducerSync();
+        qcnn::WsProducerSync();
         // weights of the chunk's stages: a thread owns channel c, its tap indices of either half are one or two 16-byte
         // granules of the channel-major block d_asmt_t ([grp][S][KgPad][tapsPad])
         const uint8_t* rowA = a.asmtT + (static_cast<size_t>(g * a.S + sA) * a.KgPad + ch0) * a.tapsPad;
@@ -338,24 +330,16 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
       for (int e = 0; e < n; e++) {
         const KStep ks = a.tab[first + s0 + e];
         const uint32_t wb = wts0 + static_cast<uint32_t>((b * KS + e) * 2 * NC) * 16u;
-        const uint64_t d1 = WgmmaDesc(wb, 0, 128), d2 = WgmmaDesc(wb + NC * 16, 0, 128);
-#pragma unroll
-        for (int m = 0; m < MB; m++) {
-          const uint64_t dA = WgmmaDesc(plA + static_cast<uint32_t>(ks.bStart + m * 64) * 16u, static_cast<uint32_t>(a.planeRows) * 16u, 128);
-          qcnn::WgmmaSS<NC>::Bf16(acc[m], dA, d1);
-          qcnn::WgmmaSS<NC>::Bf16(acc[m], dA, d2);
-        }
+        qcnn::WsMmaKStep<NC, MB>(acc, plA, ks.bStart, static_cast<uint32_t>(a.planeRows) * 16u, wb);
       }
-      qcnn::WgmmaCommit();
-      qcnn::WgmmaWaitAll();
-      __syncwarp();
-      if (lane == 0) MbarArrive(emptyW + b);
+      qcnn::WsRetireStage(emptyW + b, lane);
     }
     if (S1 && lane == 0) MbarArrive(emptyP + pb);   // (the chunk's MMAs have retired: the last stage waited for them)
   }
 
   // ---- epilogue: accumulator fragments (rows = positions r0, r0 + 8; columns = channels 8 i + 2 t4, +1) -> NHWC ----
-  const int r0 = (warp & 3) * 16 + (lane >> 2), t4 = lane & 3;
+  const qcnn::WsFrag fr = qcnn::WsFragOf(warp, lane);
+  const int r0 = fr.r0, t4 = fr.t4;
   const bool v2 = (reinterpret_cast<uintptr_t>(a.dst) & 7u) == 0;   // (Cout, g * Kg and ch0 are even: pairs are 8-byte aligned)
 #pragma unroll
   for (int m = 0; m < MB; m++) {

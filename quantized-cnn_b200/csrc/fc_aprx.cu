@@ -406,7 +406,7 @@ int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows,
   return 0;
 }
 
-static bool FcTcEligible(const qcnn_layer* L, int N) {
+bool FcTcEligible(const qcnn_layer* L, int N) {
   static const char* env = getenv("QCNN_FC_TC");
   if (env && env[0] == '0') return false;
   if (!(env && env[0] == '1') && N < 96) return false;
@@ -462,13 +462,36 @@ static bool PlanFcTc(const qcnn_layer* L, int N, GemmArgs* out) {
   return PqGemmSmemBytes(a) <= SmemOptin(L->ctx);
 }
 
-// "pq_gemm_tc mode=2 ..." when batch N takes the tensor-core path, empty otherwise (bench / DESIGN bookkeeping)
-void DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap) {
+// "pq_gemm_tc_ws(...) mode=2 ..." or "pq_gemm_tc(...) mode=2 ..." when batch N takes a tensor-core path, empty otherwise
+// (bench / DESIGN bookkeeping)
+int DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap) {
   buf[0] = 0;
+  bool ws = false;
+  if (int rc = DescribeFcWs(L, N, buf, cap, &ws)) return rc;
+  if (ws) return 0;
   GemmArgs a;
-  if (!PlanFcTc(L, N, &a)) return;
+  if (!PlanFcTc(L, N, &a)) return 0;
   snprintf(buf, cap, "pq_gemm_tc(wgmma, weights decoded into registers%s) mode=2 NT=%d GT=3 grid=%d nsplit=%d ksteps=%d",
            a.bf ? ", bf16x2" : "", a.NT, CeilDiv(N, a.NT) * a.nsplit * a.nct, a.nsplit, a.kPerSplit);
+  return 0;
+}
+
+// The activations as the plane image of every (image tile, chunk): NT images per tile, KS k-steps per chunk, bf16x2
+// (fc_prep_bf_kernel) or 3xTF32 (fc_prep_kernel) pieces, in L->d_flat
+int PrepFcPlanes(qcnn_layer* L, const float* src, int N, int NT, int KS, int nChunksAll, bool bf, cudaStream_t st) {
+  qcnn_ctx* ctx = L->ctx;
+  const int tiles = CeilDiv(N, NT);
+  const size_t total = static_cast<size_t>(tiles) * nChunksAll * KS * NT * (bf ? 1 : 2);   // 16-byte rows of one plane (hi or lo)
+  QCNN_CUDA(L->d_flat.Reserve(ctx, total * 2 * sizeof(float4), st));
+  if (bf)
+    fc_prep_bf_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(src, L->d_srcoff.as<int>(), L->d_flat.as<uint4>(),
+                                                                               N, L->Din, NT, KS, nChunksAll, tiles);
+  else
+    fc_prep_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(src, L->d_srcoff.as<int>(), L->d_flat.as<float4>(),
+                                                                            N, L->Din, NT, KS, nChunksAll, tiles);
+  QCNN_CUDA(cudaGetLastError());
+  ctx->launches++;
+  return 0;
 }
 
 int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled) {
@@ -479,19 +502,8 @@ int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
   const int tiles = CeilDiv(N, a.NT);
   a.src = src; a.dst = dst;
   a.relu = a.nsplit > 1 ? 0 : relu;
-  {
-    const size_t total = static_cast<size_t>(tiles) * a.nChunksAll * a.planeRows;   // 16-byte rows of one plane (hi or lo)
-    QCNN_CUDA(L->d_flat.Reserve(ctx, total * 2 * sizeof(float4), st));
-    a.xprep = L->d_flat.as<float>();
-    if (a.bf)
-      fc_prep_bf_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(src, L->d_srcoff.as<int>(), L->d_flat.as<uint4>(),
-                                                                                 N, L->Din, a.NT, kFcKs, a.nChunksAll, tiles);
-    else
-      fc_prep_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(src, L->d_srcoff.as<int>(), L->d_flat.as<float4>(),
-                                                                              N, L->Din, a.NT, kFcKs, a.nChunksAll, tiles);
-    QCNN_CUDA(cudaGetLastError());
-    ctx->launches++;
-  }
+  if (int rc = PrepFcPlanes(L, src, N, a.NT, kFcKs, a.nChunksAll, a.bf != 0, st)) return rc;
+  a.xprep = L->d_flat.as<float>();
   if (a.nsplit > 1) {
     QCNN_CUDA(L->d_partial.Reserve(ctx, sizeof(float) * static_cast<size_t>(a.nsplit) * N * L->DoutPad, st));
     a.partial = L->d_partial.as<float>();
@@ -511,6 +523,9 @@ int LaunchFc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaS
     bool handled = false;
     // batch <= 4: the persistent assignment-stream kernel (fc_chain.cu), here as a chain of one layer
     if (int rc = LaunchFcChain(L->ctx, &L, &relu, 1, src, N, dst, st, nullptr, &handled)) return rc;
+    if (handled) return 0;
+    // fc_ws = 1: the weight-stationary GEMM where it applies (bf16x2 operands), else pq_gemm_tc mode 2
+    if (int rc = LaunchFcWs(L, src, N, dst, relu, st, &handled)) return rc;
     if (handled) return 0;
     if (int rc = LaunchFcTc(L, src, N, dst, relu, st, &handled)) return rc;
     if (handled) return 0;

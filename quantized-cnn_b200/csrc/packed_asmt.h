@@ -52,6 +52,26 @@ __device__ __forceinline__ void UnpackFields(const uint32_t (&w)[NW], uint32_t s
     idx[c] = v & ((1u << B) - 1u);
   }
 }
+
+// The tensor-core FC GEMMs (pq_gemm_tc mode 2, fc_ws) with a bit-packed table: the 16 indices of channels [ch, ch + 16)
+// of one row (2 b bytes, from the four aligned words that cover them) -> 16 bytes idx << kshift at dst, the index block
+// the byte table would stage
+__device__ __forceinline__ void StagePackedRow(uint8_t* dst, const uint8_t* row, int ch, int b, int kshift) {
+  const uint32_t bit0 = static_cast<uint32_t>(ch) * b, sh = bit0 & 31u;
+  const uint32_t* wp = reinterpret_cast<const uint32_t*>(row) + (bit0 >> 5);
+  const uint32_t w0 = __ldg(wp), w1 = __ldg(wp + 1), w2 = __ldg(wp + 2), w3 = __ldg(wp + 3);
+  const uint32_t u0 = __funnelshift_r(w0, w1, sh), u1 = __funnelshift_r(w1, w2, sh), u2 = __funnelshift_r(w2, w3, sh), u3 = w3 >> sh;
+  const uint32_t mask = (1u << b) - 1u;
+  uint32_t o[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+  for (int c = 0; c < 16; c++) {
+    const int pos = c * b, j = pos >> 5;   // (16 b + sh <= 128 bits: the fields end inside u3)
+    const uint32_t lo = j == 0 ? u0 : (j == 1 ? u1 : (j == 2 ? u2 : u3));
+    const uint32_t hi = j == 0 ? u1 : (j == 1 ? u2 : (j == 2 ? u3 : 0u));
+    o[c >> 2] |= ((__funnelshift_r(lo, hi, pos & 31) & mask) << kshift) << (8 * (c & 3));
+  }
+  *reinterpret_cast<uint4*>(dst) = make_uint4(o[0], o[1], o[2], o[3]);
+}
 #endif
 
 }  // namespace qcnn

@@ -36,6 +36,7 @@
 //           phase planes so that a tap again is a shift; a k-step pairs two taps (4 floats each: channels + zero pad);
 //           a chunk is one phase row;
 //   mode 2  fully-connected layers: position = image, a chunk is a run of k-steps over consecutive input features.
+#include "packed_asmt.h"
 #include "qcnn_internal.h"
 #include "wgmma.h"
 
@@ -60,6 +61,7 @@ using qcnn::PackBf16x2;
 using qcnn::SmemU32;
 using qcnn::SplitBf16x4;
 using qcnn::SplitTf32x4;
+using qcnn::StagePackedRow;
 using qcnn::Wgmma;
 
 constexpr int kThreads = 384;
@@ -111,25 +113,6 @@ __host__ __device__ inline SmemMap MapSmem(const GemmArgs& a) {
   m.bars = o;   o += 8 * (8 + 2 * kCbBufs);
   m.total = o;
   return m;
-}
-
-// Mode 2 with a bit-packed FC table (packed_asmt.h): the 16 indices of channels [ch, ch + 16) of one row (2 b bytes, from
-// the four aligned words that cover them) -> 16 bytes idx << kshift at dst, the index block the byte table would stage
-__device__ __forceinline__ void StagePackedRow(uint8_t* dst, const uint8_t* row, int ch, int b, int kshift) {
-  const uint32_t bit0 = static_cast<uint32_t>(ch) * b, sh = bit0 & 31u;
-  const uint32_t* wp = reinterpret_cast<const uint32_t*>(row) + (bit0 >> 5);
-  const uint32_t w0 = __ldg(wp), w1 = __ldg(wp + 1), w2 = __ldg(wp + 2), w3 = __ldg(wp + 3);
-  const uint32_t u0 = __funnelshift_r(w0, w1, sh), u1 = __funnelshift_r(w1, w2, sh), u2 = __funnelshift_r(w2, w3, sh), u3 = w3 >> sh;
-  const uint32_t mask = (1u << b) - 1u;
-  uint32_t o[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-  for (int c = 0; c < 16; c++) {
-    const int pos = c * b, j = pos >> 5;   // (16 b + sh <= 128 bits: the fields end inside u3)
-    const uint32_t lo = j == 0 ? u0 : (j == 1 ? u1 : (j == 2 ? u2 : u3));
-    const uint32_t hi = j == 0 ? u1 : (j == 1 ? u2 : (j == 2 ? u3 : 0u));
-    o[c >> 2] |= ((__funnelshift_r(lo, hi, pos & 31) & mask) << kshift) << (8 * (c & 3));
-  }
-  *reinterpret_cast<uint4*>(dst) = make_uint4(o[0], o[1], o[2], o[3]);
 }
 
 // BF: bf16x2 operands (else 3xTF32); NT: positions per CTA = wgmma N; NT = 64 keeps the second accumulator (a.corr).

@@ -322,7 +322,13 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
     L->tunedPlans.clear();
     return SetAsmtPacked(L, value);
   }
-  if (!strcmp(name, "fc_nsplit")) L->opt_fc_nsplit = value;
+  if (!strcmp(name, "fc_ws")) {
+    // FC only: 1 runs the batched tensor-core path as the weight-stationary GEMM (fc_ws.cu) where it applies (bf16x2
+    // operands, byte table), 0 (the default of a standalone layer) keeps pq_gemm_tc mode 2
+    QCNN_CHECK(L->kind == QCNN_KIND_FC, "qcnn_layer_set_param: 'fc_ws' applies to FC layers");
+    L->opt_fc_ws = value ? 1 : 0;
+  }
+  else if (!strcmp(name, "fc_nsplit")) L->opt_fc_nsplit = value;
   else if (!strcmp(name, "fc_tn")) L->opt_fc_tn = value;
   else if (!strcmp(name, "tensor_core")) {
     // 0: LUT + gather kernels only (fp32 adds in the reference's association; the strict-parity path);
@@ -332,6 +338,16 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
     L->opt_tc_bf = value == 2 ? 1 : 0;
     L->plan_N = 0; L->tuned = 0;
     L->tunedPlans.clear();
+  }
+  else if (L->kind == QCNN_KIND_FC && (!strcmp(name, "gemm_nt") || !strcmp(name, "gemm_gt") || !strcmp(name, "gemm_nsplit") ||
+                                        !strcmp(name, "gemm_ct"))) {
+    // FC with fc_ws = 1: the fc_ws tilings with that many images per CTA (128 / 256), k-steps per stage (8 / 4), K-split
+    // factor and channels per CTA (0 = any); pq_gemm_tc mode 2 has a single tiling per batch and ignores them
+    const int v = value < 0 ? 0 : value;
+    if (!strcmp(name, "gemm_nt")) L->opt_gemm_nt = v;
+    else if (!strcmp(name, "gemm_gt")) L->opt_gemm_gt = v;
+    else if (!strcmp(name, "gemm_nsplit")) L->opt_gemm_nsplit = v;
+    else L->opt_gemm_ct = v;
   }
   else if (!strcmp(name, "force_kernel") || !strcmp(name, "autotune") || !strcmp(name, "gemm_nt") ||
            !strcmp(name, "gemm_gt") || !strcmp(name, "gemm_nsplit") || !strcmp(name, "gemm_ct")) {
@@ -359,7 +375,7 @@ int qcnn_layer_describe(qcnn_layer* L, int N, char* buf, size_t cap) {
   QCNN_CHECK(L && buf && cap > 0 && N >= 1, "qcnn_layer_describe: bad argument");
   if (L->kind == QCNN_KIND_CONV) return DescribeConv(L, N, buf, cap);
   char tc[256];
-  DescribeFcTc(L, N, tc, sizeof(tc));
+  if (int rc = DescribeFcTc(L, N, tc, sizeof(tc))) return rc;
   if (N <= 4) {
     const int relu0 = 0;
     DescribeFcChain(L->ctx, &L, &relu0, 1, tc, sizeof(tc));

@@ -288,6 +288,9 @@ struct qcnn_layer {
   int opt_gemm_gt = 0;       // conv: ... to this many k-steps per stage (0 = any)
   int opt_gemm_nsplit = 0;   // conv: ... to this K-split factor (0 = any)
   int opt_gemm_ct = 0;       // conv: restrict conv_ws tilings to this many channels per CTA (0 = any)
+                             // (FC with fc_ws: gemm_nt / gemm_gt / gemm_ct / gemm_nsplit restrict the fc_ws tilings)
+  int opt_fc_ws = 0;         // FC: 1 = the batched tensor-core path runs as the weight-stationary GEMM (fc_ws.cu) where
+                             // it can, instead of pq_gemm_tc mode 2 (the network executor sets it on every FC layer)
 };
 
 namespace qcnn {
@@ -319,8 +322,16 @@ int LaunchPqGemmArgs(qcnn_ctx* ctx, const GemmArgs& a, long long blocks, cudaStr
 int BuildCtrdBf(qcnn_layer* L);   // layer creation: the bf16x2 form of the codebook (d % 4 == 0)
 int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows, int cols, int colsPad, int nsplit, int relu,
                       cudaStream_t st);
-void DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap);
+int DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap);
 int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled);
+// fc_aprx.cu: the batched FC layer may take a tensor-core GEMM (N >= 96, no gather-kernel tuning, a decodable geometry);
+// its activations as the plane image [tile][chunk][x1, x2 (3xTF32: hi, lo)][KS][NT] in L->d_flat
+bool FcTcEligible(const qcnn_layer* L, int N);
+int PrepFcPlanes(qcnn_layer* L, const float* src, int N, int NT, int KS, int nChunksAll, bool bf, cudaStream_t st);
+// fc_ws.cu: the weight-stationary FC GEMM (fc_ws = 1, bf16x2 operands); *handled = false when the layer does
+// not take it at batch N
+int LaunchFcWs(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled);
+int DescribeFcWs(const qcnn_layer* L, int N, char* buf, size_t cap, bool* handled);
 int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
 int Mode0Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a stride-1 layer on the flat padded grid
 int Mode1Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a strided layer on bf16x2 / tf32 phase planes

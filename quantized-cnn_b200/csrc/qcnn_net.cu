@@ -117,6 +117,7 @@ static int BuildNet(qcnn_ctx* ctx, int layerCnt, const qcnn_layer_info* infos, c
         const int Din = H * W * C;
         rc = qcnn_fc_layer_create(ctx, Din, li.nodCnt, lp.S, lp.K, lp.d, lp.ctrd, lp.asmt, lp.bias, &nl.pq);
         if (rc) break;
+        nl.pq->opt_fc_ws = 1;   // the weight-stationary GEMM for batched FC layers (standalone layers keep mode 2: DESIGN.md 4a)
         // first FC layer: the reference permutes its NHWC input to NCHW first (CaffeEva.cc:236-238)
         if (!seenFc && (H > 1 || W > 1)) rc = qcnn_fc_layer_set_src_nhwc(nl.pq, H, W, C);
         seenFc = true;
