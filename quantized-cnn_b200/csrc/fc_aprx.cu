@@ -22,7 +22,6 @@
 #include "packed_asmt.h"
 
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
 #include <cstdio>
 
@@ -372,13 +371,16 @@ int Launch(const FcArgs& a, int pitch, dim3 grid, cudaStream_t st) {
   return 0;
 }
 
+// subspaces per LUT chunk of the instantiation for K codewords and tn images per CTA (LaunchK's PF, PlanFcGather's pf)
+constexpr int FcChunkLen(int K, int tn) { return tn == 1 ? (K <= 64 ? 16 : 8) : (K <= 32 ? 32 : (K <= 64 ? 16 : 8)); }
+
 template <int K, bool PRE, bool PACKED = false>
 int LaunchK(const FcArgs& a, int tn, int cpt, dim3 grid, cudaStream_t st, int pitch = 0) {
-  if (cpt == 4 && tn == 8) return Launch<K, 4, 8, (K <= 32 ? 32 : (K <= 64 ? 16 : 8)), PRE, PACKED>(a, pitch, grid, st);
+  if (cpt == 4 && tn == 8) return Launch<K, 4, 8, FcChunkLen(K, 8), PRE, PACKED>(a, pitch, grid, st);
   switch (tn) {
-    case 1: return Launch<K, 16, 1, (K <= 64 ? 16 : 8), PRE, PACKED>(a, pitch, grid, st);
-    case 4: return Launch<K, 8, 4, (K <= 32 ? 32 : (K <= 64 ? 16 : 8)), PRE, PACKED>(a, pitch, grid, st);
-    default: return Launch<K, 8, 8, (K <= 32 ? 32 : (K <= 64 ? 16 : 8)), PRE, PACKED>(a, pitch, grid, st);
+    case 1: return Launch<K, 16, 1, FcChunkLen(K, 1), PRE, PACKED>(a, pitch, grid, st);
+    case 4: return Launch<K, 8, 4, FcChunkLen(K, 4), PRE, PACKED>(a, pitch, grid, st);
+    default: return Launch<K, 8, 8, FcChunkLen(K, 8), PRE, PACKED>(a, pitch, grid, st);
   }
 }
 
@@ -386,17 +388,8 @@ int LaunchK(const FcArgs& a, int tn, int cpt, dim3 grid, cudaStream_t st, int pi
 
 namespace qcnn {
 
-// chunk length (subspaces) of the instantiation chosen for (K, tn) -- must mirror LaunchK above
-static int ChunkLen(int K, int tn) {
-  if (tn == 1) return K <= 64 ? 16 : 8;
-  return K <= 32 ? 32 : (K <= 64 ? 16 : 8);
-}
-
-// Large batches: the layer as a decode-at-use GEMM on the tensor cores (pq_gemm_tc.cu, mode 2): M = 128 outputs per CTA,
-// N = up to 128 images, K split over CTAs so that the grid fills the GPU; partial sums are reduced in fixed order by
-// fc_reduce_kernel.  QCNN_FC_TC=0 keeps the gather kernel, QCNN_FC_TC=1 forces the tensor-core path for any N.
-// dst[r][c] = sum over splits of partial[split][r][c] (+ ReLU); split 0 carries the bias.  Also used by the K-split
-// convolutions of pq_gemm_tc (rows = positions).
+// dst[r][c] = sum over splits of partial[split][r][c] (+ ReLU); split 0 carries the bias.  The K-split of every FC family
+// (fc_plan.cu) and of the pq_gemm_tc convolutions (rows = positions).
 int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows, int cols, int colsPad, int nsplit, int relu,
                       cudaStream_t st) {
   const int total = rows * cols;
@@ -406,26 +399,16 @@ int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows,
   return 0;
 }
 
-bool FcTcEligible(const qcnn_layer* L, int N) {
-  static const char* env = getenv("QCNN_FC_TC");
-  if (env && env[0] == '0') return false;
-  if (!(env && env[0] == '1') && N < 96) return false;
-  if (L->opt_fc_nsplit || L->opt_fc_tn || L->opt_no_tc) return false;   // explicit gather-kernel tuning (fc_nsplit = 1: bit-exact reference order)
-  if (L->Din % 8 != 0 || !(L->d == 1 || L->d % 4 == 0) || L->S * L->d < L->Din || L->K > 256 || L->K % 4 != 0) return false;
-  return true;
-}
-
 // k-steps per chunk of the tensor-core FC path (plane image of a chunk: 2 * 3 halves x NT images, hi + lo)
 constexpr int kFcKs = 3;
 
-// The tensor-core plan of the layer at batch N (everything but the activations, the output, the plane images and the
-// partial sums); false when the layer does not take that path.
-static bool PlanFcTc(const qcnn_layer* L, int N, GemmArgs* out) {
-  if (!FcTcEligible(L, N)) return false;
-  GemmArgs& a = *out;
+// Large batches: the layer as a decode-at-use GEMM on the tensor cores (pq_gemm_tc.cu, mode 2): M = 128 outputs per CTA,
+// N = up to 128 images, K split over CTAs so that the grid fills the GPU.  Fills p->tc (everything but the pointers) and
+// p->nsplit; false when the staging does not fit in shared memory.
+bool PlanFcMode2(const qcnn_layer* L, int N, FcPlan* p) {
+  GemmArgs& a = p->tc;
   memset(&a, 0, sizeof(a));
   a.mode = 2;
-  a.ctrd = L->d_ctrd.as<float>(); a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
   a.N = N; a.Cin = L->Din; a.Cout = L->Dout; a.G = 1; a.Cg = L->Din; a.Kg = L->Dout; a.KgPad = L->DoutPad;
   a.S = L->S; a.K = L->K; a.d = L->d; a.kshift = L->kshift;
   a.srcImg = L->Din; a.dstImg = 0;
@@ -433,7 +416,7 @@ static bool PlanFcTc(const qcnn_layer* L, int N, GemmArgs* out) {
   a.NT = N > 64 ? 128 : 64;   // the two wgmma N of pq_gemm_tc
   a.corr = a.NT <= 64 ? 1 : 0;
   a.bf = L->opt_tc_bf ? 1 : 0;
-  if (a.bf && L->d_ctrd_bf.get()) { a.ctrd = L->d_ctrd_bf.as<float>(); a.cbPre = 1; }   // (d % 4 == 0)
+  a.cbPre = a.bf && L->d_ctrd_bf.get() ? 1 : 0;   // (d % 4 == 0)
   a.GT = kFcKs;
   a.nPB = 3; a.nChunksAll = CeilDiv(L->Din / 8, kFcKs);
   a.planeF4 = kFcKs * 2 * a.NT;
@@ -459,21 +442,14 @@ static bool PlanFcTc(const qcnn_layer* L, int N, GemmArgs* out) {
   a.kPerSplit = RoundUp(CeilDiv(a.kAll, a.nsplit), kFcKs);
   a.nsplit = CeilDiv(a.kAll, a.kPerSplit);
   a.dstRow = a.nsplit > 1 ? L->DoutPad : L->Dout;
+  p->nsplit = a.nsplit;
   return PqGemmSmemBytes(a) <= SmemOptin(L->ctx);
 }
 
-// "pq_gemm_tc_ws(...) mode=2 ..." or "pq_gemm_tc(...) mode=2 ..." when batch N takes a tensor-core path, empty otherwise
-// (bench / DESIGN bookkeeping)
-int DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap) {
-  buf[0] = 0;
-  bool ws = false;
-  if (int rc = DescribeFcWs(L, N, buf, cap, &ws)) return rc;
-  if (ws) return 0;
-  GemmArgs a;
-  if (!PlanFcTc(L, N, &a)) return 0;
+void DescribeFcMode2(const qcnn_layer* L, const FcPlan& p, int N, char* buf, size_t cap) {
+  const GemmArgs& a = p.tc;
   snprintf(buf, cap, "pq_gemm_tc(wgmma, weights decoded into registers%s) mode=2 NT=%d GT=3 grid=%d nsplit=%d ksteps=%d",
            a.bf ? ", bf16x2" : "", a.NT, CeilDiv(N, a.NT) * a.nsplit * a.nct, a.nsplit, a.kPerSplit);
-  return 0;
 }
 
 // The activations as the plane image of every (image tile, chunk): NT images per tile, KS k-steps per chunk, bf16x2
@@ -494,102 +470,70 @@ int PrepFcPlanes(qcnn_layer* L, const float* src, int N, int NT, int KS, int nCh
   return 0;
 }
 
-int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled) {
-  *handled = false;
-  GemmArgs a;
-  if (!PlanFcTc(L, N, &a)) return 0;   // before any launch / allocation
-  qcnn_ctx* ctx = L->ctx;
-  const int tiles = CeilDiv(N, a.NT);
-  a.src = src; a.dst = dst;
-  a.relu = a.nsplit > 1 ? 0 : relu;
+int LaunchFcMode2(qcnn_layer* L, const FcPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
+  GemmArgs a = p.tc;
+  a.src = src; a.dst = a.partial = dst; a.relu = relu;   // (partial: read with nsplit > 1 only)
+  a.ctrd = a.cbPre ? L->d_ctrd_bf.as<float>() : L->d_ctrd.as<float>();
+  a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
   if (int rc = PrepFcPlanes(L, src, N, a.NT, kFcKs, a.nChunksAll, a.bf != 0, st)) return rc;
   a.xprep = L->d_flat.as<float>();
-  if (a.nsplit > 1) {
-    QCNN_CUDA(L->d_partial.Reserve(ctx, sizeof(float) * static_cast<size_t>(a.nsplit) * N * L->DoutPad, st));
-    a.partial = L->d_partial.as<float>();
-  }
-  if (int rc = LaunchPqGemmArgs(ctx, a, static_cast<long long>(tiles) * a.nsplit * a.nct, st, L->asmt_bits, L->asmt_pitch)) return rc;
-  ctx->launches++;
-  if (a.nsplit > 1)
-    if (int rc = LaunchSplitReduce(ctx, a.partial, dst, N, L->Dout, L->DoutPad, a.nsplit, relu, st)) return rc;
-  *handled = true;
-  return 0;
+  return LaunchPqGemmArgs(L->ctx, a, static_cast<long long>(CeilDiv(N, a.NT)) * a.nsplit * a.nct, st, L->asmt_bits, L->asmt_pitch);
 }
 
-int LaunchFc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st) {
-  QCNN_CHECK(L->kind == QCNN_KIND_FC, "qcnn_fc_aprx_forward: layer is not fully-connected");
-  QCNN_CHECK(N >= 1, "qcnn_fc_aprx_forward: N must be >= 1");
-  {
-    bool handled = false;
-    // batch <= 4: the persistent assignment-stream kernel (fc_chain.cu), here as a chain of one layer
-    if (int rc = LaunchFcChain(L->ctx, &L, &relu, 1, src, N, dst, st, nullptr, &handled)) return rc;
-    if (handled) return 0;
-    // fc_ws = 1: the weight-stationary GEMM where it applies (bf16x2 operands), else pq_gemm_tc mode 2
-    if (int rc = LaunchFcWs(L, src, N, dst, relu, st, &handled)) return rc;
-    if (handled) return 0;
-    if (int rc = LaunchFcTc(L, src, N, dst, relu, st, &handled)) return rc;
-    if (handled) return 0;
-  }
-  qcnn_ctx* ctx = L->ctx;
-  FcArgs a;
-  a.src = src; a.dst = dst; a.partial = nullptr;
-  a.ctrd = L->d_ctrd.as<float>(); a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
-  a.N = N; a.Din = L->Din; a.Dout = L->Dout; a.DoutPad = L->DoutPad; a.S = L->S; a.K = L->K; a.d = L->d;
-  a.srcoff = L->d_srcoff.as<int>();
-  a.relu = relu;
-
-  // batch tile: 1 (latency path, 16 channels/thread, 128-bit loads), 4 or 8 images per CTA
+// batch tile: 1 (latency path, 16 channels/thread, 128-bit loads), 4 or 8 images per CTA; fc_tn / fc_nsplit pin the tiling
+void PlanFcGather(const qcnn_layer* L, int N, FcPlan* p) {
   int tn = L->opt_fc_tn ? L->opt_fc_tn : (N >= 8 ? 8 : (N >= 4 ? 4 : 1));
   if (tn != 1 && tn != 4) tn = 8;
   // narrow layers (fc8: 1000 outputs) take 4 channels per thread so that a 256-thread CTA is fully populated
   const int cpt = (tn == 1) ? 16 : ((tn == 8 && L->DoutPad <= 1024) ? 4 : 8);
-  const int pf = ChunkLen(L->K, tn);
-  const int gx = CeilDiv(L->DoutPad, kFcThreads * cpt);
-  const int gy = CeilDiv(N, tn);
+  const int pf = FcChunkLen(L->K, tn);
   const int chunks = CeilDiv(L->S, pf);
   int nsplit = L->opt_fc_nsplit;
   if (nsplit <= 0) {
     // aim for >= 3 CTAs of 8 warps per SM; never more splits than chunks
-    const int want = 3 * ctx->sm_count;
-    nsplit = CeilDiv(want, gx * gy);
+    const int want = 3 * L->ctx->sm_count;
+    nsplit = CeilDiv(want, CeilDiv(L->DoutPad, kFcThreads * cpt) * CeilDiv(N, tn));
   }
   nsplit = std::max(1, std::min(nsplit, chunks));
   const int chunks_per_split = CeilDiv(chunks, nsplit);
-  nsplit = CeilDiv(chunks, chunks_per_split);
-  a.s_per_split = chunks_per_split * pf;
-  a.nsplit = nsplit;
-  if (nsplit > 1) {
-    QCNN_CUDA(L->d_partial.Reserve(ctx, sizeof(float) * static_cast<size_t>(nsplit) * N * L->DoutPad, st));
-    a.partial = L->d_partial.as<float>();
-  }
-  dim3 grid(gx, gy, nsplit);
-  int rc;
+  p->nsplit = CeilDiv(chunks, chunks_per_split);
+  p->gather = {tn, cpt, chunks_per_split * pf};
+}
+
+int LaunchFcGather(qcnn_layer* L, const FcPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
+  const int tn = p.gather.tn, cpt = p.gather.cpt;
+  FcArgs a;
+  a.src = src; a.dst = dst; a.partial = p.nsplit > 1 ? dst : nullptr;
+  a.ctrd = L->d_ctrd.as<float>(); a.asmt = L->d_asmt.as<uint8_t>(); a.bias = L->d_bias.as<float>();
+  a.N = N; a.Din = L->Din; a.Dout = L->Dout; a.DoutPad = L->DoutPad; a.S = L->S; a.K = L->K; a.d = L->d;
+  a.srcoff = L->d_srcoff.as<int>();
+  a.relu = relu;
+  a.s_per_split = p.gather.sPerSplit;
+  a.nsplit = p.nsplit;
+  const dim3 grid(CeilDiv(L->DoutPad, kFcThreads * cpt), CeilDiv(N, tn), p.nsplit);
   const bool pre = L->kshift == 2;
   if (L->asmt_bits) {   // bit-packed table: same grid, chunking and splits as the byte table
-    const int p = L->asmt_pitch;
+    const int pt = L->asmt_pitch;
     switch (L->K) {
-      case 16:  rc = LaunchK<16, false, true>(a, tn, cpt, grid, st, p); break;
-      case 32:  rc = LaunchK<32, false, true>(a, tn, cpt, grid, st, p); break;
-      case 64:  rc = LaunchK<64, false, true>(a, tn, cpt, grid, st, p); break;
-      case 128: rc = LaunchK<128, false, true>(a, tn, cpt, grid, st, p); break;
+      case 16:  return LaunchK<16, false, true>(a, tn, cpt, grid, st, pt);
+      case 32:  return LaunchK<32, false, true>(a, tn, cpt, grid, st, pt);
+      case 64:  return LaunchK<64, false, true>(a, tn, cpt, grid, st, pt);
+      case 128: return LaunchK<128, false, true>(a, tn, cpt, grid, st, pt);
       default:
         SetError("qcnn_fc_aprx_forward: no packed-table kernel for K=%d", L->K);
         return 1;
     }
-  } else switch (L->K) {
-    case 16:  rc = pre ? LaunchK<16, true>(a, tn, cpt, grid, st) : LaunchK<16, false>(a, tn, cpt, grid, st); break;
-    case 32:  rc = pre ? LaunchK<32, true>(a, tn, cpt, grid, st) : LaunchK<32, false>(a, tn, cpt, grid, st); break;
-    case 64:  rc = pre ? LaunchK<64, true>(a, tn, cpt, grid, st) : LaunchK<64, false>(a, tn, cpt, grid, st); break;
-    case 128: rc = LaunchK<128, false>(a, tn, cpt, grid, st); break;
-    case 256: rc = LaunchK<256, false>(a, tn, cpt, grid, st); break;
+  }
+  switch (L->K) {
+    case 16:  return pre ? LaunchK<16, true>(a, tn, cpt, grid, st) : LaunchK<16, false>(a, tn, cpt, grid, st);
+    case 32:  return pre ? LaunchK<32, true>(a, tn, cpt, grid, st) : LaunchK<32, false>(a, tn, cpt, grid, st);
+    case 64:  return pre ? LaunchK<64, true>(a, tn, cpt, grid, st) : LaunchK<64, false>(a, tn, cpt, grid, st);
+    case 128: return LaunchK<128, false>(a, tn, cpt, grid, st);
+    case 256: return LaunchK<256, false>(a, tn, cpt, grid, st);
     default:
       SetError("qcnn_fc_aprx_forward: unsupported codebook size K=%d (supported: 16, 32, 64, 128, 256)", L->K);
       return 1;
   }
-  if (rc) return rc;
-  ctx->launches++;
-  if (nsplit > 1) return LaunchSplitReduce(ctx, a.partial, dst, N, L->Dout, L->DoutPad, nsplit, relu, st);
-  return 0;
 }
 
 }  // namespace qcnn

@@ -557,7 +557,7 @@ static bool ChainEnabled() {
 // the per-layer kernels of fc_aprx.cu).
 // *packed: some layer keeps a bit-packed table (launch fc_chain_packed_kernel with *pk).  Eligibility and every figure
 // but the ring chunking of a packed layer are those of the byte table.
-static bool PlanChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int n, ChainArgs* out, size_t* smemBytes,
+static bool PlanChain(qcnn_ctx* ctx, const qcnn_layer* const* layers, const int* relu, int n, ChainArgs* out, size_t* smemBytes,
                       ChainPack* pk = nullptr, bool* packed = nullptr) {
   if (!ChainEnabled() || n < 1 || n > kMaxChain) return false;
   const int G = ctx->sm_count;
@@ -577,7 +577,6 @@ static bool PlanChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu,
     if (Q->DoutPad > kChunkBytes || Q->K * Q->d % 4 != 0) return false;
     ChainLayer& L = a.L[l];
     L.ctrd = Q->d_ctrd.as<float>(); L.asmt = Q->d_asmt.as<uint8_t>(); L.bias = Q->d_bias.as<float>(); L.srcoff = Q->d_srcoff.as<int>();
-    L.partial = Q->d_cpart.as<float>();
     L.Din = Q->Din; L.Dout = Q->Dout; L.DoutPad = Q->DoutPad; L.S = Q->S; L.K = Q->K; L.d = Q->d;
     L.log2K = 0;
     while ((1 << L.log2K) < Q->K) L.log2K++;
@@ -644,20 +643,20 @@ static bool PlanChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu,
   return true;
 }
 
-bool FcChainEligible(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int n, int N) {
+bool FcChainEligible(qcnn_ctx* ctx, const qcnn_layer* const* layers, const int* relu, int n, int N) {
   if (N < 1 || N > kChainMaxN) return false;
   ChainArgs a;
   size_t smem;
   return PlanChain(ctx, layers, relu, n, &a, &smem);
 }
 
-void DescribeFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int n, char* buf, size_t cap) {
+// The chain row of fc_plan.cu: one layer as a chain of one
+void DescribeFcChain(const qcnn_layer* L, const FcPlan&, int, char* buf, size_t cap) {
   ChainArgs a;
   size_t smem = 0;
-  buf[0] = 0;
-  if (!PlanChain(ctx, layers, relu, n, &a, &smem)) return;
-  snprintf(buf, cap, "fc_chain(persistent, %d layer%s, grid=%d, ring=%dx%dB, smem=%zuB)", n, n > 1 ? "s" : "", a.G, a.nStage,
-           kChunkBytes, smem);
+  const int relu0 = 0;
+  if (PlanChain(L->ctx, &L, &relu0, 1, &a, &smem))
+    snprintf(buf, cap, "fc_chain(persistent, 1 layer, grid=%d, ring=%dx%dB, smem=%zuB)", a.G, a.nStage, kChunkBytes, smem);
 }
 
 // src: [N][Din of the first layer] (or the NHWC map the first layer's srcoff folds); dst: [N][Dout of the last layer]
@@ -665,22 +664,22 @@ int LaunchFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int
                   cudaStream_t st, unsigned long long* dbg, bool* handled) {
   *handled = false;
   if (N < 1 || N > kChainMaxN) return 0;
+  ChainArgs a;
+  ChainPack pk;
+  bool packed = false;
+  size_t smem = 0;
+  if (!PlanChain(ctx, layers, relu, n, &a, &smem, &pk, &packed)) return 0;
   // partial-sum buffers: one per layer, [G][DoutPad], every word armed with the "not yet written" pattern
   for (int l = 0; l < n; l++) {
     qcnn_layer* Q = layers[l];
-    if (Q->kind != QCNN_KIND_FC) return 0;
     const size_t need = sizeof(float) * static_cast<size_t>(ctx->sm_count) * Q->DoutPad;
     bool grown = false;
     const cudaError_t e = Q->d_cpart.Reserve(ctx, need, st, &grown);
     if (e == cudaErrorStreamCaptureUnsupported) return 0;   // cannot allocate inside a capture: per-layer kernels this time
     QCNN_CUDA(e);
     if (grown) QCNN_CUDA(cudaMemsetAsync(Q->d_cpart.get(), 0xFF, need, st));
+    a.L[l].partial = Q->d_cpart.as<float>();
   }
-  ChainArgs a;
-  ChainPack pk;
-  bool packed = false;
-  size_t smem = 0;
-  if (!PlanChain(ctx, layers, relu, n, &a, &smem, &pk, &packed)) return 0;
   static bool attrSet[64] = {false};
   if (ctx->device < 64 && !attrSet[ctx->device]) {
     const int lim = static_cast<int>(SmemOptin(ctx));

@@ -303,24 +303,22 @@ int LaunchShape(const FcWsArgs& a, int nc, int mb, unsigned nb, size_t smem, cud
   return 1;
 }
 
-// A tiling of the layer at batch N: images per CTA x channels per CTA x k-steps per stage x K-split
-struct FcWsPlan {
-  int P, NC, KS, nPB, nsplit, kPerSplit, nChunksAll, idxRows;
-  size_t smem;
-};
-
 // cost-model constants on PlanPqGemm's scale (SM-cycles): the L2 -> shared bandwidth one SM can count on for the plane
 // image, and the GPU's HBM bandwidth for the partial sums of a K-split and their reduction (H100 SXM: ~5.5 TB/s and
 // 3.35 TB/s at ~1.75 GHz)
 constexpr double kL2BytesPerSmCycle = 24.0;
 constexpr double kHbmBytesPerCycle = 1900.0;
 
-FcWsArgs ArgsOf(const qcnn_layer* L, const FcWsPlan& p) {
+// the layer's arguments of a tiling (the activations, the output and N are bound at launch)
+FcWsArgs ArgsOf(const qcnn_layer* L, const FcPlan& c) {
+  const auto& p = c.ws;
   FcWsArgs a;
   memset(&a, 0, sizeof(a));
+  a.asmt = L->d_asmt.as<uint8_t>(); a.ctrd = L->d_ctrd.as<float>(); a.ctrdBf = L->d_ctrd_bf.as<uint4>(); a.bias = L->d_bias.as<float>();
   a.Dout = L->Dout; a.DoutPad = L->DoutPad; a.K = L->K; a.d = L->d; a.kshift = L->kshift;
-  a.KS = p.KS; a.nPB = p.nPB; a.nct = qcnn::CeilDiv(L->Dout, p.NC); a.nsplit = p.nsplit; a.kAll = L->Din / 8;
-  a.kPerSplit = p.kPerSplit; a.nChunksAll = p.nChunksAll; a.idxRows = p.idxRows;
+  a.KS = p.KS; a.nPB = p.nPB; a.nct = qcnn::CeilDiv(L->Dout, p.NC); a.nsplit = c.nsplit; a.kAll = L->Din / 8;
+  a.kPerSplit = p.kPerSplit; a.nChunksAll = qcnn::CeilDiv(a.kAll, p.KS);
+  a.idxRows = L->d == 1 ? 8 * p.KS : qcnn::CeilDiv(8 * p.KS, L->d) + 1;
   a.pkBits = L->asmt_bits; a.pkPitch = L->asmt_pitch;
   return a;
 }
@@ -329,18 +327,9 @@ FcWsArgs ArgsOf(const qcnn_layer* L, const FcWsPlan& p) {
 
 namespace qcnn {
 
-// fc_ws = 1 and the mode-2 conditions (FcTcEligible) with bf16x2 operands (byte or bit-packed table: a net's outputs do
-// not depend on the table's form)
-static bool FcWsEligible(const qcnn_layer* L, int N) {
-  if (!L->opt_fc_ws || !L->opt_tc_bf || !FcTcEligible(L, N)) return false;
-  return L->d == 1 || (L->d % 4 == 0 && L->d_ctrd_bf.get());
-}
-
 // The cheapest tiling of batch N under the gemm_nt / gemm_gt / gemm_ct / gemm_nsplit pins (no on-device timing: a
-// layer at a given batch computes the same sums in every process).  *ok = false when the layer does not take fc_ws.
-static int PlanFcWs(const qcnn_layer* L, int N, FcWsPlan* out, bool* ok) {
-  *ok = FcWsEligible(L, N);
-  if (!*ok) return 0;
+// layer at a given batch computes the same sums in every process); fails when the pins leave none.
+int PlanFcWs(const qcnn_layer* L, int N, FcPlan* out) {
   const int kAll = L->Din / 8;
   const size_t smemMax = SmemOptin(L->ctx);
   const int sms = L->ctx->sm_count;
@@ -353,22 +342,22 @@ static int PlanFcWs(const qcnn_layer* L, int N, FcWsPlan* out, bool* ok) {
     const int tiles = CeilDiv(N, P), nct = CeilDiv(L->Dout, NC);
     for (int KS = kFcWsMaxKS; KS >= 4; KS -= 4) {
       if (L->opt_gemm_gt && KS != L->opt_gemm_gt) continue;
-      FcWsPlan p;
+      FcPlan c;
+      auto& p = c.ws;
       p.P = P; p.NC = NC; p.KS = KS;
-      p.nChunksAll = CeilDiv(kAll, KS);
-      p.idxRows = L->d == 1 ? 8 * KS : CeilDiv(8 * KS, L->d) + 1;
+      const int nChunksAll = CeilDiv(kAll, KS);
       // a ring of three plane buffers if it fits, else two
       bool fit = false;
       for (p.nPB = 3; p.nPB >= 2 && !fit; p.nPB--) {
-        p.nsplit = 1; p.kPerSplit = kAll;
-        p.smem = static_cast<size_t>(MapFcWsSmem(ArgsOf(L, p), P, NC).total);
+        c.nsplit = 1; p.kPerSplit = kAll;
+        p.smem = static_cast<size_t>(MapFcWsSmem(ArgsOf(L, c), P, NC).total);
         if (p.smem <= smemMax) { fit = true; break; }
       }
       if (!fit) continue;
-      const int maxSplit = std::min(p.nChunksAll, 64);
+      const int maxSplit = std::min(nChunksAll, 64);
       for (int ns = 1; ns <= maxSplit; ns++) {
-        const int cps = CeilDiv(p.nChunksAll, ns);
-        if (CeilDiv(p.nChunksAll, cps) != ns) continue;   // (the same split as a smaller ns)
+        const int cps = CeilDiv(nChunksAll, ns);
+        if (CeilDiv(nChunksAll, cps) != ns) continue;   // (the same split as a smaller ns)
         if (L->opt_gemm_nsplit && ns != L->opt_gemm_nsplit) continue;
         const double ks = static_cast<double>(cps) * KS;   // k-steps of the busiest CTA
         // tensor work (as PlanConvWs), or the plane image it reads from L2 when that takes longer (every channel tile
@@ -383,9 +372,9 @@ static int PlanFcWs(const qcnn_layer* L, int N, FcWsPlan* out, bool* ok) {
         if (!found || cost < best) {
           best = cost;
           found = true;
-          *out = p;
+          out->ws = p;
           out->nsplit = ns;
-          out->kPerSplit = cps * KS;
+          out->ws.kPerSplit = cps * KS;
         }
       }
     }
@@ -395,50 +384,26 @@ static int PlanFcWs(const qcnn_layer* L, int N, FcWsPlan* out, bool* ok) {
   return 0;
 }
 
-int DescribeFcWs(const qcnn_layer* L, int N, char* buf, size_t cap, bool* handled) {
-  FcWsPlan p;
-  if (int rc = PlanFcWs(L, N, &p, handled)) return rc;
-  if (!*handled) return 0;
+void DescribeFcWs(const qcnn_layer* L, const FcPlan& p, int N, char* buf, size_t cap) {
   // (no "NT=": the executed-MAC count that bench.py derives from pq_gemm_tc( plans assumes 128-channel tiles)
-  const int nct = CeilDiv(L->Dout, p.NC);
+  const int nct = CeilDiv(L->Dout, p.ws.NC);
   snprintf(buf, cap, "pq_gemm_tc_ws(weight-stationary wgmma, weights decoded once per CTA into shared memory, bf16x2) mode=2 "
-           "N=%d images=%d ctiles=%d KS=%d smem=%zuB grid=%d planebufs=%d nsplit=%d ksteps=%d", p.NC, p.P, nct, p.KS, p.smem,
-           CeilDiv(N, p.P) * nct * p.nsplit, p.nPB, p.nsplit, p.kPerSplit);
-  return 0;
+           "N=%d images=%d ctiles=%d KS=%d smem=%zuB grid=%d planebufs=%d nsplit=%d ksteps=%d", p.ws.NC, p.ws.P, nct, p.ws.KS,
+           p.ws.smem, CeilDiv(N, p.ws.P) * nct * p.nsplit, p.ws.nPB, p.nsplit, p.ws.kPerSplit);
 }
 
-int LaunchFcWs(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled) {
-  FcWsPlan p;
-  if (int rc = PlanFcWs(L, N, &p, handled)) return rc;
-  if (!*handled) return 0;
-  *handled = false;
-  qcnn_ctx* ctx = L->ctx;
+int LaunchFcWs(qcnn_layer* L, const FcPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
   FcWsArgs a = ArgsOf(L, p);
-  a.N = N;
-  QCNN_CHECK(static_cast<size_t>(MapFcWsSmem(a, p.P, p.NC).total) == p.smem, "internal: fc_ws shared-memory carve changed after planning");
-  const long long blocks = static_cast<long long>(CeilDiv(N, p.P)) * a.nct * a.nsplit;
+  a.N = N; a.relu = relu; a.dst = dst;
+  QCNN_CHECK(static_cast<size_t>(MapFcWsSmem(a, p.ws.P, p.ws.NC).total) == p.ws.smem,
+             "internal: fc_ws shared-memory carve changed after planning");
+  const long long blocks = static_cast<long long>(CeilDiv(N, p.ws.P)) * a.nct * a.nsplit;
   QCNN_CHECK(blocks <= 2147483647LL, "qcnn_fc_aprx_forward: batch too large for the weight-stationary tiling");
-  if (int rc = PrepFcPlanes(L, src, N, p.P, p.KS, p.nChunksAll, true, st)) return rc;
+  if (int rc = PrepFcPlanes(L, src, N, p.ws.P, p.ws.KS, a.nChunksAll, true, st)) return rc;
   a.xprep = L->d_flat.as<uint4>();
-  a.asmt = L->d_asmt.as<uint8_t>();
-  a.ctrd = L->d_ctrd.as<float>();
-  a.ctrdBf = L->d_ctrd_bf.as<uint4>();
-  a.bias = L->d_bias.as<float>();
-  a.relu = a.nsplit > 1 ? 0 : relu;
-  a.dst = dst;
-  if (a.nsplit > 1) {
-    QCNN_CUDA(L->d_partial.Reserve(ctx, sizeof(float) * static_cast<size_t>(a.nsplit) * N * L->DoutPad, st));
-    a.dst = L->d_partial.as<float>();
-  }
   const unsigned nb = static_cast<unsigned>(blocks);
-  const int rc = L->d == 1 ? LaunchShape<true>(a, p.NC, p.P / 128, nb, p.smem, st, ctx)
-                           : LaunchShape<false>(a, p.NC, p.P / 128, nb, p.smem, st, ctx);
-  if (rc) return rc;
-  ctx->launches++;
-  if (a.nsplit > 1)
-    if (int rc2 = LaunchSplitReduce(ctx, a.dst, dst, N, L->Dout, L->DoutPad, a.nsplit, relu, st)) return rc2;
-  *handled = true;
-  return 0;
+  return L->d == 1 ? LaunchShape<true>(a, p.ws.NC, p.ws.P / 128, nb, p.ws.smem, st, L->ctx)
+                   : LaunchShape<false>(a, p.ws.NC, p.ws.P / 128, nb, p.ws.smem, st, L->ctx);
 }
 
 }  // namespace qcnn

@@ -318,8 +318,6 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
   if (!strcmp(name, "asmt_packed")) {
     // FC only: 1 keeps the assignment table bit-packed at log2(K) bits per index (kernels unpack it), 0 = byte table
     QCNN_CHECK(L->kind == QCNN_KIND_FC, "qcnn_layer_set_param: 'asmt_packed' applies to FC layers");
-    L->plan_N = 0; L->tuned = 0;
-    L->tunedPlans.clear();
     return SetAsmtPacked(L, value);
   }
   if (!strcmp(name, "fc_ws")) {
@@ -339,30 +337,26 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
     L->plan_N = 0; L->tuned = 0;
     L->tunedPlans.clear();
   }
-  else if (L->kind == QCNN_KIND_FC && (!strcmp(name, "gemm_nt") || !strcmp(name, "gemm_gt") || !strcmp(name, "gemm_nsplit") ||
-                                        !strcmp(name, "gemm_ct"))) {
+  else if (!strcmp(name, "gemm_nt") || !strcmp(name, "gemm_gt") || !strcmp(name, "gemm_nsplit") || !strcmp(name, "gemm_ct")) {
+    // 0 = any.  Conv: gemm_nt: positions per CTA of the pq_gemm_tc tilings (128 = one accumulator, 64 = two) and of the
+    // conv_ws tilings; gemm_gt: k-steps per stage of the pq_gemm_tc tilings (4 or 3); gemm_nsplit: their K-split factor
+    // (1 = no split, > 1 = partial sums reduced by a second kernel); gemm_ct: channels per CTA of the conv_ws tilings.
     // FC with fc_ws = 1: the fc_ws tilings with that many images per CTA (128 / 256), k-steps per stage (8 / 4), K-split
-    // factor and channels per CTA (0 = any); pq_gemm_tc mode 2 has a single tiling per batch and ignores them
+    // factor and channels per CTA; pq_gemm_tc mode 2 has a single tiling per batch and ignores them.
+    // A pin that no tiling of the layer matches fails the forward.
     const int v = value < 0 ? 0 : value;
     if (!strcmp(name, "gemm_nt")) L->opt_gemm_nt = v;
     else if (!strcmp(name, "gemm_gt")) L->opt_gemm_gt = v;
     else if (!strcmp(name, "gemm_nsplit")) L->opt_gemm_nsplit = v;
     else L->opt_gemm_ct = v;
+    L->plan_N = 0; L->tuned = 0;
+    L->tunedPlans.clear();
   }
-  else if (!strcmp(name, "force_kernel") || !strcmp(name, "autotune") || !strcmp(name, "gemm_nt") ||
-           !strcmp(name, "gemm_gt") || !strcmp(name, "gemm_nsplit") || !strcmp(name, "gemm_ct")) {
+  else if (!strcmp(name, "force_kernel") || !strcmp(name, "autotune")) {
     // conv only.  force_kernel: -1 none, else 0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc | 7 conv_ws;
-    // autotune: 0 keeps the cost model's first tiling instead of timing the candidates on the device;
-    // gemm_nt: positions per CTA of the pq_gemm_tc tilings (0 = any; 128 = one accumulator, 64 = two);
-    // gemm_gt: k-steps per stage of those tilings (0 = any; 4 or 3); gemm_nsplit: their K-split factor (0 = any; 1 = no
-    // split, > 1 = partial sums reduced by a second kernel); gemm_ct: channels per CTA of the conv_ws tilings (0 = any).
-    // A pin that no tiling of the layer matches fails the forward.
+    // autotune: 0 keeps the cost model's first tiling instead of timing the candidates on the device
     QCNN_CHECK(L->kind == QCNN_KIND_CONV, "qcnn_layer_set_param: '%s' applies to conv layers", name);
     if (name[0] == 'f') L->opt_force_kernel = value < 0 ? 0 : value + 1;
-    else if (!strcmp(name, "gemm_nt")) L->opt_gemm_nt = value < 0 ? 0 : value;
-    else if (!strcmp(name, "gemm_gt")) L->opt_gemm_gt = value < 0 ? 0 : value;
-    else if (!strcmp(name, "gemm_nsplit")) L->opt_gemm_nsplit = value < 0 ? 0 : value;
-    else if (!strcmp(name, "gemm_ct")) L->opt_gemm_ct = value < 0 ? 0 : value;
     else L->opt_no_autotune = value ? 0 : 1;
     L->plan_N = 0; L->tuned = 0;
     L->tunedPlans.clear();
@@ -374,17 +368,7 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
 int qcnn_layer_describe(qcnn_layer* L, int N, char* buf, size_t cap) {
   QCNN_CHECK(L && buf && cap > 0 && N >= 1, "qcnn_layer_describe: bad argument");
   if (L->kind == QCNN_KIND_CONV) return DescribeConv(L, N, buf, cap);
-  char tc[256];
-  if (int rc = DescribeFcTc(L, N, tc, sizeof(tc))) return rc;
-  if (N <= 4) {
-    const int relu0 = 0;
-    DescribeFcChain(L->ctx, &L, &relu0, 1, tc, sizeof(tc));
-  }
-  char packed[16] = "";
-  if (L->asmt_bits) snprintf(packed, sizeof(packed), " asmt=%dbit", L->asmt_bits);
-  snprintf(buf, cap, "fc_aprx Din=%d Dout=%d S=%d K=%d d=%d%s%s%s", L->Din, L->Dout, L->S, L->K, L->d, tc[0] ? " via " : "", tc,
-           packed);
-  return 0;
+  return DescribeFc(L, N, buf, cap);
 }
 
 void qcnn_layer_destroy(qcnn_layer* L) {

@@ -245,6 +245,20 @@ struct ConvPlan {
   GemmArgs g;           // kernels 6 (pq_gemm_tc) and 7 (conv_ws)
 };
 
+// FcPlan::kernel, in the order the rule of fc_plan.cu tries them: fc_chain.cu, fc_ws.cu, pq_gemm_tc mode 2, LUT + gather
+enum FcKernel { kFcChain, kFcWs, kFcMode2, kFcGather, kFcKernelIds };
+
+// An FC layer's family at one batch size and that family's tiling, without device pointers (bound at launch).  Made on
+// every call: qcnn_fc_aprx_forward_flat hides d_srcoff for the length of one call.
+struct FcPlan {
+  int kernel;    // FcKernel
+  int nsplit;    // K-split: > 1 = partial sums [nsplit][N][DoutPad] in d_partial, reduced in fixed order (chain: 1)
+  struct { int P, NC, KS, nPB, kPerSplit; size_t smem; } ws;   // fc_ws: images, channels per CTA, k-steps per stage and
+                                                                 // per split, plane buffers, shared memory
+  GemmArgs tc;   // mode 2
+  struct { int tn, cpt, sPerSplit; } gather;   // LUT + gather: images per CTA, channels per thread, subspaces per split
+};
+
 struct qcnn_layer {
   qcnn_ctx* ctx = nullptr;
   int kind = 0;
@@ -306,12 +320,31 @@ using ConvCands = std::vector<std::pair<double, ConvPlan>>;
 void PlanLutGather(const qcnn_layer* L, int N, ConvCands* cands);
 int LaunchLutGather(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
 void DescribeLutGather(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap);
+
+// fc_plan.cu: the choice among the FC kernel families (each plans into an FcPlan, launches and describes a plan)
 int LaunchFc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st);
-// fc_chain.cu: one persistent launch for a run of consecutive FC layers at batch <= 4 (relu[l]: ReLU after layer l)
-bool FcChainEligible(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int n, int N);
-void DescribeFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int n, char* buf, size_t cap);
+int DescribeFc(qcnn_layer* L, int N, char* buf, size_t cap);
+// fc_chain.cu: one persistent launch for a run of consecutive FC layers at batch <= 4 (relu[l]: ReLU after layer l);
+// *handled = false when the kernel does not take the layers, or cannot allocate its partial sums inside a stream capture
+bool FcChainEligible(qcnn_ctx* ctx, const qcnn_layer* const* layers, const int* relu, int n, int N);
 int LaunchFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int n, const float* src, int N, float* dst,
                   cudaStream_t st, unsigned long long* dbg, bool* handled);
+void DescribeFcChain(const qcnn_layer* L, const FcPlan& p, int N, char* buf, size_t cap);
+// fc_ws.cu: the weight-stationary FC GEMM (bf16x2 operands); PlanFcWs fails when the gemm_* pins leave no tiling
+int PlanFcWs(const qcnn_layer* L, int N, FcPlan* p);
+int LaunchFcWs(qcnn_layer* L, const FcPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
+void DescribeFcWs(const qcnn_layer* L, const FcPlan& p, int N, char* buf, size_t cap);
+// fc_aprx.cu: pq_gemm_tc mode 2 (false when it does not fit in shared memory), LUT + gather, and the activations of the
+// tensor-core families as the plane image [tile][chunk][x1, x2 (3xTF32: hi, lo)][KS][NT] in L->d_flat
+bool PlanFcMode2(const qcnn_layer* L, int N, FcPlan* p);
+int LaunchFcMode2(qcnn_layer* L, const FcPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
+void DescribeFcMode2(const qcnn_layer* L, const FcPlan& p, int N, char* buf, size_t cap);
+void PlanFcGather(const qcnn_layer* L, int N, FcPlan* p);
+int LaunchFcGather(qcnn_layer* L, const FcPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
+int PrepFcPlanes(qcnn_layer* L, const float* src, int N, int NT, int KS, int nChunksAll, bool bf, cudaStream_t st);
+int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows, int cols, int colsPad, int nsplit, int relu,
+                      cudaStream_t st);
+
 // pq_gemm_tc.cu
 void PlanPqGemm(const qcnn_layer* L, int N, ConvCands* cands);
 void DescribePqGemm(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap);
@@ -320,18 +353,6 @@ size_t PqGemmSmemBytes(const GemmArgs& a);
 // asmtBits != 0 (mode 2): a.asmt is the bit-packed FC table of packed_asmt.h with rows of asmtPitch bytes
 int LaunchPqGemmArgs(qcnn_ctx* ctx, const GemmArgs& a, long long blocks, cudaStream_t st, int asmtBits = 0, int asmtPitch = 0);
 int BuildCtrdBf(qcnn_layer* L);   // layer creation: the bf16x2 form of the codebook (d % 4 == 0)
-int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows, int cols, int colsPad, int nsplit, int relu,
-                      cudaStream_t st);
-int DescribeFcTc(const qcnn_layer* L, int N, char* buf, size_t cap);
-int LaunchFcTc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled);
-// fc_aprx.cu: the batched FC layer may take a tensor-core GEMM (N >= 96, no gather-kernel tuning, a decodable geometry);
-// its activations as the plane image [tile][chunk][x1, x2 (3xTF32: hi, lo)][KS][NT] in L->d_flat
-bool FcTcEligible(const qcnn_layer* L, int N);
-int PrepFcPlanes(qcnn_layer* L, const float* src, int N, int NT, int KS, int nChunksAll, bool bf, cudaStream_t st);
-// fc_ws.cu: the weight-stationary FC GEMM (fc_ws = 1, bf16x2 operands); *handled = false when the layer does
-// not take it at batch N
-int LaunchFcWs(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaStream_t st, bool* handled);
-int DescribeFcWs(const qcnn_layer* L, int N, char* buf, size_t cap, bool* handled);
 int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
 int Mode0Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a stride-1 layer on the flat padded grid
 int Mode1Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a strided layer on bf16x2 / tf32 phase planes

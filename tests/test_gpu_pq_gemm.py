@@ -345,7 +345,7 @@ INELIGIBLE = [pytest.param(r, bf, id="%s-%s" % (r.name, fmt(bf))) for r in CONV_
 
 
 def fc_plan(N, Din, Dout, sms):
-    """(NT, nsplit, k-steps per split) LaunchFcTc derives for batch N."""
+    """(NT, nsplit, k-steps per split) PlanFcMode2 derives for batch N."""
     NT = 128 if N > 64 else 64
     tiles, nct, kall = _ceil(N, NT), _ceil(Dout, 128), Din // 8
     ns = max(1, sms // (tiles * nct))
