@@ -80,11 +80,11 @@ int PlanConv(qcnn_layer* L, int N) {
   // "gemm_ct" its channels per CTA
   if (L->opt_gemm_nt || L->opt_gemm_gt || L->opt_gemm_nsplit || L->opt_gemm_ct) {
     keepIf([L](const ConvPlan& c) {
+      if (c.kernel == kConvWs)
+        return (!L->opt_gemm_nt || c.ws.P == L->opt_gemm_nt) && (!L->opt_gemm_ct || c.ws.NC == L->opt_gemm_ct);
       const GemmArgs& g = c.g;
-      if (c.kernel != kPqGemmTc && c.kernel != kConvWs) return true;
-      if (L->opt_gemm_nt && g.NT != L->opt_gemm_nt) return false;
-      if (c.kernel == kConvWs) return !L->opt_gemm_ct || g.Kg / g.nct == L->opt_gemm_ct;
-      return (!L->opt_gemm_gt || g.GT == L->opt_gemm_gt) && (!L->opt_gemm_nsplit || g.nsplit == L->opt_gemm_nsplit);
+      return c.kernel != kPqGemmTc || ((!L->opt_gemm_nt || g.NT == L->opt_gemm_nt) && (!L->opt_gemm_gt || g.GT == L->opt_gemm_gt) &&
+                                       (!L->opt_gemm_nsplit || g.nsplit == L->opt_gemm_nsplit));
     });
     QCNN_CHECK(!cands.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d gemm_gt=%d gemm_nsplit=%d gemm_ct=%d has no tiling for "
                "this layer at batch %d", L->opt_gemm_nt, L->opt_gemm_gt, L->opt_gemm_nsplit, L->opt_gemm_ct, N);
@@ -141,10 +141,11 @@ int LaunchConv(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
       }
       if (!ok) continue;
       static const bool tuneLog = getenv("QCNN_AUTOTUNE_LOG") != nullptr;
-      if (tuneLog) {
-        const bool gemm = kFamilies[c.kernel].cls == kGemm;
+      if (tuneLog) {   // (conv_ws: positions per CTA, KS, bf16x2, no K-split)
+        const bool ws = c.kernel == kConvWs, tc = c.kernel == kPqGemmTc;
         fprintf(stderr, "[qcnn autotune] N=%d Cout=%d k=%d cand %zu: kernel=%d NT/CPT=%d GT/J=%d bf=%d nsplit=%d smem=%zu -> %.4f ms\n",
-                N, L->Cout, L->ksz, i, c.kernel, gemm ? c.g.NT : c.CPT, gemm ? c.g.GT : c.J, c.g.bf, c.g.nsplit, c.smem, ms);
+                N, L->Cout, L->ksz, i, c.kernel, ws ? c.ws.P : tc ? c.g.NT : c.CPT, ws ? c.ws.KS : tc ? c.g.GT : c.J,
+                ws ? 1 : c.g.bf, ws ? 1 : c.g.nsplit, c.smem, ms);
       }
       if (ms < bestMs) { bestMs = ms; bestI = i; }
     }

@@ -48,20 +48,19 @@ using qcnn::SplitBf16x4;
 
 constexpr int kWsRegPos = 8;        // mode 0: float4 of a chunk's planes a producer thread stages per register pass
 
-// Shared-memory carve, read by the planner (fits / does not fit) and by the kernel.  a.NT = positions per CTA,
-// a.GT = k-steps per weight stage (KS), a.Kg / a.nct = channels per CTA (N of the MMA), a.nPB = plane buffers (mode 1:
-// one per phase row, mode 0: the ring).
+// Shared-memory carve, read by the planner (fits / does not fit) and by the kernel.  The channel count is computed as
+// Kg / nct rather than read from NC: reading NC changed the kernels' register allocation.
 struct WsSmem {  // byte offsets inside the dynamic shared memory
   int planes, wts, cb, outoff, bias, bars, total;
 };
-__host__ __device__ inline WsSmem MapWsSmem(const GemmArgs& a) {
+__host__ __device__ inline WsSmem MapWsSmem(const ConvWsArgs& a) {
   const int nc = a.Kg / a.nct;
   WsSmem m;
   int o = 0;
   m.planes = o; o += a.nPB * 2 * a.planeRows * 16;        // [buffer][x1, x2][planeRows] 16-byte rows
-  m.wts = o;    o += 2 * a.GT * 2 * nc * 16;              // [buffer][k-step][w1, w2][channel] 16-byte rows
-  m.cb = o;     o += (a.mode == 0 ? 2 : 1) * a.K * 16;    // pre-split codebook slices {w1, w2} (mode 0: one per half)
-  m.outoff = o; o += a.NT * 4;                            // destination element offset of every position (-1: none)
+  m.wts = o;    o += 2 * a.KS * 2 * nc * 16;              // [buffer][k-step][w1, w2][channel] 16-byte rows
+  m.cb = o;     o += (a.stride == 1 ? 2 : 1) * a.K * 16;  // pre-split codebook slices {w1, w2} (stride 1: one per half)
+  m.outoff = o; o += a.P * 4;                             // destination element offset of every position (-1: none)
   m.bias = o;   o += nc * 4;                              // (nc is a multiple of 16: the barriers stay 8-byte aligned)
   m.bars = o;   o += 8 * (2 * a.nPB + 4);
   m.total = o;
@@ -72,12 +71,12 @@ __host__ __device__ inline WsSmem MapWsSmem(const GemmArgs& a) {
 // WIDE (stride 1): a chunk's planes take more than one register pass of the producers, or a group has <= 3 channels
 // (kept apart so that the single-pass kernels AlexNet runs carry none of that staging)
 template <int NC, int MB, bool S1, bool WIDE>
-__global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a) {
+__global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const ConvWsArgs a) {
   constexpr int P = 128 * MB;   // positions per CTA
   extern __shared__ __align__(128) unsigned char smem[];
   const WsSmem sm = MapWsSmem(a);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int KS = a.GT, nPB = a.nPB;
+  const int KS = a.KS, nPB = a.nPB;
   const int nCh = S1 ? a.nChunks : a.stride;   // chunks: 8-channel groups (mode 0) / phase rows (mode 1)
   uint4* planes = reinterpret_cast<uint4*>(smem + sm.planes);
   uint4* wts = reinterpret_cast<uint4*>(smem + sm.wts);
@@ -104,7 +103,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
     outoff[p] = (i < a.N && ho < a.Ho && wo < a.Wo) ? (((i - i0) * a.Ho + ho) * a.Wo + wo) * a.Cout : -1;
   }
   if (!S1)
-    for (int k = tid; k < a.K; k += kWsThreads) cb[k] = __ldg(reinterpret_cast<const uint4*>(a.ctrd) + k);
+    for (int k = tid; k < a.K; k += kWsThreads) cb[k] = __ldg(a.ctrd + k);
   for (int c = tid; c < NC; c += kWsThreads) biasS[c] = __ldg(a.bias + g * a.Kg + ch0 + c);
   if (tid == 0) qcnn::WsInitBarriers(fullP, emptyP, nPB, kWsProducers, fullW, emptyW);
   __syncthreads();
@@ -119,7 +118,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
       // 4-7 of the chunk), position = p % NPOS -> pixel (r - pad, c - pad) of image i of the flat padded grid.  The 2 NPOS
       // float4 of a chunk take nPass register passes; the source offsets and validity of a pass are chunk-invariant
       // (computed once with a single pass, per pass otherwise)
-      const int taps = a.ntab;
+      const int taps = a.kt.ntab;
       const int nPass = WIDE ? (2 * a.NPOS + kWsRegPos * kWsProducers - 1) / (kWsRegPos * kWsProducers) : 1;
       const float* srcBase = a.src + static_cast<size_t>(i0) * a.srcImg + g * a.Cg;
       int poff[kWsRegPos];
@@ -215,8 +214,8 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
         const bool okB = chB < a.Cg;
         const int sA = chA / a.d, jA = chA - sA * a.d;
         const int sB = okB ? chB / a.d : 0, jB = okB ? chB - sB * a.d : 0;
-        const uint4* cA = reinterpret_cast<const uint4*>(a.ctrd) + static_cast<size_t>(sA * (a.d >> 2) + (jA >> 2)) * a.K;
-        const uint4* cB = reinterpret_cast<const uint4*>(a.ctrd) + static_cast<size_t>(sB * (a.d >> 2) + (jB >> 2)) * a.K;
+        const uint4* cA = a.ctrd + static_cast<size_t>(sA * (a.d >> 2) + (jA >> 2)) * a.K;
+        const uint4* cB = a.ctrd + static_cast<size_t>(sB * (a.d >> 2) + (jB >> 2)) * a.K;
         qcnn::WsProducerSync();   // every producer is done decoding from the previous chunk's slices
         for (int k = pt; k < a.K; k += kWsProducers) {
           cb[k] = __ldg(cA + k);
@@ -239,7 +238,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
             const uint4 b0 = __ldg(iB), b1 = a.tapsPad > 16 ? __ldg(iB + 1) : zero;
             // (no unroll pragma: see the mode-1 decode loop below)
             for (int e = 0; e < n; e++) {
-              const int t = a.tab[s0 + e].idx0;   // the tap of k-step s0 + e
+              const int t = a.kt.tab[s0 + e].idx0;   // the tap of k-step s0 + e
               const uint4 qa = cb[ByteOf32(a0, a1, t)];
               const uint4 qb = cb[a.K + ByteOf32(b0, b1, t)];
               w[(2 * e + 0) * NC + c] = make_uint4(qa.x, qa.y, qb.x, qb.y);   // [w1 of half A | w1 of half B]
@@ -283,7 +282,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // planes are read by the tensor core
       MbarArrive(fullP + ph);
       // weights of the phase row's stages: a thread owns channel c, its index row is [tapsPad] bytes of d_asmt_t
-      const int first = a.chunkFirst[ph], cnt = a.chunkCount[ph];
+      const int first = a.kt.chunkFirst[ph], cnt = a.kt.chunkCount[ph];
       for (int s0 = 0; s0 < cnt; s0 += KS, j++) {
         const int n = min(KS, cnt - s0), b = j & 1;
         if (j >= 2) MbarWait<24>(emptyW + b, ((j >> 1) - 1) & 1);   // buffer last read by the MMAs of stage j - 2
@@ -293,7 +292,7 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
           // (no unroll pragma here: under `#pragma unroll 3` the compiled loop was seen running an iteration with e == n
           // for n = 8 on the device, writing past the weight buffer into the codebook / offset regions)
           for (int e = 0; e < n; e++) {
-            const KStep ks = a.tab[first + s0 + e];
+            const KStep ks = a.kt.tab[first + s0 + e];
             const uint4 q0 = cb[__ldg(row + ks.idx0)];
             const uint4 q1 = ks.cb1 ? make_uint4(0u, 0u, 0u, 0u) : cb[__ldg(row + ks.idx1)];   // unpaired tap: zero half
             w[(2 * e + 0) * NC + c] = make_uint4(q0.x, q0.y, q1.x, q1.y);   // [w1 of half 0 | w1 of half 1]
@@ -322,13 +321,13 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
     const int pb = S1 ? kc % nPB : kc;
     MbarWait<24>(fullP + pb, S1 ? (kc / nPB) & 1 : 0);
     const uint32_t plA = planes0 + static_cast<uint32_t>(pb * 2 * a.planeRows) * 16u + static_cast<uint32_t>(wg * MB * 64) * 16u;
-    const int first = S1 ? 0 : a.chunkFirst[kc], cnt = S1 ? a.ntab : a.chunkCount[kc];
+    const int first = S1 ? 0 : a.kt.chunkFirst[kc], cnt = S1 ? a.kt.ntab : a.kt.chunkCount[kc];
     for (int s0 = 0; s0 < cnt; s0 += KS, j++) {
       const int n = min(KS, cnt - s0), b = j & 1;
       MbarWait<24>(fullW + b, (j >> 1) & 1);
       qcnn::WgmmaFence();
       for (int e = 0; e < n; e++) {
-        const KStep ks = a.tab[first + s0 + e];
+        const KStep ks = a.kt.tab[first + s0 + e];
         const uint32_t wb = wts0 + static_cast<uint32_t>((b * KS + e) * 2 * NC) * 16u;
         qcnn::WsMmaKStep<NC, MB>(acc, plA, ks.bStart, static_cast<uint32_t>(a.planeRows) * 16u, wb);
       }
@@ -363,30 +362,24 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const GemmArgs a
 // channel counts per CTA with an instantiation (N of the MMA; 192 and 256 with one m64 block per warpgroup only)
 constexpr int kWsWidths[] = {16, 32, 64, 96, 128, 192, 256};
 
-// the dynamic shared-memory limit of an instantiation is raised once per device to the opt-in maximum (as in pq_gemm_tc.cu)
 template <int NC, int MB, bool S1, bool WIDE>
-int SetSmemAndLaunch(const GemmArgs& a, unsigned blocks, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
-  static bool done[64] = {false};
-  if (ctx->device < 0 || ctx->device >= 64 || !done[ctx->device]) {
-    const int lim = static_cast<int>(qcnn::SmemOptin(ctx));
-    QCNN_CUDA(cudaFuncSetAttribute(conv_ws_kernel<NC, MB, S1, WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    if (ctx->device >= 0 && ctx->device < 64) done[ctx->device] = true;
-  }
+int LaunchInstance(const ConvWsArgs& a, unsigned blocks, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
+  if (int rc = qcnn::OptInSmem<conv_ws_kernel<NC, MB, S1, WIDE>>(ctx)) return rc;
   conv_ws_kernel<NC, MB, S1, WIDE><<<blocks, kWsThreads, smem, st>>>(a);
   QCNN_CUDA(cudaGetLastError());
   return 0;
 }
 
 template <bool S1, bool WIDE>
-int LaunchWidth(const GemmArgs& a, int nc, unsigned nb, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
-#define QCNN_WS(NC)                                                                               \
-  if (nc == NC) return a.NT == 256 ? SetSmemAndLaunch<NC, 2, S1, WIDE>(a, nb, smem, st, ctx)      \
-                                   : SetSmemAndLaunch<NC, 1, S1, WIDE>(a, nb, smem, st, ctx);
+int LaunchWidth(const ConvWsArgs& a, unsigned nb, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
+#define QCNN_WS(W)                                                                          \
+  if (a.NC == W) return a.P == 256 ? LaunchInstance<W, 2, S1, WIDE>(a, nb, smem, st, ctx)   \
+                                   : LaunchInstance<W, 1, S1, WIDE>(a, nb, smem, st, ctx);
   QCNN_WS(16) QCNN_WS(32) QCNN_WS(64) QCNN_WS(96) QCNN_WS(128)
 #undef QCNN_WS
-  if (nc == 192 && a.NT == 128) return SetSmemAndLaunch<192, 1, S1, WIDE>(a, nb, smem, st, ctx);
-  if (nc == 256 && a.NT == 128) return SetSmemAndLaunch<256, 1, S1, WIDE>(a, nb, smem, st, ctx);
-  qcnn::SetError("internal: no conv_ws instantiation for N=%d positions=%d", nc, a.NT);
+  if (a.NC == 192 && a.P == 128) return LaunchInstance<192, 1, S1, WIDE>(a, nb, smem, st, ctx);
+  if (a.NC == 256 && a.P == 128) return LaunchInstance<256, 1, S1, WIDE>(a, nb, smem, st, ctx);
+  qcnn::SetError("internal: no conv_ws instantiation for N=%d positions=%d", a.NC, a.P);
   return 1;
 }
 
@@ -420,30 +413,29 @@ static void PlanConvWsS1(const qcnn_layer* L, int N, ConvCands* cands) {
       ConvPlan p;
       memset(&p, 0, sizeof(p));
       p.kernel = kConvWs; p.threads = kWsThreads;
-      GemmArgs& ga = p.g;
-      ga.mode = 0; ga.bf = 1;
-      ga.PW = PW; ga.IB = IB; ga.NT = P;
-      ga.NPOS = RoundUp(P + (L->ksz - 1) * (PW + 1), 8);
-      ga.planeRows = ga.NPOS; ga.planeF4 = 2 * ga.NPOS;
-      ga.nChunks = CeilDiv(Cg, 8); ga.nct = Kg / W; ga.nsplit = 1;
-      ga.stride = 1; ga.Kg = Kg; ga.K = L->K;
-      ga.tapsPad = RoundUp(taps, 16);
-      Mode0Table(L, ga);
+      ConvWsArgs& a = p.ws;
+      SetGemmGeometry(L, a);
+      a.PW = PW; a.IB = IB; a.P = P; a.NC = W; a.nct = Kg / W;
+      a.NPOS = RoundUp(P + (L->ksz - 1) * (PW + 1), 8);
+      a.planeRows = a.NPOS;
+      a.nChunks = CeilDiv(Cg, 8);
+      a.tapsPad = RoundUp(taps, 16);
+      Mode0Table(L, PW, a.NPOS, a.kt);
       // k-steps per weight stage: the chunk's taps in as few equal stages as fit; a ring of three plane buffers if it fits
       bool fit = false;
       for (int stages = 1; stages <= taps && !fit; stages++) {
-        ga.GT = CeilDiv(taps, stages);
-        for (ga.nPB = 3; ga.nPB >= 2; ga.nPB--)
-          if (static_cast<size_t>(MapWsSmem(ga).total) <= smemMax) { fit = true; break; }
+        a.KS = CeilDiv(taps, stages);
+        for (a.nPB = 3; a.nPB >= 2; a.nPB--)
+          if (static_cast<size_t>(MapWsSmem(a).total) <= smemMax) { fit = true; break; }
       }
       if (!fit) continue;
-      p.smem = static_cast<size_t>(MapWsSmem(ga).total);
-      p.key = {P, ga.GT, ga.nct};
-      const int stages = ga.nChunks * CeilDiv(taps, ga.GT);
-      const double ne = static_cast<double>(ga.nChunks) * taps;
+      p.smem = static_cast<size_t>(MapWsSmem(a).total);
+      p.key = {P, a.KS, a.nct};
+      const int stages = a.nChunks * CeilDiv(taps, a.KS);
+      const double ne = static_cast<double>(a.nChunks) * taps;
       // tensor work on PlanPqGemm's scale (as PlanConvWs below), a pipeline drain per weight stage, the set-up
       const double perCta = ne * 2.0 * (P / 64) * (W / 128.0) * (3.0 * 64.0 * 1.15 / 4.0) + 600.0 * stages + 4000.0 + P * 24.0;
-      const double ctas = static_cast<double>(CeilDiv(N * IB, P)) * G * ga.nct;
+      const double ctas = static_cast<double>(CeilDiv(N * IB, P)) * G * a.nct;
       cands->emplace_back(perCta * std::ceil(ctas / L->ctx->sm_count), p);
     }
   }
@@ -471,26 +463,24 @@ void PlanConvWs(const qcnn_layer* L, int N, ConvCands* cands) {
     ConvPlan p;
     memset(&p, 0, sizeof(p));
     p.kernel = kConvWs; p.threads = kWsThreads;
-    GemmArgs& ga = p.g;
-    ga.mode = 1; ga.bf = 1;
-    ga.PW = PWp; ga.IB = IB; ga.NT = P;
-    ga.NPOS = RoundUp(P + ((L->ksz - 1) / st) * (PWp + 1), 8);
-    ga.planeRows = (st / 2) * ga.NPOS;
-    ga.planeF4 = st * ga.NPOS;
-    ga.nChunks = st; ga.nct = 1; ga.nsplit = 1; ga.nPB = st;   // every phase row resident
-    ga.stride = st; ga.Kg = Kg; ga.K = L->K;
-    ga.tapsPad = RoundUp(CeilDiv(L->ksz, st) * L->ksz, 16);
-    const int ne = Mode1Table(L, ga);
+    ConvWsArgs& a = p.ws;
+    SetGemmGeometry(L, a);
+    a.PW = PWp; a.IB = IB; a.P = P; a.NC = Kg; a.nct = 1;
+    a.NPOS = RoundUp(P + ((L->ksz - 1) / st) * (PWp + 1), 8);
+    a.planeRows = (st / 2) * a.NPOS;
+    a.nChunks = st; a.nPB = st;   // every phase row resident
+    a.tapsPad = RoundUp(CeilDiv(L->ksz, st) * L->ksz, 16);
+    const int ne = Mode1Table(L, a.NPOS, true, a.planeRows, a.kt);
     if (ne > kMaxKSteps) continue;
     int maxCnt = 0;
-    for (int ph = 0; ph < st; ph++) maxCnt = std::max(maxCnt, ga.chunkCount[ph]);
+    for (int ph = 0; ph < st; ph++) maxCnt = std::max(maxCnt, a.kt.chunkCount[ph]);
     // k-steps per weight stage: a whole phase row when it fits, else the largest count that does
-    for (ga.GT = maxCnt; ga.GT >= 1 && static_cast<size_t>(MapWsSmem(ga).total) > smemMax; ga.GT--) {}
-    if (ga.GT < 1) continue;
-    p.smem = static_cast<size_t>(MapWsSmem(ga).total);
-    p.key = {P, ga.GT, ga.nct};
+    for (a.KS = maxCnt; a.KS >= 1 && static_cast<size_t>(MapWsSmem(a).total) > smemMax; a.KS--) {}
+    if (a.KS < 1) continue;
+    p.smem = static_cast<size_t>(MapWsSmem(a).total);
+    p.key = {P, a.KS, a.nct};
     int stages = 0;
-    for (int ph = 0; ph < st; ph++) stages += CeilDiv(ga.chunkCount[ph], ga.GT);
+    for (int ph = 0; ph < st; ph++) stages += CeilDiv(a.kt.chunkCount[ph], a.KS);
     // tensor work on PlanPqGemm's scale (its 4 MMAs of m64 n128 k16 per k-step cost 3 * 64 * 1.15), a pipeline drain per
     // weight stage, the set-up and the staging of the first phase row
     const double perCta = ne * 2.0 * (P / 64) * (Kg / 128.0) * (3.0 * 64.0 * 1.15 / 4.0) + 600.0 * stages + 9000.0 + P * 24.0;
@@ -500,37 +490,37 @@ void PlanConvWs(const qcnn_layer* L, int N, ConvCands* cands) {
 }
 
 int LaunchConvWs(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
-  GemmArgs a = p.g;
-  a.src = src; a.dst = dst; a.ctrd = L->d_ctrd_bf.as<float>(); a.bias = L->d_bias.as<float>();
+  ConvWsArgs a = p.ws;
+  a.src = src; a.dst = dst; a.ctrd = L->d_ctrd_bf.as<uint4>(); a.bias = L->d_bias.as<float>();
   a.asmtT = L->d_asmt_t.as<uint8_t>();
   a.N = N; a.relu = relu;
   SetGemmGeometry(L, a);
-  QCNN_CHECK(a.mode == 1 || !L->src_nchw, "qcnn_conv_aprx_forward: the stride-1 weight-stationary tiling reads NHWC sources only");
-  const long long blocks = static_cast<long long>(CeilDiv(N * a.IB, a.NT)) * a.G * a.nct;
+  QCNN_CHECK(a.stride > 1 || !L->src_nchw, "qcnn_conv_aprx_forward: the stride-1 weight-stationary tiling reads NHWC sources only");
+  const long long blocks = static_cast<long long>(CeilDiv(N * a.IB, a.P)) * a.G * a.nct;
   QCNN_CHECK(blocks <= 2147483647LL, "qcnn_conv_aprx_forward: batch too large for the weight-stationary tiling");
   QCNN_CHECK(static_cast<size_t>(MapWsSmem(a).total) == p.smem, "internal: conv_ws shared-memory carve changed after planning");
   const unsigned nb = static_cast<unsigned>(blocks);
-  const int nc = a.Kg / a.nct;
-  if (a.mode == 1) return LaunchWidth<false, false>(a, nc, nb, p.smem, st, L->ctx);
+  if (a.stride > 1) return LaunchWidth<false, false>(a, nb, p.smem, st, L->ctx);
   const bool wide = 2 * a.NPOS > kWsRegPos * kWsProducers || a.Cg < 4;
-  return wide ? LaunchWidth<true, true>(a, nc, nb, p.smem, st, L->ctx) : LaunchWidth<true, false>(a, nc, nb, p.smem, st, L->ctx);
+  return wide ? LaunchWidth<true, true>(a, nb, p.smem, st, L->ctx) : LaunchWidth<true, false>(a, nb, p.smem, st, L->ctx);
 }
 
 void DescribeConvWs(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap) {
-  if (p.g.mode == 0) {
+  const ConvWsArgs& a = p.ws;
+  const int grid = CeilDiv(N * a.IB, a.P) * L->grp * a.nct;
+  if (a.stride == 1) {
     // stride 1: N = channels per CTA, ctiles = channel tiles per group, ksteps = chunks x taps (a CTA's k-steps), so
     // that grid x ksteps x 32 x positions x N is the executed MAC count
-    const int stages = p.g.nChunks * CeilDiv(p.g.ntab, p.g.GT);
+    const int stages = a.nChunks * CeilDiv(a.kt.ntab, a.KS);
     snprintf(buf, cap, " mode=0 N=%d positions=%d ctiles=%d KS=%d smem=%zuB grid=%d NPOS=%d planebufs=%d chunks=%d stages=%d "
-             "ksteps=%d", p.g.Kg / p.g.nct, p.g.NT, p.g.nct, p.g.GT, p.smem, CeilDiv(N * p.g.IB, p.g.NT) * L->grp * p.g.nct,
-             p.g.NPOS, p.g.nPB, p.g.nChunks, stages, p.g.nChunks * p.g.ntab);
+             "ksteps=%d", a.NC, a.P, a.nct, a.KS, p.smem, grid, a.NPOS, a.nPB, a.nChunks, stages, a.nChunks * a.kt.ntab);
     return;
   }
   // (no "NT=": the executed-MAC count that bench.py derives from pq_gemm_tc( plans assumes 128-channel tiles)
   int stages = 0;
-  for (int c = 0; c < p.g.nChunks; c++) stages += CeilDiv(p.g.chunkCount[c], p.g.GT);
-  snprintf(buf, cap, " N=%d positions=%d KS=%d smem=%zuB grid=%d NPOS=%d chunks=%d stages=%d ksteps=%d", p.g.Kg, p.g.NT,
-           p.g.GT, p.smem, CeilDiv(N * p.g.IB, p.g.NT) * L->grp, p.g.NPOS, p.g.nChunks, stages, p.g.ntab);
+  for (int c = 0; c < a.nChunks; c++) stages += CeilDiv(a.kt.chunkCount[c], a.KS);
+  snprintf(buf, cap, " N=%d positions=%d KS=%d smem=%zuB grid=%d NPOS=%d chunks=%d stages=%d ksteps=%d", a.NC, a.P, a.KS,
+           p.smem, grid, a.NPOS, a.nChunks, stages, a.kt.ntab);
 }
 
 }  // namespace qcnn

@@ -680,13 +680,7 @@ int LaunchFcChain(qcnn_ctx* ctx, qcnn_layer* const* layers, const int* relu, int
     if (grown) QCNN_CUDA(cudaMemsetAsync(Q->d_cpart.get(), 0xFF, need, st));
     a.L[l].partial = Q->d_cpart.as<float>();
   }
-  static bool attrSet[64] = {false};
-  if (ctx->device < 64 && !attrSet[ctx->device]) {
-    const int lim = static_cast<int>(SmemOptin(ctx));
-    QCNN_CUDA(cudaFuncSetAttribute(fc_chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    QCNN_CUDA(cudaFuncSetAttribute(fc_chain_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    attrSet[ctx->device] = true;
-  }
+  if (int rc = packed ? OptInSmem<fc_chain_packed_kernel>(ctx) : OptInSmem<fc_chain_kernel>(ctx)) return rc;
   a.dbg = dbg;
   const size_t srcImg = layers[0]->Din, dstImg = layers[n - 1]->Dout;
   for (int i = 0; i < N; i++) {

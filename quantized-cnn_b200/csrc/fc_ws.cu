@@ -278,15 +278,9 @@ __global__ void __launch_bounds__(kWsThreads, 1) fc_ws_kernel(const FcWsArgs a) 
 // (channels per CTA, m64 blocks per consumer warpgroup) with an instantiation, in the planner's order of preference
 constexpr int kFcWsShapes[][2] = {{256, 1}, {128, 1}, {128, 2}, {64, 1}, {64, 2}};
 
-// the dynamic shared-memory limit of an instantiation is raised once per device to the opt-in maximum
 template <int NC, int MB, bool D1>
-int SetSmemAndLaunch(const FcWsArgs& a, unsigned blocks, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
-  static bool done[64] = {false};
-  if (ctx->device < 0 || ctx->device >= 64 || !done[ctx->device]) {
-    const int lim = static_cast<int>(qcnn::SmemOptin(ctx));
-    QCNN_CUDA(cudaFuncSetAttribute(fc_ws_kernel<NC, MB, D1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    if (ctx->device >= 0 && ctx->device < 64) done[ctx->device] = true;
-  }
+int LaunchInstance(const FcWsArgs& a, unsigned blocks, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
+  if (int rc = qcnn::OptInSmem<fc_ws_kernel<NC, MB, D1>>(ctx)) return rc;
   fc_ws_kernel<NC, MB, D1><<<blocks, kWsThreads, smem, st>>>(a);
   QCNN_CUDA(cudaGetLastError());
   return 0;
@@ -294,11 +288,11 @@ int SetSmemAndLaunch(const FcWsArgs& a, unsigned blocks, size_t smem, cudaStream
 
 template <bool D1>
 int LaunchShape(const FcWsArgs& a, int nc, int mb, unsigned nb, size_t smem, cudaStream_t st, qcnn_ctx* ctx) {
-  if (nc == 256 && mb == 1) return SetSmemAndLaunch<256, 1, D1>(a, nb, smem, st, ctx);
-  if (nc == 128 && mb == 1) return SetSmemAndLaunch<128, 1, D1>(a, nb, smem, st, ctx);
-  if (nc == 128 && mb == 2) return SetSmemAndLaunch<128, 2, D1>(a, nb, smem, st, ctx);
-  if (nc == 64 && mb == 1) return SetSmemAndLaunch<64, 1, D1>(a, nb, smem, st, ctx);
-  if (nc == 64 && mb == 2) return SetSmemAndLaunch<64, 2, D1>(a, nb, smem, st, ctx);
+  if (nc == 256 && mb == 1) return LaunchInstance<256, 1, D1>(a, nb, smem, st, ctx);
+  if (nc == 128 && mb == 1) return LaunchInstance<128, 1, D1>(a, nb, smem, st, ctx);
+  if (nc == 128 && mb == 2) return LaunchInstance<128, 2, D1>(a, nb, smem, st, ctx);
+  if (nc == 64 && mb == 1) return LaunchInstance<64, 1, D1>(a, nb, smem, st, ctx);
+  if (nc == 64 && mb == 2) return LaunchInstance<64, 2, D1>(a, nb, smem, st, ctx);
   qcnn::SetError("internal: no fc_ws instantiation for N=%d images=%d", nc, 128 * mb);
   return 1;
 }

@@ -136,58 +136,6 @@ __global__ void __launch_bounds__(kThreads, 1) pq_gemm_tc_packed_kernel(const Ge
 
 namespace qcnn {
 
-// Mode 1 k-step table (strided layer on phase planes): for every phase row ph, its k-steps in (kh, kw) order, as entries
-// [chunkFirst[ph], + chunkCount[ph]) of ga.tab.  Reads ga.NPOS, ga.bf and ga.planeRows.  Returns the number of k-steps
-// (> kMaxKSteps: the table does not fit) and sets ga.ntab.  The weight-stationary kernel (conv_ws.cu) runs the same table.
-int Mode1Table(const qcnn_layer* L, GemmArgs& ga) {
-  const int st = L->stride, PWp = CeilDiv(L->Win + 2 * L->pad, st);
-  int ne = 0;
-  for (int ph = 0; ph < st; ph++) {
-    ga.chunkFirst[ph] = ne;
-    for (int kh = ph; kh < L->ksz; kh += st)
-      for (int kw = 0; kw < L->ksz; kw += 2, ne++) {
-        if (ne >= kMaxKSteps) { ne = kMaxKSteps + 1000; break; }
-        KStep& ks = ga.tab[ne];
-        // partner in the next phase column, same shift (bf16x2: the partner must be the odd column of the same pair)
-        const bool paired = kw + 1 < L->ksz && (kw % st) + 1 < st && !(ga.bf && ((kw % st) & 1));
-        ks.bStart = (kw % st) * ga.NPOS + (kh / st) * PWp + kw / st;
-        // an unpaired tap's second half (zero codebook slot) aliases its first half (LBO = 0): a shift would read
-        // the next position -- for a tile's last position, or a tap at the end of an image, another image's
-        // pixel -- and 0 * NaN / Inf would carry that image's non-finite values into this one's output
-        ks.lbo = paired ? ga.NPOS : 0;
-        if (ga.bf) {   // row = (pair of phase columns, position); K-core-matrix 1 = the x2 plane
-          ks.bStart = ((kw % st) >> 1) * ga.NPOS + (kh / st) * PWp + kw / st;
-          ks.lbo = ga.planeRows;
-        }
-        ks.idx0 = static_cast<short>((kh - ph) / st * L->ksz + kw);
-        ks.idx1 = static_cast<short>(paired ? ks.idx0 + 1 : ks.idx0);
-        ks.cb0 = 0; ks.cb1 = paired ? 0 : 1;
-        if (!paired && kw + 1 < L->ksz) kw--;   // the partner starts its own k-step
-      }
-    ga.chunkCount[ph] = ne - ga.chunkFirst[ph];
-  }
-  ga.ntab = ne;
-  return ne;
-}
-
-// Mode 0 k-step table (stride-1 layer on the flat padded grid): the taps of a chunk in (kh, kw) order, a tap being a shift
-// of the position operand's start by kh * PW + kw rows, K-core-matrix 1 (the chunk's second half / the x2 plane) NPOS rows
-// further; index row and codebook slot = (half, tap).  Reads ga.PW and ga.NPOS, sets ga.ntab and the chunk range, returns
-// the number of k-steps per chunk.  The weight-stationary kernel (conv_ws.cu) runs the same table.
-int Mode0Table(const qcnn_layer* L, GemmArgs& ga) {
-  const int taps = L->ksz * L->ksz;
-  ga.ntab = taps;
-  ga.chunkFirst[0] = 0; ga.chunkCount[0] = taps;
-  for (int t = 0; t < taps; t++) {
-    KStep& ks = ga.tab[t];
-    ks.bStart = (t / L->ksz) * ga.PW + (t % L->ksz);
-    ks.lbo = ga.NPOS;
-    ks.idx0 = static_cast<short>(t); ks.idx1 = static_cast<short>(taps + t);
-    ks.cb0 = 0; ks.cb1 = 1;
-  }
-  return taps;
-}
-
 // Candidate tilings for batch N (cost in SM-cycles, comparable with PlanLutGather's model); on-device timing chooses among them.
 void PlanPqGemm(const qcnn_layer* L, int N, ConvCands* cands) {
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, taps = L->ksz * L->ksz;
@@ -227,7 +175,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, ConvCands* cands) {
         // never wait for the MMAs and the few k-steps of a phase row (conv1: 16-18) are not what hides a global-load latency
         if (ga.bf && st <= 4) ga.nPB = st;
         ga.nct = CeilDiv(Kg, 128);
-        const int ne = Mode1Table(L, ga);
+        const int ne = Mode1Table(L, ga.NPOS, ga.bf, ga.planeRows, ga);
         if (ne > kMaxKSteps) continue;
         p.smem = static_cast<size_t>(MapSmem(ga).total);
         if (p.smem > smemMax) continue;
@@ -272,7 +220,7 @@ void PlanPqGemm(const qcnn_layer* L, int N, ConvCands* cands) {
       ga.idxT = (ga.tapsPad <= 32 && L->asmt_t_mode == 0) ? 1 : 0;
       if (ga.idxT) ga.idRows = 2 * ga.tapsPad;      // [half][128 channels][tapsPad] bytes = 2 * tapsPad rows of 128
       ga.nChunks = CeilDiv(Cg, 8);
-      Mode0Table(L, ga);
+      Mode0Table(L, ga.PW, ga.NPOS, ga);
       ga.K = L->K; ga.cbF4 = L->K; ga.nPB = 2;
       ga.nct = CeilDiv(Kg, 128);
       p.smem = static_cast<size_t>(MapSmem(ga).total);
@@ -293,43 +241,28 @@ void PlanPqGemm(const qcnn_layer* L, int N, ConvCands* cands) {
     }
   }
 }
-// dynamic shared-memory limit of the instantiations: raised once per device to the opt-in maximum (not per launch,
-// which would make the limit follow whichever layer ran last -- fragile under graph capture / concurrent streams)
-static int SetSmemLimitOnce(qcnn_ctx* ctx) {
-  static bool done[64] = {false};
-  if (ctx->device >= 0 && ctx->device < 64 && done[ctx->device]) return 0;
-  const int lim = static_cast<int>(SmemOptin(ctx));
-#define QCNN_SMEM_ATTR(...) QCNN_CUDA(cudaFuncSetAttribute(pq_gemm_tc_kernel<__VA_ARGS__>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim))
-  QCNN_SMEM_ATTR(true, 128); QCNN_SMEM_ATTR(true, 64); QCNN_SMEM_ATTR(false, 128); QCNN_SMEM_ATTR(false, 64);
-#undef QCNN_SMEM_ATTR
-#define QCNN_SMEM_ATTR(...) QCNN_CUDA(cudaFuncSetAttribute(pq_gemm_tc_packed_kernel<__VA_ARGS__>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim))
-  QCNN_SMEM_ATTR(true, 128); QCNN_SMEM_ATTR(true, 64); QCNN_SMEM_ATTR(false, 128); QCNN_SMEM_ATTR(false, 64);
-#undef QCNN_SMEM_ATTR
-  if (ctx->device >= 0 && ctx->device < 64) done[ctx->device] = true;
-  return 0;
-}
-
-static int LaunchKernel(const GemmArgs& a, unsigned blocks, size_t smem, cudaStream_t st, int pkBits = 0, int pkPitch = 0) {
-  QCNN_CHECK((a.NT == 128 || a.NT == 64) && a.corr == (a.NT == 64 ? 1 : 0) && a.GT >= 1 && a.GT <= kMaxGT,
-             "pq_gemm_tc: no instantiation for NT=%d GT=%d", a.NT, a.GT);
+template <bool BF, int NT>
+static int LaunchInstance(qcnn_ctx* ctx, const GemmArgs& a, unsigned blocks, size_t smem, cudaStream_t st, int pkBits, int pkPitch) {
   if (pkBits) {
-    QCNN_CHECK(a.mode == 2 && pkBits >= 4 && pkBits <= 7, "pq_gemm_tc: a bit-packed table is only read by mode 2 (FC)");
-    if (a.bf) {
-      if (a.NT == 128) pq_gemm_tc_packed_kernel<true, 128><<<blocks, kThreads, smem, st>>>(a, pkBits, pkPitch);
-      else pq_gemm_tc_packed_kernel<true, 64><<<blocks, kThreads, smem, st>>>(a, pkBits, pkPitch);
-    } else {
-      if (a.NT == 128) pq_gemm_tc_packed_kernel<false, 128><<<blocks, kThreads, smem, st>>>(a, pkBits, pkPitch);
-      else pq_gemm_tc_packed_kernel<false, 64><<<blocks, kThreads, smem, st>>>(a, pkBits, pkPitch);
-    }
-  } else if (a.bf) {
-    if (a.NT == 128) pq_gemm_tc_kernel<true, 128><<<blocks, kThreads, smem, st>>>(a);
-    else pq_gemm_tc_kernel<true, 64><<<blocks, kThreads, smem, st>>>(a);
+    if (int rc = OptInSmem<pq_gemm_tc_packed_kernel<BF, NT>>(ctx)) return rc;
+    pq_gemm_tc_packed_kernel<BF, NT><<<blocks, kThreads, smem, st>>>(a, pkBits, pkPitch);
   } else {
-    if (a.NT == 128) pq_gemm_tc_kernel<false, 128><<<blocks, kThreads, smem, st>>>(a);
-    else pq_gemm_tc_kernel<false, 64><<<blocks, kThreads, smem, st>>>(a);
+    if (int rc = OptInSmem<pq_gemm_tc_kernel<BF, NT>>(ctx)) return rc;
+    pq_gemm_tc_kernel<BF, NT><<<blocks, kThreads, smem, st>>>(a);
   }
   QCNN_CUDA(cudaGetLastError());
   return 0;
+}
+
+static int LaunchKernel(qcnn_ctx* ctx, const GemmArgs& a, unsigned blocks, size_t smem, cudaStream_t st, int pkBits = 0,
+                        int pkPitch = 0) {
+  QCNN_CHECK((a.NT == 128 || a.NT == 64) && a.corr == (a.NT == 64 ? 1 : 0) && a.GT >= 1 && a.GT <= kMaxGT,
+             "pq_gemm_tc: no instantiation for NT=%d GT=%d", a.NT, a.GT);
+  QCNN_CHECK(!pkBits || (a.mode == 2 && pkBits >= 4 && pkBits <= 7), "pq_gemm_tc: a bit-packed table is only read by mode 2 (FC)");
+  if (a.bf) return a.NT == 128 ? LaunchInstance<true, 128>(ctx, a, blocks, smem, st, pkBits, pkPitch)
+                               : LaunchInstance<true, 64>(ctx, a, blocks, smem, st, pkBits, pkPitch);
+  return a.NT == 128 ? LaunchInstance<false, 128>(ctx, a, blocks, smem, st, pkBits, pkPitch)
+                     : LaunchInstance<false, 64>(ctx, a, blocks, smem, st, pkBits, pkPitch);
 }
 
 // bf16x2 form of the codebook, made once per layer: every aligned 4-float piece becomes {w1 (4 x bf16), w2 (4 x bf16)},
@@ -343,16 +276,6 @@ int BuildCtrdBf(qcnn_layer* L) {
   QCNN_CUDA(cudaGetLastError());
   QCNN_CUDA(cudaDeviceSynchronize());
   return 0;
-}
-
-void SetGemmGeometry(const qcnn_layer* L, GemmArgs& a) {
-  a.Hi = L->Hin; a.Wi = L->Win; a.Cin = L->Cin; a.Ho = L->Ho; a.Wo = L->Wo; a.Cout = L->Cout;
-  a.ksz = L->ksz; a.pad = L->pad; a.stride = L->stride; a.G = L->grp; a.Cg = L->Cin / L->grp; a.Kg = L->Cout / L->grp;
-  a.KgPad = RoundUp(a.Kg, 16); a.S = L->S; a.K = L->K; a.d = L->d;
-  a.srcImg = static_cast<long long>(a.Hi) * a.Wi * a.Cin;
-  if (L->src_nchw) { a.rowStride = a.Wi; a.colStride = 1; a.chStride = a.Hi * a.Wi; }
-  else { a.rowStride = a.Wi * a.Cin; a.colStride = a.Cin; a.chStride = 1; }
-  a.dstImg = static_cast<long long>(a.Ho) * a.Wo * a.Cout;
 }
 
 int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
@@ -371,8 +294,7 @@ int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, floa
     QCNN_CUDA(L->d_partial.Reserve(L->ctx, sizeof(float) * static_cast<size_t>(a.nsplit) * N * a.dstImg, st));
     a.partial = L->d_partial.as<float>();
   }
-  if (int rc = SetSmemLimitOnce(L->ctx)) return rc;
-  if (int rc = LaunchKernel(a, static_cast<unsigned>(blocks), p.smem, st)) return rc;
+  if (int rc = LaunchKernel(L->ctx, a, static_cast<unsigned>(blocks), p.smem, st)) return rc;
   if (a.nsplit > 1)
     return LaunchSplitReduce(L->ctx, a.partial, dst, N * a.Ho * a.Wo, a.Cout, a.Cout, a.nsplit, relu, st);
   return 0;
@@ -391,8 +313,7 @@ void DescribePqGemm(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, si
 size_t PqGemmSmemBytes(const GemmArgs& a) { return static_cast<size_t>(MapSmem(a).total); }
 int LaunchPqGemmArgs(qcnn_ctx* ctx, const GemmArgs& a, long long blocks, cudaStream_t st, int asmtBits, int asmtPitch) {
   QCNN_CHECK(blocks >= 1 && blocks <= 2147483647LL, "pq_gemm_tc: bad grid");
-  if (int rc = SetSmemLimitOnce(ctx)) return rc;
-  return LaunchKernel(a, static_cast<unsigned>(blocks), PqGemmSmemBytes(a), st, asmtBits, asmtPitch);
+  return LaunchKernel(ctx, a, static_cast<unsigned>(blocks), PqGemmSmemBytes(a), st, asmtBits, asmtPitch);
 }
 
 }  // namespace qcnn

@@ -182,6 +182,12 @@ struct KStep {           // one K = 8 step of the GEMM: two 4-float halves
   short idx0, idx1;      // assignment-index row of either half inside the chunk's staged rows
   short cb0, cb1;        // codebook slot of either half inside the chunk's staged slices
 };
+// A tensor-core GEMM's k-steps in the order its accumulator chains them (Mode0Table / Mode1Table fill it)
+struct KStepTable {
+  int ntab;
+  int chunkFirst[8], chunkCount[8];   // k-step range of a chunk (mode 1: per phase row; else entry 0)
+  KStep tab[kMaxKSteps];
+};
 struct GemmArgs {
   const float* src;
   float* dst;
@@ -197,7 +203,7 @@ struct GemmArgs {
   int kshift;                   // stored assignment byte = index << kshift
   float* partial;               // mode 2, nsplit > 1: [nsplit][N][dstRow]
   int dstRow;                   // mode 2: floats per destination row
-  int nPB;                      // position-plane buffers (2; 3 for mode 2, whose planes arrive by bulk copy; conv_ws: its ring / phase rows)
+  int nPB;                      // position-plane buffers (2; 3 for mode 2, whose planes arrive by bulk copy)
   const float* xprep;           // mode 2: activations pre-split into the plane image (fc_prep_kernel), [tile][chunk][hi,lo][2KS][NT][4]
   int nChunksAll;               // mode 2: chunks of the whole layer (xprep indexing)
   int cbF4;                     // float4 per codebook slot (K for d % 4 == 0 pieces, K/4 for d == 1 scalars)
@@ -215,10 +221,11 @@ struct GemmArgs {
   int cbSlots, idRows;        // codebook slices / index rows staged per chunk
   int nChunks;
   int GT;                     // k-steps per stage (decoded into registers together, <= 4)
-  int nct;                    // channel tiles per group (pq_gemm_tc: of 128 channels; conv_ws: of Kg / nct channels)
+  int nct;                    // channel tiles of 128 channels per group
   int relu;
+  // a KStepTable's fields, kept flat: as one nested member they cost the 3xTF32 instantiations 1-2 % of their time
   int ntab;
-  int chunkFirst[8], chunkCount[8];   // k-step table range of a chunk (mode 1: per phase row; else entry 0)
+  int chunkFirst[8], chunkCount[8];
   KStep tab[kMaxKSteps];
 };
 
@@ -234,15 +241,35 @@ enum ConvKernel {
   kConvKernelIds = 8
 };
 
+// The arguments of conv_ws_kernel (conv_ws.cu), its only reader; declared here so that ConvPlan holds a tiling by value.
+// Field order chosen so that conv_ws_kernel's parameter loads and register allocation match those of its GemmArgs form.
+struct ConvWsArgs {
+  const float* src;
+  float* dst;
+  const uint4* ctrd;          // pre-split codebook (qcnn_layer::d_ctrd_bf)
+  const uint8_t* asmtT;       // channel-major index block (qcnn_layer::d_asmt_t)
+  const float* bias;
+  long long srcImg, dstImg;   // elements per source / destination image
+  int N, Hi, Wi, Cin, Ho, Wo, Cout, ksz, pad, stride, G, Cg, Kg, KgPad, S, K, d;
+  int NC, PW, IB;             // channels per CTA (N of the MMA) / grid row pitch / positions per image
+  int rowStride, colStride, chStride;   // source element strides of an input row / column / channel
+  int nPB, P, tapsPad;        // plane buffers (strided: one per phase row) / positions per CTA / index bytes per channel
+  int planeRows, NPOS;        // 16-byte rows per plane / staged positions per plane (P + halo)
+  int KS, nct, nChunks;       // k-steps per weight stage / channel tiles per group (Kg / NC) / chunks (8 channels or a phase row)
+  int relu;
+  KStepTable kt;
+};
+
 struct ConvPlan {
   int kernel;           // ConvKernel
   int CPT, J;           // LUT + gather kernels: channels per thread / positions per lane (conv_direct: output rows)
   int threads;
   size_t smem;
   std::array<int, 6> key;   // equal keys of one kernel: near-duplicates.  LUT + gather: CPT, J, nct, nstrips, rgroups, R;
-                            // pq_gemm_tc: NT, GT, nct, nsplit; conv_ws: positions, GT, nct (unused entries 0)
+                            // pq_gemm_tc: NT, GT, nct, nsplit; conv_ws: P, KS, nct (unused entries 0)
   ConvArgs a;           // kernels 0-4: geometry + tiling (pointers/N filled at launch)
-  GemmArgs g;           // kernels 6 (pq_gemm_tc) and 7 (conv_ws)
+  GemmArgs g;           // kernel 6 (pq_gemm_tc)
+  ConvWsArgs ws;        // kernel 7 (conv_ws)
 };
 
 // FcPlan::kernel, in the order the rule of fc_plan.cu tries them: fc_chain.cu, fc_ws.cu, pq_gemm_tc mode 2, LUT + gather
@@ -348,14 +375,87 @@ int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows,
 // pq_gemm_tc.cu
 void PlanPqGemm(const qcnn_layer* L, int N, ConvCands* cands);
 void DescribePqGemm(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap);
-void SetGemmGeometry(const qcnn_layer* L, GemmArgs& a);   // a conv layer's geometry and image strides, at launch
 size_t PqGemmSmemBytes(const GemmArgs& a);
 // asmtBits != 0 (mode 2): a.asmt is the bit-packed FC table of packed_asmt.h with rows of asmtPitch bytes
 int LaunchPqGemmArgs(qcnn_ctx* ctx, const GemmArgs& a, long long blocks, cudaStream_t st, int asmtBits = 0, int asmtPitch = 0);
 int BuildCtrdBf(qcnn_layer* L);   // layer creation: the bf16x2 form of the codebook (d % 4 == 0)
 int LaunchPqGemm(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
-int Mode0Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a stride-1 layer on the flat padded grid
-int Mode1Table(const qcnn_layer* L, GemmArgs& ga);   // k-step table of a strided layer on bf16x2 / tf32 phase planes
+// A conv layer's geometry and image strides in the argument block of pq_gemm_tc (GemmArgs) or conv_ws (ConvWsArgs).  Set
+// at every launch: qcnn_conv_layer_set_src_nchw may change the source strides after planning.
+template <class A>
+void SetGemmGeometry(const qcnn_layer* L, A& a) {
+  a.Hi = L->Hin; a.Wi = L->Win; a.Cin = L->Cin; a.Ho = L->Ho; a.Wo = L->Wo; a.Cout = L->Cout;
+  a.ksz = L->ksz; a.pad = L->pad; a.stride = L->stride; a.G = L->grp; a.Cg = L->Cin / L->grp; a.Kg = L->Cout / L->grp;
+  a.KgPad = RoundUp(a.Kg, 16); a.S = L->S; a.K = L->K; a.d = L->d;
+  a.srcImg = static_cast<long long>(a.Hi) * a.Wi * a.Cin;
+  if (L->src_nchw) { a.rowStride = a.Wi; a.colStride = 1; a.chStride = a.Hi * a.Wi; }
+  else { a.rowStride = a.Wi * a.Cin; a.colStride = a.Cin; a.chStride = 1; }
+  a.dstImg = static_cast<long long>(a.Ho) * a.Wo * a.Cout;
+}
+
+// Mode 1 k-step table (strided layer on phase planes of NPOS positions, bf: bf16x2 planes of planeRows rows): for every
+// phase row ph, its k-steps in (kh, kw) order, as entries [chunkFirst[ph], + chunkCount[ph]) of t.tab.  Returns the number
+// of k-steps (> kMaxKSteps: the table does not fit).  t: a KStepTable (conv_ws) or the same fields of GemmArgs (pq_gemm_tc).
+template <class T> int Mode1Table(const qcnn_layer* L, int NPOS, bool bf, int planeRows, T& t) {
+  const int st = L->stride, PWp = CeilDiv(L->Win + 2 * L->pad, st);
+  int ne = 0;
+  for (int ph = 0; ph < st; ph++) {
+    t.chunkFirst[ph] = ne;
+    for (int kh = ph; kh < L->ksz; kh += st)
+      for (int kw = 0; kw < L->ksz; kw += 2, ne++) {
+        if (ne >= kMaxKSteps) { ne = kMaxKSteps + 1000; break; }
+        KStep& ks = t.tab[ne];
+        // partner in the next phase column, same shift (bf16x2: the partner must be the odd column of the same pair)
+        const bool paired = kw + 1 < L->ksz && (kw % st) + 1 < st && !(bf && ((kw % st) & 1));
+        ks.bStart = (kw % st) * NPOS + (kh / st) * PWp + kw / st;
+        // an unpaired tap's second half (zero codebook slot) aliases its first half (LBO = 0): a shift would read
+        // the next position -- for a tile's last position, or a tap at the end of an image, another image's
+        // pixel -- and 0 * NaN / Inf would carry that image's non-finite values into this one's output
+        ks.lbo = paired ? NPOS : 0;
+        if (bf) {   // row = (pair of phase columns, position); K-core-matrix 1 = the x2 plane
+          ks.bStart = ((kw % st) >> 1) * NPOS + (kh / st) * PWp + kw / st;
+          ks.lbo = planeRows;
+        }
+        ks.idx0 = static_cast<short>((kh - ph) / st * L->ksz + kw);
+        ks.idx1 = static_cast<short>(paired ? ks.idx0 + 1 : ks.idx0);
+        ks.cb0 = 0; ks.cb1 = paired ? 0 : 1;
+        if (!paired && kw + 1 < L->ksz) kw--;   // the partner starts its own k-step
+      }
+    t.chunkCount[ph] = ne - t.chunkFirst[ph];
+  }
+  t.ntab = ne;
+  return ne;
+}
+
+// Mode 0 k-step table (stride-1 layer on the flat padded grid): the taps of a chunk in (kh, kw) order, a tap being a shift
+// of the position operand's start by kh * PW + kw rows, K-core-matrix 1 (the chunk's second half / the x2 plane) NPOS rows
+// further; index row and codebook slot = (half, tap).  Returns the number of k-steps per chunk.  t: as for Mode1Table.
+template <class T> int Mode0Table(const qcnn_layer* L, int PW, int NPOS, T& t) {
+  const int taps = L->ksz * L->ksz;
+  t.ntab = taps;
+  t.chunkFirst[0] = 0; t.chunkCount[0] = taps;
+  for (int i = 0; i < taps; i++) {
+    KStep& ks = t.tab[i];
+    ks.bStart = (i / L->ksz) * PW + (i % L->ksz);
+    ks.lbo = NPOS;
+    ks.idx0 = static_cast<short>(i); ks.idx1 = static_cast<short>(taps + i);
+    ks.cb0 = 0; ks.cb1 = 1;
+  }
+  return taps;
+}
+
+// Raises a kernel's dynamic shared-memory limit to the opt-in maximum once per kernel and device (per launch, the limit
+// would follow whichever layer ran last: fragile under graph capture).  A device id past the table is raised every call.
+template <auto Kernel>
+int OptInSmem(qcnn_ctx* ctx) {
+  static bool done[64] = {false};
+  const bool inTable = ctx->device >= 0 && ctx->device < 64;
+  if (inTable && done[ctx->device]) return 0;
+  QCNN_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(SmemOptin(ctx))));
+  if (inTable) done[ctx->device] = true;
+  return 0;
+}
+
 // conv_ws.cu: the tensor-core family's weight-stationary tilings of stride-1 layers (mode-0 geometry, channel tiles) and
 // of strided narrow-input layers (mode-1 geometry)
 void PlanConvWs(const qcnn_layer* L, int N, ConvCands* cands);
