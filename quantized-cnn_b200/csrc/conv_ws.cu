@@ -47,6 +47,17 @@ using qcnn::SmemU32;
 using qcnn::SplitBf16x4;
 
 constexpr int kWsRegPos = 8;        // mode 0: float4 of a chunk's planes a producer thread stages per register pass
+constexpr int kWsRegItems1 = 12;    // mode 1: float4 of a phase row's planes a producer thread holds (st * NPOS <= 1536)
+constexpr int kNoRow = -(1 << 30);  // mode 1: input row of an item that stages zeros in every phase row
+
+// byte t (< 48) of the 48 bytes r[0..2] held in registers: a channel's index row of one phase row (t is warp-uniform:
+// selects, no local memory)
+__device__ __forceinline__ int ByteOf48(const uint4 (&r)[3], int t) {
+  const uint4 q = (t & 32) ? r[2] : (t & 16) ? r[1] : r[0];
+  const uint32_t xy = (t & 4) ? q.y : q.x, zw = (t & 4) ? q.w : q.z;
+  const uint32_t v = (t & 8) ? zw : xy;
+  return static_cast<int>((v >> ((t & 3) * 8)) & 0xFFu);
+}
 
 // Shared-memory carve, read by the planner (fits / does not fit) and by the kernel.  The channel count is computed as
 // Kg / nct rather than read from NC: reading NC changed the kernels' register allocation.
@@ -251,50 +262,92 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const ConvWsArgs
       }
       return;
     }
-    const int st = a.stride;
+    // A phase row's planes are st * NPOS float4 items p = (position pos, phase column pw), pw fastest, so that a warp reads
+    // consecutive pixels of an input row; thread pt holds items pt + i * kWsProducers (i < kWsRegItems1) in registers.  Per
+    // item, computed once per tile: the source offset of phase row 0 and its input row hr (phase row ph reads input row
+    // hr + ph, one row pitch further per phase; kNoRow: the item is outside the image or the batch, or past the planes).
+    const int st = a.stride, sh = st >> 1, nItems = st * a.NPOS;   // (stride 2 or 4: pos = p >> sh, pw = p & (st - 1))
     const float* srcBase = a.src + static_cast<size_t>(i0) * a.srcImg + static_cast<size_t>(g) * a.Cg * a.chStride;
+    int poff[kWsRegItems1], hr[kWsRegItems1];
+#pragma unroll
+    for (int i = 0; i < kWsRegItems1; i++) {
+      const int p = pt + i * kWsProducers, pos = p >> sh, pw = p & (st - 1);
+      const int F = Q0 + pos;
+      const int im = F / a.IB, rem = F - im * a.IB;
+      const int r = rem / a.PW, c = rem - r * a.PW;
+      const int wi = c * st + pw - a.pad;
+      poff[i] = 0; hr[i] = kNoRow;
+      if (p < nItems && im < a.N && static_cast<unsigned>(wi) < static_cast<unsigned>(a.Wi)) {
+        hr[i] = r * st - a.pad;
+        poff[i] = (im - i0) * static_cast<int>(a.srcImg) + hr[i] * a.rowStride + wi * a.colStride;
+      }
+    }
+    float4 rg[kWsRegItems1];
+    auto loadRow = [&](int ph) {   // every load of the phase row is issued before any is used
+      const float* s = srcBase + ph * a.rowStride;
+#pragma unroll
+      for (int i = 0; i < kWsRegItems1; i++) {
+        rg[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (static_cast<unsigned>(hr[i] + ph) < static_cast<unsigned>(a.Hi)) {
+          const float* px = s + poff[i];
+          rg[i].x = __ldg(px);
+          if (a.Cg > 1) rg[i].y = __ldg(px + a.chStride);
+          if (a.Cg > 2) rg[i].z = __ldg(px + 2 * a.chStride);
+          if (a.Cg > 3) rg[i].w = __ldg(px + 3 * a.chStride);
+        }
+      }
+    };
+    loadRow(0);
     for (int ph = 0; ph < st; ph++) {
-      // planes of phase row ph: staged float4 p = (phase column pw, position pos) -> pixel (r*stride + ph - pad,
-      // c*stride + pw - pad) of image i; zero outside the image (and beyond the batch)
+      // a thread owns channel c (pt, then pt + 128 when NC > 128): its index row of the phase row is [tapsPad] bytes of
+      // d_asmt_t, held in registers as three 16-byte granules (the first channel's in flight during the planes' split);
+      // longer rows (more than 48 taps per phase row, e.g. 11 x 11 / 2) are read byte by byte at each k-step
+      const uint8_t* idxB = a.asmtT + static_cast<size_t>(g * st + ph) * a.KgPad * a.tapsPad;
+      const uint4* idx = reinterpret_cast<const uint4*>(idxB);
+      const bool longRow = a.tapsPad > 48;
+      const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+      auto idxRow = [&](int c, uint4 (&r)[3]) {
+        const uint4* row = idx + c * (a.tapsPad >> 4);
+        r[0] = __ldg(row);
+        r[1] = a.tapsPad > 16 ? __ldg(row + 1) : zero;
+        r[2] = a.tapsPad > 32 ? __ldg(row + 2) : zero;
+      };
+      uint4 ixA[3] = {zero, zero, zero};
+      if (pt < NC) idxRow(pt, ixA);
+      // planes of phase row ph: item p -> pixel (r*stride + ph - pad, c*stride + pw - pad) of its image (zero outside);
+      // plane row = (pair of phase columns, position), the parity of pw selects the half
       char* x1 = reinterpret_cast<char*>(planes + ph * 2 * a.planeRows);
       char* x2 = x1 + a.planeRows * 16;
-      for (int p = pt; p < st * a.NPOS; p += kWsProducers) {
-        const int pw = p / a.NPOS, pos = p - pw * a.NPOS;
-        const int F = Q0 + pos;
-        const int i = F / a.IB, rem = F - i * a.IB;
-        const int r = rem / a.PW, c = rem - r * a.PW;
-        const int hi = r * st + ph - a.pad, wi = c * st + pw - a.pad;
-        float4 v = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-        if (i < a.N && static_cast<unsigned>(hi) < static_cast<unsigned>(a.Hi) && static_cast<unsigned>(wi) < static_cast<unsigned>(a.Wi)) {
-          const float* px = srcBase + static_cast<size_t>(i - i0) * a.srcImg + hi * a.rowStride + wi * a.colStride;
-          v.x = __ldg(px);
-          if (a.Cg > 1) v.y = __ldg(px + a.chStride);
-          if (a.Cg > 2) v.z = __ldg(px + 2 * a.chStride);
-          if (a.Cg > 3) v.w = __ldg(px + 3 * a.chStride);
+#pragma unroll
+      for (int i = 0; i < kWsRegItems1; i++) {
+        const int p = pt + i * kWsProducers, pos = p >> sh, pw = p & (st - 1);
+        if (p < nItems) {
+          uint2 p1, p2;
+          SplitBf16x4(rg[i], p1, p2);
+          const int db = ((pw >> 1) * a.NPOS + pos) * 16 + (pw & 1) * 8;
+          *reinterpret_cast<uint2*>(x1 + db) = p1;
+          *reinterpret_cast<uint2*>(x2 + db) = p2;
         }
-        // row = (pair of phase columns, position), the parity selects the half
-        uint2 p1, p2;
-        SplitBf16x4(v, p1, p2);
-        const int db = ((pw >> 1) * a.NPOS + pos) * 16 + (pw & 1) * 8;
-        *reinterpret_cast<uint2*>(x1 + db) = p1;
-        *reinterpret_cast<uint2*>(x2 + db) = p2;
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // planes are read by the tensor core
       MbarArrive(fullP + ph);
-      // weights of the phase row's stages: a thread owns channel c, its index row is [tapsPad] bytes of d_asmt_t
+      if (ph + 1 < st) loadRow(ph + 1);   // in flight during the decode below
+      // weights of the phase row's stages
       const int first = a.kt.chunkFirst[ph], cnt = a.kt.chunkCount[ph];
       for (int s0 = 0; s0 < cnt; s0 += KS, j++) {
         const int n = min(KS, cnt - s0), b = j & 1;
         if (j >= 2) MbarWait<24>(emptyW + b, ((j >> 1) - 1) & 1);   // buffer last read by the MMAs of stage j - 2
         uint4* w = wts + b * KS * 2 * NC;
         for (int c = pt; c < NC; c += kWsProducers) {
-          const uint8_t* row = a.asmtT + (static_cast<size_t>(g * st + ph) * a.KgPad + c) * a.tapsPad;
+          uint4 ix[3] = {ixA[0], ixA[1], ixA[2]};
+          if (c != pt) idxRow(c, ix);
+          const uint8_t* rowB = idxB + static_cast<size_t>(c) * a.tapsPad;
           // (no unroll pragma here: under `#pragma unroll 3` the compiled loop was seen running an iteration with e == n
           // for n = 8 on the device, writing past the weight buffer into the codebook / offset regions)
           for (int e = 0; e < n; e++) {
             const KStep ks = a.kt.tab[first + s0 + e];
-            const uint4 q0 = cb[__ldg(row + ks.idx0)];
-            const uint4 q1 = ks.cb1 ? make_uint4(0u, 0u, 0u, 0u) : cb[__ldg(row + ks.idx1)];   // unpaired tap: zero half
+            const uint4 q0 = cb[longRow ? __ldg(rowB + ks.idx0) : ByteOf48(ix, ks.idx0)];
+            const uint4 q1 = ks.cb1 ? zero : cb[longRow ? __ldg(rowB + ks.idx1) : ByteOf48(ix, ks.idx1)];   // unpaired tap: zero half
             w[(2 * e + 0) * NC + c] = make_uint4(q0.x, q0.y, q1.x, q1.y);   // [w1 of half 0 | w1 of half 1]
             w[(2 * e + 1) * NC + c] = make_uint4(q0.z, q0.w, q1.z, q1.w);   // [w2 of half 0 | w2 of half 1]
           }
@@ -467,6 +520,9 @@ void PlanConvWs(const qcnn_layer* L, int N, ConvCands* cands) {
     SetGemmGeometry(L, a);
     a.PW = PWp; a.IB = IB; a.P = P; a.NC = Kg; a.nct = 1;
     a.NPOS = RoundUp(P + ((L->ksz - 1) / st) * (PWp + 1), 8);
+    // a phase row's planes in one register pass of the producers; source offsets relative to the CTA's first image in int
+    if (st * a.NPOS > kWsRegItems1 * kWsProducers ||
+        static_cast<double>(CeilDiv(a.NPOS, IB) + 1) * L->Hin * L->Win * L->Cin > 2.0e9) continue;
     a.planeRows = (st / 2) * a.NPOS;
     a.nChunks = st; a.nPB = st;   // every phase row resident
     a.tapsPad = RoundUp(CeilDiv(L->ksz, st) * L->ksz, 16);
