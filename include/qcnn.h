@@ -275,6 +275,34 @@ QCNN_API int qcnn_multi_forward_h(qcnn_multi* m, const float* img_h, int N, floa
 QCNN_API int qcnn_multi_forward(qcnn_multi* m, const float* const* img_dev, int N, const float** prob_all_dev);
 QCNN_API int qcnn_multi_sync(qcnn_multi* m);
 
+/* ---- product quantization of dense weights (DESIGN.md 4e) ------------------------------------------------------
+ * Per subspace s of d input channels, Lloyd k-means over the weight sub-vectors, on the device; synchronous, host arrays.
+ * Points: conv p = (o k + kh) k + kw over all Cout channels (one codebook for all groups), x_p[j] = knl[o][s d + j][kh][kw];
+ * FC p = o, x_p[j] = wei[o][s d + j]; j < w_s = min(d, Cg - s d) (FC: Din), S = ceil(Cg / d).  Distances are fp32 in
+ * ascending j, the lowest index wins ties, means are fp64 sums in a fixed order, an empty cluster keeps its codeword and
+ * codebook dims j >= w_s are 0.  a_0 = assign(C_0); then iters x (update, assign): every returned index is the nearest
+ * codeword of the returned codebook.  sse_h[t] (nullable, iters + 1 values) = sum over all points and subspaces of the
+ * distance to the assigned codeword after step t.  C_0 = init_ctrd_h [S][K][d] when given, else per subspace the points
+ * perm[0..K-1] of an LCG partial shuffle: x = seed + s; for i < K: x = 1664525 x + 1013904223 (mod 2^32),
+ * j = i + (x >> 8) mod (P - i), swap(perm[i], perm[j]).  Results are bit-reproducible.  Fails on non-finite weights, K that
+ * the matching layer_create refuses (conv: multiple of 8; FC: 16, 32, 64, 128, 256), d outside 1..64, iters < 0, more than
+ * 2^24 points, or fewer points than K without an init codebook. */
+QCNN_API int qcnn_pq_quantize_conv(qcnn_ctx* ctx, int Cout, int Cg, int ksz, int K, int d, int iters, uint32_t seed,
+                                   const float* knl_h /*[Cout][Cg][k][k]*/, const float* init_ctrd_h /*nullable [S][K][d]*/,
+                                   float* ctrd_h /*[S][K][d]*/, uint8_t* asmt_h /*[Cout][k][k][S], 0-based*/,
+                                   double* sse_h /*nullable [iters+1]*/);
+QCNN_API int qcnn_pq_quantize_fc(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int iters, uint32_t seed,
+                                 const float* wei_h /*[Dout][Din]*/, const float* init_ctrd_h, float* ctrd_h,
+                                 uint8_t* asmt_h /*[Dout][S]*/, double* sse_h);
+/* model table by name (as qcnn_net_create): reads <dir>/<pfx>.{convKnl|fcntWei,biasVec}.NN.bin (CaffePara::LoadLayerPara
+ * with enblAprx = false), writes <out_dir>/<out_pfx>.{ctrdLst,biasVec}.NN.bin and .asmtLst.NN.cbn (bits of the 1-based
+ * maximum K); K[l], d[l] per layer index (ignored for non-PQ layers); layer l uses seed + 65536 (l + 1) and a random
+ * init.  Dense shapes are checked against the table; biasVec is copied unchanged; no file is written unless every
+ * layer is quantized, and none is left behind by a failed write. */
+QCNN_API int qcnn_pq_quantize_model(qcnn_ctx* ctx, const char* model_name, const char* dir, const char* pfx,
+                                    const int* K, const int* d, int iters, uint32_t seed,
+                                    const char* out_dir, const char* out_pfx);
+
 /* ---- file formats (include/FileIO.h:56-178, 229-350), host only ------------------------------------------- */
 /* .bin: returns element count or -1; dims4 padded with 1; data_h may be NULL to query the shape */
 QCNN_API long qcnn_read_bin_f32(const char* path, int* dim_cnt, int* dims4, float* data_h, long cap);

@@ -126,6 +126,9 @@ _SIGS = {
     "qcnn_write_bin_f32": (_i, [_cp, _i, C.POINTER(_i), _vp]),
     "qcnn_read_cbn_u8": (C.c_long, [_cp, C.POINTER(_i), C.POINTER(_i), C.POINTER(_i), _vp, C.c_long]),
     "qcnn_write_cbn_u8": (_i, [_cp, _i, C.POINTER(_i), _vp, _i]),
+    "qcnn_pq_quantize_conv": (_i, [_vp] + [_i] * 6 + [C.c_uint32, _vp, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_quantize_fc": (_i, [_vp] + [_i] * 5 + [C.c_uint32, _vp, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_quantize_model": (_i, [_vp, _cp, _cp, _cp, C.POINTER(_i), C.POINTER(_i), _i, C.c_uint32, _cp, _cp]),
 }
 for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)
@@ -608,3 +611,47 @@ def write_cbn_u8(path, idx0, bits):
     idx0 = _np(idx0, np.uint8)
     dims = (_i * idx0.ndim)(*idx0.shape)
     _check(lib.qcnn_write_cbn_u8(path.encode(), idx0.ndim, dims, idx0.ctypes.data_as(_vp), bits))
+
+
+# ---- product quantization of dense weights (k-means on the device, DESIGN.md 4e) -----------------------------------
+def _pq_quantize(fn, ctx, w, shape_args, Cg, K, d, iters, seed, init, asmt_shape):
+    S = -(-Cg // d)
+    init_p = None
+    if init is not None:
+        init = _np(init, np.float32)
+        if init.shape != (S, K, d):
+            raise QcnnError("init codebook must be [%d, %d, %d], got %s" % (S, K, d, init.shape))
+        init_p = init.ctypes.data_as(_vp)
+    ctrd = np.empty((S, K, d), np.float32)
+    asmt = np.empty(asmt_shape + (S,), np.uint8)
+    sse = np.empty(max(iters, 0) + 1, np.float64)
+    _check(fn(ctx.h, *shape_args, K, d, iters, seed & 0xFFFFFFFF, w.ctypes.data_as(_vp), init_p,
+              ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp), sse.ctypes.data_as(_vp)))
+    return ctrd, asmt, sse
+
+
+def pq_quantize_conv(ctx, knl, K, d, iters=20, seed=0, init=None):
+    """k-means PQ of conv weights knl [Cout, Cg, k, k]: (ctrd [S, K, d], asmt [Cout, k, k, S] 0-based, sse [iters + 1])."""
+    knl = _np(knl, np.float32)
+    Cout, Cg, k, k2 = knl.shape
+    assert k == k2, knl.shape
+    return _pq_quantize(lib.qcnn_pq_quantize_conv, ctx, knl, (Cout, Cg, k), Cg, K, d, iters, seed, init, (Cout, k, k))
+
+
+def pq_quantize_fc(ctx, wei, K, d, iters=20, seed=0, init=None):
+    """k-means PQ of FC weights wei [Dout, Din]: (ctrd [S, K, d], asmt [Dout, S] 0-based, sse [iters + 1])."""
+    wei = _np(wei, np.float32)
+    Dout, Din = wei.shape
+    return _pq_quantize(lib.qcnn_pq_quantize_fc, ctx, wei, (Din, Dout), Din, K, d, iters, seed, init, (Dout,))
+
+
+def pq_quantize_model(ctx, model, dir, pfx, out_dir, out_pfx, pq, iters=20, seed=0):
+    """Dense <dir>/<pfx>.{convKnl|fcntWei,biasVec}.NN.bin of a model table -> PQ files under <out_dir>/<out_pfx>;
+    pq = {layerInd: (K, d)} for every conv / FC layer (layer l is seeded with seed + 65536 (l + 1))."""
+    n = max(pq) + 1 if pq else 0
+    n = max(n, 256)   # one entry per layer index of the table: unlisted layers are 0, which the call rejects
+    Ks, ds = (_i * n)(), (_i * n)()
+    for l, (K, d) in pq.items():
+        Ks[l], ds[l] = K, d
+    _check(lib.qcnn_pq_quantize_model(ctx.h, model.encode(), dir.encode(), pfx.encode(), Ks, ds, iters,
+                                      seed & 0xFFFFFFFF, out_dir.encode(), out_pfx.encode()))

@@ -12,6 +12,8 @@
 
 #include "../../include/qcnn.h"
 
+class CaffePara;
+
 namespace qcnn {
 
 // thread-local error text behind qcnn_last_error()
@@ -476,6 +478,12 @@ int LaunchNhwcToNchw(qcnn_ctx* ctx, const float* src, float* dst, int N, int H, 
 // preproc.cu
 int LaunchU8ToF32(qcnn_ctx* ctx, const uint8_t* src, const float* mean, float* dst, int N, int C, int HW, cudaStream_t st);
 int LaunchTopK(qcnn_ctx* ctx, const float* prob, int N, int C, int k, int mode, int* idx, float* val, cudaStream_t st);
+
+// qcnn_net.cu: a CaffePara layer table as C-ABI records, and the NHWC input dims of every layer of a table (entry
+// layerCnt: the output) -- the one shape walk of the executor and of qcnn_pq_quantize_model
+struct LayerDims { int H, W, C; };
+std::vector<qcnn_layer_info> LayerInfos(const CaffePara& para);
+std::vector<LayerDims> LayerInputDims(const std::vector<qcnn_layer_info>& infos, int imgC, int imgH, int imgW);
 
 inline int PoolOut(int in, int pad, int ksz, int stride) {
   // ceil((in + 2p - k) / s) + 1   (reference src/CaffeEva.cc:365-372)

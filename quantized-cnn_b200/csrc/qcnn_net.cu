@@ -80,12 +80,57 @@ static float* MapBuf(qcnn_net* net, int idx, int N, cudaStream_t st) {
   return net->maps[idx].as<float>();
 }
 
+namespace qcnn {
+
+std::vector<LayerDims> LayerInputDims(const std::vector<qcnn_layer_info>& infos, int imgC, int imgH, int imgW) {
+  std::vector<LayerDims> dims(infos.size() + 1);
+  int H = imgH, W = imgW, C = imgC;
+  for (size_t l = 0; l < infos.size(); l++) {
+    const qcnn_layer_info& li = infos[l];
+    dims[l] = {H, W, C};
+    switch (li.type) {
+      case QCNN_CONV: {
+        const int stride = std::max(li.stride, 1);   // qcnn_conv_layer_create refuses a stride < 1
+        H = (H + 2 * li.padSiz - li.knlSiz) / stride + 1;  // reference CaffeEva.cc:361-362
+        W = (W + 2 * li.padSiz - li.knlSiz) / stride + 1;
+        C = li.knlCnt;
+        break;
+      }
+      case QCNN_FCNT:
+        H = 1; W = 1; C = li.nodCnt;
+        break;
+      case QCNN_POOL:
+        H = PoolOut(H, li.padSiz, li.knlSiz, li.stride);
+        W = PoolOut(W, li.padSiz, li.knlSiz, li.stride);
+        break;
+      default:
+        break;
+    }
+  }
+  dims[infos.size()] = {H, W, C};
+  return dims;
+}
+
+std::vector<qcnn_layer_info> LayerInfos(const CaffePara& para) {
+  std::vector<qcnn_layer_info> infos(para.layerCnt);
+  for (int l = 0; l < para.layerCnt; l++) {
+    const LayerInfo& li = para.layerInfoLst[l];
+    qcnn_layer_info& o = infos[l];
+    o.type = static_cast<int>(li.type);
+    o.padSiz = li.padSiz; o.knlSiz = li.knlSiz; o.knlCnt = li.knlCnt; o.grpCnt = li.grpCnt; o.stride = li.stride;
+    o.nodCnt = li.nodCnt; o.lrnSiz = li.lrnSiz; o.lrnAlp = li.lrnAlp; o.lrnBet = li.lrnBet; o.lrnIni = li.lrnIni; o.drpRat = li.drpRat;
+  }
+  return infos;
+}
+
+}  // namespace qcnn
+
 static int BuildNet(qcnn_ctx* ctx, int layerCnt, const qcnn_layer_info* infos, const qcnn_layer_para* paras, int imgC, int imgH,
                     int imgW, qcnn_net** out) {
   qcnn_net* net = new qcnn_net();
   net->ctx = ctx;
   net->imgC = imgC; net->imgH = imgH; net->imgW = imgW;
-  int H = imgH, W = imgW, C = imgC;
+  const std::vector<LayerDims> dims = LayerInputDims(std::vector<qcnn_layer_info>(infos, infos + layerCnt), imgC, imgH, imgW);
   bool seenFc = false;
   int rc = 0;
   for (int l = 0; l < layerCnt && rc == 0; l++) {
@@ -93,6 +138,7 @@ static int BuildNet(qcnn_ctx* ctx, int layerCnt, const qcnn_layer_info* infos, c
     memset(&nl, 0, sizeof(nl));
     nl.info = infos[l];
     const qcnn_layer_info& li = nl.info;
+    const int H = dims[l].H, W = dims[l].W, C = dims[l].C;
     nl.Hin = H; nl.Win = W; nl.Cin = C;
     const qcnn_layer_para& lp = paras[l];
     switch (li.type) {
@@ -104,8 +150,6 @@ static int BuildNet(qcnn_ctx* ctx, int layerCnt, const qcnn_layer_info* infos, c
         }
         rc = qcnn_conv_layer_create(ctx, C, H, W, li.knlCnt, li.knlSiz, li.padSiz, li.stride, li.grpCnt, lp.S, lp.K, lp.d,
                                     lp.ctrd, lp.asmt, lp.bias, &nl.pq);
-        if (rc) break;
-        H = nl.pq->Ho; W = nl.pq->Wo; C = li.knlCnt;
         break;
       }
       case QCNN_FCNT: {
@@ -121,17 +165,12 @@ static int BuildNet(qcnn_ctx* ctx, int layerCnt, const qcnn_layer_info* infos, c
         // first FC layer: the reference permutes its NHWC input to NCHW first (CaffeEva.cc:236-238)
         if (!seenFc && (H > 1 || W > 1)) rc = qcnn_fc_layer_set_src_nhwc(nl.pq, H, W, C);
         seenFc = true;
-        H = 1; W = 1; C = li.nodCnt;
         break;
       }
-      case QCNN_POOL:
-        H = PoolOut(H, li.padSiz, li.knlSiz, li.stride);
-        W = PoolOut(W, li.padSiz, li.knlSiz, li.stride);
-        break;
       default:
         break;
     }
-    nl.Hout = H; nl.Wout = W; nl.Cout = C;
+    nl.Hout = dims[l + 1].H; nl.Wout = dims[l + 1].W; nl.Cout = dims[l + 1].C;
     net->layers.push_back(nl);
   }
   if (rc) {
@@ -156,14 +195,10 @@ static int BuildNet(qcnn_ctx* ctx, int layerCnt, const qcnn_layer_info* infos, c
 
 // parameters loaded from files: shape checks against the layer table, then the common builder
 static int BuildFromCaffePara(qcnn_ctx* ctx, CaffePara& para, qcnn_net** out) {
-  std::vector<qcnn_layer_info> infos(para.layerCnt);
+  const std::vector<qcnn_layer_info> infos = LayerInfos(para);
   std::vector<qcnn_layer_para> paras(para.layerCnt);
   for (int l = 0; l < para.layerCnt; l++) {
     const LayerInfo& li = para.layerInfoLst[l];
-    qcnn_layer_info& o = infos[l];
-    o.type = static_cast<int>(li.type);
-    o.padSiz = li.padSiz; o.knlSiz = li.knlSiz; o.knlCnt = li.knlCnt; o.grpCnt = li.grpCnt; o.stride = li.stride;
-    o.nodCnt = li.nodCnt; o.lrnSiz = li.lrnSiz; o.lrnAlp = li.lrnAlp; o.lrnBet = li.lrnBet; o.lrnIni = li.lrnIni; o.drpRat = li.drpRat;
     memset(&paras[l], 0, sizeof(qcnn_layer_para));
     if (li.type != ENUM_LyrType::Conv && li.type != ENUM_LyrType::FCnt) continue;
     const LayerPara& lp = para.layerParaLst[l];

@@ -52,6 +52,8 @@ class CaffePara {
   bool ConfigLayer_ByName(const std::string& modelName);
   bool LoadLayerPara(const bool enblAprx, const ENUM_AsmtEnc asmtEnc);
   bool CvtAsmtEnc(const ENUM_AsmtEnc asmtEncSrc, const ENUM_AsmtEnc asmtEncDst);
+  // <dirPath>/<filePfx>.<kind>.NN.<ext>, NN = layerInd + 1 (reference src/CaffePara.cc:262-281)
+  std::string ParaPath(const char* kind, int layerInd, const char* ext) const;
 
  public:
   std::string dirPath;
@@ -65,7 +67,6 @@ class CaffePara {
 
  private:
   int CalcBitCntPerEle(const Matrix<uint8_t>& asmtLst);
-  std::string ParaPath(const char* kind, int layerInd, const char* ext) const;
 };
 
 #endif  // QCNN_HOST_CAFFEPARA_H_
