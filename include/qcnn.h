@@ -82,7 +82,11 @@ QCNN_API int qcnn_conv_layer_set_src_nchw(qcnn_layer* layer, int enable);
  * channels per group, with bf16x2 operands (tensor_core = 2), as a weight-stationary GEMM whose N is the channels of one
  * CTA: Cout/grp or a tile of it, in {16, 32, 64, 96, 128, 192, 256}; describe() names it pq_gemm_tc_ws), "gemm_nt" (positions per CTA of the pq_gemm_tc tilings, and 128 / 256 for conv_ws; 0 = any), "gemm_gt"
  * (k-steps per stage of those tilings, 0 = any), "gemm_nsplit" (their K-split factor, 0 = any), "gemm_ct" (channels per
- * CTA of the conv_ws tilings, 0 = any; a pin that no tiling of the layer matches makes the forward fail), "autotune"
+ * CTA of the conv_ws tilings, 0 = any; a pin that no tiling of the layer matches makes the forward fail), "lut_cpt",
+ * "lut_j", "lut_nct", "lut_r", "lut_rgroups" (the LUT + gather tilings, force_kernel 0-4, with that many channels per
+ * thread, positions per lane -- conv_direct: output rows per thread --, channel tiles per group, output rows per strip --
+ * conv_direct: after its clamp to Ho + (Ho & 1) -- and row groups; 0 = any; a pin that no tiling matches makes the
+ * forward fail; describe() prints them as CPT, J, nct, R, rgroups), "autotune"
  * (0 = keep the cost model's first tiling instead of timing the candidates of the chosen family on the device);
  * FC layers only: "fc_ws" (1 = at N >= 96 with bf16x2 operands, run the layer as a weight-stationary
  * GEMM, describe() "pq_gemm_tc_ws(...) mode=2"; 0 = pq_gemm_tc mode 2, the default of a standalone layer; the network

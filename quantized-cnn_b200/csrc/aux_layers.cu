@@ -357,10 +357,13 @@ int LaunchLrn(qcnn_ctx* ctx, const float* src, float* dst, size_t pixels, int C,
 int LaunchMaxPool(qcnn_ctx* ctx, const float* src, float* dst, int N, int H, int W, int C, int ksz, int pad,
                   int stride, cudaStream_t st) {
   QCNN_CHECK(N >= 1 && ksz >= 1 && stride >= 1, "qcnn_maxpool: bad arguments");
+  QCNN_CHECK(PoolWindowsNonEmpty(H, pad, ksz, stride) && PoolWindowsNonEmpty(W, pad, ksz, stride),
+             "qcnn_maxpool: %dx%d map, %dx%d window, pad %d, stride %d: an output window holds no input pixel", H, W, ksz,
+             ksz, pad, stride);
   const int Ho = PoolOut(H, pad, ksz, stride), Wo = PoolOut(W, pad, ksz, stride);
   const size_t total = static_cast<size_t>(N) * Ho * Wo * C;
   // (fmaxf of a window that contains a NaN: both kernels return the maximum of the other taps, in any order)
-  if ((C & 3) == 0 && Ho >= 1 && Wo >= 1) {
+  if ((C & 3) == 0) {
     const size_t total4 = total / 4;
     if (ksz == 3 && stride <= 3 && pad <= 2) maxpool4_kernel<true><<<GridFor(ctx, total4), kThreads, 0, st>>>(reinterpret_cast<const float4*>(src), reinterpret_cast<float4*>(dst), N, H, W, C / 4, Ho, Wo, ksz, pad, stride);
     else maxpool4_kernel<false><<<GridFor(ctx, total4), kThreads, 0, st>>>(reinterpret_cast<const float4*>(src), reinterpret_cast<float4*>(dst), N, H, W, C / 4, Ho, Wo, ksz, pad, stride);
@@ -375,6 +378,9 @@ int LaunchMaxPool(qcnn_ctx* ctx, const float* src, float* dst, int N, int H, int
 int LaunchLrnMaxPool(qcnn_ctx* ctx, const float* src, float* dst, int N, int H, int W, int C, int size, float alpha,
                      float beta, float k, int ksz, int pad, int stride, cudaStream_t st) {
   QCNN_CHECK(N >= 1 && ksz >= 1 && stride >= 1 && size >= 1, "qcnn_lrn_maxpool: bad arguments");
+  QCNN_CHECK(PoolWindowsNonEmpty(H, pad, ksz, stride) && PoolWindowsNonEmpty(W, pad, ksz, stride),
+             "qcnn_lrn_maxpool: %dx%d map, %dx%d window, pad %d, stride %d: an output window holds no input pixel", H, W,
+             ksz, ksz, pad, stride);
   const int Ho = PoolOut(H, pad, ksz, stride), Wo = PoolOut(W, pad, ksz, stride);
   const size_t total = static_cast<size_t>(N) * Ho * Wo * C;
   // output rows per CTA: as many as keep two CTAs per SM (less re-normalisation of shared input rows)

@@ -977,7 +977,7 @@ void PlanLutGather(const qcnn_layer* L, int N, ConvCands* cands) {
             ConvArgs& a = p.a;
             p.kernel = kConvDirect; p.CPT = CPT; p.J = rowsPer;
             a.R = std::min(R, L->Ho + (L->Ho & 1)); a.nstrips = CeilDiv(L->Ho, a.R);
-            a.CT = CT; a.nct = nct; a.cwarps = cwarps; a.pwarps = 1; a.rgroups = rgroups;
+            a.CT = CT; a.nct = nct; a.cwarps = cwarps; a.pwarps = 1; a.rgroups = rgroups; a.ncol = 1; a.CW = L->Wo;
             a.PW = CeilDiv(L->Win + 2 * L->pad, L->stride);       // phase length
             a.PP = RoundUp(a.PW * L->stride, 4);                   // row pitch
             p.threads = 32 * cwarps * rgroups;
@@ -1032,9 +1032,9 @@ int LaunchLutGather(qcnn_layer* L, const ConvPlan& p, const float* src, int N, f
 }
 
 void DescribeLutGather(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap) {
-  snprintf(buf, cap, " CPT=%d J=%d threads=%d smem=%zuB grid=(%d,%d) R=%d strips=%d CT=%d nct=%d PP=%d pwarps=%d "
-           "cwarps=%d rgroups=%d", p.CPT, p.J, p.threads, p.smem, p.a.G * p.a.nct * p.a.nstrips, N, p.a.R, p.a.nstrips,
-           p.a.CT, p.a.nct, p.a.PP, p.a.pwarps, p.a.cwarps, p.a.rgroups);
+  snprintf(buf, cap, " CPT=%d J=%d threads=%d smem=%zuB grid=(%d,%d) R=%d strips=%d ncol=%d CW=%d CT=%d nct=%d PP=%d "
+           "pwarps=%d cwarps=%d rgroups=%d", p.CPT, p.J, p.threads, p.smem, p.a.G * p.a.nct * p.a.nstrips, N, p.a.R,
+           p.a.nstrips, p.a.ncol, p.a.CW, p.a.CT, p.a.nct, p.a.PP, p.a.pwarps, p.a.cwarps, p.a.rgroups);
 }
 
 }  // namespace qcnn

@@ -89,6 +89,19 @@ int PlanConv(qcnn_layer* L, int N) {
     QCNN_CHECK(!cands.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d gemm_gt=%d gemm_nsplit=%d gemm_ct=%d has no tiling for "
                "this layer at batch %d", L->opt_gemm_nt, L->opt_gemm_gt, L->opt_gemm_nsplit, L->opt_gemm_ct, N);
   }
+  // layer parameters "lut_cpt" / "lut_j" / "lut_nct" / "lut_r" / "lut_rgroups": only LUT + gather tilings (kernels 0-4) with
+  // that key entry (0 = any): channels per thread, positions per lane (conv_direct: output rows per thread), channel tiles
+  // per group, output rows per strip (conv_direct: after its clamp), row groups.  Tests pin the tiling they check.
+  if (L->opt_lut_cpt || L->opt_lut_j || L->opt_lut_nct || L->opt_lut_r || L->opt_lut_rgroups) {
+    keepIf([L](const ConvPlan& c) {
+      if (c.kernel > kConvDirect) return true;
+      return (!L->opt_lut_cpt || c.key[0] == L->opt_lut_cpt) && (!L->opt_lut_j || c.key[1] == L->opt_lut_j) &&
+             (!L->opt_lut_nct || c.key[2] == L->opt_lut_nct) && (!L->opt_lut_r || c.key[5] == L->opt_lut_r) &&
+             (!L->opt_lut_rgroups || c.key[4] == L->opt_lut_rgroups);
+    });
+    QCNN_CHECK(!cands.empty(), "qcnn_conv_aprx_forward: lut_cpt=%d lut_j=%d lut_nct=%d lut_r=%d lut_rgroups=%d has no tiling "
+               "for this layer at batch %d", L->opt_lut_cpt, L->opt_lut_j, L->opt_lut_nct, L->opt_lut_r, L->opt_lut_rgroups, N);
+  }
   L->cands.clear();
   for (int pass = 0; pass < 2; pass++) {
     int perKernel[kConvKernelIds] = {};

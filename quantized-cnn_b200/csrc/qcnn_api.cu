@@ -352,6 +352,21 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
     L->plan_N = 0; L->tuned = 0;
     L->tunedPlans.clear();
   }
+  else if (!strcmp(name, "lut_cpt") || !strcmp(name, "lut_j") || !strcmp(name, "lut_nct") || !strcmp(name, "lut_r") ||
+           !strcmp(name, "lut_rgroups")) {
+    // conv only, 0 = any: the LUT + gather tilings (force_kernel 0-4) with that many channels per thread, positions per
+    // lane (conv_direct: output rows per thread), channel tiles per group, output rows per strip (conv_direct: the value
+    // after its clamp to Ho + (Ho & 1)) and row groups.  A pin that no tiling of the layer matches fails the forward.
+    QCNN_CHECK(L->kind == QCNN_KIND_CONV, "qcnn_layer_set_param: '%s' applies to conv layers", name);
+    const int v = value < 0 ? 0 : value;
+    if (!strcmp(name, "lut_cpt")) L->opt_lut_cpt = v;
+    else if (!strcmp(name, "lut_j")) L->opt_lut_j = v;
+    else if (!strcmp(name, "lut_nct")) L->opt_lut_nct = v;
+    else if (!strcmp(name, "lut_r")) L->opt_lut_r = v;
+    else L->opt_lut_rgroups = v;
+    L->plan_N = 0; L->tuned = 0;
+    L->tunedPlans.clear();
+  }
   else if (!strcmp(name, "force_kernel") || !strcmp(name, "autotune")) {
     // conv only.  force_kernel: -1 none, else 0 s1 | 1 roll | 2 s1_tc | 3 roll_tc | 4 direct | 6 pq_gemm_tc | 7 conv_ws;
     // autotune: 0 keeps the cost model's first tiling instead of timing the candidates on the device

@@ -332,7 +332,12 @@ struct qcnn_layer {
   int opt_gemm_nsplit = 0;   // conv: ... to this K-split factor (0 = any)
   int opt_gemm_ct = 0;       // conv: restrict conv_ws tilings to this many channels per CTA (0 = any)
                              // (FC with fc_ws: gemm_nt / gemm_gt / gemm_ct / gemm_nsplit restrict the fc_ws tilings)
-  int opt_fc_ws = 0;         // FC: 1 = the batched tensor-core path runs as the weight-stationary GEMM (fc_ws.cu) where
+  int opt_lut_cpt = 0;       // conv: restrict LUT + gather tilings (kernels 0-4) to this ConvPlan::key[0] (CPT) (0 = any)
+  int opt_lut_j = 0;         // ... key[1]: positions per lane (conv_direct: output rows per thread)
+  int opt_lut_nct = 0;       // ... key[2]: channel tiles per group
+  int opt_lut_r = 0;         // ... key[5]: output rows per strip (conv_direct: after its clamp to Ho + (Ho & 1))
+  int opt_lut_rgroups = 0;   // ... key[4]: row groups
+  int opt_fc_ws = 0;        // FC: 1 = the batched tensor-core path runs as the weight-stationary GEMM (fc_ws.cu) where
                              // it can, instead of pq_gemm_tc mode 2 (the network executor sets it on every FC layer)
 };
 
@@ -490,6 +495,13 @@ inline int PoolOut(int in, int pad, int ksz, int stride) {
   int num = in + 2 * pad - ksz;
   int q = num >= 0 ? (num + stride - 1) / stride : -((-num) / stride);
   return q + 1;
+}
+// The windows of a pooling layer are clipped to the map, not padded, so each must hold at least one input pixel: the
+// first needs pad < ksz, the last (out - 1) * stride - pad < in.  (An empty window has no defined output: the reference
+// leaves it unwritten.)  ksz, stride >= 1.
+inline bool PoolWindowsNonEmpty(int in, int pad, int ksz, int stride) {
+  const int out = PoolOut(in, pad, ksz, stride);
+  return in >= 1 && pad >= 0 && pad < ksz && out >= 1 && (out - 1) * stride - pad < in;
 }
 
 }  // namespace qcnn

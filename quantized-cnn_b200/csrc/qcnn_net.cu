@@ -99,10 +99,12 @@ std::vector<LayerDims> LayerInputDims(const std::vector<qcnn_layer_info>& infos,
       case QCNN_FCNT:
         H = 1; W = 1; C = li.nodCnt;
         break;
-      case QCNN_POOL:
-        H = PoolOut(H, li.padSiz, li.knlSiz, li.stride);
-        W = PoolOut(W, li.padSiz, li.knlSiz, li.stride);
+      case QCNN_POOL: {
+        const int stride = std::max(li.stride, 1);   // BuildNet refuses a stride < 1
+        H = PoolOut(H, li.padSiz, li.knlSiz, stride);
+        W = PoolOut(W, li.padSiz, li.knlSiz, stride);
         break;
+      }
       default:
         break;
     }
@@ -167,6 +169,14 @@ static int BuildNet(qcnn_ctx* ctx, int layerCnt, const qcnn_layer_info* infos, c
         seenFc = true;
         break;
       }
+      case QCNN_POOL:
+        if (li.knlSiz < 1 || li.stride < 1 || !PoolWindowsNonEmpty(H, li.padSiz, li.knlSiz, li.stride) ||
+            !PoolWindowsNonEmpty(W, li.padSiz, li.knlSiz, li.stride)) {
+          SetError("layer %d: pooling a %dx%d map with a %dx%d window, pad %d, stride %d leaves an output window without "
+                   "input pixels", l + 1, H, W, li.knlSiz, li.knlSiz, li.padSiz, li.stride);
+          rc = 1;
+        }
+        break;
       default:
         break;
     }
