@@ -306,6 +306,23 @@ QCNN_API int qcnn_pq_quantize_fc(qcnn_ctx* ctx, int Din, int Dout, int K, int d,
 QCNN_API int qcnn_pq_quantize_model(qcnn_ctx* ctx, const char* model_name, const char* dir, const char* pfx,
                                     const int* K, const int* d, int iters, uint32_t seed,
                                     const char* out_dir, const char* out_pfx);
+/* Error-correcting PQ of an FC layer (DESIGN.md 4e): block coordinate descent on (ctrd, asmt) that lowers
+ * loss = sum_n |(W - W^) x_n|^2 = sum_o E_o^T G E_o, E = W - W^ (fp64), G = X^T X (fp64, fixed order), on the inputs
+ * x [N][Din] (device, fcntWei column order).  A sweep visits m = 0..S-1 in order; subspace m (dims m d .. m d + w_m - 1)
+ * is skipped when tr(G_mm) = 0, else with h_o = [G E_o]_m + G_mm w^_o:  for every non-empty cluster k,
+ * D = fp32((G_mm + lambda I)^-1 H_k / n_k) by Cholesky (H_k = sum of h_o over the cluster, lambda = 1e-10 tr(G_mm) / w_m)
+ * replaces c_k only if f(D) < f(c_k), f(D) = n_k D^T G_mm D - 2 D^T H_k; then a_o = argmin_k c_k^T G_mm c_k - 2 c_k^T h_o
+ * (lowest index on ties), and E is updated before m + 1.  ctrd_h [S][K][d] and asmt_h [Dout][S] (0-based) are the start
+ * and receive the result; loss_h (nullable, sweeps + 1 values) = the start's loss, then the loss after each sweep.
+ * Results are bit-reproducible.  Runs on `stream` (ordered after whatever produced x) and synchronises it before
+ * returning.  Device memory: 8 Din^2 bytes for G plus about 20 Dout Din bytes (E and G E^T in fp64, the weights in
+ * fp32).  Fails on what
+ * qcnn_pq_quantize_fc refuses (K, d, non-finite weights or codebook), sweeps < 0, N < 1, an assignment >= K, non-finite
+ * x, or a failed allocation (with its byte count). */
+QCNN_API int qcnn_pq_refine_fc(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps,
+                               const float* wei_h /*[Dout][Din]*/, const float* x /*device [N][Din]*/, int N,
+                               float* ctrd_h /*in/out [S][K][d]*/, uint8_t* asmt_h /*in/out [Dout][S], 0-based*/,
+                               double* loss_h /*nullable [sweeps + 1]*/, void* stream);
 
 /* ---- file formats (include/FileIO.h:56-178, 229-350), host only ------------------------------------------- */
 /* .bin: returns element count or -1; dims4 padded with 1; data_h may be NULL to query the shape */

@@ -129,6 +129,7 @@ _SIGS = {
     "qcnn_pq_quantize_conv": (_i, [_vp] + [_i] * 6 + [C.c_uint32, _vp, _vp, _vp, _vp, _vp]),
     "qcnn_pq_quantize_fc": (_i, [_vp] + [_i] * 5 + [C.c_uint32, _vp, _vp, _vp, _vp, _vp]),
     "qcnn_pq_quantize_model": (_i, [_vp, _cp, _cp, _cp, C.POINTER(_i), C.POINTER(_i), _i, C.c_uint32, _cp, _cp]),
+    "qcnn_pq_refine_fc": (_i, [_vp] + [_i] * 5 + [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
 }
 for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)
@@ -655,3 +656,24 @@ def pq_quantize_model(ctx, model, dir, pfx, out_dir, out_pfx, pq, iters=20, seed
         Ks[l], ds[l] = K, d
     _check(lib.qcnn_pq_quantize_model(ctx.h, model.encode(), dir.encode(), pfx.encode(), Ks, ds, iters,
                                       seed & 0xFFFFFFFF, out_dir.encode(), out_pfx.encode()))
+
+
+def pq_refine_fc(ctx, wei, x, ctrd, asmt, sweeps=8, stream=None):
+    """Error-correcting PQ of FC weights wei [Dout, Din] on layer inputs x (contiguous float32 CUDA tensor [N, Din],
+    fcntWei column order), starting from (ctrd [S, K, d], asmt [Dout, S] 0-based), e.g. pq_quantize_fc's output:
+    (ctrd, asmt, loss [sweeps + 1]) with loss[t] = sum_n |(W - W^) x_n|^2 after sweep t.  The arguments are not modified."""
+    wei = _np(wei, np.float32)
+    Dout, Din = wei.shape
+    ctrd = np.array(ctrd, np.float32, order="C", copy=True)
+    asmt = np.array(asmt, np.uint8, order="C", copy=True)
+    S, K, d = ctrd.shape
+    if S != -(-Din // d) or asmt.shape != (Dout, S):
+        raise QcnnError("ctrd [%d, K, d] and asmt [%d, %d] do not match a [%d, %d] layer with d=%d"
+                        % (S, Dout, S, Dout, Din, d))
+    if x.dim() != 2 or x.shape[1] != Din:
+        raise QcnnError("x must be [N, %d], got %s" % (Din, tuple(x.shape)))
+    loss = np.empty(max(sweeps, 0) + 1, np.float64)
+    _check(lib.qcnn_pq_refine_fc(ctx.h, Din, Dout, K, d, sweeps, wei.ctypes.data_as(_vp), _dptr(x), x.shape[0],
+                                 ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp),
+                                 _stream(stream)))
+    return ctrd, asmt, loss

@@ -339,11 +339,6 @@ int CheckConvK(const char* who, int K) {
   QCNN_CHECK(K >= 8 && K <= kMaxK && K % 8 == 0, "%s: K=%d must be a multiple of 8 in 8..%d", who, K, kMaxK);
   return 0;
 }
-int CheckFcK(const char* who, int K) {
-  QCNN_CHECK(K == 16 || K == 32 || K == 64 || K == 128 || K == 256, "%s: unsupported codebook size K=%d (supported: 16, 32, 64, 128, 256)",
-             who, K);
-  return 0;
-}
 
 struct QuantizedLayer {
   int l;
@@ -371,6 +366,12 @@ bool WriteFile(const std::string& path, const std::vector<char>& buf) {
 }
 
 }  // namespace
+
+int qcnn::CheckFcK(const char* who, int K) {
+  QCNN_CHECK(K == 16 || K == 32 || K == 64 || K == 128 || K == 256, "%s: unsupported codebook size K=%d (supported: 16, 32, 64, 128, 256)",
+             who, K);
+  return 0;
+}
 
 extern "C" {
 

@@ -1,0 +1,526 @@
+// Error-correcting product quantization of FC layers on the device: block coordinate descent on the codebook and the
+// assignments so that the layer's response W x is kept on given inputs (the paper's quantization with error correction).
+// Semantics, normative (DESIGN.md 4e):
+//   G = X^T X (fp64, fixed order), E = W - W^ (fp64), loss = sum_o E_o^T G E_o = sum_n |(W - W^) x_n|^2.
+//   A sweep visits subspaces m = 0..S-1 in order (Gauss-Seidel); a subspace with tr(G_mm) = 0 is skipped.
+//   h_o = [G E_o]_m + G_mm w^_o(m); H_k = sum_{a_o = k} h_o (fixed order), n_k = |{o : a_o = k}|.
+//   codebook   D = (G_mm + lambda I)^-1 H_k / n_k by the Cholesky factor, lambda = 1e-10 tr(G_mm) / w_m, rounded to fp32;
+//              D replaces c_k only if f(D) < f(c_k), f(D) = n_k D^T G_mm D - 2 D^T H_k; empty clusters keep their codeword.
+//   assign     a_o = argmin_k c_k^T G_mm c_k - 2 c_k^T h_o (fp64, new codewords), the lowest index wins ties.
+// No floating-point atomics: two calls return identical bits.
+//
+// Cost structure: G, the initial G E^T and the update of G E^T after every block of subspaces are fp64 tensor-core GEMMs
+// (DMMA m16n8k16).  Inside a block, every per-subspace step runs in one cooperative launch with two grid-wide barriers
+// per subspace (codebook step, then assignment step); a CTA owns a fixed set of outputs for the whole block, so the
+// per-output work needs no grid barrier.
+#include <cooperative_groups.h>
+#include <math.h>
+
+#include <algorithm>
+#include <vector>
+
+#include "qcnn_internal.h"
+
+using namespace qcnn;
+namespace cg = cooperative_groups;
+
+namespace {
+
+constexpr int kMaxD = 64;
+constexpr int kTile = 64;            // GEMM output tile (kTile x kTile per CTA, 2 x 2 warps of 32 x 32)
+constexpr int kKStep = 16;           // the DMMA's k
+constexpr int kLd = kTile + 4;       // smem row pitch in doubles: fragment reads hit 16 distinct 8-byte bank pairs
+constexpr int kGemmThreads = 128;
+constexpr int kSweepThreads = 256;
+constexpr int kBlockDims = 256;      // dims per block of subspaces (a multiple of d): the K of the trailing GEMM
+constexpr int kLossBlocks = 512;     // fixed, so the loss reduction order does not depend on the device
+
+__device__ __forceinline__ void Dmma(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+      "{%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]),
+        "d"(b[2]), "d"(b[3]));
+}
+
+// fp64 tensor-core GEMM, one kTile x kTile output tile per CTA, k in ascending steps of 16 (a fixed order per element).
+//   kGram:  C = X^T X for X = A [Kd][lda] fp32 (M = N = the column count): lower-triangle tiles only (blockIdx.x is the
+//           linear lower-triangle index); each element with row >= col is written to both (row, col) and (col, row), so
+//           G is exactly symmetric.
+//   else:   C [M][N] = (accumulate ? C : 0) + A [M][Kd] B [Kd][N], all fp64.
+// Operands are staged through registers (the next k-step is loaded while the current one is multiplied), widened to
+// fp64 and stored k-major, [16][kLd], in shared memory.
+template <bool kGram>
+__global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __restrict__ Ap, int lda, const void* __restrict__ Bp,
+                                                                int ldb, double* __restrict__ C, int ldc, int M, int N, int Kd,
+                                                                int accumulate) {
+  __shared__ double As[2][kKStep][kLd], Bs[2][kKStep][kLd];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int g = lane >> 2, t = lane & 3, wm = warp >> 1, wn = warp & 1;
+  int tm, tn;
+  if (kGram) {
+    const int i = blockIdx.x;
+    tm = static_cast<int>((sqrt(8.0 * i + 1.0) - 1.0) * 0.5);
+    while (tm * (tm + 1) / 2 > i) tm--;
+    while ((tm + 1) * (tm + 2) / 2 <= i) tm++;
+    tn = i - tm * (tm + 1) / 2;
+  } else {
+    tm = blockIdx.y;
+    tn = blockIdx.x;
+  }
+  const int m0 = tm * kTile, n0 = tn * kTile;
+  constexpr int kPer = kKStep * kTile / kGemmThreads;   // 8 elements of each operand per thread and k-step
+  double ra[kPer], rb[kPer];
+  auto load = [&](int k0) {
+#pragma unroll
+    for (int r = 0; r < kPer; r++) {
+      const int e = tid + r * kGemmThreads;
+      const int kk = e / kTile, nn = e % kTile;   // B (and the Gram's A): row kk of the k-step, column nn
+      const int k = k0 + kk;
+      if (kGram) {
+        const float* X = static_cast<const float*>(Ap);
+        ra[r] = (k < Kd && m0 + nn < M) ? static_cast<double>(X[static_cast<size_t>(k) * lda + m0 + nn]) : 0.0;
+        rb[r] = (k < Kd && n0 + nn < N) ? static_cast<double>(X[static_cast<size_t>(k) * lda + n0 + nn]) : 0.0;
+      } else {
+        const double* A = static_cast<const double*>(Ap);
+        const double* B = static_cast<const double*>(Bp);
+        const int mm = e / kKStep, ka = k0 + e % kKStep;   // A: row mm, k-column ka (rows of A are contiguous in k)
+        ra[r] = (ka < Kd && m0 + mm < M) ? A[static_cast<size_t>(m0 + mm) * lda + ka] : 0.0;
+        rb[r] = (k < Kd && n0 + nn < N) ? B[static_cast<size_t>(k) * ldb + n0 + nn] : 0.0;
+      }
+    }
+  };
+  auto store = [&](int buf) {
+#pragma unroll
+    for (int r = 0; r < kPer; r++) {
+      const int e = tid + r * kGemmThreads;
+      if (kGram) As[buf][e / kTile][e % kTile] = ra[r];
+      else As[buf][e % kKStep][e / kKStep] = ra[r];
+      Bs[buf][e / kTile][e % kTile] = rb[r];
+    }
+  };
+  double acc[2][4][4];
+#pragma unroll
+  for (int a = 0; a < 2; a++)
+#pragma unroll
+    for (int b = 0; b < 4; b++)
+#pragma unroll
+      for (int c = 0; c < 4; c++) acc[a][b][c] = 0.0;
+  const int nk = (Kd + kKStep - 1) / kKStep;
+  load(0);
+  store(0);
+  __syncthreads();
+  for (int kt = 0; kt < nk; kt++) {
+    const int buf = kt & 1;
+    if (kt + 1 < nk) load((kt + 1) * kKStep);
+    double fa[2][8], fb[4][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+      for (int i = 0; i < 8; i++) fa[mt][i] = As[buf][t + 4 * (i >> 1)][wm * 32 + mt * 16 + g + 8 * (i & 1)];
+#pragma unroll
+    for (int nt = 0; nt < 4; nt++)
+#pragma unroll
+      for (int i = 0; i < 4; i++) fb[nt][i] = Bs[buf][t + 4 * i][wn * 32 + nt * 8 + g];
+#pragma unroll
+    for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+      for (int nt = 0; nt < 4; nt++) Dmma(acc[mt][nt], fa[mt], fb[nt]);
+    if (kt + 1 < nk) store(buf ^ 1);
+    __syncthreads();
+  }
+#pragma unroll
+  for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+    for (int nt = 0; nt < 4; nt++)
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        const int row = m0 + wm * 32 + mt * 16 + g + 8 * (i >> 1), col = n0 + wn * 32 + nt * 8 + 2 * t + (i & 1);
+        if (row >= M || col >= N) continue;
+        if (kGram) {
+          if (row < col) continue;
+          C[static_cast<size_t>(row) * ldc + col] = acc[mt][nt][i];
+          C[static_cast<size_t>(col) * ldc + row] = acc[mt][nt][i];
+        } else {
+          double* p = C + static_cast<size_t>(row) * ldc + col;
+          *p = (accumulate ? *p : 0.0) + acc[mt][nt][i];
+        }
+      }
+}
+
+// Per subspace m (blockIdx.x): the lower-triangular inverse of the Cholesky factor of G_mm + lambda I, [w][w] at row
+// pitch d.  G does not change between sweeps, so this runs once per call.  Skipped subspaces (tr(G_mm) = 0) get none.
+__global__ void __launch_bounds__(kSweepThreads) pqr_chol_kernel(const double* __restrict__ G, double* __restrict__ Linv, int Din,
+                                                                 int d) {
+  extern __shared__ double chol_sm[];
+  const int m = blockIdx.x, c0 = m * d, w = min(d, Din - c0), ld = w + 1, tid = threadIdx.x;
+  double* L = chol_sm;            // [w][w + 1]
+  double* Li = chol_sm + w * ld;  // [w][w + 1]
+  double tr = 0.0;
+  for (int j = 0; j < w; j++) tr += G[static_cast<size_t>(c0 + j) * (Din + 1)];
+  if (tr == 0.0) return;
+  const double lam = 1e-10 * tr / w;
+  for (int e = tid; e < w * w; e += blockDim.x) {
+    const int i = e / w, j = e % w;
+    L[i * ld + j] = G[static_cast<size_t>(c0 + i) * Din + c0 + j] + (i == j ? lam : 0.0);
+  }
+  __syncthreads();
+  for (int k = 0; k < w; k++) {   // right-looking Cholesky, lower triangle
+    if (tid == 0) L[k * ld + k] = sqrt(L[k * ld + k]);
+    __syncthreads();
+    for (int i = k + 1 + tid; i < w; i += blockDim.x) L[i * ld + k] /= L[k * ld + k];
+    __syncthreads();
+    const int r = w - k - 1;
+    for (int e = tid; e < r * r; e += blockDim.x) {
+      const int i = k + 1 + e / r, j = k + 1 + e % r;
+      if (j <= i) L[i * ld + j] -= L[i * ld + k] * L[j * ld + k];
+    }
+    __syncthreads();
+  }
+  if (tid < w) {   // column c of L^-1 by forward substitution
+    const int c = tid;
+    Li[c * ld + c] = 1.0 / L[c * ld + c];
+    for (int i = c + 1; i < w; i++) {
+      double s = 0.0;
+      for (int k = c; k < i; k++) s += L[i * ld + k] * Li[k * ld + c];
+      Li[i * ld + c] = -s / L[i * ld + i];
+    }
+  }
+  __syncthreads();
+  for (int e = tid; e < w * w; e += blockDim.x) {
+    const int i = e / w, j = e % w;
+    Linv[(static_cast<size_t>(m) * d + i) * d + j] = j <= i ? Li[i * ld + j] : 0.0;
+  }
+}
+
+// E[o][c] = W[o][c] - C[c / d][A[c / d][o]][c % d] in fp64 (A held subspace-major, [S][Dout])
+__global__ void pqr_residual_kernel(const float* __restrict__ W, const float* __restrict__ C, const uint8_t* __restrict__ A,
+                                    double* __restrict__ E, int Din, int Dout, int K, int d) {
+  const size_t total = static_cast<size_t>(Dout) * Din;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int o = static_cast<int>(i / Din), c = static_cast<int>(i % Din), m = c / d;
+    const float cw = C[(static_cast<size_t>(m) * K + A[static_cast<size_t>(m) * Dout + o]) * d + c % d];
+    E[i] = static_cast<double>(W[i]) - static_cast<double>(cw);
+  }
+}
+
+// Deterministic sum of one double per thread: a fixed shuffle tree per warp, then the warps in ascending order.
+__device__ double BlockSum(double v, double* red) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double r = 0.0;
+  if (threadIdx.x == 0)
+    for (int i = 0; i < kSweepThreads / 32; i++) r += red[i];
+  return r;
+}
+
+// loss partials: CTA b sums E * GE over a fixed range of kLossBlocks equal ranges
+__global__ void __launch_bounds__(kSweepThreads) pqr_loss_partial_kernel(const double* __restrict__ E, const double* __restrict__ GE,
+                                                                         size_t n, double* __restrict__ part) {
+  __shared__ double red[kSweepThreads / 32];
+  const size_t chunk = (n + kLossBlocks - 1) / kLossBlocks, b0 = blockIdx.x * chunk, b1 = min(n, b0 + chunk);
+  double v = 0.0;
+  for (size_t i = b0 + threadIdx.x; i < b1; i += kSweepThreads) v += E[i] * GE[i];
+  const double tot = BlockSum(v, red);
+  if (threadIdx.x == 0) part[blockIdx.x] = tot;
+}
+
+__global__ void __launch_bounds__(kSweepThreads) pqr_loss_final_kernel(const double* __restrict__ part, double* __restrict__ loss) {
+  __shared__ double red[kSweepThreads / 32];
+  double v = 0.0;
+  for (int i = threadIdx.x; i < kLossBlocks; i += kSweepThreads) v += part[i];
+  const double tot = BlockSum(v, red);
+  if (threadIdx.x == 0) *loss = tot;
+}
+
+struct BlockArgs {
+  const double* G;        // [Din][Din]
+  const double* GE;       // [Dout][Din], as of the start of the block
+  const double* Linv;     // [S][d][d]
+  double* E;              // [Dout][Din]
+  double* dlt;            // [Dout][ld]: per block dim, the change of E (the old decoded weight while its subspace runs)
+  double* h;              // [Dout][d]
+  double* cconst;         // [K]: c_k^T G_mm c_k of the current subspace
+  float* C;               // [S][K][d]
+  uint8_t* A;             // [S][Dout]
+  int Din, Dout, K, d, ld, m0, m1;
+};
+
+// Subspaces [m0, m1) of one sweep, dims [blk0 = m0 d, ...).  GE is not written: the block's own earlier changes enter
+// h through dlt, and the trailing GEMM brings GE up to date afterwards.
+__global__ void __launch_bounds__(kSweepThreads) pqr_block_kernel(BlockArgs p) {
+  cg::grid_group grid = cg::this_grid();
+  extern __shared__ float4 blk_sm[];   // assignment step: Cs [K][w] fp32, then cs [K] fp64
+  __shared__ double sPart[kSweepThreads], sH[kMaxD], sY[kMaxD], sD[kMaxD], sCu[kMaxD], sRed[kMaxD];
+  __shared__ int sCnt[kSweepThreads], sN, sAcc;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int Din = p.Din, Dout = p.Dout, K = p.K, d = p.d, ld = p.ld, blk0 = p.m0 * d;
+  const int R = (Dout + gridDim.x - 1) / gridDim.x, r0 = min(Dout, static_cast<int>(blockIdx.x) * R), r1 = min(Dout, r0 + R);
+  for (size_t e = tid; e < static_cast<size_t>(r1 - r0) * ld; e += kSweepThreads) p.dlt[static_cast<size_t>(r0) * ld + e] = 0.0;
+  __syncthreads();
+  for (int m = p.m0; m < p.m1; m++) {
+    const int c0 = m * d, w = min(d, Din - c0), cb = c0 - blk0;
+    double tr = 0.0;
+    for (int j = 0; j < w; j++) tr += p.G[static_cast<size_t>(c0 + j) * (Din + 1)];
+    if (tr == 0.0) continue;   // no input energy: codebook and assignments stay
+    const uint8_t* Am = p.A + static_cast<size_t>(m) * Dout;
+    const float* Cm = p.C + static_cast<size_t>(m) * K * d;
+    // (1) h_o = GE_o[c0 + j] + sum_{c in block, c < c0} dlt_o[c] G[c0 + j][c] + sum_i G[c0 + j][c0 + i] w^_o[i]:
+    // eight lanes per (output, dim), each over every eighth dim, combined by a fixed shuffle tree
+    const int items = (r1 - r0) * w;
+    for (int base = 0; base < items * 8; base += kSweepThreads) {
+      const int it = base + tid, item = it >> 3, sub = it & 7;
+      const bool ok = item < items;
+      double acc = 0.0, wold = 0.0;
+      int o = 0, j = 0;
+      if (ok) {
+        o = r0 + item / w;
+        j = item % w;
+        const double* grow = p.G + static_cast<size_t>(c0 + j) * Din + blk0;
+        const double* drow = p.dlt + static_cast<size_t>(o) * ld;
+        for (int c = sub; c < cb; c += 8) acc += drow[c] * grow[c];
+        const float* cw = Cm + static_cast<size_t>(Am[o]) * d;
+        for (int i = sub; i < w; i += 8) acc += static_cast<double>(cw[i]) * grow[cb + i];
+        wold = static_cast<double>(cw[j]);
+      }
+      acc += __shfl_xor_sync(0xffffffffu, acc, 4);
+      acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+      acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+      if (ok && sub == 0) p.h[static_cast<size_t>(o) * d + j] = p.GE[static_cast<size_t>(o) * Din + c0 + j] + acc;
+      if (ok && sub == 1) p.dlt[static_cast<size_t>(o) * ld + cb + j] = wold;   // read by step (3); lanes above read c < cb
+    }
+    grid.sync();
+    // (2) codebook: cluster k per CTA.  H_k: nseg contiguous runs of outputs, each summed in ascending o, the runs
+    // combined in ascending order.
+    const int nseg = kSweepThreads / w;
+    for (int k = blockIdx.x; k < K; k += gridDim.x) {
+      if (tid < nseg * w) {
+        const int j = tid % w, seg = tid / w;
+        const int o0 = static_cast<int>(static_cast<long long>(Dout) * seg / nseg);
+        const int o1 = static_cast<int>(static_cast<long long>(Dout) * (seg + 1) / nseg);
+        double s = 0.0;
+        int n = 0;
+        for (int o = o0; o < o1; o++)
+          if (__ldcg(Am + o) == k) {
+            s += __ldcg(p.h + static_cast<size_t>(o) * d + j);
+            n++;
+          }
+        sPart[tid] = s;
+        if (j == 0) sCnt[seg] = n;
+      }
+      __syncthreads();
+      float* ck = p.C + (static_cast<size_t>(m) * K + k) * d;
+      if (tid < w) {
+        double s = 0.0;
+        for (int seg = 0; seg < nseg; seg++) s += sPart[seg * w + tid];
+        sH[tid] = s;
+        sCu[tid] = static_cast<double>(ck[tid]);
+      }
+      if (tid == 0) {
+        int n = 0;
+        for (int seg = 0; seg < nseg; seg++) n += sCnt[seg];
+        sN = n;
+      }
+      __syncthreads();
+      const int n = sN;
+      const double* Gmm = p.G + static_cast<size_t>(c0) * Din + c0;
+      if (n > 0) {
+        const double* Lm = p.Linv + static_cast<size_t>(m) * d * d;
+        if (tid < w) {   // y = L^-1 H / n
+          double s = 0.0;
+          for (int j = 0; j <= tid; j++) s += Lm[tid * d + j] * (sH[j] / n);
+          sY[tid] = s;
+        }
+        __syncthreads();
+        if (tid < w) {   // D = L^-T y, rounded to fp32
+          double s = 0.0;
+          for (int j = tid; j < w; j++) s += Lm[j * d + tid] * sY[j];
+          sD[tid] = static_cast<double>(static_cast<float>(s));
+        }
+        __syncthreads();
+        if (tid < w) {   // f(D) - f(c) = (D - c)^T (n G_mm (D + c) - 2 H), without the cancellation of two f values
+          double s = 0.0;
+          for (int j = 0; j < w; j++) s += Gmm[static_cast<size_t>(tid) * Din + j] * (sD[j] + sCu[j]);
+          sRed[tid] = (sD[tid] - sCu[tid]) * (static_cast<double>(n) * s - 2.0 * sH[tid]);
+        }
+        __syncthreads();
+        if (tid == 0) {
+          double s = 0.0;
+          for (int j = 0; j < w; j++) s += sRed[j];
+          sAcc = s < 0.0;
+        }
+        __syncthreads();
+        if (sAcc && tid < w) {
+          ck[tid] = static_cast<float>(sD[tid]);
+          sCu[tid] = sD[tid];
+        }
+        __syncthreads();
+      }
+      if (tid < w) {
+        double s = 0.0;
+        for (int j = 0; j < w; j++) s += Gmm[static_cast<size_t>(tid) * Din + j] * sCu[j];
+        sRed[tid] = sCu[tid] * s;
+      }
+      __syncthreads();
+      if (tid == 0) {
+        double s = 0.0;
+        for (int j = 0; j < w; j++) s += sRed[j];
+        p.cconst[k] = s;
+      }
+      __syncthreads();
+    }
+    grid.sync();
+    // (3) assignment, one warp per output; then E and dlt of the subspace's dims
+    float* Cs = reinterpret_cast<float*>(blk_sm);
+    double* cs = reinterpret_cast<double*>(blk_sm) + (K * w + 1) / 2;
+    for (int e = tid; e < K * w; e += kSweepThreads) Cs[e] = __ldcg(Cm + static_cast<size_t>(e / w) * d + e % w);
+    for (int k = tid; k < K; k += kSweepThreads) cs[k] = __ldcg(p.cconst + k);
+    __syncthreads();
+    for (int o = r0 + warp; o < r1; o += kSweepThreads / 32) {
+      const double* ho = p.h + static_cast<size_t>(o) * d;
+      double best = INFINITY;
+      int bi = K;
+      for (int k = lane; k < K; k += 32) {
+        double dot = 0.0;
+        for (int j = 0; j < w; j++) dot += static_cast<double>(Cs[k * w + j]) * ho[j];
+        const double v = cs[k] - 2.0 * dot;
+        if (v < best) { best = v; bi = k; }
+      }
+      for (int off = 16; off > 0; off >>= 1) {
+        const double ob = __shfl_xor_sync(0xffffffffu, best, off);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
+        if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
+      }
+      if (lane == 0) p.A[static_cast<size_t>(m) * Dout + o] = static_cast<uint8_t>(bi);
+      for (int j = lane; j < w; j += 32) {
+        double* dp = p.dlt + static_cast<size_t>(o) * ld + cb + j;
+        const double dE = *dp - static_cast<double>(Cs[bi * w + j]);   // E changes by w^_old - w^_new
+        *dp = dE;
+        p.E[static_cast<size_t>(o) * Din + c0 + j] += dE;
+      }
+    }
+    __syncthreads();
+  }
+}
+
+bool AllFinite(const float* v, size_t n) {
+  for (size_t i = 0; i < n; i++)
+    if (!isfinite(v[i])) return false;
+  return true;
+}
+
+int Refine(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const float* w_h, const float* x, int N, float* ctrd_h,
+           uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+  const char* who = "qcnn_pq_refine_fc";
+  QCNN_CHECK(ctx && w_h && ctrd_h && asmt_h, "%s: NULL argument", who);
+  QCNN_CHECK(Din >= 1 && Dout >= 1, "%s: bad dimensions", who);
+  if (int rc = CheckFcK(who, K)) return rc;
+  QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
+  QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
+  QCNN_CHECK(N >= 1, "%s: N=%d: at least one input is needed", who, N);
+  QCNN_CHECK(x, "%s: NULL argument", who);
+  const int S = CeilDiv(Din, d);
+  const size_t nw = static_cast<size_t>(Dout) * Din, nc = static_cast<size_t>(S) * K * d;
+  QCNN_CHECK(AllFinite(w_h, nw), "%s: the weights contain a non-finite value", who);
+  QCNN_CHECK(AllFinite(ctrd_h, nc), "%s: the codebook contains a non-finite value", who);
+  std::vector<uint8_t> at(static_cast<size_t>(S) * Dout);   // [S][Dout]
+  for (int o = 0; o < Dout; o++)
+    for (int m = 0; m < S; m++) {
+      const uint8_t a = asmt_h[static_cast<size_t>(o) * S + m];
+      QCNN_CHECK(a < K, "%s: assignment %d of output %d, subspace %d is not below K=%d", who, a, o, m, K);
+      at[static_cast<size_t>(m) * Dout + o] = a;
+    }
+  QCNN_ON_DEVICE(ctx->device);
+  const int spb = std::max(1, kBlockDims / d), ld = spb * d;
+  DeviceBuffer dG, dE, dGE, dW, dC, dA, dL, dDlt, dH, dCc, dPart, dLoss;
+  auto reserve = [&](DeviceBuffer& b, size_t bytes, const char* what) -> int {
+    const cudaError_t e = b.Reserve(ctx, bytes);
+    if (e == cudaSuccess) return 0;
+    cudaGetLastError();
+    SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
+    return 1;
+  };
+  if (reserve(dG, sizeof(double) * Din * static_cast<size_t>(Din), "the Gram matrix") ||
+      reserve(dE, sizeof(double) * nw, "the residual") || reserve(dGE, sizeof(double) * nw, "G times the residual") ||
+      reserve(dW, sizeof(float) * nw, "the weights") || reserve(dC, sizeof(float) * nc, "the codebook") ||
+      reserve(dA, at.size(), "the assignments") ||
+      reserve(dL, sizeof(double) * static_cast<size_t>(S) * d * d, "the Cholesky factors") ||
+      reserve(dDlt, sizeof(double) * Dout * static_cast<size_t>(ld), "the block's changes") ||
+      reserve(dH, sizeof(double) * Dout * static_cast<size_t>(d), "the subspace responses") ||
+      reserve(dCc, sizeof(double) * K, "the codeword norms") || reserve(dPart, sizeof(double) * kLossBlocks, "the loss") ||
+      reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss"))
+    return 1;
+  QCNN_CUDA(cudaMemcpyAsync(dW.get(), w_h, sizeof(float) * nw, cudaMemcpyHostToDevice, st));
+  QCNN_CUDA(cudaMemcpyAsync(dC.get(), ctrd_h, sizeof(float) * nc, cudaMemcpyHostToDevice, st));
+  QCNN_CUDA(cudaMemcpyAsync(dA.get(), at.data(), at.size(), cudaMemcpyHostToDevice, st));
+  // G = X^T X, then its diagonal: a NaN or Inf anywhere in x makes one entry non-finite (fp32 squares cannot overflow it)
+  const int tiles = CeilDiv(Din, kTile);
+  pqr_gemm_kernel<true><<<tiles * (tiles + 1) / 2, kGemmThreads, 0, st>>>(x, Din, nullptr, 0, dG.as<double>(), Din, Din, Din, N, 0);
+  QCNN_CUDA(cudaGetLastError());
+  std::vector<double> diag(Din);
+  QCNN_CUDA(cudaMemcpy2DAsync(diag.data(), sizeof(double), dG.get(), sizeof(double) * (static_cast<size_t>(Din) + 1),
+                              sizeof(double), Din, cudaMemcpyDeviceToHost, st));
+  QCNN_CUDA(cudaStreamSynchronize(st));
+  for (int c = 0; c < Din; c++) QCNN_CHECK(isfinite(diag[c]), "%s: x contains a non-finite value (input column %d)", who, c);
+  const size_t cholSmem = sizeof(double) * 2 * std::min(d, Din) * (std::min(d, Din) + 1);
+  if (int rc = OptInSmem<pqr_chol_kernel>(ctx)) return rc;
+  pqr_chol_kernel<<<S, kSweepThreads, cholSmem, st>>>(dG.as<double>(), dL.as<double>(), Din, d);
+  const int ewBlocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 32u * ctx->sm_count));
+  pqr_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Din, Dout, K, d);
+  const dim3 gemmGrid(tiles, CeilDiv(Dout, kTile));
+  pqr_gemm_kernel<false><<<gemmGrid, kGemmThreads, 0, st>>>(dE.get(), Din, dG.get(), Din, dGE.as<double>(), Din, Dout, Din, Din, 0);
+  QCNN_CUDA(cudaGetLastError());
+  auto loss = [&](int t) -> int {
+    pqr_loss_partial_kernel<<<kLossBlocks, kSweepThreads, 0, st>>>(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>());
+    pqr_loss_final_kernel<<<1, kSweepThreads, 0, st>>>(dPart.as<double>(), dLoss.as<double>() + t);
+    QCNN_CUDA(cudaGetLastError());
+    return 0;
+  };
+  if (int rc = loss(0)) return rc;
+  if (sweeps > 0) {
+    const size_t blkSmem = sizeof(float) * K * std::min(d, Din) + sizeof(double) * (K + 1);
+    cudaFuncAttributes fa;   // the opt-in limit covers static plus dynamic shared memory
+    QCNN_CUDA(cudaFuncGetAttributes(&fa, pqr_block_kernel));
+    QCNN_CUDA(cudaFuncSetAttribute(pqr_block_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   static_cast<int>(SmemOptin(ctx) - fa.sharedSizeBytes)));
+    int perSm = 0;
+    QCNN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, pqr_block_kernel, kSweepThreads, blkSmem));
+    QCNN_CHECK(perSm >= 1, "%s: the sweep kernel does not fit on an SM", who);
+    const int grid = std::min(std::min(perSm, 2) * ctx->sm_count, std::max(Dout, K));
+    BlockArgs a{dG.as<double>(), dGE.as<double>(), dL.as<double>(), dE.as<double>(), dDlt.as<double>(), dH.as<double>(),
+                dCc.as<double>(), dC.as<float>(), dA.as<uint8_t>(), Din, Dout, K, d, ld, 0, 0};
+    for (int t = 1; t <= sweeps; t++) {
+      for (int m0 = 0; m0 < S; m0 += spb) {
+        a.m0 = m0;
+        a.m1 = std::min(S, m0 + spb);
+        void* args[] = {&a};
+        QCNN_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(pqr_block_kernel), grid, kSweepThreads, args, blkSmem, st));
+        // GE += dlt G[block dims][:]
+        const int blk0 = m0 * d, bw = std::min(Din, a.m1 * d) - blk0;
+        pqr_gemm_kernel<false><<<gemmGrid, kGemmThreads, 0, st>>>(dDlt.get(), ld, dG.as<double>() + static_cast<size_t>(blk0) * Din,
+                                                                  Din, dGE.as<double>(), Din, Dout, Din, bw, 1);
+        QCNN_CUDA(cudaGetLastError());
+      }
+      if (int rc = loss(t)) return rc;
+    }
+  }
+  std::vector<double> lossv(sweeps + 1);
+  QCNN_CUDA(cudaMemcpyAsync(ctrd_h, dC.get(), sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
+  QCNN_CUDA(cudaMemcpyAsync(at.data(), dA.get(), at.size(), cudaMemcpyDeviceToHost, st));
+  QCNN_CUDA(cudaMemcpyAsync(lossv.data(), dLoss.get(), sizeof(double) * lossv.size(), cudaMemcpyDeviceToHost, st));
+  QCNN_CUDA(cudaStreamSynchronize(st));
+  for (int o = 0; o < Dout; o++)
+    for (int m = 0; m < S; m++) asmt_h[static_cast<size_t>(o) * S + m] = at[static_cast<size_t>(m) * Dout + o];
+  if (loss_h) std::copy(lossv.begin(), lossv.end(), loss_h);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int qcnn_pq_refine_fc(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const float* wei_h, const float* x,
+                                 int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h, void* stream) {
+  return Refine(ctx, Din, Dout, K, d, sweeps, wei_h, x, N, ctrd_h, asmt_h, loss_h, static_cast<cudaStream_t>(stream));
+}

@@ -463,6 +463,9 @@ int OptInSmem(qcnn_ctx* ctx) {
   return 0;
 }
 
+// pq_quantize.cu: K as qcnn_fc_layer_create accepts it (16, 32, 64, 128 or 256); sets the error and returns 1 otherwise
+int CheckFcK(const char* who, int K);
+
 // conv_ws.cu: the tensor-core family's weight-stationary tilings of stride-1 layers (mode-0 geometry, channel tiles) and
 // of strided narrow-input layers (mode-1 geometry)
 void PlanConvWs(const qcnn_layer* L, int N, ConvCands* cands);
