@@ -323,6 +323,36 @@ QCNN_API int qcnn_pq_refine_fc(qcnn_ctx* ctx, int Din, int Dout, int K, int d, i
                                const float* wei_h /*[Dout][Din]*/, const float* x /*device [N][Din]*/, int N,
                                float* ctrd_h /*in/out [S][K][d]*/, uint8_t* asmt_h /*in/out [Dout][S], 0-based*/,
                                double* loss_h /*nullable [sweeps + 1]*/, void* stream);
+/* Error-correcting PQ of a conv layer (DESIGN.md 4e): block coordinate descent on (ctrd, asmt) that lowers
+ * loss = sum_{n,o,y,x} conv(x, W - W^)^2 = sum_g sum_{o in g} E_o^T G_g E_o, E = W - W^ (fp64), on the layer inputs
+ * x [N][Hin][Win][Cin] (device, NHWC: what Net.featmap returns for the layer's input under keep_maps).  Geometry as
+ * qcnn_conv_layer_create; Cg = Cin / grp, S = ceil(Cg / d), subspace m covers the per-group channels m d .. m d + w_m - 1,
+ * tap t = kh k + kw, output o is in group o / (Cout / grp), and one codebook serves all taps and groups.
+ * G_g = sum p p^T (fp64, fixed order, exactly symmetric) over every image and output position, p the zero-padded
+ * Cg k^2 patch of group g's channels.  A sweep visits m = 0..S-1 in order; m is skipped when sum_g sum_t tr G^m_{g,tt} = 0
+ * (G^m_{g,tt'}: the w_m x w_m block of G_g between the dims of (m, t) and (m, t')), else:
+ *   h_{o,t} = [G_g R_o]_(m,t), R_o = E_o + W^_o(m) (the residual of the other subspaces);
+ *   codebook: over U = {k : n_k > 0} (ascending), M = sum_g sum_{t,t'} Cnt^g_{tt'} (x) G^m_{g,tt'} (Cnt^g_{tt'}[k][k'] =
+ *     |{o in g : A[o][t][m] = k, A[o][t'][m] = k'}|, g, t, t' ascending), b_k = sum of h_{o,t} over A[o][t][m] = k
+ *     (o, then t ascending); D = fp32((M + mu I)^-1 b) by fp64 Cholesky, mu = 1e-10 tr(M) / (|U| w_m), replaces C[m][U]
+ *     only if (D - C)^T (M (D + C) - 2 b) < 0; empty clusters keep their codeword, dims j >= w_m stay 0;
+ *   assignment: taps t = 0..k^2-1 in order, per output A[o][t][m] = argmin_k c_k^T G^m_{g,tt} c_k - 2 c_k^T h'_{o,t} (fp64,
+ *     lowest index on ties), h'_{o,t} = [G_g E_o]_(m,t) + G^m_{g,tt} w^_{o,t} with E current (earlier taps' changes
+ *     included); a (g, t) with tr G^m_{g,tt} = 0 keeps its assignments; E is updated before m + 1.
+ * ctrd_h [S][K][d] and asmt_h [Cout][k][k][S] (0-based) are the start and receive the result; loss_h (nullable, sweeps + 1
+ * values) = the start's loss, then the loss after each sweep.  Results are bit-reproducible.  Runs on `stream` (ordered
+ * after whatever produced x) and synchronises it before returning.  Device memory: 8 grp (Cg k^2)^2 bytes for the Grams,
+ * 20 Cout Cg k^2 for E, G E and the weights, 16 (K min(d, Cg))^2 for M and its factor, 24 Cout k^2 min(d, Cg) for one
+ * subspace's responses, and one chunk of at most 256 MiB of patches.  Fails on what qcnn_pq_quantize_conv refuses (K not
+ * a multiple of 8 in 8..256, d outside 1..64, non-finite weights or codebook), non-finite x, sweeps < 0, N < 1, an
+ * assignment >= K, Cin or Cout not divisible by grp, an empty output, K min(d, Cg) > 2048 (the size of the joint
+ * system), or a failed allocation (with its byte count). */
+QCNN_API int qcnn_pq_refine_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride,
+                                 int grp, int K, int d, int sweeps,
+                                 const float* knl_h /*[Cout][Cin/grp][k][k]*/,
+                                 const float* x /*device NHWC [N][Hin][Win][Cin]*/, int N,
+                                 float* ctrd_h /*in/out [S][K][d]*/, uint8_t* asmt_h /*in/out [Cout][k][k][S], 0-based*/,
+                                 double* loss_h /*nullable [sweeps + 1]*/, void* stream);
 
 /* ---- file formats (include/FileIO.h:56-178, 229-350), host only ------------------------------------------- */
 /* .bin: returns element count or -1; dims4 padded with 1; data_h may be NULL to query the shape */

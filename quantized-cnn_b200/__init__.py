@@ -130,6 +130,7 @@ _SIGS = {
     "qcnn_pq_quantize_fc": (_i, [_vp] + [_i] * 5 + [C.c_uint32, _vp, _vp, _vp, _vp, _vp]),
     "qcnn_pq_quantize_model": (_i, [_vp, _cp, _cp, _cp, C.POINTER(_i), C.POINTER(_i), _i, C.c_uint32, _cp, _cp]),
     "qcnn_pq_refine_fc": (_i, [_vp] + [_i] * 5 + [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_refine_conv": (_i, [_vp] + [_i] * 11 + [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
 }
 for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)
@@ -676,4 +677,27 @@ def pq_refine_fc(ctx, wei, x, ctrd, asmt, sweeps=8, stream=None):
     _check(lib.qcnn_pq_refine_fc(ctx.h, Din, Dout, K, d, sweeps, wei.ctypes.data_as(_vp), _dptr(x), x.shape[0],
                                  ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp),
                                  _stream(stream)))
+    return ctrd, asmt, loss
+
+
+def pq_refine_conv(ctx, knl, x, ctrd, asmt, pad=0, stride=1, grp=1, sweeps=8, stream=None):
+    """Error-correcting PQ of conv weights knl [Cout, Cin / grp, k, k] on layer inputs x (contiguous float32 CUDA tensor
+    [N, Hin, Win, Cin], NHWC as Net.featmap returns it), starting from (ctrd [S, K, d], asmt [Cout, k, k, S] 0-based),
+    e.g. pq_quantize_conv's output: (ctrd, asmt, loss [sweeps + 1]) with loss[t] = sum conv(x, W - W^)^2 after sweep t.
+    The arguments are not modified."""
+    knl = _np(knl, np.float32)
+    Cout, Cg, k, k2 = knl.shape
+    ctrd = np.array(ctrd, np.float32, order="C", copy=True)
+    asmt = np.array(asmt, np.uint8, order="C", copy=True)
+    S, K, d = ctrd.shape
+    if k != k2 or S != -(-Cg // d) or asmt.shape != (Cout, k, k, S):
+        raise QcnnError("ctrd [%d, K, d] and asmt %s do not match a %s kernel with d=%d"
+                        % (S, tuple(asmt.shape), tuple(knl.shape), d))
+    if x.dim() != 4 or x.shape[3] != Cg * grp:
+        raise QcnnError("x must be [N, Hin, Win, %d], got %s" % (Cg * grp, tuple(x.shape)))
+    N, Hin, Win, Cin = x.shape
+    loss = np.empty(max(sweeps, 0) + 1, np.float64)
+    _check(lib.qcnn_pq_refine_conv(ctx.h, Cin, Hin, Win, Cout, k, pad, stride, grp, K, d, sweeps,
+                                   knl.ctypes.data_as(_vp), _dptr(x), N, ctrd.ctypes.data_as(_vp),
+                                   asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp), _stream(stream)))
     return ctrd, asmt, loss

@@ -334,12 +334,6 @@ int Quantize(qcnn_ctx* ctx, const char* who, int Cout, int Cg, int ksz, int K, i
   return 0;
 }
 
-// K as qcnn_conv_layer_create / qcnn_fc_layer_create accept it, so that the output always loads
-int CheckConvK(const char* who, int K) {
-  QCNN_CHECK(K >= 8 && K <= kMaxK && K % 8 == 0, "%s: K=%d must be a multiple of 8 in 8..%d", who, K, kMaxK);
-  return 0;
-}
-
 struct QuantizedLayer {
   int l;
   Matrix<float> ctrd;
@@ -366,6 +360,12 @@ bool WriteFile(const std::string& path, const std::vector<char>& buf) {
 }
 
 }  // namespace
+
+// K as qcnn_conv_layer_create / qcnn_fc_layer_create accept it, so that the output always loads
+int qcnn::CheckConvK(const char* who, int K) {
+  QCNN_CHECK(K >= 8 && K <= kMaxK && K % 8 == 0, "%s: K=%d must be a multiple of 8 in 8..%d", who, K, kMaxK);
+  return 0;
+}
 
 int qcnn::CheckFcK(const char* who, int K) {
   QCNN_CHECK(K == 16 || K == 32 || K == 64 || K == 128 || K == 256, "%s: unsupported codebook size K=%d (supported: 16, 32, 64, 128, 256)",

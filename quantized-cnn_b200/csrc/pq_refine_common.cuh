@@ -1,0 +1,182 @@
+// Pieces shared by the error-correcting quantizers of FC layers (pq_refine.cu) and conv layers (pq_refine_conv.cu):
+// the fp64 tensor-core GEMM, the fixed-order block reduction and the loss kernels.  They sit in an anonymous namespace
+// because each including .cu file is its own device module and links its own copy.
+#ifndef QCNN_PQ_REFINE_COMMON_CUH_
+#define QCNN_PQ_REFINE_COMMON_CUH_
+
+#include <math.h>
+
+#include "qcnn_internal.h"
+
+namespace {
+
+constexpr int kTile = 64;            // GEMM output tile (kTile x kTile per CTA, 2 x 2 warps of 32 x 32)
+constexpr int kKStep = 16;           // the DMMA's k
+constexpr int kLd = kTile + 4;       // smem row pitch in doubles: fragment reads hit 16 distinct 8-byte bank pairs
+constexpr int kGemmThreads = 128;
+constexpr int kSweepThreads = 256;
+constexpr int kLossBlocks = 512;     // fixed, so the loss reduction order does not depend on the device
+
+__device__ __forceinline__ void Dmma(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+      "{%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]), "d"(b[1]),
+        "d"(b[2]), "d"(b[3]));
+}
+
+// fp64 tensor-core GEMM, one kTile x kTile output tile per CTA, k in ascending steps of 16 (a fixed order per element).
+//   kGram:  C = (accumulate ? C : 0) + X^T X for X = A [Kd][lda] fp32 (M = N = the column count): lower-triangle tiles
+//           only (blockIdx.x is the linear lower-triangle index); each element with row >= col is written to both
+//           (row, col) and (col, row), so G is exactly symmetric.
+//   else:   C [M][N] = (accumulate ? C : 0) + A [M][Kd] B [Kd][N], all fp64.
+// Operands are staged through registers (the next k-step is loaded while the current one is multiplied), widened to
+// fp64 and stored k-major, [16][kLd], in shared memory.
+template <bool kGram>
+__global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __restrict__ Ap, int lda, const void* __restrict__ Bp,
+                                                                int ldb, double* __restrict__ C, int ldc, int M, int N, int Kd,
+                                                                int accumulate) {
+  __shared__ double As[2][kKStep][kLd], Bs[2][kKStep][kLd];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int g = lane >> 2, t = lane & 3, wm = warp >> 1, wn = warp & 1;
+  int tm, tn;
+  if (kGram) {
+    const int i = blockIdx.x;
+    tm = static_cast<int>((sqrt(8.0 * i + 1.0) - 1.0) * 0.5);
+    while (tm * (tm + 1) / 2 > i) tm--;
+    while ((tm + 1) * (tm + 2) / 2 <= i) tm++;
+    tn = i - tm * (tm + 1) / 2;
+  } else {
+    tm = blockIdx.y;
+    tn = blockIdx.x;
+  }
+  const int m0 = tm * kTile, n0 = tn * kTile;
+  constexpr int kPer = kKStep * kTile / kGemmThreads;   // 8 elements of each operand per thread and k-step
+  double ra[kPer], rb[kPer];
+  auto load = [&](int k0) {
+#pragma unroll
+    for (int r = 0; r < kPer; r++) {
+      const int e = tid + r * kGemmThreads;
+      const int kk = e / kTile, nn = e % kTile;   // B (and the Gram's A): row kk of the k-step, column nn
+      const int k = k0 + kk;
+      if (kGram) {
+        const float* X = static_cast<const float*>(Ap);
+        ra[r] = (k < Kd && m0 + nn < M) ? static_cast<double>(X[static_cast<size_t>(k) * lda + m0 + nn]) : 0.0;
+        rb[r] = (k < Kd && n0 + nn < N) ? static_cast<double>(X[static_cast<size_t>(k) * lda + n0 + nn]) : 0.0;
+      } else {
+        const double* A = static_cast<const double*>(Ap);
+        const double* B = static_cast<const double*>(Bp);
+        const int mm = e / kKStep, ka = k0 + e % kKStep;   // A: row mm, k-column ka (rows of A are contiguous in k)
+        ra[r] = (ka < Kd && m0 + mm < M) ? A[static_cast<size_t>(m0 + mm) * lda + ka] : 0.0;
+        rb[r] = (k < Kd && n0 + nn < N) ? B[static_cast<size_t>(k) * ldb + n0 + nn] : 0.0;
+      }
+    }
+  };
+  auto store = [&](int buf) {
+#pragma unroll
+    for (int r = 0; r < kPer; r++) {
+      const int e = tid + r * kGemmThreads;
+      if (kGram) As[buf][e / kTile][e % kTile] = ra[r];
+      else As[buf][e % kKStep][e / kKStep] = ra[r];
+      Bs[buf][e / kTile][e % kTile] = rb[r];
+    }
+  };
+  double acc[2][4][4];
+#pragma unroll
+  for (int a = 0; a < 2; a++)
+#pragma unroll
+    for (int b = 0; b < 4; b++)
+#pragma unroll
+      for (int c = 0; c < 4; c++) acc[a][b][c] = 0.0;
+  const int nk = (Kd + kKStep - 1) / kKStep;
+  load(0);
+  store(0);
+  __syncthreads();
+  for (int kt = 0; kt < nk; kt++) {
+    const int buf = kt & 1;
+    if (kt + 1 < nk) load((kt + 1) * kKStep);
+    double fa[2][8], fb[4][4];
+#pragma unroll
+    for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+      for (int i = 0; i < 8; i++) fa[mt][i] = As[buf][t + 4 * (i >> 1)][wm * 32 + mt * 16 + g + 8 * (i & 1)];
+#pragma unroll
+    for (int nt = 0; nt < 4; nt++)
+#pragma unroll
+      for (int i = 0; i < 4; i++) fb[nt][i] = Bs[buf][t + 4 * i][wn * 32 + nt * 8 + g];
+#pragma unroll
+    for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+      for (int nt = 0; nt < 4; nt++) Dmma(acc[mt][nt], fa[mt], fb[nt]);
+    if (kt + 1 < nk) store(buf ^ 1);
+    __syncthreads();
+  }
+#pragma unroll
+  for (int mt = 0; mt < 2; mt++)
+#pragma unroll
+    for (int nt = 0; nt < 4; nt++)
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        const int row = m0 + wm * 32 + mt * 16 + g + 8 * (i >> 1), col = n0 + wn * 32 + nt * 8 + 2 * t + (i & 1);
+        if (row >= M || col >= N) continue;
+        if (kGram) {
+          if (row < col) continue;
+          double* p = C + static_cast<size_t>(row) * ldc + col;
+          const double v = accumulate ? *p + acc[mt][nt][i] : acc[mt][nt][i];
+          *p = v;
+          C[static_cast<size_t>(col) * ldc + row] = v;
+        } else {
+          double* p = C + static_cast<size_t>(row) * ldc + col;
+          *p = (accumulate ? *p : 0.0) + acc[mt][nt][i];
+        }
+      }
+}
+
+// Deterministic sum of one double per thread: a fixed shuffle tree per warp, then the warps in ascending order.
+__device__ double BlockSum(double v, double* red) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double r = 0.0;
+  if (threadIdx.x == 0)
+    for (int i = 0; i < kSweepThreads / 32; i++) r += red[i];
+  return r;
+}
+
+// loss partials: CTA b sums E * GE over a fixed range of kLossBlocks equal ranges
+__global__ void __launch_bounds__(kSweepThreads) pqr_loss_partial_kernel(const double* __restrict__ E, const double* __restrict__ GE,
+                                                                         size_t n, double* __restrict__ part) {
+  __shared__ double red[kSweepThreads / 32];
+  const size_t chunk = (n + kLossBlocks - 1) / kLossBlocks, b0 = blockIdx.x * chunk, b1 = min(n, b0 + chunk);
+  double v = 0.0;
+  for (size_t i = b0 + threadIdx.x; i < b1; i += kSweepThreads) v += E[i] * GE[i];
+  const double tot = BlockSum(v, red);
+  if (threadIdx.x == 0) part[blockIdx.x] = tot;
+}
+
+__global__ void __launch_bounds__(kSweepThreads) pqr_loss_final_kernel(const double* __restrict__ part, double* __restrict__ loss) {
+  __shared__ double red[kSweepThreads / 32];
+  double v = 0.0;
+  for (int i = threadIdx.x; i < kLossBlocks; i += kSweepThreads) v += part[i];
+  const double tot = BlockSum(v, red);
+  if (threadIdx.x == 0) *loss = tot;
+}
+
+// loss = sum E * GE over n elements, in a fixed order, written to *loss
+inline int LaunchLoss(const double* E, const double* GE, size_t n, double* part, double* loss, cudaStream_t st) {
+  pqr_loss_partial_kernel<<<kLossBlocks, kSweepThreads, 0, st>>>(E, GE, n, part);
+  pqr_loss_final_kernel<<<1, kSweepThreads, 0, st>>>(part, loss);
+  QCNN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+bool AllFinite(const float* v, size_t n) {
+  for (size_t i = 0; i < n; i++)
+    if (!isfinite(v[i])) return false;
+  return true;
+}
+
+}  // namespace
+
+#endif  // QCNN_PQ_REFINE_COMMON_CUH_

@@ -463,8 +463,10 @@ int OptInSmem(qcnn_ctx* ctx) {
   return 0;
 }
 
-// pq_quantize.cu: K as qcnn_fc_layer_create accepts it (16, 32, 64, 128 or 256); sets the error and returns 1 otherwise
+// pq_quantize.cu: K as qcnn_fc_layer_create accepts it (16, 32, 64, 128 or 256), and as qcnn_conv_layer_create accepts
+// it (a multiple of 8 in 8..256); each sets the error and returns 1 otherwise
 int CheckFcK(const char* who, int K);
+int CheckConvK(const char* who, int K);
 
 // conv_ws.cu: the tensor-core family's weight-stationary tilings of stride-1 layers (mode-0 geometry, channel tiles) and
 // of strided narrow-input layers (mode-1 geometry)

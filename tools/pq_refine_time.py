@@ -5,7 +5,15 @@ median per sweep of the sum of kernel durations (the sweeps are split at their l
 the per-block cooperative kernel and the trailing GEMMs, achieved fp64 TFLOP/s from shape-based flop counts
 (Gram: N Din (Din + 1), the useful lower triangle; sweep: 2 Dout Din^2, its GEMM work), and the loss trace.  Then, with
 the profiler off, the wall time of a whole call.  Prints the card, its power limit and max SM clock.
-    python tools/pq_refine_time.py [--sweeps 3] [--layers alexnet_fc6 ...]"""
+The conv layers (qcnn_pq_refine_conv) of AlexNet (conv1-conv5, N = 64 images) and VGG16 (13 layers, N = 8) run at the
+shipped AlexNet (K, d) and the VGG16 table of tests/test_oracle_vgg16.py (K = 128, d = 8; conv1_1 d = 4) on seeded
+Gaussian maps and weights (std 1/sqrt(fan-in)), started from pq_quantize_conv (iters = 20).  Per layer: the time of
+the patch and Gram kernels; per sweep (median) the sum of kernel durations split into the Cholesky (ridge, diagonal
+blocks, panels, their trailing GEMMs, the solve), the assignment step, the response and GE GEMMs, and the building of
+the joint system (member lists, M, b); fp64 TFLOP/s of the Gram (positions Dg (Dg + 1) per group), of the GEMMs
+(2 Cout (sum_m (k^2 w_m)^2 + Dg^2)) and of the Cholesky ((K w_m)^3 / 3 per subspace, every cluster in use); the wall
+time of a whole call with the profiler off.
+    python tools/pq_refine_time.py [--sweeps 3] [--layers alexnet_fc6 alexnet_conv1 vgg16_conv1_2 ...]"""
 import argparse
 import importlib
 import json
@@ -25,6 +33,18 @@ LAYERS = {   # name: (Din, Dout, K, d, N)
     "alexnet_fc8": (4096, 1000, 16, 1, 4 * 4096),
     "vgg16_fc6": (25088, 4096, 32, 4, 8192),
 }
+CONV_LAYERS = {   # name: (Cin, H, Cout, k, pad, stride, grp, K, d, N)
+    "alexnet_conv1": (3, 227, 96, 11, 0, 4, 1, 128, 8, 64),
+    "alexnet_conv2": (96, 27, 256, 5, 2, 1, 2, 128, 8, 64),
+    "alexnet_conv3": (256, 13, 384, 3, 1, 1, 1, 128, 8, 64),
+    "alexnet_conv4": (384, 13, 384, 3, 1, 1, 2, 128, 8, 64),
+    "alexnet_conv5": (384, 13, 256, 3, 1, 1, 2, 128, 8, 64),
+}
+for _i, (_cin, _cout, _h) in enumerate([(3, 64, 224), (64, 64, 224), (64, 128, 112), (128, 128, 112), (128, 256, 56),
+                                        (256, 256, 56), (256, 256, 56), (256, 512, 28), (512, 512, 28), (512, 512, 28),
+                                        (512, 512, 14), (512, 512, 14), (512, 512, 14)]):
+    _blk, _n = [(1, 1), (1, 2), (2, 1), (2, 2), (3, 1), (3, 2), (3, 3), (4, 1), (4, 2), (4, 3), (5, 1), (5, 2), (5, 3)][_i]
+    CONV_LAYERS["vgg16_conv%d_%d" % (_blk, _n)] = (_cin, _h, _cout, 3, 1, 1, 1, 128, 4 if _cin == 3 else 8, 8)
 
 
 def card():
@@ -37,14 +57,77 @@ def kernels(prof):
     """(name, start us, duration us) of every CUDA kernel of the trace, in start order"""
     from torch.autograd import DeviceType
     ev = [(e.name, e.time_range.start, e.time_range.end - e.time_range.start) for e in prof.events()
-          if e.device_type == DeviceType.CUDA and "pqr_" in e.name]
+          if e.device_type == DeviceType.CUDA and ("pqr_" in e.name or "pqrc_" in e.name)]
     return sorted(ev, key=lambda x: x[1])
+
+
+def time_conv(q, ctx, name, sweeps):
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    Cin, H, Cout, k, pad, stride, grp, K, d, N = CONV_LAYERS[name]
+    Cg = Cin // grp
+    W = np.random.default_rng(1).standard_normal((Cout, Cg, k, k), dtype=np.float32) / np.float32(np.sqrt(Cg * k * k))
+    g = torch.Generator(device="cuda").manual_seed(2)
+    x = torch.randn((N, H, H, Cin), generator=g, device="cuda", dtype=torch.float32)
+    c0, a0, _ = q.pq_quantize_conv(ctx, W, K, d, iters=20, seed=3)
+    q.pq_refine_conv(ctx, W, x[:1], c0, a0, pad=pad, stride=stride, grp=grp, sweeps=1)   # warm-up
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        _, _, loss = q.pq_refine_conv(ctx, W, x, c0, a0, pad=pad, stride=stride, grp=grp, sweeps=sweeps)
+        torch.cuda.synchronize()
+    ev = kernels(prof)
+    gram = sum(t for n, _, t in ev if "pqr_gemm_kernel<true>" in n or "pqrc_patch" in n)
+    ends = [i for i, (n, _, _) in enumerate(ev) if "pqr_loss_final" in n]
+    split = dict(chol=[], assign=[], gemm=[], system=[], total=[])
+    for a, b in zip(ends[:-1], ends[1:]):
+        part, in_chol = ev[a + 1:b + 1], False
+        acc = dict.fromkeys(split, 0.0)
+        for n, _, t in part:
+            if "pqrc_ridge" in n:
+                in_chol = True
+            if in_chol or "pqrc_solve" in n:
+                acc["chol"] += t
+            elif "pqrc_assign" in n or "pqrc_ccost" in n:
+                acc["assign"] += t
+            elif "pqr_gemm_kernel<false>" in n:
+                acc["gemm"] += t
+            elif "pqr_loss" not in n:
+                acc["system"] += t
+            if "pqrc_solve" in n:
+                in_chol = False
+            acc["total"] += t
+        for key in split:
+            split[key].append(acc[key])
+    med = {key: float(np.median(v)) / 1e3 for key, v in split.items()}
+    t0 = time.perf_counter()
+    q.pq_refine_conv(ctx, W, x, c0, a0, pad=pad, stride=stride, grp=grp, sweeps=sweeps)
+    wall = time.perf_counter() - t0
+    Ho = (H + 2 * pad - k) // stride + 1
+    T, Dg, S = k * k, Cg * k * k, -(-Cg // d)
+    ws = [min(d, Cg - m * d) for m in range(S)]
+    gram_flop = grp * N * Ho * Ho * Dg * (Dg + 1)
+    gemm_flop = 2.0 * Cout * (sum((T * w) ** 2 for w in ws) + Dg * Dg)
+    chol_flop = sum((K * w) ** 3 / 3.0 for w in ws)
+    r = dict(layer=name, Cin=Cin, H=H, Cout=Cout, k=k, pad=pad, stride=stride, grp=grp, K=K, d=d, N=N,
+             gram_ms=gram / 1e3, gram_tflops=gram_flop / (gram * 1e-6) / 1e12,
+             sweep_ms=med["total"], sweep_chol_ms=med["chol"], sweep_assign_ms=med["assign"], sweep_gemm_ms=med["gemm"],
+             sweep_system_ms=med["system"], gemm_tflops=gemm_flop / (med["gemm"] * 1e-3) / 1e12,
+             chol_tflops=chol_flop / (med["chol"] * 1e-3) / 1e12, call_wall_s=wall,
+             loss=[float(v) for v in loss], loss_ratio=float(loss[-1] / loss[0]))
+    print("%-14s Gram %8.2f ms (%5.1f TFLOP/s)  sweep %8.2f ms (Cholesky %.2f ms %.2f TFLOP/s, assignment %.2f ms, "
+          "GEMMs %.2f ms %.1f TFLOP/s, system %.2f ms)  call %.2f s  loss x%.3f after %d sweeps"
+          % (name, r["gram_ms"], r["gram_tflops"], r["sweep_ms"], r["sweep_chol_ms"], r["chol_tflops"],
+             r["sweep_assign_ms"], r["sweep_gemm_ms"], r["gemm_tflops"], r["sweep_system_ms"], wall, r["loss_ratio"],
+             sweeps))
+    del x
+    torch.cuda.empty_cache()
+    return r
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sweeps", type=int, default=3)
-    ap.add_argument("--layers", nargs="*", default=list(LAYERS))
+    ap.add_argument("--layers", nargs="*", default=list(LAYERS) + list(CONV_LAYERS))
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
     args = ap.parse_args()
     import torch
@@ -55,6 +138,9 @@ def main():
     print("card: %s (name, power limit, max SM clock)" % card())
     results = []
     for name in args.layers:
+        if name in CONV_LAYERS:
+            results.append(time_conv(q, ctx, name, args.sweeps))
+            continue
         Din, Dout, K, d, N = LAYERS[name]
         W = (np.random.default_rng(1).standard_normal((Dout, Din), dtype=np.float32) / np.float32(np.sqrt(Din)))
         g = torch.Generator(device="cuda").manual_seed(2)
