@@ -61,7 +61,11 @@ QCNN_API int qcnn_stream_sync(qcnn_ctx* ctx, void* stream);
  *   bias_h  [Cout] / [Dout]      f32
  * Conv: ONE codebook is shared by all `grp` groups; group g reads input channels [g*Cin/grp, (g+1)*Cin/grp) and
  * assignment columns [g*Cout/grp, ...) (src/CaffeEva.cc:795-811,847).  Subspace s covers the per-group channels
- * [s*d, s*d + min(Cin/grp - s*d, d)) (src/CaffeEva.cc:1276-1277). */
+ * [s*d, s*d + min(Cin/grp - s*d, d)) (src/CaffeEva.cc:1276-1277).
+ * FC: K is 16, 32, 64, 128 or 256, and d is bounded so that the LUT + gather kernel, which runs every batch of 5 to 95
+ * images and every batch under tensor_core = 0, can stage a chunk of codebook rows in shared memory: d <= 93 (K = 16),
+ * 48 (K = 32), 24 (K = 64, 128) or 11 (K = 256).  Larger d is refused at creation, with a message naming K and d.
+ * That kernel takes the widest batch tile that fits: at K = 256, 8 images per CTA up to d = 8, 4 up to d = 10, else 1. */
 QCNN_API int qcnn_conv_layer_create(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad,
                                     int stride, int grp, int S, int K, int d, const float* ctrd_h,
                                     const uint8_t* asmt_h, const float* bias_h, qcnn_layer** out);
@@ -73,7 +77,7 @@ QCNN_API int qcnn_fc_layer_set_src_nhwc(qcnn_layer* layer, int H, int W, int C);
 /* Conv only: the source is NCHW [N][C][H][W] (the API input of CaffeEva::ExecForwardPass, CaffeEva.cc:225-228). */
 QCNN_API int qcnn_conv_layer_set_src_nchw(qcnn_layer* layer, int enable);
 /* tuning overrides for tests/benchmarks: "fc_nsplit" (subspace splits, 0 = automatic; 1 reproduces the reference's
- * accumulation order exactly), "fc_tn" (images per CTA: 1, 4 or 8; 0 = automatic), "tensor_core" (2 = default: eligible layers
+ * accumulation order exactly), "fc_tn" (images per CTA: 1, 4 or 8; 0 = automatic; a tile whose staging does not fit fails the forward), "tensor_core" (2 = default: eligible layers
  * run as decode-at-use GEMMs on the tensor cores with bf16x2 operands; 1 = the same GEMMs with 3xTF32 operands; 0 = LUT +
  * gather kernels only, the fp32 strict-parity path -- tolerances of all three in DESIGN.md);
  * conv layers, for tests that must know which kernel they check: "force_kernel" (-1 none | 0 s1 | 1 roll | 2 s1_tc |

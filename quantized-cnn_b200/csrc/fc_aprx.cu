@@ -352,9 +352,8 @@ __global__ void fc_prep_bf_kernel(const float* __restrict__ src, const int* __re
 // PACKED: the bit-packed table, rows of `pitch` bytes (PRE is then false: the kernel scales the unpacked index itself)
 template <int K, int CPT, int TN, int PF, bool PRE, bool PACKED>
 int Launch(const FcArgs& a, int pitch, dim3 grid, cudaStream_t st) {
-  const size_t xpad = (static_cast<size_t>(TN) * PF * a.d + 3) & ~static_cast<size_t>(3);
-  const size_t smem = sizeof(float) * (static_cast<size_t>(TN) * PF * K + 2 * xpad + 2 * static_cast<size_t>(PF) * K * a.d);
-  if (smem > 200 * 1024) {
+  const size_t smem = qcnn::FcGatherSmemBytes(K, TN, a.d);   // (PlanFcGather chose a TN that fits: this is a backstop)
+  if (smem > qcnn::kFcGatherSmemMax) {
     qcnn::SetError("qcnn_fc_aprx_forward: K=%d d=%d needs %zu bytes of shared memory per CTA", K, a.d, smem);
     return 1;
   }
@@ -480,10 +479,25 @@ int LaunchFcMode2(qcnn_layer* L, const FcPlan& p, const float* src, int N, float
   return LaunchPqGemmArgs(L->ctx, a, static_cast<long long>(CeilDiv(N, a.NT)) * a.nsplit * a.nct, st, L->asmt_bits, L->asmt_pitch);
 }
 
-// batch tile: 1 (latency path, 16 channels/thread, 128-bit loads), 4 or 8 images per CTA; fc_tn / fc_nsplit pin the tiling
-void PlanFcGather(const qcnn_layer* L, int N, FcPlan* p) {
+// [TN][PF][K] LUT slice + two buffers of the input slice (TN PF d floats, padded to 4) + two of the codebook rows (PF K d)
+size_t FcGatherSmemBytes(int K, int tn, int d) {
+  const size_t pf = FcChunkLen(K, tn);
+  const size_t xpad = (static_cast<size_t>(tn) * pf * d + 3) & ~static_cast<size_t>(3);
+  return sizeof(float) * (static_cast<size_t>(tn) * pf * K + 2 * xpad + 2 * pf * K * d);
+}
+
+// batch tile: 1 (latency path, 16 channels/thread, 128-bit loads), 4 or 8 images per CTA; fc_tn / fc_nsplit pin the tiling.
+// Unpinned, the tile is the widest that fits in shared memory (K = 256: tn = 8 up to d = 8, 4 up to d = 10, else 1).
+int PlanFcGather(const qcnn_layer* L, int N, FcPlan* p) {
   int tn = L->opt_fc_tn ? L->opt_fc_tn : (N >= 8 ? 8 : (N >= 4 ? 4 : 1));
   if (tn != 1 && tn != 4) tn = 8;
+  if (!L->opt_fc_tn)
+    while (tn > 1 && FcGatherSmemBytes(L->K, tn, L->d) > kFcGatherSmemMax) tn = tn == 8 ? 4 : 1;
+  if (FcGatherSmemBytes(L->K, tn, L->d) > kFcGatherSmemMax) {
+    SetError("qcnn_fc_aprx_forward: fc_tn=%d with K=%d d=%d needs %zu bytes of shared memory per CTA (limit %zu)", tn, L->K,
+             L->d, FcGatherSmemBytes(L->K, tn, L->d), kFcGatherSmemMax);
+    return 1;
+  }
   // narrow layers (fc8: 1000 outputs) take 4 channels per thread so that a 256-thread CTA is fully populated
   const int cpt = (tn == 1) ? 16 : ((tn == 8 && L->DoutPad <= 1024) ? 4 : 8);
   const int pf = FcChunkLen(L->K, tn);
@@ -498,6 +512,13 @@ void PlanFcGather(const qcnn_layer* L, int N, FcPlan* p) {
   const int chunks_per_split = CeilDiv(chunks, nsplit);
   p->nsplit = CeilDiv(chunks, chunks_per_split);
   p->gather = {tn, cpt, chunks_per_split * pf};
+  return 0;
+}
+
+// the tiling of a LUT + gather plan; describe() writes it after the layer's geometry (no " via ": the plain kernel)
+void DescribeFcGather(const qcnn_layer* L, const FcPlan& p, int, char* buf, size_t cap) {
+  snprintf(buf, cap, "gather(tn=%d cpt=%d pf=%d nsplit=%d)", p.gather.tn, p.gather.cpt, FcChunkLen(L->K, p.gather.tn),
+           p.nsplit);
 }
 
 int LaunchFcGather(qcnn_layer* L, const FcPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {

@@ -42,8 +42,7 @@ int PlanFc(const qcnn_layer* L, int N, FcPlan* p, bool withChain = true) {
   }
   if (tc && PlanFcMode2(L, N, p)) { p->kernel = kFcMode2; return 0; }
   p->kernel = kFcGather;
-  PlanFcGather(L, N, p);
-  return 0;
+  return PlanFcGather(L, N, p);
 }
 
 }  // namespace
@@ -71,15 +70,16 @@ int LaunchFc(qcnn_layer* L, const float* src, int N, float* dst, int relu, cudaS
   return 0;
 }
 
-// "fc_aprx Din=... [via <family's text>][ asmt=<b>bit]" for batch N (bench / DESIGN bookkeeping)
+// "fc_aprx Din=... [via <family's text> | gather(<tiling>)][ asmt=<b>bit]" for batch N (bench / DESIGN bookkeeping)
 int DescribeFc(qcnn_layer* L, int N, char* buf, size_t cap) {
   FcPlan p;
   if (int rc = PlanFc(L, N, &p)) return rc;
-  char via[256] = "", packed[16] = "";
+  char via[256] = "", gather[96] = "", packed[16] = "";
   if (kFamilies[p.kernel].describe) kFamilies[p.kernel].describe(L, p, N, via, sizeof(via));
+  if (p.kernel == kFcGather) DescribeFcGather(L, p, N, gather, sizeof(gather));
   if (L->asmt_bits) snprintf(packed, sizeof(packed), " asmt=%dbit", L->asmt_bits);
-  snprintf(buf, cap, "fc_aprx Din=%d Dout=%d S=%d K=%d d=%d%s%s%s", L->Din, L->Dout, L->S, L->K, L->d, via[0] ? " via " : "",
-           via, packed);
+  snprintf(buf, cap, "fc_aprx Din=%d Dout=%d S=%d K=%d d=%d%s%s%s%s%s", L->Din, L->Dout, L->S, L->K, L->d, via[0] ? " via " : "",
+           via, gather[0] ? " " : "", gather, packed);
   return 0;
 }
 

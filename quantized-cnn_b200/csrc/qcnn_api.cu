@@ -204,6 +204,11 @@ int qcnn_fc_layer_create(qcnn_ctx* ctx, int Din, int Dout, int S, int K, int d, 
   if (int rc = CheckPq("qcnn_fc_layer_create", S, K, d, asmt_h, static_cast<size_t>(Dout) * S)) return rc;
   QCNN_CHECK(K == 16 || K == 32 || K == 64 || K == 128 || K == 256,
              "qcnn_fc_layer_create: unsupported codebook size K=%d (supported: 16, 32, 64, 128, 256)", K);
+  // every batch size must have a kernel: the LUT + gather kernel (batches 5-95, tensor_core = 0, fc_* pins) stages the
+  // codebook rows of a chunk in shared memory, which bounds d (K = 256: d <= 11)
+  QCNN_CHECK(FcGatherSmemBytes(K, 1, d) <= kFcGatherSmemMax,
+             "qcnn_fc_layer_create: K=%d d=%d is not supported: the LUT + gather kernel would stage %zu bytes of shared memory "
+             "per CTA (limit %zu)", K, d, FcGatherSmemBytes(K, 1, d), kFcGatherSmemMax);
   QCNN_ON_DEVICE(ctx->device);
   qcnn_layer* L = NewLayer(ctx, QCNN_KIND_FC);
   L->Din = Din; L->Dout = Dout; L->S = S; L->K = K; L->d = d;

@@ -373,7 +373,13 @@ void DescribeFcWs(const qcnn_layer* L, const FcPlan& p, int N, char* buf, size_t
 bool PlanFcMode2(const qcnn_layer* L, int N, FcPlan* p);
 int LaunchFcMode2(qcnn_layer* L, const FcPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
 void DescribeFcMode2(const qcnn_layer* L, const FcPlan& p, int N, char* buf, size_t cap);
-void PlanFcGather(const qcnn_layer* L, int N, FcPlan* p);
+// LUT + gather: shared memory one CTA stages for K codewords, tn images per CTA and subspaces of d dims, and its limit.
+// PlanFcGather takes the widest batch tile that fits and fails when a pinned fc_tn does not; qcnn_fc_layer_create
+// refuses (K, d) where not even tn = 1 fits (K = 256: d <= 11).
+constexpr size_t kFcGatherSmemMax = 200 * 1024;
+size_t FcGatherSmemBytes(int K, int tn, int d);
+int PlanFcGather(const qcnn_layer* L, int N, FcPlan* p);
+void DescribeFcGather(const qcnn_layer* L, const FcPlan& p, int N, char* buf, size_t cap);
 int LaunchFcGather(qcnn_layer* L, const FcPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
 int PrepFcPlanes(qcnn_layer* L, const float* src, int N, int NT, int KS, int nChunksAll, bool bf, cudaStream_t st);
 int LaunchSplitReduce(qcnn_ctx* ctx, const float* partial, float* dst, int rows, int cols, int colsPad, int nsplit, int relu,

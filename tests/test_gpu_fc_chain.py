@@ -5,7 +5,9 @@ the CPU oracle.
 Tolerance: the kernel adds the same fp32 LUT entries as the reference (LUT entries bit-identical: separate rounded
 multiply and add, ascending j) but associates the sum differently -- per CTA s-ascending over its share (one CTA per SM) of the
 subspaces, then a fixed tree over the CTAs -- so results agree to fp32 re-association noise: RTOL = 1e-4 under the
-metric of test_gpu_layers.close (measured ~1e-6), and are bit-identical from run to run (no atomics)."""
+metric of test_gpu_layers.close (measured ~1e-6), and are bit-identical from run to run (no atomics).  The stricter check
+is test_gpu_fc_gather_chain.py: every branch of the kernel against a float64 bound propagated through the chain,
+(d + S + 3) U M per layer (measured worst err / bound 0.0098 on an H100 80GB HBM3 at 700 W)."""
 import numpy as np
 import pytest
 
