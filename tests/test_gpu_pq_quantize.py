@@ -74,6 +74,34 @@ def quantize(qcnn, ctx, w, K, d, **kw):
     return (qcnn.pq_quantize_conv if w.ndim == 4 else qcnn.pq_quantize_fc)(ctx, w, K, d, **kw)
 
 
+# ---- which assignment kernel a shape runs (PickAssign / PadDims in pq_quantize.cu) ------------------------------------
+ASSIGN_THREADS = 128
+UPDATE_CHUNK = 1024   # points per CTA of the update's partial sums
+ASSIGN_KERNELS = {(D, R) for D in (4, 8, 16) for R in (8, 4, 2)} | {(32, 4), (32, 2), (64, 2)}   # the 12 instantiations
+
+
+def pad_dims(w):
+    D = 4
+    while D < w:
+        D *= 2
+    return D
+
+
+def points(shape):
+    """points per subspace: Cout k^2 (FC: Dout)"""
+    return shape[0] * (shape[2] * shape[3] if len(shape) == 4 else 1)
+
+
+def assign_plan(shape, d, sm_count):
+    """(D, R) of the pq_assign_kernel<D, R> that weights of `shape` at subspace width d run on sm_count SMs"""
+    Cg, P = shape[1], points(shape)
+    S, D = -(-Cg // d), pad_dims(min(d, Cg))
+    R = 8 if D <= 16 else 128 // D
+    while R > 2 and S * -(-P // (ASSIGN_THREADS * R)) < 2 * sm_count:
+        R //= 2
+    return D, R
+
+
 # (name, weight shape, K, d)
 CASES = [
     ("conv1", (96, 3, 11, 11), 128, 8),      # d > Cg: one partial subspace of 3 dims
@@ -82,6 +110,25 @@ CASES = [
     ("fc_d1", (300, 40), 16, 1),
     ("fc_d4", (200, 30), 32, 4),             # Din % d = 2
 ]
+# One row per assignment kernel (D, R), on 114 and on 132 SMs alike (test_assign_rows_cover_every_kernel).  Every row
+# has a partial last CTA of points and a partial last update chunk, and a partial last subspace where d > 1.  Rows at
+# d = 16 and d = 32 fill D, so the last float4 of a point carries data; the d = 12 and d = 24 rows leave it padding.
+ASSIGN_CASES = [
+    ("fc_D4_R8", (2500, 602), 32, 4),
+    ("fc_D4_R4", (1500, 402), 32, 4),
+    ("fc_D4_R2", (300, 130), 32, 4),
+    ("fc_D8_R8", (2500, 1202), 32, 8),
+    ("fc_D8_R4", (1500, 802), 32, 8),
+    ("fc_D8_R2", (300, 130), 32, 8),
+    ("fc_D16_R8", (2500, 1450), 32, 16),
+    ("fc_D16_R4", (1500, 1210), 32, 12),
+    ("fc_D16_R2", (300, 250), 32, 16),
+    ("fc_D16_R2_d12", (300, 130), 32, 12),
+    ("fc_D32_R4", (1500, 3210), 32, 32),
+    ("fc_D32_R2", (300, 250), 32, 24),
+    ("fc_D64_R2", (300, 250), 32, 64),
+]
+CASES += ASSIGN_CASES
 
 
 def weights(shape, seed):
@@ -96,6 +143,33 @@ def test_quantize_symbols_declared_and_exported(qcnn):
         assert re.search(r"QCNN_API\s+int\s+%s\s*\(" % name, text), name
         assert hasattr(lib, name), name
         assert name in qcnn.EXPORTS
+
+
+def assign_coverage(sm_count):
+    """{(D, R): names of the ASSIGN_CASES rows that run it}; asserts every row's point and subspace tails"""
+    out = {}
+    for name, shape, K, d in ASSIGN_CASES:
+        D, R = assign_plan(shape, d, sm_count)
+        P, Cg = points(shape), shape[1]
+        assert P % (ASSIGN_THREADS * R) and P % UPDATE_CHUNK, (name, sm_count)   # partial last CTA and update chunk
+        assert d == 1 or Cg % d, name                                           # partial last subspace
+        out.setdefault((D, R), []).append(name)
+    return out
+
+
+@pytest.mark.parametrize("sm_count", [132, 114])
+def test_assign_rows_cover_every_kernel(sm_count):
+    cov = assign_coverage(sm_count)
+    print("sm_count %d: %s" % (sm_count, ", ".join("D=%d R=%d: %s" % (D, R, "/".join(n)) for (D, R), n in sorted(cov.items()))))
+    assert set(cov) == ASSIGN_KERNELS
+    for D in (16, 32):   # subspaces that fill D, and subspaces that leave the last float4 padding
+        ds = {d for _, shape, _, d in ASSIGN_CASES if assign_plan(shape, d, sm_count)[0] == D}
+        assert D in ds and any(d <= D - 4 for d in ds), (D, ds)
+
+
+@pytest.mark.gpu
+def test_assign_rows_cover_every_kernel_on_this_gpu(ctx):
+    assert set(assign_coverage(ctx.sm_count)) == ASSIGN_KERNELS, ctx.sm_count
 
 
 # ---- exact steps --------------------------------------------------------------------------------------------------

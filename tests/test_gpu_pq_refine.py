@@ -15,15 +15,33 @@ def decoded(ctrd, asmt, Din):
     return decode(dict(ctrd=ctrd, asmt=asmt), Din)
 
 
-def refine_ref(W, X, ctrd, asmt, sweeps):
-    """(ctrd, asmt) after `sweeps` sweeps; asserts the margins that make the device comparison exact: every argmin's best
-    and second best differ by more than 1e-6 of the terms' scale, and every accept-or-keep decision of the codebook step
-    with D != c_k has |f(D) - f(c_k)| above 1e-9 of the terms' scale."""
+def follow_argmin(v, two, margin, m, follow):
+    """Per row of v the argmin, except that a row whose best and second best differ by at most `margin` takes the
+    device's index follow[1][:, m], which must lie within `margin` of the best.  Returns (indices, rows inside)."""
+    a = np.argmin(v, axis=1)
+    inside = (two[:, 1] - two[:, 0]) <= margin
+    if inside.any():
+        assert follow is not None, ("argmin inside its margin", m, np.nonzero(inside)[0])
+        ad = follow[1][inside, m].astype(np.int64)
+        assert (v[inside, ad] - two[inside, 0] <= margin[inside]).all(), m
+        a[inside] = ad
+    return a, int(inside.sum())
+
+
+def refine_ref(W, X, ctrd, asmt, sweeps, follow=None):
+    """(ctrd, asmt, inside) after `sweeps` sweeps.  A decision is exact outside its margin: an argmin whose best and
+    second best differ by more than 1e-6 of the terms' scale, an accept-or-keep decision of the codebook step with
+    D != c_k and |f(D) - f(c_k)| above 1e-9 of the terms' scale.  A decision inside its margin needs `follow`, the
+    device's (ctrd, asmt) after one sweep, in which every codeword and assignment is decided once: the device's choice
+    must be one of the options inside the margin (an index within the gap, a codeword within 1 ulp of D or of c_k), and
+    the restatement continues with it.  `inside` counts those decisions."""
+    assert follow is None or sweeps == 1
     X = X.astype(np.float64)
     G = X.T @ X
     Dout, Din = W.shape
     S, K, d = ctrd.shape
     ctrd, asmt = ctrd.copy(), asmt.copy()
+    inside = 0
     for _ in range(sweeps):
         for m in range(S):
             c0, w = m * d, min(d, Din - m * d)
@@ -47,7 +65,13 @@ def refine_ref(W, X, ctrd, asmt, sweeps):
                 fD, fc = f(D.astype(np.float64)), f(c.astype(np.float64))
                 if not np.array_equal(D, c):
                     scale = n * abs(D @ Gmm @ D) + n * abs(c @ Gmm @ c) + 2 * abs(D @ H) + 2 * abs(c @ H)
-                    assert abs(fD - fc) > 1e-9 * scale, (m, k, fD, fc)
+                    if abs(fD - fc) <= 1e-9 * scale:
+                        assert follow is not None, ("accept-or-keep inside its margin", m, k, fD, fc)
+                        got = follow[0][m, k, :w]
+                        assert ulps(got, D).max() <= 1.0 or ulps(got, c).max() <= 1.0, (m, k)
+                        ctrd[m, k, :w] = got
+                        inside += 1
+                        continue
                 if fD < fc:
                     ctrd[m, k, :w] = D
             Cm = ctrd[m, :, :w].astype(np.float64)
@@ -56,9 +80,9 @@ def refine_ref(W, X, ctrd, asmt, sweeps):
             v = cc[None, :] - 2 * dot
             two = np.sort(v, axis=1)[:, :2]
             scale = np.abs(cc).max() + 2 * np.abs(dot).max(axis=1)
-            assert ((two[:, 1] - two[:, 0]) > 1e-6 * scale).all(), m
-            asmt[:, m] = np.argmin(v, axis=1)
-    return ctrd, asmt
+            asmt[:, m], n_in = follow_argmin(v, two, 1e-6 * scale, m, follow)
+            inside += n_in
+    return ctrd, asmt, inside
 
 
 def response_loss(W, X, ctrd, asmt):
@@ -100,42 +124,76 @@ def test_refine_symbol_declared_and_exported(qcnn):
 
 
 # ---- sweeps = 0: the starting point and its loss -------------------------------------------------------------------
-# (name, Din, Dout, K, d, N, zero input columns)
+# (name, Din, Dout, K, d, N, first zero input column, zero input columns)
 ZERO_SWEEP = [
-    ("d1", 40, 300, 16, 1, 64, 0),
-    ("d4_partial", 30, 200, 32, 4, 50, 0),        # Din % d = 2
-    ("d64_k256", 100, 64, 256, 64, 120, 0),       # subspaces of 64 and 36 dims
-    ("n1", 48, 32, 16, 4, 1, 0),
-    ("singular", 96, 64, 32, 4, 40, 10),          # N < Din, ten zero columns: G_mm singular, whole subspaces skipped
+    ("d1", 40, 300, 16, 1, 64, 20, 0),
+    ("d4_partial", 30, 200, 32, 4, 50, 20, 0),        # Din % d = 2
+    ("d64_k256", 100, 64, 256, 64, 120, 20, 0),       # subspaces of 64 and 36 dims
+    ("n1", 48, 32, 16, 4, 1, 20, 0),
+    ("singular", 96, 64, 32, 4, 40, 20, 10),          # N < Din, ten zero columns: G_mm singular, whole subspaces skipped
+    ("singular_block2", 700, 301, 32, 4, 200, 300, 41),   # skipped subspaces 75..84 in the second block of 64
 ]
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,Din,Dout,K,d,N,zeros", ZERO_SWEEP, ids=[c[0] for c in ZERO_SWEEP])
-def test_zero_sweeps_return_the_start_and_its_loss(name, Din, Dout, K, d, N, zeros, qcnn, ctx):
+@pytest.mark.parametrize("name,Din,Dout,K,d,N,z0,zeros", ZERO_SWEEP, ids=[c[0] for c in ZERO_SWEEP])
+def test_zero_sweeps_return_the_start_and_its_loss(name, Din, Dout, K, d, N, z0, zeros, qcnn, ctx):
     W, ctrd, asmt = start(Din, Dout, K, d, 11)
     X = gaussian_inputs(N, Din, 12)
-    X[:, 20:20 + zeros] = 0
+    X[:, z0:z0 + zeros] = 0
     c, a, loss = qcnn.pq_refine_fc(ctx, W, cuda(X), ctrd, asmt, sweeps=0)
     assert c.tobytes() == ctrd.tobytes() and a.tobytes() == asmt.tobytes()
     assert loss.shape == (1,)
     want = response_loss(W, X, ctrd, asmt)
     assert abs(loss[0] - want) <= 1e-10 * want, (loss[0], want)
-    if zeros:   # a skipped subspace keeps everything even in a sweep
-        c1, a1, _ = qcnn.pq_refine_fc(ctx, W, cuda(X), ctrd, asmt, sweeps=1)
-        skipped = [m for m in range(-(-Din // d)) if 20 <= m * d and (m + 1) * d <= 20 + zeros]
+    if zeros:   # a skipped subspace keeps everything even in a sweep, and the others still lower the loss
+        c1, a1, l1 = qcnn.pq_refine_fc(ctx, W, cuda(X), ctrd, asmt, sweeps=1)
+        skipped = [m for m in range(-(-Din // d)) if z0 <= m * d and (m + 1) * d <= z0 + zeros]
         assert skipped
         assert np.array_equal(c1[skipped], ctrd[skipped]) and np.array_equal(a1[:, skipped], asmt[:, skipped])
+        want = response_loss(W, X, c1, a1)
+        assert abs(l1[1] - want) <= 1e-9 * want, (l1[1], want)
+        assert l1[1] <= l1[0]
 
 
 # ---- one sweep against the restatement -----------------------------------------------------------------------------
-# (name, Din, Dout, K, d, seed): seeds whose argmins and accept-or-keep decisions all clear the restatement's margins
+BLOCK_DIMS = 256   # dims per cooperative launch of the sweep: floor(256 / d) subspaces (pq_refine.cu)
+
+
+def blocks(Din, d):
+    """subspaces per block of one sweep"""
+    S, spb = -(-Din // d), max(1, BLOCK_DIMS // d)
+    return [min(spb, S - m0) for m0 in range(0, S, spb)]
+
+
+# (name, Din, Dout, K, d, seed).  The block rows span three blocks with a partial last one.  With the sweep kernel's grid
+# of min(2 x SMs, max(Dout, K)) CTAs (264 on 132 SMs, 228 on 114), Dout = 701 gives each CTA several outputs and the
+# last CTA with outputs a partial range, and Dout = 200 < K = 256 leaves CTAs without outputs.
 ONE_SWEEP = [
     ("d1", 24, 300, 16, 1, 22),
     ("d4_partial", 250, 200, 32, 4, 21),
     ("d8_k64", 256, 256, 64, 8, 21),
     ("d64_k256", 160, 128, 256, 64, 21),
+    ("d4_blocks", 610, 701, 32, 4, 23),        # 64 + 64 + 25 subspaces, the last of 2 dims
+    ("d12_blocks", 610, 701, 32, 12, 23),      # 21 + 21 + 9 subspaces (252 dims a block: the trailing GEMM's K % 16 = 12)
+    ("d1_blocks", 600, 701, 32, 1, 23),        # 256 + 256 + 88 subspaces
+    ("d64_blocks", 600, 200, 256, 64, 23),     # 4 + 4 + 2 subspaces, the last of 24 dims; Dout < K
 ]
+
+
+def test_block_rows_cross_blocks():
+    """Two sweep CTAs fit on an SM at every row's shared memory, so the grid is min(2 x SMs, max(Dout, K))."""
+    for name, Din, Dout, K, d, seed in ONE_SWEEP:
+        b = blocks(Din, d)
+        print("%s: blocks of %s subspaces, the last subspace %d dims" % (name, b, Din - (-(-Din // d) - 1) * d))
+        if name.endswith("_blocks"):
+            assert len(b) >= 3 and b[-1] < b[0], name
+            assert d == 1 or Din % d, name
+            for sm in (132, 114):
+                grid = min(2 * sm, max(Dout, K))
+                R = -(-Dout // grid)
+                assert grid > Dout if Dout < K else (R >= 2 and Dout % R), (name, sm)
+    assert {tuple(blocks(Din, d)) for _, Din, _, _, d, _ in ONE_SWEEP} >= {(64, 64, 25), (21, 21, 9), (256, 256, 88), (4, 4, 2)}
 
 
 @pytest.mark.gpu
@@ -143,11 +201,31 @@ ONE_SWEEP = [
 def test_one_sweep_matches_restatement(name, Din, Dout, K, d, seed, qcnn, ctx):
     W, ctrd, asmt = start(Din, Dout, K, d, seed)
     X = gaussian_inputs(2 * Din, Din, seed + 1)
-    want_c, want_a = refine_ref(W, X, ctrd, asmt, 1)
     c, a, loss = qcnn.pq_refine_fc(ctx, W, cuda(X), ctrd, asmt, sweeps=1)
+    want_c, want_a, inside = refine_ref(W, X, ctrd, asmt, 1, follow=(c, a))
+    print("%s: %d blocks, %d of %d assignments and codewords decided inside their margins"
+          % (name, len(blocks(Din, d)), inside, a.size + ctrd.shape[0] * K))
     assert ulps(c, want_c).max() <= 1.0
     assert np.array_equal(a, want_a)
     assert loss[1] <= loss[0]
+    want = response_loss(W, X, c, a)
+    assert abs(loss[1] - want) <= 1e-9 * want, (loss[1], want)
+
+
+@pytest.mark.gpu
+def test_every_sweeps_loss(qcnn, ctx):
+    Din, Dout, K, d = 610, 701, 32, 4
+    W, ctrd, asmt = start(Din, Dout, K, d, 24)
+    X = gaussian_inputs(2 * Din, Din, 25)
+    x = cuda(X)
+    prev = np.zeros(0)
+    for sweeps in (1, 2, 3):
+        c, a, loss = qcnn.pq_refine_fc(ctx, W, x, ctrd, asmt, sweeps=sweeps)
+        assert loss.shape == (sweeps + 1,)
+        assert loss[:len(prev)].tobytes() == prev.tobytes(), (sweeps, loss, prev)
+        want = response_loss(W, X, c, a)
+        assert abs(loss[-1] - want) <= 1e-9 * want, (sweeps, loss[-1], want)
+        prev = loss
 
 
 @pytest.mark.gpu

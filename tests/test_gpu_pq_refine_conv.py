@@ -40,23 +40,61 @@ def patches(X, g, Cg, k, pad, stride):
     return P.reshape(N * Ho * Wo, Cg * k * k)
 
 
-def refine_ref(W, X, ctrd, asmt, pad, stride, grp, sweeps):
-    """(ctrd, asmt) after `sweeps` sweeps; asserts the margins that make the device comparison exact: every argmin's best
-    and second best differ by more than 1e-6 of the terms' scale, and every accept-or-keep decision with D != C has
-    |f(D) - f(C)| above 1e-9 of the terms' scale."""
+def grams(X, Cg, k, pad, stride, grp, d):
+    """per group the fp64 patch Gram G_g in the internal dim order, from numpy patches"""
+    perm = dim_order(Cg, d, k * k)
+    G = []
+    for g in range(grp):
+        P = patches(X.astype(np.float64), g, Cg, k, pad, stride)[:, perm]
+        G.append(P.T @ P)
+    return G
+
+
+def grams_torch(x, Cg, k, pad, stride, grp, d, batch):
+    """The same from maps x [N][H][W][Cin] on the GPU: fp64 F.unfold over `batch` images at a time, accumulated.  For
+    layers whose fp64 patches are too large to build in numpy; it sums in another order than the device, so the two
+    differ in the last bits, which the restatement's margins absorb."""
+    import torch
+    import torch.nn.functional as F
+    Dg = Cg * k * k
+    perm = torch.from_numpy(dim_order(Cg, d, k * k)).to(x.device)
+    G = [torch.zeros((Dg, Dg), dtype=torch.float64, device=x.device) for _ in range(grp)]
+    for i in range(0, x.shape[0], batch):
+        xb = x[i:i + batch].permute(0, 3, 1, 2).double()
+        for g in range(grp):
+            P = F.unfold(xb[:, g * Cg:(g + 1) * Cg], k, padding=pad, stride=stride)   # [n][Cg k k][positions]
+            P = P.permute(0, 2, 1).reshape(-1, Dg)[:, perm]
+            G[g] += P.T @ P
+    return [Gg.cpu().numpy() for Gg in G]
+
+
+def system_sizes(Cg, d, T, asmt):
+    """n = |U| w_m of every subspace's joint codebook system in the first sweep (U: the start's used clusters)"""
+    S = -(-Cg // d)
+    A = asmt.reshape(-1, T, S)
+    return [len(np.unique(A[:, :, m])) * min(d, Cg - m * d) for m in range(S)]
+
+
+def sweep_ref(W, G, ctrd, asmt, grp, sweeps, follow=None):
+    """(ctrd, asmt, stats) after `sweeps` sweeps from the Grams G (grams / grams_torch).  A decision is exact outside its
+    margin: an argmin whose best and second best differ by more than 1e-6 of the terms' scale, an accept-or-keep
+    decision with D != C and |f(D) - f(C)| above 1e-9 of the terms' scale.  A decision inside its margin needs
+    `follow`, the device's (ctrd, asmt) after one sweep, in which every codebook and assignment is decided once: the
+    device's choice must be one of the options inside the margin (an index within the gap, a codebook within 1 ulp of
+    D or of C), and the restatement continues with it.  stats: "inside" counts those decisions, "n" lists the size
+    |U| w_m of every subspace's system."""
+    assert follow is None or sweeps == 1
     Cout, Cg, k, _ = W.shape
     T = k * k
     S, K, d = ctrd.shape
     Cpg, Dg = Cout // grp, Cg * T
     perm = dim_order(Cg, d, T)
-    G = []
-    for g in range(grp):
-        P = patches(X.astype(np.float64), g, Cg, k, pad, stride)[:, perm]
-        G.append(P.T @ P)
     Wq = W.reshape(Cout, Dg)[:, perm].astype(np.float64)
     ctrd, asmt = ctrd.copy(), asmt.copy()
     A = asmt.reshape(Cout, T, S)
+    FA = None if follow is None else follow[1].reshape(Cout, T, S)
     grp_of = np.arange(Cout) // Cpg
+    stats = {"inside": 0, "n": []}
 
     def decoded():
         return decode(dict(ctrd=ctrd, asmt=asmt), Cg).reshape(Cout, Dg)[:, perm].astype(np.float64)
@@ -73,7 +111,7 @@ def refine_ref(W, X, ctrd, asmt, pad, stride, grp, sweeps):
             h = np.empty((Cout, nb))
             for g in range(grp):
                 og = grp_of == g
-                h[og] = (E[og] @ G[g])[:, blk] + Wh[og][:, blk] @ G[g][blk, blk]
+                h[og] = E[og] @ G[g][:, blk] + Wh[og][:, blk] @ G[g][blk, blk]
             h = h.reshape(Cout, T, w)
             Am = A[:, :, m].astype(np.int64)
             U = np.nonzero(np.bincount(Am.ravel(), minlength=K))[0]
@@ -92,6 +130,7 @@ def refine_ref(W, X, ctrd, asmt, pad, stride, grp, sweeps):
                     vals = cnt[:, None, None].astype(np.float64) * Gb[t][:, t2, :].transpose(1, 0, 2)
                     np.add.at(M4, (u[:, None, None], jj[None, :, None], u2[:, None, None], jj[None, None, :]), vals)
             n = nU * w
+            stats["n"].append(n)
             M = M4.reshape(n, n)
             b = np.zeros((nU, w))
             np.add.at(b, uidx[Am.ravel()], h.reshape(-1, w))
@@ -102,10 +141,14 @@ def refine_ref(W, X, ctrd, asmt, pad, stride, grp, sweeps):
             Cu = ctrd[m, U, :w].ravel()
             Dd, Cd = D.astype(np.float64), Cu.astype(np.float64)
             diff = (Dd - Cd) @ (M @ (Dd + Cd) - 2 * b)
-            if not np.array_equal(D, Cu):
-                scale = abs(Dd @ M @ Dd) + abs(Cd @ M @ Cd) + 2 * abs(Dd @ b) + 2 * abs(Cd @ b)
-                assert abs(diff) > 1e-9 * scale, (m, diff, scale)
-            if diff < 0:
+            scale = abs(Dd @ M @ Dd) + abs(Cd @ M @ Cd) + 2 * abs(Dd @ b) + 2 * abs(Cd @ b)
+            if not np.array_equal(D, Cu) and abs(diff) <= 1e-9 * scale:
+                assert follow is not None, ("accept-or-keep inside its margin", m, diff, scale)
+                got = follow[0][m, U, :w].ravel()
+                assert ulps(got, D).max() <= 1.0 or ulps(got, Cu).max() <= 1.0, m
+                ctrd[m, U, :w] = got.reshape(nU, w)
+                stats["inside"] += 1
+            elif diff < 0:
                 ctrd[m, U, :w] = D.reshape(nU, w)
             # assignment, taps in order, E current
             E = Wq - decoded()
@@ -122,21 +165,35 @@ def refine_ref(W, X, ctrd, asmt, pad, stride, grp, sweeps):
                     dot = Cm @ hp
                     v = cc - 2 * dot
                     two = np.sort(v)[:2]
-                    scale = np.abs(cc).max() + 2 * np.abs(dot).max()
-                    assert two[1] - two[0] > 1e-6 * scale, (m, o, t)
-                    a = int(np.argmin(v))
+                    margin = 1e-6 * (np.abs(cc).max() + 2 * np.abs(dot).max())
+                    if two[1] - two[0] <= margin:
+                        assert follow is not None, ("argmin inside its margin", m, o, t)
+                        a = int(FA[o, t, m])
+                        assert v[a] - two[0] <= margin, (m, o, t)
+                        stats["inside"] += 1
+                    else:
+                        a = int(np.argmin(v))
                     A[o, t, m] = a
                     E[o, r] = Wq[o, r] - Cm[a]
-    return ctrd, asmt
+    return ctrd, asmt, stats
+
+
+def refine_ref(W, X, ctrd, asmt, pad, stride, grp, sweeps, follow=None):
+    """sweep_ref from the numpy Grams of the maps X"""
+    S, K, d = ctrd.shape
+    return sweep_ref(W, grams(X, W.shape[1], W.shape[2], pad, stride, grp, d), ctrd, asmt, grp, sweeps, follow)
 
 
 def response_loss(W, X, ctrd, asmt, pad, stride, grp):
-    """sum conv(x, W - W^)^2 from the maps themselves (torch, fp64, CPU)"""
+    """sum conv(x, W - W^)^2 from the maps themselves (torch, fp64; on the GPU when X is a CUDA tensor, else the CPU)"""
     import torch
     import torch.nn.functional as F
-    dW = W.astype(np.float64) - decode(dict(ctrd=ctrd, asmt=asmt), W.shape[1])
-    x = torch.from_numpy(np.ascontiguousarray(X, np.float64)).permute(0, 3, 1, 2)
-    y = F.conv2d(x, torch.from_numpy(dW), stride=stride, padding=pad, groups=grp)
+    dW = torch.from_numpy(W.astype(np.float64) - decode(dict(ctrd=ctrd, asmt=asmt), W.shape[1]))
+    if isinstance(X, torch.Tensor):
+        x, dW = X.double().permute(0, 3, 1, 2), dW.to(X.device)
+    else:
+        x = torch.from_numpy(np.ascontiguousarray(X, np.float64)).permute(0, 3, 1, 2)
+    y = F.conv2d(x, dW, stride=stride, padding=pad, groups=grp)
     return float((y * y).sum())
 
 
@@ -207,26 +264,89 @@ def test_zero_input_channels_skip_their_subspaces(qcnn, ctx):
 
 
 # ---- one sweep against the restatement -----------------------------------------------------------------------------
-# (name, Cin, H, Cout, k, pad, stride, grp, K, d, N, seed): seeds whose decisions all clear the restatement's margins
+PATCH_BYTES = 256 << 20   # one chunk of one group's fp32 patches (pq_refine_conv.cu)
+
+
+def patch_chunks(N, H, k, pad, stride, Cg):
+    """chunks of output positions the device's Gram of one group is accumulated over"""
+    positions, Dg = N * out_size(H, k, pad, stride) ** 2, Cg * k * k
+    return -(-positions // max(1, min(positions, PATCH_BYTES // (4 * Dg))))
+
+
+# (name, Cin, H, Cout, k, pad, stride, grp, K, d, N, seed).  The chunked rows' patches span several chunks per group,
+# the last partial; their Grams come from grams_torch, since fp64 numpy patches that large do not fit.
 ONE_SWEEP = [
     ("1x1", 24, 6, 48, 1, 0, 1, 1, 16, 8, 4, 21),
     ("3x3_grp2_partial", 20, 9, 32, 3, 1, 1, 2, 16, 4, 3, 21),   # Cg = 10, d = 4
     ("5x5_s2_p2", 12, 11, 24, 5, 2, 2, 1, 32, 4, 4, 21),
     ("conv1_like", 3, 63, 32, 11, 0, 4, 1, 128, 8, 6, 21),        # w = 3, K = 128
     ("kw_2048", 8, 6, 160, 3, 1, 1, 1, 256, 8, 6, 21),            # K w = 2048
+    ("chunked_conv1", 3, 227, 96, 11, 0, 4, 1, 128, 8, 128, 21),  # AlexNet conv1: 387 200 positions, 184 872 a chunk
+    ("chunked_grp2", 464, 32, 32, 3, 1, 1, 2, 16, 8, 100, 21),    # Dg = 2088: 102 400 positions, 32 140 a chunk
 ]
+
+
+def test_rows_cover_chunks_and_cholesky_panels():
+    """Every row's first-sweep system sizes n = |U| w_m (from the start alone: subspace m's assignments are still the
+    start's when its codebook is solved) reach a single panel (n < 64), whole panels, a partial last panel and more
+    than 16 panels; the chunked rows reach three and four patch chunks per group."""
+    ns, chunked = [], set()
+    for name, Cin, H, Cout, k, pad, stride, grp, K, d, N, seed in ONE_SWEEP:
+        _, _, asmt = start(Cout, Cin // grp, k, K, d, seed)
+        n = system_sizes(Cin // grp, d, k * k, asmt)
+        chunks = patch_chunks(N, H, k, pad, stride, Cin // grp)
+        print("%s: %d patch chunks per group, systems n = %s" % (name, chunks, n))
+        assert (chunks >= 3) == name.startswith("chunked"), name
+        if chunks > 1:
+            chunked.add(chunks)
+        ns += n
+    assert chunked == {3, 4}, chunked
+    assert min(ns) < 64, ns
+    assert any(n % 64 == 0 for n in ns), ns
+    assert any(n > 64 and n % 64 for n in ns), ns
+    assert max(ns) > 1024, ns
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,Cin,H,Cout,k,pad,stride,grp,K,d,N,seed", ONE_SWEEP, ids=[c[0] for c in ONE_SWEEP])
 def test_one_sweep_matches_restatement(name, Cin, H, Cout, k, pad, stride, grp, K, d, N, seed, qcnn, ctx):
-    W, ctrd, asmt = start(Cout, Cin // grp, k, K, d, seed)
+    Cg = Cin // grp
+    W, ctrd, asmt = start(Cout, Cg, k, K, d, seed)
     X = maps(N, H, H, Cin, seed + 1)
-    want_c, want_a = refine_ref(W, X, ctrd, asmt, pad, stride, grp, 1)
-    c, a, loss = qcnn.pq_refine_conv(ctx, W, cuda(X), ctrd, asmt, pad=pad, stride=stride, grp=grp, sweeps=1)
+    x = cuda(X)
+    chunked = patch_chunks(N, H, k, pad, stride, Cg) > 1
+    if chunked:   # the chunked Gram alone, against the response loss
+        c0, a0, l0 = qcnn.pq_refine_conv(ctx, W, x, ctrd, asmt, pad=pad, stride=stride, grp=grp, sweeps=0)
+        assert c0.tobytes() == ctrd.tobytes() and a0.tobytes() == asmt.tobytes()
+        want = response_loss(W, x, ctrd, asmt, pad, stride, grp)
+        assert abs(l0[0] - want) <= 1e-10 * want, (l0[0], want)
+        G = grams_torch(x, Cg, k, pad, stride, grp, d, batch=max(1, (64 << 20) // (8 * Cg * k * k * out_size(H, k, pad, stride) ** 2)))
+    else:
+        G = grams(X, Cg, k, pad, stride, grp, d)
+    c, a, loss = qcnn.pq_refine_conv(ctx, W, x, ctrd, asmt, pad=pad, stride=stride, grp=grp, sweeps=1)
+    want_c, want_a, stats = sweep_ref(W, G, ctrd, asmt, grp, 1, follow=(c, a))
+    print("%s: systems n = %s, %d of %d decisions inside their margins"
+          % (name, stats["n"], stats["inside"], a.size + len(stats["n"])))
+    assert stats["n"] == system_sizes(Cg, d, k * k, asmt)
     assert ulps(c, want_c).max() <= 1.0
     assert np.array_equal(a, want_a)
     assert loss[1] <= loss[0]
+
+
+@pytest.mark.gpu
+def test_every_sweeps_loss(qcnn, ctx):
+    Cin, H, Cout, k, pad, stride, grp, K, d, N = 20, 9, 32, 3, 1, 1, 2, 16, 4, 3
+    W, ctrd, asmt = start(Cout, Cin // grp, k, K, d, 24)
+    X = maps(N, H, H, Cin, 25)
+    x = cuda(X)
+    prev = np.zeros(0)
+    for sweeps in (1, 2, 3):
+        c, a, loss = qcnn.pq_refine_conv(ctx, W, x, ctrd, asmt, pad=pad, stride=stride, grp=grp, sweeps=sweeps)
+        assert loss.shape == (sweeps + 1,)
+        assert loss[:len(prev)].tobytes() == prev.tobytes(), (sweeps, loss, prev)
+        want = response_loss(W, X, c, a, pad, stride, grp)
+        assert abs(loss[-1] - want) <= 1e-9 * want, (sweeps, loss[-1], want)
+        prev = loss
 
 
 def unit_patch_maps(Cg, k, grp):
