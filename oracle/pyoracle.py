@@ -373,8 +373,10 @@ def save_model(dirpath, pfx, params):
 # whole-network oracle (the port): CaffeEva::ExecForwardPass(img, prob), src/CaffeEva.cc:213-261
 # ------------------------------------------------------------------------------------------------
 def net_forward(layers, params, img_nchw, keep=False):
-    """Returns probs [N, C] (and, with keep=True, the list featMapLst[0..L] in the reference's element order)."""
+    """Returns probs [N, C] (and, with keep=True, the list featMapLst[0..L] in NHWC element order; the reference leaves
+    the first FC layer's input in NCHW element order)."""
     x = nchw_to_nhwc(img_nchw)
+    shapes = infer_shapes(layers, img_nchw.shape[1:])
     maps = [x]
     first_fc = True
     for l, L in enumerate(layers):
@@ -384,8 +386,10 @@ def net_forward(layers, params, img_nchw, keep=False):
             x = conv_aprx(x, L, p["ctrd"], p["asmt"], p["bias"])
         elif t == FCNT:
             p = params[l]
-            if first_fc and x.ndim == 4:
-                x = nhwc_to_nchw(x)  # CaffeEva.cc:236-238
+            if first_fc:
+                # CaffeEva.cc:236-238 permutes the first FC layer's input whatever produced it: a softmax map keeps its
+                # input's H x W x C (PrepFeatMap, CaffeEva.cc:385-386) although it is held here as [N, H*W*C]
+                x = nhwc_to_nchw(x.reshape((x.shape[0],) + tuple(shapes[l])))
             first_fc = False
             x = fc_aprx(x.reshape(x.shape[0], -1), p["ctrd"], p["asmt"], p["bias"])
         elif t == RELU:
