@@ -236,7 +236,8 @@ QCNN_API qcnn_layer* qcnn_net_pq_layer(qcnn_net* net, int l);
 
 /* ---- image entry and result exit on the device (SURVEY.md 8(f1), 8(f2)) -------------------------------------------
  * k-fold arg-max of N rows of C values: first maximum wins, winner zeroed (mode: see qcnn_net_forward_topk_h);
- * idx [N][k] int32, val [N][k], device */
+ * 1 <= k <= C <= 12000.  NaNs follow the reference scans: mode 0 returns (0, NaN) for a row starting with NaN and
+ * otherwise skips them, mode 1 always skips them.  idx [N][k] int32, val [N][k], device */
 QCNN_API int qcnn_topk(qcnn_ctx* ctx, const float* prob, int N, int C, int k, int mode, int* idx, float* val, void* stream);
 /* src u8 [N][H][W][C] -> dst f32 [N][C][H][W] minus mean [C][H][W] (nullable), device */
 QCNN_API int qcnn_u8hwc_to_f32chw(qcnn_ctx* ctx, const uint8_t* src, const float* mean, float* dst, int N, int C, int H, int W,
@@ -250,7 +251,8 @@ QCNN_API void qcnn_preproc_destroy(qcnn_preproc* p);
 /* == BmpImgIO::Load after the file decode -- ReszImg, RmMeanImg, CropImg (src/BmpImgIO.cc:105-224) -- for N decoded
  * images in one launch, bit-identical to the CPU path: pix (device) holds the images' interleaved B, G, R bytes, top row
  * first, image i of hei_h[i] x wid_h[i] pixels starting at byte off_h[i] (host arrays); dst [N][3][hei_crop][wid_crop]
- * f32 NCHW (device), what ExecForwardPass takes */
+ * f32 NCHW (device), what ExecForwardPass takes.  Runs of one object on one stream are ordered; one object must not
+ * run on two streams at once (they share its descriptor buffer) */
 QCNN_API int qcnn_preproc_run(qcnn_preproc* p, const uint8_t* pix, const long long* off_h, const int* hei_h, const int* wid_h,
                               int N, float* dst, void* stream);
 

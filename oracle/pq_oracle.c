@@ -337,6 +337,22 @@ PQO_EXPORT void pqo_topk(const float* prob, int C, int k, int* idx, float* val) 
   free(tmp);
 }
 
+/* k-fold arg-max of CaffeEva::CvtFeatMapToLablVec (src/CaffeEva.cc:1162-1190): each round scans from
+ * (FLT_MIN, index 0) with a strict '<', so a value <= FLT_MIN or a NaN never wins, and index 0 is taken (and
+ * zeroed) when nothing beats FLT_MIN.  Labels only; the reference records no probability. */
+PQO_EXPORT void pqo_topk_labl(const float* prob, int C, int k, int* idx) {
+  float* tmp = (float*)malloc(sizeof(float) * C);
+  memcpy(tmp, prob, sizeof(float) * C);
+  for (int r = 0; r < k; r++) {
+    float best = 1.17549435e-38f; /* FLT_MIN */
+    int bi = 0;
+    for (int c = 0; c < C; c++) if (best < tmp[c]) { best = tmp[c]; bi = c; }
+    idx[r] = bi;
+    tmp[bi] = 0.0f;
+  }
+  free(tmp);
+}
+
 /* Synthetic image generator of SURVEY.md 8(d) / BASELINE.md 3: LCG s <- 1664525 s + 1013904223 (mod 2^32),
  * x = ((s >> 8) & 0xFFFF) / 65536 * 256 - 128, value taken after each update. */
 PQO_EXPORT void pqo_lcg_fill(uint32_t seed, float* out, long n) {

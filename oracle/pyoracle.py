@@ -492,3 +492,30 @@ def ref_get_inpd(data, ctrd_skd):
     out = np.empty((P, S, K), np.float32)
     ref().ref_get_inpd(_p(data), P, D, _p(buf), S, d, K, _p(out))
     return out
+
+
+def topk_labl(prob, k=5):
+    """Labels of CaffeEva::CvtFeatMapToLablVec's k-fold arg-max (the oracle's restatement, pqo_topk_labl)."""
+    prob = _f32(prob)
+    idx = np.empty(k, np.int32)
+    oracle().pqo_topk_labl(_p(prob), prob.size, k, _p(idx))
+    return idx
+
+
+def ref_bmp_load(bmp_path, mean_path, resz_type, mean_type, hei_full, wid_full, hei_crop, wid_crop):
+    """Reference BmpImgIO::Init + Load with the given recipe: f32 [3, hei_crop, wid_crop] (BGR, mean-subtracted)."""
+    out = np.empty((3, hei_crop, wid_crop), np.float32)
+    n = ref().ref_bmp_load(bmp_path.encode(), mean_path.encode(), resz_type, mean_type, hei_full, wid_full,
+                           hei_crop, wid_crop, _p(out), out.size)
+    if n != out.size:
+        raise IOError("ref_bmp_load(%s): %d elements" % (bmp_path, n))
+    return out
+
+
+def ref_cvt_featmap_to_labl(prob):
+    """Reference CaffeEva::CvtFeatMapToLablVec on an [N, C] matrix: uint16 [N, 5] labels."""
+    prob = _f32(prob)
+    N, Cc = prob.shape
+    out = np.empty((N, 5), np.uint16)
+    ref().ref_cvt_featmap_to_labl(_p(prob), N, Cc, _p(out))
+    return out

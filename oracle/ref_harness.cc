@@ -311,6 +311,41 @@ int ref_wrapper_proc(void* h, const char* bmpPath, int k, int* idx, float* prob)
   return 0;
 }
 
+// BmpImgIO::Init + Load (BmpImgIO.cc:16-71) with any recipe: resz_type / mean_type in ENUM_ReszType / ENUM_MeanType
+// order, mean file [3][H][W] (FileIO .bin); out [3][hei_crop][wid_crop] BGR, mean-subtracted.  Returns the element
+// count or -1.
+int ref_bmp_load(const char* bmpPath, const char* meanPath, int reszType, int meanType, int heiFull, int widFull,
+                 int heiCrop, int widCrop, float* out, int cap) {
+  StdoutMute mute(true);
+  BmpImgIOPara para;
+  para.reszType = static_cast<ENUM_ReszType>(reszType);
+  para.meanType = static_cast<ENUM_MeanType>(meanType);
+  para.imgHeiFull = heiFull;
+  para.imgWidFull = widFull;
+  para.imgHeiCrop = heiCrop;
+  para.imgWidCrop = widCrop;
+  para.filePathMean = meanPath;
+  BmpImgIO io;
+  if (!io.Init(para)) return -1;
+  Matrix<float> img;
+  if (!io.Load(bmpPath, &img)) return -1;
+  int n = img.GetEleCnt();
+  memcpy(out, img.GetDataPtr(), sizeof(float) * std::min(n, cap));
+  return n;
+}
+
+// CaffeEva::CvtFeatMapToLablVec (CaffeEva.cc:1162-1190) on a caller's [N][C] matrix: out [N][5] labels
+void ref_cvt_featmap_to_labl(const float* prob, int N, int C, uint16_t* out) {
+  CaffeEva eva;
+  eva.featMapLst = nullptr;
+  eva.caffeParaObj.layerCnt = 0;
+  Matrix<float> featMap(N, C, 1, 1);
+  memcpy(featMap.GetDataPtr(), prob, sizeof(float) * N * C);
+  Matrix<uint16_t> labl(N, 5, 1, 1);
+  eva.CvtFeatMapToLablVec(0, N - 1, featMap, &labl);
+  memcpy(out, labl.GetDataPtr(), sizeof(uint16_t) * N * 5);
+}
+
 // BmpImgIO::Load (BmpImgIO.cc:40-71) with the wrapper's AlexNet recipe: out [3][227][227] BGR, mean-subtracted
 int ref_wrapper_load_bmp(void* h, const char* bmpPath, float* out, int cap) {
   StdoutMute mute(true);

@@ -97,11 +97,14 @@ __global__ void topk_kernel(const float* __restrict__ prob, int C, int k, int mo
   for (int c = tid; c < C; c += blockDim.x) row[c] = prob[static_cast<size_t>(n) * C + c];
   __syncthreads();
   for (int r = 0; r < k; r++) {
-    // first maximum of the thread's elements (ascending index, strict <), then of the block (ties -> lower index)
+    // first maximum of the thread's elements (ascending index, strict <), then of the block (ties -> lower index).
+    // Neither reference scan ever moves onto a NaN, so a NaN is never a candidate and the merges below never see one.
     float bv = -INFINITY;
     int bi = C;
-    for (int c = tid; c < C; c += blockDim.x)
-      if (bi == C || bv < row[c]) { bv = row[c]; bi = c; }
+    for (int c = tid; c < C; c += blockDim.x) {
+      const float v = row[c];
+      if (v == v && (bi == C || bv < v)) { bv = v; bi = c; }
+    }
     for (int m = 16; m >= 1; m >>= 1) {
       const float ov = __shfl_xor_sync(0xFFFFFFFFu, bv, m);
       const int oi = __shfl_xor_sync(0xFFFFFFFFu, bi, m);
@@ -118,6 +121,8 @@ __global__ void topk_kernel(const float* __restrict__ prob, int C, int k, int mo
         if (oi < C && (bi == C || bv < ov || (bv == ov && oi < bi))) { bv = ov; bi = oi; }
       }
       if (lane == 0) {
+        // mode 0 (Proc): the scan starts from row[0], and nothing compares greater than a NaN there
+        if (mode == 0 && row[0] != row[0]) bi = 0;
         // mode 1 (CvtFeatMapToLablVec): the scan starts from FLT_MIN with index 0, so nothing <= FLT_MIN can win
         if (mode == 1 && !(FLT_MIN < bv)) bi = 0;
         if (bi >= C) bi = 0;
@@ -203,6 +208,8 @@ void qcnn_preproc_destroy(qcnn_preproc* p) {
 
 int qcnn_preproc_run(qcnn_preproc* p, const uint8_t* pix, const long long* off_h, const int* hei_h, const int* wid_h, int N,
                      float* dst, void* stream) {
+  // Each run rewrites the object's one descriptor buffer on `stream`: runs on one stream are ordered, but two streams
+  // running one object at once race on it, so give each stream its own qcnn_preproc.
   QCNN_CHECK(p && pix && off_h && hei_h && wid_h && dst && N >= 1 && N <= 65535, "qcnn_preproc_run: bad argument");
   QCNN_ON_DEVICE(p->ctx->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);

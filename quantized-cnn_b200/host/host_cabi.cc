@@ -25,6 +25,28 @@ __attribute__((visibility("default"))) int qcnn_host_load_bmp_alexnet(const char
   return n;
 }
 
+// BmpImgIO with any recipe: resz_type 0 Strict / 1 Relaxed, mean_type 0 Full / 1 Crop (the ENUM orders), mean file
+// [3][H][W]; out [3][hei_crop][wid_crop] BGR mean-subtracted; returns the element count or -1
+__attribute__((visibility("default"))) int qcnn_host_load_bmp(const char* bmpPath, const char* meanPath, int reszType,
+                                                              int meanType, int heiFull, int widFull, int heiCrop,
+                                                              int widCrop, float* out, int cap) {
+  BmpImgIOPara p;
+  p.reszType = static_cast<ENUM_ReszType>(reszType);
+  p.meanType = static_cast<ENUM_MeanType>(meanType);
+  p.imgHeiFull = heiFull;
+  p.imgWidFull = widFull;
+  p.imgHeiCrop = heiCrop;
+  p.imgWidCrop = widCrop;
+  p.filePathMean = meanPath;
+  BmpImgIO io;
+  if (!io.Init(p)) return -1;
+  Matrix<float> img;
+  if (!io.Load(bmpPath, &img)) return -1;
+  const int n = img.GetEleCnt();
+  memcpy(out, img.GetDataPtr(), sizeof(float) * (n < cap ? n : cap));
+  return n;
+}
+
 // layer table of a named model: writes up to cap records of 12 ints/floats (LayerInfo order); returns layerCnt
 __attribute__((visibility("default"))) int qcnn_host_layer_table(const char* model, int* imgChw, int* types, int cap) {
   CaffePara para;

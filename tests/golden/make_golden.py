@@ -11,6 +11,8 @@ Outputs (all small):
                     (inputs + parameters stored alongside)
   bmp_top5.npz      top-5 of CaffeEvaWrapper::Proc on the ten shipped BMPs + fingerprints of BmpImgIO::Load outputs
   cbn_vectors.npz   byte images of .cbn / .bin files written by the reference's own FileIO for 4/5/7/8-bit tables
+  preproc_topk_ref.npz  sha256 of BmpImgIO::Load's output on every generated BMP case and CvtFeatMapToLablVec's
+                    labels on every generated top-k row of tests/test_preproc_reference.py
 """
 import os
 import sys
@@ -138,6 +140,13 @@ def bmp_top5():
     np.savez_compressed(os.path.join(OUT, "bmp_top5.npz"), **out)
 
 
+def preproc_topk():
+    sys.path.insert(0, os.path.dirname(OUT))
+    from test_preproc_reference import GOLDEN, reference_goldens
+    with tempfile.TemporaryDirectory() as d:
+        np.savez_compressed(GOLDEN, **reference_goldens(po, d))
+
+
 if __name__ == "__main__":
     assert po.have_ref(), "build oracle/_ref first (make -C oracle ref data)"
     po.build()
@@ -145,5 +154,6 @@ if __name__ == "__main__":
     synth_layers()
     cbn_vectors()
     bmp_top5()
+    preproc_topk()
     for f in sorted(os.listdir(OUT)):
         print(f, os.path.getsize(os.path.join(OUT, f)))

@@ -32,20 +32,23 @@ def decode_bmp(path):
 
 
 def resz_crop_numpy(img, mean, full, crop, relaxed, mean_full):
-    """numpy restatement of BmpImgIO::Load (reference src/BmpImgIO.cc:105-224) with its float / double steps."""
+    """numpy restatement of BmpImgIO::Load (reference src/BmpImgIO.cc:105-224) with its float / double steps.
+    full and crop are a side length or a (height, width) pair."""
     f32 = np.float32
+    hf, wf = (full, full) if np.isscalar(full) else full
+    hc, wc = (crop, crop) if np.isscalar(crop) else crop
     hs, ws = img.shape[:2]
-    sh = f32(hs - 1) / f32(full - 1)
-    sw = f32(ws - 1) / f32(full - 1)
-    hd = wd = full
+    sh = f32(hs - 1) / f32(hf - 1)
+    sw = f32(ws - 1) / f32(wf - 1)
+    hd, wd = hf, wf
     if relaxed:
         sh = min(sh, sw)
         sw = min(sh, sw)
         hd = int(np.float64(f32(hs - 1) / sh) + 0.0000001) + 1
         wd = int(np.float64(f32(ws - 1) / sw) + 0.0000001) + 1
-    yo, xo = (hd - crop) // 2, (wd - crop) // 2
-    ys = np.arange(yo, yo + crop)
-    xs = np.arange(xo, xo + crop)
+    yo, xo = (hd - hc) // 2, (wd - wc) // 2
+    ys = np.arange(yo, yo + hc)
+    xs = np.arange(xo, xo + wc)
     yc = (sh * ys.astype(f32)).astype(f32)
     yl = np.maximum(0, yc.astype(np.int32))
     yh = np.minimum(hs - 1, yl + 1)
@@ -60,7 +63,7 @@ def resz_crop_numpy(img, mean, full, crop, relaxed, mean_full):
     wLB, wRB = wyh[:, None] * wxl[None, :], wyh[:, None] * wxh[None, :]
     wsum = ((wLT + wRT) + wLB) + wRB
     src = img.astype(f32)
-    out = np.empty((3, crop, crop), f32)
+    out = np.empty((3, hc, wc), f32)
     for c in range(3):
         a, b = src[yl][:, xl, c], src[yl][:, xh, c]
         e, f = src[yh][:, xl, c], src[yh][:, xh, c]
