@@ -359,6 +359,37 @@ QCNN_API int qcnn_pq_refine_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int C
                                  const float* x /*device NHWC [N][Hin][Win][Cin]*/, int N,
                                  float* ctrd_h /*in/out [S][K][d]*/, uint8_t* asmt_h /*in/out [Cout][k][k][S], 0-based*/,
                                  double* loss_h /*nullable [sweeps + 1]*/, void* stream);
+/* Error-correcting PQ toward target responses (DESIGN.md 4e, the paper's multi-layer error correction): the layer's
+ * inputs y come from the quantized network (every earlier layer already quantized) and the targets t are the original
+ * network's responses of the layer, without bias and before ReLU (e.g. t_n = W x_n on the original network's input x_n).
+ * The calls lower loss = sum_n |t_n - W^ y_n|^2 and take no dense weights: the targets carry what the weights did.
+ * FC: y [N][Din] and t [N][Dout] on the device; G = Y^T Y exactly as qcnn_pq_refine_fc forms it (same kernel and order,
+ * so bit-identical for the same y), P = T^T Y (fp64 [Dout][Din], k ascending in the GEMM's fixed steps), and
+ * loss = |T|^2 - 2 sum_o w^_o^T P_o + sum_o w^_o^T G w^_o.  The sweeps are those of qcnn_pq_refine_fc (skip rule, Cholesky
+ * codebook step with strict acceptance, argmin with the lowest index on ties, Gauss-Seidel order) with the residual
+ * response h_o = [R_o]_m + G_mm w^_o(m), R_o = P_o - G w^_o, in place of G E_o.
+ * Conv: y [N][Hin][Win][Cin] and t [N][Ho][Wo][Cout] (NHWC) on the device, geometry as qcnn_pq_refine_conv;
+ * P_g[o][q] = sum over every image and output position of t[pos][o] p_g(pos)[q] for o in group g (p_g the zero-padded
+ * patch of y, accumulated over the same patch chunks in the same ascending order as G_g), and R = P - G W^ replaces G E
+ * everywhere in qcnn_pq_refine_conv's sweep (h_{o,t}, h'_{o,t} and the update after each subspace); the joint codebook
+ * system, the tap-ordered assignment, the skip rule and every tie rule are unchanged.  The loss is formed as for FC.
+ * loss_h (nullable, sweeps + 1 values) = the start's loss, then the loss after each sweep.  This loss is a difference of
+ * large terms: its absolute rounding error is of order 1e-15 (|T|^2 + sum_o w^_o^T G w^_o), so it can rise by that much
+ * across a sweep.  |T|^2 is an fp64 sum of fp32 squares, which cannot overflow: it is non-finite exactly when t holds a
+ * NaN or Inf.  Results are bit-reproducible.  Runs on `stream` and synchronises it.  Device memory: that of the
+ * same-input call plus 8 Dout Din bytes for P (FC) or 8 Cout Cg k^2 (conv).  Fails on what the same-input call refuses
+ * apart from the weight checks (K, d, sweeps < 0, N < 1, an assignment >= K, a non-finite codebook, non-finite y, the
+ * conv geometry, the joint-system limit, a failed allocation with its byte count), and on a NULL or non-finite t. */
+QCNN_API int qcnn_pq_refine_fc_target(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps,
+                                      const float* y /*device [N][Din]*/, const float* t /*device [N][Dout]*/, int N,
+                                      float* ctrd_h /*in/out [S][K][d]*/, uint8_t* asmt_h /*in/out [Dout][S], 0-based*/,
+                                      double* loss_h /*nullable [sweeps + 1]*/, void* stream);
+QCNN_API int qcnn_pq_refine_conv_target(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride,
+                                        int grp, int K, int d, int sweeps,
+                                        const float* y /*device NHWC [N][Hin][Win][Cin]*/,
+                                        const float* t /*device NHWC [N][Ho][Wo][Cout]*/, int N,
+                                        float* ctrd_h /*in/out [S][K][d]*/, uint8_t* asmt_h /*in/out [Cout][k][k][S], 0-based*/,
+                                        double* loss_h /*nullable [sweeps + 1]*/, void* stream);
 
 /* ---- file formats (include/FileIO.h:56-178, 229-350), host only ------------------------------------------- */
 /* .bin: returns element count or -1; dims4 padded with 1; data_h may be NULL to query the shape */

@@ -131,6 +131,8 @@ _SIGS = {
     "qcnn_pq_quantize_model": (_i, [_vp, _cp, _cp, _cp, C.POINTER(_i), C.POINTER(_i), _i, C.c_uint32, _cp, _cp]),
     "qcnn_pq_refine_fc": (_i, [_vp] + [_i] * 5 + [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "qcnn_pq_refine_conv": (_i, [_vp] + [_i] * 11 + [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_refine_fc_target": (_i, [_vp] + [_i] * 5 + [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_refine_conv_target": (_i, [_vp] + [_i] * 11 + [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
 }
 for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)
@@ -700,4 +702,56 @@ def pq_refine_conv(ctx, knl, x, ctrd, asmt, pad=0, stride=1, grp=1, sweeps=8, st
     _check(lib.qcnn_pq_refine_conv(ctx.h, Cin, Hin, Win, Cout, k, pad, stride, grp, K, d, sweeps,
                                    knl.ctypes.data_as(_vp), _dptr(x), N, ctrd.ctypes.data_as(_vp),
                                    asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp), _stream(stream)))
+    return ctrd, asmt, loss
+
+
+def pq_refine_fc_target(ctx, y, t, ctrd, asmt, sweeps=8, stream=None):
+    """Error-correcting PQ of an FC layer toward target responses: y [N, Din] are the layer's inputs in the quantized
+    network and t [N, Dout] the original layer's responses without bias and before ReLU (both contiguous float32 CUDA
+    tensors, y in fcntWei column order), starting from (ctrd [S, K, d], asmt [Dout, S] 0-based): (ctrd, asmt,
+    loss [sweeps + 1]) with loss[s] = sum_n |t_n - W^ y_n|^2 after sweep s.  The arguments are not modified."""
+    ctrd = np.array(ctrd, np.float32, order="C", copy=True)
+    asmt = np.array(asmt, np.uint8, order="C", copy=True)
+    S, K, d = ctrd.shape
+    if y.dim() != 2 or t.dim() != 2 or t.shape[0] != y.shape[0]:
+        raise QcnnError("y must be [N, Din] and t [N, Dout] with the same N, got %s and %s"
+                        % (tuple(y.shape), tuple(t.shape)))
+    N, Din = y.shape
+    Dout = t.shape[1]
+    if S != -(-Din // d) or asmt.shape != (Dout, S):
+        raise QcnnError("ctrd [%d, K, d] and asmt %s do not match a [%d, %d] layer with d=%d"
+                        % (S, tuple(asmt.shape), Dout, Din, d))
+    loss = np.empty(max(sweeps, 0) + 1, np.float64)
+    _check(lib.qcnn_pq_refine_fc_target(ctx.h, Din, Dout, K, d, sweeps, _dptr(y), _dptr(t), N,
+                                        ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp),
+                                        _stream(stream)))
+    return ctrd, asmt, loss
+
+
+def pq_refine_conv_target(ctx, y, t, ctrd, asmt, ksz, pad=0, stride=1, grp=1, sweeps=8, stream=None):
+    """Error-correcting PQ of a conv layer toward target responses: y [N, Hin, Win, Cin] are the layer's inputs in the
+    quantized network and t [N, Ho, Wo, Cout] the original layer's responses without bias and before ReLU (both NHWC,
+    contiguous float32 CUDA tensors), starting from (ctrd [S, K, d], asmt [Cout, ksz, ksz, S] 0-based): (ctrd, asmt,
+    loss [sweeps + 1]) with loss[s] = sum (t - conv(y, W^))^2 after sweep s.  The arguments are not modified."""
+    ctrd = np.array(ctrd, np.float32, order="C", copy=True)
+    asmt = np.array(asmt, np.uint8, order="C", copy=True)
+    S, K, d = ctrd.shape
+    if y.dim() != 4 or t.dim() != 4 or t.shape[0] != y.shape[0]:
+        raise QcnnError("y must be [N, Hin, Win, Cin] and t [N, Ho, Wo, Cout] with the same N, got %s and %s"
+                        % (tuple(y.shape), tuple(t.shape)))
+    N, Hin, Win, Cin = y.shape
+    Cout = t.shape[3]
+    # a geometry the call refuses (grp not dividing Cin, an empty output, ...) is left to its own message
+    if ksz >= 1 and stride >= 1 and grp >= 1 and Cin % grp == 0 and Hin + 2 * pad >= ksz and Win + 2 * pad >= ksz:
+        Ho, Wo = (Hin + 2 * pad - ksz) // stride + 1, (Win + 2 * pad - ksz) // stride + 1
+        if tuple(t.shape) != (N, Ho, Wo, Cout):
+            raise QcnnError("t must be [%d, %d, %d, Cout] for a %dx%d kernel, pad %d, stride %d on %s, got %s"
+                            % (N, Ho, Wo, ksz, ksz, pad, stride, tuple(y.shape), tuple(t.shape)))
+        if S != -(-(Cin // grp) // d) or asmt.shape != (Cout, ksz, ksz, S):
+            raise QcnnError("ctrd [%d, K, d] and asmt %s do not match a [%d, %d, %d, %d] kernel with d=%d"
+                            % (S, tuple(asmt.shape), Cout, Cin // grp, ksz, ksz, d))
+    loss = np.empty(max(sweeps, 0) + 1, np.float64)
+    _check(lib.qcnn_pq_refine_conv_target(ctx.h, Cin, Hin, Win, Cout, ksz, pad, stride, grp, K, d, sweeps, _dptr(y),
+                                          _dptr(t), N, ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp),
+                                          loss.ctypes.data_as(_vp), _stream(stream)))
     return ctrd, asmt, loss

@@ -7,6 +7,10 @@
 //   codebook   D = (G_mm + lambda I)^-1 H_k / n_k by the Cholesky factor, lambda = 1e-10 tr(G_mm) / w_m, rounded to fp32;
 //              D replaces c_k only if f(D) < f(c_k), f(D) = n_k D^T G_mm D - 2 D^T H_k; empty clusters keep their codeword.
 //   assign     a_o = argmin_k c_k^T G_mm c_k - 2 c_k^T h_o (fp64, new codewords), the lowest index wins ties.
+// Target form (qcnn_pq_refine_fc_target): inputs y, targets t [N][Dout], P = T^T Y (fp64), and
+//   loss = sum_n |t_n - W^ y_n|^2 = |T|^2 - 2 sum_o w^_o^T P_o + sum_o w^_o^T G w^_o; the sweep is the same with
+//   G E_o replaced by R_o = P_o - G w^_o.  It runs on the same kernels: E = -W^ (the residual against zero weights) and
+//   the initial GE = P + E G, after which every update of E and GE is the same-input one.
 // No floating-point atomics: two calls return identical bits.
 //
 // Cost structure: G, the initial G E^T and the update of G E^T after every block of subspaces are fp64 tensor-core GEMMs
@@ -257,19 +261,21 @@ __global__ void __launch_bounds__(kSweepThreads) pqr_block_kernel(BlockArgs p) {
   }
 }
 
-int Refine(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const float* w_h, const float* x, int N, float* ctrd_h,
-           uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
-  const char* who = "qcnn_pq_refine_fc";
-  QCNN_CHECK(ctx && w_h && ctrd_h && asmt_h, "%s: NULL argument", who);
+// target: the target form on the targets t (w_h is not read); else the same-input form on the weights w_h.
+int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int sweeps, const float* w_h, const float* x, const float* t,
+           int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+  const char* who = target ? "qcnn_pq_refine_fc_target" : "qcnn_pq_refine_fc";
+  QCNN_CHECK(ctx && (target || w_h) && ctrd_h && asmt_h, "%s: NULL argument", who);
   QCNN_CHECK(Din >= 1 && Dout >= 1, "%s: bad dimensions", who);
   if (int rc = CheckFcK(who, K)) return rc;
   QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
   QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
   QCNN_CHECK(N >= 1, "%s: N=%d: at least one input is needed", who, N);
   QCNN_CHECK(x, "%s: NULL argument", who);
+  QCNN_CHECK(!target || t, "%s: NULL t", who);
   const int S = CeilDiv(Din, d);
   const size_t nw = static_cast<size_t>(Dout) * Din, nc = static_cast<size_t>(S) * K * d;
-  QCNN_CHECK(AllFinite(w_h, nw), "%s: the weights contain a non-finite value", who);
+  if (!target) QCNN_CHECK(AllFinite(w_h, nw), "%s: the weights contain a non-finite value", who);
   QCNN_CHECK(AllFinite(ctrd_h, nc), "%s: the codebook contains a non-finite value", who);
   std::vector<uint8_t> at(static_cast<size_t>(S) * Dout);   // [S][Dout]
   for (int o = 0; o < Dout; o++)
@@ -280,7 +286,7 @@ int Refine(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const flo
     }
   QCNN_ON_DEVICE(ctx->device);
   const int spb = std::max(1, kBlockDims / d), ld = spb * d;
-  DeviceBuffer dG, dE, dGE, dW, dC, dA, dL, dDlt, dH, dCc, dPart, dLoss;
+  DeviceBuffer dG, dE, dGE, dW, dC, dA, dL, dDlt, dH, dCc, dPart, dLoss, dTY, dTT;
   auto reserve = [&](DeviceBuffer& b, size_t bytes, const char* what) -> int {
     const cudaError_t e = b.Reserve(ctx, bytes);
     if (e == cudaSuccess) return 0;
@@ -296,30 +302,46 @@ int Refine(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const flo
       reserve(dDlt, sizeof(double) * Dout * static_cast<size_t>(ld), "the block's changes") ||
       reserve(dH, sizeof(double) * Dout * static_cast<size_t>(d), "the subspace responses") ||
       reserve(dCc, sizeof(double) * K, "the codeword norms") || reserve(dPart, sizeof(double) * kLossBlocks, "the loss") ||
-      reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss"))
+      reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss") ||
+      reserve(dTY, target ? sizeof(double) * nw : 0, "the targets' cross product") ||
+      reserve(dTT, target ? sizeof(double) : 0, "the targets' norm"))
     return 1;
-  QCNN_CUDA(cudaMemcpyAsync(dW.get(), w_h, sizeof(float) * nw, cudaMemcpyHostToDevice, st));
+  if (target) QCNN_CUDA(cudaMemsetAsync(dW.get(), 0, sizeof(float) * nw, st));   // E = 0 - W^
+  else QCNN_CUDA(cudaMemcpyAsync(dW.get(), w_h, sizeof(float) * nw, cudaMemcpyHostToDevice, st));
   QCNN_CUDA(cudaMemcpyAsync(dC.get(), ctrd_h, sizeof(float) * nc, cudaMemcpyHostToDevice, st));
   QCNN_CUDA(cudaMemcpyAsync(dA.get(), at.data(), at.size(), cudaMemcpyHostToDevice, st));
   // G = X^T X, then its diagonal: a NaN or Inf anywhere in x makes one entry non-finite (fp32 squares cannot overflow it)
   const int tiles = CeilDiv(Din, kTile);
-  pqr_gemm_kernel<true><<<tiles * (tiles + 1) / 2, kGemmThreads, 0, st>>>(x, Din, nullptr, 0, dG.as<double>(), Din, Din, Din, N, 0);
+  pqr_gemm_kernel<kGemmGram><<<tiles * (tiles + 1) / 2, kGemmThreads, 0, st>>>(x, Din, nullptr, 0, dG.as<double>(), Din, Din, Din, N, 0);
   QCNN_CUDA(cudaGetLastError());
+  const dim3 gemmGrid(tiles, CeilDiv(Dout, kTile));
+  double tt = 0.0;
+  if (target) {   // |T|^2 (non-finite exactly when t is) and P = T^T Y
+    if (int rc = LaunchSqNorm(t, static_cast<size_t>(N) * Dout, dPart.as<double>(), dTT.as<double>(), st)) return rc;
+    pqr_gemm_kernel<kGemmCross><<<gemmGrid, kGemmThreads, 0, st>>>(t, Dout, x, Din, dTY.as<double>(), Din, Dout, Din, N, 0);
+    QCNN_CUDA(cudaGetLastError());
+    QCNN_CUDA(cudaMemcpyAsync(&tt, dTT.get(), sizeof(double), cudaMemcpyDeviceToHost, st));
+  }
   std::vector<double> diag(Din);
   QCNN_CUDA(cudaMemcpy2DAsync(diag.data(), sizeof(double), dG.get(), sizeof(double) * (static_cast<size_t>(Din) + 1),
                               sizeof(double), Din, cudaMemcpyDeviceToHost, st));
   QCNN_CUDA(cudaStreamSynchronize(st));
-  for (int c = 0; c < Din; c++) QCNN_CHECK(isfinite(diag[c]), "%s: x contains a non-finite value (input column %d)", who, c);
+  for (int c = 0; c < Din; c++) QCNN_CHECK(isfinite(diag[c]), "%s: %s contains a non-finite value (input column %d)", who,
+                                              target ? "y" : "x", c);
+  QCNN_CHECK(isfinite(tt), "%s: t contains a non-finite value", who);
   const size_t cholSmem = sizeof(double) * 2 * std::min(d, Din) * (std::min(d, Din) + 1);
   if (int rc = OptInSmem<pqr_chol_kernel>(ctx)) return rc;
   pqr_chol_kernel<<<S, kSweepThreads, cholSmem, st>>>(dG.as<double>(), dL.as<double>(), Din, d);
   const int ewBlocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 32u * ctx->sm_count));
   pqr_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Din, Dout, K, d);
-  const dim3 gemmGrid(tiles, CeilDiv(Dout, kTile));
-  pqr_gemm_kernel<false><<<gemmGrid, kGemmThreads, 0, st>>>(dE.get(), Din, dG.get(), Din, dGE.as<double>(), Din, Dout, Din, Din, 0);
+  // GE = E G, or P + E G for a target
+  if (target) QCNN_CUDA(cudaMemcpyAsync(dGE.get(), dTY.get(), sizeof(double) * nw, cudaMemcpyDeviceToDevice, st));
+  pqr_gemm_kernel<kGemmF64><<<gemmGrid, kGemmThreads, 0, st>>>(dE.get(), Din, dG.get(), Din, dGE.as<double>(), Din, Dout, Din, Din,
+                                                               target);
   QCNN_CUDA(cudaGetLastError());
-  auto loss = [&](int t) -> int {
-    return LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + t, st);
+  auto loss = [&](int sw) -> int {
+    return LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st,
+                      target ? dTY.as<double>() : nullptr, dTT.as<double>());
   };
   if (int rc = loss(0)) return rc;
   if (sweeps > 0) {
@@ -334,7 +356,7 @@ int Refine(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const flo
     const int grid = std::min(std::min(perSm, 2) * ctx->sm_count, std::max(Dout, K));
     BlockArgs a{dG.as<double>(), dGE.as<double>(), dL.as<double>(), dE.as<double>(), dDlt.as<double>(), dH.as<double>(),
                 dCc.as<double>(), dC.as<float>(), dA.as<uint8_t>(), Din, Dout, K, d, ld, 0, 0};
-    for (int t = 1; t <= sweeps; t++) {
+    for (int sw = 1; sw <= sweeps; sw++) {
       for (int m0 = 0; m0 < S; m0 += spb) {
         a.m0 = m0;
         a.m1 = std::min(S, m0 + spb);
@@ -342,11 +364,11 @@ int Refine(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const flo
         QCNN_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(pqr_block_kernel), grid, kSweepThreads, args, blkSmem, st));
         // GE += dlt G[block dims][:]
         const int blk0 = m0 * d, bw = std::min(Din, a.m1 * d) - blk0;
-        pqr_gemm_kernel<false><<<gemmGrid, kGemmThreads, 0, st>>>(dDlt.get(), ld, dG.as<double>() + static_cast<size_t>(blk0) * Din,
+        pqr_gemm_kernel<kGemmF64><<<gemmGrid, kGemmThreads, 0, st>>>(dDlt.get(), ld, dG.as<double>() + static_cast<size_t>(blk0) * Din,
                                                                   Din, dGE.as<double>(), Din, Dout, Din, bw, 1);
         QCNN_CUDA(cudaGetLastError());
       }
-      if (int rc = loss(t)) return rc;
+      if (int rc = loss(sw)) return rc;
     }
   }
   std::vector<double> lossv(sweeps + 1);
@@ -364,5 +386,10 @@ int Refine(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const flo
 
 extern "C" int qcnn_pq_refine_fc(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const float* wei_h, const float* x,
                                  int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h, void* stream) {
-  return Refine(ctx, Din, Dout, K, d, sweeps, wei_h, x, N, ctrd_h, asmt_h, loss_h, static_cast<cudaStream_t>(stream));
+  return Refine(ctx, false, Din, Dout, K, d, sweeps, wei_h, x, nullptr, N, ctrd_h, asmt_h, loss_h, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int qcnn_pq_refine_fc_target(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const float* y, const float* t,
+                                        int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h, void* stream) {
+  return Refine(ctx, true, Din, Dout, K, d, sweeps, nullptr, y, t, N, ctrd_h, asmt_h, loss_h, static_cast<cudaStream_t>(stream));
 }

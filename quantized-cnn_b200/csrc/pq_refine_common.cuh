@@ -1,6 +1,6 @@
 // Pieces shared by the error-correcting quantizers of FC layers (pq_refine.cu) and conv layers (pq_refine_conv.cu):
-// the fp64 tensor-core GEMM, the fixed-order block reduction and the loss kernels.  They sit in an anonymous namespace
-// because each including .cu file is its own device module and links its own copy.
+// the fp64 tensor-core GEMM, the fixed-order block reduction and the loss kernels (same-input and target form).  They
+// sit in an anonymous namespace because each including .cu file is its own device module and links its own copy.
 #ifndef QCNN_PQ_REFINE_COMMON_CUH_
 #define QCNN_PQ_REFINE_COMMON_CUH_
 
@@ -26,14 +26,18 @@ __device__ __forceinline__ void Dmma(double (&c)[4], const double (&a)[8], const
         "d"(b[2]), "d"(b[3]));
 }
 
+// What pqr_gemm_kernel computes (its template argument)
+constexpr int kGemmF64 = 0;     // C [M][N] = (accumulate ? C : 0) + A [M][Kd] B [Kd][N], all fp64
+constexpr int kGemmGram = 1;    // C = (accumulate ? C : 0) + X^T X for X = A [Kd][lda] fp32 (M = N = the column count)
+constexpr int kGemmCross = 2;   // C [M][N] = (accumulate ? C : 0) + A^T B for A [Kd][lda], B [Kd][ldb] fp32
+
 // fp64 tensor-core GEMM, one kTile x kTile output tile per CTA, k in ascending steps of 16 (a fixed order per element).
-//   kGram:  C = (accumulate ? C : 0) + X^T X for X = A [Kd][lda] fp32 (M = N = the column count): lower-triangle tiles
-//           only (blockIdx.x is the linear lower-triangle index); each element with row >= col is written to both
-//           (row, col) and (col, row), so G is exactly symmetric.
-//   else:   C [M][N] = (accumulate ? C : 0) + A [M][Kd] B [Kd][N], all fp64.
+//   kGemmGram:  lower-triangle tiles only (blockIdx.x is the linear lower-triangle index); each element with row >= col
+//               is written to both (row, col) and (col, row), so G is exactly symmetric.
+//   otherwise:  the full tile grid, blockIdx.y over M and blockIdx.x over N.
 // Operands are staged through registers (the next k-step is loaded while the current one is multiplied), widened to
 // fp64 and stored k-major, [16][kLd], in shared memory.
-template <bool kGram>
+template <int kMode>
 __global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __restrict__ Ap, int lda, const void* __restrict__ Bp,
                                                                 int ldb, double* __restrict__ C, int ldc, int M, int N, int Kd,
                                                                 int accumulate) {
@@ -41,7 +45,7 @@ __global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __re
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3, wm = warp >> 1, wn = warp & 1;
   int tm, tn;
-  if (kGram) {
+  if (kMode == kGemmGram) {
     const int i = blockIdx.x;
     tm = static_cast<int>((sqrt(8.0 * i + 1.0) - 1.0) * 0.5);
     while (tm * (tm + 1) / 2 > i) tm--;
@@ -60,10 +64,15 @@ __global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __re
       const int e = tid + r * kGemmThreads;
       const int kk = e / kTile, nn = e % kTile;   // B (and the Gram's A): row kk of the k-step, column nn
       const int k = k0 + kk;
-      if (kGram) {
+      if (kMode == kGemmGram) {
         const float* X = static_cast<const float*>(Ap);
         ra[r] = (k < Kd && m0 + nn < M) ? static_cast<double>(X[static_cast<size_t>(k) * lda + m0 + nn]) : 0.0;
         rb[r] = (k < Kd && n0 + nn < N) ? static_cast<double>(X[static_cast<size_t>(k) * lda + n0 + nn]) : 0.0;
+      } else if (kMode == kGemmCross) {
+        const float* A = static_cast<const float*>(Ap);
+        const float* B = static_cast<const float*>(Bp);
+        ra[r] = (k < Kd && m0 + nn < M) ? static_cast<double>(A[static_cast<size_t>(k) * lda + m0 + nn]) : 0.0;
+        rb[r] = (k < Kd && n0 + nn < N) ? static_cast<double>(B[static_cast<size_t>(k) * ldb + n0 + nn]) : 0.0;
       } else {
         const double* A = static_cast<const double*>(Ap);
         const double* B = static_cast<const double*>(Bp);
@@ -77,7 +86,7 @@ __global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __re
 #pragma unroll
     for (int r = 0; r < kPer; r++) {
       const int e = tid + r * kGemmThreads;
-      if (kGram) As[buf][e / kTile][e % kTile] = ra[r];
+      if (kMode != kGemmF64) As[buf][e / kTile][e % kTile] = ra[r];
       else As[buf][e % kKStep][e / kKStep] = ra[r];
       Bs[buf][e / kTile][e % kTile] = rb[r];
     }
@@ -120,7 +129,7 @@ __global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __re
       for (int i = 0; i < 4; i++) {
         const int row = m0 + wm * 32 + mt * 16 + g + 8 * (i >> 1), col = n0 + wn * 32 + nt * 8 + 2 * t + (i & 1);
         if (row >= M || col >= N) continue;
-        if (kGram) {
+        if (kMode == kGemmGram) {
           if (row < col) continue;
           double* p = C + static_cast<size_t>(row) * ldc + col;
           const double v = accumulate ? *p + acc[mt][nt][i] : acc[mt][nt][i];
@@ -144,29 +153,63 @@ __device__ double BlockSum(double v, double* red) {
   return r;
 }
 
-// loss partials: CTA b sums E * GE over a fixed range of kLossBlocks equal ranges
+// loss partials: CTA b sums E * GE (kTarget: E * (P + GE)) over a fixed range of kLossBlocks equal ranges
+template <bool kTarget>
 __global__ void __launch_bounds__(kSweepThreads) pqr_loss_partial_kernel(const double* __restrict__ E, const double* __restrict__ GE,
-                                                                         size_t n, double* __restrict__ part) {
+                                                                         const double* __restrict__ P, size_t n,
+                                                                         double* __restrict__ part) {
   __shared__ double red[kSweepThreads / 32];
   const size_t chunk = (n + kLossBlocks - 1) / kLossBlocks, b0 = blockIdx.x * chunk, b1 = min(n, b0 + chunk);
   double v = 0.0;
-  for (size_t i = b0 + threadIdx.x; i < b1; i += kSweepThreads) v += E[i] * GE[i];
+  for (size_t i = b0 + threadIdx.x; i < b1; i += kSweepThreads) v += kTarget ? E[i] * (P[i] + GE[i]) : E[i] * GE[i];
   const double tot = BlockSum(v, red);
   if (threadIdx.x == 0) part[blockIdx.x] = tot;
 }
 
-__global__ void __launch_bounds__(kSweepThreads) pqr_loss_final_kernel(const double* __restrict__ part, double* __restrict__ loss) {
+// partials of |t|^2 = sum of fp32 squares in fp64, over the same fixed ranges (exact products, so no overflow)
+__global__ void __launch_bounds__(kSweepThreads) pqr_sqnorm_partial_kernel(const float* __restrict__ t, size_t n,
+                                                                           double* __restrict__ part) {
+  __shared__ double red[kSweepThreads / 32];
+  const size_t chunk = (n + kLossBlocks - 1) / kLossBlocks, b0 = blockIdx.x * chunk, b1 = min(n, b0 + chunk);
+  double v = 0.0;
+  for (size_t i = b0 + threadIdx.x; i < b1; i += kSweepThreads) {
+    const double x = static_cast<double>(t[i]);
+    v += x * x;
+  }
+  const double tot = BlockSum(v, red);
+  if (threadIdx.x == 0) part[blockIdx.x] = tot;
+}
+
+// *loss = the partials' sum (kTarget: *tt plus it)
+template <bool kTarget>
+__global__ void __launch_bounds__(kSweepThreads) pqr_loss_final_kernel(const double* __restrict__ part, const double* __restrict__ tt,
+                                                                       double* __restrict__ loss) {
   __shared__ double red[kSweepThreads / 32];
   double v = 0.0;
   for (int i = threadIdx.x; i < kLossBlocks; i += kSweepThreads) v += part[i];
   const double tot = BlockSum(v, red);
-  if (threadIdx.x == 0) *loss = tot;
+  if (threadIdx.x == 0) *loss = kTarget ? *tt + tot : tot;
 }
 
-// loss = sum E * GE over n elements, in a fixed order, written to *loss
-inline int LaunchLoss(const double* E, const double* GE, size_t n, double* part, double* loss, cudaStream_t st) {
-  pqr_loss_partial_kernel<<<kLossBlocks, kSweepThreads, 0, st>>>(E, GE, n, part);
-  pqr_loss_final_kernel<<<1, kSweepThreads, 0, st>>>(part, loss);
+// loss = sum E * GE over n elements, in a fixed order, written to *loss.  With a target (P non-null):
+// loss = *tt + sum E * (P + GE), which for E = -W^, P = T^T Y and GE = P + E G is |T|^2 - 2 sum W^ . P + sum W^ . G W^.
+inline int LaunchLoss(const double* E, const double* GE, size_t n, double* part, double* loss, cudaStream_t st,
+                      const double* P = nullptr, const double* tt = nullptr) {
+  if (P) {
+    pqr_loss_partial_kernel<true><<<kLossBlocks, kSweepThreads, 0, st>>>(E, GE, P, n, part);
+    pqr_loss_final_kernel<true><<<1, kSweepThreads, 0, st>>>(part, tt, loss);
+  } else {
+    pqr_loss_partial_kernel<false><<<kLossBlocks, kSweepThreads, 0, st>>>(E, GE, nullptr, n, part);
+    pqr_loss_final_kernel<false><<<1, kSweepThreads, 0, st>>>(part, nullptr, loss);
+  }
+  QCNN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// *out = |t|^2 over n fp32 values in a fixed order: non-finite exactly when t holds a NaN or Inf
+inline int LaunchSqNorm(const float* t, size_t n, double* part, double* out, cudaStream_t st) {
+  pqr_sqnorm_partial_kernel<<<kLossBlocks, kSweepThreads, 0, st>>>(t, n, part);
+  pqr_loss_final_kernel<false><<<1, kSweepThreads, 0, st>>>(part, nullptr, out);
   QCNN_CUDA(cudaGetLastError());
   return 0;
 }

@@ -11,6 +11,10 @@
 //              mu = 1e-10 tr(M) / (|U| w_m); D replaces C[m][U] only if (D - C)^T (M (D + C) - 2 b) < 0.
 //   assign     per output, taps t = 0..T-1 in order: a = argmin_k c_k^T G_tt c_k - 2 c_k^T h'_{o,t} (fp64, lowest index
 //              on ties), h' with E current (earlier taps' new assignments included); a (g, t) with tr G_tt = 0 keeps.
+// Target form (qcnn_pq_refine_conv_target): inputs y, targets t [N][Ho][Wo][Cout], per group
+//   P_g[o][q] = sum over positions of t[pos][o] p_g(pos)[q] (the same patch chunks, ascending), and R = P - G W^ in place
+//   of G E everywhere above; loss = |T|^2 + sum_o (-2 w^_o^T P_o + w^_o^T G_g w^_o).  It runs on the same kernels:
+//   the weights are zeros, so E = -W^, and the initial GE = P + E G.
 // No floating-point atomics: two calls return identical bits.
 //
 // Internal dim order (patches, G, E, GE, the weights): subspace-major, q = m d T + t w_m + j, so subspace m's dims are
@@ -432,13 +436,15 @@ struct Geometry {
   int Cin, Hin, Win, Cout, ksz, pad, stride, grp, Ho, Wo, Cg, Cpg, T, Dg;
 };
 
-int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const float* knl_h, const float* x, int N, float* ctrd_h,
-           uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
-  const char* who = "qcnn_pq_refine_conv";
+// t == nullptr: the same-input form on the weights knl_h; else the target form (knl_h is not read).
+int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const float* knl_h, const float* x, const float* t, int N,
+           float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+  const bool target = t != nullptr;
+  const char* who = target ? "qcnn_pq_refine_conv_target" : "qcnn_pq_refine_conv";
   const int Cout = geo.Cout, Cg = geo.Cg, Cpg = geo.Cpg, T = geo.T, Dg = geo.Dg, grp = geo.grp;
   const int S = CeilDiv(Cg, d), wmax = std::min(d, Cg);
   const size_t nw = static_cast<size_t>(Cout) * Dg, nc = static_cast<size_t>(S) * K * d;
-  QCNN_CHECK(AllFinite(knl_h, nw), "%s: the weights contain a non-finite value", who);
+  if (!target) QCNN_CHECK(AllFinite(knl_h, nw), "%s: the weights contain a non-finite value", who);
   QCNN_CHECK(AllFinite(ctrd_h, nc), "%s: the codebook contains a non-finite value", who);
   // assignments [Cout][T][S] -> [S][Cout][T]; weights [Cout][Cg][T] -> [Cout][Dg] in the internal dim order
   std::vector<uint8_t> at(static_cast<size_t>(S) * Cout * T);
@@ -449,8 +455,8 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
         QCNN_CHECK(a < K, "%s: assignment %d of output %d, tap %d, subspace %d is not below K=%d", who, a, o, t, m, K);
         at[(static_cast<size_t>(m) * Cout + o) * T + t] = a;
       }
-  std::vector<float> wp(nw);
-  for (int o = 0; o < Cout; o++)
+  std::vector<float> wp(target ? 0 : nw);
+  for (int o = 0; o < (target ? 0 : Cout); o++)
     for (int c = 0; c < Cg; c++) {
       const int m = c / d, j = c % d, w = std::min(d, Cg - m * d);
       for (int t = 0; t < T; t++)
@@ -460,7 +466,7 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
   const size_t positions = static_cast<size_t>(N) * geo.Ho * geo.Wo;
   const int chunk = static_cast<int>(std::max<size_t>(1, std::min<size_t>(positions, kPatchBytes / (sizeof(float) * Dg))));
   const size_t nbMax = static_cast<size_t>(T) * wmax, nMax = static_cast<size_t>(K) * wmax;
-  DeviceBuffer dG, dE, dGE, dW, dC, dA, dP, dWh, dH, dDlt, dM, dF, dPt, dB, dMem, dOff, dUk, dNU, dCC, dFlag, dPart, dLoss;
+  DeviceBuffer dG, dE, dGE, dW, dC, dA, dP, dWh, dH, dDlt, dM, dF, dPt, dB, dMem, dOff, dUk, dNU, dCC, dFlag, dPart, dLoss, dTY, dTT;
   auto reserve = [&](DeviceBuffer& b, size_t bytes, const char* what) -> int {
     const cudaError_t e = b.Reserve(ctx, bytes);
     if (e == cudaSuccess) return 0;
@@ -483,16 +489,21 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
       reserve(dUk, sizeof(int) * K, "the used clusters") || reserve(dNU, sizeof(int), "the used clusters") ||
       reserve(dCC, sizeof(double) * grp * static_cast<size_t>(T) * K, "the codeword norms") ||
       reserve(dFlag, sizeof(int), "a flag") || reserve(dPart, sizeof(double) * kLossBlocks, "the loss") ||
-      reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss"))
+      reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss") ||
+      reserve(dTY, target ? sizeof(double) * nw : 0, "the targets' cross product") ||
+      reserve(dTT, target ? sizeof(double) : 0, "the targets' norm"))
     return 1;
-  QCNN_CUDA(cudaMemcpyAsync(dW.get(), wp.data(), sizeof(float) * nw, cudaMemcpyHostToDevice, st));
+  if (target) QCNN_CUDA(cudaMemsetAsync(dW.get(), 0, sizeof(float) * nw, st));   // E = 0 - W^
+  else QCNN_CUDA(cudaMemcpyAsync(dW.get(), wp.data(), sizeof(float) * nw, cudaMemcpyHostToDevice, st));
   QCNN_CUDA(cudaMemcpyAsync(dC.get(), ctrd_h, sizeof(float) * nc, cudaMemcpyHostToDevice, st));
   QCNN_CUDA(cudaMemcpyAsync(dA.get(), at.data(), at.size(), cudaMemcpyHostToDevice, st));
   QCNN_CUDA(cudaMemsetAsync(dFlag.get(), 0, sizeof(int), st));
   const size_t nx = static_cast<size_t>(N) * geo.Hin * geo.Win * geo.Cin;
   const int gridX = static_cast<int>(std::min<size_t>((nx + 255) / 256, 32u * ctx->sm_count));
   pqrc_nonfinite_kernel<<<gridX, 256, 0, st>>>(x, nx, dFlag.as<int>());
-  // G_g = sum over chunks of positions, ascending
+  double tt = 0.0;   // |T|^2: non-finite exactly when t is
+  if (target && LaunchSqNorm(t, positions * Cout, dPart.as<double>(), dTT.as<double>(), st)) return 1;
+  // G_g (and P_g) = sum over chunks of positions, ascending
   const int tiles = CeilDiv(Dg, kTile);
   for (int g = 0; g < grp; g++) {
     double* Gg = dG.as<double>() + static_cast<size_t>(g) * Dg * Dg;
@@ -502,7 +513,12 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
       const int gridP = static_cast<int>(std::min<size_t>((ne + 255) / 256, 32u * ctx->sm_count));
       pqrc_patch_kernel<<<gridP, 256, 0, st>>>(x, dP.as<float>(), p0, np, g, geo.Hin, geo.Win, geo.Cin, Cg, geo.ksz, geo.pad,
                                                geo.stride, geo.Ho, geo.Wo, d);
-      pqr_gemm_kernel<true><<<tiles * (tiles + 1) / 2, kGemmThreads, 0, st>>>(dP.get(), Dg, nullptr, 0, Gg, Dg, Dg, Dg, np, p0 > 0);
+      pqr_gemm_kernel<kGemmGram><<<tiles * (tiles + 1) / 2, kGemmThreads, 0, st>>>(dP.get(), Dg, nullptr, 0, Gg, Dg, Dg, Dg, np,
+                                                                                  p0 > 0);
+      if (target)   // the chunk's target rows of group g's outputs against its patches
+        pqr_gemm_kernel<kGemmCross><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
+            t + p0 * Cout + static_cast<size_t>(g) * Cpg, Cout, dP.get(), Dg, dTY.as<double>() + static_cast<size_t>(g) * Cpg * Dg, Dg,
+            Cpg, Dg, np, p0 > 0);
       QCNN_CUDA(cudaGetLastError());
     }
   }
@@ -513,8 +529,10 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
                                 dG.as<double>() + static_cast<size_t>(g) * Dg * Dg, sizeof(double) * (static_cast<size_t>(Dg) + 1),
                                 sizeof(double), Dg, cudaMemcpyDeviceToHost, st));
   QCNN_CUDA(cudaMemcpyAsync(&flag, dFlag.get(), sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (target) QCNN_CUDA(cudaMemcpyAsync(&tt, dTT.get(), sizeof(double), cudaMemcpyDeviceToHost, st));
   QCNN_CUDA(cudaStreamSynchronize(st));
-  QCNN_CHECK(!flag, "%s: x contains a non-finite value", who);
+  QCNN_CHECK(!flag, "%s: %s contains a non-finite value", who, target ? "y" : "x");
+  QCNN_CHECK(isfinite(tt), "%s: t contains a non-finite value", who);
   std::vector<bool> skip(S);
   for (int m = 0; m < S; m++) {
     const int w = std::min(d, Cg - m * d);
@@ -525,13 +543,18 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
   }
   const int ewBlocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 32u * ctx->sm_count));
   pqrc_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Cout, Cg, K, d, T);
+  // GE = E G, or P + E G for a target
+  if (target) QCNN_CUDA(cudaMemcpyAsync(dGE.get(), dTY.get(), sizeof(double) * nw, cudaMemcpyDeviceToDevice, st));
   for (int g = 0; g < grp; g++) {
     const size_t ro = static_cast<size_t>(g) * Cpg * Dg;
-    pqr_gemm_kernel<false><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
-        dE.as<double>() + ro, Dg, dG.as<double>() + static_cast<size_t>(g) * Dg * Dg, Dg, dGE.as<double>() + ro, Dg, Cpg, Dg, Dg, 0);
+    pqr_gemm_kernel<kGemmF64><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
+        dE.as<double>() + ro, Dg, dG.as<double>() + static_cast<size_t>(g) * Dg * Dg, Dg, dGE.as<double>() + ro, Dg, Cpg, Dg, Dg,
+        target);
   }
   QCNN_CUDA(cudaGetLastError());
-  if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>(), st)) return rc;
+  const double* P = target ? dTY.as<double>() : nullptr;   // T^T Y
+  if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>(), st, P, dTT.as<double>()))
+    return rc;
   const size_t assignSmem = sizeof(double) * kAssignWarps * (kMaxD + (T + 1) / 2);
   if (assignSmem > 48 * 1024)
     QCNN_CUDA(cudaFuncSetAttribute(pqrc_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(assignSmem)));
@@ -547,7 +570,7 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
       for (int g = 0; g < grp; g++) {
         const size_t ro = static_cast<size_t>(g) * Cpg * nb;
         const double* Gm = dG.as<double>() + static_cast<size_t>(g) * Dg * Dg + static_cast<size_t>(q0) * Dg + q0;
-        pqr_gemm_kernel<false><<<dim3(CeilDiv(nb, kTile), CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
+        pqr_gemm_kernel<kGemmF64><<<dim3(CeilDiv(nb, kTile), CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
             dWh.as<double>() + ro, nb, Gm, Dg, dH.as<double>() + ro, nb, Cpg, nb, nb, 1);
       }
       // the used clusters and, per (g, t, k), their members
@@ -572,8 +595,8 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
         if (n2 == 0) break;
         pqrc_trsm_kernel<<<CeilDiv(n2, kCholBlock), kCholBlock, 0, st>>>(dF.as<double>(), dPt.as<double>(), n, kb, bw);
         double* Fp = dF.as<double>() + static_cast<size_t>(kb + bw) * n + kb;
-        pqr_gemm_kernel<false><<<dim3(CeilDiv(n2, kTile), CeilDiv(n2, kTile)), kGemmThreads, 0, st>>>(Fp, n, dPt.as<double>(), n,
-                                                                                                      Fp + bw, n, n2, n2, bw, 1);
+        pqr_gemm_kernel<kGemmF64><<<dim3(CeilDiv(n2, kTile), CeilDiv(n2, kTile)), kGemmThreads, 0, st>>>(Fp, n, dPt.as<double>(), n,
+                                                                                                         Fp + bw, n, n2, n2, bw, 1);
       }
       pqrc_solve_kernel<<<1, kSolveThreads, 0, st>>>(dF.as<double>(), dM.as<double>(), dB.as<double>(), dUk.as<int>(), dC.as<float>(), m,
                                                      K, d, w, n);
@@ -584,13 +607,15 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
           dDlt.as<double>(), m, Cout, Cpg, Dg, K, d, w, T, q0);
       for (int g = 0; g < grp; g++) {
         const double* Gb = dG.as<double>() + static_cast<size_t>(g) * Dg * Dg + static_cast<size_t>(q0) * Dg;
-        pqr_gemm_kernel<false><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
+        pqr_gemm_kernel<kGemmF64><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
             dDlt.as<double>() + static_cast<size_t>(g) * Cpg * nb, nb, Gb, Dg, dGE.as<double>() + static_cast<size_t>(g) * Cpg * Dg, Dg,
             Cpg, Dg, nb, 1);
       }
       QCNN_CUDA(cudaGetLastError());
     }
-    if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st)) return rc;
+    if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st, P,
+                            dTT.as<double>()))
+      return rc;
   }
   std::vector<double> lossv(sweeps + 1);
   QCNN_CUDA(cudaMemcpyAsync(ctrd_h, dC.get(), sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
@@ -604,13 +629,12 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
   return 0;
 }
 
-}  // namespace
-
-extern "C" int qcnn_pq_refine_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, int K,
-                                   int d, int sweeps, const float* knl_h, const float* x, int N, float* ctrd_h, uint8_t* asmt_h,
-                                   double* loss_h, void* stream) {
-  const char* who = "qcnn_pq_refine_conv";
-  QCNN_CHECK(ctx && knl_h && ctrd_h && asmt_h, "%s: NULL argument", who);
+// The checks both forms share, then Refine
+int RefineConv(bool target, qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, int K,
+               int d, int sweeps, const float* knl_h, const float* x, const float* t, int N, float* ctrd_h, uint8_t* asmt_h,
+               double* loss_h, void* stream) {
+  const char* who = target ? "qcnn_pq_refine_conv_target" : "qcnn_pq_refine_conv";
+  QCNN_CHECK(ctx && (target || knl_h) && ctrd_h && asmt_h, "%s: NULL argument", who);
   QCNN_CHECK(Cin >= 1 && Hin >= 1 && Win >= 1 && Cout >= 1 && ksz >= 1 && pad >= 0 && stride >= 1 && grp >= 1,
              "%s: bad geometry (Cin=%d Hin=%d Win=%d Cout=%d ksz=%d pad=%d stride=%d grp=%d)", who, Cin, Hin, Win, Cout, ksz, pad,
              stride, grp);
@@ -621,6 +645,7 @@ extern "C" int qcnn_pq_refine_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int
   QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
   QCNN_CHECK(N >= 1, "%s: N=%d: at least one input is needed", who, N);
   QCNN_CHECK(x, "%s: NULL argument", who);
+  QCNN_CHECK(!target || t, "%s: NULL t", who);
   Geometry geo;
   geo.Cin = Cin; geo.Hin = Hin; geo.Win = Win; geo.Cout = Cout; geo.ksz = ksz; geo.pad = pad; geo.stride = stride; geo.grp = grp;
   geo.Ho = (Hin + 2 * pad - ksz) / stride + 1;
@@ -629,5 +654,21 @@ extern "C" int qcnn_pq_refine_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int
   const long long sys = static_cast<long long>(K) * std::min(d, geo.Cg);
   QCNN_CHECK(sys <= kMaxSystem, "%s: K*min(d, Cin/grp) = %d*%d = %lld exceeds %d, the size of the joint codebook system", who, K,
              std::min(d, geo.Cg), sys, kMaxSystem);
-  return Refine(ctx, geo, K, d, sweeps, knl_h, x, N, ctrd_h, asmt_h, loss_h, static_cast<cudaStream_t>(stream));
+  return Refine(ctx, geo, K, d, sweeps, knl_h, x, t, N, ctrd_h, asmt_h, loss_h, static_cast<cudaStream_t>(stream));
+}
+
+}  // namespace
+
+extern "C" int qcnn_pq_refine_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, int K,
+                                   int d, int sweeps, const float* knl_h, const float* x, int N, float* ctrd_h, uint8_t* asmt_h,
+                                   double* loss_h, void* stream) {
+  return RefineConv(false, ctx, Cin, Hin, Win, Cout, ksz, pad, stride, grp, K, d, sweeps, knl_h, x, nullptr, N,
+                    ctrd_h, asmt_h, loss_h, stream);
+}
+
+extern "C" int qcnn_pq_refine_conv_target(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp,
+                                          int K, int d, int sweeps, const float* y, const float* t, int N, float* ctrd_h,
+                                          uint8_t* asmt_h, double* loss_h, void* stream) {
+  return RefineConv(true, ctx, Cin, Hin, Win, Cout, ksz, pad, stride, grp, K, d, sweeps, nullptr, y, t, N,
+                    ctrd_h, asmt_h, loss_h, stream);
 }

@@ -1,0 +1,186 @@
+"""The paper's multi-layer error correction on the shipped AlexNet, as a caller loop over the per-layer primitives.
+
+The shipped parameters, decoded, are the "original" network.  In layer order (conv1 ... fc8) every PQ layer is
+re-quantized coarser than shipped (conv K = 32, d = 8; fc6 / fc7 K = 16, d = 8; fc8 K = 16, d = 4) in three ways.
+conv1 has 3 input channels, so any d >= 3 gives it one 3-dim subspace; its codebook is stored d = 4 wide by default
+(the same quantization as d = 3; DESIGN.md 4e says why):
+  kmeans      pq_quantize_* only (iters = 20);
+  same-input  that start refined with pq_refine_* on the layer's inputs in the quantized network;
+  target      that start refined with pq_refine_*_target: the same inputs toward the original network's pre-bias
+              responses of the layer (t = W x on the original network's inputs x).
+The inputs of layer l come from a net in which every layer before l is already replaced by that mode's result
+(po.save_model into a temporary directory, Net.featmap under keep_maps).  Calibration and held-out images are seeded
+LCG images (po.lcg_images).  Reports per layer and mode the training loss ratio and the call time, per mode the held-out
+relative error of the final logits against the original network's (over all images, and the median of the per-image
+errors) and the top-1 / top-5 agreement with its
+predictions (top-5: the original's top-1 class is among the mode's five best), and the card, its power limit and max SM
+clock, all from the same run.
+    python tools/pq_refine_chain.py [--train 4096] [--held 1024] [--sweeps 4] [--conv 32 8] [--fc8 16 4] [--out f.json]"""
+import argparse
+import importlib
+import json
+import os
+import sys
+import tempfile
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+from pq_refine_time import card   # noqa: E402
+
+NAMES = {0: "conv1", 4: "conv2", 8: "conv3", 10: "conv4", 12: "conv5", 15: "fc6", 18: "fc7", 21: "fc8"}
+MODES = ("kmeans", "same-input", "target")
+
+
+def decode(ctrd, asmt, cin):
+    """dense weights of a PQ layer: conv [Cout][Cg][k][k] from asmt [Cout][k][k][S], FC [Dout][Din] from asmt [Dout][S]"""
+    S = ctrd.shape[0]
+    g = ctrd[np.arange(S), asmt]
+    g = g.reshape(g.shape[:-2] + (-1,))[..., :cin]
+    return np.ascontiguousarray(np.moveaxis(g, -1, 1) if g.ndim == 4 else g, np.float32)
+
+
+def layer_inputs(net, l, imgs, batch, first_fc):
+    """featMapLst[l] on every image: NHWC for a conv layer, [N][Din] in fcntWei column order for an FC layer (the first
+    FC layer's NHWC map permuted to the NCHW flattening its weights use)"""
+    import torch
+    net.set_keep_maps(True)
+    out = []
+    for i in range(0, imgs.shape[0], batch):
+        xb = imgs[i:i + batch]
+        net.forward(xb)
+        m = net.featmap(l, xb.shape[0])
+        if l == first_fc:
+            m = m.permute(0, 3, 1, 2)
+        out.append(m.reshape(m.shape[0], -1).contiguous() if l >= first_fc else m)
+    return torch.cat(out)
+
+
+def response(L, x, W, batch):
+    """the original layer's pre-bias response, fp64 arithmetic rounded to fp32 (NHWC for conv)"""
+    import torch
+    import torch.nn.functional as F
+    Wt = torch.from_numpy(W).cuda().double()
+    out = []
+    for i in range(0, x.shape[0], batch):
+        xb = x[i:i + batch].double()
+        if W.ndim == 4:
+            y = F.conv2d(xb.permute(0, 3, 1, 2), Wt, stride=L["stride"], padding=L["pad"], groups=L["grp"])
+            out.append(y.permute(0, 2, 3, 1).float().contiguous())
+        else:
+            out.append((xb @ Wt.T).float())
+    return torch.cat(out)
+
+
+def logits(net, imgs, batch):
+    import torch
+    out = []
+    for i in range(0, imgs.shape[0], batch):
+        xb = imgs[i:i + batch]
+        lg = torch.empty((xb.shape[0], net.out_len), dtype=torch.float32, device="cuda")
+        net.forward(xb, logits=lg)
+        out.append(lg)
+    return torch.cat(out)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--train", type=int, default=4096, help="calibration images")
+    ap.add_argument("--held", type=int, default=1024, help="held-out images")
+    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--sweeps", type=int, default=4)
+    ap.add_argument("--conv", type=int, nargs=2, default=(32, 8), metavar=("K", "d"))
+    ap.add_argument("--conv1-d", type=int, default=4)
+    ap.add_argument("--fc", type=int, nargs=2, default=(16, 8), metavar=("K", "d"), help="fc6 and fc7")
+    ap.add_argument("--fc8", type=int, nargs=2, default=(16, 4), metavar=("K", "d"))
+    ap.add_argument("--seed", type=int, default=1000000, help="image seed: calibration, then held-out")
+    ap.add_argument("--out", default=None, help="also write the results as JSON here")
+    args = ap.parse_args()
+    import torch
+    from oracle import pyoracle as po
+    assert torch.cuda.is_available(), "needs a GPU"
+    assert po.have_alexnet(), "needs the shipped AlexNet parameters under oracle/_ref/data"
+    q = importlib.import_module("quantized-cnn_b200")
+    ctx = q.Context(0)
+    cfg = {l: tuple(args.conv) for l in (0, 4, 8, 10, 12)}
+    cfg[0] = (args.conv[0], args.conv1_d)
+    cfg.update({15: tuple(args.fc), 18: tuple(args.fc), 21: tuple(args.fc8)})
+    layers = po.alexnet_layers()
+    shapes = po.infer_shapes(layers, po.ALEXNET_IN)
+    first_fc = min(l for l in NAMES if layers[l]["type"] == po.FCNT)
+    params = po.load_model(po.ALEXNET_DIR, po.ALEXNET_PFX, layers)
+    cin = {l: shapes[l][2] // layers[l]["grp"] if layers[l]["type"] == po.CONV else int(np.prod(shapes[l])) for l in NAMES}
+    dense = {l: decode(params[l]["ctrd"], params[l]["asmt"], cin[l]) for l in NAMES}
+    train = torch.from_numpy(po.lcg_images(args.train, args.seed)).cuda()
+    held = torch.from_numpy(po.lcg_images(args.held, args.seed + args.train)).cuda()
+    hw = card()
+    print("card: %s (name, power limit, max SM clock)" % hw)
+    orig = q.Net(ctx, po.ALEXNET_DIR, po.ALEXNET_PFX, "AlexNet")
+    ref = logits(orig, held, args.batch).double()
+    qparams = {m: dict(params) for m in MODES}
+    rows = []
+    with tempfile.TemporaryDirectory() as tmp:
+        def net_of(mode):
+            path = os.path.join(tmp, mode)
+            po.save_model(path, po.ALEXNET_PFX, qparams[mode])
+            return q.Net(ctx, path, po.ALEXNET_PFX, "AlexNet")
+
+        for l in sorted(NAMES):
+            L, W, (K, d) = layers[l], dense[l], cfg[l]
+            conv = L["type"] == po.CONV
+            quant = q.pq_quantize_conv if conv else q.pq_quantize_fc
+            c0, a0, _ = quant(ctx, W, K, d, iters=20, seed=1)
+            t = response(L, layer_inputs(orig, l, train, args.batch, first_fc), W, args.batch)
+            for mode in MODES:
+                c, a, ratio, secs = c0, a0, None, None
+                if mode != "kmeans":
+                    net = net_of(mode)
+                    y = layer_inputs(net, l, train, args.batch, first_fc)
+                    net.close()
+                    geo = dict(pad=L["pad"], stride=L["stride"], grp=L["grp"]) if conv else {}
+                    torch.cuda.synchronize()
+                    t0 = time.perf_counter()
+                    if mode == "same-input":
+                        fn = q.pq_refine_conv if conv else q.pq_refine_fc
+                        c, a, loss = fn(ctx, W, y, c0, a0, sweeps=args.sweeps, **geo)
+                    elif conv:
+                        c, a, loss = q.pq_refine_conv_target(ctx, y, t, c0, a0, L["k"], sweeps=args.sweeps, **geo)
+                    else:
+                        c, a, loss = q.pq_refine_fc_target(ctx, y, t, c0, a0, sweeps=args.sweeps)
+                    secs = time.perf_counter() - t0
+                    ratio = float(loss[-1] / loss[0])
+                    del y
+                qparams[mode][l] = dict(bias=params[l]["bias"], ctrd=c, asmt=a, bits=po.bits_for(K))
+                rows.append(dict(layer=NAMES[l], K=K, d=d, mode=mode, loss_ratio=ratio, call_s=secs))
+                if ratio is not None:
+                    print("%-6s K=%-3d d=%-2d %-10s training loss x%.4f  call %.2f s" % (NAMES[l], K, d, mode, ratio, secs))
+            del t
+            torch.cuda.empty_cache()
+        orig.close()
+        top1 = ref.argmax(1)
+        summary = []
+        for mode in MODES:
+            net = net_of(mode)
+            lg = logits(net, held, args.batch).double()
+            net.close()
+            err = ((lg - ref).norm() / ref.norm()).item()
+            med = ((lg - ref).norm(dim=1) / ref.norm(dim=1)).median().item()
+            agree1 = (lg.argmax(1) == top1).double().mean().item()
+            agree5 = (lg.topk(5, 1).indices == top1[:, None]).any(1).double().mean().item()
+            summary.append(dict(mode=mode, logit_rel_err=err, logit_rel_err_median=med, top1_agree=agree1,
+                                top5_agree=agree5))
+            print("%-10s held-out logits relative error %.4f (per image, median %.4f)  top-1 agreement %.4f  "
+                  "top-5 agreement %.4f" % (mode, err, med, agree1, agree5))
+    if args.out:
+        with open(args.out, "w") as f:
+            json.dump(dict(card=hw, train=args.train, held=args.held, sweeps=args.sweeps, layers=rows, modes=summary), f,
+                      indent=1)
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()

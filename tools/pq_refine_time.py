@@ -13,11 +13,15 @@ blocks, panels, their trailing GEMMs, the solve), the assignment step, the respo
 the joint system (member lists, M, b); fp64 TFLOP/s of the Gram (positions Dg (Dg + 1) per group), of the GEMMs
 (2 Cout (sum_m (k^2 w_m)^2 + Dg^2)) and of the Cholesky ((K w_m)^3 / 3 per subspace, every cluster in use); the wall
 time of a whole call with the profiler off.
-    python tools/pq_refine_time.py [--sweeps 3] [--layers alexnet_fc6 alexnet_conv1 vgg16_conv1_2 ...]"""
+With --target the same layers run the target form (qcnn_pq_refine_fc_target / _conv_target) on targets
+t = (the layer's response) + 0.3 (a seeded Gaussian), and each layer also reports the cross-product GEMM P = T^T Y next
+to the Gram, with its fp64 TFLOP/s (2 N Din Dout for FC, 2 positions Cout Cg k^2 for conv).
+    python tools/pq_refine_time.py [--sweeps 3] [--target] [--layers alexnet_fc6 alexnet_conv1 vgg16_conv1_2 ...]"""
 import argparse
 import importlib
 import json
 import os
+import re
 import subprocess
 import sys
 import time
@@ -61,8 +65,20 @@ def kernels(prof):
     return sorted(ev, key=lambda x: x[1])
 
 
-def time_conv(q, ctx, name, sweeps):
+def gemm_mode(name):
+    """pqr_gemm_kernel's template argument (0: fp64 GEMM, 1: Gram, 2: cross product), or None for another kernel"""
+    m = re.search(r"pqr_gemm_kernel<(?:\(int\))?(\d)>", name)
+    return int(m.group(1)) if m else None
+
+
+def loss_ends(ev):
+    """indices of the loss kernels that close the start and every sweep (not the |T|^2 reduction's final kernel)"""
+    return [i for i, (n, _, _) in enumerate(ev) if "pqr_loss_final" in n and not (i > 0 and "pqr_sqnorm" in ev[i - 1][0])]
+
+
+def time_conv(q, ctx, name, sweeps, target):
     import torch
+    import torch.nn.functional as F
     from torch.profiler import ProfilerActivity, profile
     Cin, H, Cout, k, pad, stride, grp, K, d, N = CONV_LAYERS[name]
     Cg = Cin // grp
@@ -70,14 +86,23 @@ def time_conv(q, ctx, name, sweeps):
     g = torch.Generator(device="cuda").manual_seed(2)
     x = torch.randn((N, H, H, Cin), generator=g, device="cuda", dtype=torch.float32)
     c0, a0, _ = q.pq_quantize_conv(ctx, W, K, d, iters=20, seed=3)
-    q.pq_refine_conv(ctx, W, x[:1], c0, a0, pad=pad, stride=stride, grp=grp, sweeps=1)   # warm-up
+    if target:
+        tg = F.conv2d(x.permute(0, 3, 1, 2), torch.from_numpy(W).cuda(), stride=stride, padding=pad, groups=grp)
+        tg = tg.permute(0, 2, 3, 1).contiguous()
+        tg += 0.3 * torch.randn(tg.shape, generator=g, device="cuda", dtype=torch.float32)
+        run = lambda xx, tt, s: q.pq_refine_conv_target(ctx, xx, tt, c0, a0, k, pad=pad, stride=stride, grp=grp, sweeps=s)
+    else:
+        tg = x
+        run = lambda xx, tt, s: q.pq_refine_conv(ctx, W, xx, c0, a0, pad=pad, stride=stride, grp=grp, sweeps=s)
+    run(x[:1], tg[:1], 1)   # warm-up
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        _, _, loss = q.pq_refine_conv(ctx, W, x, c0, a0, pad=pad, stride=stride, grp=grp, sweeps=sweeps)
+        _, _, loss = run(x, tg, sweeps)
         torch.cuda.synchronize()
     ev = kernels(prof)
-    gram = sum(t for n, _, t in ev if "pqr_gemm_kernel<true>" in n or "pqrc_patch" in n)
-    ends = [i for i, (n, _, _) in enumerate(ev) if "pqr_loss_final" in n]
+    gram = sum(t for n, _, t in ev if gemm_mode(n) == 1 or "pqrc_patch" in n)
+    cross = sum(t for n, _, t in ev if gemm_mode(n) == 2)
+    ends = loss_ends(ev)
     split = dict(chol=[], assign=[], gemm=[], system=[], total=[])
     for a, b in zip(ends[:-1], ends[1:]):
         part, in_chol = ev[a + 1:b + 1], False
@@ -89,7 +114,7 @@ def time_conv(q, ctx, name, sweeps):
                 acc["chol"] += t
             elif "pqrc_assign" in n or "pqrc_ccost" in n:
                 acc["assign"] += t
-            elif "pqr_gemm_kernel<false>" in n:
+            elif gemm_mode(n) == 0:
                 acc["gemm"] += t
             elif "pqr_loss" not in n:
                 acc["system"] += t
@@ -100,7 +125,7 @@ def time_conv(q, ctx, name, sweeps):
             split[key].append(acc[key])
     med = {key: float(np.median(v)) / 1e3 for key, v in split.items()}
     t0 = time.perf_counter()
-    q.pq_refine_conv(ctx, W, x, c0, a0, pad=pad, stride=stride, grp=grp, sweeps=sweeps)
+    run(x, tg, sweeps)
     wall = time.perf_counter() - t0
     Ho = (H + 2 * pad - k) // stride + 1
     T, Dg, S = k * k, Cg * k * k, -(-Cg // d)
@@ -113,13 +138,16 @@ def time_conv(q, ctx, name, sweeps):
              sweep_ms=med["total"], sweep_chol_ms=med["chol"], sweep_assign_ms=med["assign"], sweep_gemm_ms=med["gemm"],
              sweep_system_ms=med["system"], gemm_tflops=gemm_flop / (med["gemm"] * 1e-3) / 1e12,
              chol_tflops=chol_flop / (med["chol"] * 1e-3) / 1e12, call_wall_s=wall,
-             loss=[float(v) for v in loss], loss_ratio=float(loss[-1] / loss[0]))
+             loss=[float(v) for v in loss], loss_ratio=float(loss[-1] / loss[0]), target=target)
+    if target:
+        r.update(cross_ms=cross / 1e3, cross_tflops=2.0 * N * Ho * Ho * Cout * Dg / (cross * 1e-6) / 1e12)
+        print("%-14s cross product %8.2f ms (%5.1f TFLOP/s)" % (name, r["cross_ms"], r["cross_tflops"]))
     print("%-14s Gram %8.2f ms (%5.1f TFLOP/s)  sweep %8.2f ms (Cholesky %.2f ms %.2f TFLOP/s, assignment %.2f ms, "
           "GEMMs %.2f ms %.1f TFLOP/s, system %.2f ms)  call %.2f s  loss x%.3f after %d sweeps"
           % (name, r["gram_ms"], r["gram_tflops"], r["sweep_ms"], r["sweep_chol_ms"], r["chol_tflops"],
              r["sweep_assign_ms"], r["sweep_gemm_ms"], r["gemm_tflops"], r["sweep_system_ms"], wall, r["loss_ratio"],
              sweeps))
-    del x
+    del x, tg
     torch.cuda.empty_cache()
     return r
 
@@ -128,6 +156,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--sweeps", type=int, default=3)
     ap.add_argument("--layers", nargs="*", default=list(LAYERS) + list(CONV_LAYERS))
+    ap.add_argument("--target", action="store_true", help="time the target form (with the cross-product GEMM)")
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
     args = ap.parse_args()
     import torch
@@ -139,29 +168,36 @@ def main():
     results = []
     for name in args.layers:
         if name in CONV_LAYERS:
-            results.append(time_conv(q, ctx, name, args.sweeps))
+            results.append(time_conv(q, ctx, name, args.sweeps, args.target))
             continue
         Din, Dout, K, d, N = LAYERS[name]
         W = (np.random.default_rng(1).standard_normal((Dout, Din), dtype=np.float32) / np.float32(np.sqrt(Din)))
         g = torch.Generator(device="cuda").manual_seed(2)
         x = torch.randn((N, Din), generator=g, device="cuda", dtype=torch.float32)
         c0, a0, _ = q.pq_quantize_fc(ctx, W, K, d, iters=20, seed=3)
-        q.pq_refine_fc(ctx, W, x[:64], c0, a0, sweeps=1)   # warm-up: module load, smem opt-in
+        if args.target:
+            tg = x @ torch.from_numpy(W).cuda().T + 0.3 * torch.randn((N, Dout), generator=g, device="cuda")
+            run = lambda xx, tt, s: q.pq_refine_fc_target(ctx, xx, tt, c0, a0, sweeps=s)
+        else:
+            tg = x
+            run = lambda xx, tt, s: q.pq_refine_fc(ctx, W, xx, c0, a0, sweeps=s)
+        run(x[:64], tg[:64], 1)   # warm-up: module load, smem opt-in
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            _, _, loss = q.pq_refine_fc(ctx, W, x, c0, a0, sweeps=args.sweeps)
+            _, _, loss = run(x, tg, args.sweeps)
             torch.cuda.synchronize()
         ev = kernels(prof)
-        gram = sum(t for n, _, t in ev if "pqr_gemm_kernel<true>" in n)
-        ends = [i for i, (n, _, _) in enumerate(ev) if "pqr_loss_final" in n]
+        gram = sum(t for n, _, t in ev if gemm_mode(n) == 1)
+        cross = sum(t for n, _, t in ev if gemm_mode(n) == 2)
+        ends = loss_ends(ev)
         sweeps, blk, trail = [], [], []
         for a, b in zip(ends[:-1], ends[1:]):
             part = ev[a + 1:b + 1]
             sweeps.append(sum(t for _, _, t in part))
             blk.append(sum(t for n, _, t in part if "pqr_block_kernel" in n))
-            trail.append(sum(t for n, _, t in part if "pqr_gemm_kernel<false>" in n))
+            trail.append(sum(t for n, _, t in part if gemm_mode(n) == 0))
         t0 = time.perf_counter()
-        q.pq_refine_fc(ctx, W, x, c0, a0, sweeps=args.sweeps)
+        run(x, tg, args.sweeps)
         wall = time.perf_counter() - t0
         sweep_ms = float(np.median(sweeps)) / 1e3
         gram_ms = gram / 1e3
@@ -169,14 +205,17 @@ def main():
                  gram_tflops=N * Din * (Din + 1) / (gram_ms * 1e-3) / 1e12, sweep_ms=sweep_ms,
                  sweep_block_kernel_ms=float(np.median(blk)) / 1e3, sweep_gemm_ms=float(np.median(trail)) / 1e3,
                  sweep_tflops=2.0 * Dout * Din * Din / (sweep_ms * 1e-3) / 1e12, call_wall_s=wall,
-                 loss=[float(v) for v in loss], loss_ratio=float(loss[-1] / loss[0]))
+                 loss=[float(v) for v in loss], loss_ratio=float(loss[-1] / loss[0]), target=args.target)
+        if args.target:
+            r.update(cross_ms=cross / 1e3, cross_tflops=2.0 * N * Din * Dout / (cross * 1e-6) / 1e12)
+            print("%-12s cross product %8.2f ms (%5.1f TFLOP/s)" % (name, r["cross_ms"], r["cross_tflops"]))
         results.append(r)
         print("%-12s Gram %8.2f ms (%5.1f TFLOP/s)  sweep %8.2f ms (%5.1f TFLOP/s; block kernels %.2f ms, GEMMs %.2f ms)  "
               "call %.2f s  loss x%.3f after %d sweeps"
               % (name, gram_ms, r["gram_tflops"], sweep_ms, r["sweep_tflops"], r["sweep_block_kernel_ms"],
                  r["sweep_gemm_ms"], wall, r["loss_ratio"], args.sweeps))
         print("  loss trace: " + " ".join("%.6g" % v for v in loss))
-        del x
+        del x, tg
         torch.cuda.empty_cache()
     if args.out:
         with open(args.out, "w") as f:
