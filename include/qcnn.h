@@ -348,8 +348,8 @@ QCNN_API int qcnn_pq_refine_fc(qcnn_ctx* ctx, int Din, int Dout, int K, int d, i
  * ctrd_h [S][K][d] and asmt_h [Cout][k][k][S] (0-based) are the start and receive the result; loss_h (nullable, sweeps + 1
  * values) = the start's loss, then the loss after each sweep.  Results are bit-reproducible.  Runs on `stream` (ordered
  * after whatever produced x) and synchronises it before returning.  Device memory: 8 grp (Cg k^2)^2 bytes for the Grams,
- * 20 Cout Cg k^2 for E, G E and the weights, 16 (K min(d, Cg))^2 for M and its factor, 24 Cout k^2 min(d, Cg) for one
- * subspace's responses, and one chunk of at most 256 MiB of patches.  Fails on what qcnn_pq_quantize_conv refuses (K not
+ * 20 Cout Cg k^2 for E, G E and the weights, 16 (K min(d, Cg))^2 for M and its factor, and 24 Cout k^2 min(d, Cg) for
+ * one subspace's responses; the Grams read the patches straight from x.  Fails on what qcnn_pq_quantize_conv refuses (K not
  * a multiple of 8 in 8..256, d outside 1..64, non-finite weights or codebook), non-finite x, sweeps < 0, N < 1, an
  * assignment >= K, Cin or Cout not divisible by grp, an empty output, K min(d, Cg) > 2048 (the size of the joint
  * system), or a failed allocation (with its byte count). */
@@ -390,6 +390,46 @@ QCNN_API int qcnn_pq_refine_conv_target(qcnn_ctx* ctx, int Cin, int Hin, int Win
                                         const float* t /*device NHWC [N][Ho][Wo][Cout]*/, int N,
                                         float* ctrd_h /*in/out [S][K][d]*/, uint8_t* asmt_h /*in/out [Cout][k][k][S], 0-based*/,
                                         double* loss_h /*nullable [sweeps + 1]*/, void* stream);
+/* Calibration statistics of one layer for one subspace width d (DESIGN.md 4e), so that the calibration set can be
+ * streamed in batches: the refine calls above reduce their inputs to sums over images before the first sweep (G, and for
+ * the target form P and |T|^2), and these objects accumulate those sums batch by batch.  Device memory does not depend
+ * on the number of images: an FC object holds 8 Din^2 bytes (plus 8 Dout Din for a target object), a conv object
+ * 8 grp Dg^2 (plus 8 Cout Dg), Dg = Cg k^2, and about 4 KiB more.  The qcnn_pq_refine_* calls above are create, one add
+ * of all N images, refine and destroy on these objects.
+ * Dim order: FC, the input column; conv, the internal order of the refine code for d, q = m d k^2 + t w_m + j (subspace
+ *   m, tap t = kh k + kw, channel m d + j of the group, w_m = min(d, Cg - m d)), so each G^m is a diagonal block.
+ * Accumulation order (normative; one add of all N images is exactly the arithmetic of the one-shot call):
+ *   FC: an add is one fold, G <- G + Y_b^T Y_b and P <- P + T_b^T Y_b, each a fresh fixed-order GEMM; the first add
+ *   stores instead of adding.  Conv: an add folds its positions (n Ho + oy) Wo + ox (n counted within the batch) in runs
+ *   of F = max(1, min(P_b, floor(2^28 / (4 Dg)))) positions, each run a fresh sum over 16-position k-steps in ascending
+ *   order, added to G_g (and P_g) in ascending order.  |T|^2 <- |T|^2 + |T_b|^2, |T_b|^2 a fixed-order fp64 sum of the
+ *   fp32 squares.
+ * create: target != 0 also keeps P and |T|^2 (and then every add needs t).  Fails on the geometry the matching refine
+ *   call refuses, d outside 1..64, or a failed allocation.
+ * add: scans y and (target) t for NaN or Inf, synchronising `stream` once, then queues the accumulation on `stream` and
+ *   returns; y and t must stay valid until the stream reaches it.  A rejected add (non-finite y or t, t given to a
+ *   same-input object or missing on a target object, N < 1, NULL y) leaves the statistics and the count unchanged.
+ * read_h: waits for the queued adds and copies each non-NULL output (G [grp][Dg][Dg], FC [Din][Din]; P [Cout][Dg], FC
+ *   [Dout][Din]; |T|^2 one double); P and |T|^2 need a target object.  Before any add the sums are zero.
+ * refine / refine_target: the sweeps of qcnn_pq_refine_{fc,conv} / _target on the statistics, with the same arguments,
+ *   results and checks (K, the joint-system limit, an assignment >= K, a non-finite codebook or weights) plus a call
+ *   before any add; refine works on either kind of object (it reads only G), refine_target needs a target object.  They
+ *   read the statistics and never change them, so either may run any number of times.  They wait for the queued adds,
+ *   run on `stream` and synchronise it; device memory is that of the one-shot call less G and P. */
+typedef struct qcnn_pq_stats qcnn_pq_stats;
+QCNN_API int qcnn_pq_stats_create_fc(qcnn_ctx* ctx, int Din, int Dout, int d, int target, qcnn_pq_stats** out);
+QCNN_API int qcnn_pq_stats_create_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride,
+                                       int grp, int d, int target, qcnn_pq_stats** out);
+/* y: device [N][Din] / NHWC [N][Hin][Win][Cin]; t: device [N][Dout] / NHWC [N][Ho][Wo][Cout], NULL unless target */
+QCNN_API int qcnn_pq_stats_add(qcnn_pq_stats* s, const float* y, const float* t, int N, void* stream);
+QCNN_API int qcnn_pq_stats_count(const qcnn_pq_stats* s, long long* images);
+/* host copies (each nullable): G [grp][Dg][Dg] (FC: [Din][Din]), P [Cout][Dg] (FC: [Dout][Din]), |T|^2 */
+QCNN_API int qcnn_pq_stats_read_h(const qcnn_pq_stats* s, double* G_h, double* P_h, double* tt_h);
+QCNN_API int qcnn_pq_stats_refine(qcnn_pq_stats* s, int K, int sweeps, const float* wei_h /* fcntWei or convKnl */,
+                                  float* ctrd_h, uint8_t* asmt_h, double* loss_h, void* stream);
+QCNN_API int qcnn_pq_stats_refine_target(qcnn_pq_stats* s, int K, int sweeps, float* ctrd_h, uint8_t* asmt_h,
+                                         double* loss_h, void* stream);
+QCNN_API void qcnn_pq_stats_destroy(qcnn_pq_stats* s);
 
 /* ---- file formats (include/FileIO.h:56-178, 229-350), host only ------------------------------------------- */
 /* .bin: returns element count or -1; dims4 padded with 1; data_h may be NULL to query the shape */

@@ -133,6 +133,14 @@ _SIGS = {
     "qcnn_pq_refine_conv": (_i, [_vp] + [_i] * 11 + [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "qcnn_pq_refine_fc_target": (_i, [_vp] + [_i] * 5 + [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
     "qcnn_pq_refine_conv_target": (_i, [_vp] + [_i] * 11 + [_vp, _vp, _i, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_stats_create_fc": (_i, [_vp] + [_i] * 4 + [C.POINTER(_vp)]),
+    "qcnn_pq_stats_create_conv": (_i, [_vp] + [_i] * 10 + [C.POINTER(_vp)]),
+    "qcnn_pq_stats_add": (_i, [_vp, _vp, _vp, _i, _vp]),
+    "qcnn_pq_stats_count": (_i, [_vp, C.POINTER(C.c_longlong)]),
+    "qcnn_pq_stats_read_h": (_i, [_vp, _vp, _vp, _vp]),
+    "qcnn_pq_stats_refine": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_stats_refine_target": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_stats_destroy": (None, [_vp]),
 }
 for _name, (_res, _args) in _SIGS.items():
     _fn = getattr(lib, _name)
@@ -755,3 +763,129 @@ def pq_refine_conv_target(ctx, y, t, ctrd, asmt, ksz, pad=0, stride=1, grp=1, sw
                                           _dptr(t), N, ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp),
                                           loss.ctypes.data_as(_vp), _stream(stream)))
     return ctrd, asmt, loss
+
+
+class PqStats(object):
+    """Calibration statistics of one layer for one subspace width d (include/qcnn.h, DESIGN.md 4e): add() folds a batch
+    of layer inputs y (and, with target=True, the original layer's responses t) into the sums the error-correcting
+    refinement reads, so the calibration set can be streamed in batches; refine() / refine_target() then run the sweeps
+    of pq_refine_* / pq_refine_*_target on the sums, any number of times.  Device memory does not grow with the number
+    of images."""
+
+    def __init__(self, ctx, h, conv, shape, target):
+        self.ctx, self.h, self.conv, self.target = ctx, h, conv, target
+        self._shape = shape
+
+    @classmethod
+    def fc(cls, ctx, Din, Dout, d, target=False):
+        h = _vp()
+        _check(lib.qcnn_pq_stats_create_fc(ctx.h, Din, Dout, d, int(bool(target)), C.byref(h)))
+        return cls(ctx, h, False, dict(Din=Din, Dout=Dout, d=d), bool(target))
+
+    @classmethod
+    def conv(cls, ctx, Cin, Hin, Win, Cout, ksz, d, pad=0, stride=1, grp=1, target=False):
+        h = _vp()
+        _check(lib.qcnn_pq_stats_create_conv(ctx.h, Cin, Hin, Win, Cout, ksz, pad, stride, grp, d, int(bool(target)),
+                                             C.byref(h)))
+        Ho, Wo = (Hin + 2 * pad - ksz) // stride + 1, (Win + 2 * pad - ksz) // stride + 1
+        return cls(ctx, h, True, dict(Cin=Cin, Hin=Hin, Win=Win, Cout=Cout, ksz=ksz, pad=pad, stride=stride, grp=grp,
+                                      d=d, Ho=Ho, Wo=Wo), bool(target))
+
+    def _live(self):
+        if not self.h:
+            raise QcnnError("PqStats: closed")
+
+    def add(self, y, t=None, stream=None):
+        """Fold a batch: y [N, Din] (FC) or [N, Hin, Win, Cin] (NHWC conv), t [N, Dout] or [N, Ho, Wo, Cout] for a
+        target object, contiguous float32 CUDA tensors that must stay alive until the stream has run the add."""
+        self._live()
+        g = self._shape
+        N = y.shape[0] if y.dim() >= 1 else 0
+        want_y = (N, g["Din"]) if not self.conv else (N, g["Hin"], g["Win"], g["Cin"])
+        if tuple(y.shape) != want_y:
+            raise QcnnError("y must be %s, got %s" % (want_y, tuple(y.shape)))
+        if t is not None:
+            want_t = (N, g["Dout"]) if not self.conv else (N, g["Ho"], g["Wo"], g["Cout"])
+            if tuple(t.shape) != want_t:
+                raise QcnnError("t must be %s, got %s" % (want_t, tuple(t.shape)))
+        _check(lib.qcnn_pq_stats_add(self.h, _dptr(y), None if t is None else _dptr(t), N, _stream(stream)))
+
+    @property
+    def count(self):
+        """images added so far"""
+        self._live()
+        n = C.c_longlong()
+        _check(lib.qcnn_pq_stats_count(self.h, C.byref(n)))
+        return n.value
+
+    def read(self):
+        """(G, P, tt): G [grp, Dg, Dg] conv / [Din, Din] FC in the internal dim order, and for a target object
+        P [Cout, Dg] / [Dout, Din] and |T|^2 (else None, None), as float64 host arrays."""
+        self._live()
+        g = self._shape
+        if self.conv:
+            Dg = g["Cin"] // g["grp"] * g["ksz"] * g["ksz"]
+            G = np.empty((g["grp"], Dg, Dg), np.float64)
+            P = np.empty((g["Cout"], Dg), np.float64) if self.target else None
+        else:
+            G = np.empty((g["Din"], g["Din"]), np.float64)
+            P = np.empty((g["Dout"], g["Din"]), np.float64) if self.target else None
+        tt = np.empty(1, np.float64) if self.target else None
+        _check(lib.qcnn_pq_stats_read_h(self.h, G.ctypes.data_as(_vp), None if P is None else P.ctypes.data_as(_vp),
+                                        None if tt is None else tt.ctypes.data_as(_vp)))
+        return G, P, None if tt is None else float(tt[0])
+
+    def _start(self, ctrd, asmt):
+        ctrd = np.array(ctrd, np.float32, order="C", copy=True)
+        asmt = np.array(asmt, np.uint8, order="C", copy=True)
+        g = self._shape
+        S, K, d = ctrd.shape if ctrd.ndim == 3 else (0, 0, 0)
+        if self.conv:
+            Cg = g["Cin"] // g["grp"]
+            want = (g["Cout"], g["ksz"], g["ksz"], -(-Cg // g["d"]))
+            ok = d == g["d"] and S == want[3] and asmt.shape == want
+        else:
+            want = (g["Dout"], -(-g["Din"] // g["d"]))
+            ok = d == g["d"] and S == want[1] and asmt.shape == want
+        if not ok:
+            raise QcnnError("ctrd [%d, K, %d] and asmt %s must be [S, K, d] and %s" % (S, g["d"], tuple(asmt.shape), want))
+        return ctrd, asmt, K
+
+    def refine(self, wei, ctrd, asmt, sweeps=8, stream=None):
+        """The same-input sweeps (pq_refine_fc / pq_refine_conv) on the statistics and the dense weights wei
+        [Dout, Din] / [Cout, Cin / grp, k, k]: (ctrd, asmt, loss [sweeps + 1]).  The arguments are not modified."""
+        self._live()
+        ctrd, asmt, K = self._start(ctrd, asmt)
+        g = self._shape
+        wei = _np(wei, np.float32)
+        want = (g["Cout"], g["Cin"] // g["grp"], g["ksz"], g["ksz"]) if self.conv else (g["Dout"], g["Din"])
+        if wei.shape != want:
+            raise QcnnError("wei must be %s, got %s" % (want, wei.shape))
+        loss = np.empty(max(sweeps, 0) + 1, np.float64)
+        _check(lib.qcnn_pq_stats_refine(self.h, K, sweeps, wei.ctypes.data_as(_vp), ctrd.ctypes.data_as(_vp),
+                                        asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp), _stream(stream)))
+        return ctrd, asmt, loss
+
+    def refine_target(self, ctrd, asmt, sweeps=8, stream=None):
+        """The target sweeps (pq_refine_*_target) on the statistics of a target object: (ctrd, asmt, loss [sweeps + 1]).
+        The arguments are not modified."""
+        self._live()
+        ctrd, asmt, K = self._start(ctrd, asmt)
+        loss = np.empty(max(sweeps, 0) + 1, np.float64)
+        _check(lib.qcnn_pq_stats_refine_target(self.h, K, sweeps, ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp),
+                                               loss.ctypes.data_as(_vp), _stream(stream)))
+        return ctrd, asmt, loss
+
+    @property
+    def nbytes(self):
+        """device bytes of the sums (G, and for a target object P and |T|^2)"""
+        g = self._shape
+        if self.conv:
+            Dg = g["Cin"] // g["grp"] * g["ksz"] * g["ksz"]
+            return 8 * (g["grp"] * Dg * Dg + (g["Cout"] * Dg + 1 if self.target else 0))
+        return 8 * (g["Din"] * g["Din"] + (g["Dout"] * g["Din"] + 1 if self.target else 0))
+
+    def close(self):
+        if self.h:
+            lib.qcnn_pq_stats_destroy(self.h)
+            self.h = None

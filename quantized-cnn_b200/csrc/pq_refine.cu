@@ -21,6 +21,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <memory>
 #include <vector>
 
 #include "pq_refine_common.cuh"
@@ -261,32 +262,32 @@ __global__ void __launch_bounds__(kSweepThreads) pqr_block_kernel(BlockArgs p) {
   }
 }
 
-// target: the target form on the targets t (w_h is not read); else the same-input form on the weights w_h.
-int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int sweeps, const float* w_h, const float* x, const float* t,
-           int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
-  const char* who = target ? "qcnn_pq_refine_fc_target" : "qcnn_pq_refine_fc";
-  QCNN_CHECK(ctx && (target || w_h) && ctrd_h && asmt_h, "%s: NULL argument", who);
-  QCNN_CHECK(Din >= 1 && Dout >= 1, "%s: bad dimensions", who);
-  if (int rc = CheckFcK(who, K)) return rc;
-  QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
-  QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
-  QCNN_CHECK(N >= 1, "%s: N=%d: at least one input is needed", who, N);
-  QCNN_CHECK(x, "%s: NULL argument", who);
-  QCNN_CHECK(!target || t, "%s: NULL t", who);
+// The host-side checks of a refine (weights unless target, codebook, assignments) and the assignments as [S][Dout]
+int CheckFcHost(const char* who, bool target, int Din, int Dout, int K, int d, const float* w_h, const float* ctrd_h,
+                const uint8_t* asmt_h, std::vector<uint8_t>& at) {
   const int S = CeilDiv(Din, d);
   const size_t nw = static_cast<size_t>(Dout) * Din, nc = static_cast<size_t>(S) * K * d;
   if (!target) QCNN_CHECK(AllFinite(w_h, nw), "%s: the weights contain a non-finite value", who);
   QCNN_CHECK(AllFinite(ctrd_h, nc), "%s: the codebook contains a non-finite value", who);
-  std::vector<uint8_t> at(static_cast<size_t>(S) * Dout);   // [S][Dout]
+  at.assign(static_cast<size_t>(S) * Dout, 0);
   for (int o = 0; o < Dout; o++)
     for (int m = 0; m < S; m++) {
       const uint8_t a = asmt_h[static_cast<size_t>(o) * S + m];
       QCNN_CHECK(a < K, "%s: assignment %d of output %d, subspace %d is not below K=%d", who, a, o, m, K);
       at[static_cast<size_t>(m) * Dout + o] = a;
     }
+  return 0;
+}
+
+// The sweeps on the statistics of s.  target: the target form (w_h is not read); else the same-input form on w_h.
+int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* w_h, std::vector<uint8_t>& at,
+            float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+  qcnn_ctx* ctx = s->ctx;
+  const int Din = s->Din, Dout = s->Dout, d = s->d, S = CeilDiv(Din, d);
+  const size_t nw = static_cast<size_t>(Dout) * Din, nc = static_cast<size_t>(S) * K * d;
   QCNN_ON_DEVICE(ctx->device);
   const int spb = std::max(1, kBlockDims / d), ld = spb * d;
-  DeviceBuffer dG, dE, dGE, dW, dC, dA, dL, dDlt, dH, dCc, dPart, dLoss, dTY, dTT;
+  DeviceBuffer dE, dGE, dW, dC, dA, dL, dDlt, dH, dCc, dPart, dLoss;
   auto reserve = [&](DeviceBuffer& b, size_t bytes, const char* what) -> int {
     const cudaError_t e = b.Reserve(ctx, bytes);
     if (e == cudaSuccess) return 0;
@@ -294,54 +295,36 @@ int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int swee
     SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
     return 1;
   };
-  if (reserve(dG, sizeof(double) * Din * static_cast<size_t>(Din), "the Gram matrix") ||
-      reserve(dE, sizeof(double) * nw, "the residual") || reserve(dGE, sizeof(double) * nw, "G times the residual") ||
+  if (reserve(dE, sizeof(double) * nw, "the residual") || reserve(dGE, sizeof(double) * nw, "G times the residual") ||
       reserve(dW, sizeof(float) * nw, "the weights") || reserve(dC, sizeof(float) * nc, "the codebook") ||
       reserve(dA, at.size(), "the assignments") ||
       reserve(dL, sizeof(double) * static_cast<size_t>(S) * d * d, "the Cholesky factors") ||
       reserve(dDlt, sizeof(double) * Dout * static_cast<size_t>(ld), "the block's changes") ||
       reserve(dH, sizeof(double) * Dout * static_cast<size_t>(d), "the subspace responses") ||
       reserve(dCc, sizeof(double) * K, "the codeword norms") || reserve(dPart, sizeof(double) * kLossBlocks, "the loss") ||
-      reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss") ||
-      reserve(dTY, target ? sizeof(double) * nw : 0, "the targets' cross product") ||
-      reserve(dTT, target ? sizeof(double) : 0, "the targets' norm"))
+      reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss"))
     return 1;
+  const double* G = s->G.as<double>();
+  const double* TY = target ? s->P.as<double>() : nullptr;
+  QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
   if (target) QCNN_CUDA(cudaMemsetAsync(dW.get(), 0, sizeof(float) * nw, st));   // E = 0 - W^
   else QCNN_CUDA(cudaMemcpyAsync(dW.get(), w_h, sizeof(float) * nw, cudaMemcpyHostToDevice, st));
   QCNN_CUDA(cudaMemcpyAsync(dC.get(), ctrd_h, sizeof(float) * nc, cudaMemcpyHostToDevice, st));
   QCNN_CUDA(cudaMemcpyAsync(dA.get(), at.data(), at.size(), cudaMemcpyHostToDevice, st));
-  // G = X^T X, then its diagonal: a NaN or Inf anywhere in x makes one entry non-finite (fp32 squares cannot overflow it)
   const int tiles = CeilDiv(Din, kTile);
-  pqr_gemm_kernel<kGemmGram><<<tiles * (tiles + 1) / 2, kGemmThreads, 0, st>>>(x, Din, nullptr, 0, dG.as<double>(), Din, Din, Din, N, 0);
-  QCNN_CUDA(cudaGetLastError());
   const dim3 gemmGrid(tiles, CeilDiv(Dout, kTile));
-  double tt = 0.0;
-  if (target) {   // |T|^2 (non-finite exactly when t is) and P = T^T Y
-    if (int rc = LaunchSqNorm(t, static_cast<size_t>(N) * Dout, dPart.as<double>(), dTT.as<double>(), st)) return rc;
-    pqr_gemm_kernel<kGemmCross><<<gemmGrid, kGemmThreads, 0, st>>>(t, Dout, x, Din, dTY.as<double>(), Din, Dout, Din, N, 0);
-    QCNN_CUDA(cudaGetLastError());
-    QCNN_CUDA(cudaMemcpyAsync(&tt, dTT.get(), sizeof(double), cudaMemcpyDeviceToHost, st));
-  }
-  std::vector<double> diag(Din);
-  QCNN_CUDA(cudaMemcpy2DAsync(diag.data(), sizeof(double), dG.get(), sizeof(double) * (static_cast<size_t>(Din) + 1),
-                              sizeof(double), Din, cudaMemcpyDeviceToHost, st));
-  QCNN_CUDA(cudaStreamSynchronize(st));
-  for (int c = 0; c < Din; c++) QCNN_CHECK(isfinite(diag[c]), "%s: %s contains a non-finite value (input column %d)", who,
-                                              target ? "y" : "x", c);
-  QCNN_CHECK(isfinite(tt), "%s: t contains a non-finite value", who);
   const size_t cholSmem = sizeof(double) * 2 * std::min(d, Din) * (std::min(d, Din) + 1);
   if (int rc = OptInSmem<pqr_chol_kernel>(ctx)) return rc;
-  pqr_chol_kernel<<<S, kSweepThreads, cholSmem, st>>>(dG.as<double>(), dL.as<double>(), Din, d);
+  pqr_chol_kernel<<<S, kSweepThreads, cholSmem, st>>>(G, dL.as<double>(), Din, d);
   const int ewBlocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 32u * ctx->sm_count));
   pqr_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Din, Dout, K, d);
   // GE = E G, or P + E G for a target
-  if (target) QCNN_CUDA(cudaMemcpyAsync(dGE.get(), dTY.get(), sizeof(double) * nw, cudaMemcpyDeviceToDevice, st));
-  pqr_gemm_kernel<kGemmF64><<<gemmGrid, kGemmThreads, 0, st>>>(dE.get(), Din, dG.get(), Din, dGE.as<double>(), Din, Dout, Din, Din,
-                                                               target);
+  if (target) QCNN_CUDA(cudaMemcpyAsync(dGE.get(), TY, sizeof(double) * nw, cudaMemcpyDeviceToDevice, st));
+  pqr_gemm_kernel<kGemmF64><<<gemmGrid, kGemmThreads, 0, st>>>(dE.get(), Din, G, Din, dGE.as<double>(), Din, Dout, Din, Din, target);
   QCNN_CUDA(cudaGetLastError());
   auto loss = [&](int sw) -> int {
-    return LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st,
-                      target ? dTY.as<double>() : nullptr, dTT.as<double>());
+    return LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st, TY,
+                      target ? s->tt.as<double>() : nullptr);
   };
   if (int rc = loss(0)) return rc;
   if (sweeps > 0) {
@@ -354,7 +337,7 @@ int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int swee
     QCNN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, pqr_block_kernel, kSweepThreads, blkSmem));
     QCNN_CHECK(perSm >= 1, "%s: the sweep kernel does not fit on an SM", who);
     const int grid = std::min(std::min(perSm, 2) * ctx->sm_count, std::max(Dout, K));
-    BlockArgs a{dG.as<double>(), dGE.as<double>(), dL.as<double>(), dE.as<double>(), dDlt.as<double>(), dH.as<double>(),
+    BlockArgs a{G, dGE.as<double>(), dL.as<double>(), dE.as<double>(), dDlt.as<double>(), dH.as<double>(),
                 dCc.as<double>(), dC.as<float>(), dA.as<uint8_t>(), Din, Dout, K, d, ld, 0, 0};
     for (int sw = 1; sw <= sweeps; sw++) {
       for (int m0 = 0; m0 < S; m0 += spb) {
@@ -364,8 +347,8 @@ int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int swee
         QCNN_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(pqr_block_kernel), grid, kSweepThreads, args, blkSmem, st));
         // GE += dlt G[block dims][:]
         const int blk0 = m0 * d, bw = std::min(Din, a.m1 * d) - blk0;
-        pqr_gemm_kernel<kGemmF64><<<gemmGrid, kGemmThreads, 0, st>>>(dDlt.get(), ld, dG.as<double>() + static_cast<size_t>(blk0) * Din,
-                                                                  Din, dGE.as<double>(), Din, Dout, Din, bw, 1);
+        pqr_gemm_kernel<kGemmF64><<<gemmGrid, kGemmThreads, 0, st>>>(dDlt.get(), ld, G + static_cast<size_t>(blk0) * Din, Din,
+                                                                  dGE.as<double>(), Din, Dout, Din, bw, 1);
         QCNN_CUDA(cudaGetLastError());
       }
       if (int rc = loss(sw)) return rc;
@@ -382,7 +365,81 @@ int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int swee
   return 0;
 }
 
+int CreateFc(qcnn_ctx* ctx, const char* who, int Din, int Dout, int d, bool target, qcnn_pq_stats** out) {
+  QCNN_CHECK(ctx && out, "%s: NULL argument", who);
+  *out = nullptr;
+  QCNN_CHECK(Din >= 1 && Dout >= 1, "%s: bad dimensions", who);
+  QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
+  std::unique_ptr<qcnn_pq_stats> s(new qcnn_pq_stats);
+  s->ctx = ctx;
+  s->conv = false;
+  s->target = target;
+  s->d = d;
+  s->Din = Din;
+  s->Dout = Dout;
+  if (AllocStats(s.get(), who, sizeof(double) * Din * static_cast<size_t>(Din), sizeof(double) * Dout * static_cast<size_t>(Din)))
+    return 1;
+  *out = s.release();
+  return 0;
+}
+
+// The one-shot calls: create, one add of all N inputs, the sweeps, destroy (the checks keep the order of their messages)
+int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int sweeps, const float* w_h, const float* x, const float* t,
+           int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+  const char* who = target ? "qcnn_pq_refine_fc_target" : "qcnn_pq_refine_fc";
+  QCNN_CHECK(ctx && (target || w_h) && ctrd_h && asmt_h, "%s: NULL argument", who);
+  QCNN_CHECK(Din >= 1 && Dout >= 1, "%s: bad dimensions", who);
+  if (int rc = CheckFcK(who, K)) return rc;
+  QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
+  QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
+  QCNN_CHECK(N >= 1, "%s: N=%d: at least one input is needed", who, N);
+  QCNN_CHECK(x, "%s: NULL argument", who);
+  QCNN_CHECK(!target || t, "%s: NULL t", who);
+  std::vector<uint8_t> at;
+  if (int rc = CheckFcHost(who, target, Din, Dout, K, d, w_h, ctrd_h, asmt_h, at)) return rc;
+  qcnn_pq_stats* sp = nullptr;
+  if (int rc = CreateFc(ctx, who, Din, Dout, d, target, &sp)) return rc;
+  std::unique_ptr<qcnn_pq_stats> s(sp);
+  if (int rc = FcStatsAdd(s.get(), who, x, t, N, st)) return rc;
+  return SweepFc(s.get(), who, target, K, sweeps, w_h, at, ctrd_h, asmt_h, loss_h, st);
+}
+
 }  // namespace
+
+namespace qcnn {
+
+// An FC add: the scan (its message names the first input column holding a NaN or Inf), then one fold
+int FcStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st) {
+  const int Din = s->Din, Dout = s->Dout;
+  unsigned first[2];
+  if (int rc = ScanAdd(s, y, static_cast<size_t>(N) * Din, Din, t, static_cast<size_t>(N) * Dout, first, st)) return rc;
+  QCNN_CHECK(first[0] == kNoneFound, "%s: %s contains a non-finite value (input column %u)", who, s->target ? "y" : "x", first[0]);
+  QCNN_CHECK(first[1] == kNoneFound, "%s: t contains a non-finite value", who);
+  QCNN_ON_DEVICE(s->ctx->device);
+  const int acc = s->images > 0, tiles = CeilDiv(Din, kTile);
+  pqr_gemm_kernel<kGemmGram><<<tiles * (tiles + 1) / 2, kGemmThreads, 0, st>>>(y, Din, nullptr, 0, s->G.as<double>(), Din, Din, Din, N,
+                                                                              acc);
+  QCNN_CUDA(cudaGetLastError());
+  if (s->target) {   // |T|^2 and P = T^T Y
+    if (int rc = LaunchSqNorm(t, static_cast<size_t>(N) * Dout, s->scratch.as<double>(), s->tt.as<double>(), acc, st)) return rc;
+    pqr_gemm_kernel<kGemmCross><<<dim3(tiles, CeilDiv(Dout, kTile)), kGemmThreads, 0, st>>>(t, Dout, y, Din, s->P.as<double>(), Din,
+                                                                                         Dout, Din, N, acc);
+    QCNN_CUDA(cudaGetLastError());
+  }
+  QCNN_CUDA(cudaEventRecord(s->done, st));
+  s->images += N;
+  return 0;
+}
+
+int FcStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wei_h, float* ctrd_h,
+                  uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+  if (int rc = CheckFcK(who, K)) return rc;
+  std::vector<uint8_t> at;
+  if (int rc = CheckFcHost(who, target, s->Din, s->Dout, K, s->d, wei_h, ctrd_h, asmt_h, at)) return rc;
+  return SweepFc(s, who, target, K, sweeps, wei_h, at, ctrd_h, asmt_h, loss_h, st);
+}
+
+}  // namespace qcnn
 
 extern "C" int qcnn_pq_refine_fc(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const float* wei_h, const float* x,
                                  int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h, void* stream) {
@@ -392,4 +449,71 @@ extern "C" int qcnn_pq_refine_fc(qcnn_ctx* ctx, int Din, int Dout, int K, int d,
 extern "C" int qcnn_pq_refine_fc_target(qcnn_ctx* ctx, int Din, int Dout, int K, int d, int sweeps, const float* y, const float* t,
                                         int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h, void* stream) {
   return Refine(ctx, true, Din, Dout, K, d, sweeps, nullptr, y, t, N, ctrd_h, asmt_h, loss_h, static_cast<cudaStream_t>(stream));
+}
+
+// ---- the statistics objects (both kinds; the conv creation and the conv halves are in pq_refine_conv.cu)
+
+extern "C" int qcnn_pq_stats_create_fc(qcnn_ctx* ctx, int Din, int Dout, int d, int target, qcnn_pq_stats** out) {
+  return CreateFc(ctx, "qcnn_pq_stats_create_fc", Din, Dout, d, target != 0, out);
+}
+
+extern "C" int qcnn_pq_stats_add(qcnn_pq_stats* s, const float* y, const float* t, int N, void* stream) {
+  const char* who = "qcnn_pq_stats_add";
+  QCNN_CHECK(s, "%s: NULL argument", who);
+  QCNN_CHECK(N >= 1, "%s: N=%d: at least one input is needed", who, N);
+  QCNN_CHECK(y, "%s: NULL argument", who);
+  QCNN_CHECK(s->target || !t, "%s: t given to statistics created without a target", who);
+  QCNN_CHECK(!s->target || t, "%s: NULL t (the statistics were created with a target)", who);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return s->conv ? ConvStatsAdd(s, who, y, t, N, st) : FcStatsAdd(s, who, y, t, N, st);
+}
+
+extern "C" int qcnn_pq_stats_count(const qcnn_pq_stats* s, long long* images) {
+  QCNN_CHECK(s && images, "qcnn_pq_stats_count: NULL argument");
+  *images = s->images;
+  return 0;
+}
+
+extern "C" int qcnn_pq_stats_read_h(const qcnn_pq_stats* s, double* G_h, double* P_h, double* tt_h) {
+  const char* who = "qcnn_pq_stats_read_h";
+  QCNN_CHECK(s, "%s: NULL argument", who);
+  QCNN_CHECK(s->target || (!P_h && !tt_h), "%s: P and |T|^2 are kept only by statistics created with a target", who);
+  QCNN_ON_DEVICE(s->ctx->device);
+  QCNN_CUDA(cudaEventSynchronize(s->done));
+  if (G_h) QCNN_CUDA(cudaMemcpy(G_h, s->G.get(), s->G.bytes(), cudaMemcpyDeviceToHost));
+  if (P_h) QCNN_CUDA(cudaMemcpy(P_h, s->P.get(), s->P.bytes(), cudaMemcpyDeviceToHost));
+  if (tt_h) QCNN_CUDA(cudaMemcpy(tt_h, s->tt.get(), sizeof(double), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+namespace {
+
+int RefineStats(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wei_h, float* ctrd_h,
+                uint8_t* asmt_h, double* loss_h, void* stream) {
+  QCNN_CHECK(s && (target || wei_h) && ctrd_h && asmt_h, "%s: NULL argument", who);
+  QCNN_CHECK(!target || s->target, "%s: the statistics were created without a target", who);
+  QCNN_CHECK(s->images > 0, "%s: no calibration data has been added", who);
+  QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return s->conv ? ConvStatsRefine(s, who, target, K, sweeps, wei_h, ctrd_h, asmt_h, loss_h, st)
+                 : FcStatsRefine(s, who, target, K, sweeps, wei_h, ctrd_h, asmt_h, loss_h, st);
+}
+
+}  // namespace
+
+extern "C" int qcnn_pq_stats_refine(qcnn_pq_stats* s, int K, int sweeps, const float* wei_h, float* ctrd_h, uint8_t* asmt_h,
+                                    double* loss_h, void* stream) {
+  return RefineStats(s, "qcnn_pq_stats_refine", false, K, sweeps, wei_h, ctrd_h, asmt_h, loss_h, stream);
+}
+
+extern "C" int qcnn_pq_stats_refine_target(qcnn_pq_stats* s, int K, int sweeps, float* ctrd_h, uint8_t* asmt_h, double* loss_h,
+                                           void* stream) {
+  return RefineStats(s, "qcnn_pq_stats_refine_target", true, K, sweeps, nullptr, ctrd_h, asmt_h, loss_h, stream);
+}
+
+extern "C" void qcnn_pq_stats_destroy(qcnn_pq_stats* s) {
+  if (!s) return;
+  DeviceGuard guard(s->ctx->device);
+  if (s->done) cudaEventSynchronize(s->done);   // queued adds still use the buffers
+  delete s;
 }

@@ -6,6 +6,8 @@
 
 #include <math.h>
 
+#include <algorithm>
+
 #include "qcnn_internal.h"
 
 namespace {
@@ -30,6 +32,30 @@ __device__ __forceinline__ void Dmma(double (&c)[4], const double (&a)[8], const
 constexpr int kGemmF64 = 0;     // C [M][N] = (accumulate ? C : 0) + A [M][Kd] B [Kd][N], all fp64
 constexpr int kGemmGram = 1;    // C = (accumulate ? C : 0) + X^T X for X = A [Kd][lda] fp32 (M = N = the column count)
 constexpr int kGemmCross = 2;   // C [M][N] = (accumulate ? C : 0) + A^T B for A [Kd][lda], B [Kd][ldb] fp32
+constexpr int kGemmGramMap = 3;   // kGemmGram with X = the patches of an NHWC map (MapOperand), M = N = Dg
+constexpr int kGemmCrossMap = 4;  // kGemmCross with B = the patches of an NHWC map (MapOperand), N = Dg
+
+// (m, t, j) of a conv layer's internal dim q = m d T + t w_m + j: subspace m, tap t, channel m d + j of the group
+struct Dim { int m, t, j, w; };
+__device__ __forceinline__ Dim DecodeDim(int q, int Cg, int d, int T) {
+  Dim r;
+  r.m = q / (d * T);
+  const int rem = q - r.m * d * T;
+  r.w = min(d, Cg - r.m * d);
+  r.t = rem / r.w;
+  r.j = rem - r.t * r.w;
+  return r;
+}
+
+// The patch operand of the map modes: row k is output position pos0 + k = (n Ho + oy) Wo + ox of the NHWC map
+// x [N][Hin][Win][Cin], column q the internal dim (m, t, j) of group g, and the element is
+// x[n][oy stride - pad + t / ksz][ox stride - pad + t % ksz][g Cg + m d + j], zero outside the map.
+struct MapOperand {
+  const float* x;
+  long long pos0;
+  int Hin, Win, Cin, ksz, pad, stride, Ho, Wo, Cg, d, g;
+};
+constexpr int kMapFar = -(1 << 28);   // a row offset that puts an element outside any map: dims past Dg, rows past Kd
 
 // fp64 tensor-core GEMM, one kTile x kTile output tile per CTA, k in ascending steps of 16 (a fixed order per element).
 //   kGemmGram:  lower-triangle tiles only (blockIdx.x is the linear lower-triangle index); each element with row >= col
@@ -37,15 +63,24 @@ constexpr int kGemmCross = 2;   // C [M][N] = (accumulate ? C : 0) + A^T B for A
 //   otherwise:  the full tile grid, blockIdx.y over M and blockIdx.x over N.
 // Operands are staged through registers (the next k-step is loaded while the current one is multiplied), widened to
 // fp64 and stored k-major, [16][kLd], in shared memory.
+// Map modes: the patch operand's address is the sum of a row part (per k-step, its 16 positions decoded by warp 0 into
+// a double-buffered table while the previous k-step is multiplied) and a column part (per thread, its dim decoded once
+// into registers), so every element is the value the im2col patch would hold, and the products and their order are those of
+// kGemmGram / kGemmCross on the patches.
 template <int kMode>
 __global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __restrict__ Ap, int lda, const void* __restrict__ Bp,
                                                                 int ldb, double* __restrict__ C, int ldc, int M, int N, int Kd,
-                                                                int accumulate) {
+                                                                int accumulate, MapOperand map = MapOperand{}) {
+  constexpr bool kMap = kMode == kGemmGramMap || kMode == kGemmCrossMap;
+  constexpr bool kGram = kMode == kGemmGram || kMode == kGemmGramMap;
   __shared__ double As[2][kKStep][kLd], Bs[2][kKStep][kLd];
+  // map modes: per row (k-step buffer, position) the element offset of tap (0, 0) and its map row and column
+  __shared__ long long sRowOff[kMap ? 2 : 1][kKStep];
+  __shared__ int sRowY[kMap ? 2 : 1][kKStep], sRowX[kMap ? 2 : 1][kKStep];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3, wm = warp >> 1, wn = warp & 1;
   int tm, tn;
-  if (kMode == kGemmGram) {
+  if (kGram) {
     const int i = blockIdx.x;
     tm = static_cast<int>((sqrt(8.0 * i + 1.0) - 1.0) * 0.5);
     while (tm * (tm + 1) / 2 > i) tm--;
@@ -58,13 +93,84 @@ __global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __re
   const int m0 = tm * kTile, n0 = tn * kTile;
   constexpr int kPer = kKStep * kTile / kGemmThreads;   // 8 elements of each operand per thread and k-step
   double ra[kPer], rb[kPer];
+  // map modes: the k-step's raw fp32 elements, widened when they are stored, so that nothing waits for the loads until
+  // the k-step's DMMAs are issued
+  float fa_[kMap ? kPer : 1], fb_[kMap ? kPer : 1];
+  // map modes: a thread loads one column of each operand (nn = tid % kTile), so its dims are decoded once into
+  // registers: the offset of the tap and channel, and the tap's row and column (side 0: the tile's rows m0.., side 1
+  // its columns n0..; the cross mode reads only side 1); a dim past M / N is far outside the map
+  int cOff[2] = {0, 0}, cY[2] = {kMapFar, kMapFar}, cX[2] = {0, 0};
+  if (kMap) {
+#pragma unroll
+    for (int side = 0; side < 2; side++) {
+      const int q = (side ? n0 : m0) + tid % kTile;
+      if (q < (side ? N : M)) {
+        const int T = map.ksz * map.ksz;
+        const Dim dm = DecodeDim(q, map.Cg, map.d, T);
+        cY[side] = dm.t / map.ksz;
+        cX[side] = dm.t % map.ksz;
+        cOff[side] = (cY[side] * map.Win + cX[side]) * map.Cin + map.g * map.Cg + dm.m * map.d + dm.j;
+      }
+    }
+  }
+  // map modes: lanes 0..15 of warp 0 decode the rows of consecutive k-steps into buffer kt & 1, each lane stepping its
+  // position (n, oy, ox) by 16; a row past Kd is far outside the map
+  long long rn = 0;
+  int ry = 0, rx = 0;
+  if (kMap && tid < kKStep) {
+    const long long pos = map.pos0 + tid, hw = static_cast<long long>(map.Ho) * map.Wo;
+    rn = pos / hw;
+    const int yx = static_cast<int>(pos - rn * hw);
+    ry = yx / map.Wo;
+    rx = yx - ry * map.Wo;
+  }
+  auto decodeRows = [&](int kt) {
+    if (!kMap || tid >= kKStep) return;
+    long long off = 0;
+    int iy = kMapFar, ix = 0;
+    if (kt * kKStep + tid < Kd) {
+      iy = ry * map.stride - map.pad;
+      ix = rx * map.stride - map.pad;
+      off = ((rn * map.Hin + iy) * map.Win + ix) * map.Cin;
+    }
+    sRowOff[kt & 1][tid] = off;
+    sRowY[kt & 1][tid] = iy;
+    sRowX[kt & 1][tid] = ix;
+    rx += kKStep;
+    while (rx >= map.Wo) {
+      rx -= map.Wo;
+      if (++ry == map.Ho) {
+        ry = 0;
+        rn++;
+      }
+    }
+  };
+  auto mapAt = [&](int buf, int kk, int side) -> float {
+    const int iy = sRowY[buf][kk] + cY[side], ix = sRowX[buf][kk] + cX[side];
+    const bool in = static_cast<unsigned>(iy) < static_cast<unsigned>(map.Hin) &&
+                    static_cast<unsigned>(ix) < static_cast<unsigned>(map.Win);
+    return in ? __ldg(map.x + sRowOff[buf][kk] + cOff[side]) : 0.0f;
+  };
+  if (kMap) {
+    decodeRows(0);
+    decodeRows(1);
+    __syncthreads();
+  }
   auto load = [&](int k0) {
+    const int rbuf = (k0 / kKStep) & 1;
 #pragma unroll
     for (int r = 0; r < kPer; r++) {
       const int e = tid + r * kGemmThreads;
       const int kk = e / kTile, nn = e % kTile;   // B (and the Gram's A): row kk of the k-step, column nn
       const int k = k0 + kk;
-      if (kMode == kGemmGram) {
+      if (kMode == kGemmGramMap) {
+        fa_[r] = mapAt(rbuf, kk, 0);
+        fb_[r] = mapAt(rbuf, kk, 1);
+      } else if (kMode == kGemmCrossMap) {
+        const float* A = static_cast<const float*>(Ap);
+        fa_[r] = (k < Kd && m0 + nn < M) ? __ldg(A + static_cast<size_t>(k) * lda + m0 + nn) : 0.0f;
+        fb_[r] = mapAt(rbuf, kk, 1);
+      } else if (kMode == kGemmGram) {
         const float* X = static_cast<const float*>(Ap);
         ra[r] = (k < Kd && m0 + nn < M) ? static_cast<double>(X[static_cast<size_t>(k) * lda + m0 + nn]) : 0.0;
         rb[r] = (k < Kd && n0 + nn < N) ? static_cast<double>(X[static_cast<size_t>(k) * lda + n0 + nn]) : 0.0;
@@ -86,6 +192,11 @@ __global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __re
 #pragma unroll
     for (int r = 0; r < kPer; r++) {
       const int e = tid + r * kGemmThreads;
+      if (kMap) {
+        As[buf][e / kTile][e % kTile] = static_cast<double>(fa_[r]);
+        Bs[buf][e / kTile][e % kTile] = static_cast<double>(fb_[r]);
+        continue;
+      }
       if (kMode != kGemmF64) As[buf][e / kTile][e % kTile] = ra[r];
       else As[buf][e % kKStep][e / kKStep] = ra[r];
       Bs[buf][e / kTile][e % kTile] = rb[r];
@@ -105,6 +216,8 @@ __global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __re
   for (int kt = 0; kt < nk; kt++) {
     const int buf = kt & 1;
     if (kt + 1 < nk) load((kt + 1) * kKStep);
+    // buffer kt & 1 of the row table was last read by the loads of k-step kt, before the previous barrier
+    if (kMap && kt + 2 < nk) decodeRows(kt + 2);
     double fa[2][8], fb[4][4];
 #pragma unroll
     for (int mt = 0; mt < 2; mt++)
@@ -129,7 +242,7 @@ __global__ void __launch_bounds__(kGemmThreads) pqr_gemm_kernel(const void* __re
       for (int i = 0; i < 4; i++) {
         const int row = m0 + wm * 32 + mt * 16 + g + 8 * (i >> 1), col = n0 + wn * 32 + nt * 8 + 2 * t + (i & 1);
         if (row >= M || col >= N) continue;
-        if (kMode == kGemmGram) {
+        if (kGram) {
           if (row < col) continue;
           double* p = C + static_cast<size_t>(row) * ldc + col;
           const double v = accumulate ? *p + acc[mt][nt][i] : acc[mt][nt][i];
@@ -206,11 +319,74 @@ inline int LaunchLoss(const double* E, const double* GE, size_t n, double* part,
   return 0;
 }
 
-// *out = |t|^2 over n fp32 values in a fixed order: non-finite exactly when t holds a NaN or Inf
-inline int LaunchSqNorm(const float* t, size_t n, double* part, double* out, cudaStream_t st) {
+// *tt = the partials' sum (accumulate: *tt plus it), in pqr_loss_final_kernel's order
+__global__ void __launch_bounds__(kSweepThreads) pqr_sqnorm_final_kernel(const double* __restrict__ part, double* __restrict__ tt,
+                                                                         int accumulate) {
+  __shared__ double red[kSweepThreads / 32];
+  double v = 0.0;
+  for (int i = threadIdx.x; i < kLossBlocks; i += kSweepThreads) v += part[i];
+  const double tot = BlockSum(v, red);
+  if (threadIdx.x == 0) *tt = accumulate ? *tt + tot : tot;
+}
+
+// *tt (accumulate: *tt +) |t|^2 over n fp32 values in a fixed order; part holds kLossBlocks doubles
+inline int LaunchSqNorm(const float* t, size_t n, double* part, double* tt, int accumulate, cudaStream_t st) {
   pqr_sqnorm_partial_kernel<<<kLossBlocks, kSweepThreads, 0, st>>>(t, n, part);
-  pqr_loss_final_kernel<false><<<1, kSweepThreads, 0, st>>>(part, nullptr, out);
+  pqr_sqnorm_final_kernel<<<1, kSweepThreads, 0, st>>>(part, tt, accumulate);
   QCNN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// *first = min(*first, the column i % cols of every non-finite x[i]); *first starts at 0xffffffff (none)
+__global__ void pqr_nonfinite_kernel(const float* __restrict__ x, size_t n, unsigned cols, unsigned* __restrict__ first) {
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    if (!isfinite(x[i])) atomicMin(first, static_cast<unsigned>(i % cols));
+}
+
+constexpr unsigned kNoneFound = 0xffffffffu;
+
+// An add's scan, ordered after the earlier adds of s: first[0] = the lowest column (index mod ycols) of a NaN or Inf in
+// y, first[1] = 0 if t (when given) holds one, kNoneFound otherwise.  One synchronisation of st.
+inline int ScanAdd(qcnn_pq_stats* s, const float* y, size_t ny, unsigned ycols, const float* t, size_t nt, unsigned first[2],
+                   cudaStream_t st) {
+  QCNN_ON_DEVICE(s->ctx->device);
+  unsigned* flags = reinterpret_cast<unsigned*>(s->scratch.as<double>() + kLossBlocks);
+  QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
+  QCNN_CUDA(cudaMemsetAsync(flags, 0xff, 2 * sizeof(unsigned), st));
+  auto scan = [&](const float* v, size_t n, unsigned cols, unsigned* flag) {
+    const int grid = static_cast<int>(std::min<size_t>((n + 255) / 256, 32u * s->ctx->sm_count));
+    pqr_nonfinite_kernel<<<grid, 256, 0, st>>>(v, n, cols, flag);
+  };
+  scan(y, ny, ycols, flags);
+  if (t) scan(t, nt, 1, flags + 1);
+  QCNN_CUDA(cudaGetLastError());
+  QCNN_CUDA(cudaMemcpyAsync(first, flags, 2 * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+  QCNN_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// The parts of a stats object both kinds share: the sums (zero until the first add), the scratch and the event
+inline int AllocStats(qcnn_pq_stats* s, const char* who, size_t gBytes, size_t pBytes) {
+  qcnn_ctx* ctx = s->ctx;
+  auto reserve = [&](qcnn::DeviceBuffer& b, size_t bytes, const char* what) -> int {
+    const cudaError_t e = b.Reserve(ctx, bytes);
+    if (e == cudaSuccess) return 0;
+    cudaGetLastError();
+    qcnn::SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
+    return 1;
+  };
+  if (reserve(s->G, gBytes, "the Gram matrices") || reserve(s->P, s->target ? pBytes : 0, "the targets' cross product") ||
+      reserve(s->tt, s->target ? sizeof(double) : 0, "the targets' norm") ||
+      reserve(s->scratch, sizeof(double) * kLossBlocks + 2 * sizeof(unsigned), "the scan flags"))
+    return 1;
+  QCNN_ON_DEVICE(ctx->device);
+  QCNN_CUDA(cudaEventCreateWithFlags(&s->done, cudaEventDisableTiming));
+  QCNN_CUDA(cudaMemset(s->G.get(), 0, gBytes));
+  if (s->target) {
+    QCNN_CUDA(cudaMemset(s->P.get(), 0, pBytes));
+    QCNN_CUDA(cudaMemset(s->tt.get(), 0, sizeof(double)));
+  }
+  QCNN_CUDA(cudaEventRecord(s->done, nullptr));
   return 0;
 }
 

@@ -25,6 +25,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <memory>
 #include <vector>
 
 #include "pq_refine_common.cuh"
@@ -40,43 +41,7 @@ constexpr int kCholBlock = 64;                   // panel width of the blocked C
 constexpr int kSolveThreads = 1024;
 constexpr int kNormalThreads = 128;
 constexpr int kAssignWarps = 8;
-constexpr size_t kPatchBytes = size_t(256) << 20;   // one chunk of one group's patches
-
-// (m, t, j) of internal dim q: subspace m, tap t, channel m d + j
-struct Dim { int m, t, j, w; };
-__device__ __forceinline__ Dim DecodeDim(int q, int Cg, int d, int T) {
-  Dim r;
-  r.m = q / (d * T);
-  const int rem = q - r.m * d * T;
-  r.w = min(d, Cg - r.m * d);
-  r.t = rem / r.w;
-  r.j = rem - r.t * r.w;
-  return r;
-}
-
-__global__ void pqrc_nonfinite_kernel(const float* __restrict__ x, size_t n, int* __restrict__ flag) {
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x)
-    if (!isfinite(x[i])) *flag = 1;
-}
-
-// Patches [np][Dg] fp32 of group g for output positions [p0, p0 + np) (position = (n Ho + y) Wo + x), zero-padded.
-__global__ void pqrc_patch_kernel(const float* __restrict__ x, float* __restrict__ P, size_t p0, int np, int g, int Hin, int Win,
-                                  int Cin, int Cg, int ksz, int pad, int stride, int Ho, int Wo, int d) {
-  const int T = ksz * ksz, Dg = Cg * T;
-  const size_t total = static_cast<size_t>(np) * Dg;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const size_t pos = p0 + i / Dg;
-    const Dim q = DecodeDim(static_cast<int>(i % Dg), Cg, d, T);
-    const size_t img = pos / (static_cast<size_t>(Ho) * Wo);
-    const int yx = static_cast<int>(pos % (static_cast<size_t>(Ho) * Wo));
-    const int iy = (yx / Wo) * stride - pad + q.t / ksz, ix = (yx % Wo) * stride - pad + q.t % ksz;
-    float v = 0.0f;
-    if (iy >= 0 && iy < Hin && ix >= 0 && ix < Win)
-      v = x[((img * Hin + iy) * Win + ix) * Cin + static_cast<size_t>(g) * Cg + q.m * d + q.j];
-    P[i] = v;
-  }
-}
+constexpr size_t kRunBytes = size_t(256) << 20;     // an add folds its positions in runs of 2^28 / (4 Dg)
 
 // E[o][q] = W[o][q] - C[m][A[m][o][t]][j] in fp64 (A held [S][Cout][T])
 __global__ void pqrc_residual_kernel(const float* __restrict__ W, const float* __restrict__ C, const uint8_t* __restrict__ A,
@@ -432,22 +397,16 @@ __global__ void __launch_bounds__(kAssignWarps * 32) pqrc_assign_kernel(const do
   }
 }
 
-struct Geometry {
-  int Cin, Hin, Win, Cout, ksz, pad, stride, grp, Ho, Wo, Cg, Cpg, T, Dg;
-};
-
-// t == nullptr: the same-input form on the weights knl_h; else the target form (knl_h is not read).
-int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const float* knl_h, const float* x, const float* t, int N,
-           float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
-  const bool target = t != nullptr;
-  const char* who = target ? "qcnn_pq_refine_conv_target" : "qcnn_pq_refine_conv";
-  const int Cout = geo.Cout, Cg = geo.Cg, Cpg = geo.Cpg, T = geo.T, Dg = geo.Dg, grp = geo.grp;
-  const int S = CeilDiv(Cg, d), wmax = std::min(d, Cg);
+// The host-side checks of a refine (weights unless target, codebook, assignments), the assignments as [S][Cout][T] and
+// the weights [Cout][Cg][T] in the internal dim order [Cout][Dg]
+int CheckConvHost(const char* who, bool target, const PqConvGeometry& geo, int K, int d, const float* knl_h, const float* ctrd_h,
+                  const uint8_t* asmt_h, std::vector<uint8_t>& at, std::vector<float>& wp) {
+  const int Cout = geo.Cout, Cg = geo.Cg, T = geo.T, Dg = geo.Dg;
+  const int S = CeilDiv(Cg, d);
   const size_t nw = static_cast<size_t>(Cout) * Dg, nc = static_cast<size_t>(S) * K * d;
   if (!target) QCNN_CHECK(AllFinite(knl_h, nw), "%s: the weights contain a non-finite value", who);
   QCNN_CHECK(AllFinite(ctrd_h, nc), "%s: the codebook contains a non-finite value", who);
-  // assignments [Cout][T][S] -> [S][Cout][T]; weights [Cout][Cg][T] -> [Cout][Dg] in the internal dim order
-  std::vector<uint8_t> at(static_cast<size_t>(S) * Cout * T);
+  at.assign(static_cast<size_t>(S) * Cout * T, 0);
   for (int o = 0; o < Cout; o++)
     for (int t = 0; t < T; t++)
       for (int m = 0; m < S; m++) {
@@ -455,18 +414,36 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
         QCNN_CHECK(a < K, "%s: assignment %d of output %d, tap %d, subspace %d is not below K=%d", who, a, o, t, m, K);
         at[(static_cast<size_t>(m) * Cout + o) * T + t] = a;
       }
-  std::vector<float> wp(target ? 0 : nw);
+  wp.assign(target ? 0 : nw, 0.0f);
   for (int o = 0; o < (target ? 0 : Cout); o++)
     for (int c = 0; c < Cg; c++) {
       const int m = c / d, j = c % d, w = std::min(d, Cg - m * d);
       for (int t = 0; t < T; t++)
         wp[static_cast<size_t>(o) * Dg + m * d * T + t * w + j] = knl_h[(static_cast<size_t>(o) * Cg + c) * T + t];
     }
+  return 0;
+}
+
+// K and the joint-system limit
+int CheckConvSystem(const char* who, int K, int d, int Cg) {
+  if (int rc = CheckConvK(who, K)) return rc;
+  const long long sys = static_cast<long long>(K) * std::min(d, Cg);
+  QCNN_CHECK(sys <= kMaxSystem, "%s: K*min(d, Cin/grp) = %d*%d = %lld exceeds %d, the size of the joint codebook system", who, K,
+             std::min(d, Cg), sys, kMaxSystem);
+  return 0;
+}
+
+// The sweeps on the statistics of s.  target: the target form (wp is empty); else the same-input form on the weights wp.
+int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const std::vector<float>& wp,
+              std::vector<uint8_t>& at, float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+  qcnn_ctx* ctx = s->ctx;
+  const PqConvGeometry& geo = s->geo;
+  const int d = s->d, Cout = geo.Cout, Cg = geo.Cg, Cpg = geo.Cpg, T = geo.T, Dg = geo.Dg, grp = geo.grp;
+  const int S = CeilDiv(Cg, d), wmax = std::min(d, Cg);
+  const size_t nw = static_cast<size_t>(Cout) * Dg, nc = static_cast<size_t>(S) * K * d;
   QCNN_ON_DEVICE(ctx->device);
-  const size_t positions = static_cast<size_t>(N) * geo.Ho * geo.Wo;
-  const int chunk = static_cast<int>(std::max<size_t>(1, std::min<size_t>(positions, kPatchBytes / (sizeof(float) * Dg))));
   const size_t nbMax = static_cast<size_t>(T) * wmax, nMax = static_cast<size_t>(K) * wmax;
-  DeviceBuffer dG, dE, dGE, dW, dC, dA, dP, dWh, dH, dDlt, dM, dF, dPt, dB, dMem, dOff, dUk, dNU, dCC, dFlag, dPart, dLoss, dTY, dTT;
+  DeviceBuffer dE, dGE, dW, dC, dA, dWh, dH, dDlt, dM, dF, dPt, dB, dMem, dOff, dUk, dNU, dCC, dPart, dLoss;
   auto reserve = [&](DeviceBuffer& b, size_t bytes, const char* what) -> int {
     const cudaError_t e = b.Reserve(ctx, bytes);
     if (e == cudaSuccess) return 0;
@@ -474,10 +451,9 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
     SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
     return 1;
   };
-  if (reserve(dG, sizeof(double) * grp * static_cast<size_t>(Dg) * Dg, "the Gram matrices") ||
-      reserve(dE, sizeof(double) * nw, "the residual") || reserve(dGE, sizeof(double) * nw, "G times the residual") ||
+  if (reserve(dE, sizeof(double) * nw, "the residual") || reserve(dGE, sizeof(double) * nw, "G times the residual") ||
       reserve(dW, sizeof(float) * nw, "the weights") || reserve(dC, sizeof(float) * nc, "the codebook") ||
-      reserve(dA, at.size(), "the assignments") || reserve(dP, sizeof(float) * chunk * static_cast<size_t>(Dg), "the patches") ||
+      reserve(dA, at.size(), "the assignments") ||
       reserve(dWh, sizeof(double) * Cout * nbMax, "the decoded subspace") ||
       reserve(dH, sizeof(double) * Cout * nbMax, "the subspace responses") ||
       reserve(dDlt, sizeof(double) * Cout * nbMax, "the subspace's changes") ||
@@ -488,51 +464,19 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
       reserve(dOff, sizeof(int) * grp * static_cast<size_t>(T) * (K + 1), "the cluster members") ||
       reserve(dUk, sizeof(int) * K, "the used clusters") || reserve(dNU, sizeof(int), "the used clusters") ||
       reserve(dCC, sizeof(double) * grp * static_cast<size_t>(T) * K, "the codeword norms") ||
-      reserve(dFlag, sizeof(int), "a flag") || reserve(dPart, sizeof(double) * kLossBlocks, "the loss") ||
-      reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss") ||
-      reserve(dTY, target ? sizeof(double) * nw : 0, "the targets' cross product") ||
-      reserve(dTT, target ? sizeof(double) : 0, "the targets' norm"))
+      reserve(dPart, sizeof(double) * kLossBlocks, "the loss") || reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss"))
     return 1;
+  const double* G = s->G.as<double>();
+  QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
   if (target) QCNN_CUDA(cudaMemsetAsync(dW.get(), 0, sizeof(float) * nw, st));   // E = 0 - W^
   else QCNN_CUDA(cudaMemcpyAsync(dW.get(), wp.data(), sizeof(float) * nw, cudaMemcpyHostToDevice, st));
   QCNN_CUDA(cudaMemcpyAsync(dC.get(), ctrd_h, sizeof(float) * nc, cudaMemcpyHostToDevice, st));
   QCNN_CUDA(cudaMemcpyAsync(dA.get(), at.data(), at.size(), cudaMemcpyHostToDevice, st));
-  QCNN_CUDA(cudaMemsetAsync(dFlag.get(), 0, sizeof(int), st));
-  const size_t nx = static_cast<size_t>(N) * geo.Hin * geo.Win * geo.Cin;
-  const int gridX = static_cast<int>(std::min<size_t>((nx + 255) / 256, 32u * ctx->sm_count));
-  pqrc_nonfinite_kernel<<<gridX, 256, 0, st>>>(x, nx, dFlag.as<int>());
-  double tt = 0.0;   // |T|^2: non-finite exactly when t is
-  if (target && LaunchSqNorm(t, positions * Cout, dPart.as<double>(), dTT.as<double>(), st)) return 1;
-  // G_g (and P_g) = sum over chunks of positions, ascending
-  const int tiles = CeilDiv(Dg, kTile);
-  for (int g = 0; g < grp; g++) {
-    double* Gg = dG.as<double>() + static_cast<size_t>(g) * Dg * Dg;
-    for (size_t p0 = 0; p0 < positions; p0 += chunk) {
-      const int np = static_cast<int>(std::min<size_t>(chunk, positions - p0));
-      const size_t ne = static_cast<size_t>(np) * Dg;
-      const int gridP = static_cast<int>(std::min<size_t>((ne + 255) / 256, 32u * ctx->sm_count));
-      pqrc_patch_kernel<<<gridP, 256, 0, st>>>(x, dP.as<float>(), p0, np, g, geo.Hin, geo.Win, geo.Cin, Cg, geo.ksz, geo.pad,
-                                               geo.stride, geo.Ho, geo.Wo, d);
-      pqr_gemm_kernel<kGemmGram><<<tiles * (tiles + 1) / 2, kGemmThreads, 0, st>>>(dP.get(), Dg, nullptr, 0, Gg, Dg, Dg, Dg, np,
-                                                                                  p0 > 0);
-      if (target)   // the chunk's target rows of group g's outputs against its patches
-        pqr_gemm_kernel<kGemmCross><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
-            t + p0 * Cout + static_cast<size_t>(g) * Cpg, Cout, dP.get(), Dg, dTY.as<double>() + static_cast<size_t>(g) * Cpg * Dg, Dg,
-            Cpg, Dg, np, p0 > 0);
-      QCNN_CUDA(cudaGetLastError());
-    }
-  }
-  int flag = 0;
   std::vector<double> diag(static_cast<size_t>(grp) * Dg);
   for (int g = 0; g < grp; g++)
-    QCNN_CUDA(cudaMemcpy2DAsync(diag.data() + static_cast<size_t>(g) * Dg, sizeof(double),
-                                dG.as<double>() + static_cast<size_t>(g) * Dg * Dg, sizeof(double) * (static_cast<size_t>(Dg) + 1),
-                                sizeof(double), Dg, cudaMemcpyDeviceToHost, st));
-  QCNN_CUDA(cudaMemcpyAsync(&flag, dFlag.get(), sizeof(int), cudaMemcpyDeviceToHost, st));
-  if (target) QCNN_CUDA(cudaMemcpyAsync(&tt, dTT.get(), sizeof(double), cudaMemcpyDeviceToHost, st));
+    QCNN_CUDA(cudaMemcpy2DAsync(diag.data() + static_cast<size_t>(g) * Dg, sizeof(double), G + static_cast<size_t>(g) * Dg * Dg,
+                                sizeof(double) * (static_cast<size_t>(Dg) + 1), sizeof(double), Dg, cudaMemcpyDeviceToHost, st));
   QCNN_CUDA(cudaStreamSynchronize(st));
-  QCNN_CHECK(!flag, "%s: %s contains a non-finite value", who, target ? "y" : "x");
-  QCNN_CHECK(isfinite(tt), "%s: t contains a non-finite value", who);
   std::vector<bool> skip(S);
   for (int m = 0; m < S; m++) {
     const int w = std::min(d, Cg - m * d);
@@ -541,20 +485,20 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
       for (int r = 0; r < T * w; r++) tr += diag[static_cast<size_t>(g) * Dg + m * d * T + r];
     skip[m] = tr == 0.0;
   }
+  const int tiles = CeilDiv(Dg, kTile);
   const int ewBlocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 32u * ctx->sm_count));
   pqrc_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Cout, Cg, K, d, T);
   // GE = E G, or P + E G for a target
-  if (target) QCNN_CUDA(cudaMemcpyAsync(dGE.get(), dTY.get(), sizeof(double) * nw, cudaMemcpyDeviceToDevice, st));
+  const double* P = target ? s->P.as<double>() : nullptr;   // T^T Y
+  const double* TT = target ? s->tt.as<double>() : nullptr;
+  if (target) QCNN_CUDA(cudaMemcpyAsync(dGE.get(), P, sizeof(double) * nw, cudaMemcpyDeviceToDevice, st));
   for (int g = 0; g < grp; g++) {
     const size_t ro = static_cast<size_t>(g) * Cpg * Dg;
     pqr_gemm_kernel<kGemmF64><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
-        dE.as<double>() + ro, Dg, dG.as<double>() + static_cast<size_t>(g) * Dg * Dg, Dg, dGE.as<double>() + ro, Dg, Cpg, Dg, Dg,
-        target);
+        dE.as<double>() + ro, Dg, G + static_cast<size_t>(g) * Dg * Dg, Dg, dGE.as<double>() + ro, Dg, Cpg, Dg, Dg, target);
   }
   QCNN_CUDA(cudaGetLastError());
-  const double* P = target ? dTY.as<double>() : nullptr;   // T^T Y
-  if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>(), st, P, dTT.as<double>()))
-    return rc;
+  if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>(), st, P, TT)) return rc;
   const size_t assignSmem = sizeof(double) * kAssignWarps * (kMaxD + (T + 1) / 2);
   if (assignSmem > 48 * 1024)
     QCNN_CUDA(cudaFuncSetAttribute(pqrc_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(assignSmem)));
@@ -569,7 +513,7 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
                                                 Cout, Dg, K, d, w, T, q0);
       for (int g = 0; g < grp; g++) {
         const size_t ro = static_cast<size_t>(g) * Cpg * nb;
-        const double* Gm = dG.as<double>() + static_cast<size_t>(g) * Dg * Dg + static_cast<size_t>(q0) * Dg + q0;
+        const double* Gm = G + static_cast<size_t>(g) * Dg * Dg + static_cast<size_t>(q0) * Dg + q0;
         pqr_gemm_kernel<kGemmF64><<<dim3(CeilDiv(nb, kTile), CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
             dWh.as<double>() + ro, nb, Gm, Dg, dH.as<double>() + ro, nb, Cpg, nb, nb, 1);
       }
@@ -583,7 +527,7 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
       const int n = nU * w;
       // codebook: M, b, the blocked Cholesky of M + mu I, the solve and the acceptance test
       const size_t nrmSmem = sizeof(double) * w * w + sizeof(int) * T;
-      pqrc_normal_kernel<<<dim3(nU, nU), kNormalThreads, nrmSmem, st>>>(dG.as<double>(), dA.as<uint8_t>(), dMem.as<int>(), dOff.as<int>(),
+      pqrc_normal_kernel<<<dim3(nU, nU), kNormalThreads, nrmSmem, st>>>(G, dA.as<uint8_t>(), dMem.as<int>(), dOff.as<int>(),
                                                                         dUk.as<int>(), dM.as<double>(), m, grp, Cout, Cpg, Dg, K, T, w,
                                                                         q0, n);
       pqrc_rhs_kernel<<<CeilDiv(n, 128), 128, 0, st>>>(dH.as<double>(), dA.as<uint8_t>(), dUk.as<int>(), dB.as<double>(), m, Cout, T, w, n);
@@ -601,21 +545,19 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
       pqrc_solve_kernel<<<1, kSolveThreads, 0, st>>>(dF.as<double>(), dM.as<double>(), dB.as<double>(), dUk.as<int>(), dC.as<float>(), m,
                                                      K, d, w, n);
       // assignment, tap by tap per output; then GE += Dlt G[block, :]
-      pqrc_ccost_kernel<<<grp * T, 256, 0, st>>>(dG.as<double>(), dC.as<float>(), dCC.as<double>(), m, Dg, K, d, w, T, q0);
+      pqrc_ccost_kernel<<<grp * T, 256, 0, st>>>(G, dC.as<float>(), dCC.as<double>(), m, Dg, K, d, w, T, q0);
       pqrc_assign_kernel<<<CeilDiv(Cout, kAssignWarps), kAssignWarps * 32, assignSmem, st>>>(
-          dG.as<double>(), dC.as<float>(), dCC.as<double>(), dH.as<double>(), dW.as<float>(), dA.as<uint8_t>(), dE.as<double>(),
+          G, dC.as<float>(), dCC.as<double>(), dH.as<double>(), dW.as<float>(), dA.as<uint8_t>(), dE.as<double>(),
           dDlt.as<double>(), m, Cout, Cpg, Dg, K, d, w, T, q0);
       for (int g = 0; g < grp; g++) {
-        const double* Gb = dG.as<double>() + static_cast<size_t>(g) * Dg * Dg + static_cast<size_t>(q0) * Dg;
+        const double* Gb = G + static_cast<size_t>(g) * Dg * Dg + static_cast<size_t>(q0) * Dg;
         pqr_gemm_kernel<kGemmF64><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
             dDlt.as<double>() + static_cast<size_t>(g) * Cpg * nb, nb, Gb, Dg, dGE.as<double>() + static_cast<size_t>(g) * Cpg * Dg, Dg,
             Cpg, Dg, nb, 1);
       }
       QCNN_CUDA(cudaGetLastError());
     }
-    if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st, P,
-                            dTT.as<double>()))
-      return rc;
+    if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st, P, TT)) return rc;
   }
   std::vector<double> lossv(sweeps + 1);
   QCNN_CUDA(cudaMemcpyAsync(ctrd_h, dC.get(), sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
@@ -629,35 +571,111 @@ int Refine(qcnn_ctx* ctx, const Geometry& geo, int K, int d, int sweeps, const f
   return 0;
 }
 
-// The checks both forms share, then Refine
-int RefineConv(bool target, qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, int K,
-               int d, int sweeps, const float* knl_h, const float* x, const float* t, int N, float* ctrd_h, uint8_t* asmt_h,
-               double* loss_h, void* stream) {
-  const char* who = target ? "qcnn_pq_refine_conv_target" : "qcnn_pq_refine_conv";
-  QCNN_CHECK(ctx && (target || knl_h) && ctrd_h && asmt_h, "%s: NULL argument", who);
+// The geometry checks of every conv entry point, then the derived sizes
+int CheckGeometry(const char* who, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, PqConvGeometry* geo) {
   QCNN_CHECK(Cin >= 1 && Hin >= 1 && Win >= 1 && Cout >= 1 && ksz >= 1 && pad >= 0 && stride >= 1 && grp >= 1,
              "%s: bad geometry (Cin=%d Hin=%d Win=%d Cout=%d ksz=%d pad=%d stride=%d grp=%d)", who, Cin, Hin, Win, Cout, ksz, pad,
              stride, grp);
   QCNN_CHECK(Cin % grp == 0 && Cout % grp == 0, "%s: Cin=%d and Cout=%d must be divisible by grp=%d", who, Cin, Cout, grp);
   QCNN_CHECK(Hin + 2 * pad >= ksz && Win + 2 * pad >= ksz, "%s: empty output (%dx%d input, pad %d, kernel %d)", who, Hin, Win, pad, ksz);
+  geo->Cin = Cin; geo->Hin = Hin; geo->Win = Win; geo->Cout = Cout; geo->ksz = ksz; geo->pad = pad; geo->stride = stride; geo->grp = grp;
+  geo->Ho = (Hin + 2 * pad - ksz) / stride + 1;
+  geo->Wo = (Win + 2 * pad - ksz) / stride + 1;
+  geo->Cg = Cin / grp; geo->Cpg = Cout / grp; geo->T = ksz * ksz; geo->Dg = geo->Cg * geo->T;
+  return 0;
+}
+
+int CreateConv(qcnn_ctx* ctx, const char* who, const PqConvGeometry& geo, int d, bool target, qcnn_pq_stats** out) {
+  std::unique_ptr<qcnn_pq_stats> s(new qcnn_pq_stats);
+  s->ctx = ctx;
+  s->conv = true;
+  s->target = target;
+  s->d = d;
+  s->geo = geo;
+  if (AllocStats(s.get(), who, sizeof(double) * geo.grp * static_cast<size_t>(geo.Dg) * geo.Dg,
+                 sizeof(double) * geo.Cout * static_cast<size_t>(geo.Dg)))
+    return 1;
+  *out = s.release();
+  return 0;
+}
+
+// The one-shot calls: the checks both forms share (in the order of their messages), then create, one add of all N
+// inputs, the sweeps and destroy
+int RefineConv(bool target, qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, int K,
+               int d, int sweeps, const float* knl_h, const float* x, const float* t, int N, float* ctrd_h, uint8_t* asmt_h,
+               double* loss_h, void* stream) {
+  const char* who = target ? "qcnn_pq_refine_conv_target" : "qcnn_pq_refine_conv";
+  QCNN_CHECK(ctx && (target || knl_h) && ctrd_h && asmt_h, "%s: NULL argument", who);
+  PqConvGeometry geo;
+  if (int rc = CheckGeometry(who, Cin, Hin, Win, Cout, ksz, pad, stride, grp, &geo)) return rc;
   if (int rc = CheckConvK(who, K)) return rc;
   QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
   QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
   QCNN_CHECK(N >= 1, "%s: N=%d: at least one input is needed", who, N);
   QCNN_CHECK(x, "%s: NULL argument", who);
   QCNN_CHECK(!target || t, "%s: NULL t", who);
-  Geometry geo;
-  geo.Cin = Cin; geo.Hin = Hin; geo.Win = Win; geo.Cout = Cout; geo.ksz = ksz; geo.pad = pad; geo.stride = stride; geo.grp = grp;
-  geo.Ho = (Hin + 2 * pad - ksz) / stride + 1;
-  geo.Wo = (Win + 2 * pad - ksz) / stride + 1;
-  geo.Cg = Cin / grp; geo.Cpg = Cout / grp; geo.T = ksz * ksz; geo.Dg = geo.Cg * geo.T;
-  const long long sys = static_cast<long long>(K) * std::min(d, geo.Cg);
-  QCNN_CHECK(sys <= kMaxSystem, "%s: K*min(d, Cin/grp) = %d*%d = %lld exceeds %d, the size of the joint codebook system", who, K,
-             std::min(d, geo.Cg), sys, kMaxSystem);
-  return Refine(ctx, geo, K, d, sweeps, knl_h, x, t, N, ctrd_h, asmt_h, loss_h, static_cast<cudaStream_t>(stream));
+  if (int rc = CheckConvSystem(who, K, d, geo.Cg)) return rc;
+  std::vector<uint8_t> at;
+  std::vector<float> wp;
+  if (int rc = CheckConvHost(who, target, geo, K, d, knl_h, ctrd_h, asmt_h, at, wp)) return rc;
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  qcnn_pq_stats* sp = nullptr;
+  if (int rc = CreateConv(ctx, who, geo, d, target, &sp)) return rc;
+  std::unique_ptr<qcnn_pq_stats> s(sp);
+  if (int rc = ConvStatsAdd(s.get(), who, x, t, N, st)) return rc;
+  return SweepConv(s.get(), who, target, K, sweeps, wp, at, ctrd_h, asmt_h, loss_h, st);
 }
 
 }  // namespace
+
+namespace qcnn {
+
+// A conv add: the scan, then per group the positions in runs of F, each run's Gram (and cross product) read straight
+// from the maps and added in ascending order
+int ConvStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st) {
+  const PqConvGeometry& geo = s->geo;
+  const int Cout = geo.Cout, Cpg = geo.Cpg, Dg = geo.Dg, grp = geo.grp;
+  const size_t positions = static_cast<size_t>(N) * geo.Ho * geo.Wo;
+  unsigned first[2];
+  if (int rc = ScanAdd(s, y, static_cast<size_t>(N) * geo.Hin * geo.Win * geo.Cin, 1, t, positions * Cout, first, st)) return rc;
+  QCNN_CHECK(first[0] == kNoneFound, "%s: %s contains a non-finite value", who, s->target ? "y" : "x");
+  QCNN_CHECK(first[1] == kNoneFound, "%s: t contains a non-finite value", who);
+  QCNN_ON_DEVICE(s->ctx->device);
+  const bool acc0 = s->images > 0;
+  if (s->target && LaunchSqNorm(t, positions * Cout, s->scratch.as<double>(), s->tt.as<double>(), acc0, st)) return 1;
+  const size_t run = std::max<size_t>(1, std::min<size_t>(positions, kRunBytes / (sizeof(float) * Dg)));
+  const int tiles = CeilDiv(Dg, kTile);
+  for (int g = 0; g < grp; g++) {
+    double* Gg = s->G.as<double>() + static_cast<size_t>(g) * Dg * Dg;
+    for (size_t p0 = 0; p0 < positions; p0 += run) {
+      const int np = static_cast<int>(std::min<size_t>(run, positions - p0));
+      const int acc = acc0 || p0 > 0;
+      const MapOperand map{y, static_cast<long long>(p0), geo.Hin, geo.Win, geo.Cin, geo.ksz, geo.pad, geo.stride, geo.Ho, geo.Wo,
+                           geo.Cg, s->d, g};
+      pqr_gemm_kernel<kGemmGramMap><<<tiles * (tiles + 1) / 2, kGemmThreads, 0, st>>>(nullptr, 0, nullptr, 0, Gg, Dg, Dg, Dg, np, acc,
+                                                                                     map);
+      if (s->target)   // the run's target rows of group g's outputs against its patches
+        pqr_gemm_kernel<kGemmCrossMap><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
+            t + p0 * Cout + static_cast<size_t>(g) * Cpg, Cout, nullptr, 0, s->P.as<double>() + static_cast<size_t>(g) * Cpg * Dg, Dg,
+            Cpg, Dg, np, acc, map);
+      QCNN_CUDA(cudaGetLastError());
+    }
+  }
+  QCNN_CUDA(cudaEventRecord(s->done, st));
+  s->images += N;
+  return 0;
+}
+
+int ConvStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* knl_h, float* ctrd_h,
+                    uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+  if (int rc = CheckConvSystem(who, K, s->d, s->geo.Cg)) return rc;
+  std::vector<uint8_t> at;
+  std::vector<float> wp;
+  if (int rc = CheckConvHost(who, target, s->geo, K, s->d, knl_h, ctrd_h, asmt_h, at, wp)) return rc;
+  return SweepConv(s, who, target, K, sweeps, wp, at, ctrd_h, asmt_h, loss_h, st);
+}
+
+}  // namespace qcnn
 
 extern "C" int qcnn_pq_refine_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, int K,
                                    int d, int sweeps, const float* knl_h, const float* x, int N, float* ctrd_h, uint8_t* asmt_h,
@@ -671,4 +689,15 @@ extern "C" int qcnn_pq_refine_conv_target(qcnn_ctx* ctx, int Cin, int Hin, int W
                                           uint8_t* asmt_h, double* loss_h, void* stream) {
   return RefineConv(true, ctx, Cin, Hin, Win, Cout, ksz, pad, stride, grp, K, d, sweeps, nullptr, y, t, N,
                     ctrd_h, asmt_h, loss_h, stream);
+}
+
+extern "C" int qcnn_pq_stats_create_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp,
+                                         int d, int target, qcnn_pq_stats** out) {
+  const char* who = "qcnn_pq_stats_create_conv";
+  QCNN_CHECK(ctx && out, "%s: NULL argument", who);
+  *out = nullptr;
+  PqConvGeometry geo;
+  if (int rc = CheckGeometry(who, Cin, Hin, Win, Cout, ksz, pad, stride, grp, &geo)) return rc;
+  QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
+  return CreateConv(ctx, who, geo, d, target != 0, out);
 }

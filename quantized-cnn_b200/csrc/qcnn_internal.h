@@ -474,6 +474,16 @@ int OptInSmem(qcnn_ctx* ctx) {
 int CheckFcK(const char* who, int K);
 int CheckConvK(const char* who, int K);
 
+// pq_refine.cu / pq_refine_conv.cu: a conv layer's geometry as the error-correcting quantizer reads it, and the two
+// halves of the quantizer on a qcnn_pq_stats: folding a batch into the statistics, and the sweeps that read them
+struct PqConvGeometry { int Cin, Hin, Win, Cout, ksz, pad, stride, grp, Ho, Wo, Cg, Cpg, T, Dg; };
+int FcStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st);
+int ConvStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st);
+int FcStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wei_h, float* ctrd_h,
+                  uint8_t* asmt_h, double* loss_h, cudaStream_t st);
+int ConvStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* knl_h, float* ctrd_h,
+                    uint8_t* asmt_h, double* loss_h, cudaStream_t st);
+
 // conv_ws.cu: the tensor-core family's weight-stationary tilings of stride-1 layers (mode-0 geometry, channel tiles) and
 // of strided narrow-input layers (mode-1 geometry)
 void PlanConvWs(const qcnn_layer* L, int N, ConvCands* cands);
@@ -516,5 +526,23 @@ inline bool PoolWindowsNonEmpty(int in, int pad, int ksz, int stride) {
 }
 
 }  // namespace qcnn
+
+// The calibration statistics of one PQ layer for one subspace width d (DESIGN.md 4e): the sums over images that the
+// error-correcting quantizer reads, in the dim order of its sweeps.  Device buffers are owned; `done` is recorded on the
+// stream of the last add, so a refine or a read waits for the queued accumulation.
+struct qcnn_pq_stats {
+  qcnn_ctx* ctx = nullptr;
+  bool conv = false, target = false;
+  int d = 0;
+  int Din = 0, Dout = 0;          // FC
+  qcnn::PqConvGeometry geo{};     // conv
+  long long images = 0;
+  qcnn::DeviceBuffer G, P, tt;    // G [grp][Dg][Dg] (FC [Din][Din]); target: P [Cout][Dg] (FC [Dout][Din]) and |T|^2
+  qcnn::DeviceBuffer scratch;     // the |T_b|^2 partials [kLossBlocks] fp64, then the add's two scan flags
+  cudaEvent_t done = nullptr;
+  ~qcnn_pq_stats() {
+    if (done) cudaEventDestroy(done);
+  }
+};
 
 #endif  // QCNN_INTERNAL_H_

@@ -15,7 +15,13 @@ relative error of the final logits against the original network's (over all imag
 errors) and the top-1 / top-5 agreement with its
 predictions (top-5: the original's top-1 class is among the mode's five best), and the card, its power limit and max SM
 clock, all from the same run.
-    python tools/pq_refine_chain.py [--train 4096] [--held 1024] [--sweeps 4] [--conv 32 8] [--fc8 16 4] [--out f.json]"""
+With --stats the calibration images stream through in batches of --batch: per layer and mode, each batch's inputs y
+(and for the target mode the original network's responses t) are added to a PqStats object and dropped, and the
+refinement runs on the accumulated statistics (qcnn_pq_stats_refine / _refine_target), so no layer's inputs or targets
+are ever held whole and device memory does not grow with --train.  Each call time is then the accumulation plus the
+refinement, printed with the peak device memory of that layer and mode (torch's peak allocation plus the statistics).
+    python tools/pq_refine_chain.py [--train 4096] [--held 1024] [--sweeps 4] [--conv 32 8] [--fc8 16 4] [--stats]
+                                    [--out f.json]"""
 import argparse
 import importlib
 import json
@@ -87,6 +93,71 @@ def logits(net, imgs, batch):
     return torch.cat(out)
 
 
+class LcgImages(object):
+    """po.lcg_images on the device, bit for bit: image i's values are s_j = a^j seed + c (a^j - 1) / (a - 1) mod 2^32
+    (a = 1664525, c = 1013904223, j = 1 .. 3 x 227 x 227), so a batch of images is one elementwise pass from two
+    precomputed per-value tables instead of a sequential host loop per image."""
+
+    def __init__(self, chw):
+        import torch
+        n = int(np.prod(chw))
+        A, Cc = np.empty(n, np.int64), np.empty(n, np.int64)
+        a, c = 1, 0
+        for j in range(n):
+            a, c = (a * 1664525) & 0xFFFFFFFF, (c * 1664525 + 1013904223) & 0xFFFFFFFF
+            A[j], Cc[j] = a, c
+        self.A, self.C, self.chw = torch.from_numpy(A).cuda(), torch.from_numpy(Cc).cuda(), tuple(chw)
+
+    def __call__(self, count, seed0, chunk=16):
+        import torch
+        out = torch.empty((count,) + self.chw, dtype=torch.float32, device="cuda")
+        flat = out.view(count, -1)
+        for i in range(0, count, chunk):
+            seeds = (torch.arange(i, min(count, i + chunk), device="cuda", dtype=torch.int64) + seed0) & 0xFFFFFFFF
+            lo, hi = (seeds & 0xFFFF)[:, None], (seeds >> 16)[:, None]
+            s = (self.A * lo + (((self.A * hi) & 0xFFFF) << 16) + self.C) & 0xFFFFFFFF
+            flat[i:i + seeds.shape[0]] = ((s >> 8) & 0xFFFF).float() / 65536.0 * 256.0 - 128.0
+        return out
+
+
+def refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc, target):
+    """Accumulate layer l's statistics over the calibration images batch by batch (inputs from `net`, targets from the
+    original network), then refine on them: (ctrd, asmt, loss, seconds in the adds and the refine, peak device bytes)"""
+    import torch
+    conv = W.ndim == 4
+    d = c0.shape[2]
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    st, secs = None, 0.0
+    for i in range(0, args.train, args.batch):
+        b = min(args.batch, args.train - i)
+        imgs = args.lcg(b, args.seed + i)
+        y = layer_inputs(net, l, imgs, b, first_fc)
+        t = response(L, layer_inputs(orig, l, imgs, b, first_fc), W, b) if target else None
+        if st is None:
+            if conv:
+                _, Hin, Win, Cin = y.shape
+                st = q.PqStats.conv(ctx, Cin, Hin, Win, W.shape[0], L["k"], d, pad=L["pad"], stride=L["stride"],
+                                    grp=L["grp"], target=target)
+            else:
+                st = q.PqStats.fc(ctx, y.shape[1], W.shape[0], d, target=target)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        st.add(y, t)
+        torch.cuda.synchronize()   # y and t may be freed once the add has run
+        secs += time.perf_counter() - t0
+        del imgs, y, t
+    t0 = time.perf_counter()
+    if target:
+        c, a, loss = st.refine_target(c0, a0, sweeps=args.sweeps)
+    else:
+        c, a, loss = st.refine(W, c0, a0, sweeps=args.sweeps)
+    secs += time.perf_counter() - t0
+    peak = torch.cuda.max_memory_allocated() + st.nbytes
+    st.close()
+    return c, a, loss, secs, peak
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--train", type=int, default=4096, help="calibration images")
@@ -99,6 +170,7 @@ def main():
     ap.add_argument("--fc8", type=int, nargs=2, default=(16, 4), metavar=("K", "d"))
     ap.add_argument("--seed", type=int, default=1000000, help="image seed: calibration, then held-out")
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
+    ap.add_argument("--stats", action="store_true", help="stream the calibration images through PqStats objects")
     args = ap.parse_args()
     import torch
     from oracle import pyoracle as po
@@ -115,7 +187,8 @@ def main():
     params = po.load_model(po.ALEXNET_DIR, po.ALEXNET_PFX, layers)
     cin = {l: shapes[l][2] // layers[l]["grp"] if layers[l]["type"] == po.CONV else int(np.prod(shapes[l])) for l in NAMES}
     dense = {l: decode(params[l]["ctrd"], params[l]["asmt"], cin[l]) for l in NAMES}
-    train = torch.from_numpy(po.lcg_images(args.train, args.seed)).cuda()
+    train = None if args.stats else torch.from_numpy(po.lcg_images(args.train, args.seed)).cuda()
+    args.lcg = LcgImages(po.ALEXNET_IN) if args.stats else None
     held = torch.from_numpy(po.lcg_images(args.held, args.seed + args.train)).cuda()
     hw = card()
     print("card: %s (name, power limit, max SM clock)" % hw)
@@ -134,10 +207,16 @@ def main():
             conv = L["type"] == po.CONV
             quant = q.pq_quantize_conv if conv else q.pq_quantize_fc
             c0, a0, _ = quant(ctx, W, K, d, iters=20, seed=1)
-            t = response(L, layer_inputs(orig, l, train, args.batch, first_fc), W, args.batch)
+            t = None if args.stats else response(L, layer_inputs(orig, l, train, args.batch, first_fc), W, args.batch)
             for mode in MODES:
-                c, a, ratio, secs = c0, a0, None, None
-                if mode != "kmeans":
+                c, a, ratio, secs, peak = c0, a0, None, None, None
+                if mode != "kmeans" and args.stats:
+                    net = net_of(mode)
+                    c, a, loss, secs, peak = refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc,
+                                                             mode == "target")
+                    net.close()
+                    ratio = float(loss[-1] / loss[0])
+                elif mode != "kmeans":
                     net = net_of(mode)
                     y = layer_inputs(net, l, train, args.batch, first_fc)
                     net.close()
@@ -155,9 +234,10 @@ def main():
                     ratio = float(loss[-1] / loss[0])
                     del y
                 qparams[mode][l] = dict(bias=params[l]["bias"], ctrd=c, asmt=a, bits=po.bits_for(K))
-                rows.append(dict(layer=NAMES[l], K=K, d=d, mode=mode, loss_ratio=ratio, call_s=secs))
+                rows.append(dict(layer=NAMES[l], K=K, d=d, mode=mode, loss_ratio=ratio, call_s=secs, peak_bytes=peak))
                 if ratio is not None:
-                    print("%-6s K=%-3d d=%-2d %-10s training loss x%.4f  call %.2f s" % (NAMES[l], K, d, mode, ratio, secs))
+                    print("%-6s K=%-3d d=%-2d %-10s training loss x%.4f  call %.2f s%s"
+                          % (NAMES[l], K, d, mode, ratio, secs, "" if peak is None else "  peak %.2f GB" % (peak / 1e9)))
             del t
             torch.cuda.empty_cache()
         orig.close()
@@ -177,8 +257,8 @@ def main():
                   "top-5 agreement %.4f" % (mode, err, med, agree1, agree5))
     if args.out:
         with open(args.out, "w") as f:
-            json.dump(dict(card=hw, train=args.train, held=args.held, sweeps=args.sweeps, layers=rows, modes=summary), f,
-                      indent=1)
+            json.dump(dict(card=hw, train=args.train, held=args.held, sweeps=args.sweeps, stats=args.stats, layers=rows,
+                           modes=summary), f, indent=1)
     ctx.close()
 
 

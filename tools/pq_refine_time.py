@@ -16,8 +16,13 @@ time of a whole call with the profiler off.
 With --target the same layers run the target form (qcnn_pq_refine_fc_target / _conv_target) on targets
 t = (the layer's response) + 0.3 (a seeded Gaussian), and each layer also reports the cross-product GEMM P = T^T Y next
 to the Gram, with its fp64 TFLOP/s (2 N Din Dout for FC, 2 positions Cout Cg k^2 for conv).
-    python tools/pq_refine_time.py [--sweeps 3] [--target] [--layers alexnet_fc6 alexnet_conv1 vgg16_conv1_2 ...]"""
+The conv Gram and cross product read the patches straight from the maps; a library that builds them with an im2col
+kernel (pqrc_patch_kernel) has that kernel counted with the Gram, so two builds compare.  --digest prints the sha256 of
+every layer's (ctrd, asmt, loss) bytes, and --root loads the package (and so the library) from another tree, so that
+one script checks two builds for identical results:
+    python tools/pq_refine_time.py [--sweeps 3] [--target] [--digest] [--root TREE] [--layers alexnet_fc6 ...]"""
 import argparse
+import hashlib
 import importlib
 import json
 import os
@@ -29,7 +34,6 @@ import time
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
 
 LAYERS = {   # name: (Din, Dout, K, d, N)
     "alexnet_fc6": (9216, 4096, 32, 4, 4 * 9216),
@@ -66,7 +70,8 @@ def kernels(prof):
 
 
 def gemm_mode(name):
-    """pqr_gemm_kernel's template argument (0: fp64 GEMM, 1: Gram, 2: cross product), or None for another kernel"""
+    """pqr_gemm_kernel's template argument (0: fp64 GEMM, 1: Gram, 2: cross product, 3 / 4: the Gram / cross product
+    on an NHWC map), or None for another kernel"""
     m = re.search(r"pqr_gemm_kernel<(?:\(int\))?(\d)>", name)
     return int(m.group(1)) if m else None
 
@@ -74,6 +79,14 @@ def gemm_mode(name):
 def loss_ends(ev):
     """indices of the loss kernels that close the start and every sweep (not the |T|^2 reduction's final kernel)"""
     return [i for i, (n, _, _) in enumerate(ev) if "pqr_loss_final" in n and not (i > 0 and "pqr_sqnorm" in ev[i - 1][0])]
+
+
+def digest(res):
+    """sha256 of the (ctrd, asmt, loss) bytes of one call"""
+    h = hashlib.sha256()
+    for a in res:
+        h.update(np.ascontiguousarray(a).tobytes())
+    return h.hexdigest()
 
 
 def time_conv(q, ctx, name, sweeps, target):
@@ -100,8 +113,8 @@ def time_conv(q, ctx, name, sweeps, target):
         _, _, loss = run(x, tg, sweeps)
         torch.cuda.synchronize()
     ev = kernels(prof)
-    gram = sum(t for n, _, t in ev if gemm_mode(n) == 1 or "pqrc_patch" in n)
-    cross = sum(t for n, _, t in ev if gemm_mode(n) == 2)
+    gram = sum(t for n, _, t in ev if gemm_mode(n) in (1, 3) or "pqrc_patch" in n)
+    cross = sum(t for n, _, t in ev if gemm_mode(n) in (2, 4))
     ends = loss_ends(ev)
     split = dict(chol=[], assign=[], gemm=[], system=[], total=[])
     for a, b in zip(ends[:-1], ends[1:]):
@@ -125,7 +138,7 @@ def time_conv(q, ctx, name, sweeps, target):
             split[key].append(acc[key])
     med = {key: float(np.median(v)) / 1e3 for key, v in split.items()}
     t0 = time.perf_counter()
-    run(x, tg, sweeps)
+    res = run(x, tg, sweeps)
     wall = time.perf_counter() - t0
     Ho = (H + 2 * pad - k) // stride + 1
     T, Dg, S = k * k, Cg * k * k, -(-Cg // d)
@@ -138,7 +151,7 @@ def time_conv(q, ctx, name, sweeps, target):
              sweep_ms=med["total"], sweep_chol_ms=med["chol"], sweep_assign_ms=med["assign"], sweep_gemm_ms=med["gemm"],
              sweep_system_ms=med["system"], gemm_tflops=gemm_flop / (med["gemm"] * 1e-3) / 1e12,
              chol_tflops=chol_flop / (med["chol"] * 1e-3) / 1e12, call_wall_s=wall,
-             loss=[float(v) for v in loss], loss_ratio=float(loss[-1] / loss[0]), target=target)
+             loss=[float(v) for v in loss], loss_ratio=float(loss[-1] / loss[0]), target=target, digest=digest(res))
     if target:
         r.update(cross_ms=cross / 1e3, cross_tflops=2.0 * N * Ho * Ho * Cout * Dg / (cross * 1e-6) / 1e12)
         print("%-14s cross product %8.2f ms (%5.1f TFLOP/s)" % (name, r["cross_ms"], r["cross_tflops"]))
@@ -158,13 +171,17 @@ def main():
     ap.add_argument("--layers", nargs="*", default=list(LAYERS) + list(CONV_LAYERS))
     ap.add_argument("--target", action="store_true", help="time the target form (with the cross-product GEMM)")
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
+    ap.add_argument("--digest", action="store_true", help="print the sha256 of every layer's (ctrd, asmt, loss)")
+    ap.add_argument("--root", default=ROOT, help="tree to load quantized-cnn_b200 (and its library) from")
     args = ap.parse_args()
+    sys.path.insert(0, os.path.abspath(args.root))
     import torch
     from torch.profiler import ProfilerActivity, profile
     assert torch.cuda.is_available(), "needs a GPU"
     q = importlib.import_module("quantized-cnn_b200")
     ctx = q.Context(0)
     print("card: %s (name, power limit, max SM clock)" % card())
+    print("library: %s" % q.LIB_PATH)
     results = []
     for name in args.layers:
         if name in CONV_LAYERS:
@@ -197,7 +214,7 @@ def main():
             blk.append(sum(t for n, _, t in part if "pqr_block_kernel" in n))
             trail.append(sum(t for n, _, t in part if gemm_mode(n) == 0))
         t0 = time.perf_counter()
-        run(x, tg, args.sweeps)
+        res = run(x, tg, args.sweeps)
         wall = time.perf_counter() - t0
         sweep_ms = float(np.median(sweeps)) / 1e3
         gram_ms = gram / 1e3
@@ -205,7 +222,8 @@ def main():
                  gram_tflops=N * Din * (Din + 1) / (gram_ms * 1e-3) / 1e12, sweep_ms=sweep_ms,
                  sweep_block_kernel_ms=float(np.median(blk)) / 1e3, sweep_gemm_ms=float(np.median(trail)) / 1e3,
                  sweep_tflops=2.0 * Dout * Din * Din / (sweep_ms * 1e-3) / 1e12, call_wall_s=wall,
-                 loss=[float(v) for v in loss], loss_ratio=float(loss[-1] / loss[0]), target=args.target)
+                 loss=[float(v) for v in loss], loss_ratio=float(loss[-1] / loss[0]), target=args.target,
+                 digest=digest(res))
         if args.target:
             r.update(cross_ms=cross / 1e3, cross_tflops=2.0 * N * Din * Dout / (cross * 1e-6) / 1e12)
             print("%-12s cross product %8.2f ms (%5.1f TFLOP/s)" % (name, r["cross_ms"], r["cross_tflops"]))
@@ -217,6 +235,9 @@ def main():
         print("  loss trace: " + " ".join("%.6g" % v for v in loss))
         del x, tg
         torch.cuda.empty_cache()
+    if args.digest:
+        for r in results:
+            print("digest %-14s %s" % (r["layer"], r["digest"]))
     if args.out:
         with open(args.out, "w") as f:
             json.dump(dict(card=card(), sweeps=args.sweeps, results=results), f, indent=1)
