@@ -415,7 +415,32 @@ QCNN_API int qcnn_pq_refine_conv_target(qcnn_ctx* ctx, int Cin, int Hin, int Win
  *   results and checks (K, the joint-system limit, an assignment >= K, a non-finite codebook or weights) plus a call
  *   before any add; refine works on either kind of object (it reads only G), refine_target needs a target object.  They
  *   read the statistics and never change them, so either may run any number of times.  They wait for the queued adds,
- *   run on `stream` and synchronise it; device memory is that of the one-shot call less G and P. */
+ *   run on `stream` and synchronise it; device memory is that of the one-shot call less G and P.
+ * First moments (for the bias refit below): every object also sums, in fp64, s = the sum of y (FC [Din]; conv [grp][Dg]
+ *   in the dim order above, the zero-padded patches summed over every image and output position, so a tap outside the map
+ *   adds 0) and, for a target object, u = the sum of t (FC [Dout]; conv [Cout], over every image and output position);
+ *   n = the rows summed: images (FC) or images Ho Wo (conv).  Fold rule (normative): each add forms its batch's sums
+ *   fresh, in a fixed order that does not depend on the values, and adds them to the running sums with one addition per
+ *   element; the first add stores instead of adding.  So adds of y and -y leave s = 0 exactly, and the same sequence of
+ *   adds gives the same bits.  The sums are queued after the scan, so a rejected add leaves them unchanged.  They take
+ *   8 (Din + Dout) bytes (FC) or 8 (grp Dg + Cout) (conv; u only for a target object), and a conv object another
+ *   8 Hin Win Cin (target: 8 max(Hin Win Cin, Ho Wo Cout)) for an add's per-image-position sum.
+ * read_sums_h: waits for the queued adds and copies each non-NULL output; u needs a target object.
+ * refine_bias / refine_target_bias: refine / refine_target with the bias free as well.  For fixed W^ the best bias is
+ *   b^ = b + mean(t - W^ y) (target) or b + (W - W^) mean(y) (same input); with it the loss is the same quadratic in the
+ *   centered sums, so the unchanged sweeps run on centered copies, formed elementwise with every operation rounded (no
+ *   contraction): Gc[i][j] = G[i][j] - (s[i] s[j]) / n (per group for conv; exactly symmetric), Pc[o][q] = P[o][q] -
+ *   (u[o] s_g[q]) / n, |T_c|^2 = |T|^2 - sum over o ascending of (u[o] u[o]) / n.  Every rule of the sweeps (skip, ridge,
+ *   acceptance, ties) is evaluated on the centered sums.  Then, in fp64 from the final (ctrd, asmt) and g the group of
+ *   output o: delta_o = (u_o - w^_o . s_g) / n (target) or (w_o - w^_o) . s_g / n (same input), and bias_h[o] becomes
+ *   fp32(bias_h[o] + delta_o).  loss_h = the bias-optimal loss: the start's, then one value after each sweep.  The calls
+ *   reject what refine / refine_target reject, plus a NULL or non-finite bias_h; they never change the statistics.
+ *   Device memory: that of refine / refine_target plus the centered copies, 8 Din^2 (+ 8 Dout Din for the target form)
+ *   bytes (FC; VGG16 fc6: +5.0 GB) or 8 grp Dg^2 (+ 8 Cout Dg) (conv).
+ * Skip rule of every sweep: a subspace (conv: a (group, tap) in the assignment step) is skipped when !(tr > 0) for the
+ *   trace of its diagonal block, so a centered block with a rounding-level negative trace is skipped; on raw sums the
+ *   trace is a sum of squares, so this is tr == 0.  A codeword solve that is not finite (a centered block that is
+ *   singular at rounding level) fails the strict acceptance test and never enters the codebook. */
 typedef struct qcnn_pq_stats qcnn_pq_stats;
 QCNN_API int qcnn_pq_stats_create_fc(qcnn_ctx* ctx, int Din, int Dout, int d, int target, qcnn_pq_stats** out);
 QCNN_API int qcnn_pq_stats_create_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride,
@@ -429,6 +454,13 @@ QCNN_API int qcnn_pq_stats_refine(qcnn_pq_stats* s, int K, int sweeps, const flo
                                   float* ctrd_h, uint8_t* asmt_h, double* loss_h, void* stream);
 QCNN_API int qcnn_pq_stats_refine_target(qcnn_pq_stats* s, int K, int sweeps, float* ctrd_h, uint8_t* asmt_h,
                                          double* loss_h, void* stream);
+/* s [grp][Dg] (FC [Din]), internal dim order; u [Cout] (FC [Dout]), target objects only; n = images (FC) or images*Ho*Wo */
+QCNN_API int qcnn_pq_stats_read_sums_h(const qcnn_pq_stats* s, double* s_h, double* u_h, long long* n_h);
+/* refine / refine_target on the centered sums; bias_h [Dout] / [Cout] in/out: the layer's bias, replaced by the refit one */
+QCNN_API int qcnn_pq_stats_refine_bias(qcnn_pq_stats* s, int K, int sweeps, const float* wei_h, float* ctrd_h,
+                                       uint8_t* asmt_h, float* bias_h, double* loss_h, void* stream);
+QCNN_API int qcnn_pq_stats_refine_target_bias(qcnn_pq_stats* s, int K, int sweeps, float* ctrd_h, uint8_t* asmt_h,
+                                              float* bias_h, double* loss_h, void* stream);
 QCNN_API void qcnn_pq_stats_destroy(qcnn_pq_stats* s);
 
 /* ---- file formats (include/FileIO.h:56-178, 229-350), host only ------------------------------------------- */

@@ -140,6 +140,9 @@ _SIGS = {
     "qcnn_pq_stats_read_h": (_i, [_vp, _vp, _vp, _vp]),
     "qcnn_pq_stats_refine": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "qcnn_pq_stats_refine_target": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_stats_read_sums_h": (_i, [_vp, _vp, _vp, C.POINTER(C.c_longlong)]),
+    "qcnn_pq_stats_refine_bias": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_stats_refine_target_bias": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "qcnn_pq_stats_destroy": (None, [_vp]),
 }
 for _name, (_res, _args) in _SIGS.items():
@@ -769,8 +772,9 @@ class PqStats(object):
     """Calibration statistics of one layer for one subspace width d (include/qcnn.h, DESIGN.md 4e): add() folds a batch
     of layer inputs y (and, with target=True, the original layer's responses t) into the sums the error-correcting
     refinement reads, so the calibration set can be streamed in batches; refine() / refine_target() then run the sweeps
-    of pq_refine_* / pq_refine_*_target on the sums, any number of times.  Device memory does not grow with the number
-    of images."""
+    of pq_refine_* / pq_refine_*_target on the sums, any number of times; refine_bias() / refine_target_bias() also
+    refit the layer's bias, from the first moments read_sums() returns.  Device memory does not grow with the number of
+    images."""
 
     def __init__(self, ctx, h, conv, shape, target):
         self.ctx, self.h, self.conv, self.target = ctx, h, conv, target
@@ -835,6 +839,30 @@ class PqStats(object):
                                         None if tt is None else tt.ctypes.data_as(_vp)))
         return G, P, None if tt is None else float(tt[0])
 
+    def read_sums(self):
+        """(s, u, n): the sum of y, s [grp, Dg] conv (internal dim order) / [Din] FC, the sum of t, u [Cout] / [Dout]
+        for a target object (else None), as float64 host arrays, and n, the rows summed (images, conv images Ho Wo)."""
+        self._live()
+        g = self._shape
+        if self.conv:
+            sy = np.empty((g["grp"], g["Cin"] // g["grp"] * g["ksz"] * g["ksz"]), np.float64)
+        else:
+            sy = np.empty(g["Din"], np.float64)
+        u = np.empty(self._outputs(), np.float64) if self.target else None
+        n = C.c_longlong()
+        _check(lib.qcnn_pq_stats_read_sums_h(self.h, sy.ctypes.data_as(_vp), None if u is None else u.ctypes.data_as(_vp),
+                                             C.byref(n)))
+        return sy, u, n.value
+
+    def _outputs(self):
+        return self._shape["Cout"] if self.conv else self._shape["Dout"]
+
+    def _bias(self, bias):
+        bias = np.array(bias, np.float32, order="C", copy=True)
+        if bias.shape != (self._outputs(),):
+            raise QcnnError("bias must be (%d,), got %s" % (self._outputs(), bias.shape))
+        return bias
+
     def _start(self, ctrd, asmt):
         ctrd = np.array(ctrd, np.float32, order="C", copy=True)
         asmt = np.array(asmt, np.uint8, order="C", copy=True)
@@ -876,14 +904,43 @@ class PqStats(object):
                                                loss.ctypes.data_as(_vp), _stream(stream)))
         return ctrd, asmt, loss
 
+    def refine_bias(self, wei, ctrd, asmt, bias, sweeps=8, stream=None):
+        """refine() with the bias free as well: the sweeps on the centered sums, then the bias refit (include/qcnn.h).
+        bias [Dout] / [Cout] is the layer's bias.  Returns (ctrd, asmt, bias, loss [sweeps + 1]), loss the bias-optimal
+        one; the arguments are not modified."""
+        self._live()
+        ctrd, asmt, K = self._start(ctrd, asmt)
+        g = self._shape
+        wei = _np(wei, np.float32)
+        want = (g["Cout"], g["Cin"] // g["grp"], g["ksz"], g["ksz"]) if self.conv else (g["Dout"], g["Din"])
+        if wei.shape != want:
+            raise QcnnError("wei must be %s, got %s" % (want, wei.shape))
+        bias = self._bias(bias)
+        loss = np.empty(max(sweeps, 0) + 1, np.float64)
+        _check(lib.qcnn_pq_stats_refine_bias(self.h, K, sweeps, wei.ctypes.data_as(_vp), ctrd.ctypes.data_as(_vp),
+                                             asmt.ctypes.data_as(_vp), bias.ctypes.data_as(_vp), loss.ctypes.data_as(_vp),
+                                             _stream(stream)))
+        return ctrd, asmt, bias, loss
+
+    def refine_target_bias(self, ctrd, asmt, bias, sweeps=8, stream=None):
+        """refine_target() with the bias free as well: (ctrd, asmt, bias, loss [sweeps + 1]).  The arguments are not
+        modified."""
+        self._live()
+        ctrd, asmt, K = self._start(ctrd, asmt)
+        bias = self._bias(bias)
+        loss = np.empty(max(sweeps, 0) + 1, np.float64)
+        _check(lib.qcnn_pq_stats_refine_target_bias(self.h, K, sweeps, ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp),
+                                                    bias.ctypes.data_as(_vp), loss.ctypes.data_as(_vp), _stream(stream)))
+        return ctrd, asmt, bias, loss
+
     @property
     def nbytes(self):
-        """device bytes of the sums (G, and for a target object P and |T|^2)"""
+        """device bytes of the sums (G and s, and for a target object P, |T|^2 and u)"""
         g = self._shape
         if self.conv:
             Dg = g["Cin"] // g["grp"] * g["ksz"] * g["ksz"]
-            return 8 * (g["grp"] * Dg * Dg + (g["Cout"] * Dg + 1 if self.target else 0))
-        return 8 * (g["Din"] * g["Din"] + (g["Dout"] * g["Din"] + 1 if self.target else 0))
+            return 8 * (g["grp"] * Dg * (Dg + 1) + ((Dg + 1) * g["Cout"] + 1 if self.target else 0))
+        return 8 * (g["Din"] * (g["Din"] + 1) + ((g["Din"] + 1) * g["Dout"] + 1 if self.target else 0))
 
     def close(self):
         if self.h:

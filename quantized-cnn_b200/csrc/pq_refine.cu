@@ -2,7 +2,7 @@
 // assignments so that the layer's response W x is kept on given inputs (the paper's quantization with error correction).
 // Semantics, normative (DESIGN.md 4e):
 //   G = X^T X (fp64, fixed order), E = W - W^ (fp64), loss = sum_o E_o^T G E_o = sum_n |(W - W^) x_n|^2.
-//   A sweep visits subspaces m = 0..S-1 in order (Gauss-Seidel); a subspace with tr(G_mm) = 0 is skipped.
+//   A sweep visits subspaces m = 0..S-1 in order (Gauss-Seidel); a subspace with !(tr(G_mm) > 0) is skipped.
 //   h_o = [G E_o]_m + G_mm w^_o(m); H_k = sum_{a_o = k} h_o (fixed order), n_k = |{o : a_o = k}|.
 //   codebook   D = (G_mm + lambda I)^-1 H_k / n_k by the Cholesky factor, lambda = 1e-10 tr(G_mm) / w_m, rounded to fp32;
 //              D replaces c_k only if f(D) < f(c_k), f(D) = n_k D^T G_mm D - 2 D^T H_k; empty clusters keep their codeword.
@@ -36,7 +36,7 @@ constexpr int kMaxD = 64;
 constexpr int kBlockDims = 256;      // dims per block of subspaces (a multiple of d): the K of the trailing GEMM
 
 // Per subspace m (blockIdx.x): the lower-triangular inverse of the Cholesky factor of G_mm + lambda I, [w][w] at row
-// pitch d.  G does not change between sweeps, so this runs once per call.  Skipped subspaces (tr(G_mm) = 0) get none.
+// pitch d.  G does not change between sweeps, so this runs once per call.  Skipped subspaces (!(tr(G_mm) > 0)) get none.
 __global__ void __launch_bounds__(kSweepThreads) pqr_chol_kernel(const double* __restrict__ G, double* __restrict__ Linv, int Din,
                                                                  int d) {
   extern __shared__ double chol_sm[];
@@ -45,7 +45,7 @@ __global__ void __launch_bounds__(kSweepThreads) pqr_chol_kernel(const double* _
   double* Li = chol_sm + w * ld;  // [w][w + 1]
   double tr = 0.0;
   for (int j = 0; j < w; j++) tr += G[static_cast<size_t>(c0 + j) * (Din + 1)];
-  if (tr == 0.0) return;
+  if (!(tr > 0.0)) return;   // also a centered G's rounding-level negative or NaN trace
   const double lam = 1e-10 * tr / w;
   for (int e = tid; e < w * w; e += blockDim.x) {
     const int i = e / w, j = e % w;
@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(kSweepThreads) pqr_block_kernel(BlockArgs p) {
     const int c0 = m * d, w = min(d, Din - c0), cb = c0 - blk0;
     double tr = 0.0;
     for (int j = 0; j < w; j++) tr += p.G[static_cast<size_t>(c0 + j) * (Din + 1)];
-    if (tr == 0.0) continue;   // no input energy: codebook and assignments stay
+    if (!(tr > 0.0)) continue;   // no input energy: codebook and assignments stay
     const uint8_t* Am = p.A + static_cast<size_t>(m) * Dout;
     const float* Cm = p.C + static_cast<size_t>(m) * K * d;
     // (1) h_o = GE_o[c0 + j] + sum_{c in block, c < c0} dlt_o[c] G[c0 + j][c] + sum_i G[c0 + j][c0 + i] w^_o[i]:
@@ -279,9 +279,11 @@ int CheckFcHost(const char* who, bool target, int Din, int Dout, int K, int d, c
   return 0;
 }
 
-// The sweeps on the statistics of s.  target: the target form (w_h is not read); else the same-input form on w_h.
-int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* w_h, std::vector<uint8_t>& at,
-            float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+// The sweeps on the sums G, P = T^T Y and |T|^2 (those of s, or their centered copies).  target: the target form (w_h is
+// not read); else the same-input form on w_h.  bias_h non-NULL: replaced by the refit bias (RefitBias).
+int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* w_h, const double* G,
+            const double* TY, const double* TT, std::vector<uint8_t>& at, float* ctrd_h, uint8_t* asmt_h, float* bias_h,
+            double* loss_h, cudaStream_t st) {
   qcnn_ctx* ctx = s->ctx;
   const int Din = s->Din, Dout = s->Dout, d = s->d, S = CeilDiv(Din, d);
   const size_t nw = static_cast<size_t>(Dout) * Din, nc = static_cast<size_t>(S) * K * d;
@@ -304,8 +306,7 @@ int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, c
       reserve(dCc, sizeof(double) * K, "the codeword norms") || reserve(dPart, sizeof(double) * kLossBlocks, "the loss") ||
       reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss"))
     return 1;
-  const double* G = s->G.as<double>();
-  const double* TY = target ? s->P.as<double>() : nullptr;
+  if (!target) TY = TT = nullptr;
   QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
   if (target) QCNN_CUDA(cudaMemsetAsync(dW.get(), 0, sizeof(float) * nw, st));   // E = 0 - W^
   else QCNN_CUDA(cudaMemcpyAsync(dW.get(), w_h, sizeof(float) * nw, cudaMemcpyHostToDevice, st));
@@ -323,8 +324,7 @@ int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, c
   pqr_gemm_kernel<kGemmF64><<<gemmGrid, kGemmThreads, 0, st>>>(dE.get(), Din, G, Din, dGE.as<double>(), Din, Dout, Din, Din, target);
   QCNN_CUDA(cudaGetLastError());
   auto loss = [&](int sw) -> int {
-    return LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st, TY,
-                      target ? s->tt.as<double>() : nullptr);
+    return LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st, TY, TT);
   };
   if (int rc = loss(0)) return rc;
   if (sweeps > 0) {
@@ -354,6 +354,10 @@ int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, c
       if (int rc = loss(sw)) return rc;
     }
   }
+  if (bias_h) {   // E = W - W^ (target: -W^) afresh from the final codebook and assignments
+    pqr_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Din, Dout, K, d);
+    if (int rc = RefitBias(s, who, target, dE.as<double>(), 1, Din, Dout, bias_h, st)) return rc;
+  }
   std::vector<double> lossv(sweeps + 1);
   QCNN_CUDA(cudaMemcpyAsync(ctrd_h, dC.get(), sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
   QCNN_CUDA(cudaMemcpyAsync(at.data(), dA.get(), at.size(), cudaMemcpyDeviceToHost, st));
@@ -365,7 +369,7 @@ int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, c
   return 0;
 }
 
-int CreateFc(qcnn_ctx* ctx, const char* who, int Din, int Dout, int d, bool target, qcnn_pq_stats** out) {
+int CreateFc(qcnn_ctx* ctx, const char* who, int Din, int Dout, int d, bool target, bool sums, qcnn_pq_stats** out) {
   QCNN_CHECK(ctx && out, "%s: NULL argument", who);
   *out = nullptr;
   QCNN_CHECK(Din >= 1 && Dout >= 1, "%s: bad dimensions", who);
@@ -377,13 +381,16 @@ int CreateFc(qcnn_ctx* ctx, const char* who, int Din, int Dout, int d, bool targ
   s->d = d;
   s->Din = Din;
   s->Dout = Dout;
-  if (AllocStats(s.get(), who, sizeof(double) * Din * static_cast<size_t>(Din), sizeof(double) * Dout * static_cast<size_t>(Din)))
+  s->sums = sums;
+  if (AllocStats(s.get(), who, sizeof(double) * Din * static_cast<size_t>(Din), sizeof(double) * Dout * static_cast<size_t>(Din),
+                 sizeof(double) * Din, sizeof(double) * Dout, 0))
     return 1;
   *out = s.release();
   return 0;
 }
 
-// The one-shot calls: create, one add of all N inputs, the sweeps, destroy (the checks keep the order of their messages)
+// The one-shot calls: create (without the first moments, which they never read), one add of all N inputs, the sweeps,
+// destroy (the checks keep the order of their messages)
 int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int sweeps, const float* w_h, const float* x, const float* t,
            int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
   const char* who = target ? "qcnn_pq_refine_fc_target" : "qcnn_pq_refine_fc";
@@ -398,17 +405,19 @@ int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int swee
   std::vector<uint8_t> at;
   if (int rc = CheckFcHost(who, target, Din, Dout, K, d, w_h, ctrd_h, asmt_h, at)) return rc;
   qcnn_pq_stats* sp = nullptr;
-  if (int rc = CreateFc(ctx, who, Din, Dout, d, target, &sp)) return rc;
+  if (int rc = CreateFc(ctx, who, Din, Dout, d, target, false, &sp)) return rc;
   std::unique_ptr<qcnn_pq_stats> s(sp);
   if (int rc = FcStatsAdd(s.get(), who, x, t, N, st)) return rc;
-  return SweepFc(s.get(), who, target, K, sweeps, w_h, at, ctrd_h, asmt_h, loss_h, st);
+  return SweepFc(s.get(), who, target, K, sweeps, w_h, s->G.as<double>(), s->P.as<double>(), s->tt.as<double>(), at, ctrd_h,
+                 asmt_h, nullptr, loss_h, st);
 }
 
 }  // namespace
 
 namespace qcnn {
 
-// An FC add: the scan (its message names the first input column holding a NaN or Inf), then one fold
+// An FC add: the scan (its message names the first input column holding a NaN or Inf), then one fold of the sums
+// (G, then s; for a target |T|^2, P, then u)
 int FcStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st) {
   const int Din = s->Din, Dout = s->Dout;
   unsigned first[2];
@@ -420,11 +429,13 @@ int FcStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t
   pqr_gemm_kernel<kGemmGram><<<tiles * (tiles + 1) / 2, kGemmThreads, 0, st>>>(y, Din, nullptr, 0, s->G.as<double>(), Din, Din, Din, N,
                                                                               acc);
   QCNN_CUDA(cudaGetLastError());
+  if (s->sums && LaunchColSum(s->ctx, y, N, Din, s->sy.as<double>(), acc, st)) return 1;
   if (s->target) {   // |T|^2 and P = T^T Y
     if (int rc = LaunchSqNorm(t, static_cast<size_t>(N) * Dout, s->scratch.as<double>(), s->tt.as<double>(), acc, st)) return rc;
     pqr_gemm_kernel<kGemmCross><<<dim3(tiles, CeilDiv(Dout, kTile)), kGemmThreads, 0, st>>>(t, Dout, y, Din, s->P.as<double>(), Din,
                                                                                          Dout, Din, N, acc);
     QCNN_CUDA(cudaGetLastError());
+    if (s->sums && LaunchColSum(s->ctx, t, N, Dout, s->su.as<double>(), acc, st)) return 1;
   }
   QCNN_CUDA(cudaEventRecord(s->done, st));
   s->images += N;
@@ -432,11 +443,17 @@ int FcStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t
 }
 
 int FcStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wei_h, float* ctrd_h,
-                  uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+                  uint8_t* asmt_h, float* bias_h, double* loss_h, cudaStream_t st) {
   if (int rc = CheckFcK(who, K)) return rc;
   std::vector<uint8_t> at;
   if (int rc = CheckFcHost(who, target, s->Din, s->Dout, K, s->d, wei_h, ctrd_h, asmt_h, at)) return rc;
-  return SweepFc(s, who, target, K, sweeps, wei_h, at, ctrd_h, asmt_h, loss_h, st);
+  if (!bias_h)
+    return SweepFc(s, who, target, K, sweeps, wei_h, s->G.as<double>(), s->P.as<double>(), s->tt.as<double>(), at, ctrd_h, asmt_h,
+                   nullptr, loss_h, st);
+  CenteredSums c;
+  if (int rc = CenterSums(s, who, target, 1, s->Din, s->Dout, &c, st)) return rc;
+  return SweepFc(s, who, target, K, sweeps, wei_h, c.G.as<double>(), c.P.as<double>(), c.tt.as<double>(), at, ctrd_h, asmt_h,
+                 bias_h, loss_h, st);
 }
 
 }  // namespace qcnn
@@ -454,7 +471,7 @@ extern "C" int qcnn_pq_refine_fc_target(qcnn_ctx* ctx, int Din, int Dout, int K,
 // ---- the statistics objects (both kinds; the conv creation and the conv halves are in pq_refine_conv.cu)
 
 extern "C" int qcnn_pq_stats_create_fc(qcnn_ctx* ctx, int Din, int Dout, int d, int target, qcnn_pq_stats** out) {
-  return CreateFc(ctx, "qcnn_pq_stats_create_fc", Din, Dout, d, target != 0, out);
+  return CreateFc(ctx, "qcnn_pq_stats_create_fc", Din, Dout, d, target != 0, true, out);
 }
 
 extern "C" int qcnn_pq_stats_add(qcnn_pq_stats* s, const float* y, const float* t, int N, void* stream) {
@@ -486,29 +503,55 @@ extern "C" int qcnn_pq_stats_read_h(const qcnn_pq_stats* s, double* G_h, double*
   return 0;
 }
 
+extern "C" int qcnn_pq_stats_read_sums_h(const qcnn_pq_stats* s, double* s_h, double* u_h, long long* n_h) {
+  const char* who = "qcnn_pq_stats_read_sums_h";
+  QCNN_CHECK(s, "%s: NULL argument", who);
+  QCNN_CHECK(s->target || !u_h, "%s: the targets' sum is kept only by statistics created with a target", who);
+  QCNN_ON_DEVICE(s->ctx->device);
+  QCNN_CUDA(cudaEventSynchronize(s->done));
+  if (s_h) QCNN_CUDA(cudaMemcpy(s_h, s->sy.get(), s->sy.bytes(), cudaMemcpyDeviceToHost));
+  if (u_h) QCNN_CUDA(cudaMemcpy(u_h, s->su.get(), s->su.bytes(), cudaMemcpyDeviceToHost));
+  if (n_h) *n_h = StatsRows(s);
+  return 0;
+}
+
 namespace {
 
-int RefineStats(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wei_h, float* ctrd_h,
-                uint8_t* asmt_h, double* loss_h, void* stream) {
-  QCNN_CHECK(s && (target || wei_h) && ctrd_h && asmt_h, "%s: NULL argument", who);
+// bias: the bias calls, which also need bias_h (finite, [Dout] / [Cout])
+int RefineStats(qcnn_pq_stats* s, const char* who, bool target, bool bias, int K, int sweeps, const float* wei_h, float* ctrd_h,
+                uint8_t* asmt_h, float* bias_h, double* loss_h, void* stream) {
+  QCNN_CHECK(s && (target || wei_h) && ctrd_h && asmt_h && (!bias || bias_h), "%s: NULL argument", who);
   QCNN_CHECK(!target || s->target, "%s: the statistics were created without a target", who);
   QCNN_CHECK(s->images > 0, "%s: no calibration data has been added", who);
   QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
+  if (bias) QCNN_CHECK(AllFinite(bias_h, s->conv ? s->geo.Cout : s->Dout), "%s: the bias contains a non-finite value", who);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return s->conv ? ConvStatsRefine(s, who, target, K, sweeps, wei_h, ctrd_h, asmt_h, loss_h, st)
-                 : FcStatsRefine(s, who, target, K, sweeps, wei_h, ctrd_h, asmt_h, loss_h, st);
+  if (!bias) bias_h = nullptr;
+  return s->conv ? ConvStatsRefine(s, who, target, K, sweeps, wei_h, ctrd_h, asmt_h, bias_h, loss_h, st)
+                 : FcStatsRefine(s, who, target, K, sweeps, wei_h, ctrd_h, asmt_h, bias_h, loss_h, st);
 }
 
 }  // namespace
 
 extern "C" int qcnn_pq_stats_refine(qcnn_pq_stats* s, int K, int sweeps, const float* wei_h, float* ctrd_h, uint8_t* asmt_h,
                                     double* loss_h, void* stream) {
-  return RefineStats(s, "qcnn_pq_stats_refine", false, K, sweeps, wei_h, ctrd_h, asmt_h, loss_h, stream);
+  return RefineStats(s, "qcnn_pq_stats_refine", false, false, K, sweeps, wei_h, ctrd_h, asmt_h, nullptr, loss_h, stream);
 }
 
 extern "C" int qcnn_pq_stats_refine_target(qcnn_pq_stats* s, int K, int sweeps, float* ctrd_h, uint8_t* asmt_h, double* loss_h,
                                            void* stream) {
-  return RefineStats(s, "qcnn_pq_stats_refine_target", true, K, sweeps, nullptr, ctrd_h, asmt_h, loss_h, stream);
+  return RefineStats(s, "qcnn_pq_stats_refine_target", true, false, K, sweeps, nullptr, ctrd_h, asmt_h, nullptr, loss_h, stream);
+}
+
+extern "C" int qcnn_pq_stats_refine_bias(qcnn_pq_stats* s, int K, int sweeps, const float* wei_h, float* ctrd_h, uint8_t* asmt_h,
+                                         float* bias_h, double* loss_h, void* stream) {
+  return RefineStats(s, "qcnn_pq_stats_refine_bias", false, true, K, sweeps, wei_h, ctrd_h, asmt_h, bias_h, loss_h, stream);
+}
+
+extern "C" int qcnn_pq_stats_refine_target_bias(qcnn_pq_stats* s, int K, int sweeps, float* ctrd_h, uint8_t* asmt_h,
+                                                float* bias_h, double* loss_h, void* stream) {
+  return RefineStats(s, "qcnn_pq_stats_refine_target_bias", true, true, K, sweeps, nullptr, ctrd_h, asmt_h, bias_h, loss_h,
+                     stream);
 }
 
 extern "C" void qcnn_pq_stats_destroy(qcnn_pq_stats* s) {

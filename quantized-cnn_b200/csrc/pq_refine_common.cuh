@@ -7,6 +7,7 @@
 #include <math.h>
 
 #include <algorithm>
+#include <vector>
 
 #include "qcnn_internal.h"
 
@@ -365,8 +366,10 @@ inline int ScanAdd(qcnn_pq_stats* s, const float* y, size_t ny, unsigned ycols, 
   return 0;
 }
 
-// The parts of a stats object both kinds share: the sums (zero until the first add), the scratch and the event
-inline int AllocStats(qcnn_pq_stats* s, const char* who, size_t gBytes, size_t pBytes) {
+// The parts of a stats object both kinds share: the sums (zero until the first add), the scratch and the event.
+// syBytes / suBytes / planeBytes: the first moments and the conv plane, allocated only when s->sums is set.
+inline int AllocStats(qcnn_pq_stats* s, const char* who, size_t gBytes, size_t pBytes, size_t syBytes, size_t suBytes,
+                      size_t planeBytes) {
   qcnn_ctx* ctx = s->ctx;
   auto reserve = [&](qcnn::DeviceBuffer& b, size_t bytes, const char* what) -> int {
     const cudaError_t e = b.Reserve(ctx, bytes);
@@ -375,8 +378,12 @@ inline int AllocStats(qcnn_pq_stats* s, const char* who, size_t gBytes, size_t p
     qcnn::SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
     return 1;
   };
+  if (!s->sums) syBytes = suBytes = planeBytes = 0;
+  if (!s->target) suBytes = 0;
   if (reserve(s->G, gBytes, "the Gram matrices") || reserve(s->P, s->target ? pBytes : 0, "the targets' cross product") ||
       reserve(s->tt, s->target ? sizeof(double) : 0, "the targets' norm") ||
+      reserve(s->sy, syBytes, "the inputs' sum") || reserve(s->su, suBytes, "the targets' sum") ||
+      reserve(s->plane, planeBytes, "the per-add image sum") ||
       reserve(s->scratch, sizeof(double) * kLossBlocks + 2 * sizeof(unsigned), "the scan flags"))
     return 1;
   QCNN_ON_DEVICE(ctx->device);
@@ -386,7 +393,125 @@ inline int AllocStats(qcnn_pq_stats* s, const char* who, size_t gBytes, size_t p
     QCNN_CUDA(cudaMemset(s->P.get(), 0, pBytes));
     QCNN_CUDA(cudaMemset(s->tt.get(), 0, sizeof(double)));
   }
+  if (syBytes) QCNN_CUDA(cudaMemset(s->sy.get(), 0, syBytes));
+  if (suBytes) QCNN_CUDA(cudaMemset(s->su.get(), 0, suBytes));
   QCNN_CUDA(cudaEventRecord(s->done, nullptr));
+  return 0;
+}
+
+// ---- first moments and the bias refit (DESIGN.md 4e, "Bias refit")
+
+// The rows n the first moments are summed over: images (FC) or images Ho Wo (conv)
+inline long long StatsRows(const qcnn_pq_stats* s) {
+  return s->conv ? s->images * s->geo.Ho * s->geo.Wo : s->images;
+}
+
+// out[c] = (accumulate ? out[c] + f : f), f = sum over r = 0..rows-1 ascending of x[r cols + c] in fp64: one fresh
+// fixed-order sum per column, folded with one addition
+template <typename In>
+__global__ void pqr_colsum_kernel(const In* __restrict__ x, size_t rows, size_t cols, double* __restrict__ out, int accumulate) {
+  for (size_t c = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; c < cols; c += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    double f = 0.0;
+    for (size_t r = 0; r < rows; r++) f += static_cast<double>(x[r * cols + c]);
+    out[c] = accumulate ? out[c] + f : f;
+  }
+}
+
+template <typename In>
+inline int LaunchColSum(qcnn_ctx* ctx, const In* x, size_t rows, size_t cols, double* out, int accumulate, cudaStream_t st) {
+  const int grid = static_cast<int>(std::min<size_t>((cols + 255) / 256, 32u * ctx->sm_count));
+  pqr_colsum_kernel<In><<<grid, 256, 0, st>>>(x, rows, cols, out, accumulate);
+  QCNN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// out[r][c] = X[r][c] - (a[r] b[r / rpg][c]) / n, each operation rounded (no contraction): the centered G (a = s,
+// b = s per group) and P (a = u, b = s of the output's group)
+__global__ void pqr_center_kernel(const double* __restrict__ X, const double* __restrict__ a, const double* __restrict__ b,
+                                  size_t rows, size_t cols, size_t rpg, double n, double* __restrict__ out) {
+  const size_t total = rows * cols;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t r = i / cols, c = i % cols;
+    out[i] = __dsub_rn(X[i], __ddiv_rn(__dmul_rn(a[r], b[(r / rpg) * cols + c]), n));
+  }
+}
+
+// *ttc = *tt - sum over o ascending of (u[o] u[o]) / n, each operation rounded
+__global__ void pqr_center_tt_kernel(const double* __restrict__ tt, const double* __restrict__ u, int Dout, double n,
+                                     double* __restrict__ ttc) {
+  double acc = 0.0;
+  for (int o = 0; o < Dout; o++) acc = __dadd_rn(acc, __ddiv_rn(__dmul_rn(u[o], u[o]), n));
+  *ttc = __dsub_rn(*tt, acc);
+}
+
+// delta[o] = (u[o] + E_o . s_g) / n, g = o / Cpg, u = 0 without a target (E = W - W^, or -W^ for the target form): a
+// warp per output, lanes over every 32nd dim, a fixed shuffle tree
+__global__ void pqr_bias_delta_kernel(const double* __restrict__ E, const double* __restrict__ sy, const double* __restrict__ u,
+                                      int Dout, int D, int Cpg, double n, double* __restrict__ delta) {
+  const int lane = threadIdx.x & 31;
+  const int o = static_cast<int>((blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x) >> 5);
+  if (o >= Dout) return;
+  const double* e = E + static_cast<size_t>(o) * D;
+  const double* sg = sy + static_cast<size_t>(o / Cpg) * D;
+  double v = 0.0;
+  for (int q = lane; q < D; q += 32) v += e[q] * sg[q];
+  for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+  if (lane == 0) delta[o] = __ddiv_rn(u ? __dadd_rn(u[o], v) : v, n);
+}
+
+// The centered copies of a stats object's sums, for grp groups of D dims and Dout outputs (Dout / grp per group):
+// G [grp][D][D] always, P [Dout][D] and |T_c|^2 for the target form
+struct CenteredSums {
+  qcnn::DeviceBuffer G, P, tt;
+};
+
+inline int CenterSums(qcnn_pq_stats* s, const char* who, bool target, int grp, int D, int Dout, CenteredSums* c, cudaStream_t st) {
+  qcnn_ctx* ctx = s->ctx;
+  const size_t gn = static_cast<size_t>(grp) * D * D, pn = static_cast<size_t>(Dout) * D;
+  auto reserve = [&](qcnn::DeviceBuffer& b, size_t bytes, const char* what) -> int {
+    const cudaError_t e = b.Reserve(ctx, bytes);
+    if (e == cudaSuccess) return 0;
+    cudaGetLastError();
+    qcnn::SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
+    return 1;
+  };
+  if (reserve(c->G, sizeof(double) * gn, "the centered Gram matrices") ||
+      reserve(c->P, target ? sizeof(double) * pn : 0, "the centered cross product") ||
+      reserve(c->tt, target ? sizeof(double) : 0, "the centered targets' norm"))
+    return 1;
+  QCNN_ON_DEVICE(ctx->device);
+  QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
+  const double n = static_cast<double>(StatsRows(s));
+  const double* sy = s->sy.as<double>();
+  auto grid = [&](size_t total) { return static_cast<int>(std::min<size_t>((total + 255) / 256, 32u * ctx->sm_count)); };
+  pqr_center_kernel<<<grid(gn), 256, 0, st>>>(s->G.as<double>(), sy, sy, static_cast<size_t>(grp) * D, D, D, n, c->G.as<double>());
+  if (target) {
+    const double* su = s->su.as<double>();
+    pqr_center_kernel<<<grid(pn), 256, 0, st>>>(s->P.as<double>(), su, sy, Dout, D, Dout / grp, n, c->P.as<double>());
+    pqr_center_tt_kernel<<<1, 1, 0, st>>>(s->tt.as<double>(), su, Dout, n, c->tt.as<double>());
+  }
+  QCNN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// bias_h[o] = fp32(bias_h[o] + delta_o) from the final residual E [Dout][D] on the device (pqr_bias_delta_kernel)
+inline int RefitBias(qcnn_pq_stats* s, const char* who, bool target, const double* E, int grp, int D, int Dout, float* bias_h,
+                     cudaStream_t st) {
+  qcnn::DeviceBuffer dDelta;
+  const cudaError_t e = dDelta.Reserve(s->ctx, sizeof(double) * Dout);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    qcnn::SetError("%s: cannot allocate %zu bytes of device memory for the bias change (%s)", who, sizeof(double) * Dout,
+                   cudaGetErrorString(e));
+    return 1;
+  }
+  pqr_bias_delta_kernel<<<qcnn::CeilDiv(Dout, 8), 256, 0, st>>>(E, s->sy.as<double>(), target ? s->su.as<double>() : nullptr, Dout, D,
+                                                          Dout / grp, static_cast<double>(StatsRows(s)), dDelta.as<double>());
+  QCNN_CUDA(cudaGetLastError());
+  std::vector<double> delta(Dout);
+  QCNN_CUDA(cudaMemcpyAsync(delta.data(), dDelta.get(), sizeof(double) * Dout, cudaMemcpyDeviceToHost, st));
+  QCNN_CUDA(cudaStreamSynchronize(st));
+  for (int o = 0; o < Dout; o++) bias_h[o] = static_cast<float>(static_cast<double>(bias_h[o]) + delta[o]);
   return 0;
 }
 

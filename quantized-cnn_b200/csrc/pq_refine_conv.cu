@@ -4,13 +4,13 @@
 //   Cg = Cin / grp, T = k^2 taps, S = ceil(Cg / d); subspace m covers the per-group channels [m d, m d + w_m).
 //   Per group g, G_g = sum p p^T (fp64, fixed order) over the zero-padded Cg T patches p of the group's channels.
 //   E = W - W^ (fp64), loss = sum_g sum_{o in g} E_o^T G_g E_o; one codebook per subspace serves every tap and group.
-//   A sweep visits m = 0..S-1 in order; m is skipped when sum_g sum_t tr G^m_{g,tt} = 0.
+//   A sweep visits m = 0..S-1 in order; m is skipped when !(sum_g sum_t tr G^m_{g,tt} > 0).
 //   h_{o,t} = [G_g R_o]_{(m,t)}, R_o = E_o with m's taps replaced by the weights (the other subspaces' residual).
 //   codebook   over U = {k : n_k > 0}, M = sum_g sum_{t,t'} Cnt^g_{tt'} (x) G^m_{g,tt'} (ascending g, t, t'),
 //              b_k = sum of h_{o,t} assigned to k (o, then t ascending), D = fp32((M + mu I)^-1 b) by blocked Cholesky,
 //              mu = 1e-10 tr(M) / (|U| w_m); D replaces C[m][U] only if (D - C)^T (M (D + C) - 2 b) < 0.
 //   assign     per output, taps t = 0..T-1 in order: a = argmin_k c_k^T G_tt c_k - 2 c_k^T h'_{o,t} (fp64, lowest index
-//              on ties), h' with E current (earlier taps' new assignments included); a (g, t) with tr G_tt = 0 keeps.
+//              on ties), h' with E current (earlier taps' new assignments included); a (g, t) with !(tr G_tt > 0) keeps.
 // Target form (qcnn_pq_refine_conv_target): inputs y, targets t [N][Ho][Wo][Cout], per group
 //   P_g[o][q] = sum over positions of t[pos][o] p_g(pos)[q] (the same patch chunks, ascending), and R = P - G W^ in place
 //   of G E everywhere above; loss = |T|^2 + sum_o (-2 w^_o^T P_o + w^_o^T G_g w^_o).  It runs on the same kernels:
@@ -55,6 +55,30 @@ __global__ void pqrc_residual_kernel(const float* __restrict__ W, const float* _
     const uint8_t a = A[(static_cast<size_t>(q.m) * Cout + o) * T + q.t];
     E[i] = static_cast<double>(W[i]) - static_cast<double>(C[(static_cast<size_t>(q.m) * K + a) * d + q.j]);
   }
+}
+
+// s[g][q] (accumulate: s[g][q] +) the sum over output positions (oy, then ox ascending) of the image sum `plane`
+// [Hin][Win][Cin] at the input pixel tap t of dim q reads, for every (g, q) (thread g Dg + q); a tap outside the map
+// adds nothing (the zero padding)
+__global__ void pqrc_tapsum_kernel(const double* __restrict__ plane, int Hin, int Win, int Cin, int ksz, int pad, int stride,
+                                   int Ho, int Wo, int Cg, int d, int grp, double* __restrict__ s, int accumulate) {
+  const int T = ksz * ksz, Dg = Cg * T;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= grp * Dg) return;
+  const int g = i / Dg;
+  const Dim q = DecodeDim(i - g * Dg, Cg, d, T);
+  const int ky = q.t / ksz, kx = q.t % ksz;
+  const double* p = plane + g * Cg + q.m * d + q.j;
+  double f = 0.0;
+  for (int oy = 0; oy < Ho; oy++) {
+    const int iy = oy * stride - pad + ky;
+    if (iy < 0 || iy >= Hin) continue;
+    for (int ox = 0; ox < Wo; ox++) {
+      const int ix = ox * stride - pad + kx;
+      if (ix >= 0 && ix < Win) f += p[(static_cast<size_t>(iy) * Win + ix) * Cin];
+    }
+  }
+  s[i] = accumulate ? s[i] + f : f;
 }
 
 // Subspace m, nb = T w dims from q0: Wh[o][r] = the decoded weight w^ (fp64), H[o][r] = GE[o][q0 + r] (the responses'
@@ -356,7 +380,7 @@ __global__ void __launch_bounds__(kAssignWarps * 32) pqrc_assign_kernel(const do
     const double* Grow = Gg + static_cast<size_t>(q0 + t * w) * Dg + q0;   // rows (m, t, j), columns from the block's start
     double tr = 0.0;
     for (int j = 0; j < w; j++) tr += Grow[static_cast<size_t>(j) * Dg + t * w + j];
-    if (tr == 0.0) continue;
+    if (!(tr > 0.0)) continue;
     for (int j = lane; j < w; j += 32) {
       double s = 0.0;
 #pragma unroll 1
@@ -433,9 +457,11 @@ int CheckConvSystem(const char* who, int K, int d, int Cg) {
   return 0;
 }
 
-// The sweeps on the statistics of s.  target: the target form (wp is empty); else the same-input form on the weights wp.
-int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const std::vector<float>& wp,
-              std::vector<uint8_t>& at, float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+// The sweeps on the sums G, P and |T|^2 (those of s, or their centered copies).  target: the target form (wp is empty);
+// else the same-input form on the weights wp.  bias_h non-NULL: replaced by the refit bias (RefitBias).
+int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const std::vector<float>& wp, const double* G,
+              const double* P, const double* TT, std::vector<uint8_t>& at, float* ctrd_h, uint8_t* asmt_h, float* bias_h,
+              double* loss_h, cudaStream_t st) {
   qcnn_ctx* ctx = s->ctx;
   const PqConvGeometry& geo = s->geo;
   const int d = s->d, Cout = geo.Cout, Cg = geo.Cg, Cpg = geo.Cpg, T = geo.T, Dg = geo.Dg, grp = geo.grp;
@@ -466,7 +492,7 @@ int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps,
       reserve(dCC, sizeof(double) * grp * static_cast<size_t>(T) * K, "the codeword norms") ||
       reserve(dPart, sizeof(double) * kLossBlocks, "the loss") || reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss"))
     return 1;
-  const double* G = s->G.as<double>();
+  if (!target) P = TT = nullptr;   // P = T^T Y
   QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
   if (target) QCNN_CUDA(cudaMemsetAsync(dW.get(), 0, sizeof(float) * nw, st));   // E = 0 - W^
   else QCNN_CUDA(cudaMemcpyAsync(dW.get(), wp.data(), sizeof(float) * nw, cudaMemcpyHostToDevice, st));
@@ -483,14 +509,12 @@ int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps,
     double tr = 0.0;
     for (int g = 0; g < grp; g++)
       for (int r = 0; r < T * w; r++) tr += diag[static_cast<size_t>(g) * Dg + m * d * T + r];
-    skip[m] = tr == 0.0;
+    skip[m] = !(tr > 0.0);
   }
   const int tiles = CeilDiv(Dg, kTile);
   const int ewBlocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 32u * ctx->sm_count));
   pqrc_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Cout, Cg, K, d, T);
   // GE = E G, or P + E G for a target
-  const double* P = target ? s->P.as<double>() : nullptr;   // T^T Y
-  const double* TT = target ? s->tt.as<double>() : nullptr;
   if (target) QCNN_CUDA(cudaMemcpyAsync(dGE.get(), P, sizeof(double) * nw, cudaMemcpyDeviceToDevice, st));
   for (int g = 0; g < grp; g++) {
     const size_t ro = static_cast<size_t>(g) * Cpg * Dg;
@@ -559,6 +583,10 @@ int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps,
     }
     if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st, P, TT)) return rc;
   }
+  if (bias_h) {   // E = W - W^ (target: -W^) afresh from the final codebook and assignments
+    pqrc_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Cout, Cg, K, d, T);
+    if (int rc = RefitBias(s, who, target, dE.as<double>(), grp, Dg, Cout, bias_h, st)) return rc;
+  }
   std::vector<double> lossv(sweeps + 1);
   QCNN_CUDA(cudaMemcpyAsync(ctrd_h, dC.get(), sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
   QCNN_CUDA(cudaMemcpyAsync(at.data(), dA.get(), at.size(), cudaMemcpyDeviceToHost, st));
@@ -585,22 +613,25 @@ int CheckGeometry(const char* who, int Cin, int Hin, int Win, int Cout, int ksz,
   return 0;
 }
 
-int CreateConv(qcnn_ctx* ctx, const char* who, const PqConvGeometry& geo, int d, bool target, qcnn_pq_stats** out) {
+int CreateConv(qcnn_ctx* ctx, const char* who, const PqConvGeometry& geo, int d, bool target, bool sums, qcnn_pq_stats** out) {
   std::unique_ptr<qcnn_pq_stats> s(new qcnn_pq_stats);
   s->ctx = ctx;
   s->conv = true;
   s->target = target;
   s->d = d;
   s->geo = geo;
+  s->sums = sums;
+  const size_t inPlane = static_cast<size_t>(geo.Hin) * geo.Win * geo.Cin, outPlane = static_cast<size_t>(geo.Ho) * geo.Wo * geo.Cout;
   if (AllocStats(s.get(), who, sizeof(double) * geo.grp * static_cast<size_t>(geo.Dg) * geo.Dg,
-                 sizeof(double) * geo.Cout * static_cast<size_t>(geo.Dg)))
+                 sizeof(double) * geo.Cout * static_cast<size_t>(geo.Dg), sizeof(double) * geo.grp * static_cast<size_t>(geo.Dg),
+                 sizeof(double) * geo.Cout, sizeof(double) * (target ? std::max(inPlane, outPlane) : inPlane)))
     return 1;
   *out = s.release();
   return 0;
 }
 
-// The one-shot calls: the checks both forms share (in the order of their messages), then create, one add of all N
-// inputs, the sweeps and destroy
+// The one-shot calls: the checks both forms share (in the order of their messages), then create (without the first
+// moments, which they never read), one add of all N inputs, the sweeps and destroy
 int RefineConv(bool target, qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, int K,
                int d, int sweeps, const float* knl_h, const float* x, const float* t, int N, float* ctrd_h, uint8_t* asmt_h,
                double* loss_h, void* stream) {
@@ -620,10 +651,11 @@ int RefineConv(bool target, qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, 
   if (int rc = CheckConvHost(who, target, geo, K, d, knl_h, ctrd_h, asmt_h, at, wp)) return rc;
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
   qcnn_pq_stats* sp = nullptr;
-  if (int rc = CreateConv(ctx, who, geo, d, target, &sp)) return rc;
+  if (int rc = CreateConv(ctx, who, geo, d, target, false, &sp)) return rc;
   std::unique_ptr<qcnn_pq_stats> s(sp);
   if (int rc = ConvStatsAdd(s.get(), who, x, t, N, st)) return rc;
-  return SweepConv(s.get(), who, target, K, sweeps, wp, at, ctrd_h, asmt_h, loss_h, st);
+  return SweepConv(s.get(), who, target, K, sweeps, wp, s->G.as<double>(), s->P.as<double>(), s->tt.as<double>(), at, ctrd_h,
+                   asmt_h, nullptr, loss_h, st);
 }
 
 }  // namespace
@@ -631,7 +663,7 @@ int RefineConv(bool target, qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, 
 namespace qcnn {
 
 // A conv add: the scan, then per group the positions in runs of F, each run's Gram (and cross product) read straight
-// from the maps and added in ascending order
+// from the maps and added in ascending order; then the first moments (s from the image sum of y, u from that of t)
 int ConvStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st) {
   const PqConvGeometry& geo = s->geo;
   const int Cout = geo.Cout, Cpg = geo.Cpg, Dg = geo.Dg, grp = geo.grp;
@@ -661,18 +693,36 @@ int ConvStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float*
       QCNN_CUDA(cudaGetLastError());
     }
   }
+  if (s->sums) {
+    double* plane = s->plane.as<double>();
+    const size_t inPlane = static_cast<size_t>(geo.Hin) * geo.Win * geo.Cin, hw = static_cast<size_t>(geo.Ho) * geo.Wo;
+    if (LaunchColSum(s->ctx, y, N, inPlane, plane, 0, st)) return 1;
+    pqrc_tapsum_kernel<<<CeilDiv(grp * Dg, 128), 128, 0, st>>>(plane, geo.Hin, geo.Win, geo.Cin, geo.ksz, geo.pad, geo.stride, geo.Ho,
+                                                               geo.Wo, geo.Cg, s->d, grp, s->sy.as<double>(), acc0);
+    QCNN_CUDA(cudaGetLastError());
+    if (s->target) {
+      if (LaunchColSum(s->ctx, t, N, hw * Cout, plane, 0, st)) return 1;
+      if (LaunchColSum(s->ctx, static_cast<const double*>(plane), hw, Cout, s->su.as<double>(), acc0, st)) return 1;
+    }
+  }
   QCNN_CUDA(cudaEventRecord(s->done, st));
   s->images += N;
   return 0;
 }
 
 int ConvStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* knl_h, float* ctrd_h,
-                    uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
+                    uint8_t* asmt_h, float* bias_h, double* loss_h, cudaStream_t st) {
   if (int rc = CheckConvSystem(who, K, s->d, s->geo.Cg)) return rc;
   std::vector<uint8_t> at;
   std::vector<float> wp;
   if (int rc = CheckConvHost(who, target, s->geo, K, s->d, knl_h, ctrd_h, asmt_h, at, wp)) return rc;
-  return SweepConv(s, who, target, K, sweeps, wp, at, ctrd_h, asmt_h, loss_h, st);
+  if (!bias_h)
+    return SweepConv(s, who, target, K, sweeps, wp, s->G.as<double>(), s->P.as<double>(), s->tt.as<double>(), at, ctrd_h, asmt_h,
+                     nullptr, loss_h, st);
+  CenteredSums c;
+  if (int rc = CenterSums(s, who, target, s->geo.grp, s->geo.Dg, s->geo.Cout, &c, st)) return rc;
+  return SweepConv(s, who, target, K, sweeps, wp, c.G.as<double>(), c.P.as<double>(), c.tt.as<double>(), at, ctrd_h, asmt_h,
+                   bias_h, loss_h, st);
 }
 
 }  // namespace qcnn
@@ -699,5 +749,5 @@ extern "C" int qcnn_pq_stats_create_conv(qcnn_ctx* ctx, int Cin, int Hin, int Wi
   PqConvGeometry geo;
   if (int rc = CheckGeometry(who, Cin, Hin, Win, Cout, ksz, pad, stride, grp, &geo)) return rc;
   QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
-  return CreateConv(ctx, who, geo, d, target != 0, out);
+  return CreateConv(ctx, who, geo, d, target != 0, true, out);
 }

@@ -479,10 +479,11 @@ int CheckConvK(const char* who, int K);
 struct PqConvGeometry { int Cin, Hin, Win, Cout, ksz, pad, stride, grp, Ho, Wo, Cg, Cpg, T, Dg; };
 int FcStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st);
 int ConvStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st);
+// bias_h non-NULL: the sweeps run on the centered sums and bias_h [Dout] / [Cout] is replaced by the refit bias
 int FcStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wei_h, float* ctrd_h,
-                  uint8_t* asmt_h, double* loss_h, cudaStream_t st);
+                  uint8_t* asmt_h, float* bias_h, double* loss_h, cudaStream_t st);
 int ConvStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* knl_h, float* ctrd_h,
-                    uint8_t* asmt_h, double* loss_h, cudaStream_t st);
+                    uint8_t* asmt_h, float* bias_h, double* loss_h, cudaStream_t st);
 
 // conv_ws.cu: the tensor-core family's weight-stationary tilings of stride-1 layers (mode-0 geometry, channel tiles) and
 // of strided narrow-input layers (mode-1 geometry)
@@ -538,6 +539,10 @@ struct qcnn_pq_stats {
   qcnn::PqConvGeometry geo{};     // conv
   long long images = 0;
   qcnn::DeviceBuffer G, P, tt;    // G [grp][Dg][Dg] (FC [Din][Din]); target: P [Cout][Dg] (FC [Dout][Din]) and |T|^2
+  // first moments (with sums): sy = sum of y [grp][Dg] in the dim order of G (FC [Din]); target: su = sum of t [Cout]
+  // (FC [Dout]); conv: plane, an add's fresh sum over its images of y [Hin][Win][Cin] or of t [Ho][Wo][Cout]
+  bool sums = true;               // false only inside the one-shot refine calls, which never read the first moments
+  qcnn::DeviceBuffer sy, su, plane;
   qcnn::DeviceBuffer scratch;     // the |T_b|^2 partials [kLossBlocks] fp64, then the add's two scan flags
   cudaEvent_t done = nullptr;
   ~qcnn_pq_stats() {

@@ -20,8 +20,12 @@ With --stats the calibration images stream through in batches of --batch: per la
 refinement runs on the accumulated statistics (qcnn_pq_stats_refine / _refine_target), so no layer's inputs or targets
 are ever held whole and device memory does not grow with --train.  Each call time is then the accumulation plus the
 refinement, printed with the peak device memory of that layer and mode (torch's peak allocation plus the statistics).
+With --stats --bias two more modes run, same-input+bias and target+bias: the same refinements with the bias refit as
+well (qcnn_pq_stats_refine_bias / _refine_target_bias on the centered statistics).  Each saves its refit bias into its
+own model, so the next layer's inputs come from the corrected network; their training loss ratios are of the
+bias-optimal losses.
     python tools/pq_refine_chain.py [--train 4096] [--held 1024] [--sweeps 4] [--conv 32 8] [--fc8 16 4] [--stats]
-                                    [--out f.json]"""
+                                    [--bias] [--out f.json]"""
 import argparse
 import importlib
 import json
@@ -40,6 +44,7 @@ from pq_refine_time import card   # noqa: E402
 
 NAMES = {0: "conv1", 4: "conv2", 8: "conv3", 10: "conv4", 12: "conv5", 15: "fc6", 18: "fc7", 21: "fc8"}
 MODES = ("kmeans", "same-input", "target")
+BIAS_MODES = ("same-input+bias", "target+bias")
 
 
 def decode(ctrd, asmt, cin):
@@ -120,9 +125,10 @@ class LcgImages(object):
         return out
 
 
-def refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc, target):
+def refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc, target, bias=None):
     """Accumulate layer l's statistics over the calibration images batch by batch (inputs from `net`, targets from the
-    original network), then refine on them: (ctrd, asmt, loss, seconds in the adds and the refine, peak device bytes)"""
+    original network), then refine on them: (ctrd, asmt, bias, loss, seconds in the adds and the refine, peak device
+    bytes).  bias: the layer's bias, refit with the codebook and assignments (else returned as None)."""
     import torch
     conv = W.ndim == 4
     d = c0.shape[2]
@@ -148,14 +154,19 @@ def refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc, targ
         secs += time.perf_counter() - t0
         del imgs, y, t
     t0 = time.perf_counter()
-    if target:
+    b = None
+    if bias is not None and target:
+        c, a, b, loss = st.refine_target_bias(c0, a0, bias, sweeps=args.sweeps)
+    elif bias is not None:
+        c, a, b, loss = st.refine_bias(W, c0, a0, bias, sweeps=args.sweeps)
+    elif target:
         c, a, loss = st.refine_target(c0, a0, sweeps=args.sweeps)
     else:
         c, a, loss = st.refine(W, c0, a0, sweeps=args.sweeps)
     secs += time.perf_counter() - t0
     peak = torch.cuda.max_memory_allocated() + st.nbytes
     st.close()
-    return c, a, loss, secs, peak
+    return c, a, b, loss, secs, peak
 
 
 def main():
@@ -171,7 +182,11 @@ def main():
     ap.add_argument("--seed", type=int, default=1000000, help="image seed: calibration, then held-out")
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
     ap.add_argument("--stats", action="store_true", help="stream the calibration images through PqStats objects")
+    ap.add_argument("--bias", action="store_true", help="with --stats: also the modes that refit each layer's bias")
     args = ap.parse_args()
+    if args.bias and not args.stats:
+        ap.error("--bias needs --stats (the bias refit runs on calibration statistics)")
+    modes = MODES + (BIAS_MODES if args.bias else ())
     import torch
     from oracle import pyoracle as po
     assert torch.cuda.is_available(), "needs a GPU"
@@ -194,7 +209,7 @@ def main():
     print("card: %s (name, power limit, max SM clock)" % hw)
     orig = q.Net(ctx, po.ALEXNET_DIR, po.ALEXNET_PFX, "AlexNet")
     ref = logits(orig, held, args.batch).double()
-    qparams = {m: dict(params) for m in MODES}
+    qparams = {m: dict(params) for m in modes}
     rows = []
     with tempfile.TemporaryDirectory() as tmp:
         def net_of(mode):
@@ -208,12 +223,13 @@ def main():
             quant = q.pq_quantize_conv if conv else q.pq_quantize_fc
             c0, a0, _ = quant(ctx, W, K, d, iters=20, seed=1)
             t = None if args.stats else response(L, layer_inputs(orig, l, train, args.batch, first_fc), W, args.batch)
-            for mode in MODES:
-                c, a, ratio, secs, peak = c0, a0, None, None, None
+            for mode in modes:
+                c, a, b, ratio, secs, peak = c0, a0, None, None, None, None
                 if mode != "kmeans" and args.stats:
                     net = net_of(mode)
-                    c, a, loss, secs, peak = refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc,
-                                                             mode == "target")
+                    c, a, b, loss, secs, peak = refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc,
+                                                                mode.startswith("target"),
+                                                                params[l]["bias"] if mode in BIAS_MODES else None)
                     net.close()
                     ratio = float(loss[-1] / loss[0])
                 elif mode != "kmeans":
@@ -233,17 +249,17 @@ def main():
                     secs = time.perf_counter() - t0
                     ratio = float(loss[-1] / loss[0])
                     del y
-                qparams[mode][l] = dict(bias=params[l]["bias"], ctrd=c, asmt=a, bits=po.bits_for(K))
+                qparams[mode][l] = dict(bias=params[l]["bias"] if b is None else b, ctrd=c, asmt=a, bits=po.bits_for(K))
                 rows.append(dict(layer=NAMES[l], K=K, d=d, mode=mode, loss_ratio=ratio, call_s=secs, peak_bytes=peak))
                 if ratio is not None:
-                    print("%-6s K=%-3d d=%-2d %-10s training loss x%.4f  call %.2f s%s"
+                    print("%-6s K=%-3d d=%-2d %-15s training loss x%.4f  call %.2f s%s"
                           % (NAMES[l], K, d, mode, ratio, secs, "" if peak is None else "  peak %.2f GB" % (peak / 1e9)))
             del t
             torch.cuda.empty_cache()
         orig.close()
         top1 = ref.argmax(1)
         summary = []
-        for mode in MODES:
+        for mode in modes:
             net = net_of(mode)
             lg = logits(net, held, args.batch).double()
             net.close()
@@ -253,7 +269,7 @@ def main():
             agree5 = (lg.topk(5, 1).indices == top1[:, None]).any(1).double().mean().item()
             summary.append(dict(mode=mode, logit_rel_err=err, logit_rel_err_median=med, top1_agree=agree1,
                                 top5_agree=agree5))
-            print("%-10s held-out logits relative error %.4f (per image, median %.4f)  top-1 agreement %.4f  "
+            print("%-15s held-out logits relative error %.4f (per image, median %.4f)  top-1 agreement %.4f  "
                   "top-5 agreement %.4f" % (mode, err, med, agree1, agree5))
     if args.out:
         with open(args.out, "w") as f:
