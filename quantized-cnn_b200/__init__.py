@@ -672,25 +672,33 @@ def pq_quantize_model(ctx, model, dir, pfx, out_dir, out_pfx, pq, iters=20, seed
                                       seed & 0xFFFFFFFF, out_dir.encode(), out_pfx.encode()))
 
 
+def _refine_start(ctrd, asmt):
+    """Fresh C-ordered copies of a refine call's start (ctrd float32, asmt uint8), which the call overwrites."""
+    return np.array(ctrd, np.float32, order="C", copy=True), np.array(asmt, np.uint8, order="C", copy=True)
+
+
+def _refine_call(fn, args, ctrd, asmt, sweeps, stream):
+    """fn(*args, ctrd, asmt, loss, stream) with loss [sweeps + 1]: (ctrd, asmt, loss)."""
+    loss = np.empty(max(sweeps, 0) + 1, np.float64)
+    _check(fn(*args, ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp), _stream(stream)))
+    return ctrd, asmt, loss
+
+
 def pq_refine_fc(ctx, wei, x, ctrd, asmt, sweeps=8, stream=None):
     """Error-correcting PQ of FC weights wei [Dout, Din] on layer inputs x (contiguous float32 CUDA tensor [N, Din],
     fcntWei column order), starting from (ctrd [S, K, d], asmt [Dout, S] 0-based), e.g. pq_quantize_fc's output:
     (ctrd, asmt, loss [sweeps + 1]) with loss[t] = sum_n |(W - W^) x_n|^2 after sweep t.  The arguments are not modified."""
     wei = _np(wei, np.float32)
     Dout, Din = wei.shape
-    ctrd = np.array(ctrd, np.float32, order="C", copy=True)
-    asmt = np.array(asmt, np.uint8, order="C", copy=True)
+    ctrd, asmt = _refine_start(ctrd, asmt)
     S, K, d = ctrd.shape
     if S != -(-Din // d) or asmt.shape != (Dout, S):
         raise QcnnError("ctrd [%d, K, d] and asmt [%d, %d] do not match a [%d, %d] layer with d=%d"
                         % (S, Dout, S, Dout, Din, d))
     if x.dim() != 2 or x.shape[1] != Din:
         raise QcnnError("x must be [N, %d], got %s" % (Din, tuple(x.shape)))
-    loss = np.empty(max(sweeps, 0) + 1, np.float64)
-    _check(lib.qcnn_pq_refine_fc(ctx.h, Din, Dout, K, d, sweeps, wei.ctypes.data_as(_vp), _dptr(x), x.shape[0],
-                                 ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp),
-                                 _stream(stream)))
-    return ctrd, asmt, loss
+    return _refine_call(lib.qcnn_pq_refine_fc, (ctx.h, Din, Dout, K, d, sweeps, wei.ctypes.data_as(_vp), _dptr(x), x.shape[0]),
+                        ctrd, asmt, sweeps, stream)
 
 
 def pq_refine_conv(ctx, knl, x, ctrd, asmt, pad=0, stride=1, grp=1, sweeps=8, stream=None):
@@ -700,8 +708,7 @@ def pq_refine_conv(ctx, knl, x, ctrd, asmt, pad=0, stride=1, grp=1, sweeps=8, st
     The arguments are not modified."""
     knl = _np(knl, np.float32)
     Cout, Cg, k, k2 = knl.shape
-    ctrd = np.array(ctrd, np.float32, order="C", copy=True)
-    asmt = np.array(asmt, np.uint8, order="C", copy=True)
+    ctrd, asmt = _refine_start(ctrd, asmt)
     S, K, d = ctrd.shape
     if k != k2 or S != -(-Cg // d) or asmt.shape != (Cout, k, k, S):
         raise QcnnError("ctrd [%d, K, d] and asmt %s do not match a %s kernel with d=%d"
@@ -709,11 +716,8 @@ def pq_refine_conv(ctx, knl, x, ctrd, asmt, pad=0, stride=1, grp=1, sweeps=8, st
     if x.dim() != 4 or x.shape[3] != Cg * grp:
         raise QcnnError("x must be [N, Hin, Win, %d], got %s" % (Cg * grp, tuple(x.shape)))
     N, Hin, Win, Cin = x.shape
-    loss = np.empty(max(sweeps, 0) + 1, np.float64)
-    _check(lib.qcnn_pq_refine_conv(ctx.h, Cin, Hin, Win, Cout, k, pad, stride, grp, K, d, sweeps,
-                                   knl.ctypes.data_as(_vp), _dptr(x), N, ctrd.ctypes.data_as(_vp),
-                                   asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp), _stream(stream)))
-    return ctrd, asmt, loss
+    return _refine_call(lib.qcnn_pq_refine_conv, (ctx.h, Cin, Hin, Win, Cout, k, pad, stride, grp, K, d, sweeps,
+                                                  knl.ctypes.data_as(_vp), _dptr(x), N), ctrd, asmt, sweeps, stream)
 
 
 def pq_refine_fc_target(ctx, y, t, ctrd, asmt, sweeps=8, stream=None):
@@ -721,8 +725,7 @@ def pq_refine_fc_target(ctx, y, t, ctrd, asmt, sweeps=8, stream=None):
     network and t [N, Dout] the original layer's responses without bias and before ReLU (both contiguous float32 CUDA
     tensors, y in fcntWei column order), starting from (ctrd [S, K, d], asmt [Dout, S] 0-based): (ctrd, asmt,
     loss [sweeps + 1]) with loss[s] = sum_n |t_n - W^ y_n|^2 after sweep s.  The arguments are not modified."""
-    ctrd = np.array(ctrd, np.float32, order="C", copy=True)
-    asmt = np.array(asmt, np.uint8, order="C", copy=True)
+    ctrd, asmt = _refine_start(ctrd, asmt)
     S, K, d = ctrd.shape
     if y.dim() != 2 or t.dim() != 2 or t.shape[0] != y.shape[0]:
         raise QcnnError("y must be [N, Din] and t [N, Dout] with the same N, got %s and %s"
@@ -732,11 +735,8 @@ def pq_refine_fc_target(ctx, y, t, ctrd, asmt, sweeps=8, stream=None):
     if S != -(-Din // d) or asmt.shape != (Dout, S):
         raise QcnnError("ctrd [%d, K, d] and asmt %s do not match a [%d, %d] layer with d=%d"
                         % (S, tuple(asmt.shape), Dout, Din, d))
-    loss = np.empty(max(sweeps, 0) + 1, np.float64)
-    _check(lib.qcnn_pq_refine_fc_target(ctx.h, Din, Dout, K, d, sweeps, _dptr(y), _dptr(t), N,
-                                        ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp),
-                                        _stream(stream)))
-    return ctrd, asmt, loss
+    return _refine_call(lib.qcnn_pq_refine_fc_target, (ctx.h, Din, Dout, K, d, sweeps, _dptr(y), _dptr(t), N), ctrd, asmt,
+                        sweeps, stream)
 
 
 def pq_refine_conv_target(ctx, y, t, ctrd, asmt, ksz, pad=0, stride=1, grp=1, sweeps=8, stream=None):
@@ -744,8 +744,7 @@ def pq_refine_conv_target(ctx, y, t, ctrd, asmt, ksz, pad=0, stride=1, grp=1, sw
     quantized network and t [N, Ho, Wo, Cout] the original layer's responses without bias and before ReLU (both NHWC,
     contiguous float32 CUDA tensors), starting from (ctrd [S, K, d], asmt [Cout, ksz, ksz, S] 0-based): (ctrd, asmt,
     loss [sweeps + 1]) with loss[s] = sum (t - conv(y, W^))^2 after sweep s.  The arguments are not modified."""
-    ctrd = np.array(ctrd, np.float32, order="C", copy=True)
-    asmt = np.array(asmt, np.uint8, order="C", copy=True)
+    ctrd, asmt = _refine_start(ctrd, asmt)
     S, K, d = ctrd.shape
     if y.dim() != 4 or t.dim() != 4 or t.shape[0] != y.shape[0]:
         raise QcnnError("y must be [N, Hin, Win, Cin] and t [N, Ho, Wo, Cout] with the same N, got %s and %s"
@@ -761,11 +760,11 @@ def pq_refine_conv_target(ctx, y, t, ctrd, asmt, ksz, pad=0, stride=1, grp=1, sw
         if S != -(-(Cin // grp) // d) or asmt.shape != (Cout, ksz, ksz, S):
             raise QcnnError("ctrd [%d, K, d] and asmt %s do not match a [%d, %d, %d, %d] kernel with d=%d"
                             % (S, tuple(asmt.shape), Cout, Cin // grp, ksz, ksz, d))
-    loss = np.empty(max(sweeps, 0) + 1, np.float64)
-    _check(lib.qcnn_pq_refine_conv_target(ctx.h, Cin, Hin, Win, Cout, ksz, pad, stride, grp, K, d, sweeps, _dptr(y),
-                                          _dptr(t), N, ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp),
-                                          loss.ctypes.data_as(_vp), _stream(stream)))
-    return ctrd, asmt, loss
+    return _refine_call(lib.qcnn_pq_refine_conv_target, (ctx.h, Cin, Hin, Win, Cout, ksz, pad, stride, grp, K, d, sweeps,
+                                                         _dptr(y), _dptr(t), N), ctrd, asmt, sweeps, stream)
+
+
+_ABSENT = object()   # PqStats._refine: an argument the call does not take
 
 
 class PqStats(object):
@@ -778,13 +777,17 @@ class PqStats(object):
 
     def __init__(self, ctx, h, conv, shape, target):
         self.ctx, self.h, self.conv, self.target = ctx, h, conv, target
+        # d, the sums' dims (G [grp, Dg, Dg], P [outputs, Dg]), and the shapes add() and the refines check: y and t
+        # without N, wei, asmt
         self._shape = shape
+        self._groups = (shape["grp"],) if conv else ()   # FC: G [Din, Din] and s [Din]
 
     @classmethod
     def fc(cls, ctx, Din, Dout, d, target=False):
         h = _vp()
         _check(lib.qcnn_pq_stats_create_fc(ctx.h, Din, Dout, d, int(bool(target)), C.byref(h)))
-        return cls(ctx, h, False, dict(Din=Din, Dout=Dout, d=d), bool(target))
+        return cls(ctx, h, False, dict(d=d, grp=1, Dg=Din, outputs=Dout, y=(Din,), t=(Dout,), wei=(Dout, Din),
+                                       asmt=(Dout, -(-Din // d))), bool(target))
 
     @classmethod
     def conv(cls, ctx, Cin, Hin, Win, Cout, ksz, d, pad=0, stride=1, grp=1, target=False):
@@ -792,8 +795,9 @@ class PqStats(object):
         _check(lib.qcnn_pq_stats_create_conv(ctx.h, Cin, Hin, Win, Cout, ksz, pad, stride, grp, d, int(bool(target)),
                                              C.byref(h)))
         Ho, Wo = (Hin + 2 * pad - ksz) // stride + 1, (Win + 2 * pad - ksz) // stride + 1
-        return cls(ctx, h, True, dict(Cin=Cin, Hin=Hin, Win=Win, Cout=Cout, ksz=ksz, pad=pad, stride=stride, grp=grp,
-                                      d=d, Ho=Ho, Wo=Wo), bool(target))
+        Cg = Cin // grp
+        return cls(ctx, h, True, dict(d=d, grp=grp, Dg=Cg * ksz * ksz, outputs=Cout, y=(Hin, Win, Cin), t=(Ho, Wo, Cout),
+                                      wei=(Cout, Cg, ksz, ksz), asmt=(Cout, ksz, ksz, -(-Cg // d))), bool(target))
 
     def _live(self):
         if not self.h:
@@ -803,13 +807,12 @@ class PqStats(object):
         """Fold a batch: y [N, Din] (FC) or [N, Hin, Win, Cin] (NHWC conv), t [N, Dout] or [N, Ho, Wo, Cout] for a
         target object, contiguous float32 CUDA tensors that must stay alive until the stream has run the add."""
         self._live()
-        g = self._shape
         N = y.shape[0] if y.dim() >= 1 else 0
-        want_y = (N, g["Din"]) if not self.conv else (N, g["Hin"], g["Win"], g["Cin"])
+        want_y = (N,) + self._shape["y"]
         if tuple(y.shape) != want_y:
             raise QcnnError("y must be %s, got %s" % (want_y, tuple(y.shape)))
         if t is not None:
-            want_t = (N, g["Dout"]) if not self.conv else (N, g["Ho"], g["Wo"], g["Cout"])
+            want_t = (N,) + self._shape["t"]
             if tuple(t.shape) != want_t:
                 raise QcnnError("t must be %s, got %s" % (want_t, tuple(t.shape)))
         _check(lib.qcnn_pq_stats_add(self.h, _dptr(y), None if t is None else _dptr(t), N, _stream(stream)))
@@ -826,14 +829,9 @@ class PqStats(object):
         """(G, P, tt): G [grp, Dg, Dg] conv / [Din, Din] FC in the internal dim order, and for a target object
         P [Cout, Dg] / [Dout, Din] and |T|^2 (else None, None), as float64 host arrays."""
         self._live()
-        g = self._shape
-        if self.conv:
-            Dg = g["Cin"] // g["grp"] * g["ksz"] * g["ksz"]
-            G = np.empty((g["grp"], Dg, Dg), np.float64)
-            P = np.empty((g["Cout"], Dg), np.float64) if self.target else None
-        else:
-            G = np.empty((g["Din"], g["Din"]), np.float64)
-            P = np.empty((g["Dout"], g["Din"]), np.float64) if self.target else None
+        Dg, outputs = self._shape["Dg"], self._shape["outputs"]
+        G = np.empty(self._groups + (Dg, Dg), np.float64)
+        P = np.empty((outputs, Dg), np.float64) if self.target else None
         tt = np.empty(1, np.float64) if self.target else None
         _check(lib.qcnn_pq_stats_read_h(self.h, G.ctypes.data_as(_vp), None if P is None else P.ctypes.data_as(_vp),
                                         None if tt is None else tt.ctypes.data_as(_vp)))
@@ -843,104 +841,69 @@ class PqStats(object):
         """(s, u, n): the sum of y, s [grp, Dg] conv (internal dim order) / [Din] FC, the sum of t, u [Cout] / [Dout]
         for a target object (else None), as float64 host arrays, and n, the rows summed (images, conv images Ho Wo)."""
         self._live()
-        g = self._shape
-        if self.conv:
-            sy = np.empty((g["grp"], g["Cin"] // g["grp"] * g["ksz"] * g["ksz"]), np.float64)
-        else:
-            sy = np.empty(g["Din"], np.float64)
-        u = np.empty(self._outputs(), np.float64) if self.target else None
+        sy = np.empty(self._groups + (self._shape["Dg"],), np.float64)
+        u = np.empty(self._shape["outputs"], np.float64) if self.target else None
         n = C.c_longlong()
         _check(lib.qcnn_pq_stats_read_sums_h(self.h, sy.ctypes.data_as(_vp), None if u is None else u.ctypes.data_as(_vp),
                                              C.byref(n)))
         return sy, u, n.value
 
-    def _outputs(self):
-        return self._shape["Cout"] if self.conv else self._shape["Dout"]
-
-    def _bias(self, bias):
-        bias = np.array(bias, np.float32, order="C", copy=True)
-        if bias.shape != (self._outputs(),):
-            raise QcnnError("bias must be (%d,), got %s" % (self._outputs(), bias.shape))
-        return bias
-
     def _start(self, ctrd, asmt):
-        ctrd = np.array(ctrd, np.float32, order="C", copy=True)
-        asmt = np.array(asmt, np.uint8, order="C", copy=True)
+        ctrd, asmt = _refine_start(ctrd, asmt)
         g = self._shape
         S, K, d = ctrd.shape if ctrd.ndim == 3 else (0, 0, 0)
-        if self.conv:
-            Cg = g["Cin"] // g["grp"]
-            want = (g["Cout"], g["ksz"], g["ksz"], -(-Cg // g["d"]))
-            ok = d == g["d"] and S == want[3] and asmt.shape == want
-        else:
-            want = (g["Dout"], -(-g["Din"] // g["d"]))
-            ok = d == g["d"] and S == want[1] and asmt.shape == want
-        if not ok:
+        want = g["asmt"]
+        if not (d == g["d"] and S == want[-1] and asmt.shape == want):
             raise QcnnError("ctrd [%d, K, %d] and asmt %s must be [S, K, d] and %s" % (S, g["d"], tuple(asmt.shape), want))
         return ctrd, asmt, K
+
+    def _refine(self, fn, ctrd, asmt, sweeps, stream, wei=_ABSENT, bias=_ABSENT):
+        """fn on the statistics from the start (ctrd, asmt), with the dense weights and the bias when the call takes
+        them: (ctrd, asmt, loss), or (ctrd, asmt, bias, loss) with a bias."""
+        self._live()
+        ctrd, asmt, K = self._start(ctrd, asmt)
+        args = []
+        if wei is not _ABSENT:
+            wei = _np(wei, np.float32)
+            if wei.shape != self._shape["wei"]:
+                raise QcnnError("wei must be %s, got %s" % (self._shape["wei"], wei.shape))
+            args.append(wei.ctypes.data_as(_vp))
+        args += [ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp)]
+        if bias is not _ABSENT:
+            bias = np.array(bias, np.float32, order="C", copy=True)
+            if bias.shape != (self._shape["outputs"],):
+                raise QcnnError("bias must be (%d,), got %s" % (self._shape["outputs"], bias.shape))
+            args.append(bias.ctypes.data_as(_vp))
+        loss = np.empty(max(sweeps, 0) + 1, np.float64)
+        _check(fn(self.h, K, sweeps, *args, loss.ctypes.data_as(_vp), _stream(stream)))
+        return (ctrd, asmt, loss) if bias is _ABSENT else (ctrd, asmt, bias, loss)
 
     def refine(self, wei, ctrd, asmt, sweeps=8, stream=None):
         """The same-input sweeps (pq_refine_fc / pq_refine_conv) on the statistics and the dense weights wei
         [Dout, Din] / [Cout, Cin / grp, k, k]: (ctrd, asmt, loss [sweeps + 1]).  The arguments are not modified."""
-        self._live()
-        ctrd, asmt, K = self._start(ctrd, asmt)
-        g = self._shape
-        wei = _np(wei, np.float32)
-        want = (g["Cout"], g["Cin"] // g["grp"], g["ksz"], g["ksz"]) if self.conv else (g["Dout"], g["Din"])
-        if wei.shape != want:
-            raise QcnnError("wei must be %s, got %s" % (want, wei.shape))
-        loss = np.empty(max(sweeps, 0) + 1, np.float64)
-        _check(lib.qcnn_pq_stats_refine(self.h, K, sweeps, wei.ctypes.data_as(_vp), ctrd.ctypes.data_as(_vp),
-                                        asmt.ctypes.data_as(_vp), loss.ctypes.data_as(_vp), _stream(stream)))
-        return ctrd, asmt, loss
+        return self._refine(lib.qcnn_pq_stats_refine, ctrd, asmt, sweeps, stream, wei=wei)
 
     def refine_target(self, ctrd, asmt, sweeps=8, stream=None):
         """The target sweeps (pq_refine_*_target) on the statistics of a target object: (ctrd, asmt, loss [sweeps + 1]).
         The arguments are not modified."""
-        self._live()
-        ctrd, asmt, K = self._start(ctrd, asmt)
-        loss = np.empty(max(sweeps, 0) + 1, np.float64)
-        _check(lib.qcnn_pq_stats_refine_target(self.h, K, sweeps, ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp),
-                                               loss.ctypes.data_as(_vp), _stream(stream)))
-        return ctrd, asmt, loss
+        return self._refine(lib.qcnn_pq_stats_refine_target, ctrd, asmt, sweeps, stream)
 
     def refine_bias(self, wei, ctrd, asmt, bias, sweeps=8, stream=None):
         """refine() with the bias free as well: the sweeps on the centered sums, then the bias refit (include/qcnn.h).
         bias [Dout] / [Cout] is the layer's bias.  Returns (ctrd, asmt, bias, loss [sweeps + 1]), loss the bias-optimal
         one; the arguments are not modified."""
-        self._live()
-        ctrd, asmt, K = self._start(ctrd, asmt)
-        g = self._shape
-        wei = _np(wei, np.float32)
-        want = (g["Cout"], g["Cin"] // g["grp"], g["ksz"], g["ksz"]) if self.conv else (g["Dout"], g["Din"])
-        if wei.shape != want:
-            raise QcnnError("wei must be %s, got %s" % (want, wei.shape))
-        bias = self._bias(bias)
-        loss = np.empty(max(sweeps, 0) + 1, np.float64)
-        _check(lib.qcnn_pq_stats_refine_bias(self.h, K, sweeps, wei.ctypes.data_as(_vp), ctrd.ctypes.data_as(_vp),
-                                             asmt.ctypes.data_as(_vp), bias.ctypes.data_as(_vp), loss.ctypes.data_as(_vp),
-                                             _stream(stream)))
-        return ctrd, asmt, bias, loss
+        return self._refine(lib.qcnn_pq_stats_refine_bias, ctrd, asmt, sweeps, stream, wei=wei, bias=bias)
 
     def refine_target_bias(self, ctrd, asmt, bias, sweeps=8, stream=None):
         """refine_target() with the bias free as well: (ctrd, asmt, bias, loss [sweeps + 1]).  The arguments are not
         modified."""
-        self._live()
-        ctrd, asmt, K = self._start(ctrd, asmt)
-        bias = self._bias(bias)
-        loss = np.empty(max(sweeps, 0) + 1, np.float64)
-        _check(lib.qcnn_pq_stats_refine_target_bias(self.h, K, sweeps, ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp),
-                                                    bias.ctypes.data_as(_vp), loss.ctypes.data_as(_vp), _stream(stream)))
-        return ctrd, asmt, bias, loss
+        return self._refine(lib.qcnn_pq_stats_refine_target_bias, ctrd, asmt, sweeps, stream, bias=bias)
 
     @property
     def nbytes(self):
         """device bytes of the sums (G and s, and for a target object P, |T|^2 and u)"""
         g = self._shape
-        if self.conv:
-            Dg = g["Cin"] // g["grp"] * g["ksz"] * g["ksz"]
-            return 8 * (g["grp"] * Dg * (Dg + 1) + ((Dg + 1) * g["Cout"] + 1 if self.target else 0))
-        return 8 * (g["Din"] * (g["Din"] + 1) + ((g["Din"] + 1) * g["Dout"] + 1 if self.target else 0))
+        return 8 * (g["grp"] * g["Dg"] * (g["Dg"] + 1) + ((g["Dg"] + 1) * g["outputs"] + 1 if self.target else 0))
 
     def close(self):
         if self.h:

@@ -32,7 +32,6 @@ namespace cg = cooperative_groups;
 
 namespace {
 
-constexpr int kMaxD = 64;
 constexpr int kBlockDims = 256;      // dims per block of subspaces (a multiple of d): the K of the trailing GEMM
 
 // Per subspace m (blockIdx.x): the lower-triangular inverse of the Cholesky factor of G_mm + lambda I, [w][w] at row
@@ -77,18 +76,6 @@ __global__ void __launch_bounds__(kSweepThreads) pqr_chol_kernel(const double* _
   for (int e = tid; e < w * w; e += blockDim.x) {
     const int i = e / w, j = e % w;
     Linv[(static_cast<size_t>(m) * d + i) * d + j] = j <= i ? Li[i * ld + j] : 0.0;
-  }
-}
-
-// E[o][c] = W[o][c] - C[c / d][A[c / d][o]][c % d] in fp64 (A held subspace-major, [S][Dout])
-__global__ void pqr_residual_kernel(const float* __restrict__ W, const float* __restrict__ C, const uint8_t* __restrict__ A,
-                                    double* __restrict__ E, int Din, int Dout, int K, int d) {
-  const size_t total = static_cast<size_t>(Dout) * Din;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int o = static_cast<int>(i / Din), c = static_cast<int>(i % Din), m = c / d;
-    const float cw = C[(static_cast<size_t>(m) * K + A[static_cast<size_t>(m) * Dout + o]) * d + c % d];
-    E[i] = static_cast<double>(W[i]) - static_cast<double>(cw);
   }
 }
 
@@ -262,71 +249,27 @@ __global__ void __launch_bounds__(kSweepThreads) pqr_block_kernel(BlockArgs p) {
   }
 }
 
-// The host-side checks of a refine (weights unless target, codebook, assignments) and the assignments as [S][Dout]
-int CheckFcHost(const char* who, bool target, int Din, int Dout, int K, int d, const float* w_h, const float* ctrd_h,
-                const uint8_t* asmt_h, std::vector<uint8_t>& at) {
-  const int S = CeilDiv(Din, d);
-  const size_t nw = static_cast<size_t>(Dout) * Din, nc = static_cast<size_t>(S) * K * d;
-  if (!target) QCNN_CHECK(AllFinite(w_h, nw), "%s: the weights contain a non-finite value", who);
-  QCNN_CHECK(AllFinite(ctrd_h, nc), "%s: the codebook contains a non-finite value", who);
-  at.assign(static_cast<size_t>(S) * Dout, 0);
-  for (int o = 0; o < Dout; o++)
-    for (int m = 0; m < S; m++) {
-      const uint8_t a = asmt_h[static_cast<size_t>(o) * S + m];
-      QCNN_CHECK(a < K, "%s: assignment %d of output %d, subspace %d is not below K=%d", who, a, o, m, K);
-      at[static_cast<size_t>(m) * Dout + o] = a;
-    }
-  return 0;
-}
-
-// The sweeps on the sums G, P = T^T Y and |T|^2 (those of s, or their centered copies).  target: the target form (w_h is
-// not read); else the same-input form on w_h.  bias_h non-NULL: replaced by the refit bias (RefitBias).
-int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* w_h, const double* G,
-            const double* TY, const double* TT, std::vector<uint8_t>& at, float* ctrd_h, uint8_t* asmt_h, float* bias_h,
-            double* loss_h, cudaStream_t st) {
+// The FC sweeps (arguments as SweepConv's): the inverse Cholesky factors of every subspace once, then per block of
+// subspaces the cooperative block kernel and the trailing GEMM
+int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wts, std::vector<uint8_t>& at,
+            const double* G, const double* P, const double* TT, float* ctrd_h, uint8_t* asmt_h, float* bias_h, double* loss_h,
+            cudaStream_t st) {
   qcnn_ctx* ctx = s->ctx;
-  const int Din = s->Din, Dout = s->Dout, d = s->d, S = CeilDiv(Din, d);
-  const size_t nw = static_cast<size_t>(Dout) * Din, nc = static_cast<size_t>(S) * K * d;
+  const int Din = s->geo.Dg, Dout = s->geo.Cout, d = s->d, S = CeilDiv(Din, d);
   QCNN_ON_DEVICE(ctx->device);
+  SweepState ss;
+  if (int rc = BeginSweeps(&ss, s, who, target, K, sweeps, wts, at, ctrd_h, G, P, TT, st)) return rc;
   const int spb = std::max(1, kBlockDims / d), ld = spb * d;
-  DeviceBuffer dE, dGE, dW, dC, dA, dL, dDlt, dH, dCc, dPart, dLoss;
-  auto reserve = [&](DeviceBuffer& b, size_t bytes, const char* what) -> int {
-    const cudaError_t e = b.Reserve(ctx, bytes);
-    if (e == cudaSuccess) return 0;
-    cudaGetLastError();
-    SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
+  DeviceBuffer dL, dDlt, dH, dCc;
+  if (Reserve(ctx, who, dL, sizeof(double) * static_cast<size_t>(S) * d * d, "the Cholesky factors") ||
+      Reserve(ctx, who, dDlt, sizeof(double) * Dout * static_cast<size_t>(ld), "the block's changes") ||
+      Reserve(ctx, who, dH, sizeof(double) * Dout * static_cast<size_t>(d), "the subspace responses") ||
+      Reserve(ctx, who, dCc, sizeof(double) * K, "the codeword norms"))
     return 1;
-  };
-  if (reserve(dE, sizeof(double) * nw, "the residual") || reserve(dGE, sizeof(double) * nw, "G times the residual") ||
-      reserve(dW, sizeof(float) * nw, "the weights") || reserve(dC, sizeof(float) * nc, "the codebook") ||
-      reserve(dA, at.size(), "the assignments") ||
-      reserve(dL, sizeof(double) * static_cast<size_t>(S) * d * d, "the Cholesky factors") ||
-      reserve(dDlt, sizeof(double) * Dout * static_cast<size_t>(ld), "the block's changes") ||
-      reserve(dH, sizeof(double) * Dout * static_cast<size_t>(d), "the subspace responses") ||
-      reserve(dCc, sizeof(double) * K, "the codeword norms") || reserve(dPart, sizeof(double) * kLossBlocks, "the loss") ||
-      reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss"))
-    return 1;
-  if (!target) TY = TT = nullptr;
-  QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
-  if (target) QCNN_CUDA(cudaMemsetAsync(dW.get(), 0, sizeof(float) * nw, st));   // E = 0 - W^
-  else QCNN_CUDA(cudaMemcpyAsync(dW.get(), w_h, sizeof(float) * nw, cudaMemcpyHostToDevice, st));
-  QCNN_CUDA(cudaMemcpyAsync(dC.get(), ctrd_h, sizeof(float) * nc, cudaMemcpyHostToDevice, st));
-  QCNN_CUDA(cudaMemcpyAsync(dA.get(), at.data(), at.size(), cudaMemcpyHostToDevice, st));
-  const int tiles = CeilDiv(Din, kTile);
-  const dim3 gemmGrid(tiles, CeilDiv(Dout, kTile));
   const size_t cholSmem = sizeof(double) * 2 * std::min(d, Din) * (std::min(d, Din) + 1);
   if (int rc = OptInSmem<pqr_chol_kernel>(ctx)) return rc;
   pqr_chol_kernel<<<S, kSweepThreads, cholSmem, st>>>(G, dL.as<double>(), Din, d);
-  const int ewBlocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 32u * ctx->sm_count));
-  pqr_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Din, Dout, K, d);
-  // GE = E G, or P + E G for a target
-  if (target) QCNN_CUDA(cudaMemcpyAsync(dGE.get(), TY, sizeof(double) * nw, cudaMemcpyDeviceToDevice, st));
-  pqr_gemm_kernel<kGemmF64><<<gemmGrid, kGemmThreads, 0, st>>>(dE.get(), Din, G, Din, dGE.as<double>(), Din, Dout, Din, Din, target);
   QCNN_CUDA(cudaGetLastError());
-  auto loss = [&](int sw) -> int {
-    return LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st, TY, TT);
-  };
-  if (int rc = loss(0)) return rc;
   if (sweeps > 0) {
     const size_t blkSmem = sizeof(float) * K * std::min(d, Din) + sizeof(double) * (K + 1);
     cudaFuncAttributes fa;   // the opt-in limit covers static plus dynamic shared memory
@@ -337,8 +280,9 @@ int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, c
     QCNN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, pqr_block_kernel, kSweepThreads, blkSmem));
     QCNN_CHECK(perSm >= 1, "%s: the sweep kernel does not fit on an SM", who);
     const int grid = std::min(std::min(perSm, 2) * ctx->sm_count, std::max(Dout, K));
-    BlockArgs a{G, dGE.as<double>(), dL.as<double>(), dE.as<double>(), dDlt.as<double>(), dH.as<double>(),
-                dCc.as<double>(), dC.as<float>(), dA.as<uint8_t>(), Din, Dout, K, d, ld, 0, 0};
+    const dim3 gemmGrid(CeilDiv(Din, kTile), CeilDiv(Dout, kTile));
+    BlockArgs a{G, ss.GE.as<double>(), dL.as<double>(), ss.E.as<double>(), dDlt.as<double>(), dH.as<double>(),
+                dCc.as<double>(), ss.C.as<float>(), ss.A.as<uint8_t>(), Din, Dout, K, d, ld, 0, 0};
     for (int sw = 1; sw <= sweeps; sw++) {
       for (int m0 = 0; m0 < S; m0 += spb) {
         a.m0 = m0;
@@ -348,49 +292,19 @@ int SweepFc(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, c
         // GE += dlt G[block dims][:]
         const int blk0 = m0 * d, bw = std::min(Din, a.m1 * d) - blk0;
         pqr_gemm_kernel<kGemmF64><<<gemmGrid, kGemmThreads, 0, st>>>(dDlt.get(), ld, G + static_cast<size_t>(blk0) * Din, Din,
-                                                                  dGE.as<double>(), Din, Dout, Din, bw, 1);
+                                                                  ss.GE.as<double>(), Din, Dout, Din, bw, 1);
         QCNN_CUDA(cudaGetLastError());
       }
-      if (int rc = loss(sw)) return rc;
+      if (int rc = ss.Loss(sw, st)) return rc;
     }
   }
-  if (bias_h) {   // E = W - W^ (target: -W^) afresh from the final codebook and assignments
-    pqr_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Din, Dout, K, d);
-    if (int rc = RefitBias(s, who, target, dE.as<double>(), 1, Din, Dout, bias_h, st)) return rc;
-  }
-  std::vector<double> lossv(sweeps + 1);
-  QCNN_CUDA(cudaMemcpyAsync(ctrd_h, dC.get(), sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
-  QCNN_CUDA(cudaMemcpyAsync(at.data(), dA.get(), at.size(), cudaMemcpyDeviceToHost, st));
-  QCNN_CUDA(cudaMemcpyAsync(lossv.data(), dLoss.get(), sizeof(double) * lossv.size(), cudaMemcpyDeviceToHost, st));
-  QCNN_CUDA(cudaStreamSynchronize(st));
-  for (int o = 0; o < Dout; o++)
-    for (int m = 0; m < S; m++) asmt_h[static_cast<size_t>(o) * S + m] = at[static_cast<size_t>(m) * Dout + o];
-  if (loss_h) std::copy(lossv.begin(), lossv.end(), loss_h);
-  return 0;
+  return EndSweeps(ss, ctrd_h, asmt_h, bias_h, loss_h, st);
 }
 
-int CreateFc(qcnn_ctx* ctx, const char* who, int Din, int Dout, int d, bool target, bool sums, qcnn_pq_stats** out) {
-  QCNN_CHECK(ctx && out, "%s: NULL argument", who);
-  *out = nullptr;
-  QCNN_CHECK(Din >= 1 && Dout >= 1, "%s: bad dimensions", who);
-  QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
-  std::unique_ptr<qcnn_pq_stats> s(new qcnn_pq_stats);
-  s->ctx = ctx;
-  s->conv = false;
-  s->target = target;
-  s->d = d;
-  s->Din = Din;
-  s->Dout = Dout;
-  s->sums = sums;
-  if (AllocStats(s.get(), who, sizeof(double) * Din * static_cast<size_t>(Din), sizeof(double) * Dout * static_cast<size_t>(Din),
-                 sizeof(double) * Din, sizeof(double) * Dout, 0))
-    return 1;
-  *out = s.release();
-  return 0;
-}
+// An FC layer of Din inputs and Dout outputs as its 1x1 conv geometry
+PqGeometry FcGeometry(int Din, int Dout) { return PqGeometry{Din, 1, 1, Dout, 1, 0, 1, 1, 1, 1, Din, Dout, 1, Din}; }
 
-// The one-shot calls: create (without the first moments, which they never read), one add of all N inputs, the sweeps,
-// destroy (the checks keep the order of their messages)
+// The one-shot FC calls' argument checks, in the order of their messages
 int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int sweeps, const float* w_h, const float* x, const float* t,
            int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h, cudaStream_t st) {
   const char* who = target ? "qcnn_pq_refine_fc_target" : "qcnn_pq_refine_fc";
@@ -402,14 +316,22 @@ int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int swee
   QCNN_CHECK(N >= 1, "%s: N=%d: at least one input is needed", who, N);
   QCNN_CHECK(x, "%s: NULL argument", who);
   QCNN_CHECK(!target || t, "%s: NULL t", who);
-  std::vector<uint8_t> at;
-  if (int rc = CheckFcHost(who, target, Din, Dout, K, d, w_h, ctrd_h, asmt_h, at)) return rc;
-  qcnn_pq_stats* sp = nullptr;
-  if (int rc = CreateFc(ctx, who, Din, Dout, d, target, false, &sp)) return rc;
-  std::unique_ptr<qcnn_pq_stats> s(sp);
-  if (int rc = FcStatsAdd(s.get(), who, x, t, N, st)) return rc;
-  return SweepFc(s.get(), who, target, K, sweeps, w_h, s->G.as<double>(), s->P.as<double>(), s->tt.as<double>(), at, ctrd_h,
-                 asmt_h, nullptr, loss_h, st);
+  return RefineOnce(ctx, who, false, target, FcGeometry(Din, Dout), K, d, sweeps, w_h, x, t, N, ctrd_h, asmt_h, loss_h, st);
+}
+
+// The sweeps of s's kind on its sums, or with bias_h on their centered copies and followed by the bias refit
+int Sweep(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, Start& start, float* ctrd_h, uint8_t* asmt_h,
+          float* bias_h, double* loss_h, cudaStream_t st) {
+  const double *G = s->G.as<double>(), *P = s->P.as<double>(), *TT = s->tt.as<double>();
+  CenteredSums c;
+  if (bias_h) {
+    if (int rc = CenterSums(s, who, target, &c, st)) return rc;
+    G = c.G.as<double>();
+    P = c.P.as<double>();
+    TT = c.tt.as<double>();
+  }
+  return (s->conv ? SweepConv : SweepFc)(s, who, target, K, sweeps, start.w, start.at, G, P, TT, ctrd_h, asmt_h, bias_h, loss_h,
+                                         st);
 }
 
 }  // namespace
@@ -419,7 +341,7 @@ namespace qcnn {
 // An FC add: the scan (its message names the first input column holding a NaN or Inf), then one fold of the sums
 // (G, then s; for a target |T|^2, P, then u)
 int FcStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st) {
-  const int Din = s->Din, Dout = s->Dout;
+  const int Din = s->geo.Cin, Dout = s->geo.Cout;
   unsigned first[2];
   if (int rc = ScanAdd(s, y, static_cast<size_t>(N) * Din, Din, t, static_cast<size_t>(N) * Dout, first, st)) return rc;
   QCNN_CHECK(first[0] == kNoneFound, "%s: %s contains a non-finite value (input column %u)", who, s->target ? "y" : "x", first[0]);
@@ -442,18 +364,16 @@ int FcStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t
   return 0;
 }
 
-int FcStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wei_h, float* ctrd_h,
-                  uint8_t* asmt_h, float* bias_h, double* loss_h, cudaStream_t st) {
-  if (int rc = CheckFcK(who, K)) return rc;
-  std::vector<uint8_t> at;
-  if (int rc = CheckFcHost(who, target, s->Din, s->Dout, K, s->d, wei_h, ctrd_h, asmt_h, at)) return rc;
-  if (!bias_h)
-    return SweepFc(s, who, target, K, sweeps, wei_h, s->G.as<double>(), s->P.as<double>(), s->tt.as<double>(), at, ctrd_h, asmt_h,
-                   nullptr, loss_h, st);
-  CenteredSums c;
-  if (int rc = CenterSums(s, who, target, 1, s->Din, s->Dout, &c, st)) return rc;
-  return SweepFc(s, who, target, K, sweeps, wei_h, c.G.as<double>(), c.P.as<double>(), c.tt.as<double>(), at, ctrd_h, asmt_h,
-                 bias_h, loss_h, st);
+int RefineOnce(qcnn_ctx* ctx, const char* who, bool conv, bool target, const PqGeometry& geo, int K, int d, int sweeps,
+               const float* w_h, const float* x, const float* t, int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h,
+               cudaStream_t st) {
+  Start start;
+  if (int rc = CheckStart(who, conv, target, geo, K, d, w_h, ctrd_h, asmt_h, &start)) return rc;
+  qcnn_pq_stats* sp = nullptr;
+  if (int rc = CreateStats(ctx, who, conv, geo, d, target, false, &sp)) return rc;
+  std::unique_ptr<qcnn_pq_stats> s(sp);
+  if (int rc = conv ? ConvStatsAdd(s.get(), who, x, t, N, st) : FcStatsAdd(s.get(), who, x, t, N, st)) return rc;
+  return Sweep(s.get(), who, target, K, sweeps, start, ctrd_h, asmt_h, nullptr, loss_h, st);
 }
 
 }  // namespace qcnn
@@ -471,7 +391,12 @@ extern "C" int qcnn_pq_refine_fc_target(qcnn_ctx* ctx, int Din, int Dout, int K,
 // ---- the statistics objects (both kinds; the conv creation and the conv halves are in pq_refine_conv.cu)
 
 extern "C" int qcnn_pq_stats_create_fc(qcnn_ctx* ctx, int Din, int Dout, int d, int target, qcnn_pq_stats** out) {
-  return CreateFc(ctx, "qcnn_pq_stats_create_fc", Din, Dout, d, target != 0, true, out);
+  const char* who = "qcnn_pq_stats_create_fc";
+  QCNN_CHECK(ctx && out, "%s: NULL argument", who);
+  *out = nullptr;
+  QCNN_CHECK(Din >= 1 && Dout >= 1, "%s: bad dimensions", who);
+  QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
+  return CreateStats(ctx, who, false, FcGeometry(Din, Dout), d, target != 0, true, out);
 }
 
 extern "C" int qcnn_pq_stats_add(qcnn_pq_stats* s, const float* y, const float* t, int N, void* stream) {
@@ -517,18 +442,18 @@ extern "C" int qcnn_pq_stats_read_sums_h(const qcnn_pq_stats* s, double* s_h, do
 
 namespace {
 
-// bias: the bias calls, which also need bias_h (finite, [Dout] / [Cout])
+// bias: the bias calls, which also need bias_h (finite, [Cout]); without it the sweeps run on the raw sums
 int RefineStats(qcnn_pq_stats* s, const char* who, bool target, bool bias, int K, int sweeps, const float* wei_h, float* ctrd_h,
                 uint8_t* asmt_h, float* bias_h, double* loss_h, void* stream) {
   QCNN_CHECK(s && (target || wei_h) && ctrd_h && asmt_h && (!bias || bias_h), "%s: NULL argument", who);
   QCNN_CHECK(!target || s->target, "%s: the statistics were created without a target", who);
   QCNN_CHECK(s->images > 0, "%s: no calibration data has been added", who);
   QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
-  if (bias) QCNN_CHECK(AllFinite(bias_h, s->conv ? s->geo.Cout : s->Dout), "%s: the bias contains a non-finite value", who);
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (!bias) bias_h = nullptr;
-  return s->conv ? ConvStatsRefine(s, who, target, K, sweeps, wei_h, ctrd_h, asmt_h, bias_h, loss_h, st)
-                 : FcStatsRefine(s, who, target, K, sweeps, wei_h, ctrd_h, asmt_h, bias_h, loss_h, st);
+  if (bias) QCNN_CHECK(AllFinite(bias_h, s->geo.Cout), "%s: the bias contains a non-finite value", who);
+  if (int rc = s->conv ? CheckConvSystem(who, K, s->d, s->geo.Cg) : CheckFcK(who, K)) return rc;
+  Start start;
+  if (int rc = CheckStart(who, s->conv, target, s->geo, K, s->d, wei_h, ctrd_h, asmt_h, &start)) return rc;
+  return Sweep(s, who, target, K, sweeps, start, ctrd_h, asmt_h, bias ? bias_h : nullptr, loss_h, static_cast<cudaStream_t>(stream));
 }
 
 }  // namespace

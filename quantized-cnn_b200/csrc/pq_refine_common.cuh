@@ -1,5 +1,6 @@
 // Pieces shared by the error-correcting quantizers of FC layers (pq_refine.cu) and conv layers (pq_refine_conv.cu):
-// the fp64 tensor-core GEMM, the fixed-order block reduction and the loss kernels (same-input and target form).  They
+// the fp64 tensor-core GEMM, the fixed-order block reduction, the residual and loss kernels (same-input and target
+// form), and the host code around the sweeps, which treats an FC layer as its 1x1 conv geometry (PqGeometry).  They
 // sit in an anonymous namespace because each including .cu file is its own device module and links its own copy.
 #ifndef QCNN_PQ_REFINE_COMMON_CUH_
 #define QCNN_PQ_REFINE_COMMON_CUH_
@@ -7,12 +8,14 @@
 #include <math.h>
 
 #include <algorithm>
+#include <memory>
 #include <vector>
 
 #include "qcnn_internal.h"
 
 namespace {
 
+constexpr int kMaxD = 64;            // the widest subspace
 constexpr int kTile = 64;            // GEMM output tile (kTile x kTile per CTA, 2 x 2 warps of 32 x 32)
 constexpr int kKStep = 16;           // the DMMA's k
 constexpr int kLd = kTile + 4;       // smem row pitch in doubles: fragment reads hit 16 distinct 8-byte bank pairs
@@ -46,6 +49,20 @@ __device__ __forceinline__ Dim DecodeDim(int q, int Cg, int d, int T) {
   r.t = rem / r.w;
   r.j = rem - r.t * r.w;
   return r;
+}
+
+// E[o][q] = W[o][q] - C[m][A[m][o][t]][j] in fp64 (A held [S][Cout][T]; FC: T = 1, q the input column)
+__global__ void pqrc_residual_kernel(const float* __restrict__ W, const float* __restrict__ C, const uint8_t* __restrict__ A,
+                                     double* __restrict__ E, int Cout, int Cg, int K, int d, int T) {
+  const int Dg = Cg * T;
+  const size_t total = static_cast<size_t>(Cout) * Dg;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const int o = static_cast<int>(i / Dg);
+    const Dim q = DecodeDim(static_cast<int>(i % Dg), Cg, d, T);
+    const uint8_t a = A[(static_cast<size_t>(q.m) * Cout + o) * T + q.t];
+    E[i] = static_cast<double>(W[i]) - static_cast<double>(C[(static_cast<size_t>(q.m) * K + a) * d + q.j]);
+  }
 }
 
 // The patch operand of the map modes: row k is output position pos0 + k = (n Ho + oy) Wo + ox of the NHWC map
@@ -366,45 +383,57 @@ inline int ScanAdd(qcnn_pq_stats* s, const float* y, size_t ny, unsigned ycols, 
   return 0;
 }
 
-// The parts of a stats object both kinds share: the sums (zero until the first add), the scratch and the event.
-// syBytes / suBytes / planeBytes: the first moments and the conv plane, allocated only when s->sums is set.
-inline int AllocStats(qcnn_pq_stats* s, const char* who, size_t gBytes, size_t pBytes, size_t syBytes, size_t suBytes,
-                      size_t planeBytes) {
-  qcnn_ctx* ctx = s->ctx;
-  auto reserve = [&](qcnn::DeviceBuffer& b, size_t bytes, const char* what) -> int {
-    const cudaError_t e = b.Reserve(ctx, bytes);
-    if (e == cudaSuccess) return 0;
-    cudaGetLastError();
-    qcnn::SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
-    return 1;
-  };
-  if (!s->sums) syBytes = suBytes = planeBytes = 0;
-  if (!s->target) suBytes = 0;
-  if (reserve(s->G, gBytes, "the Gram matrices") || reserve(s->P, s->target ? pBytes : 0, "the targets' cross product") ||
-      reserve(s->tt, s->target ? sizeof(double) : 0, "the targets' norm") ||
-      reserve(s->sy, syBytes, "the inputs' sum") || reserve(s->su, suBytes, "the targets' sum") ||
-      reserve(s->plane, planeBytes, "the per-add image sum") ||
-      reserve(s->scratch, sizeof(double) * kLossBlocks + 2 * sizeof(unsigned), "the scan flags"))
+// Makes b hold at least bytes on ctx's device; on failure sets who's error, which names what the buffer is for
+inline int Reserve(qcnn_ctx* ctx, const char* who, qcnn::DeviceBuffer& b, size_t bytes, const char* what) {
+  const cudaError_t e = b.Reserve(ctx, bytes);
+  if (e == cudaSuccess) return 0;
+  cudaGetLastError();
+  qcnn::SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
+  return 1;
+}
+
+// A statistics object of either kind with its sums zero until the first add: G [grp][Dg][Dg], for a target P [Cout][Dg]
+// and |T|^2, the scratch and the event.  sums: also the first moments, s [grp][Dg] and for a target u [Cout], and for
+// conv the per-add plane (FC: none).
+inline int CreateStats(qcnn_ctx* ctx, const char* who, bool conv, const qcnn::PqGeometry& geo, int d, bool target, bool sums,
+                       qcnn_pq_stats** out) {
+  std::unique_ptr<qcnn_pq_stats> s(new qcnn_pq_stats);
+  s->ctx = ctx;
+  s->conv = conv;
+  s->target = target;
+  s->d = d;
+  s->geo = geo;
+  s->sums = sums;
+  const size_t gBytes = sizeof(double) * geo.grp * static_cast<size_t>(geo.Dg) * geo.Dg;
+  const size_t pBytes = target ? sizeof(double) * geo.Cout * static_cast<size_t>(geo.Dg) : 0;
+  const size_t syBytes = sums ? sizeof(double) * geo.grp * static_cast<size_t>(geo.Dg) : 0;
+  const size_t suBytes = sums && target ? sizeof(double) * geo.Cout : 0;
+  const size_t inPlane = static_cast<size_t>(geo.Hin) * geo.Win * geo.Cin, outPlane = static_cast<size_t>(geo.Ho) * geo.Wo * geo.Cout;
+  const size_t planeBytes = sums && conv ? sizeof(double) * (target ? std::max(inPlane, outPlane) : inPlane) : 0;
+  if (Reserve(ctx, who, s->G, gBytes, "the Gram matrices") || Reserve(ctx, who, s->P, pBytes, "the targets' cross product") ||
+      Reserve(ctx, who, s->tt, target ? sizeof(double) : 0, "the targets' norm") ||
+      Reserve(ctx, who, s->sy, syBytes, "the inputs' sum") || Reserve(ctx, who, s->su, suBytes, "the targets' sum") ||
+      Reserve(ctx, who, s->plane, planeBytes, "the per-add image sum") ||
+      Reserve(ctx, who, s->scratch, sizeof(double) * kLossBlocks + 2 * sizeof(unsigned), "the scan flags"))
     return 1;
   QCNN_ON_DEVICE(ctx->device);
   QCNN_CUDA(cudaEventCreateWithFlags(&s->done, cudaEventDisableTiming));
   QCNN_CUDA(cudaMemset(s->G.get(), 0, gBytes));
-  if (s->target) {
+  if (target) {
     QCNN_CUDA(cudaMemset(s->P.get(), 0, pBytes));
     QCNN_CUDA(cudaMemset(s->tt.get(), 0, sizeof(double)));
   }
   if (syBytes) QCNN_CUDA(cudaMemset(s->sy.get(), 0, syBytes));
   if (suBytes) QCNN_CUDA(cudaMemset(s->su.get(), 0, suBytes));
   QCNN_CUDA(cudaEventRecord(s->done, nullptr));
+  *out = s.release();
   return 0;
 }
 
 // ---- first moments and the bias refit (DESIGN.md 4e, "Bias refit")
 
-// The rows n the first moments are summed over: images (FC) or images Ho Wo (conv)
-inline long long StatsRows(const qcnn_pq_stats* s) {
-  return s->conv ? s->images * s->geo.Ho * s->geo.Wo : s->images;
-}
+// The rows n the first moments are summed over: images Ho Wo (FC: images)
+inline long long StatsRows(const qcnn_pq_stats* s) { return s->images * s->geo.Ho * s->geo.Wo; }
 
 // out[c] = (accumulate ? out[c] + f : f), f = sum over r = 0..rows-1 ascending of x[r cols + c] in fp64: one fresh
 // fixed-order sum per column, folded with one addition
@@ -459,25 +488,18 @@ __global__ void pqr_bias_delta_kernel(const double* __restrict__ E, const double
   if (lane == 0) delta[o] = __ddiv_rn(u ? __dadd_rn(u[o], v) : v, n);
 }
 
-// The centered copies of a stats object's sums, for grp groups of D dims and Dout outputs (Dout / grp per group):
-// G [grp][D][D] always, P [Dout][D] and |T_c|^2 for the target form
+// The centered copies of a stats object's sums: G [grp][Dg][Dg] always, P [Cout][Dg] and |T_c|^2 for the target form
 struct CenteredSums {
   qcnn::DeviceBuffer G, P, tt;
 };
 
-inline int CenterSums(qcnn_pq_stats* s, const char* who, bool target, int grp, int D, int Dout, CenteredSums* c, cudaStream_t st) {
+inline int CenterSums(qcnn_pq_stats* s, const char* who, bool target, CenteredSums* c, cudaStream_t st) {
   qcnn_ctx* ctx = s->ctx;
+  const int grp = s->geo.grp, D = s->geo.Dg, Dout = s->geo.Cout;
   const size_t gn = static_cast<size_t>(grp) * D * D, pn = static_cast<size_t>(Dout) * D;
-  auto reserve = [&](qcnn::DeviceBuffer& b, size_t bytes, const char* what) -> int {
-    const cudaError_t e = b.Reserve(ctx, bytes);
-    if (e == cudaSuccess) return 0;
-    cudaGetLastError();
-    qcnn::SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
-    return 1;
-  };
-  if (reserve(c->G, sizeof(double) * gn, "the centered Gram matrices") ||
-      reserve(c->P, target ? sizeof(double) * pn : 0, "the centered cross product") ||
-      reserve(c->tt, target ? sizeof(double) : 0, "the centered targets' norm"))
+  if (Reserve(ctx, who, c->G, sizeof(double) * gn, "the centered Gram matrices") ||
+      Reserve(ctx, who, c->P, target ? sizeof(double) * pn : 0, "the centered cross product") ||
+      Reserve(ctx, who, c->tt, target ? sizeof(double) : 0, "the centered targets' norm"))
     return 1;
   QCNN_ON_DEVICE(ctx->device);
   QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
@@ -494,19 +516,14 @@ inline int CenterSums(qcnn_pq_stats* s, const char* who, bool target, int grp, i
   return 0;
 }
 
-// bias_h[o] = fp32(bias_h[o] + delta_o) from the final residual E [Dout][D] on the device (pqr_bias_delta_kernel)
-inline int RefitBias(qcnn_pq_stats* s, const char* who, bool target, const double* E, int grp, int D, int Dout, float* bias_h,
-                     cudaStream_t st) {
+// bias_h[o] = fp32(bias_h[o] + delta_o) from the final residual E [Cout][Dg] on the device (pqr_bias_delta_kernel)
+inline int RefitBias(qcnn_pq_stats* s, const char* who, bool target, const double* E, float* bias_h, cudaStream_t st) {
+  const int Dout = s->geo.Cout;
   qcnn::DeviceBuffer dDelta;
-  const cudaError_t e = dDelta.Reserve(s->ctx, sizeof(double) * Dout);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    qcnn::SetError("%s: cannot allocate %zu bytes of device memory for the bias change (%s)", who, sizeof(double) * Dout,
-                   cudaGetErrorString(e));
-    return 1;
-  }
-  pqr_bias_delta_kernel<<<qcnn::CeilDiv(Dout, 8), 256, 0, st>>>(E, s->sy.as<double>(), target ? s->su.as<double>() : nullptr, Dout, D,
-                                                          Dout / grp, static_cast<double>(StatsRows(s)), dDelta.as<double>());
+  if (Reserve(s->ctx, who, dDelta, sizeof(double) * Dout, "the bias change")) return 1;
+  pqr_bias_delta_kernel<<<qcnn::CeilDiv(Dout, 8), 256, 0, st>>>(E, s->sy.as<double>(), target ? s->su.as<double>() : nullptr, Dout,
+                                                                s->geo.Dg, s->geo.Cpg, static_cast<double>(StatsRows(s)),
+                                                                dDelta.as<double>());
   QCNN_CUDA(cudaGetLastError());
   std::vector<double> delta(Dout);
   QCNN_CUDA(cudaMemcpyAsync(delta.data(), dDelta.get(), sizeof(double) * Dout, cudaMemcpyDeviceToHost, st));
@@ -515,10 +532,141 @@ inline int RefitBias(qcnn_pq_stats* s, const char* who, bool target, const doubl
   return 0;
 }
 
+// ---- the start and the end of the sweeps (SweepFc, SweepConv)
+
 bool AllFinite(const float* v, size_t n) {
   for (size_t i = 0; i < n; i++)
     if (!isfinite(v[i])) return false;
   return true;
+}
+
+// A refine's start as the sweeps read it: at, the assignments [Cout][T][S] as [S][Cout][T], and w, the weights
+// [Cout][Cg][T] in the internal dim order (NULL for the target form): the caller's own array when T == 1, where the
+// two orders agree, else the permuted copy wp
+struct Start {
+  std::vector<uint8_t> at;
+  std::vector<float> wp;
+  const float* w = nullptr;
+};
+
+// The host-side checks of a refine (weights unless target, codebook, assignments; the FC message names no tap), then
+// the start
+inline int CheckStart(const char* who, bool conv, bool target, const qcnn::PqGeometry& geo, int K, int d, const float* w_h,
+                      const float* ctrd_h, const uint8_t* asmt_h, Start* start) {
+  const int Cout = geo.Cout, Cg = geo.Cg, T = geo.T, Dg = geo.Dg, S = qcnn::CeilDiv(Cg, d);
+  const size_t nw = static_cast<size_t>(Cout) * Dg, nc = static_cast<size_t>(S) * K * d;
+  if (!target) QCNN_CHECK(AllFinite(w_h, nw), "%s: the weights contain a non-finite value", who);
+  QCNN_CHECK(AllFinite(ctrd_h, nc), "%s: the codebook contains a non-finite value", who);
+  start->at.assign(static_cast<size_t>(S) * Cout * T, 0);
+  for (int o = 0; o < Cout; o++)
+    for (int t = 0; t < T; t++)
+      for (int m = 0; m < S; m++) {
+        const uint8_t a = asmt_h[(static_cast<size_t>(o) * T + t) * S + m];
+        QCNN_CHECK(a < K || conv, "%s: assignment %d of output %d, subspace %d is not below K=%d", who, a, o, m, K);
+        QCNN_CHECK(a < K, "%s: assignment %d of output %d, tap %d, subspace %d is not below K=%d", who, a, o, t, m, K);
+        start->at[(static_cast<size_t>(m) * Cout + o) * T + t] = a;
+      }
+  start->w = target ? nullptr : w_h;
+  if (target || T == 1) return 0;
+  start->wp.resize(nw);
+  for (int o = 0; o < Cout; o++)
+    for (int c = 0; c < Cg; c++) {
+      const int m = c / d, j = c % d, w = std::min(d, Cg - m * d);
+      for (int t = 0; t < T; t++)
+        start->wp[static_cast<size_t>(o) * Dg + m * d * T + t * w + j] = w_h[(static_cast<size_t>(o) * Cg + c) * T + t];
+    }
+  start->w = start->wp.data();
+  return 0;
+}
+
+// What both sweep loops share: the residual E [Cout][Dg] = W - W^ in fp64 (target form: the weights are zeros, so
+// E = -W^), GE = E G per group (target: P + E G), the weights, codebook and assignments on the device, and the losses.
+// G, P and TT are the sums the sweeps run on (P and TT NULL in the same-input form); at is the start's assignments.
+struct SweepState {
+  qcnn_pq_stats* s;
+  const char* who;
+  bool target;
+  int K, sweeps;
+  const double *G, *P, *TT;
+  std::vector<uint8_t>* at;
+  size_t nw, nc;
+  qcnn::DeviceBuffer E, GE, W, C, A, part, loss;
+
+  void Residual(cudaStream_t st) {   // E afresh from W, C and A
+    const qcnn::PqGeometry& geo = s->geo;
+    const int grid = static_cast<int>(std::min<size_t>((nw + 255) / 256, 32u * s->ctx->sm_count));
+    pqrc_residual_kernel<<<grid, 256, 0, st>>>(W.as<float>(), C.as<float>(), A.as<uint8_t>(), E.as<double>(), geo.Cout, geo.Cg, K,
+                                               s->d, geo.T);
+  }
+  int Loss(int sw, cudaStream_t st) {   // loss[sw] from E and GE
+    return LaunchLoss(E.as<double>(), GE.as<double>(), nw, part.as<double>(), loss.as<double>() + sw, st, P, TT);
+  }
+};
+
+// The set-up of the sweeps on s's current device: reserves the shared buffers, uploads the weights w (zeros for the
+// target form), the codebook and the assignments at, forms E, seeds GE per group and writes loss[0]
+inline int BeginSweeps(SweepState* ss, qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* w,
+                       std::vector<uint8_t>& at, const float* ctrd_h, const double* G, const double* P, const double* TT,
+                       cudaStream_t st) {
+  qcnn_ctx* ctx = s->ctx;
+  const qcnn::PqGeometry& geo = s->geo;
+  const int Cpg = geo.Cpg, Dg = geo.Dg;
+  const size_t nw = static_cast<size_t>(geo.Cout) * Dg, nc = static_cast<size_t>(qcnn::CeilDiv(geo.Cg, s->d)) * K * s->d;
+  ss->s = s;
+  ss->who = who;
+  ss->target = target;
+  ss->K = K;
+  ss->sweeps = sweeps;
+  ss->G = G;
+  ss->P = target ? P : nullptr;   // P = T^T Y
+  ss->TT = target ? TT : nullptr;
+  ss->at = &at;
+  ss->nw = nw;
+  ss->nc = nc;
+  if (Reserve(ctx, who, ss->E, sizeof(double) * nw, "the residual") ||
+      Reserve(ctx, who, ss->GE, sizeof(double) * nw, "G times the residual") ||
+      Reserve(ctx, who, ss->W, sizeof(float) * nw, "the weights") || Reserve(ctx, who, ss->C, sizeof(float) * nc, "the codebook") ||
+      Reserve(ctx, who, ss->A, at.size(), "the assignments") ||
+      Reserve(ctx, who, ss->part, sizeof(double) * kLossBlocks, "the loss") ||
+      Reserve(ctx, who, ss->loss, sizeof(double) * (sweeps + 1), "the loss"))
+    return 1;
+  QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
+  if (target) QCNN_CUDA(cudaMemsetAsync(ss->W.get(), 0, sizeof(float) * nw, st));   // E = 0 - W^
+  else QCNN_CUDA(cudaMemcpyAsync(ss->W.get(), w, sizeof(float) * nw, cudaMemcpyHostToDevice, st));
+  QCNN_CUDA(cudaMemcpyAsync(ss->C.get(), ctrd_h, sizeof(float) * nc, cudaMemcpyHostToDevice, st));
+  QCNN_CUDA(cudaMemcpyAsync(ss->A.get(), at.data(), at.size(), cudaMemcpyHostToDevice, st));
+  ss->Residual(st);
+  // GE = E G, or P + E G for a target
+  if (target) QCNN_CUDA(cudaMemcpyAsync(ss->GE.get(), P, sizeof(double) * nw, cudaMemcpyDeviceToDevice, st));
+  for (int g = 0; g < geo.grp; g++) {
+    const size_t ro = static_cast<size_t>(g) * Cpg * Dg;
+    pqr_gemm_kernel<kGemmF64><<<dim3(qcnn::CeilDiv(Dg, kTile), qcnn::CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
+        ss->E.as<double>() + ro, Dg, G + static_cast<size_t>(g) * Dg * Dg, Dg, ss->GE.as<double>() + ro, Dg, Cpg, Dg, Dg, target);
+  }
+  QCNN_CUDA(cudaGetLastError());
+  return ss->Loss(0, st);
+}
+
+// The end of the sweeps: with bias_h, E afresh from the final codebook and assignments (target: -W^) and the bias refit;
+// then the codebook, the assignments in the caller's layout [Cout][T][S] and the losses to the host
+inline int EndSweeps(SweepState& ss, float* ctrd_h, uint8_t* asmt_h, float* bias_h, double* loss_h, cudaStream_t st) {
+  if (bias_h) {
+    ss.Residual(st);
+    if (int rc = RefitBias(ss.s, ss.who, ss.target, ss.E.as<double>(), bias_h, st)) return rc;
+  }
+  const qcnn::PqGeometry& geo = ss.s->geo;
+  const int Cout = geo.Cout, T = geo.T, S = qcnn::CeilDiv(geo.Cg, ss.s->d);
+  std::vector<uint8_t>& at = *ss.at;
+  std::vector<double> lossv(ss.sweeps + 1);
+  QCNN_CUDA(cudaMemcpyAsync(ctrd_h, ss.C.get(), sizeof(float) * ss.nc, cudaMemcpyDeviceToHost, st));
+  QCNN_CUDA(cudaMemcpyAsync(at.data(), ss.A.get(), at.size(), cudaMemcpyDeviceToHost, st));
+  QCNN_CUDA(cudaMemcpyAsync(lossv.data(), ss.loss.get(), sizeof(double) * lossv.size(), cudaMemcpyDeviceToHost, st));
+  QCNN_CUDA(cudaStreamSynchronize(st));
+  for (int o = 0; o < Cout; o++)
+    for (int t = 0; t < T; t++)
+      for (int m = 0; m < S; m++) asmt_h[(static_cast<size_t>(o) * T + t) * S + m] = at[(static_cast<size_t>(m) * Cout + o) * T + t];
+  if (loss_h) std::copy(lossv.begin(), lossv.end(), loss_h);
+  return 0;
 }
 
 }  // namespace

@@ -35,27 +35,12 @@ using namespace qcnn;
 
 namespace {
 
-constexpr int kMaxD = 64;
 constexpr int kMaxSystem = 2048;                 // K w_m: the size of the joint codebook system
 constexpr int kCholBlock = 64;                   // panel width of the blocked Cholesky
 constexpr int kSolveThreads = 1024;
 constexpr int kNormalThreads = 128;
 constexpr int kAssignWarps = 8;
 constexpr size_t kRunBytes = size_t(256) << 20;     // an add folds its positions in runs of 2^28 / (4 Dg)
-
-// E[o][q] = W[o][q] - C[m][A[m][o][t]][j] in fp64 (A held [S][Cout][T])
-__global__ void pqrc_residual_kernel(const float* __restrict__ W, const float* __restrict__ C, const uint8_t* __restrict__ A,
-                                     double* __restrict__ E, int Cout, int Cg, int K, int d, int T) {
-  const int Dg = Cg * T;
-  const size_t total = static_cast<size_t>(Cout) * Dg;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int o = static_cast<int>(i / Dg);
-    const Dim q = DecodeDim(static_cast<int>(i % Dg), Cg, d, T);
-    const uint8_t a = A[(static_cast<size_t>(q.m) * Cout + o) * T + q.t];
-    E[i] = static_cast<double>(W[i]) - static_cast<double>(C[(static_cast<size_t>(q.m) * K + a) * d + q.j]);
-  }
-}
 
 // s[g][q] (accumulate: s[g][q] +) the sum over output positions (oy, then ox ascending) of the image sum `plane`
 // [Hin][Win][Cin] at the input pixel tap t of dim q reads, for every (g, q) (thread g Dg + q); a tap outside the map
@@ -421,34 +406,43 @@ __global__ void __launch_bounds__(kAssignWarps * 32) pqrc_assign_kernel(const do
   }
 }
 
-// The host-side checks of a refine (weights unless target, codebook, assignments), the assignments as [S][Cout][T] and
-// the weights [Cout][Cg][T] in the internal dim order [Cout][Dg]
-int CheckConvHost(const char* who, bool target, const PqConvGeometry& geo, int K, int d, const float* knl_h, const float* ctrd_h,
-                  const uint8_t* asmt_h, std::vector<uint8_t>& at, std::vector<float>& wp) {
-  const int Cout = geo.Cout, Cg = geo.Cg, T = geo.T, Dg = geo.Dg;
-  const int S = CeilDiv(Cg, d);
-  const size_t nw = static_cast<size_t>(Cout) * Dg, nc = static_cast<size_t>(S) * K * d;
-  if (!target) QCNN_CHECK(AllFinite(knl_h, nw), "%s: the weights contain a non-finite value", who);
-  QCNN_CHECK(AllFinite(ctrd_h, nc), "%s: the codebook contains a non-finite value", who);
-  at.assign(static_cast<size_t>(S) * Cout * T, 0);
-  for (int o = 0; o < Cout; o++)
-    for (int t = 0; t < T; t++)
-      for (int m = 0; m < S; m++) {
-        const uint8_t a = asmt_h[(static_cast<size_t>(o) * T + t) * S + m];
-        QCNN_CHECK(a < K, "%s: assignment %d of output %d, tap %d, subspace %d is not below K=%d", who, a, o, t, m, K);
-        at[(static_cast<size_t>(m) * Cout + o) * T + t] = a;
-      }
-  wp.assign(target ? 0 : nw, 0.0f);
-  for (int o = 0; o < (target ? 0 : Cout); o++)
-    for (int c = 0; c < Cg; c++) {
-      const int m = c / d, j = c % d, w = std::min(d, Cg - m * d);
-      for (int t = 0; t < T; t++)
-        wp[static_cast<size_t>(o) * Dg + m * d * T + t * w + j] = knl_h[(static_cast<size_t>(o) * Cg + c) * T + t];
-    }
+// The geometry checks of every conv entry point, then the derived sizes
+int CheckGeometry(const char* who, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, PqGeometry* geo) {
+  QCNN_CHECK(Cin >= 1 && Hin >= 1 && Win >= 1 && Cout >= 1 && ksz >= 1 && pad >= 0 && stride >= 1 && grp >= 1,
+             "%s: bad geometry (Cin=%d Hin=%d Win=%d Cout=%d ksz=%d pad=%d stride=%d grp=%d)", who, Cin, Hin, Win, Cout, ksz, pad,
+             stride, grp);
+  QCNN_CHECK(Cin % grp == 0 && Cout % grp == 0, "%s: Cin=%d and Cout=%d must be divisible by grp=%d", who, Cin, Cout, grp);
+  QCNN_CHECK(Hin + 2 * pad >= ksz && Win + 2 * pad >= ksz, "%s: empty output (%dx%d input, pad %d, kernel %d)", who, Hin, Win, pad, ksz);
+  geo->Cin = Cin; geo->Hin = Hin; geo->Win = Win; geo->Cout = Cout; geo->ksz = ksz; geo->pad = pad; geo->stride = stride; geo->grp = grp;
+  geo->Ho = (Hin + 2 * pad - ksz) / stride + 1;
+  geo->Wo = (Win + 2 * pad - ksz) / stride + 1;
+  geo->Cg = Cin / grp; geo->Cpg = Cout / grp; geo->T = ksz * ksz; geo->Dg = geo->Cg * geo->T;
   return 0;
 }
 
-// K and the joint-system limit
+// The one-shot calls' argument checks, the same for both forms and in the order of their messages
+int RefineConv(bool target, qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, int K,
+               int d, int sweeps, const float* knl_h, const float* x, const float* t, int N, float* ctrd_h, uint8_t* asmt_h,
+               double* loss_h, void* stream) {
+  const char* who = target ? "qcnn_pq_refine_conv_target" : "qcnn_pq_refine_conv";
+  QCNN_CHECK(ctx && (target || knl_h) && ctrd_h && asmt_h, "%s: NULL argument", who);
+  PqGeometry geo;
+  if (int rc = CheckGeometry(who, Cin, Hin, Win, Cout, ksz, pad, stride, grp, &geo)) return rc;
+  if (int rc = CheckConvK(who, K)) return rc;
+  QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
+  QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
+  QCNN_CHECK(N >= 1, "%s: N=%d: at least one input is needed", who, N);
+  QCNN_CHECK(x, "%s: NULL argument", who);
+  QCNN_CHECK(!target || t, "%s: NULL t", who);
+  if (int rc = CheckConvSystem(who, K, d, geo.Cg)) return rc;
+  return RefineOnce(ctx, who, true, target, geo, K, d, sweeps, knl_h, x, t, N, ctrd_h, asmt_h, loss_h,
+                    static_cast<cudaStream_t>(stream));
+}
+
+}  // namespace
+
+namespace qcnn {
+
 int CheckConvSystem(const char* who, int K, int d, int Cg) {
   if (int rc = CheckConvK(who, K)) return rc;
   const long long sys = static_cast<long long>(K) * std::min(d, Cg);
@@ -457,47 +451,32 @@ int CheckConvSystem(const char* who, int K, int d, int Cg) {
   return 0;
 }
 
-// The sweeps on the sums G, P and |T|^2 (those of s, or their centered copies).  target: the target form (wp is empty);
-// else the same-input form on the weights wp.  bias_h non-NULL: replaced by the refit bias (RefitBias).
-int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const std::vector<float>& wp, const double* G,
-              const double* P, const double* TT, std::vector<uint8_t>& at, float* ctrd_h, uint8_t* asmt_h, float* bias_h,
+// The conv sweeps: the subspaces the sweeps skip, then per subspace the responses, the joint codebook step, the
+// tap-ordered assignment and the update of GE
+int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wts, std::vector<uint8_t>& at,
+              const double* G, const double* P, const double* TT, float* ctrd_h, uint8_t* asmt_h, float* bias_h,
               double* loss_h, cudaStream_t st) {
   qcnn_ctx* ctx = s->ctx;
-  const PqConvGeometry& geo = s->geo;
+  const PqGeometry& geo = s->geo;
   const int d = s->d, Cout = geo.Cout, Cg = geo.Cg, Cpg = geo.Cpg, T = geo.T, Dg = geo.Dg, grp = geo.grp;
   const int S = CeilDiv(Cg, d), wmax = std::min(d, Cg);
-  const size_t nw = static_cast<size_t>(Cout) * Dg, nc = static_cast<size_t>(S) * K * d;
   QCNN_ON_DEVICE(ctx->device);
+  SweepState ss;
+  if (int rc = BeginSweeps(&ss, s, who, target, K, sweeps, wts, at, ctrd_h, G, P, TT, st)) return rc;
   const size_t nbMax = static_cast<size_t>(T) * wmax, nMax = static_cast<size_t>(K) * wmax;
-  DeviceBuffer dE, dGE, dW, dC, dA, dWh, dH, dDlt, dM, dF, dPt, dB, dMem, dOff, dUk, dNU, dCC, dPart, dLoss;
-  auto reserve = [&](DeviceBuffer& b, size_t bytes, const char* what) -> int {
-    const cudaError_t e = b.Reserve(ctx, bytes);
-    if (e == cudaSuccess) return 0;
-    cudaGetLastError();
-    SetError("%s: cannot allocate %zu bytes of device memory for %s (%s)", who, bytes, what, cudaGetErrorString(e));
+  DeviceBuffer dWh, dH, dDlt, dM, dF, dPt, dB, dMem, dOff, dUk, dNU, dCC;
+  if (Reserve(ctx, who, dWh, sizeof(double) * Cout * nbMax, "the decoded subspace") ||
+      Reserve(ctx, who, dH, sizeof(double) * Cout * nbMax, "the subspace responses") ||
+      Reserve(ctx, who, dDlt, sizeof(double) * Cout * nbMax, "the subspace's changes") ||
+      Reserve(ctx, who, dM, sizeof(double) * nMax * nMax, "the joint system") ||
+      Reserve(ctx, who, dF, sizeof(double) * nMax * nMax, "its Cholesky factor") ||
+      Reserve(ctx, who, dPt, sizeof(double) * kCholBlock * nMax, "the Cholesky panel") ||
+      Reserve(ctx, who, dB, sizeof(double) * nMax, "the right-hand side") ||
+      Reserve(ctx, who, dMem, sizeof(int) * grp * static_cast<size_t>(T) * Cpg, "the cluster members") ||
+      Reserve(ctx, who, dOff, sizeof(int) * grp * static_cast<size_t>(T) * (K + 1), "the cluster members") ||
+      Reserve(ctx, who, dUk, sizeof(int) * K, "the used clusters") || Reserve(ctx, who, dNU, sizeof(int), "the used clusters") ||
+      Reserve(ctx, who, dCC, sizeof(double) * grp * static_cast<size_t>(T) * K, "the codeword norms"))
     return 1;
-  };
-  if (reserve(dE, sizeof(double) * nw, "the residual") || reserve(dGE, sizeof(double) * nw, "G times the residual") ||
-      reserve(dW, sizeof(float) * nw, "the weights") || reserve(dC, sizeof(float) * nc, "the codebook") ||
-      reserve(dA, at.size(), "the assignments") ||
-      reserve(dWh, sizeof(double) * Cout * nbMax, "the decoded subspace") ||
-      reserve(dH, sizeof(double) * Cout * nbMax, "the subspace responses") ||
-      reserve(dDlt, sizeof(double) * Cout * nbMax, "the subspace's changes") ||
-      reserve(dM, sizeof(double) * nMax * nMax, "the joint system") ||
-      reserve(dF, sizeof(double) * nMax * nMax, "its Cholesky factor") ||
-      reserve(dPt, sizeof(double) * kCholBlock * nMax, "the Cholesky panel") || reserve(dB, sizeof(double) * nMax, "the right-hand side") ||
-      reserve(dMem, sizeof(int) * grp * static_cast<size_t>(T) * Cpg, "the cluster members") ||
-      reserve(dOff, sizeof(int) * grp * static_cast<size_t>(T) * (K + 1), "the cluster members") ||
-      reserve(dUk, sizeof(int) * K, "the used clusters") || reserve(dNU, sizeof(int), "the used clusters") ||
-      reserve(dCC, sizeof(double) * grp * static_cast<size_t>(T) * K, "the codeword norms") ||
-      reserve(dPart, sizeof(double) * kLossBlocks, "the loss") || reserve(dLoss, sizeof(double) * (sweeps + 1), "the loss"))
-    return 1;
-  if (!target) P = TT = nullptr;   // P = T^T Y
-  QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
-  if (target) QCNN_CUDA(cudaMemsetAsync(dW.get(), 0, sizeof(float) * nw, st));   // E = 0 - W^
-  else QCNN_CUDA(cudaMemcpyAsync(dW.get(), wp.data(), sizeof(float) * nw, cudaMemcpyHostToDevice, st));
-  QCNN_CUDA(cudaMemcpyAsync(dC.get(), ctrd_h, sizeof(float) * nc, cudaMemcpyHostToDevice, st));
-  QCNN_CUDA(cudaMemcpyAsync(dA.get(), at.data(), at.size(), cudaMemcpyHostToDevice, st));
   std::vector<double> diag(static_cast<size_t>(grp) * Dg);
   for (int g = 0; g < grp; g++)
     QCNN_CUDA(cudaMemcpy2DAsync(diag.data() + static_cast<size_t>(g) * Dg, sizeof(double), G + static_cast<size_t>(g) * Dg * Dg,
@@ -512,17 +491,6 @@ int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps,
     skip[m] = !(tr > 0.0);
   }
   const int tiles = CeilDiv(Dg, kTile);
-  const int ewBlocks = static_cast<int>(std::min<size_t>((nw + 255) / 256, 32u * ctx->sm_count));
-  pqrc_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Cout, Cg, K, d, T);
-  // GE = E G, or P + E G for a target
-  if (target) QCNN_CUDA(cudaMemcpyAsync(dGE.get(), P, sizeof(double) * nw, cudaMemcpyDeviceToDevice, st));
-  for (int g = 0; g < grp; g++) {
-    const size_t ro = static_cast<size_t>(g) * Cpg * Dg;
-    pqr_gemm_kernel<kGemmF64><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
-        dE.as<double>() + ro, Dg, G + static_cast<size_t>(g) * Dg * Dg, Dg, dGE.as<double>() + ro, Dg, Cpg, Dg, Dg, target);
-  }
-  QCNN_CUDA(cudaGetLastError());
-  if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>(), st, P, TT)) return rc;
   const size_t assignSmem = sizeof(double) * kAssignWarps * (kMaxD + (T + 1) / 2);
   if (assignSmem > 48 * 1024)
     QCNN_CUDA(cudaFuncSetAttribute(pqrc_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(assignSmem)));
@@ -533,8 +501,8 @@ int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps,
       const size_t nwb = static_cast<size_t>(Cout) * nb;
       const int gridB = static_cast<int>(std::min<size_t>((nwb + 255) / 256, 32u * ctx->sm_count));
       // responses h = GE[:, block] + W^_m G^m
-      pqrc_decode_kernel<<<gridB, 256, 0, st>>>(dC.as<float>(), dA.as<uint8_t>(), dGE.as<double>(), dWh.as<double>(), dH.as<double>(), m,
-                                                Cout, Dg, K, d, w, T, q0);
+      pqrc_decode_kernel<<<gridB, 256, 0, st>>>(ss.C.as<float>(), ss.A.as<uint8_t>(), ss.GE.as<double>(), dWh.as<double>(),
+                                                dH.as<double>(), m, Cout, Dg, K, d, w, T, q0);
       for (int g = 0; g < grp; g++) {
         const size_t ro = static_cast<size_t>(g) * Cpg * nb;
         const double* Gm = G + static_cast<size_t>(g) * Dg * Dg + static_cast<size_t>(q0) * Dg + q0;
@@ -542,7 +510,7 @@ int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps,
             dWh.as<double>() + ro, nb, Gm, Dg, dH.as<double>() + ro, nb, Cpg, nb, nb, 1);
       }
       // the used clusters and, per (g, t, k), their members
-      pqrc_lists_kernel<<<grp * T, 256, 0, st>>>(dA.as<uint8_t>(), dMem.as<int>(), dOff.as<int>(), m, Cout, Cpg, K, T);
+      pqrc_lists_kernel<<<grp * T, 256, 0, st>>>(ss.A.as<uint8_t>(), dMem.as<int>(), dOff.as<int>(), m, Cout, Cpg, K, T);
       pqrc_used_kernel<<<1, 256, 0, st>>>(dOff.as<int>(), dUk.as<int>(), dNU.as<int>(), grp * T, K);
       QCNN_CUDA(cudaGetLastError());
       int nU = 0;
@@ -551,10 +519,11 @@ int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps,
       const int n = nU * w;
       // codebook: M, b, the blocked Cholesky of M + mu I, the solve and the acceptance test
       const size_t nrmSmem = sizeof(double) * w * w + sizeof(int) * T;
-      pqrc_normal_kernel<<<dim3(nU, nU), kNormalThreads, nrmSmem, st>>>(G, dA.as<uint8_t>(), dMem.as<int>(), dOff.as<int>(),
+      pqrc_normal_kernel<<<dim3(nU, nU), kNormalThreads, nrmSmem, st>>>(G, ss.A.as<uint8_t>(), dMem.as<int>(), dOff.as<int>(),
                                                                         dUk.as<int>(), dM.as<double>(), m, grp, Cout, Cpg, Dg, K, T, w,
                                                                         q0, n);
-      pqrc_rhs_kernel<<<CeilDiv(n, 128), 128, 0, st>>>(dH.as<double>(), dA.as<uint8_t>(), dUk.as<int>(), dB.as<double>(), m, Cout, T, w, n);
+      pqrc_rhs_kernel<<<CeilDiv(n, 128), 128, 0, st>>>(dH.as<double>(), ss.A.as<uint8_t>(), dUk.as<int>(), dB.as<double>(), m, Cout,
+                                                       T, w, n);
       const int gridF = static_cast<int>(std::min<size_t>((static_cast<size_t>(n) * n + 255) / 256, 8u * ctx->sm_count));
       pqrc_ridge_kernel<<<gridF, 256, 0, st>>>(dM.as<double>(), dF.as<double>(), n);
       for (int kb = 0; kb < n; kb += kCholBlock) {
@@ -566,106 +535,30 @@ int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps,
         pqr_gemm_kernel<kGemmF64><<<dim3(CeilDiv(n2, kTile), CeilDiv(n2, kTile)), kGemmThreads, 0, st>>>(Fp, n, dPt.as<double>(), n,
                                                                                                          Fp + bw, n, n2, n2, bw, 1);
       }
-      pqrc_solve_kernel<<<1, kSolveThreads, 0, st>>>(dF.as<double>(), dM.as<double>(), dB.as<double>(), dUk.as<int>(), dC.as<float>(), m,
-                                                     K, d, w, n);
+      pqrc_solve_kernel<<<1, kSolveThreads, 0, st>>>(dF.as<double>(), dM.as<double>(), dB.as<double>(), dUk.as<int>(),
+                                                     ss.C.as<float>(), m, K, d, w, n);
       // assignment, tap by tap per output; then GE += Dlt G[block, :]
-      pqrc_ccost_kernel<<<grp * T, 256, 0, st>>>(G, dC.as<float>(), dCC.as<double>(), m, Dg, K, d, w, T, q0);
+      pqrc_ccost_kernel<<<grp * T, 256, 0, st>>>(G, ss.C.as<float>(), dCC.as<double>(), m, Dg, K, d, w, T, q0);
       pqrc_assign_kernel<<<CeilDiv(Cout, kAssignWarps), kAssignWarps * 32, assignSmem, st>>>(
-          G, dC.as<float>(), dCC.as<double>(), dH.as<double>(), dW.as<float>(), dA.as<uint8_t>(), dE.as<double>(),
+          G, ss.C.as<float>(), dCC.as<double>(), dH.as<double>(), ss.W.as<float>(), ss.A.as<uint8_t>(), ss.E.as<double>(),
           dDlt.as<double>(), m, Cout, Cpg, Dg, K, d, w, T, q0);
       for (int g = 0; g < grp; g++) {
         const double* Gb = G + static_cast<size_t>(g) * Dg * Dg + static_cast<size_t>(q0) * Dg;
         pqr_gemm_kernel<kGemmF64><<<dim3(tiles, CeilDiv(Cpg, kTile)), kGemmThreads, 0, st>>>(
-            dDlt.as<double>() + static_cast<size_t>(g) * Cpg * nb, nb, Gb, Dg, dGE.as<double>() + static_cast<size_t>(g) * Cpg * Dg, Dg,
-            Cpg, Dg, nb, 1);
+            dDlt.as<double>() + static_cast<size_t>(g) * Cpg * nb, nb, Gb, Dg, ss.GE.as<double>() + static_cast<size_t>(g) * Cpg * Dg,
+            Dg, Cpg, Dg, nb, 1);
       }
       QCNN_CUDA(cudaGetLastError());
     }
-    if (int rc = LaunchLoss(dE.as<double>(), dGE.as<double>(), nw, dPart.as<double>(), dLoss.as<double>() + sw, st, P, TT)) return rc;
+    if (int rc = ss.Loss(sw, st)) return rc;
   }
-  if (bias_h) {   // E = W - W^ (target: -W^) afresh from the final codebook and assignments
-    pqrc_residual_kernel<<<ewBlocks, 256, 0, st>>>(dW.as<float>(), dC.as<float>(), dA.as<uint8_t>(), dE.as<double>(), Cout, Cg, K, d, T);
-    if (int rc = RefitBias(s, who, target, dE.as<double>(), grp, Dg, Cout, bias_h, st)) return rc;
-  }
-  std::vector<double> lossv(sweeps + 1);
-  QCNN_CUDA(cudaMemcpyAsync(ctrd_h, dC.get(), sizeof(float) * nc, cudaMemcpyDeviceToHost, st));
-  QCNN_CUDA(cudaMemcpyAsync(at.data(), dA.get(), at.size(), cudaMemcpyDeviceToHost, st));
-  QCNN_CUDA(cudaMemcpyAsync(lossv.data(), dLoss.get(), sizeof(double) * lossv.size(), cudaMemcpyDeviceToHost, st));
-  QCNN_CUDA(cudaStreamSynchronize(st));
-  for (int o = 0; o < Cout; o++)
-    for (int t = 0; t < T; t++)
-      for (int m = 0; m < S; m++) asmt_h[(static_cast<size_t>(o) * T + t) * S + m] = at[(static_cast<size_t>(m) * Cout + o) * T + t];
-  if (loss_h) std::copy(lossv.begin(), lossv.end(), loss_h);
-  return 0;
+  return EndSweeps(ss, ctrd_h, asmt_h, bias_h, loss_h, st);
 }
-
-// The geometry checks of every conv entry point, then the derived sizes
-int CheckGeometry(const char* who, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, PqConvGeometry* geo) {
-  QCNN_CHECK(Cin >= 1 && Hin >= 1 && Win >= 1 && Cout >= 1 && ksz >= 1 && pad >= 0 && stride >= 1 && grp >= 1,
-             "%s: bad geometry (Cin=%d Hin=%d Win=%d Cout=%d ksz=%d pad=%d stride=%d grp=%d)", who, Cin, Hin, Win, Cout, ksz, pad,
-             stride, grp);
-  QCNN_CHECK(Cin % grp == 0 && Cout % grp == 0, "%s: Cin=%d and Cout=%d must be divisible by grp=%d", who, Cin, Cout, grp);
-  QCNN_CHECK(Hin + 2 * pad >= ksz && Win + 2 * pad >= ksz, "%s: empty output (%dx%d input, pad %d, kernel %d)", who, Hin, Win, pad, ksz);
-  geo->Cin = Cin; geo->Hin = Hin; geo->Win = Win; geo->Cout = Cout; geo->ksz = ksz; geo->pad = pad; geo->stride = stride; geo->grp = grp;
-  geo->Ho = (Hin + 2 * pad - ksz) / stride + 1;
-  geo->Wo = (Win + 2 * pad - ksz) / stride + 1;
-  geo->Cg = Cin / grp; geo->Cpg = Cout / grp; geo->T = ksz * ksz; geo->Dg = geo->Cg * geo->T;
-  return 0;
-}
-
-int CreateConv(qcnn_ctx* ctx, const char* who, const PqConvGeometry& geo, int d, bool target, bool sums, qcnn_pq_stats** out) {
-  std::unique_ptr<qcnn_pq_stats> s(new qcnn_pq_stats);
-  s->ctx = ctx;
-  s->conv = true;
-  s->target = target;
-  s->d = d;
-  s->geo = geo;
-  s->sums = sums;
-  const size_t inPlane = static_cast<size_t>(geo.Hin) * geo.Win * geo.Cin, outPlane = static_cast<size_t>(geo.Ho) * geo.Wo * geo.Cout;
-  if (AllocStats(s.get(), who, sizeof(double) * geo.grp * static_cast<size_t>(geo.Dg) * geo.Dg,
-                 sizeof(double) * geo.Cout * static_cast<size_t>(geo.Dg), sizeof(double) * geo.grp * static_cast<size_t>(geo.Dg),
-                 sizeof(double) * geo.Cout, sizeof(double) * (target ? std::max(inPlane, outPlane) : inPlane)))
-    return 1;
-  *out = s.release();
-  return 0;
-}
-
-// The one-shot calls: the checks both forms share (in the order of their messages), then create (without the first
-// moments, which they never read), one add of all N inputs, the sweeps and destroy
-int RefineConv(bool target, qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, int K,
-               int d, int sweeps, const float* knl_h, const float* x, const float* t, int N, float* ctrd_h, uint8_t* asmt_h,
-               double* loss_h, void* stream) {
-  const char* who = target ? "qcnn_pq_refine_conv_target" : "qcnn_pq_refine_conv";
-  QCNN_CHECK(ctx && (target || knl_h) && ctrd_h && asmt_h, "%s: NULL argument", who);
-  PqConvGeometry geo;
-  if (int rc = CheckGeometry(who, Cin, Hin, Win, Cout, ksz, pad, stride, grp, &geo)) return rc;
-  if (int rc = CheckConvK(who, K)) return rc;
-  QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
-  QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
-  QCNN_CHECK(N >= 1, "%s: N=%d: at least one input is needed", who, N);
-  QCNN_CHECK(x, "%s: NULL argument", who);
-  QCNN_CHECK(!target || t, "%s: NULL t", who);
-  if (int rc = CheckConvSystem(who, K, d, geo.Cg)) return rc;
-  std::vector<uint8_t> at;
-  std::vector<float> wp;
-  if (int rc = CheckConvHost(who, target, geo, K, d, knl_h, ctrd_h, asmt_h, at, wp)) return rc;
-  const cudaStream_t st = static_cast<cudaStream_t>(stream);
-  qcnn_pq_stats* sp = nullptr;
-  if (int rc = CreateConv(ctx, who, geo, d, target, false, &sp)) return rc;
-  std::unique_ptr<qcnn_pq_stats> s(sp);
-  if (int rc = ConvStatsAdd(s.get(), who, x, t, N, st)) return rc;
-  return SweepConv(s.get(), who, target, K, sweeps, wp, s->G.as<double>(), s->P.as<double>(), s->tt.as<double>(), at, ctrd_h,
-                   asmt_h, nullptr, loss_h, st);
-}
-
-}  // namespace
-
-namespace qcnn {
 
 // A conv add: the scan, then per group the positions in runs of F, each run's Gram (and cross product) read straight
 // from the maps and added in ascending order; then the first moments (s from the image sum of y, u from that of t)
 int ConvStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st) {
-  const PqConvGeometry& geo = s->geo;
+  const PqGeometry& geo = s->geo;
   const int Cout = geo.Cout, Cpg = geo.Cpg, Dg = geo.Dg, grp = geo.grp;
   const size_t positions = static_cast<size_t>(N) * geo.Ho * geo.Wo;
   unsigned first[2];
@@ -710,21 +603,6 @@ int ConvStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float*
   return 0;
 }
 
-int ConvStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* knl_h, float* ctrd_h,
-                    uint8_t* asmt_h, float* bias_h, double* loss_h, cudaStream_t st) {
-  if (int rc = CheckConvSystem(who, K, s->d, s->geo.Cg)) return rc;
-  std::vector<uint8_t> at;
-  std::vector<float> wp;
-  if (int rc = CheckConvHost(who, target, s->geo, K, s->d, knl_h, ctrd_h, asmt_h, at, wp)) return rc;
-  if (!bias_h)
-    return SweepConv(s, who, target, K, sweeps, wp, s->G.as<double>(), s->P.as<double>(), s->tt.as<double>(), at, ctrd_h, asmt_h,
-                     nullptr, loss_h, st);
-  CenteredSums c;
-  if (int rc = CenterSums(s, who, target, s->geo.grp, s->geo.Dg, s->geo.Cout, &c, st)) return rc;
-  return SweepConv(s, who, target, K, sweeps, wp, c.G.as<double>(), c.P.as<double>(), c.tt.as<double>(), at, ctrd_h, asmt_h,
-                   bias_h, loss_h, st);
-}
-
 }  // namespace qcnn
 
 extern "C" int qcnn_pq_refine_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride, int grp, int K,
@@ -746,8 +624,8 @@ extern "C" int qcnn_pq_stats_create_conv(qcnn_ctx* ctx, int Cin, int Hin, int Wi
   const char* who = "qcnn_pq_stats_create_conv";
   QCNN_CHECK(ctx && out, "%s: NULL argument", who);
   *out = nullptr;
-  PqConvGeometry geo;
+  PqGeometry geo;
   if (int rc = CheckGeometry(who, Cin, Hin, Win, Cout, ksz, pad, stride, grp, &geo)) return rc;
   QCNN_CHECK(d >= 1 && d <= kMaxD, "%s: d=%d is outside 1..%d", who, d, kMaxD);
-  return CreateConv(ctx, who, geo, d, target != 0, true, out);
+  return CreateStats(ctx, who, true, geo, d, target != 0, true, out);
 }

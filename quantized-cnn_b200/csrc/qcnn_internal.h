@@ -474,16 +474,25 @@ int OptInSmem(qcnn_ctx* ctx) {
 int CheckFcK(const char* who, int K);
 int CheckConvK(const char* who, int K);
 
-// pq_refine.cu / pq_refine_conv.cu: a conv layer's geometry as the error-correcting quantizer reads it, and the two
-// halves of the quantizer on a qcnn_pq_stats: folding a batch into the statistics, and the sweeps that read them
-struct PqConvGeometry { int Cin, Hin, Win, Cout, ksz, pad, stride, grp, Ho, Wo, Cg, Cpg, T, Dg; };
+// pq_refine.cu / pq_refine_conv.cu: a layer's geometry as the error-correcting quantizer reads it (an FC layer of Din
+// inputs and Dout outputs is the one-group 1x1 conv on a 1x1 map: Cg = Dg = Din, Cpg = Cout = Dout, T = Ho = Wo = 1),
+// and the halves of the quantizer on a qcnn_pq_stats: folding a batch into the statistics, and the sweeps that read them
+struct PqGeometry { int Cin, Hin, Win, Cout, ksz, pad, stride, grp, Ho, Wo, Cg, Cpg, T, Dg; };
 int FcStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st);
 int ConvStatsAdd(qcnn_pq_stats* s, const char* who, const float* y, const float* t, int N, cudaStream_t st);
-// bias_h non-NULL: the sweeps run on the centered sums and bias_h [Dout] / [Cout] is replaced by the refit bias
-int FcStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wei_h, float* ctrd_h,
-                  uint8_t* asmt_h, float* bias_h, double* loss_h, cudaStream_t st);
-int ConvStatsRefine(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* knl_h, float* ctrd_h,
-                    uint8_t* asmt_h, float* bias_h, double* loss_h, cudaStream_t st);
+// K and the joint-system limit of a conv refine
+int CheckConvSystem(const char* who, int K, int d, int Cg);
+// The conv sweeps on the sums G, P and |T|^2 (those of s, or their centered copies), from the weights wts in the internal
+// dim order (not read by the target form) and the assignments at [S][Cout][T].  bias_h non-NULL: replaced by the refit
+// bias.
+int SweepConv(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, const float* wts, std::vector<uint8_t>& at,
+              const double* G, const double* P, const double* TT, float* ctrd_h, uint8_t* asmt_h, float* bias_h,
+              double* loss_h, cudaStream_t st);
+// The one-shot calls after their own argument checks: check the start, create the statistics (without the first
+// moments, which they never read), one add of all N inputs, the sweeps, destroy
+int RefineOnce(qcnn_ctx* ctx, const char* who, bool conv, bool target, const PqGeometry& geo, int K, int d, int sweeps,
+               const float* w_h, const float* x, const float* t, int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h,
+               cudaStream_t st);
 
 // conv_ws.cu: the tensor-core family's weight-stationary tilings of stride-1 layers (mode-0 geometry, channel tiles) and
 // of strided narrow-input layers (mode-1 geometry)
@@ -533,10 +542,9 @@ inline bool PoolWindowsNonEmpty(int in, int pad, int ksz, int stride) {
 // stream of the last add, so a refine or a read waits for the queued accumulation.
 struct qcnn_pq_stats {
   qcnn_ctx* ctx = nullptr;
-  bool conv = false, target = false;
+  bool conv = false, target = false;   // conv: chooses the add and the sweep loop
   int d = 0;
-  int Din = 0, Dout = 0;          // FC
-  qcnn::PqConvGeometry geo{};     // conv
+  qcnn::PqGeometry geo{};
   long long images = 0;
   qcnn::DeviceBuffer G, P, tt;    // G [grp][Dg][Dg] (FC [Din][Din]); target: P [Cout][Dg] (FC [Dout][Din]) and |T|^2
   // first moments (with sums): sy = sum of y [grp][Dg] in the dim order of G (FC [Din]); target: su = sum of t [Cout]
