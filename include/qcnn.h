@@ -440,7 +440,27 @@ QCNN_API int qcnn_pq_refine_conv_target(qcnn_ctx* ctx, int Cin, int Hin, int Win
  * Skip rule of every sweep: a subspace (conv: a (group, tap) in the assignment step) is skipped when !(tr > 0) for the
  *   trace of its diagonal block, so a centered block with a rounding-level negative trace is skipped; on raw sums the
  *   trace is a sum of squares, so this is tr == 0.  A codeword solve that is not finite (a centered block that is
- *   singular at rounding level) fails the strict acceptance test and never enters the codebook. */
+ *   singular at rounding level) fails the strict acceptance test and never enters the codebook.
+ * refine_damped: the sweeps with a damping term that pulls the fit toward the original weights W (wei_h, fcntWei /
+ *   convKnl, required in both forms), minimising loss + sum_g lambda_g |W_g - W^_g|_F^2 over the groups g.  target = 0 runs
+ *   the same-input form on either kind of object, target = 1 the target form on a target object; bias_h NULL runs on the
+ *   raw sums, otherwise on the centered sums with the bias refit of refine_bias / refine_target_bias (the damping term
+ *   does not involve the bias, so its closed form is unchanged).  Base sums: the sums those calls' sweeps read.
+ *   Per group, on the base sums: tr_g = sum over i ascending of G_g[i][i] (fp64), lambda_g = damp (tr_g / Dg) with each
+ *   operation rounded, and lambda_g = 0 when !(tr_g > 0) (such a group is skipped as before); FC is one group, Dg = Din.
+ *   The sweeps run unchanged (skip rule, ridge, acceptance, ties, order) on damped copies formed elementwise with every
+ *   operation rounded (no contraction): G'_g[i][i] = G_g[i][i] + lambda_g, every other entry copied (so G' stays exactly
+ *   symmetric); target form: P'[o][q] = P[o][q] + lambda_g W[o][q] (W in the dim order above, g the group of output o)
+ *   and |T'|^2 = |T|^2 + (sum over g ascending of lambda_g |W_g|^2), |W_g|^2 the fixed-order fp64 sum of group g's squared
+ *   weights; |T'|^2 enters only the reported loss.  With lambda_g > 0 no subspace of group g has a zero trace, so a
+ *   subspace without input energy is no longer skipped: its codewords and assignments are fitted to W in the Euclidean
+ *   metric, which is what the damping term asks for.  loss_h = the damped objective (bias-optimal with bias_h): the
+ *   start's, then one value after each sweep.  damp = 0 gives the bits of refine, refine_target, refine_bias or
+ *   refine_target_bias, whichever matches.  Rejects what those calls reject, plus a NULL wei_h, damp < 0, NaN or Inf,
+ *   target not 0 or 1, target = 1 on a same-input object, and non-finite weights in either form; never changes the
+ *   statistics.  Device memory: that of the matching call plus the damped copies, 8 grp Dg^2 (+ 8 Cout Dg for the target
+ *   form) bytes, and for the target form 4 Cout Dg bytes of weights until the sweeps start; with bias_h the centered
+ *   copies are damped in place, so no more than refine_bias / refine_target_bias. */
 typedef struct qcnn_pq_stats qcnn_pq_stats;
 QCNN_API int qcnn_pq_stats_create_fc(qcnn_ctx* ctx, int Din, int Dout, int d, int target, qcnn_pq_stats** out);
 QCNN_API int qcnn_pq_stats_create_conv(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, int ksz, int pad, int stride,
@@ -461,6 +481,10 @@ QCNN_API int qcnn_pq_stats_refine_bias(qcnn_pq_stats* s, int K, int sweeps, cons
                                        uint8_t* asmt_h, float* bias_h, double* loss_h, void* stream);
 QCNN_API int qcnn_pq_stats_refine_target_bias(qcnn_pq_stats* s, int K, int sweeps, float* ctrd_h, uint8_t* asmt_h,
                                               float* bias_h, double* loss_h, void* stream);
+/* refine or refine_target (target = 0 / 1) with the weight anchor; bias_h nullable: with it, _bias's refit */
+QCNN_API int qcnn_pq_stats_refine_damped(qcnn_pq_stats* s, int target, double damp, int K, int sweeps,
+                                         const float* wei_h /* fcntWei or convKnl */, float* ctrd_h, uint8_t* asmt_h,
+                                         float* bias_h, double* loss_h, void* stream);
 QCNN_API void qcnn_pq_stats_destroy(qcnn_pq_stats* s);
 
 /* ---- file formats (include/FileIO.h:56-178, 229-350), host only ------------------------------------------- */

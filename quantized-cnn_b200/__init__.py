@@ -143,6 +143,7 @@ _SIGS = {
     "qcnn_pq_stats_read_sums_h": (_i, [_vp, _vp, _vp, C.POINTER(C.c_longlong)]),
     "qcnn_pq_stats_refine_bias": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "qcnn_pq_stats_refine_target_bias": (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "qcnn_pq_stats_refine_damped": (_i, [_vp, _i, C.c_double, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "qcnn_pq_stats_destroy": (None, [_vp]),
 }
 for _name, (_res, _args) in _SIGS.items():
@@ -772,8 +773,8 @@ class PqStats(object):
     of layer inputs y (and, with target=True, the original layer's responses t) into the sums the error-correcting
     refinement reads, so the calibration set can be streamed in batches; refine() / refine_target() then run the sweeps
     of pq_refine_* / pq_refine_*_target on the sums, any number of times; refine_bias() / refine_target_bias() also
-    refit the layer's bias, from the first moments read_sums() returns.  Device memory does not grow with the number of
-    images."""
+    refit the layer's bias, from the first moments read_sums() returns; refine_damped() runs either form, with or
+    without the bias, damped toward the dense weights.  Device memory does not grow with the number of images."""
 
     def __init__(self, ctx, h, conv, shape, target):
         self.ctx, self.h, self.conv, self.target = ctx, h, conv, target
@@ -857,9 +858,10 @@ class PqStats(object):
             raise QcnnError("ctrd [%d, K, %d] and asmt %s must be [S, K, d] and %s" % (S, g["d"], tuple(asmt.shape), want))
         return ctrd, asmt, K
 
-    def _refine(self, fn, ctrd, asmt, sweeps, stream, wei=_ABSENT, bias=_ABSENT):
-        """fn on the statistics from the start (ctrd, asmt), with the dense weights and the bias when the call takes
-        them: (ctrd, asmt, loss), or (ctrd, asmt, bias, loss) with a bias."""
+    def _refine(self, fn, ctrd, asmt, sweeps, stream, wei=_ABSENT, bias=_ABSENT, lead=()):
+        """fn(h, *lead, K, sweeps, ...) on the statistics from the start (ctrd, asmt), with the dense weights and the
+        bias when the call takes them (bias None: a NULL bias): (ctrd, asmt, loss), or (ctrd, asmt, bias, loss) with a
+        bias."""
         self._live()
         ctrd, asmt, K = self._start(ctrd, asmt)
         args = []
@@ -869,14 +871,16 @@ class PqStats(object):
                 raise QcnnError("wei must be %s, got %s" % (self._shape["wei"], wei.shape))
             args.append(wei.ctypes.data_as(_vp))
         args += [ctrd.ctypes.data_as(_vp), asmt.ctypes.data_as(_vp)]
-        if bias is not _ABSENT:
+        if bias is None:
+            args.append(None)
+        elif bias is not _ABSENT:
             bias = np.array(bias, np.float32, order="C", copy=True)
             if bias.shape != (self._shape["outputs"],):
                 raise QcnnError("bias must be (%d,), got %s" % (self._shape["outputs"], bias.shape))
             args.append(bias.ctypes.data_as(_vp))
         loss = np.empty(max(sweeps, 0) + 1, np.float64)
-        _check(fn(self.h, K, sweeps, *args, loss.ctypes.data_as(_vp), _stream(stream)))
-        return (ctrd, asmt, loss) if bias is _ABSENT else (ctrd, asmt, bias, loss)
+        _check(fn(self.h, *lead, K, sweeps, *args, loss.ctypes.data_as(_vp), _stream(stream)))
+        return (ctrd, asmt, loss) if bias is _ABSENT or bias is None else (ctrd, asmt, bias, loss)
 
     def refine(self, wei, ctrd, asmt, sweeps=8, stream=None):
         """The same-input sweeps (pq_refine_fc / pq_refine_conv) on the statistics and the dense weights wei
@@ -898,6 +902,15 @@ class PqStats(object):
         """refine_target() with the bias free as well: (ctrd, asmt, bias, loss [sweeps + 1]).  The arguments are not
         modified."""
         return self._refine(lib.qcnn_pq_stats_refine_target_bias, ctrd, asmt, sweeps, stream, bias=bias)
+
+    def refine_damped(self, wei, ctrd, asmt, damp, target=False, bias=None, sweeps=8, stream=None):
+        """refine() (target=False) or refine_target() (target=True, a target object) with a damping term that pulls the
+        fit toward the dense weights wei: the loss plus lambda_g |W_g - W^_g|^2 per group, lambda_g = damp tr(G_g) / Dg
+        (include/qcnn.h).  With bias [Dout] / [Cout] the bias is refit as by refine_bias() / refine_target_bias().
+        Returns (ctrd, asmt, loss [sweeps + 1]), or (ctrd, asmt, bias, loss) with a bias, loss the damped objective;
+        damp = 0 gives the undamped call's bits.  The arguments are not modified."""
+        return self._refine(lib.qcnn_pq_stats_refine_damped, ctrd, asmt, sweeps, stream, wei=wei, bias=bias,
+                            lead=(int(bool(target)), float(damp)))
 
     @property
     def nbytes(self):

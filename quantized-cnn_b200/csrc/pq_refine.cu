@@ -319,13 +319,20 @@ int Refine(qcnn_ctx* ctx, bool target, int Din, int Dout, int K, int d, int swee
   return RefineOnce(ctx, who, false, target, FcGeometry(Din, Dout), K, d, sweeps, w_h, x, t, N, ctrd_h, asmt_h, loss_h, st);
 }
 
-// The sweeps of s's kind on its sums, or with bias_h on their centered copies and followed by the bias refit
-int Sweep(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, Start& start, float* ctrd_h, uint8_t* asmt_h,
-          float* bias_h, double* loss_h, cudaStream_t st) {
+// The sweeps of s's kind on its sums, or with bias_h on their centered copies and followed by the bias refit; with
+// damp > 0 on the damped copies of those (damp = 0: on them as they are)
+int Sweep(qcnn_pq_stats* s, const char* who, bool target, int K, int sweeps, Start& start, double damp, float* ctrd_h,
+          uint8_t* asmt_h, float* bias_h, double* loss_h, cudaStream_t st) {
   const double *G = s->G.as<double>(), *P = s->P.as<double>(), *TT = s->tt.as<double>();
   CenteredSums c;
   if (bias_h) {
     if (int rc = CenterSums(s, who, target, &c, st)) return rc;
+    G = c.G.as<double>();
+    P = c.P.as<double>();
+    TT = c.tt.as<double>();
+  }
+  if (damp > 0.0) {
+    if (int rc = DampSums(s, who, target, damp, start.w, G, P, TT, &c, st)) return rc;
     G = c.G.as<double>();
     P = c.P.as<double>();
     TT = c.tt.as<double>();
@@ -368,12 +375,12 @@ int RefineOnce(qcnn_ctx* ctx, const char* who, bool conv, bool target, const PqG
                const float* w_h, const float* x, const float* t, int N, float* ctrd_h, uint8_t* asmt_h, double* loss_h,
                cudaStream_t st) {
   Start start;
-  if (int rc = CheckStart(who, conv, target, geo, K, d, w_h, ctrd_h, asmt_h, &start)) return rc;
+  if (int rc = CheckStart(who, conv, geo, K, d, w_h, ctrd_h, asmt_h, &start)) return rc;
   qcnn_pq_stats* sp = nullptr;
   if (int rc = CreateStats(ctx, who, conv, geo, d, target, false, &sp)) return rc;
   std::unique_ptr<qcnn_pq_stats> s(sp);
   if (int rc = conv ? ConvStatsAdd(s.get(), who, x, t, N, st) : FcStatsAdd(s.get(), who, x, t, N, st)) return rc;
-  return Sweep(s.get(), who, target, K, sweeps, start, ctrd_h, asmt_h, nullptr, loss_h, st);
+  return Sweep(s.get(), who, target, K, sweeps, start, 0.0, ctrd_h, asmt_h, nullptr, loss_h, st);
 }
 
 }  // namespace qcnn
@@ -442,41 +449,54 @@ extern "C" int qcnn_pq_stats_read_sums_h(const qcnn_pq_stats* s, double* s_h, do
 
 namespace {
 
-// bias: the bias calls, which also need bias_h (finite, [Cout]); without it the sweeps run on the raw sums
-int RefineStats(qcnn_pq_stats* s, const char* who, bool target, bool bias, int K, int sweeps, const float* wei_h, float* ctrd_h,
-                uint8_t* asmt_h, float* bias_h, double* loss_h, void* stream) {
-  QCNN_CHECK(s && (target || wei_h) && ctrd_h && asmt_h && (!bias || bias_h), "%s: NULL argument", who);
+// bias: the bias calls, which also need bias_h (finite, [Cout]); without it the sweeps run on the raw sums.  damped: the
+// damped call, which needs the weights in both forms and a finite damp >= 0 (the others pass damp = 0).
+int RefineStats(qcnn_pq_stats* s, const char* who, bool target, bool bias, bool damped, double damp, int K, int sweeps,
+                const float* wei_h, float* ctrd_h, uint8_t* asmt_h, float* bias_h, double* loss_h, void* stream) {
+  QCNN_CHECK(s && ((target && !damped) || wei_h) && ctrd_h && asmt_h && (!bias || bias_h), "%s: NULL argument", who);
   QCNN_CHECK(!target || s->target, "%s: the statistics were created without a target", who);
   QCNN_CHECK(s->images > 0, "%s: no calibration data has been added", who);
   QCNN_CHECK(sweeps >= 0, "%s: sweeps=%d is negative", who, sweeps);
+  if (damped) QCNN_CHECK(isfinite(damp) && damp >= 0.0, "%s: damp=%g is not a finite number >= 0", who, damp);
   if (bias) QCNN_CHECK(AllFinite(bias_h, s->geo.Cout), "%s: the bias contains a non-finite value", who);
   if (int rc = s->conv ? CheckConvSystem(who, K, s->d, s->geo.Cg) : CheckFcK(who, K)) return rc;
   Start start;
-  if (int rc = CheckStart(who, s->conv, target, s->geo, K, s->d, wei_h, ctrd_h, asmt_h, &start)) return rc;
-  return Sweep(s, who, target, K, sweeps, start, ctrd_h, asmt_h, bias ? bias_h : nullptr, loss_h, static_cast<cudaStream_t>(stream));
+  if (int rc = CheckStart(who, s->conv, s->geo, K, s->d, wei_h, ctrd_h, asmt_h, &start)) return rc;
+  return Sweep(s, who, target, K, sweeps, start, damp, ctrd_h, asmt_h, bias ? bias_h : nullptr, loss_h,
+               static_cast<cudaStream_t>(stream));
 }
 
 }  // namespace
 
 extern "C" int qcnn_pq_stats_refine(qcnn_pq_stats* s, int K, int sweeps, const float* wei_h, float* ctrd_h, uint8_t* asmt_h,
                                     double* loss_h, void* stream) {
-  return RefineStats(s, "qcnn_pq_stats_refine", false, false, K, sweeps, wei_h, ctrd_h, asmt_h, nullptr, loss_h, stream);
+  return RefineStats(s, "qcnn_pq_stats_refine", false, false, false, 0.0, K, sweeps, wei_h, ctrd_h, asmt_h, nullptr, loss_h,
+                     stream);
 }
 
 extern "C" int qcnn_pq_stats_refine_target(qcnn_pq_stats* s, int K, int sweeps, float* ctrd_h, uint8_t* asmt_h, double* loss_h,
                                            void* stream) {
-  return RefineStats(s, "qcnn_pq_stats_refine_target", true, false, K, sweeps, nullptr, ctrd_h, asmt_h, nullptr, loss_h, stream);
+  return RefineStats(s, "qcnn_pq_stats_refine_target", true, false, false, 0.0, K, sweeps, nullptr, ctrd_h, asmt_h, nullptr,
+                     loss_h, stream);
 }
 
 extern "C" int qcnn_pq_stats_refine_bias(qcnn_pq_stats* s, int K, int sweeps, const float* wei_h, float* ctrd_h, uint8_t* asmt_h,
                                          float* bias_h, double* loss_h, void* stream) {
-  return RefineStats(s, "qcnn_pq_stats_refine_bias", false, true, K, sweeps, wei_h, ctrd_h, asmt_h, bias_h, loss_h, stream);
+  return RefineStats(s, "qcnn_pq_stats_refine_bias", false, true, false, 0.0, K, sweeps, wei_h, ctrd_h, asmt_h, bias_h, loss_h,
+                     stream);
 }
 
 extern "C" int qcnn_pq_stats_refine_target_bias(qcnn_pq_stats* s, int K, int sweeps, float* ctrd_h, uint8_t* asmt_h,
                                                 float* bias_h, double* loss_h, void* stream) {
-  return RefineStats(s, "qcnn_pq_stats_refine_target_bias", true, true, K, sweeps, nullptr, ctrd_h, asmt_h, bias_h, loss_h,
-                     stream);
+  return RefineStats(s, "qcnn_pq_stats_refine_target_bias", true, true, false, 0.0, K, sweeps, nullptr, ctrd_h, asmt_h, bias_h,
+                     loss_h, stream);
+}
+
+extern "C" int qcnn_pq_stats_refine_damped(qcnn_pq_stats* s, int target, double damp, int K, int sweeps, const float* wei_h,
+                                           float* ctrd_h, uint8_t* asmt_h, float* bias_h, double* loss_h, void* stream) {
+  const char* who = "qcnn_pq_stats_refine_damped";
+  QCNN_CHECK(target == 0 || target == 1, "%s: target=%d is not 0 or 1", who, target);
+  return RefineStats(s, who, target != 0, bias_h != nullptr, true, damp, K, sweeps, wei_h, ctrd_h, asmt_h, bias_h, loss_h, stream);
 }
 
 extern "C" void qcnn_pq_stats_destroy(qcnn_pq_stats* s) {

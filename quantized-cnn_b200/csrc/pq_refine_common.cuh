@@ -489,6 +489,7 @@ __global__ void pqr_bias_delta_kernel(const double* __restrict__ E, const double
 }
 
 // The centered copies of a stats object's sums: G [grp][Dg][Dg] always, P [Cout][Dg] and |T_c|^2 for the target form
+// (DampSums also damps them in place, or holds its damped copies of the raw sums here)
 struct CenteredSums {
   qcnn::DeviceBuffer G, P, tt;
 };
@@ -513,6 +514,91 @@ inline int CenterSums(qcnn_pq_stats* s, const char* who, bool target, CenteredSu
     pqr_center_tt_kernel<<<1, 1, 0, st>>>(s->tt.as<double>(), su, Dout, n, c->tt.as<double>());
   }
   QCNN_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---- damping toward the original weights (DESIGN.md 4e, "Damping toward the original weights")
+
+constexpr int kTraceChunk = 1024;   // diagonal entries staged per step of pqr_damp_lambda_kernel
+
+// Per group g (blockIdx.x): lam[g] = damp (tr_g / Dg), tr_g = the sum over i ascending of G_g[i][i], every operation
+// rounded; 0 when !(tr_g > 0).  The block stages the strided diagonal in chunks, thread 0 adds them in order.
+__global__ void __launch_bounds__(kSweepThreads) pqr_damp_lambda_kernel(const double* __restrict__ G, int Dg, double damp,
+                                                                        double* __restrict__ lam) {
+  __shared__ double diag[kTraceChunk];
+  const double* Gg = G + static_cast<size_t>(blockIdx.x) * Dg * Dg;
+  double tr = 0.0;
+  for (int i0 = 0; i0 < Dg; i0 += kTraceChunk) {
+    const int n = min(kTraceChunk, Dg - i0);
+    for (int i = threadIdx.x; i < n; i += kSweepThreads) diag[i] = Gg[static_cast<size_t>(i0 + i) * (Dg + 1)];
+    __syncthreads();
+    if (threadIdx.x == 0)
+      for (int i = 0; i < n; i++) tr = __dadd_rn(tr, diag[i]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) lam[blockIdx.x] = tr > 0.0 ? __dmul_rn(damp, __ddiv_rn(tr, static_cast<double>(Dg))) : 0.0;
+}
+
+// The damped copies, elementwise with every operation rounded; X and out may be the same array.
+//   W NULL:  the diagonals, out[g][i][i] = X[g][i][i] + lam[g] over rows = grp Dg entries (rpg = Dg, cols = Dg).
+//   else:    out[o][q] = X[o][q] + lam[o / rpg] W[o][q] over rows = Cout outputs of cols = Dg dims (rpg = Cpg).
+__global__ void pqr_damp_kernel(const double* X, const float* __restrict__ W, const double* __restrict__ lam, size_t rows,
+                                size_t cols, size_t rpg, double* out) {
+  const size_t total = W ? rows * cols : rows;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    if (W) {
+      out[i] = __dadd_rn(X[i], __dmul_rn(lam[i / cols / rpg], static_cast<double>(W[i])));
+    } else {
+      const size_t e = (i / rpg) * rpg * cols + (i % rpg) * (cols + 1);   // group i / Dg, diagonal entry i % Dg
+      out[e] = __dadd_rn(X[e], lam[i / rpg]);
+    }
+  }
+}
+
+// *ttd = *tt + sum over g ascending of lam[g] wsq[g], every operation rounded (*ttd may be *tt)
+__global__ void pqr_damp_tt_kernel(const double* tt, const double* __restrict__ lam, const double* __restrict__ wsq, int grp,
+                                   double* ttd) {
+  double acc = 0.0;
+  for (int g = 0; g < grp; g++) acc = __dadd_rn(acc, __dmul_rn(lam[g], wsq[g]));
+  *ttd = __dadd_rn(*tt, acc);
+}
+
+// The damped copies of the sums G, P and TT the sweeps would otherwise read (the statistics' own, or c's centered
+// copies): per group lam_g from G's trace, G' = G + lam_g I, and for the target form P' = P + lam_g W (g the output's
+// group) and |T'|^2 = |T|^2 + sum_g lam_g |W_g|^2, w_h the host weights [Cout][Dg] in the internal dim order.  They are
+// written to c: in place when the base sums are c's, otherwise into c's buffers, reserved here.  Synchronises st.
+inline int DampSums(qcnn_pq_stats* s, const char* who, bool target, double damp, const float* w_h, const double* G,
+                    const double* P, const double* TT, CenteredSums* c, cudaStream_t st) {
+  qcnn_ctx* ctx = s->ctx;
+  const int grp = s->geo.grp, D = s->geo.Dg, Dout = s->geo.Cout, Cpg = s->geo.Cpg;
+  const size_t gn = static_cast<size_t>(grp) * D * D, pn = static_cast<size_t>(Dout) * D;
+  qcnn::DeviceBuffer scratch, dW;   // lam [grp], |W_g|^2 [grp], the |W_g|^2 partials [kLossBlocks]; the weights
+  if (Reserve(ctx, who, c->G, sizeof(double) * gn, "the damped Gram matrices") ||
+      Reserve(ctx, who, c->P, target ? sizeof(double) * pn : 0, "the damped cross product") ||
+      Reserve(ctx, who, c->tt, target ? sizeof(double) : 0, "the damped targets' norm") ||
+      Reserve(ctx, who, scratch, sizeof(double) * (2 * grp + kLossBlocks), "the damping weights") ||
+      Reserve(ctx, who, dW, target ? sizeof(float) * pn : 0, "the weights"))
+    return 1;
+  QCNN_ON_DEVICE(ctx->device);
+  QCNN_CUDA(cudaStreamWaitEvent(st, s->done, 0));
+  double *lam = scratch.as<double>(), *wsq = lam + grp, *part = wsq + grp;
+  auto grid = [&](size_t total) { return static_cast<int>(std::min<size_t>((total + 255) / 256, 32u * ctx->sm_count)); };
+  pqr_damp_lambda_kernel<<<grp, kSweepThreads, 0, st>>>(G, D, damp, lam);
+  double* Gd = c->G.as<double>();
+  if (Gd != G) QCNN_CUDA(cudaMemcpyAsync(Gd, G, sizeof(double) * gn, cudaMemcpyDeviceToDevice, st));
+  pqr_damp_kernel<<<grid(static_cast<size_t>(grp) * D), 256, 0, st>>>(Gd, nullptr, lam, static_cast<size_t>(grp) * D, D, D, Gd);
+  QCNN_CUDA(cudaGetLastError());
+  if (target) {
+    QCNN_CUDA(cudaMemcpyAsync(dW.get(), w_h, sizeof(float) * pn, cudaMemcpyHostToDevice, st));
+    pqr_damp_kernel<<<grid(pn), 256, 0, st>>>(P, dW.as<float>(), lam, Dout, D, Cpg, c->P.as<double>());
+    for (int g = 0; g < grp; g++)
+      if (int rc = LaunchSqNorm(dW.as<float>() + static_cast<size_t>(g) * Cpg * D, static_cast<size_t>(Cpg) * D, part, wsq + g, 0,
+                                st))
+        return rc;
+    pqr_damp_tt_kernel<<<1, 1, 0, st>>>(TT, lam, wsq, grp, c->tt.as<double>());
+    QCNN_CUDA(cudaGetLastError());
+  }
+  QCNN_CUDA(cudaStreamSynchronize(st));   // scratch and dW are freed on return
   return 0;
 }
 
@@ -541,21 +627,21 @@ bool AllFinite(const float* v, size_t n) {
 }
 
 // A refine's start as the sweeps read it: at, the assignments [Cout][T][S] as [S][Cout][T], and w, the weights
-// [Cout][Cg][T] in the internal dim order (NULL for the target form): the caller's own array when T == 1, where the
-// two orders agree, else the permuted copy wp
+// [Cout][Cg][T] in the internal dim order (NULL when the call takes none; the target form reads them only to damp P):
+// the caller's own array when T == 1, where the two orders agree, else the permuted copy wp
 struct Start {
   std::vector<uint8_t> at;
   std::vector<float> wp;
   const float* w = nullptr;
 };
 
-// The host-side checks of a refine (weights unless target, codebook, assignments; the FC message names no tap), then
-// the start
-inline int CheckStart(const char* who, bool conv, bool target, const qcnn::PqGeometry& geo, int K, int d, const float* w_h,
+// The host-side checks of a refine (weights when given, codebook, assignments; the FC message names no tap), then
+// the start.  Both forms go through the same checks: the target calls pass w_h NULL, the damped call its anchor.
+inline int CheckStart(const char* who, bool conv, const qcnn::PqGeometry& geo, int K, int d, const float* w_h,
                       const float* ctrd_h, const uint8_t* asmt_h, Start* start) {
   const int Cout = geo.Cout, Cg = geo.Cg, T = geo.T, Dg = geo.Dg, S = qcnn::CeilDiv(Cg, d);
   const size_t nw = static_cast<size_t>(Cout) * Dg, nc = static_cast<size_t>(S) * K * d;
-  if (!target) QCNN_CHECK(AllFinite(w_h, nw), "%s: the weights contain a non-finite value", who);
+  if (w_h) QCNN_CHECK(AllFinite(w_h, nw), "%s: the weights contain a non-finite value", who);
   QCNN_CHECK(AllFinite(ctrd_h, nc), "%s: the codebook contains a non-finite value", who);
   start->at.assign(static_cast<size_t>(S) * Cout * T, 0);
   for (int o = 0; o < Cout; o++)
@@ -566,8 +652,8 @@ inline int CheckStart(const char* who, bool conv, bool target, const qcnn::PqGeo
         QCNN_CHECK(a < K, "%s: assignment %d of output %d, tap %d, subspace %d is not below K=%d", who, a, o, t, m, K);
         start->at[(static_cast<size_t>(m) * Cout + o) * T + t] = a;
       }
-  start->w = target ? nullptr : w_h;
-  if (target || T == 1) return 0;
+  start->w = w_h;
+  if (!w_h || T == 1) return 0;
   start->wp.resize(nw);
   for (int o = 0; o < Cout; o++)
     for (int c = 0; c < Cg; c++) {

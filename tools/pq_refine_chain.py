@@ -19,13 +19,19 @@ With --stats the calibration images stream through in batches of --batch: per la
 (and for the target mode the original network's responses t) are added to a PqStats object and dropped, and the
 refinement runs on the accumulated statistics (qcnn_pq_stats_refine / _refine_target), so no layer's inputs or targets
 are ever held whole and device memory does not grow with --train.  Each call time is then the accumulation plus the
-refinement, printed with the peak device memory of that layer and mode (torch's peak allocation plus the statistics).
+refinement, printed with the peak device memory of that layer and mode (torch's peak allocation plus the statistics;
+the buffers the library allocates for the refine call itself are not included).
 With --stats --bias two more modes run, same-input+bias and target+bias: the same refinements with the bias refit as
 well (qcnn_pq_stats_refine_bias / _refine_target_bias on the centered statistics).  Each saves its refit bias into its
 own model, so the next layer's inputs come from the corrected network; their training loss ratios are of the
 bias-optimal losses.
+With --stats --damp R [R ...] each value adds the mode target+damp=R (and with --bias also target+bias+damp=R): the
+target refinement damped toward the original weights (qcnn_pq_stats_refine_damped, lambda_g = R tr(G_g) / Dg); their
+training loss ratios are of the damped losses.
+--modes M [M ...] runs only those of the modes above (each mode's chain depends on no other mode), so that a large
+--train can be split over several runs.
     python tools/pq_refine_chain.py [--train 4096] [--held 1024] [--sweeps 4] [--conv 32 8] [--fc8 16 4] [--stats]
-                                    [--bias] [--out f.json]"""
+                                    [--bias] [--damp R [R ...]] [--modes M [M ...]] [--out f.json]"""
 import argparse
 import importlib
 import json
@@ -125,10 +131,11 @@ class LcgImages(object):
         return out
 
 
-def refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc, target, bias=None):
+def refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc, target, bias=None, damp=None):
     """Accumulate layer l's statistics over the calibration images batch by batch (inputs from `net`, targets from the
     original network), then refine on them: (ctrd, asmt, bias, loss, seconds in the adds and the refine, peak device
-    bytes).  bias: the layer's bias, refit with the codebook and assignments (else returned as None)."""
+    bytes).  bias: the layer's bias, refit with the codebook and assignments (else returned as None).  damp: the
+    refinement damped toward W with this weight."""
     import torch
     conv = W.ndim == 4
     d = c0.shape[2]
@@ -155,7 +162,11 @@ def refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc, targ
         del imgs, y, t
     t0 = time.perf_counter()
     b = None
-    if bias is not None and target:
+    if damp is not None:
+        r = st.refine_damped(W, c0, a0, damp, target=target, bias=bias, sweeps=args.sweeps)
+        c, a, loss = r[0], r[1], r[-1]
+        b = r[2] if bias is not None else None
+    elif bias is not None and target:
         c, a, b, loss = st.refine_target_bias(c0, a0, bias, sweeps=args.sweeps)
     elif bias is not None:
         c, a, b, loss = st.refine_bias(W, c0, a0, bias, sweeps=args.sweeps)
@@ -183,10 +194,26 @@ def main():
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
     ap.add_argument("--stats", action="store_true", help="stream the calibration images through PqStats objects")
     ap.add_argument("--bias", action="store_true", help="with --stats: also the modes that refit each layer's bias")
+    ap.add_argument("--damp", nargs="+", default=[], metavar="R",
+                    help="with --stats: also target+damp=R (and with --bias target+bias+damp=R) for each R")
+    ap.add_argument("--modes", nargs="+", default=None, metavar="M", help="run only these modes")
     args = ap.parse_args()
     if args.bias and not args.stats:
         ap.error("--bias needs --stats (the bias refit runs on calibration statistics)")
-    modes = MODES + (BIAS_MODES if args.bias else ())
+    if args.damp and not args.stats:
+        ap.error("--damp needs --stats (the damped refinement runs on calibration statistics)")
+    damp_of = {}   # mode: its damping weight
+    for r in args.damp:
+        damp_of["target+damp=" + r] = float(r)
+        if args.bias:
+            damp_of["target+bias+damp=" + r] = float(r)
+    modes = MODES + (BIAS_MODES if args.bias else ()) + tuple(damp_of)
+    if args.modes:
+        unknown = sorted(set(args.modes) - set(modes))
+        if unknown:
+            ap.error("--modes: %s not among %s" % (", ".join(unknown), ", ".join(modes)))
+        modes = tuple(m for m in modes if m in args.modes)
+    width = max([15] + [len(m) for m in modes])
     import torch
     from oracle import pyoracle as po
     assert torch.cuda.is_available(), "needs a GPU"
@@ -229,7 +256,8 @@ def main():
                     net = net_of(mode)
                     c, a, b, loss, secs, peak = refine_streamed(q, po, ctx, args, orig, net, l, L, W, c0, a0, first_fc,
                                                                 mode.startswith("target"),
-                                                                params[l]["bias"] if mode in BIAS_MODES else None)
+                                                                params[l]["bias"] if "+bias" in mode else None,
+                                                                damp_of.get(mode))
                     net.close()
                     ratio = float(loss[-1] / loss[0])
                 elif mode != "kmeans":
@@ -252,8 +280,9 @@ def main():
                 qparams[mode][l] = dict(bias=params[l]["bias"] if b is None else b, ctrd=c, asmt=a, bits=po.bits_for(K))
                 rows.append(dict(layer=NAMES[l], K=K, d=d, mode=mode, loss_ratio=ratio, call_s=secs, peak_bytes=peak))
                 if ratio is not None:
-                    print("%-6s K=%-3d d=%-2d %-15s training loss x%.4f  call %.2f s%s"
-                          % (NAMES[l], K, d, mode, ratio, secs, "" if peak is None else "  peak %.2f GB" % (peak / 1e9)))
+                    print("%-6s K=%-3d d=%-2d %-*s training loss x%.4f  call %.2f s%s"
+                          % (NAMES[l], K, d, width, mode, ratio, secs,
+                             "" if peak is None else "  peak %.2f GB" % (peak / 1e9)))
             del t
             torch.cuda.empty_cache()
         orig.close()
@@ -269,8 +298,8 @@ def main():
             agree5 = (lg.topk(5, 1).indices == top1[:, None]).any(1).double().mean().item()
             summary.append(dict(mode=mode, logit_rel_err=err, logit_rel_err_median=med, top1_agree=agree1,
                                 top5_agree=agree5))
-            print("%-15s held-out logits relative error %.4f (per image, median %.4f)  top-1 agreement %.4f  "
-                  "top-5 agreement %.4f" % (mode, err, med, agree1, agree5))
+            print("%-*s held-out logits relative error %.4f (per image, median %.4f)  top-1 agreement %.4f  "
+                  "top-5 agreement %.4f" % (width, mode, err, med, agree1, agree5))
     if args.out:
         with open(args.out, "w") as f:
             json.dump(dict(card=hw, train=args.train, held=args.held, sweeps=args.sweeps, stats=args.stats, layers=rows,
