@@ -33,7 +33,7 @@ constexpr ConvFamily kFamilies[kConvKernelIds] = {
     {"conv_direct", kFp32Lut, 8, LaunchLutGather, DescribeLutGather},
     {nullptr, kGemm, 0, nullptr, nullptr},   // 5: retired
     {"pq_gemm_tc", kGemm, 6, LaunchPqGemm, DescribePqGemm},
-    {"pq_gemm_tc_ws(weight-stationary wgmma, weights decoded once per CTA into shared memory, bf16x2)", kGemm, 6, LaunchConvWs,
+    {"pq_gemm_tc_ws(weight-stationary wgmma, weights decoded once per layer and bulk-copied into shared memory, bf16x2)", kGemm, 6, LaunchConvWs,
      DescribeConvWs},
 };
 
@@ -76,12 +76,13 @@ int PlanConv(qcnn_layer* L, int N) {
     keepIf([&](const ConvPlan& c) { return kFamilies[c.kernel].cls == want; });
   }
   // layer parameters "gemm_nt" / "gemm_gt" / "gemm_nsplit": only pq_gemm_tc tilings with that many positions per CTA,
-  // k-steps per stage and K-split factor (0 = any); "gemm_nt" also restricts the positions per CTA of conv_ws, and
-  // "gemm_ct" its channels per CTA
+  // k-steps per stage and K-split factor (0 = any); "gemm_nt" and "gemm_gt" also restrict the positions per CTA and the
+  // k-steps per weight stage of conv_ws, and "gemm_ct" its channels per CTA
   if (L->opt_gemm_nt || L->opt_gemm_gt || L->opt_gemm_nsplit || L->opt_gemm_ct) {
     keepIf([L](const ConvPlan& c) {
       if (c.kernel == kConvWs)
-        return (!L->opt_gemm_nt || c.ws.P == L->opt_gemm_nt) && (!L->opt_gemm_ct || c.ws.NC == L->opt_gemm_ct);
+        return (!L->opt_gemm_nt || c.ws.P == L->opt_gemm_nt) && (!L->opt_gemm_gt || c.ws.KS == L->opt_gemm_gt) &&
+               (!L->opt_gemm_ct || c.ws.NC == L->opt_gemm_ct);
       const GemmArgs& g = c.g;
       return c.kernel != kPqGemmTc || ((!L->opt_gemm_nt || g.NT == L->opt_gemm_nt) && (!L->opt_gemm_gt || g.GT == L->opt_gemm_gt) &&
                                        (!L->opt_gemm_nsplit || g.nsplit == L->opt_gemm_nsplit));

@@ -12,8 +12,10 @@
 // A = positions: bf16x2 planes (x = x1 + x2; K-core-matrix 0 in the x1 plane, 1 in the x2 plane: LBO = plane distance),
 //     read by descriptor.
 // B = decoded weights in shared memory, N = the channels of one CTA: Cout / grp, or a 1/nct tile of it (any instantiated
-//     width up to 256: no channel padding).  Per k-step, [w1 | w1] and [w2 | w2] are 16-byte rows per channel; the
-//     duplicated half is the same core matrix read twice (LBO = 0).  Two MMAs per k-step into one accumulator:
+//     width up to 256: no channel padding).  They are decoded once per layer, at its creation, into the weight image
+//     qcnn_layer::d_w_ws (conv_ws_image_kernel below), and a CTA streams them into a ring of nWB stage buffers by bulk
+//     copy.  Per k-step, [w1 | w1] and [w2 | w2] are 16-byte rows per channel; the duplicated half is the same core
+//     matrix read twice (LBO = 0).  Two MMAs per k-step into one accumulator:
 //     [x1|x2].[w1|w1] + [x1|x2].[w2|w2] = (x1 + x2)(w1 + w2), the same k-steps in the same order as pq_gemm_tc's one-
 //     accumulator tiling of the same geometry (the error bound depends on that chain, DESIGN.md 2).
 //
@@ -21,10 +23,9 @@
 //   warps 0-7   two consumer warpgroups; each owns MB m64 blocks of the CTA's 128 MB positions and issues
 //               wgmma.mma_async (both operands in shared memory) into MB accumulators of N / 2 registers per thread.
 //   warps 8-11  producers: stage the position planes (global -> bf16x2 split -> planes; mode 1: every phase row resident,
-//               mode 0: a ring of plane buffers, one chunk each, with a full / empty mbarrier pair per buffer), and decode
-//               the weights of one stage (<= KS k-steps of one chunk, all N channels) from the pre-split codebook and the
-//               channel-major index block into one of two weight buffers.  The decode is done once per CTA and reused by
-//               both warpgroups and every m64 block; decoded weights never reach global memory.
+//               mode 0: a ring of plane buffers, one chunk each, with a full / empty mbarrier pair per buffer).  One
+//               producer thread also fills the weight ring: a stage (<= KS k-steps of one chunk, all N channels) is one
+//               bulk copy from the image (nct > 1: one per k-step and piece), counted on the buffer's full mbarrier.
 //   epilogue    the consumers add the bias (+ ReLU) and store pairs of consecutive channels of one NHWC pixel.
 #include "qcnn_internal.h"
 #include "wgmma.h"
@@ -37,7 +38,6 @@
 
 namespace {
 
-using qcnn::ByteOf32;
 using qcnn::kWsConsumers;
 using qcnn::kWsProducers;
 using qcnn::kWsThreads;
@@ -50,30 +50,20 @@ constexpr int kWsRegPos = 8;        // mode 0: float4 of a chunk's planes a prod
 constexpr int kWsRegItems1 = 12;    // mode 1: float4 of a phase row's planes a producer thread holds (st * NPOS <= 1536)
 constexpr int kNoRow = -(1 << 30);  // mode 1: input row of an item that stages zeros in every phase row
 
-// byte t (< 48) of the 48 bytes r[0..2] held in registers: a channel's index row of one phase row (t is warp-uniform:
-// selects, no local memory)
-__device__ __forceinline__ int ByteOf48(const uint4 (&r)[3], int t) {
-  const uint4 q = (t & 32) ? r[2] : (t & 16) ? r[1] : r[0];
-  const uint32_t xy = (t & 4) ? q.y : q.x, zw = (t & 4) ? q.w : q.z;
-  const uint32_t v = (t & 8) ? zw : xy;
-  return static_cast<int>((v >> ((t & 3) * 8)) & 0xFFu);
-}
-
 // Shared-memory carve, read by the planner (fits / does not fit) and by the kernel.  The channel count is computed as
 // Kg / nct rather than read from NC: reading NC changed the kernels' register allocation.
 struct WsSmem {  // byte offsets inside the dynamic shared memory
-  int planes, wts, cb, outoff, bias, bars, total;
+  int planes, wts, outoff, bias, bars, total;
 };
 __host__ __device__ inline WsSmem MapWsSmem(const ConvWsArgs& a) {
   const int nc = a.Kg / a.nct;
   WsSmem m;
   int o = 0;
   m.planes = o; o += a.nPB * 2 * a.planeRows * 16;        // [buffer][x1, x2][planeRows] 16-byte rows
-  m.wts = o;    o += 2 * a.KS * 2 * nc * 16;              // [buffer][k-step][w1, w2][channel] 16-byte rows
-  m.cb = o;     o += (a.stride == 1 ? 2 : 1) * a.K * 16;  // pre-split codebook slices {w1, w2} (stride 1: one per half)
+  m.wts = o;    o += a.nWB * a.KS * 2 * nc * 16;          // [buffer][k-step][w1, w2][channel] 16-byte rows (bulk-copy targets)
   m.outoff = o; o += a.P * 4;                             // destination element offset of every position (-1: none)
   m.bias = o;   o += nc * 4;                              // (nc is a multiple of 16: the barriers stay 8-byte aligned)
-  m.bars = o;   o += 8 * (2 * a.nPB + 4);
+  m.bars = o;   o += 8 * (2 * a.nPB + 2 * a.nWB);
   m.total = o;
   return m;
 }
@@ -87,17 +77,16 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const ConvWsArgs
   extern __shared__ __align__(128) unsigned char smem[];
   const WsSmem sm = MapWsSmem(a);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int KS = a.KS, nPB = a.nPB;
+  const int KS = a.KS, nPB = a.nPB, nWB = a.nWB;
   const int nCh = S1 ? a.nChunks : a.stride;   // chunks: 8-channel groups (mode 0) / phase rows (mode 1)
   uint4* planes = reinterpret_cast<uint4*>(smem + sm.planes);
   uint4* wts = reinterpret_cast<uint4*>(smem + sm.wts);
-  uint4* cb = reinterpret_cast<uint4*>(smem + sm.cb);
   int* outoff = reinterpret_cast<int*>(smem + sm.outoff);
   float* biasS = reinterpret_cast<float*>(smem + sm.bias);
   uint64_t* fullP = reinterpret_cast<uint64_t*>(smem + sm.bars);   // [nPB] planes of a chunk staged: producers -> consumers
   uint64_t* emptyP = fullP + nPB;                                   // [nPB] (mode 0) planes' MMAs retired: consumers -> producers
-  uint64_t* fullW = emptyP + nPB;                                   // [2] weight buffer decoded: producers -> consumers
-  uint64_t* emptyW = fullW + 2;                                     // [2] weight buffer's MMAs retired: consumers -> producers
+  uint64_t* fullW = emptyP + nPB;                                   // [nWB] weight stage copied: bulk copy -> consumers
+  uint64_t* emptyW = fullW + nWB;                                   // [nWB] weight stage's MMAs retired: consumers -> producer
   int bi = blockIdx.x;
   const int ct = bi % a.nct; bi /= a.nct;   // (channel tile, group, position tile)
   const int g = bi % a.G, tile = bi / a.G;
@@ -113,23 +102,48 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const ConvWsArgs
     const int ho = rem / a.PW, wo = rem - ho * a.PW;
     outoff[p] = (i < a.N && ho < a.Ho && wo < a.Wo) ? (((i - i0) * a.Ho + ho) * a.Wo + wo) * a.Cout : -1;
   }
-  if (!S1)
-    for (int k = tid; k < a.K; k += kWsThreads) cb[k] = __ldg(a.ctrd + k);
   for (int c = tid; c < NC; c += kWsThreads) biasS[c] = __ldg(a.bias + g * a.Kg + ch0 + c);
-  if (tid == 0) qcnn::WsInitBarriers(fullP, emptyP, nPB, kWsProducers, fullW, emptyW);
+  if (tid == 0) {
+    for (int i = 0; i < nPB; i++) { qcnn::MbarInit(fullP + i, kWsProducers); qcnn::MbarInit(emptyP + i, kWsConsumers / 32); }
+    for (int i = 0; i < nWB; i++) { qcnn::MbarInit(fullW + i, 1); qcnn::MbarInit(emptyW + i, kWsConsumers / 32); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
   __syncthreads();
 
   const int warpU = __shfl_sync(0xffffffffu, warp, 0);   // provably warp-uniform role selector
   if (warpU >= kWsConsumers / 32) {
     // =========================== producers ===========================
     const int pt = tid - kWsConsumers;
-    int j = 0;   // weight stage counter (buffer j & 1)
+    // the weight ring, filled by producer thread 0: stage jI = k-steps [s0I, + KS) of chunk kcI into buffer jI % nWB, once
+    // the MMAs of stage jI - nWB have retired.  The image holds [grp][entry][w1, w2][Kg] 16-byte rows, an entry being a
+    // k-step of the layer (mode 0: chunk x tap, mode 1: the k-step table's order); a stage's entries are consecutive.
+    const int nE = S1 ? nCh * a.kt.ntab : a.kt.ntab;
+    int jI = 0, kcI = 0, s0I = 0;
+    auto issueStage = [&]() {
+      const int cnt = S1 ? a.kt.ntab : a.kt.chunkCount[kcI];
+      const int n = min(KS, cnt - s0I), b = jI % nWB;
+      if (jI >= nWB) MbarWait<24>(emptyW + b, ((jI / nWB) - 1) & 1);
+      const uint32_t bytes = static_cast<uint32_t>(n * 2 * NC * 16);
+      qcnn::MbarExpectTx(fullW + b, bytes);
+      uint4* w = wts + b * KS * 2 * NC;
+      const int e0 = (S1 ? kcI * a.kt.ntab : a.kt.chunkFirst[kcI]) + s0I;
+      const uint4* src = a.wimg + (static_cast<size_t>(g) * nE + e0) * 2 * a.Kg + ch0;
+      if (a.nct == 1) {
+        qcnn::BulkLoad(w, src, bytes, fullW + b);   // (NC = Kg: the stage's rows are contiguous in the image)
+      } else {
+        for (int r = 0; r < 2 * n; r++) qcnn::BulkLoad(w + r * NC, src + static_cast<size_t>(r) * a.Kg, NC * 16, fullW + b);
+      }
+      jI++;
+      s0I += KS;
+      if (s0I >= cnt) { s0I = 0; kcI++; }
+    };
+    if (pt == 0)   // the first stages are in flight before any position is loaded
+      while (jI < nWB && kcI < nCh) issueStage();
     if constexpr (S1) {
       // float4 p = pt + (q * kWsRegPos + i) * kWsProducers of pass q of a chunk's planes: half = p / NPOS (channels 0-3 /
       // 4-7 of the chunk), position = p % NPOS -> pixel (r - pad, c - pad) of image i of the flat padded grid.  The 2 NPOS
       // float4 of a chunk take nPass register passes; the source offsets and validity of a pass are chunk-invariant
       // (computed once with a single pass, per pass otherwise)
-      const int taps = a.kt.ntab;
       const int nPass = WIDE ? (2 * a.NPOS + kWsRegPos * kWsProducers - 1) / (kWsRegPos * kWsProducers) : 1;
       const float* srcBase = a.src + static_cast<size_t>(i0) * a.srcImg + g * a.Cg;
       int poff[kWsRegPos];
@@ -215,50 +229,12 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const ConvWsArgs
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // planes are read by the tensor core
         MbarArrive(fullP + pb);
-        if (kc + 1 < nCh) {   // in flight during the decode below
+        if (kc + 1 < nCh) {   // in flight during the weight copies below
           if (nPass > 1) passPos(0);
           loadPos(kc + 1);
         }
-        // the chunk's two 4-channel halves: subspace and piece of each (as pq_gemm_tc's fetchChunk); a half beyond the
-        // group's channels gets a zero codebook slice (its positions are zeros too)
-        const int chA = kc * 8, chB = chA + 4;
-        const bool okB = chB < a.Cg;
-        const int sA = chA / a.d, jA = chA - sA * a.d;
-        const int sB = okB ? chB / a.d : 0, jB = okB ? chB - sB * a.d : 0;
-        const uint4* cA = a.ctrd + static_cast<size_t>(sA * (a.d >> 2) + (jA >> 2)) * a.K;
-        const uint4* cB = a.ctrd + static_cast<size_t>(sB * (a.d >> 2) + (jB >> 2)) * a.K;
-        qcnn::WsProducerSync();   // every producer is done decoding from the previous chunk's slices
-        for (int k = pt; k < a.K; k += kWsProducers) {
-          cb[k] = __ldg(cA + k);
-          cb[a.K + k] = okB ? __ldg(cB + k) : make_uint4(0u, 0u, 0u, 0u);
-        }
-        qcnn::WsProducerSync();
-        // weights of the chunk's stages: a thread owns channel c, its tap indices of either half are one or two 16-byte
-        // granules of the channel-major block d_asmt_t ([grp][S][KgPad][tapsPad])
-        const uint8_t* rowA = a.asmtT + (static_cast<size_t>(g * a.S + sA) * a.KgPad + ch0) * a.tapsPad;
-        const uint8_t* rowB = a.asmtT + (static_cast<size_t>(g * a.S + sB) * a.KgPad + ch0) * a.tapsPad;
-        for (int s0 = 0; s0 < taps; s0 += KS, j++) {
-          const int n = min(KS, taps - s0), b = j & 1;
-          if (j >= 2) MbarWait<24>(emptyW + b, ((j >> 1) - 1) & 1);   // buffer last read by the MMAs of stage j - 2
-          uint4* w = wts + b * KS * 2 * NC;
-          for (int c = pt; c < NC; c += kWsProducers) {
-            const uint4* iA = reinterpret_cast<const uint4*>(rowA + static_cast<size_t>(c) * a.tapsPad);
-            const uint4* iB = reinterpret_cast<const uint4*>(rowB + static_cast<size_t>(c) * a.tapsPad);
-            const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
-            const uint4 a0 = __ldg(iA), a1 = a.tapsPad > 16 ? __ldg(iA + 1) : zero;
-            const uint4 b0 = __ldg(iB), b1 = a.tapsPad > 16 ? __ldg(iB + 1) : zero;
-            // (no unroll pragma: see the mode-1 decode loop below)
-            for (int e = 0; e < n; e++) {
-              const int t = a.kt.tab[s0 + e].idx0;   // the tap of k-step s0 + e
-              const uint4 qa = cb[ByteOf32(a0, a1, t)];
-              const uint4 qb = cb[a.K + ByteOf32(b0, b1, t)];
-              w[(2 * e + 0) * NC + c] = make_uint4(qa.x, qa.y, qb.x, qb.y);   // [w1 of half A | w1 of half B]
-              w[(2 * e + 1) * NC + c] = make_uint4(qa.z, qa.w, qb.z, qb.w);   // [w2 of half A | w2 of half B]
-            }
-          }
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          MbarArrive(fullW + b);
-        }
+        if (pt == 0)
+          while (kcI <= kc) issueStage();   // the chunk's stages not issued yet
       }
       return;
     }
@@ -299,21 +275,6 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const ConvWsArgs
     };
     loadRow(0);
     for (int ph = 0; ph < st; ph++) {
-      // a thread owns channel c (pt, then pt + 128 when NC > 128): its index row of the phase row is [tapsPad] bytes of
-      // d_asmt_t, held in registers as three 16-byte granules (the first channel's in flight during the planes' split);
-      // longer rows (more than 48 taps per phase row, e.g. 11 x 11 / 2) are read byte by byte at each k-step
-      const uint8_t* idxB = a.asmtT + static_cast<size_t>(g * st + ph) * a.KgPad * a.tapsPad;
-      const uint4* idx = reinterpret_cast<const uint4*>(idxB);
-      const bool longRow = a.tapsPad > 48;
-      const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
-      auto idxRow = [&](int c, uint4 (&r)[3]) {
-        const uint4* row = idx + c * (a.tapsPad >> 4);
-        r[0] = __ldg(row);
-        r[1] = a.tapsPad > 16 ? __ldg(row + 1) : zero;
-        r[2] = a.tapsPad > 32 ? __ldg(row + 2) : zero;
-      };
-      uint4 ixA[3] = {zero, zero, zero};
-      if (pt < NC) idxRow(pt, ixA);
       // planes of phase row ph: item p -> pixel (r*stride + ph - pad, c*stride + pw - pad) of its image (zero outside);
       // plane row = (pair of phase columns, position), the parity of pw selects the half
       char* x1 = reinterpret_cast<char*>(planes + ph * 2 * a.planeRows);
@@ -331,30 +292,9 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const ConvWsArgs
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // planes are read by the tensor core
       MbarArrive(fullP + ph);
-      if (ph + 1 < st) loadRow(ph + 1);   // in flight during the decode below
-      // weights of the phase row's stages
-      const int first = a.kt.chunkFirst[ph], cnt = a.kt.chunkCount[ph];
-      for (int s0 = 0; s0 < cnt; s0 += KS, j++) {
-        const int n = min(KS, cnt - s0), b = j & 1;
-        if (j >= 2) MbarWait<24>(emptyW + b, ((j >> 1) - 1) & 1);   // buffer last read by the MMAs of stage j - 2
-        uint4* w = wts + b * KS * 2 * NC;
-        for (int c = pt; c < NC; c += kWsProducers) {
-          uint4 ix[3] = {ixA[0], ixA[1], ixA[2]};
-          if (c != pt) idxRow(c, ix);
-          const uint8_t* rowB = idxB + static_cast<size_t>(c) * a.tapsPad;
-          // (no unroll pragma here: under `#pragma unroll 3` the compiled loop was seen running an iteration with e == n
-          // for n = 8 on the device, writing past the weight buffer into the codebook / offset regions)
-          for (int e = 0; e < n; e++) {
-            const KStep ks = a.kt.tab[first + s0 + e];
-            const uint4 q0 = cb[longRow ? __ldg(rowB + ks.idx0) : ByteOf48(ix, ks.idx0)];
-            const uint4 q1 = ks.cb1 ? zero : cb[longRow ? __ldg(rowB + ks.idx1) : ByteOf48(ix, ks.idx1)];   // unpaired tap: zero half
-            w[(2 * e + 0) * NC + c] = make_uint4(q0.x, q0.y, q1.x, q1.y);   // [w1 of half 0 | w1 of half 1]
-            w[(2 * e + 1) * NC + c] = make_uint4(q0.z, q0.w, q1.z, q1.w);   // [w2 of half 0 | w2 of half 1]
-          }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        MbarArrive(fullW + b);
-      }
+      if (ph + 1 < st) loadRow(ph + 1);   // in flight during the weight copies below
+      if (pt == 0)
+        while (kcI <= ph) issueStage();   // the phase row's stages not issued yet
     }
     return;
   }
@@ -376,8 +316,8 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const ConvWsArgs
     const uint32_t plA = planes0 + static_cast<uint32_t>(pb * 2 * a.planeRows) * 16u + static_cast<uint32_t>(wg * MB * 64) * 16u;
     const int first = S1 ? 0 : a.kt.chunkFirst[kc], cnt = S1 ? a.kt.ntab : a.kt.chunkCount[kc];
     for (int s0 = 0; s0 < cnt; s0 += KS, j++) {
-      const int n = min(KS, cnt - s0), b = j & 1;
-      MbarWait<24>(fullW + b, (j >> 1) & 1);
+      const int n = min(KS, cnt - s0), b = j % nWB;
+      MbarWait<24>(fullW + b, (j / nWB) & 1);
       qcnn::WgmmaFence();
       for (int e = 0; e < n; e++) {
         const KStep ks = a.kt.tab[first + s0 + e];
@@ -438,21 +378,126 @@ int LaunchWidth(const ConvWsArgs& a, unsigned nb, size_t smem, cudaStream_t st, 
 
 bool WsWidth(int w) { return std::find(std::begin(kWsWidths), std::end(kWsWidths), w) != std::end(kWsWidths); }
 
+// The weight image of a layer (qcnn_layer::d_w_ws), [grp][entry][w1, w2][Kg] 16-byte rows: one thread per (group, entry,
+// channel) writes the entry's rows [w1 of half 0 | w1 of half 1] and [w2 of half 0 | w2 of half 1] of the channel from
+// the pre-split codebook (d_ctrd_bf) and the channel-major index block (d_asmt_t).  These are the rows that conv_ws
+// stages for the k-step, so its MMAs read the same bits as pq_gemm_tc's decoders produce.
+struct WsImageArgs {
+  const uint4* ctrd;
+  const uint8_t* asmtT;
+  uint4* img;
+  int G, Kg, KgPad, S, K, d, Cg, stride, tapsPad, nE;   // nE: entries per group
+  KStepTable kt;                                        // Mode0Table / Mode1Table (only the index fields are read)
+};
+
+__global__ void conv_ws_image_kernel(const WsImageArgs a) {
+  const long long total = static_cast<long long>(a.G) * a.nE * a.Kg;
+  const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(i % a.Kg);
+    const long long r = i / a.Kg;
+    const int e = static_cast<int>(r % a.nE), g = static_cast<int>(r / a.nE);
+    uint4 q0, q1;
+    if (a.stride == 1) {
+      // entry = (chunk kc of 8 input channels, tap t); the chunk's two 4-channel halves: subspace and piece of each (as
+      // pq_gemm_tc's fetchChunk); a half beyond the group's channels is zero (its positions are zeros too)
+      const int taps = a.kt.ntab, kc = e / taps, t = e - kc * taps;
+      const int chA = kc * 8, chB = chA + 4;
+      const int sA = chA / a.d, jA = chA - sA * a.d;
+      const int iA = a.asmtT[(static_cast<size_t>(g * a.S + sA) * a.KgPad + c) * a.tapsPad + t];
+      q0 = a.ctrd[static_cast<size_t>(sA * (a.d >> 2) + (jA >> 2)) * a.K + iA];
+      q1 = zero;
+      if (chB < a.Cg) {
+        const int sB = chB / a.d, jB = chB - sB * a.d;
+        const int iB = a.asmtT[(static_cast<size_t>(g * a.S + sB) * a.KgPad + c) * a.tapsPad + t];
+        q1 = a.ctrd[static_cast<size_t>(sB * (a.d >> 2) + (jB >> 2)) * a.K + iB];
+      }
+    } else {
+      // entry = k-step e of the table, in phase row ph: its taps' indices are bytes idx0 / idx1 of the channel's row of
+      // the phase row; an unpaired tap's second half is zero
+      int ph = 0;
+      while (ph + 1 < a.stride && e >= a.kt.chunkFirst[ph + 1]) ph++;
+      const KStep ks = a.kt.tab[e];
+      const uint8_t* row = a.asmtT + (static_cast<size_t>(g * a.stride + ph) * a.KgPad + c) * a.tapsPad;
+      q0 = a.ctrd[row[ks.idx0]];
+      q1 = ks.cb1 ? zero : a.ctrd[row[ks.idx1]];
+    }
+    uint4* o = a.img + static_cast<size_t>(g * a.nE + e) * 2 * a.Kg + c;
+    o[0] = make_uint4(q0.x, q0.y, q1.x, q1.y);      // [w1 of half 0 | w1 of half 1]
+    o[a.Kg] = make_uint4(q0.z, q0.w, q1.z, q1.w);   // [w2 of half 0 | w2 of half 1]
+  }
+}
+
+// mode 1: staged positions per phase plane for P positions per CTA (P + the taps' reach in phase rows and columns)
+int StridedNpos(const qcnn_layer* L, int P) {
+  const int st = L->stride, PWp = qcnn::CeilDiv(L->Win + 2 * L->pad, st);
+  return qcnn::RoundUp(P + ((L->ksz - 1) / st) * (PWp + 1), 8);
+}
+
+// A strided layer's tile of P positions: a phase row's planes in one register pass of the producers, and source offsets
+// relative to the CTA's first image in int
+bool StridedTileFits(const qcnn_layer* L, int P) {
+  const int st = L->stride, NPOS = StridedNpos(L, P);
+  const int IB = qcnn::CeilDiv(L->Hin + 2 * L->pad, st) * qcnn::CeilDiv(L->Win + 2 * L->pad, st);
+  return st * NPOS <= kWsRegItems1 * kWsProducers &&
+         static_cast<double>(qcnn::CeilDiv(NPOS, IB) + 1) * L->Hin * L->Win * L->Cin <= 2.0e9;
+}
+
+// The conditions of conv_ws that depend on the layer alone (not on the batch, the operand format or the source layout):
+// the layers that get a weight image.  Stride 1: those of pq_gemm_tc mode 0 (or <= 3 channels per group) with at most
+// 32 taps per channel-major index row.  Strided: those of its mode 1 over <= 4 input channels, an instantiated width,
+// and a tile height whose phase row fits one register pass.
+bool WsLayerTakes(const qcnn_layer* L) {
+  const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, st = L->stride, taps = L->ksz * L->ksz;
+  if (L->kind != QCNN_KIND_CONV || L->K < 1 || L->K > 256) return false;
+  if (st == 1) {
+    return L->d % 4 == 0 && (Cg <= 3 || (Cg % 4 == 0 && L->Cin % 4 == 0)) && L->S * L->d >= Cg && taps <= kMaxKSteps &&
+           L->asmt_t_mode == 0 && qcnn::RoundUp(taps, 16) <= 32 && L->Ho <= L->Hin + L->pad && L->Wo <= L->Win + L->pad;
+  }
+  if (st > 4 || (st & 1)) return false;
+  if (Cg > 4 || L->S != 1 || L->d < Cg || L->d % 4 != 0 || L->asmt_t_mode != 1 || !WsWidth(Kg)) return false;
+  if (L->Wo > qcnn::CeilDiv(L->Win + 2 * L->pad, st) || static_cast<double>(L->Hin) * L->Win * L->Cin * 4 > 2.0e9) return false;
+  KStepTable t;
+  if (qcnn::Mode1Table(L, 0, true, 0, t) > kMaxKSteps) return false;
+  return StridedTileFits(L, 128) || (Kg <= 128 && StridedTileFits(L, 256));
+}
+
 }  // namespace
 
 namespace qcnn {
 
+int BuildConvWsImage(qcnn_layer* L) {
+  if (!WsLayerTakes(L) || L->d_w_ws.get()) return 0;
+  WsImageArgs a;
+  memset(&a, 0, sizeof(a));
+  a.G = L->grp; a.Kg = L->Cout / L->grp; a.KgPad = RoundUp(a.Kg, 16); a.S = L->S; a.K = L->K; a.d = L->d;
+  a.Cg = L->Cin / L->grp; a.stride = L->stride;
+  if (a.stride == 1) {
+    Mode0Table(L, 0, 0, a.kt);
+    a.nE = CeilDiv(a.Cg, 8) * a.kt.ntab;
+    a.tapsPad = RoundUp(a.kt.ntab, 16);
+  } else {
+    a.nE = Mode1Table(L, 0, true, 0, a.kt);
+    a.tapsPad = RoundUp(CeilDiv(L->ksz, a.stride) * L->ksz, 16);
+  }
+  const size_t rows = static_cast<size_t>(a.G) * a.nE * 2 * a.Kg;
+  QCNN_CUDA(L->d_w_ws.Reserve(L->ctx, rows * sizeof(uint4)));
+  a.ctrd = L->d_ctrd_bf.as<uint4>(); a.asmtT = L->d_asmt_t.as<uint8_t>(); a.img = L->d_w_ws.as<uint4>();
+  conv_ws_image_kernel<<<static_cast<unsigned>(std::min<size_t>((rows / 2 + 255) / 256, 4096)), 256>>>(a);
+  QCNN_CUDA(cudaGetLastError());
+  QCNN_CUDA(cudaDeviceSynchronize());
+  return 0;
+}
+
 // Stride-1 tilings (mode-0 geometry): positions per CTA x channels per CTA (an instantiated width dividing Cout / grp)
-// x k-steps per weight stage, under the conditions of pq_gemm_tc mode 0 (or <= 3 channels per group) plus the pre-split
-// codebook and the channel-major index block of at most 32 taps.  The positions of a CTA need not fit one register pass
-// of the producers: any plane ring that fits in shared memory is a tiling.
+// x k-steps per weight stage x weight buffers.  The positions of a CTA need not fit one register pass of the producers:
+// any plane ring that fits in shared memory is a tiling.
 static void PlanConvWsS1(const qcnn_layer* L, int N, ConvCands* cands) {
   const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, taps = L->ksz * L->ksz;
-  // (Cg <= 3: one chunk, half A read as scalars; wider groups: whole 4-channel halves read as float4)
-  if (L->src_nchw || L->d % 4 != 0 || (Cg > 3 && (Cg % 4 != 0 || L->Cin % 4 != 0)) || L->S * L->d < Cg || taps > kMaxKSteps) return;
-  if (L->asmt_t_mode != 0 || RoundUp(taps, 16) > 32) return;
+  if (L->src_nchw) return;
   const int PW = L->Win + L->pad, IB = (L->Hin + L->pad) * PW;
-  if (L->Ho > L->Hin + L->pad || L->Wo > PW || static_cast<double>(N) * IB > 2.0e9) return;
+  if (static_cast<double>(N) * IB > 2.0e9) return;
   const size_t smemMax = SmemOptin(L->ctx);
   // widths: every instantiated divisor of Kg from 64 up (narrower tiles re-stage the same positions for few channels),
   // or the widest divisor when all are narrower
@@ -472,85 +517,85 @@ static void PlanConvWsS1(const qcnn_layer* L, int N, ConvCands* cands) {
       a.NPOS = RoundUp(P + (L->ksz - 1) * (PW + 1), 8);
       a.planeRows = a.NPOS;
       a.nChunks = CeilDiv(Cg, 8);
-      a.tapsPad = RoundUp(taps, 16);
       Mode0Table(L, PW, a.NPOS, a.kt);
-      // k-steps per weight stage: the chunk's taps in as few equal stages as fit; a ring of three plane buffers if it fits
-      bool fit = false;
-      for (int stages = 1; stages <= taps && !fit; stages++) {
-        a.KS = CeilDiv(taps, stages);
-        for (a.nPB = 3; a.nPB >= 2; a.nPB--)
-          if (static_cast<size_t>(MapWsSmem(a).total) <= smemMax) { fit = true; break; }
+      // per depth of the weight ring (4, 3, 2 buffers): k-steps per stage = the chunk's taps in as few equal stages as
+      // fit (gemm_gt: that many), a ring of three plane buffers if it fits
+      for (a.nWB = 4; a.nWB >= 2; a.nWB--) {
+        bool fit = false;
+        for (int stages = 1; stages <= taps && !fit; stages++) {
+          a.KS = L->opt_gemm_gt ? L->opt_gemm_gt : CeilDiv(taps, stages);
+          if (a.KS > taps) break;
+          for (a.nPB = 3; a.nPB >= 2; a.nPB--)
+            if (static_cast<size_t>(MapWsSmem(a).total) <= smemMax) { fit = true; break; }
+          if (L->opt_gemm_gt) break;
+        }
+        if (!fit) continue;
+        p.smem = static_cast<size_t>(MapWsSmem(a).total);
+        p.key = {P, a.KS, a.nct, a.nWB};
+        const double ne = static_cast<double>(a.nChunks) * taps;
+        // tensor work on PlanPqGemm's scale (as PlanConvWs below) and the set-up
+        const double perCta = ne * 2.0 * (P / 64) * (W / 128.0) * (3.0 * 64.0 * 1.15 / 4.0) + 4000.0 + P * 24.0;
+        const double ctas = static_cast<double>(CeilDiv(N * IB, P)) * G * a.nct;
+        cands->emplace_back(perCta * std::ceil(ctas / L->ctx->sm_count), p);
       }
-      if (!fit) continue;
-      p.smem = static_cast<size_t>(MapWsSmem(a).total);
-      p.key = {P, a.KS, a.nct};
-      const int stages = a.nChunks * CeilDiv(taps, a.KS);
-      const double ne = static_cast<double>(a.nChunks) * taps;
-      // tensor work on PlanPqGemm's scale (as PlanConvWs below), a pipeline drain per weight stage, the set-up
-      const double perCta = ne * 2.0 * (P / 64) * (W / 128.0) * (3.0 * 64.0 * 1.15 / 4.0) + 600.0 * stages + 4000.0 + P * 24.0;
-      const double ctas = static_cast<double>(CeilDiv(N * IB, P)) * G * a.nct;
-      cands->emplace_back(perCta * std::ceil(ctas / L->ctx->sm_count), p);
     }
   }
 }
 
 // Candidate tilings for batch N (cost in SM-cycles, the scale of PlanPqGemm's model): positions per CTA x k-steps per
-// weight stage (x channel tiles, stride 1).  Eligible: bf16x2 operands, an instantiated channel width, the pre-split
-// codebook and the channel-major index block; stride 1 under the conditions of pq_gemm_tc mode 0, strided layers under
-// those of its mode 1.
+// weight stage x weight buffers (x channel tiles, stride 1), for the layers with a weight image (WsLayerTakes) at bf16x2
+// operands.
 void PlanConvWs(const qcnn_layer* L, int N, ConvCands* cands) {
-  const int G = L->grp, Cg = L->Cin / G, Kg = L->Cout / G, st = L->stride;
-  if (!L->opt_tc_bf || L->K < 1 || L->K > 256) return;
+  const int G = L->grp, Kg = L->Cout / G, st = L->stride;
+  if (!L->opt_tc_bf || !L->d_w_ws.get()) return;
   if (st == 1) { PlanConvWsS1(L, N, cands); return; }
-  if (st < 2 || st > 4 || (st & 1)) return;
-  if (Cg > 4 || L->S != 1 || L->d < Cg || L->d % 4 != 0 || L->asmt_t_mode != 1) return;
-  if (!WsWidth(Kg)) return;
   const int PWp = CeilDiv(L->Win + 2 * L->pad, st), PHp = CeilDiv(L->Hin + 2 * L->pad, st);
-  if (L->Wo > PWp) return;
   const int IB = PHp * PWp;
-  if (static_cast<double>(N) * IB > 2.0e9 || static_cast<double>(L->Hin) * L->Win * L->Cin * 4 > 2.0e9) return;
+  if (static_cast<double>(N) * IB > 2.0e9) return;
   const size_t smemMax = SmemOptin(L->ctx);
   for (int MB = 2; MB >= 1; MB--) {
     if (MB == 2 && Kg > 128) continue;   // (2 x 128 accumulator registers do not fit)
     const int P = 128 * MB;
+    if (!StridedTileFits(L, P)) continue;
     ConvPlan p;
     memset(&p, 0, sizeof(p));
     p.kernel = kConvWs; p.threads = kWsThreads;
     ConvWsArgs& a = p.ws;
     SetGemmGeometry(L, a);
     a.PW = PWp; a.IB = IB; a.P = P; a.NC = Kg; a.nct = 1;
-    a.NPOS = RoundUp(P + ((L->ksz - 1) / st) * (PWp + 1), 8);
-    // a phase row's planes in one register pass of the producers; source offsets relative to the CTA's first image in int
-    if (st * a.NPOS > kWsRegItems1 * kWsProducers ||
-        static_cast<double>(CeilDiv(a.NPOS, IB) + 1) * L->Hin * L->Win * L->Cin > 2.0e9) continue;
+    a.NPOS = StridedNpos(L, P);
     a.planeRows = (st / 2) * a.NPOS;
     a.nChunks = st; a.nPB = st;   // every phase row resident
-    a.tapsPad = RoundUp(CeilDiv(L->ksz, st) * L->ksz, 16);
     const int ne = Mode1Table(L, a.NPOS, true, a.planeRows, a.kt);
-    if (ne > kMaxKSteps) continue;
     int maxCnt = 0;
     for (int ph = 0; ph < st; ph++) maxCnt = std::max(maxCnt, a.kt.chunkCount[ph]);
-    // k-steps per weight stage: a whole phase row when it fits, else the largest count that does
-    for (a.KS = maxCnt; a.KS >= 1 && static_cast<size_t>(MapWsSmem(a).total) > smemMax; a.KS--) {}
-    if (a.KS < 1) continue;
-    p.smem = static_cast<size_t>(MapWsSmem(a).total);
-    p.key = {P, a.KS, a.nct};
-    int stages = 0;
-    for (int ph = 0; ph < st; ph++) stages += CeilDiv(a.kt.chunkCount[ph], a.KS);
-    // tensor work on PlanPqGemm's scale (its 4 MMAs of m64 n128 k16 per k-step cost 3 * 64 * 1.15), a pipeline drain per
-    // weight stage, the set-up and the staging of the first phase row
-    const double perCta = ne * 2.0 * (P / 64) * (Kg / 128.0) * (3.0 * 64.0 * 1.15 / 4.0) + 600.0 * stages + 9000.0 + P * 24.0;
-    const double ctas = static_cast<double>(CeilDiv(N * IB, P)) * G;
-    cands->emplace_back(perCta * std::ceil(ctas / L->ctx->sm_count), p);
+    // per depth of the weight ring: k-steps per stage = a whole phase row when it fits, else the largest count that does
+    // (gemm_gt: that many)
+    for (a.nWB = 4; a.nWB >= 2; a.nWB--) {
+      if (L->opt_gemm_gt) {
+        a.KS = L->opt_gemm_gt;
+        if (a.KS > maxCnt || static_cast<size_t>(MapWsSmem(a).total) > smemMax) continue;
+      } else {
+        for (a.KS = maxCnt; a.KS >= 1 && static_cast<size_t>(MapWsSmem(a).total) > smemMax; a.KS--) {}
+        if (a.KS < 1) continue;
+      }
+      p.smem = static_cast<size_t>(MapWsSmem(a).total);
+      p.key = {P, a.KS, a.nct, a.nWB};
+      // tensor work on PlanPqGemm's scale (its 4 MMAs of m64 n128 k16 per k-step cost 3 * 64 * 1.15), the set-up and the
+      // staging of the first phase row
+      const double perCta = ne * 2.0 * (P / 64) * (Kg / 128.0) * (3.0 * 64.0 * 1.15 / 4.0) + 9000.0 + P * 24.0;
+      const double ctas = static_cast<double>(CeilDiv(N * IB, P)) * G;
+      cands->emplace_back(perCta * std::ceil(ctas / L->ctx->sm_count), p);
+    }
   }
 }
 
 int LaunchConvWs(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st) {
   ConvWsArgs a = p.ws;
-  a.src = src; a.dst = dst; a.ctrd = L->d_ctrd_bf.as<uint4>(); a.bias = L->d_bias.as<float>();
-  a.asmtT = L->d_asmt_t.as<uint8_t>();
+  a.src = src; a.dst = dst; a.wimg = L->d_w_ws.as<uint4>(); a.bias = L->d_bias.as<float>();
   a.N = N; a.relu = relu;
   SetGemmGeometry(L, a);
+  QCNN_CHECK(a.wimg, "internal: conv_ws planned for a layer without a weight image");
   QCNN_CHECK(a.stride > 1 || !L->src_nchw, "qcnn_conv_aprx_forward: the stride-1 weight-stationary tiling reads NHWC sources only");
   const long long blocks = static_cast<long long>(CeilDiv(N * a.IB, a.P)) * a.G * a.nct;
   QCNN_CHECK(blocks <= 2147483647LL, "qcnn_conv_aprx_forward: batch too large for the weight-stationary tiling");
@@ -566,17 +611,18 @@ void DescribeConvWs(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, si
   const int grid = CeilDiv(N * a.IB, a.P) * L->grp * a.nct;
   if (a.stride == 1) {
     // stride 1: N = channels per CTA, ctiles = channel tiles per group, ksteps = chunks x taps (a CTA's k-steps), so
-    // that grid x ksteps x 32 x positions x N is the executed MAC count
+    // that grid x ksteps x 32 x positions x N is the executed MAC count; wbufs = weight stage buffers
     const int stages = a.nChunks * CeilDiv(a.kt.ntab, a.KS);
     snprintf(buf, cap, " mode=0 N=%d positions=%d ctiles=%d KS=%d smem=%zuB grid=%d NPOS=%d planebufs=%d chunks=%d stages=%d "
-             "ksteps=%d", a.NC, a.P, a.nct, a.KS, p.smem, grid, a.NPOS, a.nPB, a.nChunks, stages, a.nChunks * a.kt.ntab);
+             "ksteps=%d wbufs=%d", a.NC, a.P, a.nct, a.KS, p.smem, grid, a.NPOS, a.nPB, a.nChunks, stages,
+             a.nChunks * a.kt.ntab, a.nWB);
     return;
   }
   // (no "NT=": the executed-MAC count that bench.py derives from pq_gemm_tc( plans assumes 128-channel tiles)
   int stages = 0;
   for (int c = 0; c < a.nChunks; c++) stages += CeilDiv(a.kt.chunkCount[c], a.KS);
-  snprintf(buf, cap, " N=%d positions=%d KS=%d smem=%zuB grid=%d NPOS=%d chunks=%d stages=%d ksteps=%d", a.NC, a.P, a.KS,
-           p.smem, grid, a.NPOS, a.nChunks, stages, a.kt.ntab);
+  snprintf(buf, cap, " N=%d positions=%d KS=%d smem=%zuB grid=%d NPOS=%d chunks=%d stages=%d ksteps=%d wbufs=%d", a.NC, a.P,
+           a.KS, p.smem, grid, a.NPOS, a.nChunks, stages, a.kt.ntab, a.nWB);
 }
 
 }  // namespace qcnn

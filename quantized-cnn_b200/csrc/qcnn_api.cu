@@ -187,7 +187,7 @@ int qcnn_conv_layer_create(qcnn_ctx* ctx, int Cin, int Hin, int Win, int Cout, i
     qcnn_layer_destroy(L);
     return 2;
   }
-  if (BuildCtrdBf(L)) { qcnn_layer_destroy(L); return 2; }
+  if (BuildCtrdBf(L) || BuildConvWsImage(L)) { qcnn_layer_destroy(L); return 2; }
   if (PlanConv(L, 256)) {  // validates that a tiling exists; re-planned per batch size at launch
     qcnn_layer_destroy(L);
     return 1;

@@ -248,14 +248,13 @@ enum ConvKernel {
 struct ConvWsArgs {
   const float* src;
   float* dst;
-  const uint4* ctrd;          // pre-split codebook (qcnn_layer::d_ctrd_bf)
-  const uint8_t* asmtT;       // channel-major index block (qcnn_layer::d_asmt_t)
+  const uint4* wimg;          // weight image (qcnn_layer::d_w_ws)
   const float* bias;
   long long srcImg, dstImg;   // elements per source / destination image
   int N, Hi, Wi, Cin, Ho, Wo, Cout, ksz, pad, stride, G, Cg, Kg, KgPad, S, K, d;
   int NC, PW, IB;             // channels per CTA (N of the MMA) / grid row pitch / positions per image
   int rowStride, colStride, chStride;   // source element strides of an input row / column / channel
-  int nPB, P, tapsPad;        // plane buffers (strided: one per phase row) / positions per CTA / index bytes per channel
+  int nPB, P, nWB;            // plane buffers (strided: one per phase row) / positions per CTA / weight stage buffers
   int planeRows, NPOS;        // 16-byte rows per plane / staged positions per plane (P + halo)
   int KS, nct, nChunks;       // k-steps per weight stage / channel tiles per group (Kg / NC) / chunks (8 channels or a phase row)
   int relu;
@@ -268,7 +267,7 @@ struct ConvPlan {
   int threads;
   size_t smem;
   std::array<int, 6> key;   // equal keys of one kernel: near-duplicates.  LUT + gather: CPT, J, nct, nstrips, rgroups, R;
-                            // pq_gemm_tc: NT, GT, nct, nsplit; conv_ws: P, KS, nct (unused entries 0)
+                            // pq_gemm_tc: NT, GT, nct, nsplit; conv_ws: P, KS, nct, nWB (unused entries 0)
   ConvArgs a;           // kernels 0-4: geometry + tiling (pointers/N filled at launch)
   GemmArgs g;           // kernel 6 (pq_gemm_tc)
   ConvWsArgs ws;        // kernel 7 (conv_ws)
@@ -319,6 +318,8 @@ struct qcnn_layer {
   qcnn::DeviceBuffer d_partial;  // float
   qcnn::DeviceBuffer d_flat;     // tensor-core FC path: source pre-split into hi/lo plane images (fc_prep_kernel)
   qcnn::DeviceBuffer d_ctrd_bf;  // present exactly when d % 4 == 0: codebook pre-split into bf16 pieces (pq_gemm_tc.cu, conv_ws.cu, bf16x2 operands): [S][d/4 pieces][K] x {w1 (4 x bf16), w2 (4 x bf16)}: a (subspace, piece) slice is contiguous
+  qcnn::DeviceBuffer d_w_ws;     // conv layers conv_ws can take: the decoded weights of every k-step, [grp][k-step][w1, w2][Kg]
+                                 // 16-byte rows (conv_ws.cu builds and reads it); a CTA bulk-copies its stages from here
   qcnn::DeviceBuffer d_cpart;    // chain kernel (fc_chain.cu): per-CTA partial sums [sm_count][DoutPad], words double as ready flags
   // tuning overrides (0 = automatic)
   int opt_fc_nsplit = 0;
@@ -497,6 +498,7 @@ int RefineOnce(qcnn_ctx* ctx, const char* who, bool conv, bool target, const PqG
 // conv_ws.cu: the tensor-core family's weight-stationary tilings of stride-1 layers (mode-0 geometry, channel tiles) and
 // of strided narrow-input layers (mode-1 geometry)
 void PlanConvWs(const qcnn_layer* L, int N, ConvCands* cands);
+int BuildConvWsImage(qcnn_layer* L);   // layer creation, after BuildCtrdBf: d_w_ws for the layers conv_ws can take
 int LaunchConvWs(qcnn_layer* L, const ConvPlan& p, const float* src, int N, float* dst, int relu, cudaStream_t st);
 void DescribeConvWs(const qcnn_layer* L, const ConvPlan& p, int N, char* buf, size_t cap);
 
