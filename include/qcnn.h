@@ -86,7 +86,8 @@ QCNN_API int qcnn_conv_layer_set_src_nchw(qcnn_layer* layer, int enable);
  * channels per group, with bf16x2 operands (tensor_core = 2), as a weight-stationary GEMM whose N is the channels of one
  * CTA: Cout/grp or a tile of it, in {16, 32, 64, 96, 128, 192, 256}; describe() names it pq_gemm_tc_ws), "gemm_nt" (positions per CTA of the pq_gemm_tc tilings, and 128 / 256 for conv_ws; 0 = any), "gemm_gt"
  * (k-steps per stage of those tilings, 0 = any), "gemm_nsplit" (their K-split factor, 0 = any), "gemm_ct" (channels per
- * CTA of the conv_ws tilings, 0 = any; a pin that no tiling of the layer matches makes the forward fail), "lut_cpt",
+ * CTA of the conv_ws tilings, 0 = any), "gemm_wb" (conv only: weight stage buffers of the conv_ws tilings' ring, 2, 3
+ * or 4, 0 = any; the other families ignore it; a pin that no tiling of the layer matches makes the forward fail), "lut_cpt",
  * "lut_j", "lut_nct", "lut_r", "lut_rgroups" (the LUT + gather tilings, force_kernel 0-4, with that many channels per
  * thread, positions per lane -- conv_direct: output rows per thread --, channel tiles per group, output rows per strip --
  * conv_direct: after its clamp to Ho + (Ho & 1) -- and row groups; 0 = any; a pin that no tiling matches makes the
@@ -115,6 +116,14 @@ QCNN_API int qcnn_layer_work(const qcnn_layer* layer, int N, double* alg_bytes, 
 /* device copy of the re-laid-out assignment table, decoded back to plain 0-based indices in the reference's
  * asmtBuf order ([kh][kw][S][Cout] / [S][Dout], CaffeEva.cc:585-586, 610-611) -- for bit-exact index tests */
 QCNN_API int qcnn_layer_read_asmt_h(const qcnn_layer* layer, uint8_t* out_h, size_t cap);
+/* device copy of a conv layer's weight image, the decoded bf16x2 weights conv_ws streams into shared memory (for
+ * byte-exact tests): *bytes = its size, G x entries x 2 x (Cout/grp) x 16 bytes, laid out [grp][entry][w1, w2][Cout/grp]
+ * 16-byte rows, an entry being one k-step (stride 1: a chunk of 8 input channels x one tap, chunk by chunk; strided: the
+ * k-steps of each phase row in turn).  A k-step has two halves of 4 weights (stride 1: input channels 0-3 and 4-7 of the
+ * chunk; strided: a tap and its paired tap), each split as w = w1 + w2 into bf16 pieces: the w1 row holds the 4 w1 of
+ * either half, the w2 row the w2; a half the k-step does not have is zero.  0 bytes for a layer without an image (an FC
+ * layer, a conv layer conv_ws does not take).  out_h may be NULL to query the size; otherwise cap must be >= *bytes. */
+QCNN_API int qcnn_layer_read_w_ws(const qcnn_layer* layer, void* out_h, size_t cap, size_t* bytes);
 
 /* ---- hot path -------------------------------------------------------------------------------------------- */
 /* replaces CaffeEva::CalcFeatMap_ConvAprx (src/CaffeEva.cc:760-868) incl. its GetInPdMat call (:810, :1261-1296)

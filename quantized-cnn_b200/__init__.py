@@ -73,6 +73,7 @@ _SIGS = {
     "qcnn_layer_out_dims": (_i, [_vp, C.POINTER(_i)]),
     "qcnn_layer_work": (_i, [_vp, _i, _dp, _dp, _dp]),
     "qcnn_layer_read_asmt_h": (_i, [_vp, _vp, _sz]),
+    "qcnn_layer_read_w_ws": (_i, [_vp, _vp, _sz, C.POINTER(_sz)]),
     "qcnn_conv_aprx_forward": (_i, [_vp, _vp, _i, _vp, _i, _vp]),
     "qcnn_fc_aprx_forward": (_i, [_vp, _vp, _i, _vp, _i, _vp]),
     "qcnn_fc_aprx_forward_flat": (_i, [_vp, _vp, _i, _vp, _i, _vp]),
@@ -292,6 +293,15 @@ class _Layer(object):
     def read_asmt(self, n):
         out = np.empty(n, np.uint8)
         _check(lib.qcnn_layer_read_asmt_h(self.h, out.ctypes.data_as(_vp), out.size))
+        return out
+
+    def read_w_ws(self):
+        """The layer's weight image as uint8 bytes (include/qcnn.h: qcnn_layer_read_w_ws); empty without one."""
+        n = _sz()
+        _check(lib.qcnn_layer_read_w_ws(self.h, None, 0, C.byref(n)))
+        out = np.empty(n.value, np.uint8)
+        if out.size:
+            _check(lib.qcnn_layer_read_w_ws(self.h, out.ctypes.data_as(_vp), out.size, C.byref(n)))
         return out
 
 

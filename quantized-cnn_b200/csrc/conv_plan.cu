@@ -77,18 +77,19 @@ int PlanConv(qcnn_layer* L, int N) {
   }
   // layer parameters "gemm_nt" / "gemm_gt" / "gemm_nsplit": only pq_gemm_tc tilings with that many positions per CTA,
   // k-steps per stage and K-split factor (0 = any); "gemm_nt" and "gemm_gt" also restrict the positions per CTA and the
-  // k-steps per weight stage of conv_ws, and "gemm_ct" its channels per CTA
-  if (L->opt_gemm_nt || L->opt_gemm_gt || L->opt_gemm_nsplit || L->opt_gemm_ct) {
+  // k-steps per weight stage of conv_ws, "gemm_ct" its channels per CTA and "gemm_wb" the depth of its weight ring
+  if (L->opt_gemm_nt || L->opt_gemm_gt || L->opt_gemm_nsplit || L->opt_gemm_ct || L->opt_gemm_wb) {
     keepIf([L](const ConvPlan& c) {
       if (c.kernel == kConvWs)
         return (!L->opt_gemm_nt || c.ws.P == L->opt_gemm_nt) && (!L->opt_gemm_gt || c.ws.KS == L->opt_gemm_gt) &&
-               (!L->opt_gemm_ct || c.ws.NC == L->opt_gemm_ct);
+               (!L->opt_gemm_ct || c.ws.NC == L->opt_gemm_ct) && (!L->opt_gemm_wb || c.ws.nWB == L->opt_gemm_wb);
       const GemmArgs& g = c.g;
       return c.kernel != kPqGemmTc || ((!L->opt_gemm_nt || g.NT == L->opt_gemm_nt) && (!L->opt_gemm_gt || g.GT == L->opt_gemm_gt) &&
                                        (!L->opt_gemm_nsplit || g.nsplit == L->opt_gemm_nsplit));
     });
-    QCNN_CHECK(!cands.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d gemm_gt=%d gemm_nsplit=%d gemm_ct=%d has no tiling for "
-               "this layer at batch %d", L->opt_gemm_nt, L->opt_gemm_gt, L->opt_gemm_nsplit, L->opt_gemm_ct, N);
+    QCNN_CHECK(!cands.empty(), "qcnn_conv_aprx_forward: gemm_nt=%d gemm_gt=%d gemm_nsplit=%d gemm_ct=%d gemm_wb=%d has no "
+               "tiling for this layer at batch %d", L->opt_gemm_nt, L->opt_gemm_gt, L->opt_gemm_nsplit, L->opt_gemm_ct,
+               L->opt_gemm_wb, N);
   }
   // layer parameters "lut_cpt" / "lut_j" / "lut_nct" / "lut_r" / "lut_rgroups": only LUT + gather tilings (kernels 0-4) with
   // that key entry (0 = any): channels per thread, positions per lane (conv_direct: output rows per thread), channel tiles
@@ -155,11 +156,13 @@ int LaunchConv(qcnn_layer* L, const float* src, int N, float* dst, int relu, cud
       }
       if (!ok) continue;
       static const bool tuneLog = getenv("QCNN_AUTOTUNE_LOG") != nullptr;
-      if (tuneLog) {   // (conv_ws: positions per CTA, KS, bf16x2, no K-split)
+      if (tuneLog) {   // (conv_ws: positions per CTA, KS, bf16x2, no K-split, and its weight buffers)
         const bool ws = c.kernel == kConvWs, tc = c.kernel == kPqGemmTc;
-        fprintf(stderr, "[qcnn autotune] N=%d Cout=%d k=%d cand %zu: kernel=%d NT/CPT=%d GT/J=%d bf=%d nsplit=%d smem=%zu -> %.4f ms\n",
+        char wsTail[16] = "";
+        if (ws) snprintf(wsTail, sizeof(wsTail), " wb=%d", c.ws.nWB);
+        fprintf(stderr, "[qcnn autotune] N=%d Cout=%d k=%d cand %zu: kernel=%d NT/CPT=%d GT/J=%d bf=%d nsplit=%d%s smem=%zu -> %.4f ms\n",
                 N, L->Cout, L->ksz, i, c.kernel, ws ? c.ws.P : tc ? c.g.NT : c.CPT, ws ? c.ws.KS : tc ? c.g.GT : c.J,
-                ws ? 1 : c.g.bf, ws ? 1 : c.g.nsplit, c.smem, ms);
+                ws ? 1 : c.g.bf, ws ? 1 : c.g.nsplit, wsTail, c.smem, ms);
       }
       if (ms < bestMs) { bestMs = ms; bestI = i; }
     }

@@ -117,6 +117,8 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const ConvWsArgs
     // the weight ring, filled by producer thread 0: stage jI = k-steps [s0I, + KS) of chunk kcI into buffer jI % nWB, once
     // the MMAs of stage jI - nWB have retired.  The image holds [grp][entry][w1, w2][Kg] 16-byte rows, an entry being a
     // k-step of the layer (mode 0: chunk x tap, mode 1: the k-step table's order); a stage's entries are consecutive.
+    // The stages are exactly those the consumers wait for: ceil(count / KS) per chunk, none for a phase row without
+    // k-steps (ksz < stride: the trailing rows; the chunk advance steps over them).
     const int nE = S1 ? nCh * a.kt.ntab : a.kt.ntab;
     int jI = 0, kcI = 0, s0I = 0;
     auto issueStage = [&]() {
@@ -135,7 +137,12 @@ __global__ void __launch_bounds__(kWsThreads, 1) conv_ws_kernel(const ConvWsArgs
       }
       jI++;
       s0I += KS;
-      if (s0I >= cnt) { s0I = 0; kcI++; }
+      if (s0I >= cnt) {
+        s0I = 0;
+        kcI++;
+        if constexpr (!S1)
+          while (kcI < nCh && a.kt.chunkCount[kcI] == 0) kcI++;
+      }
     };
     if (pt == 0)   // the first stages are in flight before any position is loaded
       while (jI < nWB && kcI < nCh) issueStage();

@@ -357,6 +357,14 @@ int qcnn_layer_set_param(qcnn_layer* L, const char* name, int value) {
     L->plan_N = 0; L->tuned = 0;
     L->tunedPlans.clear();
   }
+  else if (!strcmp(name, "gemm_wb")) {
+    // conv only, 0 = any: the conv_ws tilings with that many weight stage buffers (2, 3 or 4) in their ring.  A pin that
+    // no tiling of the layer matches fails the forward.
+    QCNN_CHECK(L->kind == QCNN_KIND_CONV, "qcnn_layer_set_param: 'gemm_wb' applies to conv layers");
+    L->opt_gemm_wb = value < 0 ? 0 : value;
+    L->plan_N = 0; L->tuned = 0;
+    L->tunedPlans.clear();
+  }
   else if (!strcmp(name, "lut_cpt") || !strcmp(name, "lut_j") || !strcmp(name, "lut_nct") || !strcmp(name, "lut_r") ||
            !strcmp(name, "lut_rgroups")) {
     // conv only, 0 = any: the LUT + gather tilings (force_kernel 0-4) with that many channels per thread, positions per
@@ -466,6 +474,16 @@ int qcnn_layer_read_asmt_h(const qcnn_layer* L, uint8_t* out_h, size_t cap) {
         out_h[(static_cast<size_t>(t) * L->S + s) * L->Cout + c] =
             dev[((static_cast<size_t>(g) * L->S + s) * taps + t) * KgPad + cl];
       }
+  return 0;
+}
+
+int qcnn_layer_read_w_ws(const qcnn_layer* L, void* out_h, size_t cap, size_t* bytes) {
+  QCNN_CHECK(L && bytes, "qcnn_layer_read_w_ws: NULL argument");
+  *bytes = L->d_w_ws.bytes();
+  if (!out_h || *bytes == 0) return 0;
+  QCNN_CHECK(cap >= *bytes, "qcnn_layer_read_w_ws: buffer too small (%zu < %zu bytes)", cap, *bytes);
+  QCNN_ON_DEVICE(L->ctx->device);
+  QCNN_CUDA(cudaMemcpy(out_h, L->d_w_ws.get(), *bytes, cudaMemcpyDeviceToHost));
   return 0;
 }
 

@@ -332,6 +332,7 @@ struct qcnn_layer {
   int opt_gemm_gt = 0;       // conv: ... to this many k-steps per stage (0 = any)
   int opt_gemm_nsplit = 0;   // conv: ... to this K-split factor (0 = any)
   int opt_gemm_ct = 0;       // conv: restrict conv_ws tilings to this many channels per CTA (0 = any)
+  int opt_gemm_wb = 0;       // conv: ... to this many weight stage buffers (0 = any)
                              // (FC with fc_ws: gemm_nt / gemm_gt / gemm_ct / gemm_nsplit restrict the fc_ws tilings)
   int opt_lut_cpt = 0;       // conv: restrict LUT + gather tilings (kernels 0-4) to this ConvPlan::key[0] (CPT) (0 = any)
   int opt_lut_j = 0;         // ... key[1]: positions per lane (conv_direct: output rows per thread)
